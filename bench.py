@@ -49,7 +49,7 @@ def measured_peaks():
             return float(j["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "data sheet (H100 SXM 3.35 TB/s HBM3), not measured"
 
 
 def measured_tensor_peak():
@@ -60,7 +60,7 @@ def measured_tensor_peak():
             return float(json.load(open(path))["bf16_tflops_sustained"]), "measured (MEASURED_PEAKS.json bf16_tflops_sustained)"
         except Exception:
             pass
-    return 1590.0, "fallback (B200_PROFILING.md 1.59 PFLOP/s bf16)"
+    return 989.0, "data sheet (H100 SXM 989 TFLOP/s dense bf16), not measured"
 
 
 class ClockSampler:
@@ -197,6 +197,30 @@ def ncu_traffic_per_position():
         return None
 
 
+def fetch_tokens(model, utts, n_new):
+    """Generated tokens of every utterance slot as mvb_s1_fetch hands them to a caller: [utts, n_new] int32."""
+    import ctypes as C
+    import numpy as np
+    from mvb200 import _lib
+    out = np.zeros((utts, n_new), dtype=np.int32)
+    for u in range(utts):
+        buf = np.zeros(n_new, dtype=np.int32)
+        n, d = C.c_int32(0), C.c_int32(0)
+        _lib.check(model._lib.mvb_s1_fetch(model.handle, u, buf.ctypes.data_as(C.c_void_p), n_new, C.byref(n), C.byref(d),
+                                           model._stream()))
+        torch.cuda.synchronize()
+        out[u, : int(n.value)] = buf[: int(n.value)]
+    return out
+
+
+def dump_outputs(out_dir, arrays):
+    """Write each array as <out_dir>/<name>.npy in float64 (token ids are exact in float64)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, arr in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.asarray(arr, dtype=np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -207,6 +231,8 @@ def main():
     ap.add_argument("--skip-cpu-baseline", action="store_true")
     ap.add_argument("--skip-pipeline", action="store_true")
     ap.add_argument("--skip-configs", action="store_true", help="skip the batch-8 / long-form legs (BASELINE configs[2], [3])")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the tokens the last timed step generated to DIR/tokens.npy (float64)")
     a = ap.parse_args()
     rank = int(os.environ.get("RANK", "0")); world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
@@ -273,6 +299,8 @@ def main():
     launches = model._lib.mvb_s1_launch_count(model.handle) - lc0
     ms = e0.elapsed_time(e1)
     assert tokens_generated(model, utts) == [N_NEW] * utts
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, {"tokens": fetch_tokens(model, utts, N_NEW)})
 
     # ---- decode roofline: one persistent launch of `reps` positions at mid-utterance context ----
     reps = 200
@@ -345,7 +373,7 @@ def main():
         "config": {"workload": "BASELINE configs[1] stage-1: 1.2B causal LM, T=48 prompt, 750 new tokens (5.0 s audio), "
                                "top_p=0.95 guidance=3.0 temperature=1.0, CFG pair per utterance",
                    "utts_per_gpu": utts, "parallelism": f"replicas x{world}, utterances sharded, weights NCCL-broadcast at init",
-                   "l2": "not flushed: 2.48 GB of weights are streamed every token (>> 126 MB L2)",
+                   "l2": "not flushed: 2.48 GB of weights are streamed every token (>> 50 MB L2)",
                    "stage2_vocoder_in_timed_region": False},
         "e2e": {"value": round(e2e_toks * world / (e2e_ms_max * 1e-3), 2), "unit": "tokens/s",
                 "h2d_bytes_per_step": int(utts * (T_PROMPT * 4 * 2 + 256 * 4 + 32)), "d2h_bytes_per_step": int(utts * (N_NEW * 4 + 8))},
@@ -418,7 +446,7 @@ def pipeline_leg(model, prompts, spk, h_spk_pinned, utts, steps, device, world, 
     pipe_s = time.perf_counter() - t0
     audio_s, s1_s, s2_s, voc_s, mbd_s, post_s = acc
     # rooflines of the downstream stages (one utterance): stage-2 streams its bf16 weights once per forward (HBM-bound);
-    # the SEANet decoder is fp32 CUDA-core work; the diffusion UNets are tcgen05 GEMM work (bf16 taps, two-term activations)
+    # the SEANet decoder is fp32 CUDA-core work; the diffusion UNets are tensor-core GEMM work (bf16 taps, two-term activations)
     hbm_peak, tensor_peak = measured_peaks()[0], measured_tensor_peak()[0]
     n_u = steps * utts
     s2_bytes = sum(v.numel() for k, v in synth.stage2_checkpoint(synth.S2_FULL, 1)["model"].items() if v.ndim == 2) * 2
@@ -444,7 +472,7 @@ def pipeline_leg(model, prompts, spk, h_spk_pinned, utts, steps, device, world, 
                             "audio_post_pcm16": round(post_s / steps * 1e3, 2)},
             "mbd_config": f"PARAMETRISED, parity unpinned: {mbd_cfg.n_models} band UNets (hidden {u.hidden}, depth {u.depth}, growth {u.growth}, "
                           f"k{u.kernel}/s{u.stride}, {u.res_blocks} res block) x {len(mbd_cfg.steps()) - 1} calls, {mbd_cfg.eq_bands}-band re-EQ; "
-                          "convolutions with >= 32 input channels on tcgen05 (bf16 taps, two-term bf16 activations, fp32 accumulate), the 1-channel input conv and the 1x1 condition conv on fp32 CUDA cores",
+                          "convolutions with >= 32 input channels on the tensor cores (bf16 taps, two-term bf16 activations, fp32 accumulate), the 1-channel input conv and the 1x1 condition conv on fp32 CUDA cores",
             "stage_rooflines": stage_rooflines,
             "coverage": "stage-1 (750 tokens) + token adapters + stage-2 (6 codebooks) + EnCodec SEANet decoder + multi-band diffusion "
                         "+ loudness/compressor/PCM16 on device, wav bytes on the host; DeepFilterNet is NOT implemented"}

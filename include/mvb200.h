@@ -1,5 +1,5 @@
 /*
- * mvb200.h -- C ABI of libmvb200.so: the B200 (sm_100a) engine behind MetaVoice-1B's
+ * mvb200.h -- C ABI of libmvb200.so: the H100 (sm_90a) engine behind MetaVoice-1B's
  * TTS.synthesise() hot path.  Plain pointers and sizes only; no torch types.
  *
  * Every entry point names the reference interface it replaces (paths relative to the
@@ -162,7 +162,7 @@ uint64_t mvb_s1_launch_count(const mvb_s1* h);
 int mvb_s1_fetch_sampled(mvb_s1* h, int32_t utt, int32_t* out_tokens, int32_t cap, void* stream);
 int mvb_s1_trace_fetch(mvb_s1* h, long long* out, int32_t max_ctas, void* stream);
 
-/* Tensor-core linear operator (tcgen05 + TMA weight streaming), the building block of the batched /
+/* Tensor-core linear operator (TMA weight streaming + mma.sync), the building block of the batched /
  * prefill path and of the stage-2 model: y[R, M] (+)= f(x)[R, K] . W[M, K]^T, W bf16 row-major [out, in]
  * as every nn.Linear weight in the reference checkpoints (e.g. fast_model.py:194-195, layers/attn.py:61-64).
  * f = optional RMSNorm with bf16 gain (fast_model.py:250-261) when d_gain != NULL.  split_lo != 0 carries the

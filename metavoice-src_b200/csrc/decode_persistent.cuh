@@ -9,18 +9,15 @@
 //     guarded by full/empty mbarriers.  Weights do not depend on activations, so the producer never waits for a grid
 //     barrier: the HBM stream keeps running across phase, layer AND token boundaries (the next token's first weight
 //     tiles land while the grid is still sampling).
-//   * warp 1 = MMA ISSUER (tcgen05.mma, fp32 accumulators double-buffered in TMEM).  Two operand assignments:
-//       WB = true : the streamed weight tile [256 rows x 64 k] is the UMMA *B* operand (N = 256), the staged activation
-//                   rows (hi + lo bf16 halves, <= 32 rows) the *A* operand (M = 128; rows past NB read whatever follows in
-//                   shared memory, their accumulator lanes are never looked at).  An SS-mode UMMA fetches A at one row
-//                   per cycle, so an instruction costs ~130-150 cycles whether it multiplies 16 or 256 weight rows:
-//                   8 KB of weights per instruction.
-//       WB = false: weight tile [128 x 64] as the A operand (M = 128), activations as B (N = NB): 4 KB per instruction
-//                   (round-1 formulation, kept selectable for A/B measurements).
+//   * warp 1 = MMA WARP: the weight tile [128 rows x 64 k] is the A operand, the staged activation rows (hi + lo bf16
+//     halves, NB rows) the B operand of mma.sync.m16n8k16; fragments come from the 128B-swizzled tiles by ldmatrix and the
+//     hi and lo products accumulate into one fp32 register tile [128 x NB/2].  At the end of a tile the warp parks the
+//     accumulator in one of two shared-memory slots (acc_full / acc_empty hand-off) and goes on with the next tile.
+//     (A warpgroup-wide wgmma would need four issuing warps; at N <= 32 one warp keeps pace with the weight stream.)
 //   * warps 2..5 = COMPUTE: wait for the previous phase grid-wide (split arrive/wait counter with release/acquire
 //     atomics), stage the activation operand into swizzled smem (RMSNorm gain / attention-merge / SiLU*mul fused
-//     here), run the epilogues (tcgen05.ld -> red.global.add.f32 split-K accumulation), the decode attention on smem
-//     KV tiles (online softmax per half-warp) and the grid-distributed sampler.
+//     here), run the epilogues (accumulator slot -> red.global.add.f32 split-K accumulation), the decode attention on
+//     smem KV tiles (online softmax per half-warp) and the grid-distributed sampler.
 //   * warp 6 = optional L2 PREFETCHER: keeps a window of the flat weight-tile schedule in flight with
 //     cp.async.bulk.prefetch.tensor so that HBM keeps streaming while the grid synchronises.
 //   * RMSNorm statistic without a full-row re-read: every CTA stages x[k-slice] * gain; the CTAs of tile group 0 add
@@ -56,8 +53,7 @@ struct AttTile {
 
 struct PcShared {   // small shared state behind the big buffers
   uint64_t b_full[8], b_empty[8], b_ready, acc_full[2], acc_empty[2], kv_full[PC_NKV_MAX], kv_empty[PC_NKV_MAX], tab_ready;
-  uint32_t tmem_slot;
-  int prod_pos;                      // weight tiles issued so far (producer -> L2 prefetcher)
+  int prod_pos;                     // weight tiles issued so far (producer -> L2 prefetcher)
   int n_att_tiles;
   // every CTA's private copy of the decode state of the batch (kept in lock-step: the same deterministic update
   // from the same arg-max in every CTA; only the owner CTA writes it back to global memory)
@@ -78,22 +74,24 @@ struct PcShared {   // small shared state behind the big buffers
   AttTile att_tab[PC_MAX_TILES];
 };
 
-template <int NB, bool WB> struct PcCfg {
-  static constexpr int TILE_ROWS = WB ? 256 : 128;
+template <int NB> struct PcCfg {
+  static constexpr int TILE_ROWS = 128;
   static constexpr int STAGE_BYTES = TILE_ROWS * 128;     // [TILE_ROWS x 64 k] bf16
+  // ring depth: what fits in 227 KB next to the activation operand, the KV slots and the accumulator slots
 #ifdef PC_DEEP_KV   // A/B: trade weight-ring depth for KV tiles in flight (the attention phase is bound by KV load latency)
-  static constexpr int STAGES = WB ? ((NB == 16) ? 4 : 3) : ((NB == 16) ? 6 : 4);
-  static constexpr int NKV = WB ? 2 : 3;
+  static constexpr int STAGES = (NB == 16) ? 6 : 4;
+  static constexpr int NKV = 3;
 #else
-  static constexpr int STAGES = WB ? ((NB == 16) ? 4 : 3) : ((NB == 16) ? 8 : 6);
+  static constexpr int STAGES = (NB == 16) ? 7 : 5;
   static constexpr int NKV = 2;
 #endif
   static constexpr int B_BYTES = PC_BKB_MAX * NB * 128;
   static constexpr int RH = NB / 2;                       // activation rows carried (hi rows; lo rows follow)
-  static constexpr int ACC_COLS = WB ? 256 : NB;          // TMEM columns of one accumulator
-  static constexpr int TMEM_COLS = WB ? 512 : 64;
-  static constexpr size_t SMEM = 1024 + (size_t)STAGES * STAGE_BYTES + B_BYTES + (size_t)NKV * 2 * PC_KV_TILE_BYTES +
-                                 sizeof(PcShared) + 64;
+  static constexpr int ACC_LD = TILE_ROWS + 4;            // accumulator slot [RH][ACC_LD] fp32 (pad: conflict-free stores)
+  static constexpr int ACC_BYTES = (2 * RH * ACC_LD * 4 + 1023) / 1024 * 1024;   // two slots (keeps kvbuf 1 KB aligned)
+  static constexpr size_t SMEM = 1024 + (size_t)STAGES * STAGE_BYTES + B_BYTES + ACC_BYTES +
+                                 (size_t)NKV * 2 * PC_KV_TILE_BYTES + sizeof(PcShared) + 64;
+  static_assert(SMEM <= 227 * 1024, "persistent decode kernel exceeds the 227 KB shared-memory opt-in");
 };
 
 struct PcMat {     // one weight matrix kind, static decomposition
@@ -110,7 +108,6 @@ struct PcParams {
   int pf_mode;     // 0: no L2 prefetch, 1: by the producer while the ring is full, 2: dedicated prefetch warp
   int pf_ahead;    // weight tiles prefetched into L2 ahead of the smem ring
   int kv_pf;       // 1: L2-prefetch the next layer's KV tiles while this layer's projections stream
-  int epi_mode;    // WB epilogue: 0 = 32x32b loads + red.v4, 1 = 32x32b loads + scalar red, 2 = 16x256b fragment loads + scalar red
   float eps;
   PcMat m_qkv, m_o, m_w13, m_w2, m_head;
   const __nv_bfloat16* attn_norm;   // layer 0; layer l at + l * layer_stride
@@ -149,9 +146,6 @@ __device__ __forceinline__ void red_release_inc(unsigned* p) {
 }
 __device__ __forceinline__ void compute_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void red_add_v4(float* p, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
 
 __device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
@@ -166,38 +160,6 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const void* tmap, uint
 __device__ __forceinline__ void tma_prefetch_3d(const void* tmap, int c0, int c1, int c2) {
   asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];" ::"l"(tmap), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
-// 32 lanes x 64 consecutive 32-bit columns of tensor memory
-__device__ __forceinline__ void tmem_ld64(uint32_t taddr, uint32_t (&r)[64]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x64.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
-      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, [%64];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31]), "=r"(r[32]), "=r"(r[33]), "=r"(r[34]), "=r"(r[35]), "=r"(r[36]),
-        "=r"(r[37]), "=r"(r[38]), "=r"(r[39]), "=r"(r[40]), "=r"(r[41]), "=r"(r[42]), "=r"(r[43]), "=r"(r[44]), "=r"(r[45]),
-        "=r"(r[46]), "=r"(r[47]), "=r"(r[48]), "=r"(r[49]), "=r"(r[50]), "=r"(r[51]), "=r"(r[52]), "=r"(r[53]), "=r"(r[54]),
-        "=r"(r[55]), "=r"(r[56]), "=r"(r[57]), "=r"(r[58]), "=r"(r[59]), "=r"(r[60]), "=r"(r[61]), "=r"(r[62]), "=r"(r[63])
-      : "r"(taddr)
-      : "memory");
-}
-
-// 16 lanes x 64 consecutive 32-bit columns, fragment layout (PTX tcgen05.ld .16x256b; cute SM100_TMEM_LOAD_16dp256b8x):
-// thread T holds, for repetition i = 0..7, r[4i+0..1] = (lane T/4, columns 8i + 2(T%4) + {0,1}) and
-// r[4i+2..3] = (lane T/4 + 8, same columns).  All 32 threads carry data as soon as 8 rows are live.
-__device__ __forceinline__ void tmem_ld_16x256b_x8(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.16x256b.x8.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-
 // byte offset of the 16-byte chunk holding k..k+7 of activation row `row` inside the activation operand
 // (K-major, 128B swizzle, [k-block][NB rows][128 B])
 template <int NB>
@@ -300,23 +262,42 @@ __device__ __forceinline__ int float_to_ordered(float f) {
   return i >= 0 ? i : i ^ 0x7fffffff;
 }
 __device__ __forceinline__ float ordered_to_float(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7fffffff); }
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-// D[16x8] += A[16x16] * B[16x8], bf16 operands, fp32 accumulate (fragment layouts: PTX ISA, mma.m16n8k16)
-__device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 // (x0, x1) -> packed bf16 pair of the high terms and of the residuals (x = hi + lo to 2^-17)
 __device__ __forceinline__ void pack_hi_lo(float x0, float x1, uint32_t& hi, uint32_t& lo) {
   const __nv_bfloat16 h0 = __float2bfloat16_rn(x0), h1 = __float2bfloat16_rn(x1);
   const __nv_bfloat16 l0 = __float2bfloat16_rn(x0 - __bfloat162float(h0)), l1 = __float2bfloat16_rn(x1 - __bfloat162float(h1));
   hi = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
   lo = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
+}
+
+// acc[m][c] += W[16 m .. 16 m + 15][0 .. 63] * (hi + lo)[8 c .. 8 c + 7][0 .. 63] over one weight stage (128 rows x 64 k)
+// and one k-block of the activation operand (NB rows: RH hi rows, then RH lo rows).  One warp, mma.sync.m16n8k16.
+template <int NB>
+__device__ __forceinline__ void pc_mma_stage(uint32_t w_base, uint32_t x_base, int lane, float (&acc)[8][NB / 16][4]) {
+  constexpr int NC = NB / 16;   // n8 chunks per half
+  const int q = lane >> 3, r8 = lane & 7;
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) {
+    uint32_t b[2 * NC][2];
+#pragma unroll
+    for (int g = 0; g < NB / 16; ++g) {   // rows 16 g .. 16 g + 15: two n8 chunks, both k halves
+      uint32_t r[4];
+      const int row = 16 * g + r8 + ((q >> 1) << 3);
+      ldsm_x4(x_base + sw128_off(row, 2 * kk + (q & 1)), r);
+      b[2 * g][0] = r[0]; b[2 * g][1] = r[1]; b[2 * g + 1][0] = r[2]; b[2 * g + 1][1] = r[3];
+    }
+#pragma unroll
+    for (int m = 0; m < 8; ++m) {
+      uint32_t a[4];
+      const int row = 16 * m + r8 + ((q & 1) << 3);
+      ldsm_x4(w_base + sw128_off(row, 2 * kk + (q >> 1)), a);
+#pragma unroll
+      for (int c = 0; c < NC; ++c) {
+        mma_bf16_16816(acc[m][c], a, b[c][0], b[c][1]);            // hi rows
+        mma_bf16_16816(acc[m][c], a, b[NC + c][0], b[NC + c][1]);  // lo rows
+      }
+    }
+  }
 }
 
 template <bool KV_FP32>
@@ -332,13 +313,13 @@ __device__ __forceinline__ void load8s(const uint8_t* tile, int p, int sub, floa
   }
 }
 
-template <bool KV_FP32, int NB, bool WB>
+template <bool KV_FP32, int NB>
 __global__ void __launch_bounds__(PC_THREADS, 1)
 k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_o,
                     const __grid_constant__ CUtensorMap tm_w1, const __grid_constant__ CUtensorMap tm_w3,
                     const __grid_constant__ CUtensorMap tm_w2, const __grid_constant__ CUtensorMap tm_head,
                     const __grid_constant__ CUtensorMap tm_kv, const PcParams p) {
-  using Cfg = PcCfg<NB, WB>;
+  using Cfg = PcCfg<NB>;
   constexpr int STAGES = Cfg::STAGES;
   constexpr int RH = Cfg::RH;
   constexpr int STAGE_BYTES = Cfg::STAGE_BYTES;
@@ -350,7 +331,8 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* ring = smem;
   uint8_t* Bop = ring + STAGES * STAGE_BYTES;
-  uint8_t* kvbuf = Bop + Cfg::B_BYTES;                       // [NKV][K tile | V tile]; sampler scratch between tokens
+  float* accbuf = reinterpret_cast<float*>(Bop + Cfg::B_BYTES);   // [2][RH][ACC_LD]: MMA warp -> epilogue
+  uint8_t* kvbuf = Bop + Cfg::B_BYTES + Cfg::ACC_BYTES;     // [NKV][K tile | V tile]; sampler scratch between tokens
   PcShared& sh = *reinterpret_cast<PcShared*>(kvbuf + Cfg::NKV * 2 * PC_KV_TILE_BYTES);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -365,8 +347,8 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
     }
     ptx::mbar_init(ptx::smem_u32(&sh.b_ready), 1);
     for (int i = 0; i < 2; ++i) {
-      ptx::mbar_init(ptx::smem_u32(sh.acc_full + i), 1);
-      ptx::mbar_init(ptx::smem_u32(sh.acc_empty + i), WB ? 1 : 128);   // WB: one arrive by the TMEM-reading warp
+      ptx::mbar_init(ptx::smem_u32(sh.acc_full + i), 32);     // every lane of the MMA warp after its slot stores
+      ptx::mbar_init(ptx::smem_u32(sh.acc_empty + i), 128);   // every compute thread after its slot loads
     }
     for (int i = 0; i < Cfg::NKV; ++i) {
       ptx::mbar_init(ptx::smem_u32(sh.kv_full + i), 1);
@@ -376,18 +358,11 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
     sh.prod_pos = 0;
     ptx::fence_barrier_init();
   }
-  if (warp == 1) {
-    ptx::tmem_alloc(ptx::smem_u32(&sh.tmem_slot), Cfg::TMEM_COLS);
-    ptx::tmem_relinquish();
-  }
   // zero the activation operand once: rows >= R (hi and lo halves) must read as zero forever
   for (int i = tid; i < Cfg::B_BYTES / 16; i += PC_THREADS) reinterpret_cast<uint4*>(Bop)[i] = make_uint4(0, 0, 0, 0);
   if (tid < PC_RPAD) sh.ss[tid] = 0.f;
   fence_async_smem();
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, sh.tmem_slot, 0);   // provably warp-uniform (no operand waterfall at the tcgen05 sites)
   pdl_launch_dependents();
 
   const PcSlice s_qkv = pc_slice(p.m_qkv, cta), s_o = pc_slice(p.m_o, cta), s_w13 = pc_slice(p.m_w13, cta),
@@ -553,41 +528,46 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
       }
     }
   } else if (warp == 1) {
-    // =================================== MMA ISSUER =================================================
-    // The WHOLE warp walks the schedule (waits, counters, descriptor arithmetic stay warp-uniform -> uniform
-    // registers) and one elected lane issues the tcgen05 instructions.
-    const uint32_t idesc = WB ? ptx::umma_idesc_bf16(128, 256) : ptx::umma_idesc_bf16(128, NB);
+    // =================================== MMA WARP ===================================================
+    // The whole warp walks the schedule (waits and counters stay warp-uniform) and multiplies every weight stage of a
+    // tile into registers; the finished tile goes to accumulator slot (tile_ctr & 1) for the epilogue of the compute warps.
     uint32_t slot = 0, tile_ctr = 0, bphase = 0;
+    const uint32_t bop_u32 = ptx::smem_u32(Bop), ring_u32 = ptx::smem_u32(ring);
     auto gemm_phase = [&](const PcSlice& sl) {
       if (sl.nt == 0) return;
       ptx::mbar_wait(ptx::smem_u32(&sh.b_ready), bphase & 1u);   // activation operand of this phase staged
       ++bphase;
-      ptx::tc_fence_after();
       for (int i = 0; i < sl.nt; ++i) {
         const uint32_t ab = tile_ctr & 1u, aph = (tile_ctr >> 1) & 1u;
-        ptx::mbar_wait(ptx::smem_u32(sh.acc_empty + ab), aph ^ 1u);   // epilogue drained this accumulator
-        ptx::tc_fence_after();
-        const uint32_t dcol = tmem_base + ab * Cfg::ACC_COLS;
+        float acc[8][NB / 16][4];
+#pragma unroll
+        for (int m = 0; m < 8; ++m)
+#pragma unroll
+          for (int c = 0; c < NB / 16; ++c)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) acc[m][c][e] = 0.f;
         for (int kb = sl.kb0; kb < sl.kb1; ++kb) {
           const uint32_t s = slot % STAGES, ph = (slot / STAGES) & 1u;
           ++slot;
           ptx::mbar_wait(ptx::smem_u32(sh.b_full + s), ph);
-          ptx::tc_fence_after();
-          const uint64_t wd = ptx::umma_desc_k_sw128(ptx::smem_u32(ring + (size_t)s * STAGE_BYTES));
-          const uint64_t xd = ptx::umma_desc_k_sw128(ptx::smem_u32(Bop + (size_t)(kb - sl.kb0) * (NB * 128)));
-          const uint32_t first = (uint32_t)(kb != sl.kb0);
-          if (ptx::elect_one()) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              if (WB) ptx::umma_bf16(dcol, xd + 2 * k, wd + 2 * k, idesc, first | (uint32_t)(k != 0));
-              else ptx::umma_bf16(dcol, wd + 2 * k, xd + 2 * k, idesc, first | (uint32_t)(k != 0));
-            }
-            ptx::umma_commit(ptx::smem_u32(sh.b_empty + s));
-          }
-          __syncwarp();
+          pc_mma_stage<NB>(ring_u32 + s * STAGE_BYTES, bop_u32 + (uint32_t)(kb - sl.kb0) * (NB * 128), lane, acc);
+          __syncwarp();                     // every lane's fragment loads of this stage are done
+          if (lane == 0) ptx::mbar_arrive(ptx::smem_u32(sh.b_empty + s));
         }
-        if (ptx::elect_one()) ptx::umma_commit(ptx::smem_u32(sh.acc_full + ab));
-        __syncwarp();
+        ptx::mbar_wait(ptx::smem_u32(sh.acc_empty + ab), aph ^ 1u);   // epilogue drained this slot
+        float* slot_p = accbuf + ab * (RH * Cfg::ACC_LD);
+        const int r0 = lane >> 2, n0 = 2 * (lane & 3);
+#pragma unroll
+        for (int m = 0; m < 8; ++m)
+#pragma unroll
+          for (int c = 0; c < NB / 16; ++c) {
+            float* d = slot_p + (8 * c + n0) * Cfg::ACC_LD + 16 * m + r0;
+            d[0] = acc[m][c][0];
+            d[Cfg::ACC_LD] = acc[m][c][1];
+            d[8] = acc[m][c][2];
+            d[Cfg::ACC_LD + 8] = acc[m][c][3];
+          }
+        ptx::mbar_arrive(ptx::smem_u32(sh.acc_full + ab));
         ++tile_ctr;
       }
     };
@@ -604,7 +584,6 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
     // =================================== COMPUTE WARPS ==============================================
     const int ct = tid - 64;            // 0..127
     const int cw = ct >> 5;             // 0..3
-    const int quad = warp & 3;          // TMEM lane quadrant this warp may read
     uint32_t tile_ctr = 0, bar_idx = 0, kv_ctr = 0;
     const float inv_D = 1.f / (float)p.D;
     pdl_wait();                         // state / x inputs of the previous kernels are visible
@@ -729,7 +708,7 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
         sh.ss[ct] = 0.f;
       }
     };
-    // epilogue of this CTA's tiles: TMEM -> red.add into out[n][col0 + row]
+    // epilogue of this CTA's tiles: accumulator slot -> red.add into out[n][col0 + row]
     auto epilogue = [&](const PcSlice& sl, float* out, int ldo, int M, int split_t, float* out2) {
       for (int i = 0; i < sl.nt; ++i) {
         const int t = sl.t0 + i * sl.G;
@@ -737,101 +716,17 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
         ++tile_ctr;
         float* o = (t < split_t) ? out : out2;
         const int col0 = ((t < split_t) ? t : t - split_t) * TILE_ROWS;
-        if (WB) {
-          // accumulator = D[activation row (TMEM lane)][weight row (column)]: hi halves in lanes [0, RH), lo halves in
-          // lanes [RH, 2 RH) -- all inside lane quadrant 0, which only the compute warp with warp % 4 == 0 may read.
-          // That warp adds the CTA's split-K partial into out[n][col0 .. col0 + 255] with vectorised red.add.
-          if (quad != 0) continue;
-          ptx::mbar_wait(ptx::smem_u32(sh.acc_full + ab), aph);
-          ptx::tc_fence_after();
-          if (p.epi_mode == 2) {
-            // fragment loads: thread T owns activation rows T/4 and T/4 + 8 and two adjacent weight rows per 8 columns
-            const int qrow = lane >> 2, qcol = 2 * (lane & 3);
-            // NB = 16: lanes 0-7 = hi halves, 8-15 = lo halves of rows 0-7            -> one load, hi + lo inside the thread
-            // NB = 32: lanes 0-15 = hi halves of rows 0-15, lanes 16-31 = lo halves    -> two loads (lane offset 16)
-#pragma unroll 1
-            for (int c0 = 0; c0 < 256; c0 += 64) {
-              uint32_t va[32], vb[32];
-              tmem_ld_16x256b_x8(tmem_base + ab * 256 + c0, va);
-              if (NB == 32) tmem_ld_16x256b_x8(tmem_base + (16u << 16) + ab * 256 + c0, vb);
-              ptx::tmem_ld_wait();
-              if (c0 == 192) {                       // accumulator fully read: hand it back before the atomics
-                ptx::tc_fence_before();
-                __syncwarp();
-                if (lane == 0) ptx::mbar_arrive(ptx::smem_u32(sh.acc_empty + ab));
-              }
+        ptx::mbar_wait(ptx::smem_u32(sh.acc_full + ab), aph);
+        const float* slot_p = accbuf + ab * (RH * Cfg::ACC_LD) + ct;
+        float acc[RH];
 #pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const int col = col0 + c0 + 8 * i + qcol;
-                if (NB == 16) {
-                  if (qrow < p.R) {
-                    float* orow = o + (size_t)qrow * ldo + col;
-                    if (col < M) atomicAdd(orow, __uint_as_float(va[4 * i]) + __uint_as_float(va[4 * i + 2]));
-                    if (col + 1 < M) atomicAdd(orow + 1, __uint_as_float(va[4 * i + 1]) + __uint_as_float(va[4 * i + 3]));
-                  }
-                } else {
+        for (int n = 0; n < RH; ++n) acc[n] = slot_p[n * Cfg::ACC_LD];
+        ptx::mbar_arrive(ptx::smem_u32(sh.acc_empty + ab));
+        const int j = col0 + ct;
+        if (j < M) {
 #pragma unroll
-                  for (int hrow = 0; hrow < 2; ++hrow) {
-                    const int n = qrow + 8 * hrow;
-                    if (n < p.R) {
-                      float* orow = o + (size_t)n * ldo + col;
-                      if (col < M) atomicAdd(orow, __uint_as_float(va[4 * i + 2 * hrow]) + __uint_as_float(vb[4 * i + 2 * hrow]));
-                      if (col + 1 < M) atomicAdd(orow + 1, __uint_as_float(va[4 * i + 2 * hrow + 1]) + __uint_as_float(vb[4 * i + 2 * hrow + 1]));
-                    }
-                  }
-                }
-              }
-            }
-            continue;
-          }
-          const bool vec = ((ldo & 3) == 0) && p.epi_mode == 0;
-#pragma unroll 1
-          for (int c0 = 0; c0 < 256; c0 += 64) {
-            uint32_t v[64];
-            tmem_ld64(tmem_base + ab * 256 + c0, v);
-            ptx::tmem_ld_wait();
-            if (c0 == 192) {                       // accumulator fully read: hand it back before the atomics
-              ptx::tc_fence_before();
-              __syncwarp();
-              if (lane == 0) ptx::mbar_arrive(ptx::smem_u32(sh.acc_empty + ab));
-            }
-            float* orow = o + (size_t)lane * ldo + col0 + c0;
-#pragma unroll
-            for (int j = 0; j < 64; j += 4) {
-              float f[4];
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const float hi = __uint_as_float(v[j + e]);
-                f[e] = hi + __shfl_down_sync(0xffffffffu, hi, RH);   // lane n + RH: the lo-half product of row n
-              }
-              if (lane < p.R) {
-                const int col = col0 + c0 + j;
-                if (vec && col + 3 < M) {
-                  red_add_v4(orow + j, f[0], f[1], f[2], f[3]);
-                } else {
-#pragma unroll
-                  for (int e = 0; e < 4; ++e)
-                    if (col + e < M) atomicAdd(orow + j + e, f[e]);
-                }
-              }
-            }
-          }
-        } else {
-          ptx::mbar_wait(ptx::smem_u32(sh.acc_full + ab), aph);
-          ptx::tc_fence_after();
-          uint32_t acc[NB];
-          const uint32_t ta = tmem_base + ((uint32_t)(32 * quad) << 16) + ab * NB;
-          ptx::tmem_ld16(ta, *reinterpret_cast<uint32_t(*)[16]>(&acc[0]));
-          if (NB == 32) ptx::tmem_ld16(ta + 16, *reinterpret_cast<uint32_t(*)[16]>(&acc[NB - 16]));
-          ptx::tmem_ld_wait();
-          ptx::tc_fence_before();
-          ptx::mbar_arrive(ptx::smem_u32(sh.acc_empty + ab));
-          const int j = col0 + 32 * quad + lane;
-          if (j < M) {
-#pragma unroll
-            for (int n = 0; n < RH; ++n)
-              if (n < p.R) atomicAdd(o + (size_t)n * ldo + j, __uint_as_float(acc[n]) + __uint_as_float(acc[RH + n]));
-          }
+          for (int n = 0; n < RH; ++n)
+            if (n < p.R) atomicAdd(o + (size_t)n * ldo + j, acc[n]);
         }
       }
     };
@@ -1580,12 +1475,6 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
     }
     // bookkeeping of the last draw (no further position to embed)
     if (p.fused) finish_sample(p.n_steps - 1);
-    ptx::tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
   }
 }
 

@@ -29,7 +29,7 @@ extern "C" int mvb_linear(const void* d_W, int32_t M, int32_t K, const float* d_
   if (K % 64 || R < 1 || R > 128) return mvb::set_error(MVB_ERR_UNSUPPORTED, "mvb_linear: K %% 64 == 0 and 1 <= R <= 128 required");
   const int Rpad = (R + 15) / 16 * 16;
   const int NB = Rpad * (split_lo ? 2 : 1);
-  int n_sm = 148, dev = 0;
+  int n_sm = 132, dev = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
   GemmPlan g = plan_gemm(M, K, NB, false, n_sm);

@@ -628,7 +628,7 @@ static int launch_conv_tc(mvb_mbd* h, cudaStream_t s, const ConvP& p, int widx, 
     }
   }
   const int n_cot = (p.Cout + 127) / 128;
-  k_mbd_tc_conv<<<dim3(t.n_ph * n_cot, (q.Ncols + 127) / 128), 256, TC_SMEM, s>>>(w.tmA, tBhi, tBlo, q);
+  k_mbd_tc_conv<<<dim3(t.n_ph * n_cot, (q.Ncols + 127) / 128), TC_THREADS, TC_SMEM, s>>>(w.tmA, tBhi, tBlo, q);
   MCK(cudaGetLastError());
   (void)w.K;
   return MVB_OK;

@@ -1,15 +1,15 @@
 // Tensor-core lowering of the wide multi-band-diffusion convolutions (csrc/mbd.cu): every Conv1d / ConvTranspose1d whose
-// input width is a multiple of 64 channels runs as a sum of shifted GEMMs on tcgen05,
+// input width is a multiple of 64 channels runs as a sum of shifted GEMMs on the tensor cores,
 //     out[co][n * ostride + ph] = bias[co] + emb[co] + resid[..] + sum_slot sum_ci  W_slot[co][ci] * F[n + shift_slot][col_slot + ci]
 // where F is the TIME-major copy of the layer input after its GroupNorm + ReLU (k_mbd_prep_t), split into two bf16 terms
 // F = hi + lo so the activations keep 16 mantissa bits, and W_slot is tap `slot` of the kernel repacked to bf16 [tap][Cout][Cin]
 // at create time (k_mbd_pack_w).  Zero padding of the convolution = TMA out-of-bounds fill (negative / past-the-end rows read
 // as zero), the stride-s convolution reads the same buffer through a [T/s][s * Cin] view, and the transposed convolution is
 // s output phases with two taps each.  One CTA = 128 output channels x 128 time columns: A tiles (weights, 16 KB) and the
-// two B tiles (hi, lo: 128 rows each, together the N = 256 UMMA operand) arrive by TMA into a 4-stage ring, one elected
-// thread issues 4 x tcgen05.mma (128 x 256 x 16) per 64-channel block, the fp32 accumulator lives in 256 TMEM columns and
-// four epilogue warps add hi + lo + bias, transpose 32 x 32 blocks through shared memory and add the residual / store
-// channel-major rows with the lanes along time (coalesced).
+// two B tiles (hi, lo: 128 rows each) arrive by TMA into a 4-stage ring; eight consumer warps own 16 output channels each
+// and run ldmatrix + mma.sync.m16n8k16 over all 128 columns, the hi and lo products accumulating into one fp32 register
+// tile.  The epilogue adds bias, transposes each warp's 16 x 128 block through shared memory (the drained ring) and adds
+// the residual / stores channel-major rows with the lanes along time (coalesced).
 //
 // Numerics: weights are rounded to bf16 (the reference's own convolutions run in TF32 under torch's cuDNN default
 // `allow_tf32=True`, 10-bit mantissa on BOTH operands); activations are exact to 2^-17; accumulation is fp32.
@@ -34,21 +34,23 @@ struct TcConvP {
 
 constexpr int TC_STAGES = 4;
 constexpr int TC_A_BYTES = 128 * 64 * 2, TC_B_BYTES = 256 * 64 * 2, TC_STAGE_BYTES = TC_A_BYTES + TC_B_BYTES;
-constexpr size_t TC_SMEM = 1024 + (size_t)TC_STAGES * TC_STAGE_BYTES + (2 * TC_STAGES + 1) * 8 + 64 + 4 * 32 * 33 * 4;   // + epilogue transpose tiles
+constexpr int TC_THREADS = 288;          // TMA producer warp + 8 consumer warps
+constexpr int TC_TP_LD = 128 + 4;        // epilogue transpose tile [16][TC_TP_LD] fp32 per consumer warp (inside the ring)
+constexpr size_t TC_SMEM = 1024 + (size_t)TC_STAGES * TC_STAGE_BYTES + 2 * TC_STAGES * 8 + 64;
+static_assert(8 * 16 * TC_TP_LD * 4 <= TC_STAGES * TC_STAGE_BYTES, "transpose tiles must fit in the ring");
 
 __device__ __forceinline__ void tc_tma3(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1, int c2) {
   asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
                ::"r"(dst), "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
 
-static __global__ void __launch_bounds__(256, 1)
+static __global__ void __launch_bounds__(TC_THREADS, 1)
 k_mbd_tc_conv(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmBhi,
               const __grid_constant__ CUtensorMap tmBlo, const TcConvP p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
   constexpr int S = TC_STAGES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)S * TC_STAGE_BYTES);   // full[S], empty[S], acc
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * S + 1);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)S * TC_STAGE_BYTES);   // full[S], empty[S]
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int n_cot = (p.M + 127) >> 7;
   const int ph = blockIdx.x / n_cot, cot = blockIdx.x - ph * n_cot;
@@ -59,22 +61,14 @@ k_mbd_tc_conv(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
   if (warp == 0 && lane == 0) {
     for (int s = 0; s < S; ++s) {
       ptx::mbar_init(ptx::smem_u32(bars + s), 1);
-      ptx::mbar_init(ptx::smem_u32(bars + S + s), 1);
+      ptx::mbar_init(ptx::smem_u32(bars + S + s), 8);   // one arrive per consumer warp
     }
-    ptx::mbar_init(ptx::smem_u32(bars + 2 * S), 1);
     ptx::fence_barrier_init();
     ptx::prefetch_tensormap(&tmA);
     ptx::prefetch_tensormap(&tmBhi);
     ptx::prefetch_tensormap(&tmBlo);
   }
-  if (warp == 2) {
-    ptx::tmem_alloc(ptx::smem_u32(tmem_slot), 256);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);
 
   if (warp == 0) {
     int slot = 0, kb = 0;
@@ -94,75 +88,76 @@ k_mbd_tc_conv(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
       __syncwarp();
       if (++kb == nkb) { kb = 0; ++slot; }
     }
-  } else if (warp == 1) {
-    const uint32_t idesc = ptx::umma_idesc_bf16(128, 256);
-    for (int it = 0; it < n_it; ++it) {
-      const int s = it % S;
-      const uint32_t par = (uint32_t)(it / S) & 1u;
-      ptx::mbar_wait(ptx::smem_u32(bars + s), par);
-      ptx::tc_fence_after();
-      uint8_t* st = smem + (size_t)s * TC_STAGE_BYTES;
-      const uint64_t ad = ptx::umma_desc_k_sw128(ptx::smem_u32(st));
-      const uint64_t bd = ptx::umma_desc_k_sw128(ptx::smem_u32(st + TC_A_BYTES));
-      if (ptx::elect_one()) {
-#pragma unroll
-        for (int k = 0; k < 4; ++k) ptx::umma_bf16(tmem_base, ad + 2 * k, bd + 2 * k, idesc, (uint32_t)((it | k) != 0));
-        ptx::umma_commit(ptx::smem_u32(bars + S + s));
-      }
-      __syncwarp();
-    }
-    if (ptx::elect_one()) ptx::umma_commit(ptx::smem_u32(bars + 2 * S));
-    __syncwarp();
-  } else if (warp >= 4) {
-    // Epilogue: each warp owns 32 accumulator lanes (output channels).  A 32 x 32 block goes TMEM -> registers (lane = channel)
-    // -> a padded smem tile -> global with lane = TIME, so that the residual reads and the stores are contiguous 128-byte rows
-    // instead of 32 scattered sectors per instruction (the channel-major activations have stride ldo between channels).
-    const int w4 = warp - 4;
-    const int co_w = cot * 128 + 32 * w4;               // first channel of this warp
-    const uint32_t tbase = tmem_base + ((uint32_t)(32 * w4) << 16);
-    float* tp = reinterpret_cast<float*>(tmem_slot + 4) + w4 * (32 * 33);
-    ptx::mbar_wait(ptx::smem_u32(bars + 2 * S), 0);
-    ptx::tc_fence_after();
-    if (co_w < p.M) {
-      const int co = co_w + lane;
-      float add = 0.f;
-      if (co < p.M) add = (p.bias ? p.bias[co] : 0.f) + (p.emb ? p.emb[co] : 0.f);
-      const int rows = min(32, p.M - co_w);
-      for (int c0 = 0; c0 < 128 && t0 + c0 < p.Ncols; c0 += 32) {
-        uint32_t hi[32], lo[32];
-        ptx::tmem_ld16(tbase + c0, *reinterpret_cast<uint32_t(*)[16]>(hi));
-        ptx::tmem_ld16(tbase + c0 + 16, *reinterpret_cast<uint32_t(*)[16]>(hi + 16));
-        ptx::tmem_ld16(tbase + 128 + c0, *reinterpret_cast<uint32_t(*)[16]>(lo));
-        ptx::tmem_ld16(tbase + 128 + c0 + 16, *reinterpret_cast<uint32_t(*)[16]>(lo + 16));
-        ptx::tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) tp[lane * 33 + i] = __uint_as_float(hi[i]) + __uint_as_float(lo[i]) + add;
-        __syncwarp();
-        const int n = t0 + c0 + lane;
-        if (n < p.Ncols) {
-          const size_t col = (size_t)n * p.ostride + ph;
-          // residual reads in batches of 8 rows: issued back to back, not one dependent load -> store pair per row
-          for (int r0 = 0; r0 < rows; r0 += 8) {
-            float rv[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const int r = min(r0 + j, rows - 1);
-              rv[j] = p.resid ? __ldg(p.resid + (size_t)(co_w + r) * p.ldo + col) : 0.f;
-            }
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              if (r0 + j < rows) p.out[(size_t)(co_w + r0 + j) * p.ldo + col] = tp[(r0 + j) * 33 + lane] + rv[j];
-          }
-        }
-        __syncwarp();
-      }
-    }
-    ptx::tc_fence_before();
+    return;
   }
-  __syncthreads();
-  if (warp == 2) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, 256);
+
+  // consumers: warp w owns output channels [16 (w - 1), 16 w) of the tile
+  const int w16 = 16 * (warp - 1);
+  const int q = lane >> 3, r8 = lane & 7;
+  float acc[16][4];
+#pragma unroll
+  for (int c = 0; c < 16; ++c)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) acc[c][e] = 0.f;
+  for (int it = 0; it < n_it; ++it) {
+    const int s = it % S;
+    ptx::mbar_wait(ptx::smem_u32(bars + s), (uint32_t)(it / S) & 1u);
+    const uint32_t st = ptx::smem_u32(smem + (size_t)s * TC_STAGE_BYTES);
+    const uint32_t bst = st + TC_A_BYTES;    // rows 0..127: hi terms, rows 128..255: lo terms
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      uint32_t a[4];
+      ldsm_x4(st + sw128_off(w16 + r8 + ((q & 1) << 3), 2 * kk + (q >> 1)), a);
+#pragma unroll
+      for (int g = 0; g < 8; ++g)
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+          uint32_t b[4];
+          ldsm_x4(bst + sw128_off(128 * half + 16 * g + r8 + ((q >> 1) << 3), 2 * kk + (q & 1)), b);
+          mma_bf16_16816(acc[2 * g], a, b[0], b[1]);
+          mma_bf16_16816(acc[2 * g + 1], a, b[2], b[3]);
+        }
+    }
+    __syncwarp();                          // every lane's fragment loads of this stage are done
+    if (lane == 0) ptx::mbar_arrive(ptx::smem_u32(bars + S + s));
+  }
+  // Epilogue: accumulator (lane holds channels w16 + lane/4 (+8), columns 8c + 2(lane%4) (+1)) -> padded smem tile in the
+  // drained ring -> global with lane = TIME, so that the residual reads and the stores are contiguous 128-byte rows
+  // instead of scattered sectors (the channel-major activations have stride ldo between channels).
+  asm volatile("bar.sync 1, 256;" ::: "memory");   // every consumer is done with the ring
+  float* tp = reinterpret_cast<float*>(smem) + (warp - 1) * (16 * TC_TP_LD);
+  const int co_w = cot * 128 + w16;               // first channel of this warp
+  if (co_w < p.M) {
+    const int rows = min(16, p.M - co_w);
+#pragma unroll
+    for (int h8 = 0; h8 < 2; ++h8) {
+      const int r = (lane >> 2) + 8 * h8, co = co_w + r;
+      const float add = co < p.M ? (p.bias ? p.bias[co] : 0.f) + (p.emb ? p.emb[co] : 0.f) : 0.f;
+#pragma unroll
+      for (int c = 0; c < 16; ++c) {
+        tp[r * TC_TP_LD + 8 * c + 2 * (lane & 3)] = acc[c][2 * h8] + add;
+        tp[r * TC_TP_LD + 8 * c + 2 * (lane & 3) + 1] = acc[c][2 * h8 + 1] + add;
+      }
+    }
+    __syncwarp();
+    for (int c0 = 0; c0 < 128 && t0 + c0 < p.Ncols; c0 += 32) {
+      const int n = t0 + c0 + lane;
+      if (n < p.Ncols) {
+        const size_t col = (size_t)n * p.ostride + ph;
+        // residual reads in batches of 8 rows: issued back to back, not one dependent load -> store pair per row
+        for (int r0 = 0; r0 < rows; r0 += 8) {
+          float rv[8];
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const int r = min(r0 + j, rows - 1);
+            rv[j] = p.resid ? __ldg(p.resid + (size_t)(co_w + r) * p.ldo + col) : 0.f;
+          }
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            if (r0 + j < rows) p.out[(size_t)(co_w + r0 + j) * p.ldo + col] = tp[(r0 + j) * TC_TP_LD + c0 + lane] + rv[j];
+        }
+      }
+    }
   }
 }
 

@@ -107,7 +107,7 @@ static WsLayout make_layout(const mvb_s1_config& c) {
     size_t sc = 0;
     const size_t mats[5][3] = {{3 * D, D, 1}, {D, D, 1}, {F, D, 2}, {D, F, 1}, {V, D, 1}};
     for (auto& m : mats) {
-      GemmPlan g = plan_gemm((int)m[0], (int)m[1], (int)NBM, m[2] == 2, 148);
+      GemmPlan g = plan_gemm((int)m[0], (int)m[1], (int)NBM, m[2] == 2, 132);
       if (g.scratch_floats > sc) sc = g.scratch_floats;
     }
     L.b_scratch = take(sc * 4);
@@ -132,7 +132,7 @@ static WsLayout make_layout(const mvb_s1_config& c) {
 
 struct mvb_s1 {
   mvb_s1_config cfg;
-  int n_sm = 148;
+  int n_sm = 132;
   const char* arena = nullptr;
   std::vector<uint64_t> off;
   char* kv = nullptr;
@@ -157,15 +157,13 @@ struct mvb_s1 {
   bool path_c = true;
   bool pc_ok = false;
   bool trace = false;
-  // persistent-kernel switches, read once at create (MVB_PC_WB, MVB_PC_FUSED, MVB_PF_MODE, MVB_PF_AHEAD)
-  bool wb = false;                                    // streamed weights as the N = 256 UMMA B operand (measured slower: off)
+  // persistent-kernel switches, read once at create (MVB_PC_FUSED, MVB_PF_MODE, MVB_PF_AHEAD)
   bool fused = true;                                  // sample inside the persistent kernel (multi-token launches)
-  int pf_mode = 1, pf_ahead = 8, epi_mode = 2, kv_pf = 0;
+  int pf_mode = 1, pf_ahead = 8, kv_pf = 0;
   int att_mma = 1;                                    // bf16 cache: attention on mma.sync over TMA-swizzled KV tiles (MVB_PC_ATT_MMA=0: scalar)
   CUtensorMap tm_kv;                                  // 2-D map over the whole bf16 KV arena: [rows = layer, k|v, cache row, head, pos][128]
-  CUtensorMap tm3[2][6];                              // [WB] 3-D (k, row, layer) maps: wqkv, wo, w1, w3, w2, head
-  PcMat pm[2][5];
-  bool pc_ok2[2] = {false, false};
+  CUtensorMap tm3[6];                                 // 3-D (k, row, layer) maps: wqkv, wo, w1, w3, w2, head
+  PcMat pm[5];
   std::vector<int> h_topk;                            // top_k of every utterance slot as installed by mvb_s1_begin
   size_t layer_stride_elems = 0;
 
@@ -191,10 +189,9 @@ static PcMat plan_pc(int M, int K, int ctas, int tile_rows, int force_S = 0) {
     const int tiles_per = (T + Gp - 1) / Gp;
     const int kb_per = (KB + S - 1) / S;
     if (kb_per > PC_BKB_MAX) continue;
-    // Cost of a phase in tile-load units (fitted on B200, profiles/r2_step_time_ksplit_sweep.jsonl): every tile a CTA owns
-    // costs its k-blocks plus ~2.5 for the accumulator drain (tcgen05.ld + red.add), and staging the activation operand
-    // costs ~2 per k-block of the CTA's K slice (one dependent L2 round trip per 256 chunks).  The round-1 cost
-    // (tiles x k-blocks only) chose 3 / 8 / 8 / 9 splits for qkv / wo / w1|w3 / w2; this one chooses 8 / 16 / 8 / 22.
+    // Cost of a phase in tile-load units: every tile a CTA owns costs its k-blocks plus ~2.5 for the accumulator drain
+    // (slot loads + red.add), and staging the activation operand costs ~2 per k-block of the CTA's K slice (one
+    // dependent L2 round trip per 256 chunks).
     const long cost = (long)tiles_per * (2 * kb_per + 5) + 4 * kb_per;
     if (best_cost < 0 || cost < best_cost) {
       best_cost = cost;
@@ -240,7 +237,7 @@ extern "C" int mvb_s1_create(const mvb_s1_config* cfg, const void* d_arena, size
   CK(cudaGetDevice(&dev));
   CK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
   CK(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
-  if (major != 10) return fail(MVB_ERR_UNSUPPORTED, "libmvb200 is built for sm_100a only; device is sm_%d%d", major, minor);
+  if (major != 9 || minor != 0) return fail(MVB_ERR_UNSUPPORTED, "libmvb200 is built for sm_90a only; device is sm_%d%d", major, minor);
   struct Guard {   // frees the half-built handle on every early return below
     mvb_s1* h;
     ~Guard() { if (h) mvb_s1_destroy(h); }
@@ -298,7 +295,6 @@ extern "C" int mvb_s1_create(const mvb_s1_config* cfg, const void* d_arena, size
   if (const char* e = getenv("MVB_PC_TRACE")) h->trace = atoi(e) != 0;
   if (const char* e = getenv("MVB_PF_AHEAD")) h->pf_ahead = atoi(e);
   if (const char* e = getenv("MVB_PF_MODE")) h->pf_mode = atoi(e);
-  if (const char* e = getenv("MVB_PC_EPI")) h->epi_mode = atoi(e);
   if (const char* e = getenv("MVB_PC_KVPF")) h->kv_pf = atoi(e);
   if (const char* e = getenv("MVB_PC_ATT_MMA")) h->att_mma = atoi(e);
   memset(&h->tm_kv, 0, sizeof(h->tm_kv));
@@ -317,7 +313,6 @@ extern "C" int mvb_s1_create(const mvb_s1_config* cfg, const void* d_arena, size
            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
       h->att_mma = 0;
   }
-  if (const char* e = getenv("MVB_PC_WB")) h->wb = atoi(e) != 0;
   if (const char* e = getenv("MVB_PC_FUSED")) h->fused = atoi(e) != 0;
   h->h_topk.assign(cfg->max_utts, 0);
   {
@@ -332,37 +327,29 @@ extern "C" int mvb_s1_create(const mvb_s1_config* cfg, const void* d_arena, size
     ok = ok && (stride % 16 == 0);
     h->layer_stride_elems = stride / 2;
     const uint64_t NL = cfg->n_layer;
-    for (int wbv = 0; wbv < 2; ++wbv) {
-      const int rows = wbv ? 256 : 128;
-      bool okv = ok;
-      okv = okv && make_tmap_bf16_3d(&h->tm3[wbv][0], h->lw(0, 1), D, 3 * D, NL, stride, rows);
-      okv = okv && make_tmap_bf16_3d(&h->tm3[wbv][1], h->lw(0, 2), D, D, NL, stride, rows);
-      okv = okv && make_tmap_bf16_3d(&h->tm3[wbv][2], h->lw(0, 4), D, F, NL, stride, rows);
-      okv = okv && make_tmap_bf16_3d(&h->tm3[wbv][3], h->lw(0, 5), D, F, NL, stride, rows);
-      okv = okv && make_tmap_bf16_3d(&h->tm3[wbv][4], h->lw(0, 6), F, D, NL, stride, rows);
-      okv = okv && make_tmap_bf16_3d(&h->tm3[wbv][5], h->w(4), D, V, 1, (uint64_t)V * D * 2, rows);
-      int fs[5] = {0, 0, 0, 0, 0};               // MVB_PC_SPLITS="q_o_w13_w2_head": force the K split of a matrix (0 = planner)
-      if (const char* e = getenv("MVB_PC_SPLITS")) sscanf(e, "%d_%d_%d_%d_%d", &fs[0], &fs[1], &fs[2], &fs[3], &fs[4]);
-      h->pm[wbv][0] = plan_pc(3 * D, D, h->n_sm, rows, fs[0]);
-      h->pm[wbv][1] = plan_pc(D, D, h->n_sm, rows, fs[1]);
-      h->pm[wbv][2] = plan_pc(2 * F, D, h->n_sm, rows, fs[2]);
-      h->pm[wbv][3] = plan_pc(D, F, h->n_sm, rows, fs[3]);
-      h->pm[wbv][4] = plan_pc(V, D, h->n_sm, rows, fs[4]);
-      for (int i = 0; i < 5; ++i) okv = okv && h->pm[wbv][i].S > 0;
-      okv = okv && (F % rows == 0) && (D % rows == 0);     // w1 | w3 share one tile index space: F must be whole tiles
-      h->pc_ok2[wbv] = okv;
-    }
-    if (!h->pc_ok2[1]) h->wb = false;
-    ok = h->pc_ok2[h->wb ? 1 : 0];
+    const int rows = PcCfg<16>::TILE_ROWS;
+    ok = ok && make_tmap_bf16_3d(&h->tm3[0], h->lw(0, 1), D, 3 * D, NL, stride, rows);
+    ok = ok && make_tmap_bf16_3d(&h->tm3[1], h->lw(0, 2), D, D, NL, stride, rows);
+    ok = ok && make_tmap_bf16_3d(&h->tm3[2], h->lw(0, 4), D, F, NL, stride, rows);
+    ok = ok && make_tmap_bf16_3d(&h->tm3[3], h->lw(0, 5), D, F, NL, stride, rows);
+    ok = ok && make_tmap_bf16_3d(&h->tm3[4], h->lw(0, 6), F, D, NL, stride, rows);
+    ok = ok && make_tmap_bf16_3d(&h->tm3[5], h->w(4), D, V, 1, (uint64_t)V * D * 2, rows);
+    int fs[5] = {0, 0, 0, 0, 0};               // MVB_PC_SPLITS="q_o_w13_w2_head": force the K split of a matrix (0 = planner)
+    if (const char* e = getenv("MVB_PC_SPLITS")) sscanf(e, "%d_%d_%d_%d_%d", &fs[0], &fs[1], &fs[2], &fs[3], &fs[4]);
+    h->pm[0] = plan_pc(3 * D, D, h->n_sm, rows, fs[0]);
+    h->pm[1] = plan_pc(D, D, h->n_sm, rows, fs[1]);
+    h->pm[2] = plan_pc(2 * F, D, h->n_sm, rows, fs[2]);
+    h->pm[3] = plan_pc(D, F, h->n_sm, rows, fs[3]);
+    h->pm[4] = plan_pc(V, D, h->n_sm, rows, fs[4]);
+    for (int i = 0; i < 5; ++i) ok = ok && h->pm[i].S > 0;
+    ok = ok && (F % rows == 0) && (D % rows == 0);     // w1 | w3 share one tile index space: F must be whole tiles
     h->pc_ok = ok;
   }
   // Opt-in shared-memory size is a per-device function attribute: set it for the device this handle lives on
   // (a process may hold engines on several GPUs).
-#define MVB_PC_ATTR(FP, NBV, WBV)                                                                                   \
-  CK(cudaFuncSetAttribute(k_decode_persistent<FP, NBV, WBV>, cudaFuncAttributeMaxDynamicSharedMemorySize,           \
-                          (int)PcCfg<NBV, WBV>::SMEM))
-  MVB_PC_ATTR(true, 32, false); MVB_PC_ATTR(true, 16, false); MVB_PC_ATTR(false, 32, false); MVB_PC_ATTR(false, 16, false);
-  MVB_PC_ATTR(true, 32, true); MVB_PC_ATTR(true, 16, true); MVB_PC_ATTR(false, 32, true); MVB_PC_ATTR(false, 16, true);
+#define MVB_PC_ATTR(FP, NBV)                                                                                        \
+  CK(cudaFuncSetAttribute(k_decode_persistent<FP, NBV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PcCfg<NBV>::SMEM))
+  MVB_PC_ATTR(true, 32); MVB_PC_ATTR(true, 16); MVB_PC_ATTR(false, 32); MVB_PC_ATTR(false, 16);
 #undef MVB_PC_ATTR
   CK(cudaStreamCreateWithFlags(&h->cap_stream, cudaStreamNonBlocking));
   CK(cudaMallocHost(&h->h_flags, sizeof(int) * 4 * 64));
@@ -563,13 +550,12 @@ static int launch_body_b(mvb_s1* h, cudaStream_t s, int n_utts) {
 // Path C: one persistent kernel per decode position (decode_persistent.cuh) followed by the sampler.
 static int launch_persistent(mvb_s1* h, cudaStream_t s, int n_utts, int n_steps, bool fused) {
   const mvb_s1_config& c = h->cfg;
-  const int wbv = h->wb ? 1 : 0;
   PcParams p{};
   p.n_layer = c.n_layer; p.D = c.dim; p.F = c.intermediate; p.V = c.vocab; p.H = c.n_head; p.S_max = c.block_size;
   p.n_steps = n_steps; p.fused = fused ? 1 : 0;
-  p.pf_mode = h->pf_mode; p.pf_ahead = h->pf_ahead; p.epi_mode = h->epi_mode; p.kv_pf = h->kv_pf;
+  p.pf_mode = h->pf_mode; p.pf_ahead = h->pf_ahead; p.kv_pf = h->kv_pf;
   p.R = 2 * n_utts; p.n_utts = n_utts; p.kv_fp32 = c.kv_dtype == MVB_KV_FP32; p.eps = c.norm_eps;
-  p.m_qkv = h->pm[wbv][0]; p.m_o = h->pm[wbv][1]; p.m_w13 = h->pm[wbv][2]; p.m_w2 = h->pm[wbv][3]; p.m_head = h->pm[wbv][4];
+  p.m_qkv = h->pm[0]; p.m_o = h->pm[1]; p.m_w13 = h->pm[2]; p.m_w2 = h->pm[3]; p.m_head = h->pm[4];
   p.attn_norm = h->lw(0, 0); p.ffn_norm = h->lw(0, 3); p.out_norm = h->w(3);
   p.layer_stride = h->layer_stride_elems;
   p.tok_emb = h->w(0); p.pos_emb = h->w(1); p.spk_proj = h->wsp<float>(h->L.spk);
@@ -590,21 +576,14 @@ static int launch_persistent(mvb_s1* h, cudaStream_t s, int n_utts, int n_steps,
   CK(cudaMemsetAsync(p.samp_best, 0, sizeof(unsigned long long) * 2 * (PC_RPAD / 2), s));
   h->launches++;
   const bool fp = p.kv_fp32 != 0, wide = p.R > 8;
-  const CUtensorMap* tm = h->tm3[wbv];
-#define MVB_PC_LAUNCH(FP, NBV, WBV)                                                                                   \
-  CK(launch_pdl(h->pdl, k_decode_persistent<FP, NBV, WBV>, dim3(h->n_sm), dim3(PC_THREADS), PcCfg<NBV, WBV>::SMEM, s, \
+  const CUtensorMap* tm = h->tm3;
+#define MVB_PC_LAUNCH(FP, NBV)                                                                                        \
+  CK(launch_pdl(h->pdl, k_decode_persistent<FP, NBV>, dim3(h->n_sm), dim3(PC_THREADS), PcCfg<NBV>::SMEM, s,           \
                 tm[0], tm[1], tm[2], tm[3], tm[4], tm[5], h->tm_kv, p))
-  if (wbv) {
-    if (fp && wide) MVB_PC_LAUNCH(true, 32, true);
-    else if (fp) MVB_PC_LAUNCH(true, 16, true);
-    else if (wide) MVB_PC_LAUNCH(false, 32, true);
-    else MVB_PC_LAUNCH(false, 16, true);
-  } else {
-    if (fp && wide) MVB_PC_LAUNCH(true, 32, false);
-    else if (fp) MVB_PC_LAUNCH(true, 16, false);
-    else if (wide) MVB_PC_LAUNCH(false, 32, false);
-    else MVB_PC_LAUNCH(false, 16, false);
-  }
+  if (fp && wide) MVB_PC_LAUNCH(true, 32);
+  else if (fp) MVB_PC_LAUNCH(true, 16);
+  else if (wide) MVB_PC_LAUNCH(false, 32);
+  else MVB_PC_LAUNCH(false, 16);
 #undef MVB_PC_LAUNCH
   return MVB_OK;
 }

@@ -223,7 +223,7 @@ __global__ void __launch_bounds__(256) k_s2_sample(const float* __restrict__ log
 
 struct mvb_s2 {
   mvb_s2_config cfg;
-  int n_sm = 148, hidden = 0;
+  int n_sm = 132, hidden = 0;
   const char* arena = nullptr;
   std::vector<uint64_t> off;
   char* ws = nullptr;
@@ -273,7 +273,7 @@ static size_t s2_layout(const mvb_s2_config* c, size_t* o_x, size_t* o_qkv, size
   size_t sc = 0;
   const size_t mats[5][3] = {{3 * E, E, 1}, {E, E, 1}, {Hd, E, 2}, {E, Hd, 1}, {vmax, E, 1}};
   for (auto& m : mats) {
-    GemmPlan g = plan_gemm((int)m[0], (int)m[1], 2 * S2_ROWS, m[2] == 2, 148);
+    GemmPlan g = plan_gemm((int)m[0], (int)m[1], 2 * S2_ROWS, m[2] == 2, 132);
     sc = sc > g.scratch_floats ? sc : g.scratch_floats;
   }
   *o_scratch = take(sc * 4);

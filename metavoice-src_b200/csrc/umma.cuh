@@ -1,6 +1,5 @@
-// Raw sm_100a building blocks: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (UMMA + TMEM).
-// Hand-written inline PTX; descriptor bit layouts follow the PTX ISA "tcgen05 matrix descriptors"
-// (cross-checked against cute/arch/mma_sm100_desc.hpp field tables).
+// Raw sm_90a building blocks: mbarrier, TMA (cp.async.bulk.tensor), ldmatrix + mma.sync on 128B-swizzled tiles.
+// Hand-written inline PTX (fragment layouts: PTX ISA, ldmatrix and mma.m16n8k16).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -90,81 +89,6 @@ __device__ __forceinline__ uint64_t policy_evict_last() {
   return p;
 }
 
-// ---- TMEM -------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// 32 lanes x 16 consecutive 32-bit columns: thread t of warp w reads TMEM lane 32*(w%4)+t.
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---- UMMA -------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor for a K-major bf16 tile stored as [rows][64] (128 B per row) with the
-// 128-byte swizzle TMA writes (CU_TENSOR_MAP_SWIZZLE_128B); tile base must be 1024-byte aligned.
-//   [0,14) start>>4 | [16,30) LBO>>4 (=1, unused for swizzled K-major) | [32,46) SBO>>4 (= 8 rows * 128 B)
-//   [46,48) version = 1 (sm_100) | [49,52) base offset = 0 | [61,64) layout = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
-  const uint64_t lo = (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16);
-  const uint64_t hi = (uint64_t)(1024u >> 4) | (1ull << 14) | (2ull << 29);
-  return lo | (hi << 32);
-}
-// Same, for a tile stored as [rows][16] bf16 (32 B per row, one UMMA K step) with the 32-byte swizzle
-// (CU_TENSOR_MAP_SWIZZLE_32B): 8-row groups are 256 B apart, so one MMA reads a dense 4 KB block.
-__device__ __forceinline__ uint64_t umma_desc_k_sw32(uint32_t smem_addr) {
-  const uint64_t lo = (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16);
-  const uint64_t hi = (uint64_t)(256u >> 4) | (1ull << 14) | (6ull << 29);
-  return lo | (hi << 32);
-}
-// Instruction descriptor: D=f32, A=B=bf16, both K-major, shape M x N x 16.
-//   [4,6) D fmt (1=f32) | [7,10) A fmt (1=bf16) | [10,13) B fmt | bit15/16 majors (0=K) | [17,23) N>>3 | [24,29) M>>4
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread on behalf of the CTA.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Same, with the A operand (M x 16 bf16: lane = row, 8 packed 32-bit columns) read from tensor memory.
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Copy a 128-row x 256-bit matrix (one K = 16 bf16 slice of a K-major tile, same smem descriptor as the UMMA A
-// operand) from shared memory into tensor memory: lane = row, 8 consecutive columns.  Asynchronous; ordered with the
-// tcgen05.mma / tcgen05.commit instructions issued by the same thread.
-__device__ __forceinline__ void tmem_cp_128x256b(uint32_t taddr, uint64_t sdesc) {
-  asm volatile("tcgen05.cp.cta_group::1.128x256b [%0], %1;" ::"r"(taddr), "l"(sdesc) : "memory");
-}
-// Arrive on an mbarrier when all previously issued UMMAs of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -176,4 +100,22 @@ __device__ __forceinline__ bool elect_one() {
 }
 
 }  // namespace ptx
+
+__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr) : "memory");
+}
+__device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
+}
+
+// D[16x8] += A[16x16] * B[16x8], bf16 operands, fp32 accumulate (fragment layouts: PTX ISA, mma.m16n8k16)
+__device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
+// byte offset of 16-byte chunk `ch` of row `row` in a K-major tile of 128-byte rows written with the 128B swizzle
+// (TMA CU_TENSOR_MAP_SWIZZLE_128B / b_chunk_off; the tile base is 1024-byte aligned)
+__device__ __forceinline__ uint32_t sw128_off(int row, int ch) { return (uint32_t)(row * 128 + ((ch ^ (row & 7)) << 4)); }
+
 }  // namespace mvb

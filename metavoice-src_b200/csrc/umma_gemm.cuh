@@ -1,19 +1,19 @@
-// Weight-streaming skinny GEMM on the 5th-gen tensor cores ("path B"): Y[n, j] = sum_k X[n, k] * W[j, k].
+// Weight-streaming skinny GEMM on the tensor cores ("path B"): Y[n, j] = sum_k X[n, k] * W[j, k].
 //
 // The projection weights are the big operand (W[M, K] bf16, row-major = K-major), the activations the
-// skinny one (N <= 256 rows), so the roles are swapped with respect to a textbook GEMM: a 128-row tile
-// of W is the UMMA "A" operand (M = 128), the activation rows are the "B" operand (N = padded row
-// count), and the fp32 accumulator D[128, N] lives in TMEM.  Weights go HBM -> TMA -> 128B-swizzled
-// shared memory -> tcgen05.mma without ever touching registers; one elected thread issues the MMAs.
+// skinny one (R <= 128 rows), so the roles are swapped with respect to a textbook GEMM: a 128-row tile
+// of W is the MMA "A" operand, the activation rows are the "B" operand.  Weights go HBM -> TMA ->
+// 128B-swizzled shared memory -> ldmatrix -> mma.sync.m16n8k16 with fp32 accumulators in registers.
 //
 // Precision: weights are exactly bf16; activations are split x = hi + lo (two bf16 terms, 16 mantissa
-// bits) and both terms ride along as extra B rows, so the product matches an fp32-activation GEMM to
-// ~1e-5 while the MMA count stays irrelevant (the kernel is HBM-bound on W).
+// bits); the lo rows follow the hi rows in the B buffer and both products go into the same accumulator,
+// so the product matches an fp32-activation GEMM to ~1e-5 while the MMA count stays irrelevant (the
+// kernel is HBM-bound on W).
 //
-// Warp roles (256 threads): warp 0 = TMA producer, warp 1 = MMA issuer, warp 2 = TMEM allocator,
-// warps 4..7 = epilogue (tcgen05.ld -> registers -> fused epilogue).  grid = (row tiles, K splits);
-// split-K partial tiles go through a scratch buffer and the last-arriving split reduces them in a fixed
-// order (deterministic), then applies the operator epilogue.
+// Warp roles (288 threads): warp 0 = TMA producer, warps 1..8 = consumers; consumer w owns weight rows
+// [16 (w - 1), 16 w) of the tile and every activation row, and runs the fused epilogue straight from its
+// registers.  grid = (row tiles, K splits); split-K partial tiles go through a scratch buffer, every split
+// of a tile reduces its share of the rows in a fixed order (deterministic), then applies the operator epilogue.
 #pragma once
 #include "common.cuh"
 #include "umma.cuh"
@@ -24,13 +24,13 @@ enum { G_STORE = 0, G_RESID = 1, G_SWIGLU = 2, G_QKV = 3 };
 
 struct GemmP {
   int M, K;        // weight matrix [M, K]
-  int NB;          // UMMA N = rows of the B buffer = Rpad * (1 + split_lo); multiple of 16, <= 256
-  int Rpad;        // rows reserved for the hi terms (multiple of 16)
+  int NB;          // rows of the B buffer = Rpad * (1 + split_lo)
+  int Rpad;        // rows reserved for the hi terms (multiple of 16, <= 128)
   int R;           // real activation rows (<= Rpad)
   int split_lo;    // 1: rows [Rpad, 2*Rpad) of B hold the lo terms
   int ksplit;      // gridDim.y
   int stages;      // smem ring depth
-  float* scratch;  // [tiles][ksplit][ncols][128] fp32 partial tiles (ksplit > 1)
+  float* scratch;  // [tiles][ksplit][(1 + swiglu) * Rpad][128] fp32 partial tiles (ksplit > 1)
   unsigned* tickets;  // [256]: arrivals per tile in [0, 128), completions per tile in [128, 256)
   float* out;
   int ldo;
@@ -43,6 +43,7 @@ struct GemmP {
 };
 
 constexpr int GEMM_A_BYTES = 128 * 64 * 2;  // one 128-row x 64-k bf16 tile
+constexpr int GEMM_THREADS = 288;
 
 template <int EPI>
 __device__ __forceinline__ void gemm_apply(const GemmP& p, int n, int j, float y, float y3) {
@@ -68,8 +69,9 @@ __device__ __forceinline__ void gemm_apply(const GemmP& p, int n, int j, float y
   }
 }
 
-template <int EPI>
-__global__ void __launch_bounds__(256, 1)
+// NC = n8 column chunks the accumulator holds (>= Rpad / 8; the chunks past Rpad / 8 are skipped at run time)
+template <int EPI, int NC>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
 k_umma_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA3,
             const __grid_constant__ CUtensorMap tmB, const GemmP p) {
   constexpr int NA = (EPI == G_SWIGLU) ? 2 : 1;
@@ -80,8 +82,7 @@ k_umma_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   const int S = p.stages;
   const int b_bytes = p.NB * 128;
   const int stage_bytes = NA * GEMM_A_BYTES + b_bytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)S * stage_bytes);  // full[S], empty[S], acc_full
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * S + 1);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)S * stage_bytes);  // full[S], empty[S]
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int tile = blockIdx.x, split = blockIdx.y;
@@ -89,186 +90,143 @@ k_umma_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   const int kb0 = (int)(((long long)split * nkb) / p.ksplit);
   const int kb1 = (int)(((long long)(split + 1) * nkb) / p.ksplit);
   const int n_it = kb1 - kb0;
-  const int ncols = NA * p.NB;
-  uint32_t ncols_alloc = 32;
-  while ((int)ncols_alloc < ncols) ncols_alloc <<= 1;
 
   if (warp == 0 && lane == 0) {
     for (int s = 0; s < S; ++s) {
       ptx::mbar_init(ptx::smem_u32(bars + s), 1);
-      ptx::mbar_init(ptx::smem_u32(bars + S + s), 1);
+      ptx::mbar_init(ptx::smem_u32(bars + S + s), 8);   // one arrive per consumer warp
     }
-    ptx::mbar_init(ptx::smem_u32(bars + 2 * S), 1);
     ptx::fence_barrier_init();
     ptx::prefetch_tensormap(&tmA);
     ptx::prefetch_tensormap(&tmB);
     if (NA == 2) ptx::prefetch_tensormap(&tmA3);
   }
-  if (warp == 2) {
-    ptx::tmem_alloc(ptx::smem_u32(tmem_slot), ncols_alloc);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);   // provably warp-uniform (see decode_persistent.cuh)
 
   if (warp == 0) {
     // ===== TMA producer: the whole warp walks the loop (uniform operands), one elected lane issues =====
-    {
-      const uint64_t pol_w = ptx::policy_evict_first();  // weights are streamed exactly once per pass
-      for (int it = 0; it < n_it; ++it) {
-        const int s = it % S;
-        const uint32_t ph = (uint32_t)(it / S) & 1u;
-        ptx::mbar_wait(ptx::smem_u32(bars + S + s), ph ^ 1u);
-        if (ptx::elect_one()) {
-          const uint32_t full = ptx::smem_u32(bars + s);
-          ptx::mbar_arrive_expect_tx(full, (uint32_t)stage_bytes);
-          uint8_t* st = smem + (size_t)s * stage_bytes;
-          const int kc = (kb0 + it) * 64;
-          ptx::tma_load_2d_hint(ptx::smem_u32(st), &tmA, full, kc, tile * 128, pol_w);
-          if (NA == 2) ptx::tma_load_2d_hint(ptx::smem_u32(st + GEMM_A_BYTES), &tmA3, full, kc, tile * 128, pol_w);
-          ptx::tma_load_2d(ptx::smem_u32(st + NA * GEMM_A_BYTES), &tmB, full, kc, 0);
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp == 1) {
-    // ===== MMA issuer: warp-uniform loop, one elected lane issues (a lane-0 branch costs ~40 cycles per UMMA) =====
-    {
-      const uint32_t idesc = ptx::umma_idesc_bf16(128, p.NB);
-      for (int it = 0; it < n_it; ++it) {
-        const int s = it % S;
-        const uint32_t ph = (uint32_t)(it / S) & 1u;
-        ptx::mbar_wait(ptx::smem_u32(bars + s), ph);
-        ptx::tc_fence_after();
+    const uint64_t pol_w = ptx::policy_evict_first();  // weights are streamed exactly once per pass
+    for (int it = 0; it < n_it; ++it) {
+      const int s = it % S;
+      const uint32_t ph = (uint32_t)(it / S) & 1u;
+      ptx::mbar_wait(ptx::smem_u32(bars + S + s), ph ^ 1u);
+      if (ptx::elect_one()) {
+        const uint32_t full = ptx::smem_u32(bars + s);
+        ptx::mbar_arrive_expect_tx(full, (uint32_t)stage_bytes);
         uint8_t* st = smem + (size_t)s * stage_bytes;
-        const uint64_t ad = ptx::umma_desc_k_sw128(ptx::smem_u32(st));
-        const uint64_t bd = ptx::umma_desc_k_sw128(ptx::smem_u32(st + NA * GEMM_A_BYTES));
-        const uint64_t a3 = ptx::umma_desc_k_sw128(ptx::smem_u32(st + GEMM_A_BYTES));
-        if (ptx::elect_one()) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k)  // 4 x (K = 16) per 64-wide k-block: +32 B along K inside the swizzle atom
-            ptx::umma_bf16(tmem_base, ad + 2 * k, bd + 2 * k, idesc, (uint32_t)((it | k) != 0));
-          if (NA == 2) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              ptx::umma_bf16(tmem_base + (uint32_t)p.NB, a3 + 2 * k, bd + 2 * k, idesc, (uint32_t)((it | k) != 0));
-          }
-          ptx::umma_commit(ptx::smem_u32(bars + S + s));  // frees the smem stage when these MMAs retire
-        }
-        __syncwarp();
+        const int kc = (kb0 + it) * 64;
+        ptx::tma_load_2d_hint(ptx::smem_u32(st), &tmA, full, kc, tile * 128, pol_w);
+        if (NA == 2) ptx::tma_load_2d_hint(ptx::smem_u32(st + GEMM_A_BYTES), &tmA3, full, kc, tile * 128, pol_w);
+        ptx::tma_load_2d(ptx::smem_u32(st + NA * GEMM_A_BYTES), &tmB, full, kc, 0);
       }
-      if (ptx::elect_one()) ptx::umma_commit(ptx::smem_u32(bars + 2 * S));     // accumulator complete
       __syncwarp();
     }
-  } else if (warp >= 4) {
-    // ===== epilogue: TMEM -> registers -> (split-K reduce) -> fused operator epilogue =====
-    const int w4 = warp - 4;
-    const int row_local = 32 * w4 + lane;
-    const int j = tile * 128 + row_local;
-    const uint32_t tbase = tmem_base + ((uint32_t)(32 * w4) << 16);
-    ptx::mbar_wait(ptx::smem_u32(bars + 2 * S), 0);
-    ptx::tc_fence_after();
-    if (p.ksplit == 1) {
-      for (int c0 = 0; c0 < p.Rpad; c0 += 16) {
-        uint32_t hi[16], lo[16], hi3[16], lo3[16];
-        ptx::tmem_ld16(tbase + c0, hi);
-        if (p.split_lo) ptx::tmem_ld16(tbase + p.Rpad + c0, lo);
-        if (NA == 2) {
-          ptx::tmem_ld16(tbase + p.NB + c0, hi3);
-          if (p.split_lo) ptx::tmem_ld16(tbase + p.NB + p.Rpad + c0, lo3);
-        }
-        ptx::tmem_ld_wait();
+    return;
+  }
+
+  // ===== consumers: ldmatrix + mma.sync into registers, then the epilogue =====
+  const int ct = tid - 32;                 // 0..255
+  const int w16 = 16 * (warp - 1);         // first weight row of this warp inside the tile
+  const int q = lane >> 3, r8 = lane & 7;
+  const int nc = p.Rpad >> 3;
+  float acc[NA][NC][4];
 #pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const int n = c0 + i;
-          if (n < p.R && j < p.M) {
-            float y = __uint_as_float(hi[i]);
-            if (p.split_lo) y += __uint_as_float(lo[i]);
-            float y3 = 0.f;
-            if (NA == 2) {
-              y3 = __uint_as_float(hi3[i]);
-              if (p.split_lo) y3 += __uint_as_float(lo3[i]);
-            }
-            gemm_apply<EPI>(p, n, j, y, y3);
+  for (int a = 0; a < NA; ++a)
+#pragma unroll
+    for (int c = 0; c < NC; ++c)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) acc[a][c][e] = 0.f;
+  for (int it = 0; it < n_it; ++it) {
+    const int s = it % S;
+    ptx::mbar_wait(ptx::smem_u32(bars + s), (uint32_t)(it / S) & 1u);
+    const uint32_t st = ptx::smem_u32(smem + (size_t)s * stage_bytes);
+    const uint32_t bst = st + NA * GEMM_A_BYTES;
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      uint32_t af[NA][4];
+      const int arow = w16 + r8 + ((q & 1) << 3);
+#pragma unroll
+      for (int a = 0; a < NA; ++a) ldsm_x4(st + a * GEMM_A_BYTES + sw128_off(arow, 2 * kk + (q >> 1)), af[a]);
+#pragma unroll
+      for (int g = 0; g < NC / 2; ++g) {
+        if (2 * g >= nc) break;
+        const int brow = 16 * g + r8 + ((q >> 1) << 3), bch = 2 * kk + (q & 1);
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {   // hi rows, then (split_lo) the lo rows into the same accumulator
+          if (half == 1 && !p.split_lo) break;
+          uint32_t b[4];
+          ldsm_x4(bst + sw128_off(half * p.Rpad + brow, bch), b);
+#pragma unroll
+          for (int a = 0; a < NA; ++a) {
+            mma_bf16_16816(acc[a][2 * g], af[a], b[0], b[1]);
+            mma_bf16_16816(acc[a][2 * g + 1], af[a], b[2], b[3]);
           }
-        }
-      }
-    } else {
-      float* mine = p.scratch + ((size_t)(tile * p.ksplit + split) * ncols) * 128;
-      for (int c0 = 0; c0 < ncols; c0 += 16) {
-        uint32_t v[16];
-        ptx::tmem_ld16(tbase + c0, v);
-        ptx::tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 16; ++i) mine[(size_t)(c0 + i) * 128 + row_local] = __uint_as_float(v[i]);
-      }
-      __threadfence();
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      // Every split of this tile waits for all of them (grid = tiles x ksplit <= SM count: all co-resident), then reduces
-      // ITS OWN share of the activation rows -- the reduction is spread over the ksplit CTAs instead of serialising
-      // R x ksplit dependent L2 round trips in the last arriver (that was 100 us of a 109 us prefill GEMM).  The
-      // summation order over splits is fixed, so the result stays run-to-run deterministic.
-      if (tid == 128) {
-        atomicAdd(&p.tickets[tile], 1u);
-        const long long t0 = clock64();
-        unsigned v;
-        do {
-          asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p.tickets + tile) : "memory");
-          if (clock64() - t0 > 4000000000ll) __trap();
-        } while (v < (unsigned)p.ksplit);
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      {
-        const int r_lo = (int)(((long long)split * p.R) / p.ksplit), r_hi = (int)(((long long)(split + 1) * p.R) / p.ksplit);
-        const float* base = p.scratch + ((size_t)tile * p.ksplit * ncols) * 128 + row_local;
-        for (int n0 = r_lo; n0 < r_hi; n0 += 2) {     // 2 rows x ksplit splits x {hi, lo} (x 2 matrices) loads in flight
-          float y[2] = {0.f, 0.f}, y3[2] = {0.f, 0.f};
-          for (int s0 = 0; s0 < p.ksplit; s0 += 8) {
-            float a[2][8], al[2][8], b3[2][8], bl[2][8];
-#pragma unroll
-            for (int i = 0; i < 2; ++i)
-#pragma unroll
-              for (int q = 0; q < 8; ++q) {
-                const int n = n0 + i, sp = s0 + q;
-                const bool ok = n < r_hi && sp < p.ksplit;
-                const float* ps = base + ((size_t)sp * ncols) * 128;
-                a[i][q] = ok ? __ldcg(ps + (size_t)n * 128) : 0.f;
-                al[i][q] = (ok && p.split_lo) ? __ldcg(ps + (size_t)(p.Rpad + n) * 128) : 0.f;
-                if (NA == 2) {
-                  b3[i][q] = ok ? __ldcg(ps + (size_t)(p.NB + n) * 128) : 0.f;
-                  bl[i][q] = (ok && p.split_lo) ? __ldcg(ps + (size_t)(p.NB + p.Rpad + n) * 128) : 0.f;
-                }
-              }
-#pragma unroll
-            for (int i = 0; i < 2; ++i)
-#pragma unroll
-              for (int q = 0; q < 8; ++q) {
-                y[i] += a[i][q] + al[i][q];
-                if (NA == 2) y3[i] += b3[i][q] + bl[i][q];
-              }
-          }
-#pragma unroll
-          for (int i = 0; i < 2; ++i)
-            if (n0 + i < r_hi && j < p.M) gemm_apply<EPI>(p, n0 + i, j, y[i], y3[i]);
-        }
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (tid == 128) {                       // the split that finishes last re-arms both counters for the next launch
-        const unsigned t = atomicAdd(&p.tickets[128 + tile], 1u);
-        if (t == (unsigned)p.ksplit - 1u) {
-          p.tickets[128 + tile] = 0u;
-          p.tickets[tile] = 0u;
         }
       }
     }
-    ptx::tc_fence_before();
+    __syncwarp();                          // every lane's fragment loads of this stage are done
+    if (lane == 0) ptx::mbar_arrive(ptx::smem_u32(bars + S + s));
   }
-  __syncthreads();
-  if (warp == 2) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, ncols_alloc);
+
+  // accumulator element e of chunk c: weight row w16 + (lane >> 2) + 8 (e >> 1), activation row 8 c + 2 (lane & 3) + (e & 1)
+  const int rl0 = w16 + (lane >> 2), n0 = 2 * (lane & 3);
+  if (p.ksplit == 1) {
+#pragma unroll
+    for (int c = 0; c < NC; ++c)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int n = 8 * c + n0 + (e & 1), j = tile * 128 + rl0 + 8 * (e >> 1);
+        if (c < nc && n < p.R && j < p.M) gemm_apply<EPI>(p, n, j, acc[0][c][e], acc[NA - 1][c][e]);
+      }
+    return;
+  }
+  const int ncols = NA * p.Rpad;
+  float* mine = p.scratch + ((size_t)(tile * p.ksplit + split) * ncols) * 128;
+#pragma unroll
+  for (int a = 0; a < NA; ++a)
+#pragma unroll
+    for (int c = 0; c < NC; ++c)
+#pragma unroll
+      for (int e = 0; e < 4; ++e)
+        if (c < nc) mine[(size_t)(a * p.Rpad + 8 * c + n0 + (e & 1)) * 128 + rl0 + 8 * (e >> 1)] = acc[a][c][e];
+  __threadfence();
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+  // Every split of this tile waits for all of them (grid = tiles x ksplit <= SM count: all co-resident), then reduces
+  // ITS OWN share of the activation rows -- the reduction is spread over the ksplit CTAs instead of serialising
+  // R x ksplit dependent L2 round trips in the last arriver.  The summation order over splits is fixed, so the result
+  // stays run-to-run deterministic.
+  if (ct == 0) {
+    atomicAdd(&p.tickets[tile], 1u);
+    const long long t0 = clock64();
+    unsigned v;
+    do {
+      asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p.tickets + tile) : "memory");
+      if (clock64() - t0 > 4000000000ll) __trap();
+    } while (v < (unsigned)p.ksplit);
+  }
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+  {
+    const int row_local = ct & 127, j = tile * 128 + row_local;
+    const int r_lo = (int)(((long long)split * p.R) / p.ksplit), r_hi = (int)(((long long)(split + 1) * p.R) / p.ksplit);
+    const float* base = p.scratch + ((size_t)tile * p.ksplit * ncols) * 128 + row_local;
+    for (int n = r_lo + (ct >> 7); n < r_hi; n += 2) {
+      float y = 0.f, y3 = 0.f;
+#pragma unroll 8
+      for (int sp = 0; sp < p.ksplit; ++sp) {
+        const float* ps = base + ((size_t)sp * ncols) * 128;
+        y += __ldcg(ps + (size_t)n * 128);
+        if (NA == 2) y3 += __ldcg(ps + (size_t)(p.Rpad + n) * 128);
+      }
+      if (j < p.M) gemm_apply<EPI>(p, n, j, y, y3);
+    }
+  }
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+  if (ct == 0) {                          // the split that finishes last re-arms both counters for the next launch
+    const unsigned t = atomicAdd(&p.tickets[128 + tile], 1u);
+    if (t == (unsigned)p.ksplit - 1u) {
+      p.tickets[128 + tile] = 0u;
+      p.tickets[tile] = 0u;
+    }
   }
 }
 

@@ -1,4 +1,4 @@
-// Host-side helpers for the tcgen05 GEMM path: TMA tensor maps (driver entry point resolved at run
+// Host-side helpers for the tensor-core GEMM path: TMA tensor maps (driver entry point resolved at run
 // time, so libmvb200 does not link libcuda) and launch configuration.
 #pragma once
 #include <cuda.h>
@@ -26,7 +26,7 @@ static inline EncodeTiledFn encode_tiled_fn() {
   return fn;
 }
 
-// bf16 row-major [rows, cols] -> tiles of [box_rows, 64] with the 128-byte swizzle UMMA expects.
+// bf16 row-major [rows, cols] -> tiles of [box_rows, 64] with the 128-byte swizzle the MMA fragment loads expect.
 static inline bool make_tmap_bf16(CUtensorMap* tm, const void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows) {
   EncodeTiledFn fn = encode_tiled_fn();
   if (!fn) return false;
@@ -79,24 +79,35 @@ static inline GemmPlan plan_gemm(int M, int K, int NB, bool swiglu, int n_sm) {
   const int per = (nkb + ks - 1) / ks;
   if (st > per) st = per < 2 ? 2 : per;
   g.stages = st;
-  g.smem_bytes = 1024 + (size_t)st * stage_bytes + (2 * st + 1) * 8 + 64;
+  g.smem_bytes = 1024 + (size_t)st * stage_bytes + 2 * st * 8 + 64;
   g.scratch_floats = (size_t)g.tiles * ks * (swiglu ? 2 : 1) * NB * 128;
   return g;
 }
 
-template <int EPI>
-static inline cudaError_t launch_umma_gemm(cudaStream_t s, const CUtensorMap& tA, const CUtensorMap& tA3, const CUtensorMap& tB,
-                                           GemmP p, const GemmPlan& g) {
+template <int EPI, int NC>
+static inline cudaError_t launch_umma_gemm_nc(cudaStream_t s, const CUtensorMap& tA, const CUtensorMap& tA3, const CUtensorMap& tB,
+                                              const GemmP& p, const GemmPlan& g) {
   static PerDeviceOnce attr_set;
   if (attr_set.pending()) {
-    cudaError_t e = cudaFuncSetAttribute(k_umma_gemm<EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(k_umma_gemm<EPI, NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) return e;
     attr_set.mark();
   }
+  k_umma_gemm<EPI, NC><<<dim3(g.tiles, g.ksplit), GEMM_THREADS, g.smem_bytes, s>>>(tA, tA3, tB, p);
+  return cudaGetLastError();
+}
+
+// The accumulator size is a template parameter (registers): the smallest of 16 / 32 / 64 / 128 columns that holds Rpad.
+template <int EPI>
+static inline cudaError_t launch_umma_gemm(cudaStream_t s, const CUtensorMap& tA, const CUtensorMap& tA3, const CUtensorMap& tB,
+                                           GemmP p, const GemmPlan& g) {
+  if (p.Rpad < 16 || p.Rpad > 128 || p.Rpad % 16) return cudaErrorInvalidValue;
   p.ksplit = g.ksplit;
   p.stages = g.stages;
-  k_umma_gemm<EPI><<<dim3(g.tiles, g.ksplit), 256, g.smem_bytes, s>>>(tA, tA3, tB, p);
-  return cudaGetLastError();
+  if (p.Rpad <= 16) return launch_umma_gemm_nc<EPI, 2>(s, tA, tA3, tB, p, g);
+  if (p.Rpad <= 32) return launch_umma_gemm_nc<EPI, 4>(s, tA, tA3, tB, p, g);
+  if (p.Rpad <= 64) return launch_umma_gemm_nc<EPI, 8>(s, tA, tA3, tB, p, g);
+  return launch_umma_gemm_nc<EPI, 16>(s, tA, tA3, tB, p, g);
 }
 
 }  // namespace mvb

@@ -235,7 +235,7 @@ def build_model(*, precision: torch.dtype = torch.bfloat16, checkpoint_path: Pat
     model.setup_spk_cond_mask()
     model.setup_caches(max_batch_size=2 * max_utts, max_seq_length=model.config.block_size, kv_dtype=kv_dtype)
     sample.default_model = model
-    # `compile` / `compile_prefill` are accepted and ignored: kernels are ahead-of-time sm_100a code.
+    # `compile` / `compile_prefill` are accepted and ignored: kernels are ahead-of-time sm_90a code.
     return model, tokenizer, smodel, model_size
 
 

@@ -134,7 +134,7 @@ class Transformer:
     def setup_caches(self, max_batch_size: int, max_seq_length: int, kv_dtype: str = "bf16", max_new: Optional[int] = None,
                      tensor_core_path: Optional[bool] = None):
         """fast_model.py:136-148.  ``max_batch_size`` counts rows: 2 per utterance (CFG pair).
-        ``tensor_core_path`` (test hook): force the tcgen05 rows path on/off for prefill and batched decode."""
+        ``tensor_core_path`` (test hook): force the tensor-core rows path on/off for prefill and batched decode."""
         if (self._handle is not None and self.max_seq_length >= max_seq_length and self.max_batch_size >= max_batch_size
                 and kv_dtype == self.kv_dtype and tensor_core_path is None):
             return

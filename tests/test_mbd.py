@@ -68,7 +68,7 @@ def _round_conv_weights_to_bf16(ck):
 @pytest.mark.gpu
 @pytest.mark.parametrize("kernel,stride,frames,hidden", [(8, 4, 12, 64), (8, 4, 33, 64), (4, 2, 12, 64), (8, 4, 12, 48)])
 def test_mbd_tensor_core_convs_vs_restatement(kernel, stride, frames, hidden, monkeypatch):
-    """Input widths >= 32 channels take the tcgen05 path (csrc/mbd_tc.cuh): shifted-GEMM Conv1d (dilation 1
+    """Input widths >= 32 channels take the tensor-core path (csrc/mbd_tc.cuh): shifted-GEMM Conv1d (dilation 1
     and 2), the strided encoder convolution and the phase-decomposed ConvTranspose1d.  With conv weights representable in
     bf16 the path is exact to fp32 round-off against the fp32 restatement; with arbitrary fp32 weights the only deviation
     is the bf16 rounding of the taps (reported, bounded)."""

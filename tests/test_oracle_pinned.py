@@ -6,7 +6,7 @@ import pytest
 import torch
 
 from mvb200 import synth
-from oracle import ref_harness, stage1_port as P
+from oracle import stage1_port as P
 
 
 def _load(golden_dir, name):
@@ -92,22 +92,17 @@ def test_prompt_too_long_raises():
         P.generate(m, synth.synthetic_prompt(2048), synth.synthetic_speaker(), guidance_scale=3.0, temperature=1.0)
 
 
-@pytest.mark.skipif(not ref_harness.available(), reason="reference tree not mounted (GPU box)")
-def test_port_matches_live_reference():
-    d = synth.TINY
-    sd = synth.stage1_state_dict(d, 3)
-    ref = ref_harness.build_reference_model(sd, d, torch.float32)
+def test_port_matches_live_reference(golden_dir):
+    """The reference Transformer's logits and generate() tokens, recorded by oracle/make_golden_live.py."""
+    from oracle import make_golden_live as L
+    g = np.load(f"{golden_dir}/reference_calls.npz")
+    d, sd, prompt, spk = L.stage1_inputs()
     m = P.Stage1Oracle(sd, d.n_head, d.norm_eps, torch.float32); m.setup_caches()
-    prompt = synth.synthetic_prompt(9, seed=5); spk = synth.synthetic_speaker(seed=2)
     idx = prompt.view(1, -1).repeat(2, 1)
     with torch.no_grad():
-        a = ref(idx, spk, torch.arange(9)); b = m.forward(idx, spk, torch.arange(9))
-    assert (a - b).abs().max() < 1e-5
-    fiu = ref_harness.reference_functions()
-    ref2 = ref_harness.build_reference_model(sd, d, torch.float32)
-    kw = dict(temperature=torch.tensor(0.8), top_p=torch.tensor(0.9), guidance_scale=torch.tensor(2.0), top_k=None)
-    torch.manual_seed(5)
-    ya = fiu.generate(ref2, prompt, spk, max_new_tokens=12, end_of_audio_token=9999, **kw)
+        b = m.forward(idx, spk, torch.arange(9))
+    assert (torch.from_numpy(g["s1_logits"]) - b).abs().max() < 1e-5
+    ya = g["s1_tokens"]
     m2 = P.Stage1Oracle(sd, d.n_head, d.norm_eps, torch.float32); m2.setup_caches()
     torch.manual_seed(5)
     yb = P.generate(m2, prompt, spk, max_new_tokens=12, end_of_audio_token=9999, temperature=0.8, top_p=0.9,

@@ -5,7 +5,7 @@ import torch
 
 from mvb200 import synth
 from mvb200.second_stage import build_stage2_input, flattened_interleaved_decode, tilted_decode
-from oracle import ref_harness, stage2_port as P
+from oracle import stage2_port as P
 
 
 @pytest.mark.parametrize("tag,dims", [("tiny", synth.S2_TINY), ("full", synth.S2_FULL)])
@@ -38,17 +38,17 @@ def test_adapters_match_oracle_and_reference_semantics():
         assert codes[0] == [3, 4, 5] and codes[2] == [9, 9, 2]   # "first-N-valid" truncation (tilted_encodec.py:31-37)
 
 
-@pytest.mark.skipif(not ref_harness.available(), reason="reference tree not mounted (GPU box)")
-def test_adapters_match_live_reference():
-    ref_harness._import_reference()
-    from fam.llm.adapters import FlattenedInterleavedEncodec2Codebook, TiltedEncodec
-    g = torch.Generator().manual_seed(0)
-    flat = torch.randint(0, 2562, (300,), generator=g).tolist()
-    a = FlattenedInterleavedEncodec2Codebook(end_of_audio_token=1024).decode([flat])
-    assert tuple(a) == tuple(flattened_interleaved_decode(flat))
-    hier = torch.randint(0, 1100, (8, 200), generator=g).tolist()
-    b = TiltedEncodec(end_of_audio_token=1024).decode(hier)
-    assert tuple(b) == tuple(tilted_decode(hier))
+def test_adapters_match_live_reference(golden_dir):
+    """The reference adapters' decode(), recorded by oracle/make_golden_live.py."""
+    from oracle import make_golden_live as L
+    g = np.load(f"{golden_dir}/reference_calls.npz")
+    flat, hier = L.adapter_inputs()
+    text, cb = flattened_interleaved_decode(flat)
+    assert list(text) == g["flat_text"].tolist()
+    assert len(cb) == int(g["flat_n_cb"]) and all(list(c) == g[f"flat_cb_{i}"].tolist() for i, c in enumerate(cb))
+    text, codes = tilted_decode(hier)
+    assert list(text) == g["tilted_text"].tolist()
+    assert len(codes) == int(g["tilted_n_codes"]) and all(list(c) == g[f"tilted_codes_{i}"].tolist() for i, c in enumerate(codes))
 
 
 def test_input_builder_layout():
@@ -73,19 +73,11 @@ def test_product_input_builder_matches_reference_golden(golden_dir, tag):
         assert np.array_equal(P.build_input(g[f"{tag}_text_{i}"].tolist(), *g[f"{tag}_codes_{i}"].tolist(), bs).numpy(), ref[i])
 
 
-@pytest.mark.skipif(not ref_harness.available(), reason="reference tree not mounted (GPU box)")
-def test_product_input_builder_matches_live_reference():
-    import importlib.util
-    import os
-    spec = importlib.util.spec_from_file_location("mk_s2in", os.path.join(os.path.dirname(P.__file__), "make_golden_stage2_input.py"))
-    mk = importlib.util.module_from_spec(spec); spec.loader.exec_module(mk)
-    from mvb200.tokenise import TrainedBPETokeniser
-    tok = TrainedBPETokeniser(**synth.synthetic_tokenizer_meta(n_text_tokens=512, offset=1025))
-    Model = mk.reference_model_class()
-    g = torch.Generator().manual_seed(77)
-    texts = ["a b c", "the quick brown fox", "x"]
-    codes = [torch.randint(0, 1024, (1, 2, n), generator=g) for n in (10, 300, 255)]
-    in_x = mk.reference_in_x(Model, tok, texts, codes, 256)
-    for i in range(3):
-        got = build_stage2_input(tok.encode(texts[i]), codes[i][0].tolist(), 256)
-        assert torch.equal(got.long(), in_x[i])
+def test_product_input_builder_matches_live_reference(golden_dir):
+    """The stage-2 input the reference's Model built, recorded by oracle/make_golden_live.py."""
+    from oracle import make_golden_live as L
+    g = np.load(f"{golden_dir}/reference_calls.npz")
+    tok, codes = L.stage2_inputs()
+    for i, text in enumerate(L.S2_TEXTS):
+        got = build_stage2_input(tok.encode(text), codes[i][0].tolist(), 256)
+        assert np.array_equal(got.long().numpy(), g[f"s2_in_x_{i}"])

@@ -176,7 +176,7 @@ def test_batched_mixed_lengths_equal_single_runs(tiny_sd):
 
 @pytest.mark.parametrize("lens", [[5, 17, 9], [5, 17, 9, 12, 3, 20, 8]], ids=["batch3_n16", "batch7_n32"])
 def test_persistent_kernel_batch_logits_match_single(tiny_sd, lens):
-    """Same state, batch of 3 (16-column UMMA variant) / 7 (32-column variant) vs each utterance alone through the
+    """Same state, batch of 3 (16-row activation operand) / 7 (32-row variant) vs each utterance alone through the
     persistent kernel: logits agree to reduction-order noise (fp32 KV) / bf16 rounding flips of the appended K,V
     (bf16 KV)."""
     import ctypes as C
@@ -253,7 +253,7 @@ def test_full_size_logits_vs_reference_golden(golden_dir, full_sd):
 
 @pytest.mark.parametrize("tc", [False, True])
 def test_prefill_paths_vs_oracle_chunked(tiny_sd, tc):
-    """Prefill through the CUDA-core path (one position at a time) and through the tcgen05 rows path (64-token
+    """Prefill through the CUDA-core path (one position at a time) and through the tensor-core rows path (64-token
     chunks; T=70 crosses a chunk boundary), all positions, against the oracle; then a decode step on top of the
     cache each path wrote."""
     from oracle import stage1_port as P
@@ -273,7 +273,7 @@ def test_prefill_paths_vs_oracle_chunked(tiny_sd, tc):
 
 
 def test_batched_decode_tensor_core_path_equals_cuda_core_path(tiny_sd):
-    """CUDA-core kernels only / tcgen05 rows path / + persistent fused decode kernel: free-running token ids of the
+    """CUDA-core kernels only / tensor-core rows path / + persistent fused decode kernel: free-running token ids of the
     first two are identical (both deterministic); the persistent kernel is compared under teacher forcing."""
     from mvb200 import fast_inference_utils as U
     d = synth.TINY
@@ -289,7 +289,7 @@ def test_batched_decode_tensor_core_path_equals_cuda_core_path(tiny_sd):
     forced = torch.stack([y.to(torch.int32) for y in ya])
     _, sc = U.generate_batch(_mk(d, tiny_sd, "fp32", utts=4, tc="BC"), prompts, spk, forced=forced, return_sampled=True, **kw)
     mism_c = sum(int(a != b) for y, s_ in zip(ya, sc) for a, b in zip(y.tolist(), s_.tolist()))
-    print(f"sequences differing CUDA-core vs tcgen05 rows path: {mism_b}/4; sampled ids differing vs persistent kernel: {mism_c}/{4 * n_new}")
+    print(f"sequences differing CUDA-core vs tensor-core rows path: {mism_b}/4; sampled ids differing vs persistent kernel: {mism_c}/{4 * n_new}")
     assert mism_b <= 1 and mism_c <= 2 and all(len(y) == n_new for y in ya)
 
 

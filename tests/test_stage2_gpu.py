@@ -1,4 +1,4 @@
-"""GPU: stage-2 engine (tcgen05 GEMMs + bidirectional attention + sampler) through the C ABI vs golden vectors from
+"""GPU: stage-2 engine (tensor-core GEMMs + bidirectional attention + sampler) through the C ABI vs golden vectors from
 the reference's own GPT and vs the CPU oracle."""
 import numpy as np
 import pytest

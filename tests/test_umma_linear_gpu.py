@@ -1,4 +1,4 @@
-"""GPU: the tcgen05/TMA weight-streaming linear operator in isolation, against a plain fp32 torch matmul on the
+"""GPU: the TMA / tensor-core weight-streaming linear operator in isolation, against a plain fp32 torch matmul on the
 same bf16-rounded weights (the op-level reference for a floating-point kernel)."""
 import ctypes as C
 

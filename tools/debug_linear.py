@@ -1,4 +1,4 @@
-"""GPU debug aid: run the tcgen05 linear op on structured inputs and dump outputs + references so descriptor /
+"""GPU debug aid: run the tensor-core linear op on structured inputs and dump outputs + references so descriptor /
 swizzle mistakes can be diagnosed offline from one gpurun call.  Writes gpurun_out/linear_debug.npz."""
 import ctypes as C
 import os
