@@ -145,10 +145,11 @@ int mvb_s1_begin(mvb_s1* h, int32_t utt, int32_t first_token, int32_t pos, const
 int mvb_s1_fetch(mvb_s1* h, int32_t utt, int32_t* out_tokens, int32_t cap, int32_t* n_out,
                  int32_t* done, void* stream);
 
-/* Parity hook for the persistent fused decode kernel: one decode position (== Transformer.forward with S = 1,
- * fast_model.py:150-163) for utterances [0, n_utts) from the state installed by mvb_s1_begin, through the single
- * persistent kernel; logits fp32 [2*n_utts, vocab] are copied to d_logits, nothing is sampled, positions do not
- * advance (the KV cache is appended at the current positions). */
+/* Parity hook for the decode body: one decode position (== Transformer.forward with S = 1, fast_model.py:150-163)
+ * for utterances [0, n_utts) from the state installed by mvb_s1_begin, through the body mvb_s1_decode runs for that
+ * batch: the persistent fused kernel up to 8 utterances (when enabled), the per-layer path otherwise (tensor-core
+ * rows path up to max_utts = 64 utterances); logits fp32 [2*n_utts, vocab] are copied to d_logits, nothing is sampled,
+ * positions do not advance (the KV cache is appended at the current positions). */
 int mvb_s1_step_logits(mvb_s1* h, int32_t n_utts, float* d_logits, void* stream);
 
 /* Kernel launches issued by this handle since creation (bench.py "gpu_launches"). */
@@ -171,6 +172,30 @@ int mvb_s1_trace_fetch(mvb_s1* h, long long* out, int32_t max_ctas, void* stream
 int mvb_linear(const void* d_W, int32_t M, int32_t K, const float* d_x, int32_t ldx, int32_t R,
                const void* d_gain, float eps, int32_t split_lo, int32_t ksplit_override, float* d_out,
                int32_t ldo, int32_t accumulate, void* stream);
+
+/* Test hooks for the op-level tests of two tensor-core kernels (not part of the drop-in surface):
+ *   mvb_gemm_test     : mvb_linear's operator with any epilogue of the weight-streaming GEMM (csrc/umma_gemm.cuh):
+ *                       epi 0 store, 1 residual add, 2 SwiGLU  out = silu(x W^T) * (x W3^T)  (d_W3 bf16 [M, K]),
+ *                       3 QKV  out = x W^T plus the K / V thirds scattered to d_kcache / d_vcache
+ *                       [rows][H][S_max][128] (fp32 when kv_fp32, else bf16) at cache row d_row_cache[n], position
+ *                       d_row_pos[n] (device int32 [R]; D = 128 H, M = 3 D).  Unused pointers may be NULL.
+ *   mvb_mbd_conv_test : one multi-band-diffusion convolution (csrc/mbd.cu) without an mvb_mbd handle.  kind 0: Conv1d,
+ *                       stride 1, pad = dil (K - 1) / 2; 1: Conv1d(K = 2 stride) over the input right-padded to a
+ *                       multiple of stride; 2: ConvTranspose1d(K = 2 stride), no bias / emb / resid.  d_x fp32
+ *                       [Cin, Tin]; d_w fp32 in PyTorch layout ([Cout, Cin, K], transposed [Cin, Cout, K]); optional
+ *                       input transform relu(GroupNorm) from caller-supplied d_gn_stats [groups][mean, rstd], d_gn_w,
+ *                       d_gn_b [Cin]; optional d_bias, d_emb [Cout], d_resid [Cout, Tout]; d_y fp32 [Cout, Tout], Tout =
+ *                       Tin, ceil(Tin / stride), Tin * stride.  use_tc != 0: the tensor-core kernel with the engine's
+ *                       weight packing; 0: the CUDA-core kernels.
+ * Both synchronise `stream`. */
+int mvb_gemm_test(int32_t epi, const void* d_W, const void* d_W3, int32_t M, int32_t K, const float* d_x, int32_t ldx,
+                  int32_t R, const void* d_gain, float eps, int32_t split_lo, int32_t ksplit_override, float* d_out,
+                  int32_t ldo, void* d_kcache, void* d_vcache, const int32_t* d_row_cache, const int32_t* d_row_pos,
+                  int32_t H, int32_t S_max, int32_t D, int32_t kv_fp32, void* stream);
+int mvb_mbd_conv_test(int32_t kind, const float* d_x, int32_t Cin, int32_t Tin, const float* d_w, int32_t Cout, int32_t K,
+                      int32_t stride, int32_t dil, int32_t pad, const float* d_gn_stats, const float* d_gn_w,
+                      const float* d_gn_b, int32_t groups, const float* d_bias, const float* d_emb, const float* d_resid,
+                      float* d_y, int32_t use_tc, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Stage 2: the non-causal codebook-expansion model (fam/llm/model.py:195-314 with causal=False) and its sampler

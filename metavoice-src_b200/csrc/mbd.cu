@@ -590,11 +590,9 @@ static int gn_stats(mvb_mbd* h, cudaStream_t s, const float* x, int C, int T, in
 
 // One convolution on the tensor cores (mbd_tc.cuh).  kind 0: Conv1d stride 1 ('same', pad = dil * (K - 1) / 2);
 // 1: Conv1d(K = 2s, stride s, pad s/2) over the right-padded input; 2: ConvTranspose1d(K = 2s, stride s, pad s/2).
-static int launch_conv_tc(mvb_mbd* h, cudaStream_t s, const ConvP& p, int widx, int kind, int K, int stride) {
-  const mvb_mbd::TcW& w = h->tcw[h->tc_of[widx]];
-  const MbdWs L = mbd_layout(&h->cfg);
-  __nv_bfloat16* hi = reinterpret_cast<__nv_bfloat16*>(h->base + L.xt_hi);
-  __nv_bfloat16* lo = reinterpret_cast<__nv_bfloat16*>(h->base + L.xt_lo);
+// tmA: the taps packed by k_mbd_pack_w; hi / lo: room for the time-major copy of the input (Tpad x Cp bf16 each).
+static int conv_tc(cudaStream_t s, const ConvP& p, const CUtensorMap& tmA, __nv_bfloat16* hi, __nv_bfloat16* lo, int kind, int K,
+                   int stride) {
   const int Tpad = kind == 1 ? (p.Tin + stride - 1) / stride * stride : p.Tin;
   const int Cp = mbd_tc_cpad(p.Cin);
   k_mbd_prep_t<<<dim3((Tpad + 31) / 32, Cp / 64), 256, 0, s>>>(p.x, p.Cin, Cp, p.Tin, Tpad, p.gn_stats, p.gn_w, p.gn_b,
@@ -628,10 +626,14 @@ static int launch_conv_tc(mvb_mbd* h, cudaStream_t s, const ConvP& p, int widx, 
     }
   }
   const int n_cot = (p.Cout + 127) / 128;
-  k_mbd_tc_conv<<<dim3(t.n_ph * n_cot, (q.Ncols + 127) / 128), TC_THREADS, TC_SMEM, s>>>(w.tmA, tBhi, tBlo, q);
+  k_mbd_tc_conv<<<dim3(t.n_ph * n_cot, (q.Ncols + 127) / 128), TC_THREADS, TC_SMEM, s>>>(tmA, tBhi, tBlo, q);
   MCK(cudaGetLastError());
-  (void)w.K;
   return MVB_OK;
+}
+static int launch_conv_tc(mvb_mbd* h, cudaStream_t s, const ConvP& p, int widx, int kind, int K, int stride) {
+  const MbdWs L = mbd_layout(&h->cfg);
+  return conv_tc(s, p, h->tcw[h->tc_of[widx]].tmA, reinterpret_cast<__nv_bfloat16*>(h->base + L.xt_hi),
+                 reinterpret_cast<__nv_bfloat16*>(h->base + L.xt_lo), kind, K, stride);
 }
 
 // ResBlock (unet.py): x + conv2(relu(norm2(conv1(relu(norm1(x)))))), kernel 3, dilation 2^j; `emb` is added to the block output
@@ -824,4 +826,62 @@ extern "C" int mvb_mbd_tokens_to_wav(mvb_mbd* h, const float* d_cond, int32_t n_
   k_band_mix<<<148 * 2, 256, 0, s>>>(low_w, wav, T, c.eq_bands, stdv + 64, stdv, nullptr, d_wav_out, 0);
   MCK(cudaGetLastError());
   return MVB_OK;
+}
+
+// Test hook: one convolution of the kinds unet_forward runs, outside any mvb_mbd handle, with the taps packed by
+// k_mbd_pack_w and the input prepared by k_mbd_prep_t exactly as in the engine (use_tc != 0), or through the CUDA-core
+// kernels (use_tc == 0).  Buffers for the packed taps and the time-major input are allocated per call.  Synchronises `stream`.
+extern "C" int mvb_mbd_conv_test(int32_t kind, const float* d_x, int32_t Cin, int32_t Tin, const float* d_w, int32_t Cout, int32_t K,
+                                 int32_t stride, int32_t dil, int32_t pad, const float* d_gn_stats, const float* d_gn_w,
+                                 const float* d_gn_b, int32_t groups, const float* d_bias, const float* d_emb, const float* d_resid,
+                                 float* d_y, int32_t use_tc, void* stream) {
+  if (!d_x || !d_w || !d_y) return mvb::set_error(MVB_ERR_ARG, "null argument");
+  if (kind < 0 || kind > 2 || Cin < 1 || Cout < 1 || Tin < 1 || K < 1 || stride < 1 || dil < 1 || pad < 0)
+    return mvb::set_error(MVB_ERR_ARG, "mvb_mbd_conv_test: bad shape");
+  if (d_gn_stats && (!d_gn_w || !d_gn_b || groups < 1 || Cin % groups)) return mvb::set_error(MVB_ERR_ARG, "mvb_mbd_conv_test: GroupNorm");
+  if ((kind == 0 && (stride != 1 || 2 * pad != dil * (K - 1))) || (kind != 0 && (K != 2 * stride || dil != 1)) ||
+      (kind == 2 && (d_bias || d_emb || d_resid)))
+    return mvb::set_error(MVB_ERR_UNSUPPORTED, "mvb_mbd_conv_test: kind %d with K %d stride %d dil %d pad %d", kind, K, stride, dil, pad);
+  cudaStream_t s = (cudaStream_t)stream;
+  ConvP p{};
+  p.x = d_x; p.Cin = Cin; p.Tin = Tin; p.w = d_w; p.bias = d_bias; p.y = d_y; p.Cout = Cout;
+  p.Tout = kind == 0 ? Tin : kind == 1 ? (Tin + stride - 1) / stride : Tin * stride;
+  p.dil = dil; p.pad = pad;
+  p.gn_stats = d_gn_stats; p.gn_w = d_gn_w; p.gn_b = d_gn_b; p.groups = groups;
+  p.resid = d_resid; p.emb = d_emb;
+  if (!use_tc) {
+    if (kind != 2) {
+      if (int e = launch_conv(s, p, K, stride)) return e;
+    } else if (stride == 4) k_mbd_convtr<4><<<dim3((p.Tout + 255) / 256, (Cout + 31) / 32), 256, 0, s>>>(p);
+    else if (stride == 2) k_mbd_convtr<2><<<dim3((p.Tout + 255) / 256, (Cout + 31) / 32), 256, 0, s>>>(p);
+    else return mvb::set_error(MVB_ERR_UNSUPPORTED, "mvb_mbd_conv_test: transposed stride %d", stride);
+    MCK(cudaGetLastError());
+    MCK(cudaStreamSynchronize(s));
+    return MVB_OK;
+  }
+  if ((kind != 2 && K > 8) || (kind == 2 && stride > 4)) return mvb::set_error(MVB_ERR_UNSUPPORTED, "mvb_mbd_conv_test: too many taps");
+  if (!encode_tiled_fn()) return mvb::set_error(MVB_ERR_CUDA, "mvb_mbd_conv_test: no cuTensorMapEncodeTiled");
+  const int Cp = mbd_tc_cpad(Cin);
+  const int Tpad = kind == 1 ? (Tin + stride - 1) / stride * stride : Tin;
+  const size_t wbytes = (size_t)K * Cout * Cp * 2, xbytes = (size_t)Tpad * Cp * 2;
+  void* buf = nullptr;
+  MCK(cudaMalloc(&buf, wbytes + 2 * ((xbytes + 255) / 256 * 256) + 256));
+  __nv_bfloat16* wp = reinterpret_cast<__nv_bfloat16*>(buf);
+  __nv_bfloat16* hi = reinterpret_cast<__nv_bfloat16*>(reinterpret_cast<char*>(buf) + (wbytes + 255) / 256 * 256);
+  __nv_bfloat16* lo = reinterpret_cast<__nv_bfloat16*>(reinterpret_cast<char*>(hi) + (xbytes + 255) / 256 * 256);
+  int rc = MVB_OK;
+  cudaError_t e = cudaFuncSetAttribute(k_mbd_tc_conv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM);
+  CUtensorMap tmA;
+  if (e == cudaSuccess) {
+    k_mbd_pack_w<<<148 * 4, 256, 0, s>>>(d_w, Cout, Cin, Cp, K, kind == 2 ? 1 : 0, wp);
+    e = cudaGetLastError();
+  }
+  if (e != cudaSuccess) rc = mvb::set_error(MVB_ERR_CUDA, "mvb_mbd_conv_test: %s", cudaGetErrorString(e));
+  else if (!make_tmap_bf16_3d(&tmA, wp, (uint64_t)Cp, (uint64_t)Cout, (uint64_t)K, (uint64_t)Cout * Cp * 2, 128))
+    rc = mvb::set_error(MVB_ERR_CUDA, "mvb_mbd_conv_test: weight tensor map");
+  else rc = conv_tc(s, p, tmA, hi, lo, kind, K, stride);
+  e = cudaStreamSynchronize(s);    // (also on an error path: the buffer is freed only once nothing can still use it)
+  if (rc == MVB_OK && e != cudaSuccess) rc = mvb::set_error(MVB_ERR_CUDA, "mvb_mbd_conv_test: %s", cudaGetErrorString(e));
+  cudaFree(buf);
+  return rc;
 }

@@ -841,18 +841,24 @@ extern "C" int mvb_s1_decode(mvb_s1* h, int32_t n_utts, int32_t n_steps, void* s
 }
 
 
-// Parity hook for the persistent decode kernel: one fused position for utterances [0, n_utts) from the current
-// decode state (tokens/positions installed with mvb_s1_begin), logits copied out, no sampling, state untouched
-// except for the KV-cache append at the current positions.
+// Parity hook for the decode body: one position for utterances [0, n_utts) from the current decode state (tokens /
+// positions installed with mvb_s1_begin) through the body mvb_s1_decode runs for that batch, logits copied out, no
+// sampling, state untouched except for the KV-cache append at the current positions.  That body is the persistent
+// fused kernel where mvb_s1_decode would use it (up to 8 utterances), else the per-layer path (tensor-core rows path
+// from decode_b_min utterances up).
 extern "C" int mvb_s1_step_logits(mvb_s1* h, int32_t n_utts, float* d_logits, void* stream) {
   if (!h || !d_logits) return fail(MVB_ERR_ARG, "null argument");
-  if (n_utts < 1 || n_utts > h->cfg.max_utts || 2 * n_utts > PC_RPAD) return fail(MVB_ERR_ARG, "n_utts %d out of range", n_utts);
-  if (!h->pc_ok) return fail(MVB_ERR_UNSUPPORTED, "persistent decode kernel unavailable for this configuration");
+  if (n_utts < 1 || n_utts > h->cfg.max_utts) return fail(MVB_ERR_ARG, "n_utts %d out of range", n_utts);
   cudaStream_t s = (cudaStream_t)stream;
   const size_t bytes = sizeof(float) * 2 * (size_t)n_utts * h->cfg.vocab;
   k_identity_slots<<<1, 64, 0, s>>>(h->st, n_utts);
   h->launches++;
   CK(cudaGetLastError());
+  if (!(h->path_c && h->pc_ok && 2 * n_utts <= PC_RPAD)) {
+    if (int e = run_body(h, s, n_utts)) return e;
+    CK(cudaMemcpyAsync(d_logits, h->wsp<float>(h->L.logits), bytes, cudaMemcpyDeviceToDevice, s));
+    return MVB_OK;
+  }
   CK(cudaMemsetAsync(h->wsp<float>(h->L.logits), 0, bytes, s));
   CK(cudaMemsetAsync(h->wsp<unsigned>(h->L.c_bar), 0, 4, s));
   if (int e = launch_persistent(h, s, n_utts, 1, false)) return e;

@@ -109,6 +109,12 @@ SIGNATURES = {
     # test / debug hooks (declared in the header as such)
     "mvb_s1_fetch_sampled": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]),
     "mvb_s1_trace_fetch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
+    "mvb_gemm_test": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32,
+                                C.c_void_p, C.c_float, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
+    "mvb_mbd_conv_test": (C.c_int, [C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                    C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                    C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
 }
 ABI_VERSION = 2
 

@@ -95,6 +95,31 @@ def test_mbd_tensor_core_convs_vs_restatement(kernel, stride, frames, hidden, mo
         assert err < (2e-3 if exact else 3e-2)
 
 
+@pytest.mark.gpu
+def test_mbd_default_config_vs_restatement(monkeypatch):
+    """The shipped UNet (default UnetSettings: hidden 48, growth 4, depth 4, widths 48 / 192 / 768 / 3072) end to end:
+    workspace sizing (mbd_layout) and layer wiring at those widths, 2 band models, 2 sampler calls, 12 frames
+    (3833 samples), bf16-representable taps."""
+    monkeypatch.delenv("MVB_MBD_NO_TC", raising=False)
+    from mvb200.mbd import MBDSettings, MultiBandDiffusionEngine
+    steps = [999, 499, 0]
+    cfg = M.MBDConfig(n_models=2, step_list=steps)
+    settings = MBDSettings(n_models=2, step_list=steps)
+    frames = 12
+    T = frames * 320 - 7
+    g = torch.Generator().manual_seed(7)
+    cond = torch.randn(128, frames, generator=g)
+    wav_e = torch.from_numpy(synth.synthetic_waveform(frames * 320 / 24000.0, 24000, seed=5))[:T]
+    noise = torch.randn(2, len(steps) - 1, T, generator=g)
+    ck = _round_conv_weights_to_bf16(synth.mbd_checkpoint(cfg, 2))
+    eng = MultiBandDiffusionEngine(ck, settings, device="cuda:0", max_seconds=1.0)
+    want = M.MBDOracle(ck, cfg).tokens_to_wav(wav_e, cond, noise)
+    got = eng.tokens_to_wav(cond, wav_e, noise=noise).cpu()
+    err = float((got - want).abs().max() / want.abs().max())
+    print(f"MBD default configuration ({T} samples, 2 band models, 2 calls): rel err vs restatement {err:.2e}")
+    assert err < 2e-3
+
+
 def test_flop_accounting_matches_the_restatement_shapes():
     """bench.py's MBD roofline uses MultiBandDiffusionEngine.flops(): check it against a direct count over the restatement's
     own layer shapes for the default parametrised configuration (187 GFLOP per UNet pass, 80 passes per utterance)."""

@@ -517,3 +517,51 @@ def test_resident_forward_then_decode_equals_generate(tiny_sd):
     mism = sum(int(a != b) for a, b in zip(got.tolist(), ref.tolist()))
     print("resident forward+decode vs generate: sampled-id mismatches", mism, "of", n_new)
     assert mism <= 1
+
+
+@pytest.mark.parametrize("n", [12, 40])
+def test_path_b_decode_above_8_utterances_vs_oracle(tiny_sd, n):
+    """Decode bodies for 9..64 utterances run on the tensor-core rows path (k_umma_gemm at 2n = 24 / 80 rows: NC = 4 / 16,
+    k_attn_rows at mixed per-row positions).  Three teacher-forced positions through mvb_s1_step_logits for n
+    mixed-length utterances (fp32 KV): every utterance's logits against the CPU oracle, and against the same utterance
+    decoded alone."""
+    import ctypes as C
+    from mvb200 import _lib
+    from oracle import stage1_port as P
+    d = synth.TINY
+    lens = [3 + (7 * i) % 29 for i in range(n)]
+    prompts = [synth.synthetic_prompt(T, seed=200 + i) for i, T in enumerate(lens)]
+    spks = [synth.synthetic_speaker(seed=300 + i) for i in range(n)]
+    feed = lambda i, step: 100 + 37 * i + 11 * step      # noqa: E731  teacher-forced token of utterance i at `step`
+
+    def run(n_slots, which):
+        m = _mk(d, tiny_sd, "fp32", utts=n_slots)
+        lib, h, st = m._lib, m.handle, m._stream()
+        sp = _lib.Sampling(2.0, 1.0, 0.9, 0, 9999, 1)
+        for slot, i in enumerate(which):
+            m.forward(prompts[i].view(1, -1).repeat(2, 1).cuda(), spks[i].cuda(), torch.arange(lens[i]), utt=slot)
+        outs = []
+        for step in range(3):
+            for slot, i in enumerate(which):
+                _lib.check(lib.mvb_s1_begin(h, slot, feed(i, step), lens[i] + step, C.byref(sp), None, None, st))
+            lg = torch.empty(2 * len(which), d.vocab_size, device="cuda")
+            _lib.check(lib.mvb_s1_step_logits(h, len(which), lg.data_ptr(), st))
+            outs.append(lg.cpu())
+        m.close()
+        return outs
+
+    batch = run(n, list(range(n)))
+    worst_o = worst_s = 0.0
+    for i in range(n):
+        o = P.Stage1Oracle(tiny_sd, d.n_head, d.norm_eps, torch.float32, faithful_full_cache=False); o.setup_caches()
+        o.forward(prompts[i].view(1, -1).repeat(2, 1), spks[i], torch.arange(lens[i]))
+        single = run(1, [i])
+        for step in range(3):
+            t = torch.full((2, 1), feed(i, step), dtype=torch.int32)
+            want = o.forward(t, spks[i], torch.tensor([lens[i] + step]))[:, -1]
+            got = batch[step][2 * i:2 * i + 2]
+            worst_o = max(worst_o, _rel(got, want))
+            worst_s = max(worst_s, _rel(got, single[step]))
+    print(f"{n} utterances (R = {2 * n}) on the tensor-core rows path: worst logits rel err vs oracle {worst_o:.2e}, "
+          f"vs single runs {worst_s:.2e}")
+    assert worst_o < TOL and worst_s < TOL
