@@ -147,7 +147,8 @@ int mvb_s1_fetch(mvb_s1* h, int32_t utt, int32_t* out_tokens, int32_t cap, int32
 
 /* Parity hook for the decode body: one decode position (== Transformer.forward with S = 1, fast_model.py:150-163)
  * for utterances [0, n_utts) from the state installed by mvb_s1_begin, through the body mvb_s1_decode runs for that
- * batch: the persistent fused kernel up to 8 utterances (when enabled), the per-layer path otherwise (tensor-core
+ * batch: the persistent fused kernel up to 8 utterances (when enabled and its per-CTA attention tile table can hold every
+ * position of the context), the per-layer path otherwise (tensor-core
  * rows path up to max_utts = 64 utterances); logits fp32 [2*n_utts, vocab] are copied to d_logits, nothing is sampled,
  * positions do not advance (the KV cache is appended at the current positions). */
 int mvb_s1_step_logits(mvb_s1* h, int32_t n_utts, float* d_logits, void* stream);
@@ -229,6 +230,11 @@ int mvb_s2_destroy(mvb_s2* h);
 int mvb_s2_forward(mvb_s2* h, int32_t batch, const int32_t* d_idx, const float* d_spk, float temperature,
                    int32_t top_k, const float* d_noise, uint64_t seed, int32_t* d_tokens, float* d_logits_out,
                    void* stream);
+/* Test hook (not part of the drop-in surface): one stage-2 bidirectional attention (k_s2_attn, launched as
+ * mvb_s2_forward launches it) without an mvb_s2 handle.  d_qkv fp32 [B * t, 3 E] rows {q | k | v}, head h at columns
+ * h * hs of each third (hs = E / n_head, 64 or 128); d_out fp32 [B * t, E] = softmax(q k^T / sqrt(hs)) v per (row block,
+ * head).  Synchronises `stream`. */
+int mvb_s2_attn_test(const float* d_qkv, int32_t B, int32_t t, int32_t E, int32_t n_head, float* d_out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Vocoder, EnCodec-24 kHz decode path: RVQ decode (the diffusion condition `decode_latent`) and the SEANet decoder

@@ -588,6 +588,31 @@ static int launch_persistent(mvb_s1* h, cudaStream_t s, int n_utts, int n_steps,
   return MVB_OK;
 }
 
+// Host-side capacity check of the persistent kernel's per-CTA attention tile table (build_att_table, which traps once a
+// CTA would own more than PC_MAX_TILES tiles).  With G = n_sm CTAs, R = 2 n_utts rows, ppc positions per tile and
+// zmax = max(1, G / (R H)), a row of L <= block_size positions has tt = ceil(L / ppc) <= TT = ceil(block_size / ppc)
+// tiles, cut into nz = ceil(tt / tps) splits of tps = ceil(tt / min(zmax, tt)) tiles.  Then
+//   nz <= min(zmax, tt) <= Z = min(zmax, TT)        (tps >= tt / min(zmax, tt)), and
+//   tps <= ceil(TT / Z)                             (tps = 1 while tt <= zmax, else ceil(tt / zmax) <= ceil(TT / zmax)),
+// so the batch has at most R H Z units of at most ceil(TT / Z) tiles each.  Units are dealt round-robin over the G CTAs,
+// so no CTA owns more than ceil(R H Z / G) units, i.e. ceil(R H Z / G) * ceil(TT / Z) tiles, whatever the positions.
+// The same Z bounds the split count that indexes the PC_MAX_CHUNKS partial slots of every (row, head).
+// At block_size 2048, H = 16 on 132 SMs the worst case (fp32 cache, 8 utterances: Z = 1, TT = 64) is exactly 128.
+static bool pc_att_fits(const mvb_s1* h, int n_utts) {
+  const int R = 2 * n_utts, H = h->cfg.n_head, G = h->n_sm;
+  const int ppc = PC_KV_TILE_BYTES / (128 * (int)h->kv_elem());
+  const long long TT = (h->cfg.block_size + ppc - 1) / ppc;
+  const long long zmax = G / (R * H) > 1 ? G / (R * H) : 1;
+  const long long Z = zmax < TT ? zmax : TT;
+  const long long units_per_cta = ((long long)R * H * Z + G - 1) / G;
+  return Z <= PC_MAX_CHUNKS && units_per_cta * ((TT + Z - 1) / Z) <= PC_MAX_TILES;
+}
+
+// The persistent decode kernel serves the batch (else the per-layer path does).
+static bool use_path_c(const mvb_s1* h, int n_utts) {
+  return h->path_c && h->pc_ok && 2 * n_utts <= PC_RPAD && pc_att_fits(h, n_utts);
+}
+
 static int run_body(mvb_s1* h, cudaStream_t s, int n_utts, bool allow_b = true) {
   // Path A (CUDA-core GEMV) streams the weights once per utterance; from 2 utterances up the tensor-core
   // rows path streams them once per step for the whole batch.  slot_map must be the identity for path B
@@ -817,7 +842,7 @@ extern "C" int mvb_s1_decode(mvb_s1* h, int32_t n_utts, int32_t n_steps, void* s
   k_identity_slots<<<1, 64, 0, s>>>(h->st, n_utts);
   h->launches++;
   CK(cudaGetLastError());
-  const bool use_c = h->path_c && h->pc_ok && 2 * n_utts <= PC_RPAD;
+  const bool use_c = use_path_c(h, n_utts);
   if (use_c) {
     // The persistent kernel ACCUMULATES split-K partial logits (red.add); a prefill (mvb_s1_forward) leaves the last
     // position's logits in the same rows, so they must be zero before the first fused step.  Its grid-barrier counter
@@ -854,7 +879,7 @@ extern "C" int mvb_s1_step_logits(mvb_s1* h, int32_t n_utts, float* d_logits, vo
   k_identity_slots<<<1, 64, 0, s>>>(h->st, n_utts);
   h->launches++;
   CK(cudaGetLastError());
-  if (!(h->path_c && h->pc_ok && 2 * n_utts <= PC_RPAD)) {
+  if (!use_path_c(h, n_utts)) {
     if (int e = run_body(h, s, n_utts)) return e;
     CK(cudaMemcpyAsync(d_logits, h->wsp<float>(h->L.logits), bytes, cudaMemcpyDeviceToDevice, s));
     return MVB_OK;

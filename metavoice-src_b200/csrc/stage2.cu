@@ -367,6 +367,24 @@ extern "C" int mvb_s2_destroy(mvb_s2* h) {
   return MVB_OK;
 }
 
+// Launches the bidirectional attention of one layer exactly as s2_body does.
+static cudaError_t launch_s2_attn(cudaStream_t s, const float* qkv, float* out, int batch, int t, int E, int n_head) {
+  const dim3 ag((t + 31) / 32, n_head, batch);
+  if (E / n_head == 64) k_s2_attn<64><<<ag, 128, 0, s>>>(qkv, out, t, E, n_head);
+  else k_s2_attn<128><<<ag, 128, 0, s>>>(qkv, out, t, E, n_head);
+  return cudaGetLastError();
+}
+
+extern "C" int mvb_s2_attn_test(const float* d_qkv, int32_t B, int32_t t, int32_t E, int32_t n_head, float* d_out, void* stream) {
+  if (!d_qkv || !d_out) return mvb::set_error(MVB_ERR_ARG, "null argument");
+  if (B < 1 || t < 1 || n_head < 1 || E != n_head * (E / n_head) || (E / n_head != 64 && E / n_head != 128))
+    return mvb::set_error(MVB_ERR_UNSUPPORTED, "mvb_s2_attn_test: B, t >= 1 and head size E / n_head of 64 or 128 required");
+  cudaStream_t s = (cudaStream_t)stream;
+  SCK(launch_s2_attn(s, d_qkv, d_out, B, t, E, n_head));
+  SCK(cudaStreamSynchronize(s));
+  return MVB_OK;
+}
+
 // y[rows, M] (+)= f(x)[rows, K] . W^T in passes of 128 rows through the tensor-core GEMM
 template <int EPI>
 static int s2_linear(mvb_s2* h, cudaStream_t s, int rows, const float* x, int ldx, const __nv_bfloat16* gain, int widx, int widx3, int M, int K,
@@ -396,13 +414,9 @@ static int s2_body(mvb_s2* h, cudaStream_t s, int batch, bool has_spk, const flo
   }
   k_s2_embed<<<rows, 128, 0, s>>>(h->idx_stage, c.n_in, t, h->wte_dev, h->w(h->g_wpe()), has_spk ? h->spk_proj : nullptr, h->x, E);
   SCK(cudaGetLastError());
-  const int hs = E / c.n_head;
   for (int l = 0; l < c.n_layer; ++l) {
     if (int e = s2_linear<G_STORE>(h, s, rows, h->x, E, h->w(h->g_layer(l, 0)), l * 5 + 0, l * 5 + 0, 3 * E, E, h->qkv, 3 * E)) return e;
-    dim3 ag((t + 31) / 32, c.n_head, batch);
-    if (hs == 64) k_s2_attn<64><<<ag, 128, 0, s>>>(h->qkv, h->att, t, E, c.n_head);
-    else k_s2_attn<128><<<ag, 128, 0, s>>>(h->qkv, h->att, t, E, c.n_head);
-    SCK(cudaGetLastError());
+    SCK(launch_s2_attn(s, h->qkv, h->att, batch, t, E, c.n_head));
     if (int e = s2_linear<G_RESID>(h, s, rows, h->att, E, nullptr, l * 5 + 1, l * 5 + 1, E, E, h->x, E)) return e;
     if (int e = s2_linear<G_SWIGLU>(h, s, rows, h->x, E, h->w(h->g_layer(l, 3)), l * 5 + 2, l * 5 + 3, Hd, E, h->ffn, Hd)) return e;
     if (int e = s2_linear<G_RESID>(h, s, rows, h->ffn, Hd, nullptr, l * 5 + 4, l * 5 + 4, E, Hd, h->x, E)) return e;

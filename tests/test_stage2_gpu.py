@@ -82,3 +82,23 @@ def test_stage2_graph_replay_equals_eager_launches(monkeypatch):
         b = eager.forward_tokens(idx, spk, temp, 200, seed=seed).cpu()
         assert torch.equal(a, b)
     assert not torch.equal(graph.forward_tokens(idx, spk, 1.0, 200, seed=7).cpu(), graph.forward_tokens(idx, spk, 1.0, 200, seed=9).cpu())
+
+
+@pytest.mark.parametrize("tag,dims", [("tiny", synth.S2_TINY),
+                                      ("head128", synth.Stage2Dims(n_layer=2, n_head=2, n_embd=256, block_size=256))])
+def test_stage2_logits_vs_oracle_port(tag, dims):
+    """Head size 64 (k_s2_attn<64>) and 128 (k_s2_attn<128>) through the captured graph of mvb_s2_forward, against the
+    float64 oracle port on the same checkpoint, input and speaker."""
+    from mvb200.second_stage import SecondStage
+    from oracle import stage2_port as P
+    ck = synth.stage2_checkpoint(dims, 1)
+    m = SecondStage(ck, device="cuda:0")
+    text, cb0, cb1 = synth.synthetic_stage2_input(dims, 50)
+    idx = m.build_input(text, [cb0, cb1])[None]
+    spk = synth.synthetic_speaker(seed=2)[None]
+    _, lg = m.forward_tokens(idx, spk, 1.0, 200, seed=3, return_logits=True)
+    o = P.Stage2Oracle(ck["model"], dims.n_head, dims.rmsnorm_eps, dtype=torch.float64)
+    ref = torch.stack([l[0] for l in o.forward(idx.long(), spk.double())])
+    err = float((lg.cpu().double() - ref).abs().max() / ref.abs().max())
+    print(f"stage-2 {tag} (head size {dims.n_embd // dims.n_head}): logits rel err vs float64 oracle {err:.2e}")
+    assert err < 1e-4
