@@ -175,7 +175,7 @@ int mvb_linear(const void* d_W, int32_t M, int32_t K, const float* d_x, int32_t 
                int32_t ldo, int32_t accumulate, void* stream);
 
 /* Test hooks for the op-level tests of two tensor-core kernels (not part of the drop-in surface):
- *   mvb_gemm_test     : mvb_linear's operator with any epilogue of the weight-streaming GEMM (csrc/umma_gemm.cuh):
+ *   mvb_gemm_test     : mvb_linear's operator with any epilogue of the weight-streaming GEMM (csrc/tc_gemm.cuh):
  *                       epi 0 store, 1 residual add, 2 SwiGLU  out = silu(x W^T) * (x W3^T)  (d_W3 bf16 [M, K]),
  *                       3 QKV  out = x W^T plus the K / V thirds scattered to d_kcache / d_vcache
  *                       [rows][H][S_max][128] (fp32 when kv_fp32, else bf16) at cache row d_row_cache[n], position

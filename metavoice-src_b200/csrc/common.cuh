@@ -53,6 +53,26 @@ __device__ __forceinline__ void fma8(float& acc, const uint4& w, const float4& a
   acc = fmaf(bf_hi(w.w), b.w, acc);
 }
 
+// Bound of every spin wait (mbarrier, grid counter): 4e9 cycles (~2 s at H100 clocks).  A protocol bug must surface as
+// a launch failure, never as a hung GPU.
+__device__ __forceinline__ void trap_if_stuck(long long t0) {
+  if (clock64() - t0 > 4000000000ll) __trap();
+}
+
+__device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
+  unsigned v;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void red_release_inc(unsigned* p) {
+  asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(p) : "memory");
+}
+// Grid-wide counter wait: spin until *ctr >= target, with acquire ordering (pairs with red_release_inc / atomics).
+__device__ __forceinline__ void wait_counter(const unsigned* ctr, unsigned target) {
+  const long long t0 = clock64();
+  while (ld_acquire_u32(ctr) < target) trap_if_stuck(t0);
+}
+
 // Programmatic dependent launch: let the next kernel in the stream start its independent
 // prologue early / wait for the previous kernel's memory to be visible.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }

@@ -30,7 +30,7 @@
 //     embeds the next token.
 #pragma once
 #include "stage1_kernels.cuh"
-#include "umma.cuh"
+#include "tc.cuh"
 
 namespace mvb {
 
@@ -136,35 +136,13 @@ struct PcParams {
 };
 
 // ---- small device helpers -------------------------------------------------------------------------
-__device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
-  unsigned v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void red_release_inc(unsigned* p) {
-  asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(p) : "memory");
-}
 __device__ __forceinline__ void compute_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-__device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1, int c2, uint64_t pol) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4, %5}], [%2], %6;"
-      ::"r"(dst), "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "l"(pol) : "memory");
-}
-// Pull a weight tile into L2 only (no smem, no barrier): HBM keeps streaming while the ring is full.
-__device__ __forceinline__ void tma_prefetch_3d(const void* tmap, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];" ::"l"(tmap), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
 // byte offset of the 16-byte chunk holding k..k+7 of activation row `row` inside the activation operand
 // (K-major, 128B swizzle, [k-block][NB rows][128 B])
 template <int NB>
 __device__ __forceinline__ uint32_t b_chunk_off(int kb_local, int row, int kchunk /* (k % 64) / 8 */) {
-  return (uint32_t)(kb_local * (NB * 128) + (row >> 3) * 1024 + (row & 7) * 128 + ((kchunk ^ (row & 7)) << 4));
+  return (uint32_t)(kb_local * (NB * 128)) + sw128_off(row, kchunk);
 }
 
 // split 8 fp32 into bf16 hi / lo and store both rows' chunks
@@ -172,13 +150,7 @@ template <int NB>
 __device__ __forceinline__ void b_store8(uint8_t* B, int kb_local, int n, int kchunk, const float (&v)[8]) {
   uint32_t hi[4], lo[4];
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const __nv_bfloat16 h0 = __float2bfloat16_rn(v[2 * i]), h1 = __float2bfloat16_rn(v[2 * i + 1]);
-    const __nv_bfloat16 l0 = __float2bfloat16_rn(v[2 * i] - __bfloat162float(h0));
-    const __nv_bfloat16 l1 = __float2bfloat16_rn(v[2 * i + 1] - __bfloat162float(h1));
-    hi[i] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-    lo[i] = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
-  }
+  for (int i = 0; i < 4; ++i) pack_hi_lo(v[2 * i], v[2 * i + 1], hi[i], lo[i]);
   *reinterpret_cast<uint4*>(B + b_chunk_off<NB>(kb_local, n, kchunk)) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
   *reinterpret_cast<uint4*>(B + b_chunk_off<NB>(kb_local, NB / 2 + n, kchunk)) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
 }
@@ -262,13 +234,6 @@ __device__ __forceinline__ int float_to_ordered(float f) {
   return i >= 0 ? i : i ^ 0x7fffffff;
 }
 __device__ __forceinline__ float ordered_to_float(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7fffffff); }
-// (x0, x1) -> packed bf16 pair of the high terms and of the residuals (x = hi + lo to 2^-17)
-__device__ __forceinline__ void pack_hi_lo(float x0, float x1, uint32_t& hi, uint32_t& lo) {
-  const __nv_bfloat16 h0 = __float2bfloat16_rn(x0), h1 = __float2bfloat16_rn(x1);
-  const __nv_bfloat16 l0 = __float2bfloat16_rn(x0 - __bfloat162float(h0)), l1 = __float2bfloat16_rn(x1 - __bfloat162float(h1));
-  hi = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-  lo = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
-}
 
 // acc[m][c] += W[16 m .. 16 m + 15][0 .. 63] * (hi + lo)[8 c .. 8 c + 7][0 .. 63] over one weight stage (128 rows x 64 k)
 // and one k-block of the activation operand (NB rows: RH hi rows, then RH lo rows).  One warp, mma.sync.m16n8k16.
@@ -282,15 +247,13 @@ __device__ __forceinline__ void pc_mma_stage(uint32_t w_base, uint32_t x_base, i
 #pragma unroll
     for (int g = 0; g < NB / 16; ++g) {   // rows 16 g .. 16 g + 15: two n8 chunks, both k halves
       uint32_t r[4];
-      const int row = 16 * g + r8 + ((q >> 1) << 3);
-      ldsm_x4(x_base + sw128_off(row, 2 * kk + (q & 1)), r);
+      ldsm_b(x_base, 16 * g, kk, q, r8, r);
       b[2 * g][0] = r[0]; b[2 * g][1] = r[1]; b[2 * g + 1][0] = r[2]; b[2 * g + 1][1] = r[3];
     }
 #pragma unroll
     for (int m = 0; m < 8; ++m) {
       uint32_t a[4];
-      const int row = 16 * m + r8 + ((q & 1) << 3);
-      ldsm_x4(w_base + sw128_off(row, 2 * kk + (q >> 1)), a);
+      ldsm_a(w_base, 16 * m, kk, q, r8, a);
 #pragma unroll
       for (int c = 0; c < NC; ++c) {
         mma_bf16_16816(acc[m][c], a, b[c][0], b[c][1]);            // hi rows
@@ -326,10 +289,7 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
   constexpr int TILE_ROWS = Cfg::TILE_ROWS;
   constexpr int SG = 2;   // activation chunks staged per thread per trip (3-4 were measured: the arrays spill, staging gets slower)
   extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment by POINTER ARITHMETIC on the shared array: an integer round trip would lose the .shared state
-  // space and turn every access below into a generic LD/ST (higher latency, no LDS/STS)
-  uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* ring = smem;
+  uint8_t* ring = smem_raw + smem_pad_1024(smem_raw);
   uint8_t* Bop = ring + STAGES * STAGE_BYTES;
   float* accbuf = reinterpret_cast<float*>(Bop + Cfg::B_BYTES);   // [2][RH][ACC_LD]: MMA warp -> epilogue
   uint8_t* kvbuf = Bop + Cfg::B_BYTES + Cfg::ACC_BYTES;     // [NKV][K tile | V tile]; sampler scratch between tokens
@@ -361,7 +321,7 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
   // zero the activation operand once: rows >= R (hi and lo halves) must read as zero forever
   for (int i = tid; i < Cfg::B_BYTES / 16; i += PC_THREADS) reinterpret_cast<uint4*>(Bop)[i] = make_uint4(0, 0, 0, 0);
   if (tid < PC_RPAD) sh.ss[tid] = 0.f;
-  fence_async_smem();
+  ptx::fence_async_smem();
   __syncthreads();
   pdl_launch_dependents();
 
@@ -397,7 +357,7 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
       const int ti = m / nk, kb = sl->kb0 + (m - ti * nk);
       int t = sl->t0 + ti * sl->G;
       if (sl == &s_w13 && t >= T1) { t -= T1; tm = &tm_w3; }
-      if (ptx::elect_one()) tma_prefetch_3d(tm, kb * 64, t * TILE_ROWS, layer);
+      if (ptx::elect_one()) ptx::tma_prefetch_3d(tm, kb * 64, t * TILE_ROWS, layer);
       __syncwarp();
     };
     const long long total_all = (long long)total_tiles * p.n_steps;
@@ -427,7 +387,7 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
           const CUtensorMap* tm = (t < split_t) ? tmA : tmB2;
           const int tt = (t < split_t) ? t : t - split_t;
           for (int kb = sl.kb0; kb < sl.kb1; ++kb) {
-            const uint32_t s = slot % STAGES, ph = (slot / STAGES) & 1u;
+            const auto [s, ph] = ring_pos(slot, STAGES);
             ++slot;
             const uint32_t eb = ptx::smem_u32(sh.b_empty + s);
             if (p.pf_mode == 1 && !ptx::mbar_test_wait(eb, ph ^ 1u)) {
@@ -443,7 +403,7 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
             if (ptx::elect_one()) {
               const uint32_t full = ptx::smem_u32(sh.b_full + s);
               ptx::mbar_arrive_expect_tx(full, STAGE_BYTES);
-              tma_load_3d(ptx::smem_u32(ring + (size_t)s * STAGE_BYTES), tm, full, kb * 64, tt * TILE_ROWS, layer, pol);
+              ptx::tma_load_3d_hint(ptx::smem_u32(ring + (size_t)s * STAGE_BYTES), tm, full, kb * 64, tt * TILE_ROWS, layer, pol);
               asm volatile("st.shared.u32 [%0], %1;" ::"r"(pp), "r"((int)issued) : "memory");
             }
             __syncwarp();
@@ -463,7 +423,7 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
           const int my = idx++;
           if (my < from) continue;
           if (my >= to) break;
-          const uint32_t ks = kv_ctr % Cfg::NKV, ph = (kv_ctr / Cfg::NKV) & 1u;
+          const auto [ks, ph] = ring_pos(kv_ctr, Cfg::NKV);
           ++kv_ctr;
           ptx::mbar_wait(ptx::smem_u32(sh.kv_empty + ks), ph ^ 1u);
           if (ptx::elect_one()) {
@@ -482,8 +442,8 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
             } else {
               const uint32_t bytes = (uint32_t)npos * 128 * esz;
               ptx::mbar_arrive_expect_tx(full, 2 * bytes);
-              bulk_load(ptx::smem_u32(dst), kbase + e.off, bytes, full);
-              bulk_load(ptx::smem_u32(dst + PC_KV_TILE_BYTES), vbase + e.off, bytes, full);
+              ptx::bulk_load(ptx::smem_u32(dst), kbase + e.off, bytes, full);
+              ptx::bulk_load(ptx::smem_u32(dst + PC_KV_TILE_BYTES), vbase + e.off, bytes, full);
             }
           }
           __syncwarp();
@@ -538,7 +498,7 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
       ptx::mbar_wait(ptx::smem_u32(&sh.b_ready), bphase & 1u);   // activation operand of this phase staged
       ++bphase;
       for (int i = 0; i < sl.nt; ++i) {
-        const uint32_t ab = tile_ctr & 1u, aph = (tile_ctr >> 1) & 1u;
+        const auto [ab, aph] = ring_pos(tile_ctr, 2);
         float acc[8][NB / 16][4];
 #pragma unroll
         for (int m = 0; m < 8; ++m)
@@ -547,7 +507,7 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
 #pragma unroll
             for (int e = 0; e < 4; ++e) acc[m][c][e] = 0.f;
         for (int kb = sl.kb0; kb < sl.kb1; ++kb) {
-          const uint32_t s = slot % STAGES, ph = (slot / STAGES) & 1u;
+          const auto [s, ph] = ring_pos(slot, STAGES);
           ++slot;
           ptx::mbar_wait(ptx::smem_u32(sh.b_full + s), ph);
           pc_mma_stage<NB>(ring_u32 + s * STAGE_BYTES, bop_u32 + (uint32_t)(kb - sl.kb0) * (NB * 128), lane, acc);
@@ -599,17 +559,11 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
       ++bar_idx;
     };
     auto grid_wait = [&]() {            // wait for arrival #bar_idx of every CTA
-      if (ct == 0) {
-        const unsigned target = bar_idx * (unsigned)G;
-        const long long t0 = clock64();
-        while (ld_acquire_u32(p.bar) < target) {
-          if (clock64() - t0 > 4000000000ll) __trap();
-        }
-      }
+      if (ct == 0) wait_counter(p.bar, bar_idx * (unsigned)G);
       compute_sync();
     };
     auto b_publish = [&]() {            // generic-proxy smem writes -> visible to the tensor core
-      fence_async_smem();
+      ptx::fence_async_smem();
       compute_sync();
       if (ct == 0) ptx::mbar_arrive(ptx::smem_u32(&sh.b_ready));
     };
@@ -712,7 +666,7 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
     auto epilogue = [&](const PcSlice& sl, float* out, int ldo, int M, int split_t, float* out2) {
       for (int i = 0; i < sl.nt; ++i) {
         const int t = sl.t0 + i * sl.G;
-        const uint32_t ab = tile_ctr & 1u, aph = (tile_ctr >> 1) & 1u;
+        const auto [ab, aph] = ring_pos(tile_ctr, 2);
         ++tile_ctr;
         float* o = (t < split_t) ? out : out2;
         const int col0 = ((t < split_t) ? t : t - split_t) * TILE_ROWS;
@@ -908,7 +862,7 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
             }
             PC_ATT_MARK(1)
             if (npos > 0) {
-              const uint32_t ks = kv_ctr % Cfg::NKV, ph = (kv_ctr / Cfg::NKV) & 1u;
+              const auto [ks, ph] = ring_pos(kv_ctr, Cfg::NKV);
               ++kv_ctr;
               ptx::mbar_wait(ptx::smem_u32(sh.kv_full + ks), ph);
               PC_ATT_MARK(2)
@@ -926,7 +880,7 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
                 for (int k8 = 0; k8 < 8; ++k8) {
                   const int chunk = ((k8 & 3) << 1) + (mat >> 1);
                   uint32_t a[4];
-                  ldsm_x4(kt + (uint32_t)((k8 >> 2) * 8192 + rr * 128 + ((chunk ^ (rr & 7)) << 4)), a);
+                  ldsm_x4(kt + (uint32_t)((k8 >> 2) * 8192) + sw128_off(rr, chunk), a);
                   const uint32_t bh0 = lane < 4 ? q_hi[k8 * 8 + t4] : 0u, bh1 = lane < 4 ? q_hi[k8 * 8 + t4 + 4] : 0u;
                   const uint32_t bl0 = lane < 4 ? q_lo[k8 * 8 + t4] : 0u, bl1 = lane < 4 ? q_lo[k8 * 8 + t4 + 4] : 0u;
                   mma_bf16_16816(c4[(k8 & 1) * 2], a, bh0, bh1);
@@ -976,7 +930,7 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
                     const int d0 = 32 * cw + 16 * mb;
                     const int chunk = ((d0 & 63) >> 3) + (mat & 1);
                     uint32_t a[4];
-                    ldsm_x4_t(vt + (uint32_t)((d0 >> 6) * 8192 + pos * 128 + ((chunk ^ (pos & 7)) << 4)), a);
+                    ldsm_x4_t(vt + (uint32_t)((d0 >> 6) * 8192) + sw128_off(pos, chunk), a);
                     mma_bf16_16816(oacc[mb], a, bh0, bh1);
                     mma_bf16_16816(olo[mb], a, bl0, bl1);
                   }
@@ -987,7 +941,7 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
               PC_ATT_MARK(3)
             }
             if (npos > 0 || has_cur) compute_sync();   // KV tile fully consumed; sh.cur visible
-            if (npos > 0 && ct == 0) ptx::mbar_arrive(ptx::smem_u32(sh.kv_empty + ((kv_ctr - 1) % Cfg::NKV)));
+            if (npos > 0 && ct == 0) ptx::mbar_arrive(ptx::smem_u32(sh.kv_empty + ring_pos(kv_ctr - 1, Cfg::NKV).stage));
             if (has_cur) {
               // the current token (its k, v never left the chip): every warp applies the same update to its dims
               float sd = 0.f;
@@ -1089,7 +1043,7 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
             }
             PC_ATT_MARK(1)
             if (npos > 0) {
-              const uint32_t ks = kv_ctr % Cfg::NKV, ph = (kv_ctr / Cfg::NKV) & 1u;
+              const auto [ks, ph] = ring_pos(kv_ctr, Cfg::NKV);
               ++kv_ctr;
               ptx::mbar_wait(ptx::smem_u32(sh.kv_full + ks), ph);
               PC_ATT_MARK(2)
@@ -1135,7 +1089,7 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
               }
             }
             if (npos > 0 || has_cur) compute_sync();   // KV tile fully consumed; sh.cur visible
-            if (npos > 0 && ct == 0) ptx::mbar_arrive(ptx::smem_u32(sh.kv_empty + ((kv_ctr - 1) % Cfg::NKV)));
+            if (npos > 0 && ct == 0) ptx::mbar_arrive(ptx::smem_u32(sh.kv_empty + ring_pos(kv_ctr - 1, Cfg::NKV).stage));
             if (has_cur && hw == 0) {
               float sdot = 0.f;
 #pragma unroll

@@ -1,10 +1,10 @@
-// Standalone tensor-core linear operator (C ABI): y[R, M] (+)= f(x)[R, K] . W[M, K]^T with W in bf16.
-// Used by the parity tests to validate the TMA / mma.sync path in isolation and by the stage-2 model.
+// The weight-streaming tensor-core GEMM: tc_gemm, which the stage-1 and stage-2 engines call, and the standalone
+// operator of the C ABI, y[R, M] (+)= f(x)[R, K] . W[M, K]^T with W in bf16, that tests use to check it in isolation.
 #include <cstdio>
 #include <string>
 
 #include "../../include/mvb200.h"
-#include "umma_host.cuh"
+#include "tc_gemm.cuh"
 
 using namespace mvb;
 
@@ -20,36 +20,71 @@ namespace mvb { int set_error(int code, const char* fmt, ...); }
     }                                                                                               \
   } while (0)
 
+namespace mvb {
+
+template <int EPI, int NC>
+static cudaError_t launch_tc_gemm_nc(cudaStream_t s, const CUtensorMap& tA, const CUtensorMap& tA3, const CUtensorMap& tB,
+                                     const GemmP& p, const GemmPlan& g) {
+  static PerDeviceOnce attr_set;
+  if (attr_set.pending()) {
+    cudaError_t e = cudaFuncSetAttribute(k_tc_gemm<EPI, NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    if (e != cudaSuccess) return e;
+    attr_set.mark();
+  }
+  k_tc_gemm<EPI, NC><<<dim3(g.tiles, g.ksplit), GEMM_THREADS, g.smem_bytes, s>>>(tA, tA3, tB, p);
+  return cudaGetLastError();
+}
+
+// The accumulator size is a template parameter (registers): the smallest of 16 / 32 / 64 / 128 columns that holds Rpad.
+template <int EPI>
+static cudaError_t launch_tc_gemm(cudaStream_t s, const CUtensorMap& tA, const CUtensorMap& tA3, const CUtensorMap& tB,
+                                  GemmP p, const GemmPlan& g) {
+  p.ksplit = g.ksplit;
+  p.stages = g.stages;
+  if (p.Rpad <= 16) return launch_tc_gemm_nc<EPI, 2>(s, tA, tA3, tB, p, g);
+  if (p.Rpad <= 32) return launch_tc_gemm_nc<EPI, 4>(s, tA, tA3, tB, p, g);
+  if (p.Rpad <= 64) return launch_tc_gemm_nc<EPI, 8>(s, tA, tA3, tB, p, g);
+  return launch_tc_gemm_nc<EPI, 16>(s, tA, tA3, tB, p, g);
+}
+
+cudaError_t tc_gemm(cudaStream_t s, const TcGemm& a) {
+  if (a.Rpad < 16 || a.Rpad > 128 || a.Rpad % 16) return cudaErrorInvalidValue;
+  const int NB = a.Rpad * (a.split_lo ? 2 : 1);
+  k_prep_b<<<a.Rpad, 256, 0, s>>>(a.x, a.ldx, a.gain, a.eps, a.K, a.Rpad, a.R, a.split_lo ? 1 : 0, a.B);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  GemmP p{};
+  p.M = a.M; p.K = a.K; p.NB = NB; p.Rpad = a.Rpad; p.R = a.R; p.split_lo = a.split_lo ? 1 : 0;
+  p.scratch = a.scratch; p.tickets = a.tickets; p.out = a.out; p.ldo = a.ldo;
+  p.kcache = a.kcache; p.vcache = a.vcache; p.row_cache = a.row_cache; p.row_pos = a.row_pos;
+  p.H = a.H; p.S_max = a.S_max; p.D = a.D; p.kv_fp32 = a.kv_fp32 ? 1 : 0;
+  const GemmPlan g = plan_gemm(a.M, a.K, NB, a.epi == G_SWIGLU, a.n_sm, a.ksplit);
+  const CUtensorMap& tA3 = a.epi == G_SWIGLU ? *a.tmW3 : *a.tmW;
+  switch (a.epi) {
+    case G_STORE: return launch_tc_gemm<G_STORE>(s, *a.tmW, tA3, *a.tmB, p, g);
+    case G_RESID: return launch_tc_gemm<G_RESID>(s, *a.tmW, tA3, *a.tmB, p, g);
+    case G_SWIGLU: return launch_tc_gemm<G_SWIGLU>(s, *a.tmW, tA3, *a.tmB, p, g);
+    default: return launch_tc_gemm<G_QKV>(s, *a.tmW, tA3, *a.tmB, p, g);
+  }
+}
+
+}  // namespace mvb
+
 namespace {
 
-// Fields of GemmP the caller chooses for one epilogue: the output and, for G_QKV, the KV-cache scatter.
-struct EpiArgs {
-  float* out; int ldo;
-  void* kcache; void* vcache; const int* row_cache; const int* row_pos;
-  int H, S_max, D, kv_fp32;
-};
-
-// One k_umma_gemm launch with the RMSNorm / hi-lo prologue of k_prep_b, for any epilogue (W3 is the second weight of
-// G_SWIGLU).  Synchronises `s`.
-int run_gemm(int epi, const void* d_W, const void* d_W3, int M, int K, const float* d_x, int ldx, int R, const void* d_gain,
-             float eps, int split_lo, int ksplit_override, const EpiArgs& ea, cudaStream_t s) {
+// mvb_linear / mvb_gemm_test: `a` carries the rows, the epilogue and the ksplit override; the B buffer, scratch and
+// tickets come from buffers cached per device that only ever grow (no allocation on the steady-state path; this
+// standalone operator has no caller-provided workspace, unlike the engine handles).  W3 is the second weight of
+// G_SWIGLU.  Synchronises `s`.
+int run_gemm(TcGemm a, const void* d_W, const void* d_W3, cudaStream_t s) {
   int rc = MVB_OK;
-  const bool swiglu = epi == G_SWIGLU;
-  const int Rpad = (R + 15) / 16 * 16;
-  const int NB = Rpad * (split_lo ? 2 : 1);
-  int n_sm = 132, dev = 0;
+  a.Rpad = (a.R + 15) / 16 * 16;
+  const int NB = a.Rpad * (a.split_lo ? 2 : 1);
+  int dev = 0;
+  a.n_sm = 132;
   cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
-  GemmPlan g = plan_gemm(M, K, NB, swiglu, n_sm);
-  if (ksplit_override > 0) {
-    // every split of a tile waits for its siblings inside the kernel: all tiles x ksplit CTAs must be co-resident
-    const int cap = n_sm / g.tiles > 0 ? n_sm / g.tiles : 1;
-    g.ksplit = ksplit_override < cap ? ksplit_override : cap;
-    if (g.tiles > 128) g.ksplit = 1;
-    g.scratch_floats = (size_t)g.tiles * g.ksplit * (swiglu ? 2 : 1) * NB * 128;
-  }
-  // Scratch buffers are cached per device and only ever grow (no allocation on the steady-state path; this standalone
-  // operator has no caller-provided workspace, unlike the engine handles).
+  cudaDeviceGetAttribute(&a.n_sm, cudaDevAttrMultiProcessorCount, dev);
+  const GemmPlan g = plan_gemm(a.M, a.K, NB, a.epi == G_SWIGLU, a.n_sm, a.ksplit);
   struct Cache { void* p = nullptr; size_t cap = 0; };
   static Cache cB[16], cS[16], cT[16];
   auto ensure = [&](Cache& c, size_t bytes) -> cudaError_t {
@@ -61,37 +96,23 @@ int run_gemm(int epi, const void* d_W, const void* d_W3, int M, int K, const flo
     return e;
   };
   if (dev < 0 || dev >= 16) return mvb::set_error(MVB_ERR_UNSUPPORTED, "mvb_linear: device index %d", dev);
-  __nv_bfloat16* B = nullptr;
-  float* scratch = nullptr;
-  unsigned* tickets = nullptr;
   CUtensorMap tA, tA3, tB;
-  GemmP p{};
-  LCK(ensure(cB[dev], (size_t)NB * K * 2));
+  LCK(ensure(cB[dev], (size_t)NB * a.K * 2));
   LCK(ensure(cS[dev], sizeof(float) * (g.scratch_floats ? g.scratch_floats : 1)));
   LCK(ensure(cT[dev], sizeof(unsigned) * 256));
-  B = reinterpret_cast<__nv_bfloat16*>(cB[dev].p);
-  scratch = reinterpret_cast<float*>(cS[dev].p);
-  tickets = reinterpret_cast<unsigned*>(cT[dev].p);
-  LCK(cudaMemsetAsync(B, 0, (size_t)NB * K * 2, s));
-  LCK(cudaMemsetAsync(tickets, 0, sizeof(unsigned) * 256, s));
-  if (!make_tmap_bf16(&tA, d_W, (uint64_t)M, (uint64_t)K, 128) ||
-      (swiglu && !make_tmap_bf16(&tA3, d_W3, (uint64_t)M, (uint64_t)K, 128)) ||
-      !make_tmap_bf16(&tB, B, (uint64_t)NB, (uint64_t)K, (uint32_t)NB)) {
+  a.B = reinterpret_cast<__nv_bfloat16*>(cB[dev].p);
+  a.scratch = reinterpret_cast<float*>(cS[dev].p);
+  a.tickets = reinterpret_cast<unsigned*>(cT[dev].p);
+  LCK(cudaMemsetAsync(a.B, 0, (size_t)NB * a.K * 2, s));
+  LCK(cudaMemsetAsync(a.tickets, 0, sizeof(unsigned) * 256, s));
+  if (!make_tmap_bf16(&tA, d_W, (uint64_t)a.M, (uint64_t)a.K, 128) ||
+      (a.epi == G_SWIGLU && !make_tmap_bf16(&tA3, d_W3, (uint64_t)a.M, (uint64_t)a.K, 128)) ||
+      !make_tmap_bf16(&tB, a.B, (uint64_t)NB, (uint64_t)a.K, (uint32_t)NB)) {
     rc = mvb::set_error(MVB_ERR_CUDA, "cuTensorMapEncodeTiled failed");
     goto done;
   }
-  k_prep_b<<<Rpad, 256, 0, s>>>(d_x, ldx, reinterpret_cast<const __nv_bfloat16*>(d_gain), eps, K, Rpad, R, split_lo ? 1 : 0, B);
-  LCK(cudaGetLastError());
-  p.M = M; p.K = K; p.NB = NB; p.Rpad = Rpad; p.R = R; p.split_lo = split_lo ? 1 : 0;
-  p.scratch = scratch; p.tickets = tickets; p.out = ea.out; p.ldo = ea.ldo;
-  p.kcache = ea.kcache; p.vcache = ea.vcache; p.row_cache = ea.row_cache; p.row_pos = ea.row_pos;
-  p.H = ea.H; p.S_max = ea.S_max; p.D = ea.D; p.kv_fp32 = ea.kv_fp32 ? 1 : 0;
-  switch (epi) {
-    case G_STORE: LCK(launch_umma_gemm<G_STORE>(s, tA, tA, tB, p, g)); break;
-    case G_RESID: LCK(launch_umma_gemm<G_RESID>(s, tA, tA, tB, p, g)); break;
-    case G_SWIGLU: LCK(launch_umma_gemm<G_SWIGLU>(s, tA, tA3, tB, p, g)); break;
-    default: LCK(launch_umma_gemm<G_QKV>(s, tA, tA, tB, p, g)); break;
-  }
+  a.tmW = &tA; a.tmW3 = &tA3; a.tmB = &tB;
+  LCK(tc_gemm(s, a));
   LCK(cudaStreamSynchronize(s));
 done:
   return rc;
@@ -104,10 +125,12 @@ extern "C" int mvb_linear(const void* d_W, int32_t M, int32_t K, const float* d_
                           int32_t ldo, int32_t accumulate, void* stream) {
   if (!d_W || !d_x || !d_out) return mvb::set_error(MVB_ERR_ARG, "null argument");
   if (K % 64 || R < 1 || R > 128) return mvb::set_error(MVB_ERR_UNSUPPORTED, "mvb_linear: K %% 64 == 0 and 1 <= R <= 128 required");
-  EpiArgs ea{};
-  ea.out = d_out; ea.ldo = ldo;
-  return run_gemm(accumulate ? G_RESID : G_STORE, d_W, nullptr, M, K, d_x, ldx, R, d_gain, eps, split_lo, ksplit_override, ea,
-                  (cudaStream_t)stream);
+  TcGemm a{};
+  a.epi = accumulate ? G_RESID : G_STORE;
+  a.x = d_x; a.ldx = ldx; a.gain = reinterpret_cast<const __nv_bfloat16*>(d_gain); a.eps = eps;
+  a.M = M; a.K = K; a.R = R; a.split_lo = split_lo; a.ksplit = ksplit_override;
+  a.out = d_out; a.ldo = ldo;
+  return run_gemm(a, d_W, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" int mvb_gemm_test(int32_t epi, const void* d_W, const void* d_W3, int32_t M, int32_t K, const float* d_x, int32_t ldx,
@@ -125,9 +148,12 @@ extern "C" int mvb_gemm_test(int32_t epi, const void* d_W, const void* d_W3, int
     if (D < 128 || D != 128 * H || M != 3 * D || S_max < 1)
       return mvb::set_error(MVB_ERR_UNSUPPORTED, "mvb_gemm_test: QKV needs D == 128 H, M == 3 D, S_max >= 1");
   }
-  EpiArgs ea{};
-  ea.out = d_out; ea.ldo = ldo;
-  ea.kcache = d_kcache; ea.vcache = d_vcache; ea.row_cache = d_row_cache; ea.row_pos = d_row_pos;
-  ea.H = H; ea.S_max = S_max; ea.D = D; ea.kv_fp32 = kv_fp32;
-  return run_gemm(epi, d_W, d_W3, M, K, d_x, ldx, R, d_gain, eps, split_lo, ksplit_override, ea, (cudaStream_t)stream);
+  TcGemm a{};
+  a.epi = epi;
+  a.x = d_x; a.ldx = ldx; a.gain = reinterpret_cast<const __nv_bfloat16*>(d_gain); a.eps = eps;
+  a.M = M; a.K = K; a.R = R; a.split_lo = split_lo; a.ksplit = ksplit_override;
+  a.out = d_out; a.ldo = ldo;
+  a.kcache = d_kcache; a.vcache = d_vcache; a.row_cache = d_row_cache; a.row_pos = d_row_pos;
+  a.H = H; a.S_max = S_max; a.D = D; a.kv_fp32 = kv_fp32;
+  return run_gemm(a, d_W, d_W3, (cudaStream_t)stream);
 }

@@ -20,7 +20,7 @@
 #include "../../include/mvb200.h"
 #include "common.cuh"
 #include "mbd_tc.cuh"
-#include "umma_host.cuh"
+#include "tc_gemm_host.cuh"
 
 using namespace mvb;
 namespace mvb { int set_error(int code, const char* fmt, ...); }

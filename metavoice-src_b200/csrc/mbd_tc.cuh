@@ -8,14 +8,14 @@
 // s output phases with two taps each.  One CTA = 128 output channels x 128 time columns: A tiles (weights, 16 KB) and the
 // two B tiles (hi, lo: 128 rows each) arrive by TMA into a 4-stage ring; eight consumer warps own 16 output channels each
 // and run ldmatrix + mma.sync.m16n8k16 over all 128 columns, the hi and lo products accumulating into one fp32 register
-// tile.  The epilogue adds bias, transposes each warp's 16 x 128 block through shared memory (the drained ring) and adds
-// the residual / stores channel-major rows with the lanes along time (coalesced).
+// tile (tc_mainloop, shared with the weight-streaming GEMM).  The epilogue adds bias, transposes each warp's 16 x 128
+// block through shared memory (the drained ring) and adds the residual / stores channel-major rows with the lanes along
+// time (coalesced).
 //
 // Numerics: weights are rounded to bf16 (the reference's own convolutions run in TF32 under torch's cuDNN default
 // `allow_tf32=True`, 10-bit mantissa on BOTH operands); activations are exact to 2^-17; accumulation is fp32.
 #pragma once
-#include "common.cuh"
-#include "umma.cuh"
+#include "tc.cuh"
 
 namespace mvb {
 
@@ -39,88 +39,38 @@ constexpr int TC_TP_LD = 128 + 4;        // epilogue transpose tile [16][TC_TP_L
 constexpr size_t TC_SMEM = 1024 + (size_t)TC_STAGES * TC_STAGE_BYTES + 2 * TC_STAGES * 8 + 64;
 static_assert(8 * 16 * TC_TP_LD * 4 <= TC_STAGES * TC_STAGE_BYTES, "transpose tiles must fit in the ring");
 
-__device__ __forceinline__ void tc_tma3(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-               ::"r"(dst), "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-
 static __global__ void __launch_bounds__(TC_THREADS, 1)
 k_mbd_tc_conv(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmBhi,
               const __grid_constant__ CUtensorMap tmBlo, const TcConvP p) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
-  constexpr int S = TC_STAGES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)S * TC_STAGE_BYTES);   // full[S], empty[S]
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  uint8_t* smem = smem_raw + smem_pad_1024(smem_raw);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_cot = (p.M + 127) >> 7;
   const int ph = blockIdx.x / n_cot, cot = blockIdx.x - ph * n_cot;
   const int t0 = blockIdx.y * 128;
   const int nkb = p.Cin >> 6;
-  const int n_it = p.taps.n_slots * nkb;
 
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < S; ++s) {
-      ptx::mbar_init(ptx::smem_u32(bars + s), 1);
-      ptx::mbar_init(ptx::smem_u32(bars + S + s), 8);   // one arrive per consumer warp
-    }
-    ptx::fence_barrier_init();
+  if (threadIdx.x == 0) {
     ptx::prefetch_tensormap(&tmA);
     ptx::prefetch_tensormap(&tmBhi);
     ptx::prefetch_tensormap(&tmBlo);
   }
-  __syncthreads();
-
-  if (warp == 0) {
-    int slot = 0, kb = 0;
-    for (int it = 0; it < n_it; ++it) {
-      const int s = it % S;
-      const uint32_t par = (uint32_t)(it / S) & 1u;
-      ptx::mbar_wait(ptx::smem_u32(bars + S + s), par ^ 1u);
-      if (ptx::elect_one()) {
-        const uint32_t full = ptx::smem_u32(bars + s);
-        ptx::mbar_arrive_expect_tx(full, (uint32_t)TC_STAGE_BYTES);
-        uint8_t* st = smem + (size_t)s * TC_STAGE_BYTES;
+  // the B tile holds 128 hi rows, then the 128 lo rows
+  float acc[1][16][4];
+  const bool consumer = tc_mainloop<1, 16>(
+      smem, TC_STAGES, TC_STAGE_BYTES, TC_A_BYTES, p.taps.n_slots * nkb, 16, 128, true,
+      [&](int it, uint32_t st, uint32_t full) {
+        const int slot = it / nkb, kb = it - slot * nkb;
         const int row = t0 + p.taps.b_shift[ph][slot], col = p.taps.b_col[ph][slot] + kb * 64;
-        tc_tma3(ptx::smem_u32(st), &tmA, full, kb * 64, cot * 128, p.taps.a_z[ph][slot]);
-        ptx::tma_load_2d(ptx::smem_u32(st + TC_A_BYTES), &tmBhi, full, col, row);
-        ptx::tma_load_2d(ptx::smem_u32(st + TC_A_BYTES + TC_B_BYTES / 2), &tmBlo, full, col, row);
-      }
-      __syncwarp();
-      if (++kb == nkb) { kb = 0; ++slot; }
-    }
-    return;
-  }
+        ptx::tma_load_3d(st, &tmA, full, kb * 64, cot * 128, p.taps.a_z[ph][slot]);
+        ptx::tma_load_2d(st + TC_A_BYTES, &tmBhi, full, col, row);
+        ptx::tma_load_2d(st + TC_A_BYTES + TC_B_BYTES / 2, &tmBlo, full, col, row);
+      },
+      acc);
+  if (!consumer) return;
 
   // consumers: warp w owns output channels [16 (w - 1), 16 w) of the tile
   const int w16 = 16 * (warp - 1);
-  const int q = lane >> 3, r8 = lane & 7;
-  float acc[16][4];
-#pragma unroll
-  for (int c = 0; c < 16; ++c)
-#pragma unroll
-    for (int e = 0; e < 4; ++e) acc[c][e] = 0.f;
-  for (int it = 0; it < n_it; ++it) {
-    const int s = it % S;
-    ptx::mbar_wait(ptx::smem_u32(bars + s), (uint32_t)(it / S) & 1u);
-    const uint32_t st = ptx::smem_u32(smem + (size_t)s * TC_STAGE_BYTES);
-    const uint32_t bst = st + TC_A_BYTES;    // rows 0..127: hi terms, rows 128..255: lo terms
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      uint32_t a[4];
-      ldsm_x4(st + sw128_off(w16 + r8 + ((q & 1) << 3), 2 * kk + (q >> 1)), a);
-#pragma unroll
-      for (int g = 0; g < 8; ++g)
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          uint32_t b[4];
-          ldsm_x4(bst + sw128_off(128 * half + 16 * g + r8 + ((q >> 1) << 3), 2 * kk + (q & 1)), b);
-          mma_bf16_16816(acc[2 * g], a, b[0], b[1]);
-          mma_bf16_16816(acc[2 * g + 1], a, b[2], b[3]);
-        }
-    }
-    __syncwarp();                          // every lane's fragment loads of this stage are done
-    if (lane == 0) ptx::mbar_arrive(ptx::smem_u32(bars + S + s));
-  }
   // Epilogue: accumulator (lane holds channels w16 + lane/4 (+8), columns 8c + 2(lane%4) (+1)) -> padded smem tile in the
   // drained ring -> global with lane = TIME, so that the residual reads and the stores are contiguous 128-byte rows
   // instead of scattered sectors (the channel-major activations have stride ldo between channels).
@@ -135,8 +85,8 @@ k_mbd_tc_conv(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
       const float add = co < p.M ? (p.bias ? p.bias[co] : 0.f) + (p.emb ? p.emb[co] : 0.f) : 0.f;
 #pragma unroll
       for (int c = 0; c < 16; ++c) {
-        tp[r * TC_TP_LD + 8 * c + 2 * (lane & 3)] = acc[c][2 * h8] + add;
-        tp[r * TC_TP_LD + 8 * c + 2 * (lane & 3) + 1] = acc[c][2 * h8 + 1] + add;
+        tp[r * TC_TP_LD + 8 * c + 2 * (lane & 3)] = acc[0][c][2 * h8] + add;
+        tp[r * TC_TP_LD + 8 * c + 2 * (lane & 3) + 1] = acc[0][c][2 * h8 + 1] + add;
       }
     }
     __syncwarp();
@@ -187,14 +137,10 @@ static __global__ void __launch_bounds__(256) k_mbd_prep_t(const float* __restri
   for (int i = 0; i < 4; ++i) {
     const int tl = ty * 4 + i, t = t0 + tl, c = c0 + 2 * tx;
     if (t < Tpad && c < Cp) {       // columns C .. Cp-1 (channel padding to a multiple of 64) are written as zero
-      const float a = tile[2 * tx][tl], b = tile[2 * tx + 1][tl];
-      const __nv_bfloat16 ah = __float2bfloat16_rn(a), bh = __float2bfloat16_rn(b);
-      __nv_bfloat162 h2, l2;
-      h2.x = ah; h2.y = bh;
-      l2.x = __float2bfloat16_rn(a - __bfloat162float(ah));
-      l2.y = __float2bfloat16_rn(b - __bfloat162float(bh));
-      *reinterpret_cast<__nv_bfloat162*>(hi + (size_t)t * Cp + c) = h2;
-      *reinterpret_cast<__nv_bfloat162*>(lo + (size_t)t * Cp + c) = l2;
+      uint32_t h2, l2;
+      pack_hi_lo(tile[2 * tx][tl], tile[2 * tx + 1][tl], h2, l2);
+      *reinterpret_cast<uint32_t*>(hi + (size_t)t * Cp + c) = h2;
+      *reinterpret_cast<uint32_t*>(lo + (size_t)t * Cp + c) = l2;
     }
   }
 }

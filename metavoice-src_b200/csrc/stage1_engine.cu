@@ -12,7 +12,7 @@
 
 #include "../../include/mvb200.h"
 #include "stage1_kernels.cuh"
-#include "umma_host.cuh"
+#include "tc_gemm_host.cuh"
 #include "decode_persistent.cuh"
 
 using namespace mvb;
@@ -107,7 +107,7 @@ static WsLayout make_layout(const mvb_s1_config& c) {
     size_t sc = 0;
     const size_t mats[5][3] = {{3 * D, D, 1}, {D, D, 1}, {F, D, 2}, {D, F, 1}, {V, D, 1}};
     for (auto& m : mats) {
-      GemmPlan g = plan_gemm((int)m[0], (int)m[1], (int)NBM, m[2] == 2, 132);
+      GemmPlan g = plan_gemm((int)m[0], (int)m[1], (int)NBM, m[2] == 2, GEMM_MAX_SM);
       if (g.scratch_floats > sc) sc = g.scratch_floats;
     }
     L.b_scratch = take(sc * 4);
@@ -302,16 +302,8 @@ extern "C" int mvb_s1_create(const mvb_s1_config* cfg, const void* d_arena, size
   if (h->att_mma) {
     // the tensor-core attention reads whole 64-position boxes: positions past the valid ones must hold finite values
     CK(cudaMemset(h->kv, 0, (size_t)cfg->n_layer * 2 * h->kv_half_bytes()));
-    EncodeTiledFn fn = encode_tiled_fn();
     const uint64_t rows = (uint64_t)cfg->n_layer * 2 * (h->kv_half_bytes() / 256);
-    cuuint64_t dims[2] = {128, rows};
-    cuuint64_t strides[1] = {256};
-    cuuint32_t box[2] = {64, 64};
-    cuuint32_t estr[2] = {1, 1};
-    if (!fn || rows >= (1ull << 31) ||
-        fn(&h->tm_kv, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, h->kv, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      h->att_mma = 0;
+    if (rows >= (1ull << 31) || !make_tmap_bf16(&h->tm_kv, h->kv, rows, 128, 64)) h->att_mma = 0;
   }
   if (const char* e = getenv("MVB_PC_FUSED")) h->fused = atoi(e) != 0;
   h->h_topk.assign(cfg->max_utts, 0);
@@ -456,7 +448,7 @@ static int launch_body(mvb_s1* h, cudaStream_t s, int n_utts) {
 
 
 // ------------------------------------------------------------------------------------------------
-// Path B: the same forward pass for R arbitrary activation rows on the tensor cores (umma_gemm.cuh).
+// Path B: the same forward pass for R arbitrary activation rows on the tensor cores (tc_gemm, linear.cu).
 // Used for batched decode (R = 2 * n_utts) and for prefill chunks (R = 2 * tokens).
 static const CUtensorMap* tmap_b(mvb_s1* h, int NB, int K) {
   auto key = std::make_pair(NB, K);
@@ -479,24 +471,21 @@ struct LinB {
 template <int EPI>
 static int linear_b(mvb_s1* h, cudaStream_t s, int R, const LinB& a, void* kc = nullptr, void* vc = nullptr) {
   const mvb_s1_config& c = h->cfg;
-  const int Rpad = (R + 15) / 16 * 16;
-  const int NB = Rpad * (h->split_lo ? 2 : 1);
-  const CUtensorMap* tB = tmap_b(h, NB, a.K);
-  if (!tB) return fail(MVB_ERR_CUDA, "cuTensorMapEncodeTiled failed for the activation buffer");
-  __nv_bfloat16* B = h->wsp<__nv_bfloat16>(h->L.b_B);
-  k_prep_b<<<Rpad, 256, 0, s>>>(a.x, a.ldx, a.gain, c.norm_eps, a.K, Rpad, R, h->split_lo, B);
-  h->launches++;
-  CK(cudaGetLastError());
-  GemmP p{};
-  p.M = a.M; p.K = a.K; p.NB = NB; p.Rpad = Rpad; p.R = R; p.split_lo = h->split_lo;
-  p.scratch = h->wsp<float>(h->L.b_scratch);
-  p.tickets = h->wsp<unsigned>(h->L.b_tickets);
-  p.out = a.out; p.ldo = a.ldo;
-  p.kcache = kc; p.vcache = vc; p.row_cache = h->rows.cache_row; p.row_pos = h->rows.pos;
-  p.H = c.n_head; p.S_max = c.block_size; p.D = c.dim; p.kv_fp32 = c.kv_dtype == MVB_KV_FP32;
-  const GemmPlan g = plan_gemm(a.M, a.K, NB, EPI == G_SWIGLU, h->n_sm);
-  CK(launch_umma_gemm<EPI>(s, h->tmW[a.widx], h->tmW[a.widx3], *tB, p, g));
-  h->launches++;
+  TcGemm g{};
+  g.epi = EPI; g.R = R; g.Rpad = (R + 15) / 16 * 16; g.split_lo = h->split_lo;
+  g.tmB = tmap_b(h, g.Rpad * (h->split_lo ? 2 : 1), a.K);
+  if (!g.tmB) return fail(MVB_ERR_CUDA, "cuTensorMapEncodeTiled failed for the activation buffer");
+  g.tmW = &h->tmW[a.widx]; g.tmW3 = &h->tmW[a.widx3];
+  g.B = h->wsp<__nv_bfloat16>(h->L.b_B);
+  g.x = a.x; g.ldx = a.ldx; g.gain = a.gain; g.eps = c.norm_eps;
+  g.M = a.M; g.K = a.K; g.out = a.out; g.ldo = a.ldo;
+  g.kcache = kc; g.vcache = vc; g.row_cache = h->rows.cache_row; g.row_pos = h->rows.pos;
+  g.H = c.n_head; g.S_max = c.block_size; g.D = c.dim; g.kv_fp32 = c.kv_dtype == MVB_KV_FP32;
+  g.scratch = h->wsp<float>(h->L.b_scratch);
+  g.tickets = h->wsp<unsigned>(h->L.b_tickets);
+  g.n_sm = h->n_sm;
+  CK(tc_gemm(s, g));
+  h->launches += 2;   // k_prep_b + k_tc_gemm
   return MVB_OK;
 }
 

@@ -2,7 +2,7 @@
 //   GPT.forward, causal=False      fam/llm/model.py:195-314   (sum of hierarchy embeddings + wpe + speaker)
 //   Block / SelfAttention / MLP    fam/llm/layers/combined.py:40-52, attn.py:122-185, layers.py:36-72
 //   _non_causal_sample             fam/llm/mixins/non_causal.py:15-67 (temperature, top-k, softmax, multinomial)
-// Every Linear runs on the tcgen05/TMA weight-streaming GEMM of umma_gemm.cuh (128 activation rows per pass,
+// Every Linear runs on the TMA + mma.sync weight-streaming GEMM (tc_gemm, linear.cu; 128 activation rows per pass,
 // hi+lo bf16 activations); attention is a full bidirectional softmax over the block (no padding mask, as in
 // the reference); sampling is one CTA per (hierarchy, position).
 #include <cuda_runtime.h>
@@ -12,7 +12,8 @@
 #include <vector>
 
 #include "../../include/mvb200.h"
-#include "umma_host.cuh"
+#include "common.cuh"
+#include "tc_gemm_host.cuh"
 
 using namespace mvb;
 namespace mvb { int set_error(int code, const char* fmt, ...); }
@@ -273,7 +274,7 @@ static size_t s2_layout(const mvb_s2_config* c, size_t* o_x, size_t* o_qkv, size
   size_t sc = 0;
   const size_t mats[5][3] = {{3 * E, E, 1}, {E, E, 1}, {Hd, E, 2}, {E, Hd, 1}, {vmax, E, 1}};
   for (auto& m : mats) {
-    GemmPlan g = plan_gemm((int)m[0], (int)m[1], 2 * S2_ROWS, m[2] == 2, 132);
+    GemmPlan g = plan_gemm((int)m[0], (int)m[1], 2 * S2_ROWS, m[2] == 2, GEMM_MAX_SM);
     sc = sc > g.scratch_floats ? sc : g.scratch_floats;
   }
   *o_scratch = take(sc * 4);
@@ -389,16 +390,18 @@ extern "C" int mvb_s2_attn_test(const float* d_qkv, int32_t B, int32_t t, int32_
 template <int EPI>
 static int s2_linear(mvb_s2* h, cudaStream_t s, int rows, const float* x, int ldx, const __nv_bfloat16* gain, int widx, int widx3, int M, int K,
                      float* out, int ldo) {
-  const CUtensorMap& tB = (K == h->cfg.n_embd) ? h->tmB_E : h->tmB_H;
-  const GemmPlan g = plan_gemm(M, K, 2 * S2_ROWS, EPI == G_SWIGLU, h->n_sm);
+  TcGemm g{};
+  g.epi = EPI; g.Rpad = S2_ROWS; g.split_lo = 1;
+  g.tmW = &h->tmW[widx]; g.tmW3 = &h->tmW[widx3];
+  g.B = h->B; g.tmB = (K == h->cfg.n_embd) ? &h->tmB_E : &h->tmB_H;
+  g.ldx = ldx; g.gain = gain; g.eps = h->cfg.norm_eps;
+  g.M = M; g.K = K; g.ldo = ldo;
+  g.scratch = h->scratch; g.tickets = h->tickets; g.n_sm = h->n_sm;
   for (int r0 = 0; r0 < rows; r0 += S2_ROWS) {
-    const int R = rows - r0 < S2_ROWS ? rows - r0 : S2_ROWS;
-    k_prep_b<<<S2_ROWS, 256, 0, s>>>(x + (size_t)r0 * ldx, ldx, gain, h->cfg.norm_eps, K, S2_ROWS, R, 1, h->B);
-    SCK(cudaGetLastError());
-    GemmP p{};
-    p.M = M; p.K = K; p.NB = 2 * S2_ROWS; p.Rpad = S2_ROWS; p.R = R; p.split_lo = 1;
-    p.scratch = h->scratch; p.tickets = h->tickets; p.out = out + (size_t)r0 * ldo; p.ldo = ldo;
-    SCK(launch_umma_gemm<EPI>(s, h->tmW[widx], h->tmW[widx3], tB, p, g));
+    g.R = rows - r0 < S2_ROWS ? rows - r0 : S2_ROWS;
+    g.x = x + (size_t)r0 * ldx;
+    g.out = out + (size_t)r0 * ldo;
+    SCK(tc_gemm(s, g));
   }
   return MVB_OK;
 }

@@ -232,15 +232,7 @@ __global__ void __launch_bounds__(128) k_lstm_layer(const float* __restrict__ pr
   __syncthreads();
   for (int t = 0; t < T; ++t) {
     if (t > 0) {
-      if (tid == 0) {
-        const unsigned target = (unsigned)t * gridDim.x;
-        const long long t0 = clock64();
-        unsigned v;
-        do {
-          asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(bar) : "memory");
-          if (clock64() - t0 > 4000000000ll) __trap();
-        } while (v < target);
-      }
+      if (tid == 0) wait_counter(bar, (unsigned)t * gridDim.x);
       __syncthreads();
       const float* hp = hbuf + (size_t)((t - 1) & 1) * H;
       for (int k = tid; k < H; k += 128) hs[k] = __ldcg(hp + k);
@@ -272,7 +264,7 @@ __global__ void __launch_bounds__(128) k_lstm_layer(const float* __restrict__ pr
       out[(size_t)(u0 + tid) * T + t] = skip ? h + skip[(size_t)(u0 + tid) * T + t] : h;
     }
     __syncthreads();
-    if (tid == 0) asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(bar) : "memory");
+    if (tid == 0) red_release_inc(bar);
   }
 }
 

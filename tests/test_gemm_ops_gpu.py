@@ -1,4 +1,4 @@
-"""GPU: the weight-streaming tensor-core GEMM (csrc/umma_gemm.cuh, k_umma_gemm<EPI, NC>) at every epilogue and
+"""GPU: the weight-streaming tensor-core GEMM (csrc/tc_gemm.cuh, k_tc_gemm<EPI, NC>) at every epilogue and
 accumulator instance, against a float64 computation of the same operation.
 
 Reference.  It reproduces every rounding the kernel declares, so that the only difference left is fp32 accumulation:
@@ -9,7 +9,7 @@ in float64, followed by the epilogue in float64.
 
 Elementwise bound.  With A = |x^| . |W|^T (x^ = hi + lo, all in float64) every element must satisfy
     |out - ref| <= gamma_K * A + tiny.
-Derivation of gamma_K for this kernel's summation order.  Each mma.sync.m16n8k16 adds 16 exact bf16 x bf16 products to
+Derivation of gamma_K for this kernel's order of accumulation.  Each mma.sync.m16n8k16 adds 16 exact bf16 x bf16 products to
 the fp32 accumulator c.  Modelled worst case (alignment of the 17 addends to the largest exponent with truncation, then a
 truncating normalisation): one MMA changes the exact value by at most 18 u (|c| + sum |p_i|), u = 2^-23.  A split runs
 n = 4 (1 + split_lo) MMAs per 64-wide k-block, sequentially over its k-blocks (hi then lo into the same accumulator);

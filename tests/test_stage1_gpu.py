@@ -521,7 +521,7 @@ def test_resident_forward_then_decode_equals_generate(tiny_sd):
 
 @pytest.mark.parametrize("n", [12, 40])
 def test_path_b_decode_above_8_utterances_vs_oracle(tiny_sd, n):
-    """Decode bodies for 9..64 utterances run on the tensor-core rows path (k_umma_gemm at 2n = 24 / 80 rows: NC = 4 / 16,
+    """Decode bodies for 9..64 utterances run on the tensor-core rows path (k_tc_gemm at 2n = 24 / 80 rows: NC = 4 / 16,
     k_attn_rows at mixed per-row positions).  Three teacher-forced positions through mvb_s1_step_logits for n
     mixed-length utterances (fp32 KV): every utterance's logits against the CPU oracle, and against the same utterance
     decoded alone."""
