@@ -235,6 +235,13 @@ int mvb_s2_forward(mvb_s2* h, int32_t batch, const int32_t* d_idx, const float* 
  * h * hs of each third (hs = E / n_head, 64 or 128); d_out fp32 [B * t, E] = softmax(q k^T / sqrt(hs)) v per (row block,
  * head).  Synchronises `stream`. */
 int mvb_s2_attn_test(const float* d_qkv, int32_t B, int32_t t, int32_t E, int32_t n_head, float* d_out, void* stream);
+/* Test hook (not part of the drop-in surface): the stage-2 sampler (k_s2_sample, launched as mvb_s2_forward launches
+ * it) on caller logits without an mvb_s2 handle.  d_logits fp32 [n_hier, n_rows, V], 1 <= V <= 2048; d_params DEVICE
+ * buffer of 16 bytes {float temperature; int32 top_k (<= 0 disables); uint64 seed}; d_noise fp32 [n_hier, n_rows, V]
+ * Exp(1) draws or NULL (on-device Philox keyed on (entry, row, hierarchy, seed)); d_tokens int32 [n_hier, n_rows].
+ * Allocates nothing; synchronises `stream`. */
+int mvb_s2_sample_test(const float* d_logits, int32_t n_hier, int32_t n_rows, int32_t V, const void* d_params,
+                       const float* d_noise, int32_t* d_tokens, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Vocoder, EnCodec-24 kHz decode path: RVQ decode (the diffusion condition `decode_latent`) and the SEANet decoder

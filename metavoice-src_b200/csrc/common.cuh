@@ -92,4 +92,13 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 ctr, uint2 key) {
   return ctr;
 }
 
+// Exp(1) draw from one Philox word: uni = ((x >> 8) + 0.5) 2^-24 lies in (0, 1) in real arithmetic, but in fp32 the
+// top value 2^24 - 0.5 rounds to 2^24, i.e. uni = 1 and q = -0, and a score p / q of -inf (p > 0) or NaN (p = 0, a
+// dropped entry) wins the unsigned arg-max.  That value is clamped to the largest float below 1; every other draw is
+// unchanged.
+__device__ __forceinline__ float philox_exp1(uint32_t x) {
+  const float uni = fminf(((float)(x >> 8) + 0.5f) * (1.0f / 16777216.0f), 0x1.fffffep-1f);
+  return -logf(uni);
+}
+
 }  // namespace mvb

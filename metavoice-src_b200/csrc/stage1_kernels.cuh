@@ -660,8 +660,7 @@ __global__ void __launch_bounds__(SAMP_THREADS) k_sample(SampleP p, S1State st) 
     } else {
       const uint4 rnd = philox4x32_10(make_uint4((unsigned)v, (unsigned)step, (unsigned)(step >> 32), (unsigned)u),
                                       make_uint2((unsigned)sp.seed, (unsigned)(sp.seed >> 32)));
-      const float uni = ((float)(rnd.x >> 8) + 0.5f) * (1.0f / 16777216.0f);  // (0,1)
-      qv = -logf(uni);
+      qv = philox_exp1(rnd.x);
     }
     const float score = __fdiv_rn(pr, qv);
     // order-preserving key for non-negative floats; ties resolve to the lowest index like torch.argmax

@@ -200,7 +200,7 @@ __global__ void __launch_bounds__(256) k_s2_sample(const float* __restrict__ log
     } else {
       const uint4 r = philox4x32_10(make_uint4((unsigned)v, (unsigned)row, (unsigned)hier, 0x5eed2u),
                                     make_uint2((unsigned)seed, (unsigned)(seed >> 32)));
-      qv = -logf(((float)(r.x >> 8) + 0.5f) * (1.0f / 16777216.0f));
+      qv = philox_exp1(r.x);
     }
     const unsigned long long cand =
         ((unsigned long long)__float_as_uint(__fdiv_rn(pr, qv)) << 32) | (unsigned long long)(0xffffffffu - (unsigned)v);
@@ -386,6 +386,24 @@ extern "C" int mvb_s2_attn_test(const float* d_qkv, int32_t B, int32_t t, int32_
   return MVB_OK;
 }
 
+// Launches the sampler over n_out hierarchies x rows logits rows of V entries exactly as s2_body does.
+static cudaError_t launch_s2_sample(cudaStream_t s, const float* logits, int V, const S2SampleParams* prm, const float* noise,
+                                    int* tokens, int rows, int n_out) {
+  k_s2_sample<<<dim3(rows, n_out), 256, 0, s>>>(logits, V, prm, noise, tokens, rows);
+  return cudaGetLastError();
+}
+
+extern "C" int mvb_s2_sample_test(const float* d_logits, int32_t n_hier, int32_t n_rows, int32_t V, const void* d_params,
+                                  const float* d_noise, int32_t* d_tokens, void* stream) {
+  if (!d_logits || !d_params || !d_tokens) return mvb::set_error(MVB_ERR_ARG, "null argument");
+  if (n_hier < 1 || n_rows < 1 || V < 1 || V > S2_PAD)
+    return mvb::set_error(MVB_ERR_UNSUPPORTED, "mvb_s2_sample_test: n_hier, n_rows >= 1 and 1 <= V <= %d required", S2_PAD);
+  cudaStream_t s = (cudaStream_t)stream;
+  SCK(launch_s2_sample(s, d_logits, V, reinterpret_cast<const S2SampleParams*>(d_params), d_noise, d_tokens, n_rows, n_hier));
+  SCK(cudaStreamSynchronize(s));
+  return MVB_OK;
+}
+
 // y[rows, M] (+)= f(x)[rows, K] . W^T in passes of 128 rows through the tensor-core GEMM
 template <int EPI>
 static int s2_linear(mvb_s2* h, cudaStream_t s, int rows, const float* x, int ldx, const __nv_bfloat16* gain, int widx, int widx3, int M, int K,
@@ -429,8 +447,7 @@ static int s2_body(mvb_s2* h, cudaStream_t s, int batch, bool has_spk, const flo
     const int hw = c.n_layer * 5 + i;
     if (int e = s2_linear<G_STORE>(h, s, rows, h->x, E, h->w(h->g_lnf()), hw, hw, vmax, E, h->logits + (size_t)i * rows * vmax, vmax)) return e;
   }
-  k_s2_sample<<<dim3(rows, c.n_out), 256, 0, s>>>(h->logits, vmax, h->params, d_noise, h->tokens, rows);
-  SCK(cudaGetLastError());
+  SCK(launch_s2_sample(s, h->logits, vmax, h->params, d_noise, h->tokens, rows, c.n_out));
   return MVB_OK;
 }
 

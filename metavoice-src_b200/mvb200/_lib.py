@@ -116,6 +116,8 @@ SIGNATURES = {
                                     C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
     "mvb_s2_attn_test": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "mvb_s2_sample_test": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                     C.c_void_p]),
 }
 ABI_VERSION = 2
 
