@@ -153,6 +153,22 @@ int mvb_s1_fetch(mvb_s1* h, int32_t utt, int32_t* out_tokens, int32_t cap, int32
  * positions do not advance (the KV cache is appended at the current positions). */
 int mvb_s1_step_logits(mvb_s1* h, int32_t n_utts, float* d_logits, void* stream);
 
+/* Weight-only int4 engine (quantisation_mode="int4", fast_inference_utils.py:297-306).  Same offset table as mvb_s1_create,
+ * but the entries of every layer's wqkv, wo, w1, w3 and w2 point at an int4 PACKED MATRIX [M, K] (K % 256 == 0):
+ *   nibbles  uint32 [M][K/8], q in [0, 15]: word w of row m holds q(m, 8w + 2i) in bits 4i..4i+3 and q(m, 8w + 2i + 1)
+ *            in bits 16+4i..19+4i, i = 0..3 (a pair of consecutive k lands in the two bf16 halves of a register);
+ *   then, at the next 256-byte boundary, bf16 [M][K/128][2] = {scale s, zero z} of every 128-wide group of a row.
+ * (produced only by mvb200/quantize.py:pack_matrix; the quantiser is the reference's group_quantize_tensor(w, 4, 128)).
+ * Dequantised weight: W_deq = bf16_rn((q - 8) s + z) -- the exact value rounded once to bf16 -- in every kernel.  All other
+ * tensors are bf16 as for mvb_s1_create (speaker_cond_pos holds its W_deq; lm_head stays unquantised).
+ * Decode always runs the per-layer CUDA-core path through the int4 GEMV (never the persistent kernel, never the tensor-core
+ * rows path); prefill runs the tensor-core GEMM over one layer at a time dequantised into a scratch that is part of the
+ * workspace: mvb_s1_int4_workspace_bytes = the bf16 workspace + one layer of bf16 weights.  Every other mvb_s1_* call
+ * accepts the handle. */
+size_t mvb_s1_int4_workspace_bytes(const mvb_s1_config* cfg);
+int mvb_s1_create_int4(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
+                       void* d_kv, void* d_workspace, mvb_s1** out);
+
 /* Kernel launches issued by this handle since creation (bench.py "gpu_launches"). */
 uint64_t mvb_s1_launch_count(const mvb_s1* h);
 
@@ -193,6 +209,19 @@ int mvb_gemm_test(int32_t epi, const void* d_W, const void* d_W3, int32_t M, int
                   int32_t R, const void* d_gain, float eps, int32_t split_lo, int32_t ksplit_override, float* d_out,
                   int32_t ldo, void* d_kcache, void* d_vcache, const int32_t* d_row_cache, const int32_t* d_row_pos,
                   int32_t H, int32_t S_max, int32_t D, int32_t kv_fp32, void* stream);
+/* Test hooks for the int4 kernels (not part of the drop-in surface):
+ *   mvb_w4_gemv_test    : the int4 GEMV (csrc/gemv_w4.cuh k_gemv_w4) as the int4 engine's decode launches it, for
+ *                         utterances u in [0, n_utts): rows 2 s, 2 s + 1 (s = d_slot_map[u]) of d_x fp32 [*, ldx] and d_out
+ *                         [*, ldo]; epi 0 store, 1 residual add, 2 SwiGLU with d_W3, 3 QKV plus the K / V thirds scattered to
+ *                         d_kcache / d_vcache [rows][H][S_max][128] at position d_pos[s] (D = 128 H, M = 3 D).  d_W / d_W3 are
+ *                         packed matrices [M, K]; d_gain optional bf16 [K] (RMSNorm prologue).  K % 256 == 0, 2 K floats <= 48 KB.
+ *   mvb_w4_dequant_test : k_w4_dequant of one packed matrix into d_out bf16 row-major [M, K].
+ * Both synchronise `stream`. */
+int mvb_w4_gemv_test(int32_t epi, const void* d_W, const void* d_W3, int32_t M, int32_t K, const float* d_x, int32_t ldx,
+                     int32_t n_utts, const void* d_gain, float eps, float* d_out, int32_t ldo, void* d_kcache, void* d_vcache,
+                     const int32_t* d_slot_map, const int32_t* d_pos, int32_t H, int32_t S_max, int32_t D, int32_t kv_fp32,
+                     void* stream);
+int mvb_w4_dequant_test(const void* d_W, int32_t M, int32_t K, void* d_out, void* stream);
 int mvb_mbd_conv_test(int32_t kind, const float* d_x, int32_t Cin, int32_t Tin, const float* d_w, int32_t Cout, int32_t K,
                       int32_t stride, int32_t dil, int32_t pad, const float* d_gn_stats, const float* d_gn_w,
                       const float* d_gn_b, int32_t groups, const float* d_bias, const float* d_emb, const float* d_resid,

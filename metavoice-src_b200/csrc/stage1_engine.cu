@@ -14,6 +14,7 @@
 #include "stage1_kernels.cuh"
 #include "tc_gemm_host.cuh"
 #include "decode_persistent.cuh"
+#include "gemv_w4.cuh"
 
 using namespace mvb;
 
@@ -166,11 +167,23 @@ struct mvb_s1 {
   PcMat pm[5];
   std::vector<int> h_topk;                            // top_k of every utterance slot as installed by mvb_s1_begin
   size_t layer_stride_elems = 0;
+  // int4 engine (mvb_s1_create_int4): wqkv / wo / w1 / w3 / w2 are packed matrices; path A streams them through
+  // k_gemv_w4, path B dequantises one layer at a time into w4_scratch (bf16 [wqkv | wo | w1 | w3 | w2]).
+  bool int4 = false;
+  __nv_bfloat16* w4_scratch = nullptr;
 
   template <typename T>
   T* wsp(size_t o) const { return reinterpret_cast<T*>(ws + o); }
   const __nv_bfloat16* w(int i) const { return reinterpret_cast<const __nv_bfloat16*>(arena + off[i]); }
   const __nv_bfloat16* lw(int layer, int t) const { return w(MVB_S1_GLOBAL_TENSORS + layer * MVB_S1_LAYER_TENSORS + t); }
+  // The one weight-source accessor of the tensor-core path: the bf16 matrix t (1 wqkv, 2 wo, 4 w1, 5 w3, 6 w2) of a layer,
+  // i.e. the arena tensor, or for an int4 engine its slot in the dequantised-layer scratch (filled by k_w4_dequant).
+  const __nv_bfloat16* tc_w(int layer, int t) const {
+    if (!int4) return lw(layer, t);
+    const size_t D = cfg.dim, F = cfg.intermediate;
+    const size_t at[7] = {0, 0, 3 * D * D, 0, 4 * D * D, 4 * D * D + F * D, 4 * D * D + 2 * F * D};
+    return w4_scratch + at[t];
+  }
   size_t kv_elem() const { return cfg.kv_dtype == MVB_KV_FP32 ? 4 : 2; }
   size_t kv_half_bytes() const {
     return (size_t)2 * cfg.max_utts * cfg.n_head * cfg.block_size * cfg.head_dim * kv_elem();
@@ -229,8 +242,32 @@ extern "C" size_t mvb_s1_workspace_bytes(const mvb_s1_config* c) {
   return make_layout(*c).total;
 }
 
+// elements of one layer's dequantised weights: wqkv, wo, w1, w3, w2
+static size_t w4_layer_elems(const mvb_s1_config& c) {
+  const size_t D = c.dim, F = c.intermediate;
+  return 4 * D * D + 3 * D * F;
+}
+
+extern "C" size_t mvb_s1_int4_workspace_bytes(const mvb_s1_config* c) {
+  if (validate(c)) return 0;
+  return align_up(make_layout(*c).total) + align_up(w4_layer_elems(*c) * 2);
+}
+
+static int create_engine(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
+                         void* d_kv, void* d_ws, mvb_s1** out, bool int4);
+
 extern "C" int mvb_s1_create(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
                              void* d_kv, void* d_ws, mvb_s1** out) {
+  return create_engine(cfg, d_arena, arena_bytes, offsets, d_kv, d_ws, out, false);
+}
+
+extern "C" int mvb_s1_create_int4(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
+                                  void* d_kv, void* d_ws, mvb_s1** out) {
+  return create_engine(cfg, d_arena, arena_bytes, offsets, d_kv, d_ws, out, true);
+}
+
+static int create_engine(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
+                         void* d_kv, void* d_ws, mvb_s1** out, bool int4) {
   if (int e = validate(cfg)) return e;
   if (!d_arena || !offsets || !d_kv || !d_ws || !out) return fail(MVB_ERR_ARG, "null pointer argument");
   int dev = 0, major = 0, minor = 0;
@@ -253,6 +290,18 @@ extern "C" int mvb_s1_create(const mvb_s1_config* cfg, const void* d_arena, size
   h->kv = reinterpret_cast<char*>(d_kv);
   h->ws = reinterpret_cast<char*>(d_ws);
   h->L = make_layout(*cfg);
+  h->int4 = int4;
+  if (int4) {
+    h->w4_scratch = h->wsp<__nv_bfloat16>(align_up(h->L.total));
+    const int D = cfg->dim, F = cfg->intermediate;
+    const int MK[7][2] = {{0, 0}, {3 * D, D}, {D, D}, {0, 0}, {F, D}, {F, D}, {D, F}};
+    for (int l = 0; l < cfg->n_layer; ++l)
+      for (int t : {1, 2, 4, 5, 6}) {
+        const uint64_t o = h->off[MVB_S1_GLOBAL_TENSORS + l * MVB_S1_LAYER_TENSORS + t];
+        if (o + w4_packed_bytes(MK[t][0], MK[t][1]) > arena_bytes)
+          return fail(MVB_ERR_ARG, "int4 packed matrix %d of layer %d runs past the end of the arena", t, l);
+      }
+  }
   S1State& s = h->st;
   s.slot_map = h->wsp<int>(h->L.slot_map);
   s.pos = h->wsp<int>(h->L.pos);
@@ -282,11 +331,11 @@ extern "C" int mvb_s1_create(const mvb_s1_config* cfg, const void* d_arena, size
     h->tmW.resize((size_t)cfg->n_layer * 5 + 1);
     bool ok = true;
     for (int l = 0; l < cfg->n_layer && ok; ++l) {
-      ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 0], h->lw(l, 1), 3 * D, D, 128);
-      ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 1], h->lw(l, 2), D, D, 128);
-      ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 2], h->lw(l, 4), F, D, 128);
-      ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 3], h->lw(l, 5), F, D, 128);
-      ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 4], h->lw(l, 6), D, F, 128);
+      ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 0], h->tc_w(l, 1), 3 * D, D, 128);
+      ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 1], h->tc_w(l, 2), D, D, 128);
+      ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 2], h->tc_w(l, 4), F, D, 128);
+      ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 3], h->tc_w(l, 5), F, D, 128);
+      ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 4], h->tc_w(l, 6), D, F, 128);
     }
     ok = ok && make_tmap_bf16(&h->tmW[(size_t)cfg->n_layer * 5], h->w(4), cfg->vocab, D, 128);
     if (!ok) return fail(MVB_ERR_CUDA, "cuTensorMapEncodeTiled failed for a weight matrix");
@@ -310,7 +359,7 @@ extern "C" int mvb_s1_create(const mvb_s1_config* cfg, const void* d_arena, size
   {
     // persistent decode kernel: needs a uniform layer stride (true for arenas packed in checkpoint order)
     const int D = cfg->dim, F = cfg->intermediate, V = cfg->vocab;
-    bool ok = cfg->n_layer >= 1;
+    bool ok = cfg->n_layer >= 1 && !int4;            // an int4 engine never uses path C
     const int o0 = MVB_S1_GLOBAL_TENSORS;
     uint64_t stride = cfg->n_layer > 1 ? h->off[o0 + MVB_S1_LAYER_TENSORS] - h->off[o0] : 2 * (uint64_t)(4 * D * D + 3 * D * F + 2 * D);
     for (int l = 1; l < cfg->n_layer && ok; ++l)
@@ -386,12 +435,14 @@ static cudaError_t launch_pdl(bool pdl, void (*kernel)(KArgs...), dim3 grid, dim
   return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
 
+// w4: p.W / p.W3 are int4 packed matrices (k_gemv_w4), else bf16 (k_gemv); both take one item per warp.
 template <int EPI>
-static cudaError_t launch_gemv(mvb_s1* h, cudaStream_t s, int n_utts, GemvP p) {
+static cudaError_t launch_gemv(mvb_s1* h, cudaStream_t s, int n_utts, GemvP p, bool w4 = false) {
   const int n_items = (EPI == EPI_SWIGLU) ? p.M : p.M / 2;
   dim3 grid(gemv_grid(n_items, h->n_sm), n_utts);
   const size_t smem = (size_t)2 * p.K * sizeof(float);
   h->launches++;
+  if (w4) return launch_pdl(h->pdl, k_gemv_w4<EPI>, grid, dim3(256), smem, s, p, h->st);
   return launch_pdl(h->pdl, k_gemv<EPI>, grid, dim3(256), smem, s, p, h->st);
 }
 
@@ -417,7 +468,7 @@ static int launch_body(mvb_s1* h, cudaStream_t s, int n_utts) {
     p.W = h->lw(l, 1); p.W3 = nullptr; p.x = x; p.ldx = D; p.gain = h->lw(l, 0);
     p.out = qkv; p.ldo = 3 * D; p.M = 3 * D; p.K = D;
     p.kcache = kc; p.vcache = vc; p.H = H; p.S_max = c.block_size; p.D = D; p.kv_fp32 = c.kv_dtype == MVB_KV_FP32;
-    CK(launch_gemv<EPI_QKV>(h, s, n_utts, p));
+    CK(launch_gemv<EPI_QKV>(h, s, n_utts, p, h->int4));
     // attention over [0, pos]
     dim3 ag(H, 2 * n_utts, ATT_SPLITS);
     if (c.kv_dtype == MVB_KV_FP32)
@@ -431,13 +482,13 @@ static int launch_body(mvb_s1* h, cudaStream_t s, int n_utts) {
     p = GemvP{};
     p.eps = c.norm_eps;
     p.W = h->lw(l, 2); p.x = att; p.ldx = D; p.gain = nullptr; p.out = x; p.ldo = D; p.M = D; p.K = D;
-    CK(launch_gemv<EPI_RESID>(h, s, n_utts, p));
+    CK(launch_gemv<EPI_RESID>(h, s, n_utts, p, h->int4));
     // ffn_norm + silu(w1 x) * w3 x
     p.W = h->lw(l, 4); p.W3 = h->lw(l, 5); p.x = x; p.ldx = D; p.gain = h->lw(l, 3); p.out = ffn; p.ldo = F; p.M = F; p.K = D;
-    CK(launch_gemv<EPI_SWIGLU>(h, s, n_utts, p));
+    CK(launch_gemv<EPI_SWIGLU>(h, s, n_utts, p, h->int4));
     // w2 + residual
     p.W = h->lw(l, 6); p.W3 = nullptr; p.x = ffn; p.ldx = F; p.gain = nullptr; p.out = x; p.ldo = D; p.M = D; p.K = F;
-    CK(launch_gemv<EPI_RESID>(h, s, n_utts, p));
+    CK(launch_gemv<EPI_RESID>(h, s, n_utts, p, h->int4));
   }
   GemvP p{};
   p.eps = c.norm_eps;
@@ -504,6 +555,19 @@ static int launch_layers_b(mvb_s1* h, cudaStream_t s, int R) {
   for (int l = 0; l < c.n_layer; ++l) {
     char* kc = h->kv + (size_t)l * 2 * half;
     char* vc = kc + half;
+    if (h->int4) {   // this layer's W_deq -> the scratch the tensor maps of every layer point at
+      W4Mats m{};
+      const int MK[5][3] = {{1, 3 * D, D}, {2, D, D}, {4, F, D}, {5, F, D}, {6, D, F}};
+      for (int i = 0; i < 5; ++i) {
+        m.src[i] = reinterpret_cast<const uint8_t*>(h->lw(l, MK[i][0]));
+        m.dst[i] = const_cast<__nv_bfloat16*>(h->tc_w(l, MK[i][0]));
+        m.M[i] = MK[i][1]; m.K[i] = MK[i][2];
+      }
+      m.n = 5;
+      k_w4_dequant<<<4 * h->n_sm, 256, 0, s>>>(m);
+      h->launches++;
+      CK(cudaGetLastError());
+    }
     if (int e = linear_b<G_QKV>(h, s, R, LinB{x, D, h->lw(l, 0), l * 5 + 0, l * 5 + 0, 3 * D, D, qkv, 3 * D}, kc, vc)) return e;
     dim3 ag(H, R, ATT_SPLITS);
     if (c.kv_dtype == MVB_KV_FP32)
@@ -606,7 +670,7 @@ static int run_body(mvb_s1* h, cudaStream_t s, int n_utts, bool allow_b = true) 
   // Path A (CUDA-core GEMV) streams the weights once per utterance; from 2 utterances up the tensor-core
   // rows path streams them once per step for the whole batch.  slot_map must be the identity for path B
   // (its logits rows are batch-ordered), which mvb_s1_decode guarantees.
-  const bool use_b = allow_b && h->path_b && n_utts >= h->decode_b_min;
+  const bool use_b = allow_b && h->path_b && !h->int4 && n_utts >= h->decode_b_min;   // int4 decode: always path A
   auto body = [&](cudaStream_t st) { return use_b ? launch_body_b(h, st, n_utts) : launch_body(h, st, n_utts); };
   if (!h->use_graph) return body(s);
   const int key = n_utts + (use_b ? 1000 : 0);
@@ -1023,4 +1087,54 @@ extern "C" int mvb_s1_generate(mvb_s1* h, int32_t n_utts, const int32_t* prompts
     CK(cudaStreamSynchronize(s));
   }
   return rc;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Test hooks of the int4 kernels (include/mvb200.h): k_gemv_w4<epi> exactly as path A launches it, over a caller-built
+// decode state (slot map and positions), and k_w4_dequant on one packed matrix.
+extern "C" int mvb_w4_gemv_test(int32_t epi, const void* d_W, const void* d_W3, int32_t M, int32_t K, const float* d_x,
+                                int32_t ldx, int32_t n_utts, const void* d_gain, float eps, float* d_out, int32_t ldo,
+                                void* d_kcache, void* d_vcache, const int32_t* d_slot_map, const int32_t* d_pos, int32_t H,
+                                int32_t S_max, int32_t D, int32_t kv_fp32, void* stream) {
+  if (!d_W || !d_x || !d_out || !d_slot_map || !d_pos) return fail(MVB_ERR_ARG, "null argument");
+  if (epi < EPI_STORE || epi > EPI_QKV) return fail(MVB_ERR_ARG, "bad epilogue %d", epi);
+  if (K < 256 || K % 256 || M < 2 || M % 2 || n_utts < 1 || n_utts > 64) return fail(MVB_ERR_ARG, "bad shape M=%d K=%d n_utts=%d", M, K, n_utts);
+  if ((size_t)2 * K * sizeof(float) > 48 * 1024) return fail(MVB_ERR_UNSUPPORTED, "K=%d exceeds the staging buffer", K);
+  if (epi == EPI_SWIGLU && !d_W3) return fail(MVB_ERR_ARG, "SwiGLU needs W3");
+  if (epi == EPI_QKV && (!d_kcache || !d_vcache || M != 3 * D || D != 128 * H)) return fail(MVB_ERR_ARG, "bad QKV arguments");
+  mvb_s1 h{};
+  h.n_sm = 132;
+  CK(cudaDeviceGetAttribute(&h.n_sm, cudaDevAttrMultiProcessorCount, 0));
+  h.st.slot_map = const_cast<int*>(d_slot_map);
+  h.st.pos = const_cast<int*>(d_pos);
+  GemvP p{};
+  p.W = reinterpret_cast<const __nv_bfloat16*>(d_W); p.W3 = reinterpret_cast<const __nv_bfloat16*>(d_W3);
+  p.x = d_x; p.ldx = ldx; p.gain = reinterpret_cast<const __nv_bfloat16*>(d_gain); p.eps = eps;
+  p.out = d_out; p.ldo = ldo; p.M = M; p.K = K;
+  p.kcache = d_kcache; p.vcache = d_vcache; p.H = H; p.S_max = S_max; p.D = D; p.kv_fp32 = kv_fp32;
+  cudaStream_t s = (cudaStream_t)stream;
+  switch (epi) {
+    case EPI_STORE: CK(launch_gemv<EPI_STORE>(&h, s, n_utts, p, true)); break;
+    case EPI_RESID: CK(launch_gemv<EPI_RESID>(&h, s, n_utts, p, true)); break;
+    case EPI_SWIGLU: CK(launch_gemv<EPI_SWIGLU>(&h, s, n_utts, p, true)); break;
+    default: CK(launch_gemv<EPI_QKV>(&h, s, n_utts, p, true)); break;
+  }
+  CK(cudaStreamSynchronize(s));
+  return MVB_OK;
+}
+
+extern "C" int mvb_w4_dequant_test(const void* d_W, int32_t M, int32_t K, void* d_out, void* stream) {
+  if (!d_W || !d_out) return fail(MVB_ERR_ARG, "null argument");
+  if (M < 1 || K < 256 || K % 256) return fail(MVB_ERR_ARG, "bad shape M=%d K=%d", M, K);
+  W4Mats m{};
+  m.src[0] = reinterpret_cast<const uint8_t*>(d_W);
+  m.dst[0] = reinterpret_cast<__nv_bfloat16*>(d_out);
+  m.M[0] = M; m.K[0] = K; m.n = 1;
+  int n_sm = 132;
+  CK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, 0));
+  cudaStream_t s = (cudaStream_t)stream;
+  k_w4_dequant<<<4 * n_sm, 256, 0, s>>>(m);
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(s));
+  return MVB_OK;
 }

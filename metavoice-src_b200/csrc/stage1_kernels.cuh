@@ -145,6 +145,7 @@ __device__ __forceinline__ void gemv_rows(const GemvP& p, int item, int lane, co
   }
 }
 
+// k_gemv_w4 (gemv_w4.cuh) repeats this prologue and these epilogues over int4 weights: a fix to one belongs in the other.
 template <int EPI>
 __global__ void __launch_bounds__(256, 2) k_gemv(GemvP p, S1State st) {
   extern __shared__ float xs[];  // [2][K] permuted

@@ -9,6 +9,7 @@ from __future__ import annotations
 
 import ctypes as C
 import time
+import warnings
 from pathlib import Path
 from typing import Optional, Tuple
 
@@ -197,7 +198,8 @@ def _load_model(checkpoint_path, spk_emb_ckpt_path, device, precision, quantisat
     if quantisation_mode is not None:
         if quantisation_mode not in ("int4", "int8"):
             raise Exception(f"Invalid quantisation mode {quantisation_mode}! Must be either 'int4' or 'int8'!")
-        raise NotImplementedError("weight-only quantisation is outside the bf16 hot path (SURVEY.md §2 row 4)")
+        if quantisation_mode == "int8":
+            raise NotImplementedError("int8 weight-only quantisation is not implemented; use quantisation_mode='int4' or None")
     checkpoint = torch.load(str(checkpoint_path), mmap=True, weights_only=False)
     sd = checkpoint["model"]
     args = checkpoint.get("model_args", {})
@@ -209,7 +211,9 @@ def _load_model(checkpoint_path, spk_emb_ckpt_path, device, precision, quantisat
                        n_head=n_head, dim=dim, speaker_emb_dim=sd0["speaker_cond_pos.weight"].shape[1],
                        intermediate_size=sd0["transformer.h.0.mlp.swiglu.w1.weight"].shape[0],
                        norm_eps=args.get("rmsnorm_eps") or 1e-5)
-    model = Transformer.from_state_dict(sd0, config, device=device)
+    if quantisation_mode == "int4":   # utils:297-306: quantised at load from the bf16 checkpoint
+        warnings.warn("quantisation will degrade the quality of the audio! Please set optimisation_mode to `None` for best quality.")
+    model = Transformer.from_state_dict(sd0, config, device=device, quantisation_mode=quantisation_mode)
     tokenizer = None
     tok_info = checkpoint.get("meta", {}).get("tokenizer", {})
     if tok_info:

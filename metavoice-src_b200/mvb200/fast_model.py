@@ -95,8 +95,12 @@ class KVCache:
 class Transformer:
     """Mirror of fam/llm/fast_model.py:116-167 backed by an ``mvb_s1`` engine handle."""
 
-    def __init__(self, config: ModelArgs, arena: torch.Tensor, offsets: List[int], device="cuda"):
+    def __init__(self, config: ModelArgs, arena: torch.Tensor, offsets: List[int], device="cuda",
+                 quantisation_mode: Optional[str] = None):
+        if quantisation_mode not in (None, "int4"):
+            raise NotImplementedError(f"quantisation_mode={quantisation_mode!r} is not implemented (only None and 'int4')")
         self.config = config
+        self.quantisation_mode = quantisation_mode
         self.device = torch.device(device)
         self._lib = _lib.load()
         self._arena = arena.to(self.device) if arena.device != self.device else arena
@@ -115,16 +119,39 @@ class Transformer:
         raise RuntimeError("mvb200.Transformer holds device weights; use Transformer.from_state_dict(...)")
 
     @classmethod
-    def from_state_dict(cls, state_dict, config: ModelArgs, device="cuda"):
-        arena, offsets = pack_arena(state_dict, config.n_layer)
-        return cls(config, arena, offsets, device)
+    def from_state_dict(cls, state_dict, config: ModelArgs, device="cuda", quantisation_mode: Optional[str] = None):
+        """``quantisation_mode="int4"`` quantises wqkv / wo / w1 / w3 / w2 at load (mvb200/quantize.py) and builds an int4
+        engine: decode streams the packed weights through k_gemv_w4, prefill dequantises one layer at a time."""
+        if quantisation_mode == "int4":
+            from .quantize import pack_arena_int4
+            arena, offsets, _ = pack_arena_int4(state_dict, config.n_layer)
+        elif quantisation_mode is None:
+            arena, offsets = pack_arena(state_dict, config.n_layer)
+        else:
+            raise NotImplementedError(f"quantisation_mode={quantisation_mode!r} is not implemented (only None and 'int4')")
+        return cls(config, arena, offsets, device, quantisation_mode)
 
-    def model_size_bytes(self) -> int:
-        """Σ numel*itemsize of parameters == the reference's ``model_size`` (utils:348) before caches."""
-        c = self.config
+    @staticmethod
+    def bf16_model_size_bytes(c: ModelArgs) -> int:
         per_layer = 4 * c.dim * c.dim + 3 * c.dim * c.intermediate_size + 2 * c.dim
         n = c.n_layer * per_layer + 2 * c.vocab_size * c.dim + c.block_size * c.dim + c.speaker_emb_dim * c.dim + c.dim
         return n * 2
+
+    @staticmethod
+    def int4_model_size_bytes(c: ModelArgs) -> int:
+        """Bytes of the int4 arena's tensors: 4-bit weights plus one bf16 (scale, zero) pair per 128 of them for the five
+        layer matrices, bf16 for everything else (speaker_cond_pos is held as its dequantised bf16 weight)."""
+        mats = 4 * c.dim * c.dim + 3 * c.dim * c.intermediate_size
+        per_layer = mats // 2 + mats // 128 * 4 + 2 * c.dim * 2
+        rest = 2 * c.vocab_size * c.dim + c.block_size * c.dim + c.speaker_emb_dim * c.dim + c.dim
+        return c.n_layer * per_layer + rest * 2
+
+    def model_size_bytes(self) -> int:
+        """Σ numel*itemsize of parameters == the reference's ``model_size`` (utils:348) before caches; for an int4 engine
+        the bytes its arena's tensors occupy, so that main()'s bandwidth figure counts the bytes actually read."""
+        if self.quantisation_mode == "int4":
+            return self.int4_model_size_bytes(self.config)
+        return self.bf16_model_size_bytes(self.config)
 
     def setup_spk_cond_mask(self):
         # fast_model.py:132-134: row 0 conditioned, row 1 unconditioned -- built into the kernels.
@@ -151,8 +178,9 @@ class Transformer:
                             c.speaker_emb_dim, c.norm_eps, self.max_utts,
                             _lib.MVB_KV_FP32 if kv_dtype == "fp32" else _lib.MVB_KV_BF16, max_new or c.block_size)
         self._cfg = cfg
+        int4 = self.quantisation_mode == "int4"
         kvb = self._lib.mvb_s1_kv_bytes(C.byref(cfg))
-        wsb = self._lib.mvb_s1_workspace_bytes(C.byref(cfg))
+        wsb = (self._lib.mvb_s1_int4_workspace_bytes if int4 else self._lib.mvb_s1_workspace_bytes)(C.byref(cfg))
         if kvb == 0 or wsb == 0:
             _lib.check(_lib.MVB_ERR_UNSUPPORTED)
         self._kv = torch.zeros(kvb, dtype=torch.uint8, device=self.device)
@@ -170,8 +198,9 @@ class Transformer:
             os.environ["MVB_PATHC"] = "1" if "C" in paths else "0"
         try:
             with torch.cuda.device(self.device):
-                rc = self._lib.mvb_s1_create(C.byref(cfg), self._arena.data_ptr(), self._arena.numel(), offs,
-                                             self._kv.data_ptr(), self._ws.data_ptr(), C.byref(h))
+                create = self._lib.mvb_s1_create_int4 if int4 else self._lib.mvb_s1_create
+                rc = create(C.byref(cfg), self._arena.data_ptr(), self._arena.numel(), offs, self._kv.data_ptr(),
+                            self._ws.data_ptr(), C.byref(h))
         finally:
             if tensor_core_path is not None:
                 for k, v in saved.items():

@@ -1,0 +1,191 @@
+"""Weight-only int4 quantisation of the stage-1 model (``quantisation_mode="int4"``, fast_inference_utils.py:297-306).
+
+Semantics, defined once here and in include/mvb200.h ("int4 packed matrix"):
+
+* Which tensors.  A Linear weight [out, in] is quantised when ``out % 8 == 0`` and ``in % 128 == 0`` (the rule of the
+  reference's ``WeightOnlyInt4QuantHandler``, fast_quantize.py:270-299, with groupsize 128).  A Linear with
+  ``out % 8 == 0`` whose ``in`` is not a multiple of 128 is rejected (the reference would pad it through a module that does
+  not exist).  For MetaVoice-1B that quantises wqkv, wo, w1, w3, w2 of every layer and speaker_cond_pos; lm_head
+  (2562 outputs), the embeddings and the norms stay bf16.
+* Quantiser.  Per group of 128 consecutive inputs of a row, with every intermediate rounded to bf16 as the reference's
+  bf16 tensor arithmetic does: ``s = bf16(bf16(max - min).clamp(1e-6) / 15)``, ``z = bf16(min + 8 s)``,
+  ``q = clamp(round_half_even(bf16(bf16(w - bf16(z - 8 s)) / s)), 0, 15)``.  Bit-identical to the reference's
+  ``group_quantize_tensor(w, 4, 128)`` (pinned by tests/golden/int4_quant.npz).
+* Dequantised weight.  ``W_deq = bf16_rn((q - 8) s + z)``: the exact value rounded once to bf16 (a fused multiply-add
+  with a single rounding, ``fma.rn.bf16x2``), the value both CUDA kernels (k_gemv_w4 and k_w4_dequant) use.  The
+  reference's Python dequantiser ``group_dequantize_tensor_from_qparams`` rounds twice instead (bf16 after the multiply
+  and after the add); how its CUDA int4 matmul (``_weight_int4pack_mm``) rounds could not be checked.  The two values are
+  equal wherever the reference's product rounding is exact; elsewhere they differ by at most half a bf16 ulp of the product
+  (the reference's first rounding, which cancellation against z can make larger than an ulp of the result) plus one ulp of
+  the result (tests/test_int4_quant.py).
+* Consequence.  An int4 engine computes the same function as a bf16 engine whose arena holds ``W_deq``.
+"""
+from __future__ import annotations
+
+from typing import Dict, List, Tuple
+
+import torch
+
+GROUP = 128
+N_BIT = 4
+_ALIGN = 256
+
+
+def is_quantised(out_features: int, in_features: int, name: str = "") -> bool:
+    """The tensor-selection rule.  Raises for a Linear int4 cannot represent without padding."""
+    if out_features % 8 != 0:
+        return False
+    if in_features % GROUP != 0:
+        raise ValueError(f"int4 quantisation needs in_features % {GROUP} == 0; {name or 'a Linear'} has "
+                         f"in_features={in_features} (padding is not supported)")
+    return True
+
+
+def group_quantize(w: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """w [M, K] -> (q uint8 [M, K] in [0, 15], scales bf16 [M, K/128], zeros bf16 [M, K/128])."""
+    M, K = w.shape
+    if K % GROUP:
+        raise ValueError(f"K={K} is not a multiple of {GROUP}")
+    g = w.detach().to("cpu", torch.bfloat16).reshape(M * (K // GROUP), GROUP)
+    if torch.isnan(g).any():
+        raise ValueError("cannot quantise a weight holding NaN")
+    lo = g.amin(dim=1, keepdim=True)
+    hi = g.amax(dim=1, keepdim=True)
+    rng = (hi - lo).clamp(min=1e-6)                  # bf16 tensors: every step below rounds to bf16
+    s = rng / (2 ** N_BIT - 1)
+    z = lo + s * (2 ** (N_BIT - 1))
+    base = z - s * (2 ** (N_BIT - 1))
+    q = ((g - base) / s).round().clamp(0, 2 ** N_BIT - 1).to(torch.uint8)
+    return q.reshape(M, K), s.reshape(M, K // GROUP), z.reshape(M, K // GROUP)
+
+
+def _round_to_bf16(v: torch.Tensor) -> torch.Tensor:
+    """float64 -> bf16 with ONE round-to-nearest-even at bf16's 8-bit significand (torch's own conversion goes through fp32
+    and would round twice).  Exact for results in bf16's normal range."""
+    b = v.contiguous().view(torch.int64)
+    keep = 52 - 7                                       # float64 fraction bits below bf16's 7
+    b = (b + ((1 << (keep - 1)) - 1) + ((b >> keep) & 1)) & ~((1 << keep) - 1)
+    return b.view(torch.float64).to(torch.float32).to(torch.bfloat16)   # now exact in fp32 and in bf16
+
+
+def dequantize(q: torch.Tensor, s: torch.Tensor, z: torch.Tensor) -> torch.Tensor:
+    """W_deq = bf16_rn((q - 8) s + z), bf16 [M, K].  The float64 value (q - 8) s + z is exact for every bf16 (s, z) pair
+    whose exponents are less than 41 apart (every group the quantiser produces from finite weights)."""
+    M, K = q.shape
+    qd = q.to(torch.float64).reshape(M, K // GROUP, GROUP) - 2 ** (N_BIT - 1)
+    v = qd * s.to(torch.float64)[..., None] + z.to(torch.float64)[..., None]
+    return _round_to_bf16(v).reshape(M, K)
+
+
+# nibble slot n (bits 4n..4n+3) of a little-endian 32-bit word holds k = 8w + _SLOT_K[n]: the even k of the word in slots
+# 0-3, the odd ones in slots 4-7, so pair (2i, 2i + 1) sits at bits 4i and 16 + 4i (one shift and mask per bf16x2 pair)
+_SLOT_K = [0, 2, 4, 6, 1, 3, 5, 7]
+
+
+def pack_nibbles(q: torch.Tensor) -> torch.Tensor:
+    """q uint8 [M, K] -> uint8 [M, K/2] in the word layout of include/mvb200.h (8 consecutive k per 32-bit word)."""
+    M, K = q.shape
+    g = q.to(torch.int64).reshape(M, K // 8, 8)
+    w = torch.zeros(M, K // 8, dtype=torch.int64)
+    for n, k in enumerate(_SLOT_K):
+        w |= g[..., k] << (4 * n)
+    return w.to(torch.int32).contiguous().view(torch.uint8).reshape(M, K // 2)
+
+
+def unpack_nibbles(p: torch.Tensor) -> torch.Tensor:
+    M, Kh = p.shape
+    w = p.contiguous().view(torch.int32).to(torch.int64) & 0xFFFFFFFF
+    out = torch.empty(M, Kh // 4, 8, dtype=torch.uint8)
+    for n, k in enumerate(_SLOT_K):
+        out[..., k] = ((w >> (4 * n)) & 0xF).to(torch.uint8)
+    return out.reshape(M, 2 * Kh)
+
+
+def packed_bytes(M: int, K: int) -> int:
+    """Bytes of one packed matrix: the nibble block padded to 256 bytes, then the (scale, zero) block."""
+    return (M * K // 2 + _ALIGN - 1) // _ALIGN * _ALIGN + M * (K // GROUP) * 4
+
+
+def pack_matrix(q: torch.Tensor, s: torch.Tensor, z: torch.Tensor) -> torch.Tensor:
+    """The int4 packed matrix of include/mvb200.h: nibbles [M, K/2] bytes, then at the next 256-byte boundary
+    bf16 [M, K/128, 2] = {scale, zero} of every group."""
+    M, K = q.shape
+    buf = torch.zeros(packed_bytes(M, K), dtype=torch.uint8)
+    nb = M * K // 2
+    buf[:nb] = pack_nibbles(q).reshape(-1)
+    sz = torch.stack([s, z], dim=-1).contiguous().reshape(-1)
+    so = (nb + _ALIGN - 1) // _ALIGN * _ALIGN
+    buf[so:] = sz.view(torch.uint8)
+    return buf
+
+
+def unpack_matrix(buf: torch.Tensor, M: int, K: int):
+    """Inverse of pack_matrix: (q, scales, zeros)."""
+    nb = M * K // 2
+    so = (nb + _ALIGN - 1) // _ALIGN * _ALIGN
+    q = unpack_nibbles(buf[:nb].reshape(M, K // 2))
+    sz = buf[so:so + M * (K // GROUP) * 4].clone().view(torch.bfloat16).reshape(M, K // GROUP, 2)
+    return q, sz[..., 0].contiguous(), sz[..., 1].contiguous()
+
+
+# arena order == include/mvb200.h; which entries are Linear weights, and which of those the engine streams as int4
+_GLOBAL_KEYS = ["transformer.wtes.0.weight", "transformer.wpe.weight", "speaker_cond_pos.weight",
+                "transformer.ln_f.weight", "lm_heads.0.weight"]
+_LAYER_KEYS = ["ln_1.weight", "attn.c_attn.weight", "attn.c_proj.weight", "ln_2.weight",
+               "mlp.swiglu.w1.weight", "mlp.swiglu.w3.weight", "mlp.c_proj.weight"]
+_GLOBAL_LINEAR = {2, 4}            # speaker_cond_pos, lm_head
+_LAYER_PACKED = {1, 2, 4, 5, 6}    # wqkv, wo, w1, w3, w2: int4 packed matrices read by k_gemv_w4 / k_w4_dequant
+
+
+def _keys(n_layer: int) -> List[Tuple[str, bool, bool]]:
+    """(checkpoint key, is a Linear weight, stored packed) in arena order."""
+    out = [(k, i in _GLOBAL_LINEAR, False) for i, k in enumerate(_GLOBAL_KEYS)]
+    for l in range(n_layer):
+        out += [(f"transformer.h.{l}.{k}", t in _LAYER_PACKED, t in _LAYER_PACKED) for t, k in enumerate(_LAYER_KEYS)]
+    return out
+
+
+def pack_arena_int4(state_dict: Dict[str, torch.Tensor], n_layer: int):
+    """Checkpoint state dict -> (uint8 arena, byte offsets, bytes the arena's tensors occupy without padding).
+    Per layer wqkv / wo / w1 / w3 / w2 become int4 packed matrices (the offset points at the nibble block); a quantised
+    Linear the engine does not stream in int4 (speaker_cond_pos, and lm_head when its out % 8 == 0) is stored as W_deq in
+    bf16, so it computes what the reference's int4 Linear computes; everything else is the bf16 tensor."""
+    sd = {(k[len("_orig_mod."):] if k.startswith("_orig_mod.") else k): v for k, v in state_dict.items()}
+    blobs: List[torch.Tensor] = []
+    payload = 0
+    for k, linear, packed in _keys(n_layer):
+        if k not in sd:
+            raise KeyError(f"checkpoint is missing {k}")
+        t = sd[k].detach().to(torch.bfloat16)
+        if linear and is_quantised(t.shape[0], t.shape[1], k):
+            q, s, z = group_quantize(t)
+            if packed:
+                blob = pack_matrix(q, s, z)
+                payload += t.numel() // 2 + s.numel() * 4
+                blobs.append(blob)
+                continue
+            t = dequantize(q, s, z)
+        elif packed:
+            raise ValueError(f"{k}: the int4 engine streams this matrix packed, but out % 8 != 0")
+        blobs.append(t.contiguous().reshape(-1).view(torch.uint8))
+        payload += t.numel() * 2
+    offsets: List[int] = []
+    total = 0
+    for b in blobs:
+        offsets.append(total)
+        total = (total + b.numel() + _ALIGN - 1) // _ALIGN * _ALIGN
+    arena = torch.zeros(total, dtype=torch.uint8)
+    for b, o in zip(blobs, offsets):
+        arena[o:o + b.numel()] = b
+    return arena, offsets, payload
+
+
+def dequantized_state_dict(state_dict: Dict[str, torch.Tensor], n_layer: int) -> Dict[str, torch.Tensor]:
+    """The checkpoint with every quantised Linear replaced by W_deq (bf16): the bf16 model an int4 engine equals."""
+    sd = {(k[len("_orig_mod."):] if k.startswith("_orig_mod.") else k): v for k, v in state_dict.items()}
+    out = dict(sd)
+    for k, linear, _ in _keys(n_layer):
+        t = sd[k]
+        if linear and is_quantised(t.shape[0], t.shape[1], k):
+            out[k] = dequantize(*group_quantize(t.to(torch.bfloat16)))
+    return out
