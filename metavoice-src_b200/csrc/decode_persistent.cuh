@@ -8,7 +8,8 @@
 //     swizzle) into a ring of smem stages, KV-cache tiles via cp.async.bulk into two dedicated (K,V) tile slots -- all
 //     guarded by full/empty mbarriers.  Weights do not depend on activations, so the producer never waits for a grid
 //     barrier: the HBM stream keeps running across phase, layer AND token boundaries (the next token's first weight
-//     tiles land while the grid is still sampling).
+//     tiles land while the grid is still sampling).  While the ring is full it pulls the next PC_PF_AHEAD weight tiles
+//     of its schedule into L2 (cp.async.bulk.prefetch.tensor), so that HBM keeps streaming while the grid synchronises.
 //   * warp 1 = MMA WARP: the weight tile [128 rows x 64 k] is the A operand, the staged activation rows (hi + lo bf16
 //     halves, NB rows) the B operand of mma.sync.m16n8k16; fragments come from the 128B-swizzled tiles by ldmatrix and the
 //     hi and lo products accumulate into one fp32 register tile [128 x NB/2].  At the end of a tile the warp parks the
@@ -17,9 +18,8 @@
 //   * warps 2..5 = COMPUTE: wait for the previous phase grid-wide (split arrive/wait counter with release/acquire
 //     atomics), stage the activation operand into swizzled smem (RMSNorm gain / attention-merge / SiLU*mul fused
 //     here), run the epilogues (accumulator slot -> red.global.add.f32 split-K accumulation), the decode attention on
-//     smem KV tiles (online softmax per half-warp) and the grid-distributed sampler.
-//   * warp 6 = optional L2 PREFETCHER: keeps a window of the flat weight-tile schedule in flight with
-//     cp.async.bulk.prefetch.tensor so that HBM keeps streaming while the grid synchronises.
+//     smem KV tiles (mma.sync for the bf16 cache, online softmax per half-warp for the fp32 cache) and the
+//     grid-distributed sampler.
 //   * RMSNorm statistic without a full-row re-read: every CTA stages x[k-slice] * gain; the CTAs of tile group 0 add
 //     their slice's sum of squares into stat[norm][row] (one red.add per row); the CONSUMER of the projection applies
 //     rsqrt(stat / D + eps): attention scales q, k, v; the w2 staging scales g, u; the sampler scales the logits.
@@ -34,7 +34,8 @@
 
 namespace mvb {
 
-constexpr int PC_THREADS = 224;      // producer warp + MMA warp + 4 compute warps + L2 prefetch warp
+constexpr int PC_THREADS = 192;      // producer warp + MMA warp + 4 compute warps
+constexpr int PC_PF_AHEAD = 8;       // weight tiles the producer prefetches into L2 ahead of the smem ring
 constexpr int PC_KV_TILE_BYTES = 16384;   // K (or V) tile of one (row, head): 64 bf16 / 32 fp32 positions
 constexpr int PC_RPAD = 16;          // rows of the fp32 activation buffers (8 utterances x 2 CFG rows)
 constexpr int PC_BKB_MAX = 12;       // k-blocks of the activation operand one CTA may own in a phase
@@ -53,7 +54,6 @@ struct AttTile {
 
 struct PcShared {   // small shared state behind the big buffers
   uint64_t b_full[8], b_empty[8], b_ready, acc_full[2], acc_empty[2], kv_full[PC_NKV_MAX], kv_empty[PC_NKV_MAX], tab_ready;
-  int prod_pos;                     // weight tiles issued so far (producer -> L2 prefetcher)
   int n_att_tiles;
   // every CTA's private copy of the decode state of the batch (kept in lock-step: the same deterministic update
   // from the same arg-max in every CTA; only the owner CTA writes it back to global memory)
@@ -78,13 +78,8 @@ template <int NB> struct PcCfg {
   static constexpr int TILE_ROWS = 128;
   static constexpr int STAGE_BYTES = TILE_ROWS * 128;     // [TILE_ROWS x 64 k] bf16
   // ring depth: what fits in 227 KB next to the activation operand, the KV slots and the accumulator slots
-#ifdef PC_DEEP_KV   // A/B: trade weight-ring depth for KV tiles in flight (the attention phase is bound by KV load latency)
-  static constexpr int STAGES = (NB == 16) ? 6 : 4;
-  static constexpr int NKV = 3;
-#else
   static constexpr int STAGES = (NB == 16) ? 7 : 5;
   static constexpr int NKV = 2;
-#endif
   static constexpr int B_BYTES = PC_BKB_MAX * NB * 128;
   static constexpr int RH = NB / 2;                       // activation rows carried (hi rows; lo rows follow)
   static constexpr int ACC_LD = TILE_ROWS + 4;            // accumulator slot [RH][ACC_LD] fp32 (pad: conflict-free stores)
@@ -105,9 +100,6 @@ struct PcParams {
   int n_layer, D, F, V, H, S_max, R, n_utts, kv_fp32;
   int n_steps;     // decode positions this launch runs
   int fused;       // 1: sample in the kernel and advance the decode state (top_k == 0 only); 0: leave normalised logits
-  int pf_mode;     // 0: no L2 prefetch, 1: by the producer while the ring is full, 2: dedicated prefetch warp
-  int pf_ahead;    // weight tiles prefetched into L2 ahead of the smem ring
-  int kv_pf;       // 1: L2-prefetch the next layer's KV tiles while this layer's projections stream
   float eps;
   PcMat m_qkv, m_o, m_w13, m_w2, m_head;
   const __nv_bfloat16* attn_norm;   // layer 0; layer l at + l * layer_stride
@@ -129,8 +121,7 @@ struct PcParams {
   char* kv;
   size_t kv_half;  // bytes of one layer's K (or V) region
   unsigned* bar;   // grid-wide arrival counter (zero at launch)
-  int att_mma;       // 1: bf16 KV tiles arrive 128B-swizzled through tm_kv and the attention runs on mma.sync (see the attention phase)
-  long long kv_rows_half;   // cache rows (positions) of one layer's K (or V) region = kv_half / 256
+  long long kv_rows_half;   // bf16 cache: rows (positions) of one layer's K (or V) region in tm_kv = kv_half / 256
   long long* trace;  // optional [gridDim][PC_TRACE_EVENTS] clock64 stamps of compute-thread 0 (debug)
   S1State st;
 };
@@ -263,17 +254,11 @@ __device__ __forceinline__ void pc_mma_stage(uint32_t w_base, uint32_t x_base, i
   }
 }
 
-template <bool KV_FP32>
+// dims 8 sub .. 8 sub + 7 of position p of an fp32 KV tile
 __device__ __forceinline__ void load8s(const uint8_t* tile, int p, int sub, float (&v)[8]) {
-  if (KV_FP32) {
-    const float4* q = reinterpret_cast<const float4*>(tile + (size_t)p * 512 + sub * 32);
-    const float4 a = q[0], b = q[1];
-    v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
-  } else {
-    const uint4 w = *reinterpret_cast<const uint4*>(tile + (size_t)p * 256 + sub * 16);
-    v[0] = bf_lo(w.x); v[1] = bf_hi(w.x); v[2] = bf_lo(w.y); v[3] = bf_hi(w.y);
-    v[4] = bf_lo(w.z); v[5] = bf_hi(w.z); v[6] = bf_lo(w.w); v[7] = bf_hi(w.w);
-  }
+  const float4* q = reinterpret_cast<const float4*>(tile + (size_t)p * 512 + sub * 32);
+  const float4 a = q[0], b = q[1];
+  v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
 }
 
 template <bool KV_FP32, int NB>
@@ -315,7 +300,6 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
       ptx::mbar_init(ptx::smem_u32(sh.kv_empty + i), 1);
     }
     ptx::mbar_init(ptx::smem_u32(&sh.tab_ready), 1);
-    sh.prod_pos = 0;
     ptx::fence_barrier_init();
   }
   // zero the activation operand once: rows >= R (hi and lo halves) must read as zero forever
@@ -335,8 +319,11 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
   const int per_layer = c_q + c_o + c_f + c_2;
   const int total_tiles = p.n_layer * per_layer + s_head.nt * nk_h;
 
+  // There is no warp 6 (PC_THREADS = 192).  Testing for it anyway makes ptxas place the producer's loop ahead of the
+  // compute warps' code; with `warp == 0` alone the loop lands at the end of the kernel, and 8-utterance decode measured
+  // 1.5 % slower on an H100 SXM at 700 W.
   if (warp == 0 || warp == 6) {
-    // =================================== PRODUCER / L2 PREFETCHER ===================================
+    // =================================== PRODUCER ===================================================
     // The whole warp walks the schedule (warp-uniform control flow and operands); one elected lane issues the TMA /
     // bulk-copy instructions.  Issuing them from a `lane == 0` branch makes the compiler wrap each UTMALDG in an
     // ELECT + 4 x R2UR.BROADCAST + vote loop, which capped one producer at a tile per ~0.25 us.
@@ -361,131 +348,94 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
       __syncwarp();
     };
     const long long total_all = (long long)total_tiles * p.n_steps;
-    if (warp == 6) {
-      if (p.pf_mode == 2 && total_tiles > 0) {
-        // Dedicated L2 prefetcher: keeps the window (issued, issued + pf_ahead] of the flat tile schedule in flight so
-        // that HBM keeps streaming while the grid synchronises; it never touches the smem ring.
-        const uint32_t pp = ptx::smem_u32(&sh.prod_pos);
-        long long n = STAGES;
-        while (n < total_all) {
-          int pos_l;
-          asm volatile("ld.volatile.shared.u32 %0, [%1];" : "=r"(pos_l) : "r"(pp) : "memory");
-          const long long pos = __shfl_sync(0xffffffffu, pos_l, 0);   // one value for the whole warp
-          if (n < pos) n = pos;
-          if (n < pos + p.pf_ahead) { prefetch_flat((int)(n % total_tiles)); ++n; }
-          else __nanosleep(64);
+    const uint64_t pol = ptx::policy_evict_first();
+    uint32_t slot = 0, kv_ctr = 0;
+    long long issued = 0, pf_next = 0;   // L2 prefetch only while the ring is full
+    auto gemm_tiles = [&](const CUtensorMap* tmA, const CUtensorMap* tmB2, int split_t, const PcSlice& sl, int layer) {
+      for (int i = 0; i < sl.nt; ++i) {
+        const int t = sl.t0 + i * sl.G;
+        const CUtensorMap* tm = (t < split_t) ? tmA : tmB2;
+        const int tt = (t < split_t) ? t : t - split_t;
+        for (int kb = sl.kb0; kb < sl.kb1; ++kb) {
+          const auto [s, ph] = ring_pos(slot, STAGES);
+          ++slot;
+          const uint32_t eb = ptx::smem_u32(sh.b_empty + s);
+          if (!ptx::mbar_test_wait(eb, ph ^ 1u)) {
+            // the ring is full: spend the idle time pulling upcoming tiles into L2 (non-blocking probe)
+            if (pf_next <= issued) pf_next = issued + 1;      // never prefetch a tile that is about to be loaded
+            while (pf_next < issued + 1 + PC_PF_AHEAD && pf_next < total_all && !ptx::mbar_test_wait(eb, ph ^ 1u)) {
+              prefetch_flat((int)(pf_next % total_tiles));
+              ++pf_next;
+            }
+          }
+          ptx::mbar_wait(eb, ph ^ 1u);
+          ++issued;
+          if (ptx::elect_one()) {
+            const uint32_t full = ptx::smem_u32(sh.b_full + s);
+            ptx::mbar_arrive_expect_tx(full, STAGE_BYTES);
+            ptx::tma_load_3d_hint(ptx::smem_u32(ring + (size_t)s * STAGE_BYTES), tm, full, kb * 64, tt * TILE_ROWS, layer, pol);
+          }
+          __syncwarp();
         }
       }
-    } else {
-      const uint64_t pol = ptx::policy_evict_first();
-      const uint32_t pp = ptx::smem_u32(&sh.prod_pos);
-      uint32_t slot = 0, kv_ctr = 0;
-      long long issued = 0, pf_next = 0;   // inline prefetch (pf_mode 1) only while the ring is full
-      auto gemm_tiles = [&](const CUtensorMap* tmA, const CUtensorMap* tmB2, int split_t, const PcSlice& sl, int layer) {
-        for (int i = 0; i < sl.nt; ++i) {
-          const int t = sl.t0 + i * sl.G;
-          const CUtensorMap* tm = (t < split_t) ? tmA : tmB2;
-          const int tt = (t < split_t) ? t : t - split_t;
-          for (int kb = sl.kb0; kb < sl.kb1; ++kb) {
-            const auto [s, ph] = ring_pos(slot, STAGES);
-            ++slot;
-            const uint32_t eb = ptx::smem_u32(sh.b_empty + s);
-            if (p.pf_mode == 1 && !ptx::mbar_test_wait(eb, ph ^ 1u)) {
-              // the ring is full: spend the idle time pulling upcoming tiles into L2 (non-blocking probe)
-              if (pf_next <= issued) pf_next = issued + 1;      // never prefetch a tile that is about to be loaded
-              while (pf_next < issued + 1 + p.pf_ahead && pf_next < total_all && !ptx::mbar_test_wait(eb, ph ^ 1u)) {
-                prefetch_flat((int)(pf_next % total_tiles));
-                ++pf_next;
-              }
-            }
-            ptx::mbar_wait(eb, ph ^ 1u);
-            ++issued;
-            if (ptx::elect_one()) {
-              const uint32_t full = ptx::smem_u32(sh.b_full + s);
-              ptx::mbar_arrive_expect_tx(full, STAGE_BYTES);
-              ptx::tma_load_3d_hint(ptx::smem_u32(ring + (size_t)s * STAGE_BYTES), tm, full, kb * 64, tt * TILE_ROWS, layer, pol);
-              asm volatile("st.shared.u32 [%0], %1;" ::"r"(pp), "r"((int)issued) : "memory");
-            }
-            __syncwarp();
-          }
-        }
-      };
-      // KV tiles [from, to) (in this CTA's table order) of layer l; positions < pos come from earlier steps
-      auto kv_units = [&](int l, int from, int to) {
-        const char* kbase = p.kv + (size_t)l * 2 * p.kv_half;
-        const char* vbase = kbase + p.kv_half;
-        const int n_tiles = sh.n_att_tiles;
-        int idx = 0;
-        for (int i = 0; i < n_tiles; ++i) {
-          const AttTile e = sh.att_tab[i];
-          const int npos = (int)(e.meta & 0xffu);
-          if (npos == 0) continue;                 // only the current position: it comes from registers
-          const int my = idx++;
-          if (my < from) continue;
-          if (my >= to) break;
-          const auto [ks, ph] = ring_pos(kv_ctr, Cfg::NKV);
-          ++kv_ctr;
-          ptx::mbar_wait(ptx::smem_u32(sh.kv_empty + ks), ph ^ 1u);
-          if (ptx::elect_one()) {
-            const uint32_t full = ptx::smem_u32(sh.kv_full + ks);
-            uint8_t* dst = kvbuf + (size_t)ks * 2 * PC_KV_TILE_BYTES;
-            if (!KV_FP32 && p.att_mma) {
-              // 64 positions x 128 dims as two 128B-swizzled [64 x 64] boxes per operand (conflict-free ldmatrix); rows past
-              // npos are older / zero cache contents and are masked by the consumer
-              const int row = (int)((long long)l * 2 * p.kv_rows_half + (long long)(e.off >> 8));
-              const int rowv = row + (int)p.kv_rows_half;
-              ptx::mbar_arrive_expect_tx(full, 2u * PC_KV_TILE_BYTES);
-              ptx::tma_load_2d(ptx::smem_u32(dst), &tm_kv, full, 0, row);
-              ptx::tma_load_2d(ptx::smem_u32(dst + 8192), &tm_kv, full, 64, row);
-              ptx::tma_load_2d(ptx::smem_u32(dst + PC_KV_TILE_BYTES), &tm_kv, full, 0, rowv);
-              ptx::tma_load_2d(ptx::smem_u32(dst + PC_KV_TILE_BYTES + 8192), &tm_kv, full, 64, rowv);
-            } else {
-              const uint32_t bytes = (uint32_t)npos * 128 * esz;
-              ptx::mbar_arrive_expect_tx(full, 2 * bytes);
-              ptx::bulk_load(ptx::smem_u32(dst), kbase + e.off, bytes, full);
-              ptx::bulk_load(ptx::smem_u32(dst + PC_KV_TILE_BYTES), vbase + e.off, bytes, full);
-            }
-          }
-          __syncwarp();
-        }
-      };
-      // Pull every KV tile this CTA will need for layer l into L2 ahead of time: with only Cfg::NKV tile slots in shared
-      // memory the attention phase would otherwise pay an HBM round trip per tile (batch 8: 55 MB of K/V per layer).
-      auto kv_prefetch_l2 = [&](int l) {
-        const char* kbase = p.kv + (size_t)l * 2 * p.kv_half;
-        const char* vbase = kbase + p.kv_half;
-        const int n_tiles = sh.n_att_tiles;
-        for (int i = 0; i < n_tiles; ++i) {
-          const AttTile e = sh.att_tab[i];
-          const uint32_t bytes = (e.meta & 0xffu) * 128u * (uint32_t)esz;
-          if (bytes == 0) continue;
-          if (ptx::elect_one()) {
-            asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(kbase + e.off), "r"(bytes) : "memory");
-            asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(vbase + e.off), "r"(bytes) : "memory");
-          }
-          __syncwarp();
-        }
-      };
-      for (int step = 0; step < p.n_steps; ++step) {
-        for (int l = 0; l < p.n_layer; ++l) {
-          if (l == 0) {
-            gemm_tiles(&tm_qkv, &tm_qkv, 1 << 30, s_qkv, 0);   // weights first: they need nothing from the previous token
-            ptx::mbar_wait(ptx::smem_u32(&sh.tab_ready), step & 1u);   // this token's tile table is built
-            kv_units(0, 0, 1 << 30);
+    };
+    // KV tiles [from, to) (in this CTA's table order) of layer l; positions < pos come from earlier steps
+    auto kv_units = [&](int l, int from, int to) {
+      const char* kbase = p.kv + (size_t)l * 2 * p.kv_half;
+      const char* vbase = kbase + p.kv_half;
+      const int n_tiles = sh.n_att_tiles;
+      int idx = 0;
+      for (int i = 0; i < n_tiles; ++i) {
+        const AttTile e = sh.att_tab[i];
+        const int npos = (int)(e.meta & 0xffu);
+        if (npos == 0) continue;                 // only the current position: it comes from registers
+        const int my = idx++;
+        if (my < from) continue;
+        if (my >= to) break;
+        const auto [ks, ph] = ring_pos(kv_ctr, Cfg::NKV);
+        ++kv_ctr;
+        ptx::mbar_wait(ptx::smem_u32(sh.kv_empty + ks), ph ^ 1u);
+        if (ptx::elect_one()) {
+          const uint32_t full = ptx::smem_u32(sh.kv_full + ks);
+          uint8_t* dst = kvbuf + (size_t)ks * 2 * PC_KV_TILE_BYTES;
+          if constexpr (!KV_FP32) {
+            // 64 positions x 128 dims as two 128B-swizzled [64 x 64] boxes per operand (conflict-free ldmatrix); rows past
+            // npos are older / zero cache contents and are masked by the consumer
+            const int row = (int)((long long)l * 2 * p.kv_rows_half + (long long)(e.off >> 8));
+            const int rowv = row + (int)p.kv_rows_half;
+            ptx::mbar_arrive_expect_tx(full, 2u * PC_KV_TILE_BYTES);
+            ptx::tma_load_2d(ptx::smem_u32(dst), &tm_kv, full, 0, row);
+            ptx::tma_load_2d(ptx::smem_u32(dst + 8192), &tm_kv, full, 64, row);
+            ptx::tma_load_2d(ptx::smem_u32(dst + PC_KV_TILE_BYTES), &tm_kv, full, 0, rowv);
+            ptx::tma_load_2d(ptx::smem_u32(dst + PC_KV_TILE_BYTES + 8192), &tm_kv, full, 64, rowv);
           } else {
-            kv_units(l, Cfg::NKV, 1 << 30);                       // (units beyond the prefetched ones)
-          }
-          if (p.kv_pf && l + 1 < p.n_layer) kv_prefetch_l2(l + 1);
-          gemm_tiles(&tm_o, &tm_o, 1 << 30, s_o, l);
-          gemm_tiles(&tm_w1, &tm_w3, T1, s_w13, l);
-          gemm_tiles(&tm_w2, &tm_w2, 1 << 30, s_w2, l);
-          if (l + 1 < p.n_layer) {
-            kv_units(l + 1, 0, Cfg::NKV);                         // next layer's first KV tiles ride ahead of its QKV GEMM
-            gemm_tiles(&tm_qkv, &tm_qkv, 1 << 30, s_qkv, l + 1);
+            const uint32_t bytes = (uint32_t)npos * 128 * esz;
+            ptx::mbar_arrive_expect_tx(full, 2 * bytes);
+            ptx::bulk_load(ptx::smem_u32(dst), kbase + e.off, bytes, full);
+            ptx::bulk_load(ptx::smem_u32(dst + PC_KV_TILE_BYTES), vbase + e.off, bytes, full);
           }
         }
-        gemm_tiles(&tm_head, &tm_head, 1 << 30, s_head, 0);
+        __syncwarp();
       }
+    };
+    for (int step = 0; step < p.n_steps; ++step) {
+      for (int l = 0; l < p.n_layer; ++l) {
+        if (l == 0) {
+          gemm_tiles(&tm_qkv, &tm_qkv, 1 << 30, s_qkv, 0);   // weights first: they need nothing from the previous token
+          ptx::mbar_wait(ptx::smem_u32(&sh.tab_ready), step & 1u);   // this token's tile table is built
+          kv_units(0, 0, 1 << 30);
+        } else {
+          kv_units(l, Cfg::NKV, 1 << 30);                       // (units beyond the prefetched ones)
+        }
+        gemm_tiles(&tm_o, &tm_o, 1 << 30, s_o, l);
+        gemm_tiles(&tm_w1, &tm_w3, T1, s_w13, l);
+        gemm_tiles(&tm_w2, &tm_w2, 1 << 30, s_w2, l);
+        if (l + 1 < p.n_layer) {
+          kv_units(l + 1, 0, Cfg::NKV);                         // next layer's first KV tiles ride ahead of its QKV GEMM
+          gemm_tiles(&tm_qkv, &tm_qkv, 1 << 30, s_qkv, l + 1);
+        }
+      }
+      gemm_tiles(&tm_head, &tm_head, 1 << 30, s_head, 0);
     }
   } else if (warp == 1) {
     // =================================== MMA WARP ===================================================
@@ -797,15 +747,15 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
         zero_slice(p.gu, (size_t)PC_RPAD * 2 * p.F);   // free since the previous layer's w2 phase; ordered by the next arrive
         grid_wait();
         stamp();
-        if (!KV_FP32 && p.att_mma) {
+        if constexpr (!KV_FP32) {
           // ===== tensor-core attention (bf16 cache): per 64-position tile  S = K q  and  o += V^T p  as mma.sync m16n8k16 with the
           // vector operand in column 0 of the 8-wide B fragment (lanes 0..3), K / V^T blocks through ldmatrix from the
           // 128B-swizzled tiles.  q and p ride as two bf16 terms (hi + lo, 2^-17), K and V are exactly the cache contents,
-          // accumulation is fp32: the same numerics class as the scalar path.  Warp w scores positions [16w, 16w+16) and
+          // accumulation is fp32: the same numerics class as the fp32-cache loop.  Warp w scores positions [16w, 16w+16) and
           // accumulates output dims [32w, 32w+32); every warp keeps the identical running (max, sum).
           char* kbase = p.kv + (size_t)l * 2 * p.kv_half;
           char* vbase = kbase + p.kv_half;
-          uint32_t* q_hi = reinterpret_cast<uint32_t*>(sh.o);     // [64] packed pairs   (sh.o is the scalar path's merge buffer)
+          uint32_t* q_hi = reinterpret_cast<uint32_t*>(sh.o);     // [64] packed pairs   (sh.o is the fp32-cache loop's merge buffer)
           uint32_t* q_lo = q_hi + 64;                             // [64]
           float* scv = reinterpret_cast<float*>(q_lo + 64);       // [64] scores of the tile
           float* qf = scv + 64;                                   // [128] fp32 q (current-token dot product)
@@ -814,12 +764,6 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
           float m = -INFINITY, lsum = 0.f, kcur = 0.f, vcur = 0.f;
           float oacc[2][4];
           const int n_tiles = sh.n_att_tiles;
-#ifdef PC_ATT_PROF
-          long long a_t[5] = {0, 0, 0, 0, 0}, a_c = clock64();   // begin | append cur | kv wait | tile math | cur + unit end
-#define PC_ATT_MARK(k) { const long long _n = clock64(); a_t[k] += _n - a_c; a_c = _n; }
-#else
-#define PC_ATT_MARK(k)
-#endif
           for (int ti = 0; ti < n_tiles; ++ti) {
             const AttTile e = sh.att_tab[ti];
             const int npos = (int)(e.meta & 0xffu);
@@ -847,7 +791,6 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
               for (int i = 0; i < 4; ++i) { oacc[0][i] = 0.f; oacc[1][i] = 0.f; }
               compute_sync();                                    // q visible to every warp
             }
-            PC_ATT_MARK(0)
             if (has_cur) {
               // append the new token's k, v to the cache, rounded as the cache stores them; share them via smem
               const size_t ce = (((size_t)cr * p.H + h) * p.S_max + (L - 1)) * 128 + ct;
@@ -860,12 +803,10 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
               sh.cur[ct] = kcur;
               sh.cur[128 + ct] = vcur;
             }
-            PC_ATT_MARK(1)
             if (npos > 0) {
               const auto [ks, ph] = ring_pos(kv_ctr, Cfg::NKV);
               ++kv_ctr;
               ptx::mbar_wait(ptx::smem_u32(sh.kv_full + ks), ph);
-              PC_ATT_MARK(2)
               const uint32_t kt = ptx::smem_u32(kvbuf + (size_t)ks * 2 * PC_KV_TILE_BYTES);
               const uint32_t vt = kt + PC_KV_TILE_BYTES;
               if (16 * cw < npos) {
@@ -938,7 +879,6 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
               }
 #pragma unroll
               for (int i = 0; i < 4; ++i) { oacc[0][i] += olo[0][i]; oacc[1][i] += olo[1][i]; }
-              PC_ATT_MARK(3)
             }
             if (npos > 0 || has_cur) compute_sync();   // KV tile fully consumed; sh.cur visible
             if (npos > 0 && ct == 0) ptx::mbar_arrive(ptx::smem_u32(sh.kv_empty + ring_pos(kv_ctr - 1, Cfg::NKV).stage));
@@ -972,28 +912,16 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
               const float ltot = warp_sum(lsum);
               if (ct == 0) { p.part_ml[pidx * 2] = m; p.part_ml[pidx * 2 + 1] = ltot; }
               compute_sync();   // q / score scratch and sh.cur are reused by the next unit
-              PC_ATT_MARK(4)
             }
           }
-#ifdef PC_ATT_PROF
-          if (p.trace != nullptr && ct == 0)
-            for (int k = 0; k < 5; ++k) p.trace[(size_t)cta * PC_TRACE_EVENTS + 380 + l * 5 + k] = a_t[k];
-#endif
-#undef PC_ATT_MARK
-        } else
-        {
+        } else {
+          // ===== fp32 cache: each half-warp runs an online softmax over its share of the tile's positions
           char* kbase = p.kv + (size_t)l * 2 * p.kv_half;
           char* vbase = kbase + p.kv_half;
           const int half = lane >> 4, sub = lane & 15;
           const int hw = cw * 2 + half;               // half-warp id 0..7
           float q[8], o[8], m = -INFINITY, lsum = 0.f, kcur = 0.f, vcur = 0.f;
           const int n_tiles = sh.n_att_tiles;
-#ifdef PC_ATT_PROF
-          long long a_t[5] = {0, 0, 0, 0, 0}, a_c = clock64();   // begin | append cur | kv wait | tile math | unit end
-#define PC_ATT_MARK(k) { const long long _n = clock64(); a_t[k] += _n - a_c; a_c = _n; }
-#else
-#define PC_ATT_MARK(k)
-#endif
           for (int ti = 0; ti < n_tiles; ++ti) {
             const AttTile e = sh.att_tab[ti];
             const int npos = (int)(e.meta & 0xffu);
@@ -1021,32 +949,21 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
 #pragma unroll
               for (int i = 0; i < 8; ++i) o[i] = 0.f;
             }
-            PC_ATT_MARK(0)
             // ---- one KV tile (and, on the row's last tile, the current token)
             if (has_cur) {
-              // append the new token's k, v to the cache, rounded as the cache stores them; share them via smem
+              // append the new token's k, v to the cache; share them via smem
               const size_t ce = (((size_t)cr * p.H + h) * p.S_max + (L - 1)) * 128 + ct;
-              if (KV_FP32) {
-                reinterpret_cast<float*>(kbase)[ce] = kcur;
-                reinterpret_cast<float*>(vbase)[ce] = vcur;
-              } else {
-                const __nv_bfloat16 kb16 = __float2bfloat16_rn(kcur), vb16 = __float2bfloat16_rn(vcur);
-                reinterpret_cast<__nv_bfloat16*>(kbase)[ce] = kb16;
-                reinterpret_cast<__nv_bfloat16*>(vbase)[ce] = vb16;
-                kcur = __bfloat162float(kb16);
-                vcur = __bfloat162float(vb16);
-              }
+              reinterpret_cast<float*>(kbase)[ce] = kcur;
+              reinterpret_cast<float*>(vbase)[ce] = vcur;
               // the next token's KV tiles are fetched with cp.async.bulk (async proxy) inside this same launch
               asm volatile("fence.proxy.async.global;" ::: "memory");
               sh.cur[ct] = kcur;
               sh.cur[128 + ct] = vcur;
             }
-            PC_ATT_MARK(1)
             if (npos > 0) {
               const auto [ks, ph] = ring_pos(kv_ctr, Cfg::NKV);
               ++kv_ctr;
               ptx::mbar_wait(ptx::smem_u32(sh.kv_full + ks), ph);
-              PC_ATT_MARK(2)
               const uint8_t* kt = kvbuf + (size_t)ks * 2 * PC_KV_TILE_BYTES;
               const uint8_t* vt = kt + PC_KV_TILE_BYTES;
               // each half-warp owns positions hw, hw+8, ... (hw = 2 * warp + half); two positions per trip for ILP (four per
@@ -1059,8 +976,8 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
                 const bool vA = pA0 < npos, vB = pB0 < npos;
                 const int pA = vA ? pA0 : 0, pB = vB ? pB0 : 0;
                 float ka[8], kb2[8], sA = 0.f, sA1 = 0.f, sB = 0.f, sB1 = 0.f;
-                load8s<KV_FP32>(kt, pA, sub, ka);
-                load8s<KV_FP32>(kt, pB, sub, kb2);
+                load8s(kt, pA, sub, ka);
+                load8s(kt, pB, sub, kb2);
 #pragma unroll
                 for (int i = 0; i < 8; i += 2) {
                   sA = fmaf(q[i], ka[i], sA);
@@ -1075,8 +992,8 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
                   sA += __shfl_xor_sync(0xffffffffu, sA, off);
                   sB += __shfl_xor_sync(0xffffffffu, sB, off);
                 }
-                load8s<KV_FP32>(vt, pA, sub, ka);
-                load8s<KV_FP32>(vt, pB, sub, kb2);
+                load8s(vt, pA, sub, ka);
+                load8s(vt, pB, sub, kb2);
                 sA = vA ? sA : -INFINITY;
                 sB = vB ? sB : -INFINITY;
                 const float mn = fmaxf(m, fmaxf(sA, sB));
@@ -1102,7 +1019,6 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
               for (int i = 0; i < 8; ++i) o[i] = o[i] * corr + pw * sh.cur[128 + sub * 8 + i];
               m = mn;
             }
-            PC_ATT_MARK(3)
             if (unit_last) {
               // ---- unit end: merge the 8 half-warp states -> one partial (m, l, o[128]) for split z
               if (sub == 0) { sh.m[hw] = m; sh.l[hw] = lsum; }
@@ -1127,12 +1043,7 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
               }
               compute_sync();   // sh.o / sh.m / sh.cur are reused by the next unit
             }
-            PC_ATT_MARK(4)
           }
-#ifdef PC_ATT_PROF
-          if (p.trace != nullptr && ct == 0)
-            for (int k = 0; k < 5; ++k) p.trace[(size_t)cta * PC_TRACE_EVENTS + 380 + l * 5 + k] = a_t[k];
-#endif
         }
         stamp();
         grid_arrive();

@@ -144,25 +144,19 @@ struct mvb_s1 {
   cudaStream_t cap_stream = nullptr;
   uint64_t launches = 0;
   std::map<int, int> graph_nodes;
-  bool use_graph = true;
   int* h_flags = nullptr;  // pinned: done flags / counters read back by generate()
   // path B
   std::vector<CUtensorMap> tmW;                       // per layer {wqkv, wo, w1, w3, w2}, then lm_head
   std::map<std::pair<int, int>, CUtensorMap> tmB;     // (NB, K) -> activation buffer map
   bool path_b = true;                                 // tensor-core rows path for batched decode and prefill
   bool pdl = true;                                    // programmatic dependent launch between body kernels
-  int decode_b_min = 2;                               // utterances from which decode uses the tensor-core rows path
-  int split_lo = 1;                                   // carry activations as hi+lo bf16 terms
   RowsDev rows;
   // path C
   bool path_c = true;
   bool pc_ok = false;
   bool trace = false;
-  // persistent-kernel switches, read once at create (MVB_PC_FUSED, MVB_PF_MODE, MVB_PF_AHEAD)
-  bool fused = true;                                  // sample inside the persistent kernel (multi-token launches)
-  int pf_mode = 1, pf_ahead = 8, kv_pf = 0;
-  int att_mma = 1;                                    // bf16 cache: attention on mma.sync over TMA-swizzled KV tiles (MVB_PC_ATT_MMA=0: scalar)
-  CUtensorMap tm_kv;                                  // 2-D map over the whole bf16 KV arena: [rows = layer, k|v, cache row, head, pos][128]
+  bool fused = true;                                  // sample inside the persistent kernel (multi-token launches; MVB_PC_FUSED)
+  CUtensorMap tm_kv;                                  // bf16 cache: 2-D map over the whole KV arena: [rows = layer, k|v, cache row, head, pos][128]
   CUtensorMap tm3[6];                                 // 3-D (k, row, layer) maps: wqkv, wo, w1, w3, w2, head
   PcMat pm[5];
   std::vector<int> h_topk;                            // top_k of every utterance slot as installed by mvb_s1_begin
@@ -192,12 +186,11 @@ struct mvb_s1 {
 
 
 // Static decomposition of one matrix over `ctas` CTAs: the K split that minimises the busiest CTA's modelled phase time.
-static PcMat plan_pc(int M, int K, int ctas, int tile_rows, int force_S = 0) {
+static PcMat plan_pc(int M, int K, int ctas, int tile_rows) {
   PcMat best{};
   long best_cost = -1;
   const int T = (M + tile_rows - 1) / tile_rows, KB = K / 64;
   for (int S = 1; S <= KB && S <= 32 && S <= ctas; ++S) {
-    if (force_S > 0 && S != force_S) continue;   // MVB_PC_SPLITS experiment switch
     const int Gp = ctas / S;
     const int tiles_per = (T + Gp - 1) / Gp;
     const int kb_per = (KB + S - 1) / S;
@@ -318,11 +311,8 @@ static int create_engine(const mvb_s1_config* cfg, const void* d_arena, size_t a
   s.noise_base = h->wsp<int>(h->L.noise_base);
   s.max_new = cfg->max_new;
   s.block_size = cfg->block_size;
-  h->use_graph = getenv("MVB_NO_GRAPH") == nullptr;
   if (const char* e = getenv("MVB_PATHB")) h->path_b = atoi(e) != 0;
   if (const char* e = getenv("MVB_PDL")) h->pdl = atoi(e) != 0;
-  if (const char* e = getenv("MVB_DECODE_B_MIN")) h->decode_b_min = atoi(e);
-  if (const char* e = getenv("MVB_SPLIT_LO")) h->split_lo = atoi(e) != 0;
   {
     int* rb = h->wsp<int>(h->L.b_rows);
     h->rows.cache_row = rb; h->rows.pos = rb + RB_MAX; h->rows.tok = rb + 2 * RB_MAX; h->rows.utt = rb + 3 * RB_MAX;
@@ -342,24 +332,21 @@ static int create_engine(const mvb_s1_config* cfg, const void* d_arena, size_t a
   }
   if (const char* e = getenv("MVB_PATHC")) h->path_c = atoi(e) != 0;
   if (const char* e = getenv("MVB_PC_TRACE")) h->trace = atoi(e) != 0;
-  if (const char* e = getenv("MVB_PF_AHEAD")) h->pf_ahead = atoi(e);
-  if (const char* e = getenv("MVB_PF_MODE")) h->pf_mode = atoi(e);
-  if (const char* e = getenv("MVB_PC_KVPF")) h->kv_pf = atoi(e);
-  if (const char* e = getenv("MVB_PC_ATT_MMA")) h->att_mma = atoi(e);
+  if (const char* e = getenv("MVB_PC_FUSED")) h->fused = atoi(e) != 0;
+  // The persistent kernel's bf16-cache attention fetches KV tiles through tm_kv as whole 64-position boxes: positions
+  // past the valid ones must hold finite values, and the map must be encodable.  Where it is not, path C is declined.
   memset(&h->tm_kv, 0, sizeof(h->tm_kv));
-  if (cfg->kv_dtype != MVB_KV_BF16 || cfg->block_size % 64 || cfg->head_dim != 128) h->att_mma = 0;
-  if (h->att_mma) {
-    // the tensor-core attention reads whole 64-position boxes: positions past the valid ones must hold finite values
+  bool kv_ok = cfg->kv_dtype == MVB_KV_FP32;
+  if (cfg->kv_dtype == MVB_KV_BF16 && cfg->block_size % 64 == 0) {
     CK(cudaMemset(h->kv, 0, (size_t)cfg->n_layer * 2 * h->kv_half_bytes()));
     const uint64_t rows = (uint64_t)cfg->n_layer * 2 * (h->kv_half_bytes() / 256);
-    if (rows >= (1ull << 31) || !make_tmap_bf16(&h->tm_kv, h->kv, rows, 128, 64)) h->att_mma = 0;
+    kv_ok = rows < (1ull << 31) && make_tmap_bf16(&h->tm_kv, h->kv, rows, 128, 64);
   }
-  if (const char* e = getenv("MVB_PC_FUSED")) h->fused = atoi(e) != 0;
   h->h_topk.assign(cfg->max_utts, 0);
   {
     // persistent decode kernel: needs a uniform layer stride (true for arenas packed in checkpoint order)
     const int D = cfg->dim, F = cfg->intermediate, V = cfg->vocab;
-    bool ok = cfg->n_layer >= 1 && !int4;            // an int4 engine never uses path C
+    bool ok = cfg->n_layer >= 1 && !int4 && kv_ok;   // an int4 engine never uses path C
     const int o0 = MVB_S1_GLOBAL_TENSORS;
     uint64_t stride = cfg->n_layer > 1 ? h->off[o0 + MVB_S1_LAYER_TENSORS] - h->off[o0] : 2 * (uint64_t)(4 * D * D + 3 * D * F + 2 * D);
     for (int l = 1; l < cfg->n_layer && ok; ++l)
@@ -375,13 +362,11 @@ static int create_engine(const mvb_s1_config* cfg, const void* d_arena, size_t a
     ok = ok && make_tmap_bf16_3d(&h->tm3[3], h->lw(0, 5), D, F, NL, stride, rows);
     ok = ok && make_tmap_bf16_3d(&h->tm3[4], h->lw(0, 6), F, D, NL, stride, rows);
     ok = ok && make_tmap_bf16_3d(&h->tm3[5], h->w(4), D, V, 1, (uint64_t)V * D * 2, rows);
-    int fs[5] = {0, 0, 0, 0, 0};               // MVB_PC_SPLITS="q_o_w13_w2_head": force the K split of a matrix (0 = planner)
-    if (const char* e = getenv("MVB_PC_SPLITS")) sscanf(e, "%d_%d_%d_%d_%d", &fs[0], &fs[1], &fs[2], &fs[3], &fs[4]);
-    h->pm[0] = plan_pc(3 * D, D, h->n_sm, rows, fs[0]);
-    h->pm[1] = plan_pc(D, D, h->n_sm, rows, fs[1]);
-    h->pm[2] = plan_pc(2 * F, D, h->n_sm, rows, fs[2]);
-    h->pm[3] = plan_pc(D, F, h->n_sm, rows, fs[3]);
-    h->pm[4] = plan_pc(V, D, h->n_sm, rows, fs[4]);
+    h->pm[0] = plan_pc(3 * D, D, h->n_sm, rows);
+    h->pm[1] = plan_pc(D, D, h->n_sm, rows);
+    h->pm[2] = plan_pc(2 * F, D, h->n_sm, rows);
+    h->pm[3] = plan_pc(D, F, h->n_sm, rows);
+    h->pm[4] = plan_pc(V, D, h->n_sm, rows);
     for (int i = 0; i < 5; ++i) ok = ok && h->pm[i].S > 0;
     ok = ok && (F % rows == 0) && (D % rows == 0);     // w1 | w3 share one tile index space: F must be whole tiles
     h->pc_ok = ok;
@@ -523,8 +508,8 @@ template <int EPI>
 static int linear_b(mvb_s1* h, cudaStream_t s, int R, const LinB& a, void* kc = nullptr, void* vc = nullptr) {
   const mvb_s1_config& c = h->cfg;
   TcGemm g{};
-  g.epi = EPI; g.R = R; g.Rpad = (R + 15) / 16 * 16; g.split_lo = h->split_lo;
-  g.tmB = tmap_b(h, g.Rpad * (h->split_lo ? 2 : 1), a.K);
+  g.epi = EPI; g.R = R; g.Rpad = (R + 15) / 16 * 16; g.split_lo = 1;   // activations as hi + lo bf16 terms
+  g.tmB = tmap_b(h, 2 * g.Rpad, a.K);
   if (!g.tmB) return fail(MVB_ERR_CUDA, "cuTensorMapEncodeTiled failed for the activation buffer");
   g.tmW = &h->tmW[a.widx]; g.tmW3 = &h->tmW[a.widx3];
   g.B = h->wsp<__nv_bfloat16>(h->L.b_B);
@@ -606,7 +591,6 @@ static int launch_persistent(mvb_s1* h, cudaStream_t s, int n_utts, int n_steps,
   PcParams p{};
   p.n_layer = c.n_layer; p.D = c.dim; p.F = c.intermediate; p.V = c.vocab; p.H = c.n_head; p.S_max = c.block_size;
   p.n_steps = n_steps; p.fused = fused ? 1 : 0;
-  p.pf_mode = h->pf_mode; p.pf_ahead = h->pf_ahead; p.kv_pf = h->kv_pf;
   p.R = 2 * n_utts; p.n_utts = n_utts; p.kv_fp32 = c.kv_dtype == MVB_KV_FP32; p.eps = c.norm_eps;
   p.m_qkv = h->pm[0]; p.m_o = h->pm[1]; p.m_w13 = h->pm[2]; p.m_w2 = h->pm[3]; p.m_head = h->pm[4];
   p.attn_norm = h->lw(0, 0); p.ffn_norm = h->lw(0, 3); p.out_norm = h->w(3);
@@ -619,7 +603,7 @@ static int launch_persistent(mvb_s1* h, cudaStream_t s, int n_utts, int n_steps,
   p.samp_part = h->wsp<float>(h->L.c_samp_part);
   p.samp_best = h->wsp<unsigned long long>(h->L.c_samp_best);
   p.kv = h->kv; p.kv_half = h->kv_half_bytes();
-  p.att_mma = h->att_mma; p.kv_rows_half = (long long)(h->kv_half_bytes() / 256);
+  p.kv_rows_half = (long long)(h->kv_half_bytes() / 256);
   p.bar = h->wsp<unsigned>(h->L.c_bar);
   p.trace = (h->trace && h->n_sm <= 160) ? h->wsp<long long>(h->L.c_trace) : nullptr;
   p.st = h->st;
@@ -670,9 +654,8 @@ static int run_body(mvb_s1* h, cudaStream_t s, int n_utts, bool allow_b = true) 
   // Path A (CUDA-core GEMV) streams the weights once per utterance; from 2 utterances up the tensor-core
   // rows path streams them once per step for the whole batch.  slot_map must be the identity for path B
   // (its logits rows are batch-ordered), which mvb_s1_decode guarantees.
-  const bool use_b = allow_b && h->path_b && !h->int4 && n_utts >= h->decode_b_min;   // int4 decode: always path A
+  const bool use_b = allow_b && h->path_b && !h->int4 && n_utts >= 2;   // int4 decode: always path A
   auto body = [&](cudaStream_t st) { return use_b ? launch_body_b(h, st, n_utts) : launch_body(h, st, n_utts); };
-  if (!h->use_graph) return body(s);
   const int key = n_utts + (use_b ? 1000 : 0);
   auto it = h->graphs.find(key);
   if (it == h->graphs.end()) {
@@ -923,7 +906,7 @@ extern "C" int mvb_s1_decode(mvb_s1* h, int32_t n_utts, int32_t n_steps, void* s
 // positions installed with mvb_s1_begin) through the body mvb_s1_decode runs for that batch, logits copied out, no
 // sampling, state untouched except for the KV-cache append at the current positions.  That body is the persistent
 // fused kernel where mvb_s1_decode would use it (up to 8 utterances), else the per-layer path (tensor-core rows path
-// from decode_b_min utterances up).
+// from 2 utterances up).
 extern "C" int mvb_s1_step_logits(mvb_s1* h, int32_t n_utts, float* d_logits, void* stream) {
   if (!h || !d_logits) return fail(MVB_ERR_ARG, "null argument");
   if (n_utts < 1 || n_utts > h->cfg.max_utts) return fail(MVB_ERR_ARG, "n_utts %d out of range", n_utts);

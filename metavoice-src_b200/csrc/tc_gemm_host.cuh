@@ -4,7 +4,6 @@
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
-#include <stdlib.h>
 
 namespace mvb {
 
@@ -77,7 +76,7 @@ static inline GemmPlan plan_gemm(int M, int K, int NB, bool swiglu, int n_sm, in
   int ks = n_sm / g.tiles;
   if (ks < 1) ks = 1;
   if (ks > nkb / 2) ks = nkb / 2 > 0 ? nkb / 2 : 1;   // at least two k-blocks per split: tiny K is latency-, not bandwidth-bound
-  if (nkb <= 8 && getenv("MVB_GEMM_SPLIT_TINY") == nullptr) ks = 1;   // K <= 512 (stage-2 width): the split-K hand-off costs more than it buys
+  if (nkb <= 8) ks = 1;                                // K <= 512 (stage-2 width): the split-K hand-off costs more than it buys
   if (ks > 16) ks = 16;
   if (g.tiles > 128) ks = 1;                           // (the split-K arrival counters cover 128 tiles)
   g.ksplit = ks;

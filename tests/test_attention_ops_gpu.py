@@ -1,7 +1,7 @@
 """GPU: every attention kernel against a float64 softmax(q K^T / sqrt(128)) V, up to the full 2048-position context.
 
-Stage 1 (k_attn_decode / k_attn_rows over attn_core, and the attention phase of k_decode_persistent in its fp32-cache,
-bf16 mma.sync and bf16 scalar forms) is fused into engine launches whose merged output never reaches global memory, so it
+Stage 1 (k_attn_decode / k_attn_rows over attn_core, and the attention phase of k_decode_persistent in its fp32-cache
+and bf16 mma.sync forms) is fused into engine launches whose merged output never reaches global memory, so it
 is observed through a PROBE MODEL that the engine runs unchanged: one layer, attn_norm = ffn_norm = ln_f = 1,
 w1 = w3 = w2 = 0 (the FFN adds exactly 0), wo = I, lm_head = [I_D; 0], speaker projection 0.  Then
     logits[:, :D] = RMSNorm(x + y^)        (y^ = the merged attention output, x = tok_emb[tok] + pos_emb[pos])
@@ -35,9 +35,9 @@ in the normalisation, so each weight is off by exp(d_i) with |d_i| <= dw, and no
     scale factors common to all scores move them by <= |s| * 2^-21;
   * rho_p = 2^-17 for the mma form, which multiplies V by p as hi + lo bf16 while the row sum uses fp32 p.
 n_resc: rescales of one accumulator.  attn_core (paths A, B): a half-warp visits ceil(L/8)/8 positions, L/64 + 2;
-persistent scalar loop: one per 2-position trip of a half-warp, L/16 + 2; mma: one per 64-position tile, L/64 + 2.
+persistent fp32-cache loop: one per 2-position trip of a half-warp, L/16 + 2; mma: one per 64-position tile, L/64 + 2.
 n_acc: fp32 roundings along one output sum (and, separately, along the row sum; hence the factor 2): attn_core 2 per
-visited position + 8 half-warp and 8 split merges (x 2): L/32 + 40; scalar loop 3 per trip + 8 half-warp merges +
+visited position + 8 half-warp and 8 split merges (x 2): L/32 + 40; fp32-cache loop 3 per trip + 8 half-warp merges +
 <= 64 split merges (x 2) + current token: 3 L/16 + 160; mma: per tile 4 hi + 4 lo m16n8k16 into two accumulators at
 18u each plus the rescale and the add, i.e. <= 150u per 64 positions: 2.5 L + 160.
 Observation chain (tau_obs = 2^-15 for paths B and C, 2^-20 for path A): paths B and C carry y^ into wo as hi + lo bf16
@@ -90,15 +90,14 @@ MIXED_8 = [1, 2048, 33, 65, 129, 1000, 2, 1025]     # 8 utterances in one step, 
 # C: the persistent kernel
 BODY_LAUNCHES = {"A": 1 + 7, "B": 1 + 13, "C": 1 + 1}
 
-# path form -> (kv dtype, tensor_core_path, MVB_PC_ATT_MMA, body it must run)
+# path form -> (kv dtype, tensor_core_path, body it must run); on path C the bf16 cache runs the mma.sync form
 FORMS = {
-    "A-fp32": ("fp32", "", None, "A"),
-    "A-bf16": ("bf16", "", None, "A"),
-    "B-fp32": ("fp32", "B", None, "B"),
-    "B-bf16": ("bf16", "B", None, "B"),
-    "C-fp32": ("fp32", None, None, "C"),
-    "C-mma": ("bf16", None, "1", "C"),
-    "C-scalar": ("bf16", None, "0", "C"),
+    "A-fp32": ("fp32", "", "A"),
+    "A-bf16": ("bf16", "", "A"),
+    "B-fp32": ("fp32", "B", "B"),
+    "B-bf16": ("bf16", "B", "B"),
+    "C-fp32": ("fp32", None, "C"),
+    "C-mma": ("bf16", None, "C"),
 }
 
 
@@ -125,10 +124,10 @@ def expected_body(p, n_utts):
 
 def _params(form, L, body):
     """(n_resc, n_acc, rho_p) of the docstring for the body that ran."""
-    kv, _, mma, _ = FORMS[form]
+    kv = FORMS[form][0]
     if body in ("A", "B"):
         return L / 64 + 2, L / 32 + 40, 0.0
-    if kv == "bf16" and mma == "1":
+    if kv == "bf16":
         return L / 64 + 2, 2.5 * L + 160, 2.0 ** -17
     return L / 16 + 2, 3 * L / 16 + 160, 0.0
 
@@ -146,7 +145,7 @@ def softmax_eps(s, A, n_resc, n_acc, kappa, rho_p):
 class Probe:
     def __init__(self, H, form, utts, seed=0, n_layer=1):
         from mvb200.fast_model import ModelArgs, Transformer
-        kv, tc, mma, body = FORMS[form]
+        kv, tc, body = FORMS[form]
         self.H, self.D, self.form, self.body, self.kv = H, 128 * H, form, body, kv
         D = self.D
         self.V = 512 if D <= 256 else 2562
@@ -184,24 +183,14 @@ class Probe:
                        "transformer.h.1.mlp.c_proj.weight": torch.zeros(D, F)})
         sd = {k: v.to(torch.bfloat16) for k, v in sd.items()}
         cfg = ModelArgs(block_size=BLOCK, vocab_size=self.V, n_layer=n_layer, n_head=H, dim=D, intermediate_size=F)
-        import os
-        saved = os.environ.get("MVB_PC_ATT_MMA")
-        if mma is not None:
-            os.environ["MVB_PC_ATT_MMA"] = mma                      # read once in mvb_s1_create
-        try:
-            self.m = Transformer.from_state_dict(sd, cfg, device="cuda:0")
-            self.m.setup_caches(2 * utts, BLOCK, kv_dtype=kv, tensor_core_path=tc)
-        finally:
-            if saved is None:
-                os.environ.pop("MVB_PC_ATT_MMA", None)
-            else:
-                os.environ["MVB_PC_ATT_MMA"] = saved
+        self.m = Transformer.from_state_dict(sd, cfg, device="cuda:0")
+        self.m.setup_caches(2 * utts, BLOCK, kv_dtype=kv, tensor_core_path=tc)
         dt = torch.float32 if kv == "fp32" else torch.bfloat16
         self.kv_all = self.m._kv.view(dt).view(n_layer, 2, 2 * utts, H, BLOCK, 128)   # [layer][K|V][row][head][pos][128]
         self.cache = self.kv_all[0]
         self.tok_d, self.pos_d = self.tok.double().cuda(), self.pos.double().cuda()
         self.perm_d = [p.cuda() for p in self.perm]
-        if mma == "1":
+        if kv == "bf16" and body == "C":
             i = torch.arange(BLOCK, device="cuda")[:, None] + torch.arange(128, device="cuda")[None]
             self.poison = ((i % 2) * 2 - 1).to(dt) * 8192 * (1 + (i % 5).to(dt) / 8)   # finite: the mma form reads whole boxes
         else:
@@ -437,7 +426,7 @@ def test_split_merge_above_four_splits(probes):
     """H = 2, one utterance: zmax = n_sm / 4, so long rows are cut into more than 4 splits and the wo staging takes its
     nch > 4 merge branch (fp32: up to 64 tiles -> min(zmax, 64) splits)."""
     n_sm = torch.cuda.get_device_properties(0).multi_processor_count
-    for form, ppc in (("C-fp32", 32), ("C-mma", 64), ("C-scalar", 64)):
+    for form, ppc in (("C-fp32", 32), ("C-mma", 64)):
         p = probes(2, form, 8)
         for L in (1000, 2048):
             tt = (L + ppc - 1) // ppc
@@ -513,24 +502,9 @@ def test_prefill_every_position(probes, form, pos0):
     print(f"prefill {form} pos0={pos0}, 70 positions: max |err|/bound {worst:.2e}, normwise {nw:.2e}")
 
 
-def test_mma_and_scalar_forms_both_ran(probes):
-    """C-mma and C-scalar differ only in MVB_PC_ATT_MMA at engine creation.  The mma form carries q and p as hi + lo bf16
-    and sums in another order, so on identical inputs its logits are not bit-identical to the scalar loop's: an engine
-    that silently dropped to the scalar loop would fail here."""
-    out = {}
-    for form in ("C-mma", "C-scalar"):
-        p = probes(2, form, 8)
-        rows = run_decode(p, [2048], "wide", seed=11)
-        check_rows(p, rows, f"{form} form check")
-        out[form] = torch.stack([r["logits"] for r in rows])
-    diff = float((out["C-mma"] - out["C-scalar"]).abs().max())
-    print(f"C-mma vs C-scalar logits on identical inputs (L = 2048): max |diff| {diff:.2e}")
-    assert not torch.equal(out["C-mma"], out["C-scalar"])
-
-
 # ---- the fused multi-step burst ------------------------------------------------------------------------------------
 # (form, first position, last position): bursts that cross fp32 (32) and bf16 (64) tile boundaries, and the context end
-BURSTS = [("C-fp32", 28, 40), ("C-mma", 60, 70), ("C-scalar", 60, 70), ("C-fp32", 2030, 2047), ("C-mma", 2030, 2047)]
+BURSTS = [("C-fp32", 28, 40), ("C-mma", 60, 70), ("C-fp32", 2030, 2047), ("C-mma", 2030, 2047)]
 
 
 @pytest.mark.parametrize("n_utts", [1, 8])
@@ -618,7 +592,7 @@ def test_fused_burst_reads_back_its_own_appends(probes, form, first, last, n_utt
 
 
 # ---- sensitivity -------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("form", ["A-bf16", "B-fp32", "C-fp32", "C-mma", "C-scalar"])
+@pytest.mark.parametrize("form", ["A-bf16", "B-fp32", "C-fp32", "C-mma"])
 def test_altered_references_violate_the_bound(probes, form):
     p = probes(2, form, 8)
     nb = 2 if p.body == "B" else 1

@@ -16,7 +16,7 @@ from mvb200.fast_model import ModelArgs, Transformer, pack_arena  # noqa: E402
 
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 1
 L_mid = int(sys.argv[2]) if len(sys.argv) > 2 else 423
-for kv in (sys.argv[3].split("+") if len(sys.argv) > 3 and sys.argv[3] else []):   # e.g. MVB_PC_WB=0+MVB_PF_MODE=2
+for kv in (sys.argv[3].split("+") if len(sys.argv) > 3 and sys.argv[3] else []):   # e.g. MVB_PDL=0
     k, v = kv.split("=")
     os.environ[k] = v
 dev = torch.device("cuda:0"); torch.cuda.set_device(dev)
@@ -33,8 +33,9 @@ for u in range(n):
     _lib.check(lib.mvb_s1_begin(h, u, 100 + u, L_mid - 30, C.byref(sp), None, None, st))
 _lib.check(lib.mvb_s1_decode(h, n, 30, st))
 torch.cuda.synchronize()
-buf = np.zeros((148, 512), dtype=np.int64)
-got = lib.mvb_s1_trace_fetch(h, buf.ctypes.data_as(C.c_void_p), 148, st)
+G = torch.cuda.get_device_properties(dev).multi_processor_count   # one CTA per SM
+buf = np.zeros((G, 512), dtype=np.int64)
+got = lib.mvb_s1_trace_fetch(h, buf.ctypes.data_as(C.c_void_p), G, st)
 os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
 np.save(os.path.join(ROOT, "gpurun_out", f"trace_{n}.npy"), buf)
 t = buf[:, :2 + 14 * 24 + 4].astype(np.float64)
@@ -43,13 +44,8 @@ names = ["qkv.wait", "qkv.stage", "qkv.epi", "att.wait", "att.work", "o.wait", "
          "w13.epi", "w2.wait", "w2.stage", "w2.epi"]
 dt = np.diff(t, axis=1)          # interval ending at event i+1
 print("total us (median over CTAs):", np.median(t[:, -1]))
-per = dt[:, 1:1 + 14 * 24].reshape(148, 24, 14)   # skip start->embed
+per = dt[:, 1:1 + 14 * 24].reshape(G, 24, 14)   # skip start->embed
 for j, nm in enumerate(names):
     v = per[:, 2:, j]
     print(f"{nm:10s} median {np.median(v):7.2f}  mean {v.mean():7.2f}  p90 {np.percentile(v, 90):7.2f}  max {v.max():7.2f}")
 print("per-layer sum (median CTA):", np.median(per[:, 2:, :].sum(axis=2)))
-sub = buf[:, 380:380 + 5 * 24].astype(np.float64).reshape(148, 24, 5) / 1.9e3
-if sub.any():      # library built with -DPC_ATT_PROF: cumulative attention sub-phase clocks per layer
-    for j, nm in enumerate(["att.begin(q load)", "att.append_cur", "att.kv_wait", "att.tile_math", "att.unit_end"]):
-        v = sub[:, 2:, j]
-        print(f"{nm:18s} median {np.median(v):7.2f}  mean {v.mean():7.2f}  p90 {np.percentile(v, 90):7.2f}  max {v.max():7.2f}")
