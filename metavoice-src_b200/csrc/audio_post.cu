@@ -11,18 +11,10 @@
 #include <cuda_runtime.h>
 #include <math.h>
 
-#include "../../include/mvb200.h"
 #include "common.cuh"
+#include "host.cuh"
 
 using namespace mvb;
-namespace mvb { int set_error(int code, const char* fmt, ...); }
-
-#define ACK(expr)                                                                                    \
-  do {                                                                                               \
-    cudaError_t _e = (expr);                                                                         \
-    if (_e != cudaSuccess)                                                                           \
-      return mvb::set_error(MVB_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
-  } while (0)
 
 namespace {
 
@@ -120,11 +112,15 @@ static Biquad highpass(double sr, double f0, double Q) {                      //
   return Biquad{(float)(b0 / a0), (float)(b1 / a0), (float)(b2 / a0), (float)(a1 / a0), (float)(a2 / a0)};
 }
 
+// Workspace for n samples: K-weighted copy | ENERGY_BYTES of block energies + result scalars (at energy_offset(n))
+constexpr size_t ENERGY_BYTES = 65536;
+size_t energy_offset(size_t n) { WsBump ws; ws.take(n * 4); return ws.take(ENERGY_BYTES); }
+
 }  // namespace
 
 extern "C" size_t mvb_audio_post_workspace_bytes(int32_t max_samples) {
   if (max_samples < 1) return 0;
-  return ((size_t)max_samples * 4 + 255) / 256 * 256 + 65536;     // K-weighted copy | block energies + result scalars
+  return energy_offset(max_samples) + ENERGY_BYTES;
 }
 
 extern "C" int mvb_audio_post(const float* d_wav, int32_t n_samples, int32_t sample_rate, float loudness_headroom_db,
@@ -134,7 +130,7 @@ extern "C" int mvb_audio_post(const float* d_wav, int32_t n_samples, int32_t sam
   if (n_samples < 1 || sample_rate < 8000) return mvb::set_error(MVB_ERR_ARG, "audio_post: bad length / sample rate");
   cudaStream_t s = (cudaStream_t)stream;
   float* y = reinterpret_cast<float*>(d_workspace);
-  float* energy = reinterpret_cast<float*>(reinterpret_cast<char*>(d_workspace) + ((size_t)n_samples * 4 + 255) / 256 * 256);
+  float* energy = reinterpret_cast<float*>(reinterpret_cast<char*>(d_workspace) + energy_offset(n_samples));
   const int gate = (int)lround(0.4 * sample_rate), step = (int)lround(gate * 0.25);
   const int n_blocks = n_samples >= gate ? (n_samples - gate) / step + 1 : 0;
   if (n_blocks + 4 > 16000) return mvb::set_error(MVB_ERR_UNSUPPORTED, "audio_post: signal too long for the workspace");
@@ -142,13 +138,13 @@ extern "C" int mvb_audio_post(const float* d_wav, int32_t n_samples, int32_t sam
   const int chunks = (n_samples + KW_CHUNK - 1) / KW_CHUNK;
   k_kweight<<<(chunks + 127) / 128, 128, 0, s>>>(d_wav, n_samples, treble_shelf(sample_rate, 4.0, 1500.0, 1.0 / sqrt(2.0)),
                                                  highpass(sample_rate, 38.0, 0.5), y);
-  ACK(cudaGetLastError());
+  MVB_CK(cudaGetLastError());
   k_block_energy<<<n_blocks + 1, 256, 0, s>>>(y, d_wav, n_samples, gate, step, n_blocks, energy);
-  ACK(cudaGetLastError());
+  MVB_CK(cudaGetLastError());
   k_loudness_gain<<<1, 32, 0, s>>>(energy, n_blocks, n_samples, loudness_headroom_db, 2e-3f, res);
-  ACK(cudaGetLastError());
-  k_apply_pcm16<<<148 * 4, 256, 0, s>>>(d_wav, n_samples, res, loudness_compressor, d_pcm16, d_wav_out);
-  ACK(cudaGetLastError());
-  if (d_lkfs_gain) ACK(cudaMemcpyAsync(d_lkfs_gain, res, 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  MVB_CK(cudaGetLastError());
+  k_apply_pcm16<<<GRID_STRIDE_CTAS * 4, 256, 0, s>>>(d_wav, n_samples, res, loudness_compressor, d_pcm16, d_wav_out);
+  MVB_CK(cudaGetLastError());
+  if (d_lkfs_gain) MVB_CK(cudaMemcpyAsync(d_lkfs_gain, res, 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
   return MVB_OK;
 }

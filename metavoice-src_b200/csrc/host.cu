@@ -1,0 +1,38 @@
+// Definitions of the shared host helpers (host.cuh) and of the library-wide C ABI entry points.
+#include <cstdarg>
+#include <cstdio>
+#include <string>
+
+#include "host.cuh"
+
+static thread_local std::string g_err;
+
+extern "C" int mvb_abi_version(void) { return MVB_ABI_VERSION; }
+extern "C" const char* mvb_last_error(void) { return g_err.c_str(); }
+
+namespace mvb {
+
+int set_error(int code, const char* fmt, ...) {
+  char buf[1024];
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(buf, sizeof(buf), fmt, ap);
+  va_end(ap);
+  g_err = buf;
+  return code;
+}
+
+int check_offsets(const uint64_t* off, size_t n, size_t arena_bytes, const char* what) {
+  for (size_t i = 0; i < n; ++i)
+    if (off[i] % 16 || off[i] >= arena_bytes)
+      return set_error(MVB_ERR_ARG, "%s %llu not 16B-aligned or outside the arena", what, (unsigned long long)off[i]);
+  return MVB_OK;
+}
+
+int current_device(int* dev, int* n_sm) {
+  MVB_CK(cudaGetDevice(dev));
+  MVB_CK(cudaDeviceGetAttribute(n_sm, cudaDevAttrMultiProcessorCount, *dev));
+  return MVB_OK;
+}
+
+}  // namespace mvb

@@ -1,24 +1,9 @@
 // The weight-streaming tensor-core GEMM: tc_gemm, which the stage-1 and stage-2 engines call, and the standalone
 // operator of the C ABI, y[R, M] (+)= f(x)[R, K] . W[M, K]^T with W in bf16, that tests use to check it in isolation.
-#include <cstdio>
-#include <string>
-
-#include "../../include/mvb200.h"
+#include "host.cuh"
 #include "tc_gemm.cuh"
 
 using namespace mvb;
-
-extern "C" const char* mvb_last_error(void);
-namespace mvb { int set_error(int code, const char* fmt, ...); }
-
-#define LCK(expr)                                                                                   \
-  do {                                                                                              \
-    cudaError_t _e = (expr);                                                                        \
-    if (_e != cudaSuccess) {                                                                        \
-      rc = mvb::set_error(MVB_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
-      goto done;                                                                                    \
-    }                                                                                               \
-  } while (0)
 
 namespace mvb {
 
@@ -77,13 +62,10 @@ namespace {
 // standalone operator has no caller-provided workspace, unlike the engine handles).  W3 is the second weight of
 // G_SWIGLU.  Synchronises `s`.
 int run_gemm(TcGemm a, const void* d_W, const void* d_W3, cudaStream_t s) {
-  int rc = MVB_OK;
   a.Rpad = (a.R + 15) / 16 * 16;
   const int NB = a.Rpad * (a.split_lo ? 2 : 1);
   int dev = 0;
-  a.n_sm = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&a.n_sm, cudaDevAttrMultiProcessorCount, dev);
+  if (int e = current_device(&dev, &a.n_sm)) return e;
   const GemmPlan g = plan_gemm(a.M, a.K, NB, a.epi == G_SWIGLU, a.n_sm, a.ksplit);
   struct Cache { void* p = nullptr; size_t cap = 0; };
   static Cache cB[16], cS[16], cT[16];
@@ -97,25 +79,22 @@ int run_gemm(TcGemm a, const void* d_W, const void* d_W3, cudaStream_t s) {
   };
   if (dev < 0 || dev >= 16) return mvb::set_error(MVB_ERR_UNSUPPORTED, "mvb_linear: device index %d", dev);
   CUtensorMap tA, tA3, tB;
-  LCK(ensure(cB[dev], (size_t)NB * a.K * 2));
-  LCK(ensure(cS[dev], sizeof(float) * (g.scratch_floats ? g.scratch_floats : 1)));
-  LCK(ensure(cT[dev], sizeof(unsigned) * 256));
+  MVB_CK(ensure(cB[dev], (size_t)NB * a.K * 2));
+  MVB_CK(ensure(cS[dev], sizeof(float) * (g.scratch_floats ? g.scratch_floats : 1)));
+  MVB_CK(ensure(cT[dev], sizeof(unsigned) * 256));
   a.B = reinterpret_cast<__nv_bfloat16*>(cB[dev].p);
   a.scratch = reinterpret_cast<float*>(cS[dev].p);
   a.tickets = reinterpret_cast<unsigned*>(cT[dev].p);
-  LCK(cudaMemsetAsync(a.B, 0, (size_t)NB * a.K * 2, s));
-  LCK(cudaMemsetAsync(a.tickets, 0, sizeof(unsigned) * 256, s));
+  MVB_CK(cudaMemsetAsync(a.B, 0, (size_t)NB * a.K * 2, s));
+  MVB_CK(cudaMemsetAsync(a.tickets, 0, sizeof(unsigned) * 256, s));
   if (!make_tmap_bf16(&tA, d_W, (uint64_t)a.M, (uint64_t)a.K, 128) ||
       (a.epi == G_SWIGLU && !make_tmap_bf16(&tA3, d_W3, (uint64_t)a.M, (uint64_t)a.K, 128)) ||
-      !make_tmap_bf16(&tB, a.B, (uint64_t)NB, (uint64_t)a.K, (uint32_t)NB)) {
-    rc = mvb::set_error(MVB_ERR_CUDA, "cuTensorMapEncodeTiled failed");
-    goto done;
-  }
+      !make_tmap_bf16(&tB, a.B, (uint64_t)NB, (uint64_t)a.K, (uint32_t)NB))
+    return mvb::set_error(MVB_ERR_CUDA, "cuTensorMapEncodeTiled failed");
   a.tmW = &tA; a.tmW3 = &tA3; a.tmB = &tB;
-  LCK(tc_gemm(s, a));
-  LCK(cudaStreamSynchronize(s));
-done:
-  return rc;
+  MVB_CK(tc_gemm(s, a));
+  MVB_CK(cudaStreamSynchronize(s));
+  return MVB_OK;
 }
 
 }  // namespace

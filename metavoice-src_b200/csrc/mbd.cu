@@ -17,20 +17,12 @@
 
 #include <vector>
 
-#include "../../include/mvb200.h"
 #include "common.cuh"
+#include "host.cuh"
 #include "mbd_tc.cuh"
 #include "tc_gemm_host.cuh"
 
 using namespace mvb;
-namespace mvb { int set_error(int code, const char* fmt, ...); }
-
-#define MCK(expr)                                                                                    \
-  do {                                                                                               \
-    cudaError_t _e = (expr);                                                                         \
-    if (_e != cudaSuccess)                                                                           \
-      return mvb::set_error(MVB_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
-  } while (0)
 
 namespace {
 
@@ -379,6 +371,14 @@ __global__ void k_gn_relu_inplace(float* x, int C, int T, int cpg, const float* 
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------------------------
+// Workspace layout, fixed at create time together with the MVB_MBD_NO_TC / MVB_MBD_STREAMS switches it depends on
+struct MbdWs {
+  size_t cur, est, noise, wav, cond, gn, gn_part, stdv, low, skip[8], tmp[3], xt_hi, xt_lo;   // offsets inside one activation block
+  size_t blk, wpack, total;   // block size; the packed taps follow n_blk blocks (one block per concurrently running band model)
+  int n_blk;
+  bool tc;                    // convolutions with input widths >= 32 run on the tensor cores
+};
+
 struct mvb_mbd {
   mvb_mbd_config cfg;
   const char* arena;
@@ -391,7 +391,7 @@ struct mvb_mbd {
   char* base = nullptr;      // activation block of the band model whose kernels are being enqueued (host-side cursor)
   cudaStream_t st[8] = {};   // one stream per band model (n_blk > 1)
   cudaEvent_t ev_fork = nullptr, ev_join[8] = {};
-  int n_blk = 1;
+  MbdWs L{};
   std::vector<int> tc_of;    // [n tensors] -> index into tcw, or -1 (CUDA-core path)
   std::vector<TcW> tcw;
   const float* w(int i) const { return reinterpret_cast<const float*>(arena + off[i]); }
@@ -416,11 +416,6 @@ static int mbd_validate(const mvb_mbd_config* c) {
 }
 static int mbd_per_model(const mvb_mbd_config* c) { return c->depth * (3 + 8 * c->res_blocks + 1) + 2 + c->depth * (8 * c->res_blocks + 3) + 2; }
 
-struct MbdWs {
-  size_t cur, est, noise, wav, cond, gn, gn_part, stdv, low, skip[8], tmp[3], xt_hi, xt_lo;   // offsets inside one activation block
-  size_t blk, wpack, total;   // block size; the packed taps follow n_blk blocks (one block per concurrently running band model)
-  int n_blk;
-};
 // Convolutions of one band model in tensor order: fn(tensor index relative to the model, Cin, Cout, K, transposed)
 template <class F>
 static void mbd_for_each_conv(const mvb_mbd_config* c, F fn) {
@@ -447,22 +442,11 @@ static void mbd_for_each_conv(const mvb_mbd_config* c, F fn) {
 // Input widths >= 32 take the tensor-core path; the time-major copy and the packed taps are zero-padded to a multiple of 64 channels
 static bool mbd_tc_eligible(int cin) { return cin >= 32; }
 static int mbd_tc_cpad(int cin) { return (cin + 63) / 64 * 64; }
-static bool mbd_tc_enabled() {
-  const char* e = getenv("MVB_MBD_NO_TC");
-  return !(e && e[0] == '1');
-}
-// The band models are independent until their outputs are summed: each runs on its own stream with its own activation
-// block, so the many sub-wave kernels of one UNet (96-CTA convolutions, 4-CTA reductions) overlap with the other models'.
-static bool mbd_streams_enabled() {
-  const char* e = getenv("MVB_MBD_STREAMS");
-  return !(e && e[0] == '0');
-}
 static MbdWs mbd_layout(const mvb_mbd_config* c) {
   MbdWs L{};
-  size_t o = 0;
-  auto take = [&](size_t b) { size_t r = o; o = (o + b + 255) / 256 * 256; return r; };
+  WsBump ws;
   const size_t T = c->max_samples;
-  L.cur = take(T * 4); L.est = take(T * 4); L.noise = take(T * 4); L.wav = take(T * 4);
+  L.cur = ws.take(T * 4); L.est = ws.take(T * 4); L.noise = ws.take(T * 4); L.wav = ws.take(T * 4);
   int h = c->hidden;
   size_t tl = T, big = 0;
   std::vector<size_t> lev;
@@ -475,27 +459,32 @@ static MbdWs mbd_layout(const mvb_mbd_config* c) {
   // the transposed convolutions write (stride x longer, growth x narrower) tensors: size the temporaries for the widest case
   size_t tmpsz = big * (size_t)(c->stride > c->growth ? c->stride / (c->growth > 1 ? c->growth : 1) + 1 : 2);
   if (tmpsz < T + 64) tmpsz = T + 64;
-  L.cond = take((size_t)(h / (int)c->growth) * (c->max_samples / 320 + 8) * 4);
-  L.gn = take(4096);
-  L.gn_part = take((size_t)64 * GN_SPLIT * 16);
-  L.stdv = take(4096);
+  L.cond = ws.take((size_t)(h / (int)c->growth) * (c->max_samples / 320 + 8) * 4);
+  L.gn = ws.take(4096);
+  L.gn_part = ws.take((size_t)64 * GN_SPLIT * 16);
+  L.stdv = ws.take(4096);
   const int fb = (c->eq_bands > c->proc_bands ? c->eq_bands : c->proc_bands);
-  L.low = take((size_t)2 * fb * T * 4);
-  for (int i = 0; i < c->depth; ++i) L.skip[i] = take(lev[i] * 4);
-  for (int i = 0; i < 3; ++i) L.tmp[i] = take(tmpsz * 4);
+  L.low = ws.take((size_t)2 * fb * T * 4);
+  for (int i = 0; i < c->depth; ++i) L.skip[i] = ws.take(lev[i] * 4);
+  for (int i = 0; i < 3; ++i) L.tmp[i] = ws.take(tmpsz * 4);
   // time-major bf16 copies of one layer input (hi / lo) and the packed bf16 taps of every tensor-core convolution
   const size_t xt = (big * 2 + (size_t)h * (c->stride + 32)) * 2;   // (x2: widths below 64 are padded to 64 columns)
-  L.xt_hi = take(xt);
-  L.xt_lo = take(xt);
-  size_t wp = 0;
-  if (mbd_tc_enabled())
+  L.xt_hi = ws.take(xt);
+  L.xt_lo = ws.take(xt);
+  WsBump wp;   // the packed taps of one band model
+  const char* no_tc = getenv("MVB_MBD_NO_TC");
+  L.tc = !(no_tc && no_tc[0] == '1');
+  if (L.tc)
     mbd_for_each_conv(c, [&](int, int cin, int cout, int k, int) {
-      if (mbd_tc_eligible(cin)) wp += ((size_t)k * cout * mbd_tc_cpad(cin) * 2 + 255) / 256 * 256;
+      if (mbd_tc_eligible(cin)) wp.take((size_t)k * cout * mbd_tc_cpad(cin) * 2);
     });
-  L.blk = (o + 4095) / 4096 * 4096;
-  L.n_blk = (mbd_streams_enabled() && c->n_models > 1) ? c->n_models : 1;
+  L.blk = (ws.end + 4095) / 4096 * 4096;
+  // The band models are independent until their outputs are summed: each runs on its own stream with its own activation
+  // block, so the many sub-wave kernels of one UNet (96-CTA convolutions, 4-CTA reductions) overlap with the other models'.
+  const char* streams = getenv("MVB_MBD_STREAMS");
+  L.n_blk = (!(streams && streams[0] == '0') && c->n_models > 1) ? c->n_models : 1;
   L.wpack = L.blk * L.n_blk;
-  L.total = L.wpack + wp * c->n_models + 256;
+  L.total = L.wpack + wp.end * c->n_models + 256;
   return L;
 }
 
@@ -508,54 +497,51 @@ extern "C" int mvb_mbd_create(const mvb_mbd_config* cfg, const void* d_arena, si
                               mvb_mbd** out) {
   if (int e = mbd_validate(cfg)) return e;
   if (!d_arena || !offsets || !d_ws || !out) return mvb::set_error(MVB_ERR_ARG, "null pointer argument");
-  mvb_mbd* h = new mvb_mbd();
+  const int per_model = mbd_per_model(cfg), n_off = cfg->n_models * per_model + 3;
+  if (int e = check_offsets(offsets, n_off, arena_bytes, "mbd: tensor offset")) return e;
+  Building<mvb_mbd> hb(new mvb_mbd(), mvb_mbd_destroy);
+  mvb_mbd* h = hb.get();
   h->cfg = *cfg;
   h->arena = reinterpret_cast<const char*>(d_arena);
-  h->per_model = mbd_per_model(cfg);
-  const int n_off = cfg->n_models * h->per_model + 3;
+  h->per_model = per_model;
   h->off.assign(offsets, offsets + n_off);
-  for (uint64_t o : h->off)
-    if (o % 16 || o >= arena_bytes) { delete h; return mvb::set_error(MVB_ERR_ARG, "mbd: bad tensor offset"); }
   h->ws = reinterpret_cast<char*>(d_ws);
   int c = cfg->hidden;
   for (int i = 0; i < cfg->depth; ++i) { h->ch.push_back(c); c = (int)(c * cfg->growth); }
-  // tensor-core path: repack the taps of every eligible convolution to bf16 [tap][Cout][Cin] and build their A maps
-  h->n_blk = mbd_layout(cfg).n_blk;
+  h->L = mbd_layout(cfg);
+  const MbdWs& L = h->L;
   h->base = h->ws;
-  if (h->n_blk > 1) {
+  if (L.n_blk > 1) {
     bool ok_s = cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming) == cudaSuccess;
-    for (int i = 0; i < h->n_blk && ok_s; ++i)
+    for (int i = 0; i < L.n_blk && ok_s; ++i)
       ok_s = cudaStreamCreateWithFlags(&h->st[i], cudaStreamNonBlocking) == cudaSuccess &&
              cudaEventCreateWithFlags(&h->ev_join[i], cudaEventDisableTiming) == cudaSuccess;
-    if (!ok_s) { mvb_mbd_destroy(h); return mvb::set_error(MVB_ERR_CUDA, "mbd: stream / event creation failed"); }
+    if (!ok_s) return mvb::set_error(MVB_ERR_CUDA, "mbd: stream / event creation failed");
   }
+  // tensor-core path: repack the taps of every eligible convolution to bf16 [tap][Cout][Cin] and build their A maps
   h->tc_of.assign(n_off, -1);
-  if (mbd_tc_enabled() && encode_tiled_fn()) {
-    const MbdWs L = mbd_layout(cfg);
-    size_t wo = 0;
+  if (L.tc && encode_tiled_fn()) {
+    WsBump wo;
     bool ok = true;
     for (int m = 0; m < cfg->n_models && ok; ++m)
       mbd_for_each_conv(cfg, [&](int ti, int cin, int cout, int k, int tr) {
         if (!ok || !mbd_tc_eligible(cin)) return;
         const int gi = m * h->per_model + ti;
-        __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(h->ws + L.wpack + wo);
         const int cp = mbd_tc_cpad(cin);
-        k_mbd_pack_w<<<148 * 4, 256>>>(h->w(gi), cout, cin, cp, k, tr, dst);
+        __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(h->ws + L.wpack + wo.take((size_t)k * cout * cp * 2));
+        k_mbd_pack_w<<<GRID_STRIDE_CTAS * 4, 256>>>(h->w(gi), cout, cin, cp, k, tr, dst);
         mvb_mbd::TcW w{};
         w.Cin = cin; w.Cout = cout; w.K = k;
         ok = ok && make_tmap_bf16_3d(&w.tmA, dst, (uint64_t)cp, (uint64_t)cout, (uint64_t)k, (uint64_t)cout * cp * 2, 128);
         h->tc_of[gi] = (int)h->tcw.size();
         h->tcw.push_back(w);
-        wo += ((size_t)k * cout * cp * 2 + 255) / 256 * 256;
       });
     cudaError_t e = cudaDeviceSynchronize();
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_mbd_tc_conv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM);
-    if (!ok || e != cudaSuccess) {
-      delete h;
+    if (!ok || e != cudaSuccess)
       return mvb::set_error(MVB_ERR_CUDA, "mbd: tensor-core weight repack failed (%s)", ok ? cudaGetErrorString(e) : "tensor map");
-    }
   }
-  *out = h;
+  *out = hb.release();
   return MVB_OK;
 }
 extern "C" int mvb_mbd_destroy(mvb_mbd* h) {
@@ -576,15 +562,15 @@ static int launch_conv(cudaStream_t s, const ConvP& p, int K, int stride) {
   else if (K == 8 && stride == 4) k_mbd_conv<8, 4, 1><<<dim3((p.Tout + 63) / 64, (p.Cout + 31) / 32), 256, 0, s>>>(p);
   else if (K == 4 && stride == 2) k_mbd_conv<4, 2, 2><<<dim3((p.Tout + 127) / 128, (p.Cout + 31) / 32), 256, 0, s>>>(p);
   else return mvb::set_error(MVB_ERR_UNSUPPORTED, "mbd: conv (k=%d, s=%d)", K, stride);
-  MCK(cudaGetLastError());
+  MVB_CK(cudaGetLastError());
   return MVB_OK;
 }
 static int gn_stats(mvb_mbd* h, cudaStream_t s, const float* x, int C, int T, int groups, float* stats) {
-  double* part = reinterpret_cast<double*>(h->base + mbd_layout(&h->cfg).gn_part);
+  double* part = reinterpret_cast<double*>(h->base + h->L.gn_part);
   const size_t n = (size_t)(C / groups) * T;
   k_gn_partial<<<dim3(groups, GN_SPLIT), 256, 0, s>>>(x, n, part);
   k_gn_final<<<groups, 32, 0, s>>>(part, groups, (double)n, 1e-5f, stats);
-  MCK(cudaGetLastError());
+  MVB_CK(cudaGetLastError());
   return MVB_OK;
 }
 
@@ -597,7 +583,7 @@ static int conv_tc(cudaStream_t s, const ConvP& p, const CUtensorMap& tmA, __nv_
   const int Cp = mbd_tc_cpad(p.Cin);
   k_mbd_prep_t<<<dim3((Tpad + 31) / 32, Cp / 64), 256, 0, s>>>(p.x, p.Cin, Cp, p.Tin, Tpad, p.gn_stats, p.gn_w, p.gn_b,
                                                               p.gn_stats ? p.Cin / p.groups : 1, hi, lo);
-  MCK(cudaGetLastError());
+  MVB_CK(cudaGetLastError());
   const uint64_t rows = kind == 1 ? Tpad / stride : p.Tin, cols = kind == 1 ? (uint64_t)stride * Cp : Cp;
   CUtensorMap tBhi, tBlo;
   if (!make_tmap_bf16(&tBhi, hi, rows, cols, 128) || !make_tmap_bf16(&tBlo, lo, rows, cols, 128))
@@ -627,11 +613,11 @@ static int conv_tc(cudaStream_t s, const ConvP& p, const CUtensorMap& tmA, __nv_
   }
   const int n_cot = (p.Cout + 127) / 128;
   k_mbd_tc_conv<<<dim3(t.n_ph * n_cot, (q.Ncols + 127) / 128), TC_THREADS, TC_SMEM, s>>>(tmA, tBhi, tBlo, q);
-  MCK(cudaGetLastError());
+  MVB_CK(cudaGetLastError());
   return MVB_OK;
 }
 static int launch_conv_tc(mvb_mbd* h, cudaStream_t s, const ConvP& p, int widx, int kind, int K, int stride) {
-  const MbdWs L = mbd_layout(&h->cfg);
+  const MbdWs& L = h->L;
   return conv_tc(s, p, h->tcw[h->tc_of[widx]].tmA, reinterpret_cast<__nv_bfloat16*>(h->base + L.xt_hi),
                  reinterpret_cast<__nv_bfloat16*>(h->base + L.xt_lo), kind, K, stride);
 }
@@ -653,7 +639,7 @@ static int res_block(mvb_mbd* h, cudaStream_t s, int base, int C, int T, int dil
 // DiffusionUnet.forward (unet.py) for band model m: est <- model(cur, step, cond)
 static int unet_forward(mvb_mbd* h, cudaStream_t s, int m, int step, const float* cur, int T, const float* d_cond, int Tf, float* est) {
   const mvb_mbd_config& c = h->cfg;
-  const MbdWs L = mbd_layout(&c);
+  const MbdWs& L = h->L;
   float* stats = reinterpret_cast<float*>(h->base + L.gn);
   float* tmp[3] = {reinterpret_cast<float*>(h->base + L.tmp[0]), reinterpret_cast<float*>(h->base + L.tmp[1]), reinterpret_cast<float*>(h->base + L.tmp[2])};
   const int pad_k = (c.kernel - c.stride) / 2, G = c.norm_groups;
@@ -669,8 +655,8 @@ static int unet_forward(mvb_mbd* h, cudaStream_t s, int m, int step, const float
     if (int e = h->tc_of[ti] >= 0 ? launch_conv_tc(h, s, p, ti, 1, c.kernel, c.stride) : launch_conv(s, p, c.kernel, c.stride)) return e;
     // norm -> relu -> res_blocks: the first ResBlock input is relu(GN(conv)); materialise it (it is also the residual)
     if (int e = gn_stats(h, s, tmp[0], C, To, G, stats + 128)) return e;
-    k_gn_relu_inplace<<<148 * 4, 256, 0, s>>>(tmp[0], C, To, C / G, stats + 128, h->w(ti + 1), h->w(ti + 2));
-    MCK(cudaGetLastError());
+    k_gn_relu_inplace<<<GRID_STRIDE_CTAS * 4, 256, 0, s>>>(tmp[0], C, To, C / G, stats + 128, h->w(ti + 1), h->w(ti + 2));
+    MVB_CK(cudaGetLastError());
     ti += 3;
     float* a = tmp[0];
     float* b = tmp[1];
@@ -696,9 +682,9 @@ static int unet_forward(mvb_mbd* h, cudaStream_t s, int m, int step, const float
     p.x = d_cond; p.Cin = c.codec_dim; p.Tin = Tf; p.w = h->w(ti); p.bias = h->w(ti + 1); p.y = cemb; p.Cout = Cb; p.Tout = Tf; p.dil = 1; p.pad = 0;
     if (int e = launch_conv(s, p, 1, 1)) return e;
     if (Tf > 2 * Tl) return mvb::set_error(MVB_ERR_ARG, "mbd: condition is downsampled by >= 2 (%d vs %d)", Tf, Tl);
-    MCK(cudaMemcpyAsync(z, x, sizeof(float) * (size_t)Cb * Tl, cudaMemcpyDeviceToDevice, s));
-    k_add_interp<<<148 * 2, 256, 0, s>>>(z, Tl, cemb, Tf, Cb);
-    MCK(cudaGetLastError());
+    MVB_CK(cudaMemcpyAsync(z, x, sizeof(float) * (size_t)Cb * Tl, cudaMemcpyDeviceToDevice, s));
+    k_add_interp<<<GRID_STRIDE_CTAS * 2, 256, 0, s>>>(z, Tl, cemb, Tf, Cb);
+    MVB_CK(cudaGetLastError());
     ti += 2;
   }
   // decoders (deepest first): z = crop(z) + skip; res_blocks; norm; relu; convtr.  Three temporaries rotate: z lives in
@@ -710,8 +696,8 @@ static int unet_forward(mvb_mbd* h, cudaStream_t s, int m, int step, const float
     float* a = tmp[(zi + 1) % 3];
     float* b = tmp[zi];                   // free once the skip sum has been formed
     float* scratch = tmp[(zi + 2) % 3];
-    k_add_crop<<<148 * 2, 256, 0, s>>>(z, Tz, skip, Tsk, C, a);
-    MCK(cudaGetLastError());
+    k_add_crop<<<GRID_STRIDE_CTAS * 2, 256, 0, s>>>(z, Tz, skip, Tsk, C, a);
+    MVB_CK(cudaGetLastError());
     for (int j = 0; j < c.res_blocks; ++j) {
       if (int e = res_block(h, s, ti + 8 * j, C, Tsk, 1 << j, a, scratch, b, stats, nullptr)) return e;
       float* t = a; a = b; b = t;
@@ -727,22 +713,22 @@ static int unet_forward(mvb_mbd* h, cudaStream_t s, int m, int step, const float
       if (int e = launch_conv_tc(h, s, p, ti + 2, 2, c.kernel, c.stride)) return e;
     } else if (c.stride == 4) k_mbd_convtr<4><<<dim3((To + 255) / 256, (Cout + 31) / 32), 256, 0, s>>>(p);
     else k_mbd_convtr<2><<<dim3((To + 255) / 256, (Cout + 31) / 32), 256, 0, s>>>(p);
-    MCK(cudaGetLastError());
+    MVB_CK(cudaGetLastError());
     ti += 3;
     z = scratch; Tz = To; zi = (zi + 2) % 3;
   }
   // crop to the input length
-  MCK(cudaMemcpyAsync(est, z, sizeof(float) * (size_t)T, cudaMemcpyDeviceToDevice, s));
+  MVB_CK(cudaMemcpyAsync(est, z, sizeof(float) * (size_t)T, cudaMemcpyDeviceToDevice, s));
   return MVB_OK;
 }
 
 static int split_lows(mvb_mbd* h, cudaStream_t s, const float* x, int T, int n_bands, const float* bank, int L, float* low) {
   const size_t smem = (size_t)(FIR_TT + 3 * L) * 4;
   static PerDeviceOnce attr;
-  if (attr.pending()) { MCK(cudaFuncSetAttribute(k_fir_bank, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024)); attr.mark(); }
+  if (attr.pending()) { MVB_CK(cudaFuncSetAttribute(k_fir_bank, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024)); attr.mark(); }
   if (smem > 64 * 1024) return mvb::set_error(MVB_ERR_UNSUPPORTED, "mbd: filter length %d", L);
   k_fir_bank<<<dim3((T + FIR_TT - 1) / FIR_TT, (n_bands - 1 + 1) / 2), 256, smem, s>>>(x, T, bank, L, n_bands - 1, low);
-  MCK(cudaGetLastError());
+  MVB_CK(cudaGetLastError());
   (void)h;
   return MVB_OK;
 }
@@ -754,9 +740,9 @@ extern "C" int mvb_mbd_tokens_to_wav(mvb_mbd* h, const float* d_cond, int32_t n_
   if (n_samples < 16 * c.stride || n_samples > c.max_samples) return mvb::set_error(MVB_ERR_ARG, "mbd: n_samples %d out of range", n_samples);
   if (n_frames < 1) return mvb::set_error(MVB_ERR_ARG, "mbd: n_frames");
   cudaStream_t s = (cudaStream_t)stream;
-  const MbdWs L = mbd_layout(&c);
+  const MbdWs& L = h->L;
   const int T = n_samples;
-  const bool multi = h->n_blk > 1;
+  const bool multi = L.n_blk > 1;
   h->base = h->ws;
   float* wav = reinterpret_cast<float*>(h->ws + L.wav);      // block 0: the sum over the band models, then the re-EQ input
   float* low = reinterpret_cast<float*>(h->ws + L.low);
@@ -764,15 +750,15 @@ extern "C" int mvb_mbd_tokens_to_wav(mvb_mbd* h, const float* d_cond, int32_t n_
   const int g0 = c.n_models * h->per_model;          // globals: processor bank, eq bank, schedule table
   const float* sched = h->w(g0 + 2);                 // [n_calls][4] = a, b, sigma, step
   std::vector<float> hs((size_t)c.n_calls * 4);
-  MCK(cudaMemcpyAsync(hs.data(), sched, sizeof(float) * hs.size(), cudaMemcpyDeviceToHost, s));
-  MCK(cudaStreamSynchronize(s));
-  if (!multi) MCK(cudaMemsetAsync(wav, 0, sizeof(float) * T, s));
-  if (multi) MCK(cudaEventRecord(h->ev_fork, s));
+  MVB_CK(cudaMemcpyAsync(hs.data(), sched, sizeof(float) * hs.size(), cudaMemcpyDeviceToHost, s));
+  MVB_CK(cudaStreamSynchronize(s));
+  if (!multi) MVB_CK(cudaMemsetAsync(wav, 0, sizeof(float) * T, s));
+  if (multi) MVB_CK(cudaEventRecord(h->ev_fork, s));
   int rc = MVB_OK;
   for (int m = 0; m < c.n_models && rc == MVB_OK; ++m) {
     cudaStream_t sm = multi ? h->st[m] : s;
     h->base = h->ws + (multi ? (size_t)m * L.blk : 0);
-    if (multi) MCK(cudaStreamWaitEvent(sm, h->ev_fork, 0));
+    if (multi) MVB_CK(cudaStreamWaitEvent(sm, h->ev_fork, 0));
     float* cur = reinterpret_cast<float*>(h->base + L.cur);
     float* est = reinterpret_cast<float*>(h->base + L.est);
     float* nz = reinterpret_cast<float*>(h->base + L.noise);
@@ -780,9 +766,9 @@ extern "C" int mvb_mbd_tokens_to_wav(mvb_mbd* h, const float* d_cond, int32_t n_
     float* low_m = reinterpret_cast<float*>(h->base + L.low);
     // initial = randn * noise_scale
     const float* n0 = d_noise ? d_noise + ((size_t)m * c.n_calls) * T : nz;
-    if (!d_noise) { k_randn<<<148, 256, 0, sm>>>(nz, T, seed, (unsigned)(m * 1024)); MCK(cudaGetLastError()); }
-    k_scale_copy<<<148, 256, 0, sm>>>(n0, c.noise_scale, cur, T);
-    MCK(cudaGetLastError());
+    if (!d_noise) { k_randn<<<GRID_STRIDE_CTAS, 256, 0, sm>>>(nz, T, seed, (unsigned)(m * 1024)); MVB_CK(cudaGetLastError()); }
+    k_scale_copy<<<GRID_STRIDE_CTAS, 256, 0, sm>>>(n0, c.noise_scale, cur, T);
+    MVB_CK(cudaGetLastError());
     for (int i = 0; i < c.n_calls; ++i) {
       const float a = hs[4 * i], b = hs[4 * i + 1], sigma = hs[4 * i + 2];
       const int step = (int)hs[4 * i + 3];
@@ -790,27 +776,27 @@ extern "C" int mvb_mbd_tokens_to_wav(mvb_mbd* h, const float* d_cond, int32_t n_
       const float* ni = nullptr;
       if (sigma > 0.f) {
         if (d_noise) ni = d_noise + ((size_t)m * c.n_calls + i + 1) * T;      // row i + 1: the draw added after call i
-        else { k_randn<<<148, 256, 0, sm>>>(nz, T, seed, (unsigned)(m * 1024 + i + 1)); MCK(cudaGetLastError()); ni = nz; }
+        else { k_randn<<<GRID_STRIDE_CTAS, 256, 0, sm>>>(nz, T, seed, (unsigned)(m * 1024 + i + 1)); MVB_CK(cudaGetLastError()); ni = nz; }
       }
-      k_sched_step<<<148 * 2, 256, 0, sm>>>(cur, est, ni, a, b, sigma, c.noise_scale, c.clip, T);
-      MCK(cudaGetLastError());
+      k_sched_step<<<GRID_STRIDE_CTAS * 2, 256, 0, sm>>>(cur, est, ni, a, b, sigma, c.noise_scale, c.clip, T);
+      MVB_CK(cudaGetLastError());
     }
     if (rc != MVB_OK) break;
     // MultiBandProcessor.return_sample: bands * (std / target_std) ** power_std + mean, summed; the band models' outputs are
     // added up in model order (one stream: accumulated in place; several streams: per-model buffers summed after the join)
     const int pb = m * h->per_model + h->per_model - 2;
     if ((rc = split_lows(h, sm, cur, T, c.proc_bands, h->w(g0), c.proc_taps, low_m)) != MVB_OK) break;
-    k_band_mix<<<148 * 2, 256, 0, sm>>>(low_m, cur, T, c.proc_bands, h->w(pb), nullptr, h->w(pb + 1), wav_m, multi ? 0 : 1);
-    MCK(cudaGetLastError());
-    if (multi) MCK(cudaEventRecord(h->ev_join[m], sm));
+    k_band_mix<<<GRID_STRIDE_CTAS * 2, 256, 0, sm>>>(low_m, cur, T, c.proc_bands, h->w(pb), nullptr, h->w(pb + 1), wav_m, multi ? 0 : 1);
+    MVB_CK(cudaGetLastError());
+    if (multi) MVB_CK(cudaEventRecord(h->ev_join[m], sm));
   }
   h->base = h->ws;
   if (multi) {
     // always re-join the caller's stream, also on an error path, so no work is left running behind the caller's back
-    for (int m = 0; m < c.n_models; ++m) MCK(cudaStreamWaitEvent(s, h->ev_join[m], 0));   // (an event never recorded in this call is complete)
+    for (int m = 0; m < c.n_models; ++m) MVB_CK(cudaStreamWaitEvent(s, h->ev_join[m], 0));   // (an event never recorded in this call is complete)
     if (rc == MVB_OK) {
-      k_sum_blocks<<<148 * 2, 256, 0, s>>>(wav, L.blk / 4, c.n_models, T);
-      MCK(cudaGetLastError());
+      k_sum_blocks<<<GRID_STRIDE_CTAS * 2, 256, 0, s>>>(wav, L.blk / 4, c.n_models, T);
+      MVB_CK(cudaGetLastError());
     }
   }
   if (rc != MVB_OK) return rc;
@@ -820,11 +806,11 @@ extern "C" int mvb_mbd_tokens_to_wav(mvb_mbd* h, const float* d_cond, int32_t n_
   if (int e = split_lows(h, s, wav, T, c.eq_bands, h->w(g0 + 1), c.eq_taps, low_w)) return e;
   if (int e = split_lows(h, s, d_wav_encodec, T, c.eq_bands, h->w(g0 + 1), c.eq_taps, low_r)) return e;
   k_band_std<<<c.eq_bands, 256, 0, s>>>(low_w, wav, T, c.eq_bands, stdv);
-  MCK(cudaGetLastError());
+  MVB_CK(cudaGetLastError());
   k_band_std<<<c.eq_bands, 256, 0, s>>>(low_r, d_wav_encodec, T, c.eq_bands, stdv + 64);
-  MCK(cudaGetLastError());
-  k_band_mix<<<148 * 2, 256, 0, s>>>(low_w, wav, T, c.eq_bands, stdv + 64, stdv, nullptr, d_wav_out, 0);
-  MCK(cudaGetLastError());
+  MVB_CK(cudaGetLastError());
+  k_band_mix<<<GRID_STRIDE_CTAS * 2, 256, 0, s>>>(low_w, wav, T, c.eq_bands, stdv + 64, stdv, nullptr, d_wav_out, 0);
+  MVB_CK(cudaGetLastError());
   return MVB_OK;
 }
 
@@ -855,8 +841,8 @@ extern "C" int mvb_mbd_conv_test(int32_t kind, const float* d_x, int32_t Cin, in
     } else if (stride == 4) k_mbd_convtr<4><<<dim3((p.Tout + 255) / 256, (Cout + 31) / 32), 256, 0, s>>>(p);
     else if (stride == 2) k_mbd_convtr<2><<<dim3((p.Tout + 255) / 256, (Cout + 31) / 32), 256, 0, s>>>(p);
     else return mvb::set_error(MVB_ERR_UNSUPPORTED, "mvb_mbd_conv_test: transposed stride %d", stride);
-    MCK(cudaGetLastError());
-    MCK(cudaStreamSynchronize(s));
+    MVB_CK(cudaGetLastError());
+    MVB_CK(cudaStreamSynchronize(s));
     return MVB_OK;
   }
   if ((kind != 2 && K > 8) || (kind == 2 && stride > 4)) return mvb::set_error(MVB_ERR_UNSUPPORTED, "mvb_mbd_conv_test: too many taps");
@@ -864,16 +850,18 @@ extern "C" int mvb_mbd_conv_test(int32_t kind, const float* d_x, int32_t Cin, in
   const int Cp = mbd_tc_cpad(Cin);
   const int Tpad = kind == 1 ? (Tin + stride - 1) / stride * stride : Tin;
   const size_t wbytes = (size_t)K * Cout * Cp * 2, xbytes = (size_t)Tpad * Cp * 2;
-  void* buf = nullptr;
-  MCK(cudaMalloc(&buf, wbytes + 2 * ((xbytes + 255) / 256 * 256) + 256));
-  __nv_bfloat16* wp = reinterpret_cast<__nv_bfloat16*>(buf);
-  __nv_bfloat16* hi = reinterpret_cast<__nv_bfloat16*>(reinterpret_cast<char*>(buf) + (wbytes + 255) / 256 * 256);
-  __nv_bfloat16* lo = reinterpret_cast<__nv_bfloat16*>(reinterpret_cast<char*>(hi) + (xbytes + 255) / 256 * 256);
+  WsBump ws;
+  const size_t o_wp = ws.take(wbytes), o_hi = ws.take(xbytes), o_lo = ws.take(xbytes);
+  char* buf = nullptr;
+  MVB_CK(cudaMalloc(&buf, ws.end + 256));
+  __nv_bfloat16* wp = reinterpret_cast<__nv_bfloat16*>(buf + o_wp);
+  __nv_bfloat16* hi = reinterpret_cast<__nv_bfloat16*>(buf + o_hi);
+  __nv_bfloat16* lo = reinterpret_cast<__nv_bfloat16*>(buf + o_lo);
   int rc = MVB_OK;
   cudaError_t e = cudaFuncSetAttribute(k_mbd_tc_conv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM);
   CUtensorMap tmA;
   if (e == cudaSuccess) {
-    k_mbd_pack_w<<<148 * 4, 256, 0, s>>>(d_w, Cout, Cin, Cp, K, kind == 2 ? 1 : 0, wp);
+    k_mbd_pack_w<<<GRID_STRIDE_CTAS * 4, 256, 0, s>>>(d_w, Cout, Cin, Cp, K, kind == 2 ? 1 : 0, wp);
     e = cudaGetLastError();
   }
   if (e != cudaSuccess) rc = mvb::set_error(MVB_ERR_CUDA, "mvb_mbd_conv_test: %s", cudaGetErrorString(e));

@@ -12,18 +12,10 @@
 
 #include <vector>
 
-#include "../../include/mvb200.h"
 #include "common.cuh"
+#include "host.cuh"
 
 using namespace mvb;
-namespace mvb { int set_error(int code, const char* fmt, ...); }
-
-#define SCK(expr)                                                                                    \
-  do {                                                                                               \
-    cudaError_t _e = (expr);                                                                         \
-    if (_e != cudaSuccess)                                                                           \
-      return mvb::set_error(MVB_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
-  } while (0)
 
 namespace {
 
@@ -154,17 +146,25 @@ __global__ void __launch_bounds__(SPK_THREADS) k_spk_mean(const float* __restric
 
 }  // namespace
 
+// Workspace: mel spectrogram of the longest input | <= 1024 partial starts | <= 1024 partial embeddings
+struct SpkLayout { size_t starts, partials, total; };
+static SpkLayout spk_layout(const mvb_spk_config* c) {
+  WsBump ws;
+  ws.take((size_t)(1 + c->max_samples / c->hop) * c->n_mels * 4);   // the mel spectrogram starts the workspace
+  const size_t starts = ws.take(4096), partials = ws.take((size_t)1024 * 256 * 4);
+  return {starts, partials, ws.end};
+}
+
 struct mvb_spk {
   mvb_spk_config cfg;
   const char* arena;
   std::vector<uint64_t> off;
   char* ws;
+  SpkLayout L;
   const float* w(int i) const { return reinterpret_cast<const float*>(arena + off[i]); }
-  size_t mel_bytes() const { return ((size_t)max_frames() * cfg.n_mels * 4 + 255) / 256 * 256; }
-  int max_frames() const { return 1 + cfg.max_samples / cfg.hop; }
   float* mel() const { return reinterpret_cast<float*>(ws); }
-  int* starts() const { return reinterpret_cast<int*>(ws + mel_bytes()); }
-  float* partials() const { return reinterpret_cast<float*>(ws + mel_bytes() + 4096); }
+  int* starts() const { return reinterpret_cast<int*>(ws + L.starts); }
+  float* partials() const { return reinterpret_cast<float*>(ws + L.partials); }
 };
 
 static int spk_validate(const mvb_spk_config* c) {
@@ -178,23 +178,22 @@ static int spk_validate(const mvb_spk_config* c) {
 
 extern "C" size_t mvb_spk_workspace_bytes(const mvb_spk_config* c) {
   if (spk_validate(c)) return 0;
-  mvb_spk t{};
-  t.cfg = *c;
-  return t.mel_bytes() + 4096 + (size_t)1024 * 256 * 4;     // mel | <= 1024 partial starts | <= 1024 partial embeddings
+  return spk_layout(c).total;
 }
 
 extern "C" int mvb_spk_create(const mvb_spk_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
                               void* d_ws, mvb_spk** out) {
   if (int e = spk_validate(cfg)) return e;
   if (!d_arena || !offsets || !d_ws || !out) return mvb::set_error(MVB_ERR_ARG, "null pointer argument");
-  mvb_spk* h = new mvb_spk();
+  if (int e = check_offsets(offsets, MVB_SPK_TENSORS, arena_bytes, "speaker encoder: tensor offset")) return e;
+  Building<mvb_spk> hb(new mvb_spk(), mvb_spk_destroy);
+  mvb_spk* h = hb.get();
   h->cfg = *cfg;
   h->arena = reinterpret_cast<const char*>(d_arena);
   h->off.assign(offsets, offsets + MVB_SPK_TENSORS);
-  for (uint64_t o : h->off)
-    if (o % 16 || o >= arena_bytes) { delete h; return mvb::set_error(MVB_ERR_ARG, "speaker encoder: bad tensor offset"); }
   h->ws = reinterpret_cast<char*>(d_ws);
-  *out = h;
+  h->L = spk_layout(cfg);
+  *out = hb.release();
   return MVB_OK;
 }
 
@@ -209,7 +208,7 @@ static int spk_mel(mvb_spk* h, const float* d_wav, int n_samples, float* d_mel, 
   const size_t smem = (size_t)(c.n_fft + c.n_fft / 2 + 1) * 4;
   // tensors: 3 x {w_ih, w_hh, b}, linear w, linear b, mel filterbank, window, cos table, sin table
   k_spk_mel<<<n_frames, SPK_THREADS, smem, s>>>(d_wav, n_samples, c.n_fft, c.hop, h->w(12), h->w(13), h->w(14), h->w(11), c.n_mels, d_mel);
-  SCK(cudaGetLastError());
+  MVB_CK(cudaGetLastError());
   return MVB_OK;
 }
 
@@ -228,15 +227,15 @@ extern "C" int mvb_spk_embed(mvb_spk* h, const float* d_wav, int32_t n_samples, 
   const mvb_spk_config& c = h->cfg;
   const int n_frames = 1 + n_samples / c.hop;
   if (int e = spk_mel(h, d_wav, n_samples, h->mel(), s)) return e;
-  SCK(cudaMemcpyAsync(h->starts(), slice_starts, sizeof(int) * n_partials, cudaMemcpyHostToDevice, s));
+  MVB_CK(cudaMemcpyAsync(h->starts(), slice_starts, sizeof(int) * n_partials, cudaMemcpyHostToDevice, s));
   SpkW W;
   for (int l = 0; l < 3; ++l) { W.w_ih[l] = h->w(3 * l); W.w_hh[l] = h->w(3 * l + 1); W.b[l] = h->w(3 * l + 2); }
   W.lw = h->w(9); W.lb = h->w(10);
   k_spk_lstm<<<n_partials, SPK_THREADS, 0, s>>>(h->mel(), h->starts(), n_frames, c.partial_frames, c.n_mels, W, h->partials());
-  SCK(cudaGetLastError());
+  MVB_CK(cudaGetLastError());
   k_spk_mean<<<1, SPK_THREADS, 0, s>>>(h->partials(), n_partials, d_embed);
-  SCK(cudaGetLastError());
+  MVB_CK(cudaGetLastError());
   if (d_partials_out)
-    SCK(cudaMemcpyAsync(d_partials_out, h->partials(), sizeof(float) * (size_t)n_partials * 256, cudaMemcpyDeviceToDevice, s));
+    MVB_CK(cudaMemcpyAsync(d_partials_out, h->partials(), sizeof(float) * (size_t)n_partials * 256, cudaMemcpyDeviceToDevice, s));
   return MVB_OK;
 }

@@ -2,53 +2,18 @@
 // No torch, no CPU fallback: every entry point either runs the CUDA path or fails loudly.
 #include <cuda_runtime.h>
 
-#include <cstdarg>
-#include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <map>
-#include <string>
 #include <vector>
 
-#include "../../include/mvb200.h"
+#include "host.cuh"
 #include "stage1_kernels.cuh"
 #include "tc_gemm_host.cuh"
 #include "decode_persistent.cuh"
 #include "gemv_w4.cuh"
 
 using namespace mvb;
-
-static thread_local std::string g_err;
-
-static int fail(int code, const char* fmt, ...) {
-  char buf[1024];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  g_err = buf;
-  return code;
-}
-namespace mvb {
-int set_error(int code, const char* fmt, ...) {  // shared with the other translation units
-  char buf[1024];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  g_err = buf;
-  return code;
-}
-}  // namespace mvb
-
-#define CK(expr)                                                                                   \
-  do {                                                                                             \
-    cudaError_t _e = (expr);                                                                       \
-    if (_e != cudaSuccess)                                                                         \
-      return fail(MVB_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
-  } while (0)
-
-static inline size_t align_up(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
 
 struct WsLayout {
   size_t x, qkv, att, ffn, logits, spk, part_o, part_ml;
@@ -59,75 +24,84 @@ struct WsLayout {
   // path C (persistent decode kernel)
   size_t c_x, c_qkv, c_gu, c_part_o, c_part_ml, c_bar, c_trace, c_stat, c_samp_part, c_samp_best;
   size_t total;
+  // an int4 engine's workspace continues with the dequantised-layer scratch
+  size_t w4_scratch, total_int4;
 };
 
 constexpr int RB_MAX = 128;        // rows per tensor-core pass: 64-token prefill chunk x 2 CFG rows, or 64 utterances
 constexpr int PREFILL_CHUNK = 64;
 constexpr int GEN_BURST = 32;       // decode steps between two host polls of the done flags in mvb_s1_generate
 
+// elements of one layer's dequantised weights: wqkv, wo, w1, w3, w2
+static size_t w4_layer_elems(const mvb_s1_config& c) {
+  const size_t D = c.dim, F = c.intermediate;
+  return 4 * D * D + 3 * D * F;
+}
+
 static WsLayout make_layout(const mvb_s1_config& c) {
   WsLayout L;
   const size_t U = c.max_utts, R = 2 * U, D = c.dim, F = c.intermediate, V = c.vocab, H = c.n_head;
-  size_t o = 0;
-  auto take = [&](size_t bytes) { size_t r = o; o = align_up(o + bytes); return r; };
-  L.x = take(R * D * 4);
-  L.qkv = take(R * 3 * D * 4);
-  L.att = take(R * D * 4);
-  L.ffn = take(R * F * 4);
-  L.logits = take(R * V * 4);
-  L.spk = take(U * D * 4);
-  L.part_o = take(R * H * ATT_SPLITS * 128 * 4);
-  L.part_ml = take(R * H * ATT_SPLITS * 2 * 4);
-  L.slot_map = take(U * 4);
-  L.pos = take(U * 4);
-  L.row_tok = take(R * 4);
-  L.done = take(U * 4);
-  L.n_gen = take(U * 4);
-  L.gen_tokens = take(U * (size_t)c.max_new * 4);
-  L.sampled = take(U * (size_t)c.max_new * 4);
-  L.samp = take(U * sizeof(SamplingDev));
-  L.noise = take(U * sizeof(void*));
-  L.forced = take(U * sizeof(void*));
-  L.ticket = take(R * H * 4);
-  L.budget = take(U * 4);
-  L.noise_base = take(U * 4);
-  L.stage_idx = take(U * 2 * (size_t)c.block_size * 4);
-  L.stage_spk = take(U * (size_t)c.spk_dim * 4);
-  L.stage_forced = take(U * (size_t)c.max_new * 4);
-  L.stage_noise = take(U * (size_t)GEN_BURST * V * 4);   // host-supplied Exp(1) draws are staged one burst at a time
+  WsBump ws;
+  L.x = ws.take(R * D * 4);
+  L.qkv = ws.take(R * 3 * D * 4);
+  L.att = ws.take(R * D * 4);
+  L.ffn = ws.take(R * F * 4);
+  L.logits = ws.take(R * V * 4);
+  L.spk = ws.take(U * D * 4);
+  L.part_o = ws.take(R * H * ATT_SPLITS * 128 * 4);
+  L.part_ml = ws.take(R * H * ATT_SPLITS * 2 * 4);
+  L.slot_map = ws.take(U * 4);
+  L.pos = ws.take(U * 4);
+  L.row_tok = ws.take(R * 4);
+  L.done = ws.take(U * 4);
+  L.n_gen = ws.take(U * 4);
+  L.gen_tokens = ws.take(U * (size_t)c.max_new * 4);
+  L.sampled = ws.take(U * (size_t)c.max_new * 4);
+  L.samp = ws.take(U * sizeof(SamplingDev));
+  L.noise = ws.take(U * sizeof(void*));
+  L.forced = ws.take(U * sizeof(void*));
+  L.ticket = ws.take(R * H * 4);
+  L.budget = ws.take(U * 4);
+  L.noise_base = ws.take(U * 4);
+  L.stage_idx = ws.take(U * 2 * (size_t)c.block_size * 4);
+  L.stage_spk = ws.take(U * (size_t)c.spk_dim * 4);
+  L.stage_forced = ws.take(U * (size_t)c.max_new * 4);
+  L.stage_noise = ws.take(U * (size_t)GEN_BURST * V * 4);   // host-supplied Exp(1) draws are staged one burst at a time
   {
     const size_t RB = RB_MAX, NBM = 2 * RB_MAX;
-    L.b_x = take(RB * D * 4);
-    L.b_qkv = take(RB * 3 * D * 4);
-    L.b_att = take(RB * D * 4);
-    L.b_ffn = take(RB * F * 4);
-    L.b_logits = take(RB * V * 4);
-    L.b_last = take(2 * D * 4);
-    L.b_B = take(NBM * (F > D ? F : D) * 2);
-    L.b_rows = take(5 * RB * 4);
+    L.b_x = ws.take(RB * D * 4);
+    L.b_qkv = ws.take(RB * 3 * D * 4);
+    L.b_att = ws.take(RB * D * 4);
+    L.b_ffn = ws.take(RB * F * 4);
+    L.b_logits = ws.take(RB * V * 4);
+    L.b_last = ws.take(2 * D * 4);
+    L.b_B = ws.take(NBM * (F > D ? F : D) * 2);
+    L.b_rows = ws.take(5 * RB * 4);
     size_t sc = 0;
     const size_t mats[5][3] = {{3 * D, D, 1}, {D, D, 1}, {F, D, 2}, {D, F, 1}, {V, D, 1}};
     for (auto& m : mats) {
       GemmPlan g = plan_gemm((int)m[0], (int)m[1], (int)NBM, m[2] == 2, GEMM_MAX_SM);
       if (g.scratch_floats > sc) sc = g.scratch_floats;
     }
-    L.b_scratch = take(sc * 4);
-    L.b_tickets = take(256 * 4);
-    L.b_part_o = take(RB * H * ATT_SPLITS * 128 * 4);
-    L.b_part_ml = take(RB * H * ATT_SPLITS * 2 * 4);
-    L.b_att_tickets = take(RB * H * 4);
+    L.b_scratch = ws.take(sc * 4);
+    L.b_tickets = ws.take(256 * 4);
+    L.b_part_o = ws.take(RB * H * ATT_SPLITS * 128 * 4);
+    L.b_part_ml = ws.take(RB * H * ATT_SPLITS * 2 * 4);
+    L.b_att_tickets = ws.take(RB * H * 4);
   }
-  L.c_x = take((size_t)PC_RPAD * D * 4);
-  L.c_qkv = take((size_t)PC_RPAD * 3 * D * 4);
-  L.c_gu = take((size_t)PC_RPAD * 2 * F * 4);
-  L.c_part_o = take((size_t)PC_RPAD * H * PC_MAX_CHUNKS * 128 * 4);
-  L.c_part_ml = take((size_t)PC_RPAD * H * PC_MAX_CHUNKS * 2 * 4);
-  L.c_bar = take(256);
-  L.c_trace = take((size_t)160 * PC_TRACE_EVENTS * 8);
-  L.c_stat = take((size_t)(2 * c.n_layer + 1) * PC_RPAD * 4);
-  L.c_samp_part = take((size_t)(PC_RPAD / 2) * 256 * 4);
-  L.c_samp_best = take((size_t)2 * (PC_RPAD / 2) * 8);
-  L.total = o;
+  L.c_x = ws.take((size_t)PC_RPAD * D * 4);
+  L.c_qkv = ws.take((size_t)PC_RPAD * 3 * D * 4);
+  L.c_gu = ws.take((size_t)PC_RPAD * 2 * F * 4);
+  L.c_part_o = ws.take((size_t)PC_RPAD * H * PC_MAX_CHUNKS * 128 * 4);
+  L.c_part_ml = ws.take((size_t)PC_RPAD * H * PC_MAX_CHUNKS * 2 * 4);
+  L.c_bar = ws.take(256);
+  L.c_trace = ws.take((size_t)160 * PC_TRACE_EVENTS * 8);
+  L.c_stat = ws.take((size_t)(2 * c.n_layer + 1) * PC_RPAD * 4);
+  L.c_samp_part = ws.take((size_t)(PC_RPAD / 2) * 256 * 4);
+  L.c_samp_best = ws.take((size_t)2 * (PC_RPAD / 2) * 8);
+  L.total = ws.end;
+  L.w4_scratch = ws.take(w4_layer_elems(c) * 2);
+  L.total_int4 = ws.end;
   return L;
 }
 
@@ -209,20 +183,17 @@ static PcMat plan_pc(int M, int K, int ctas, int tile_rows) {
 }
 
 static int validate(const mvb_s1_config* c) {
-  if (!c) return fail(MVB_ERR_ARG, "null config");
-  if (c->head_dim != 128) return fail(MVB_ERR_UNSUPPORTED, "head_dim must be 128 (got %d)", c->head_dim);
-  if (c->dim != c->n_head * c->head_dim) return fail(MVB_ERR_ARG, "dim != n_head*head_dim");
-  if (c->dim % 256 || c->intermediate % 256) return fail(MVB_ERR_UNSUPPORTED, "dim and intermediate must be multiples of 256");
-  if (c->vocab % 2 || c->vocab > SAMP_PAD) return fail(MVB_ERR_UNSUPPORTED, "vocab must be even and <= %d", SAMP_PAD);
-  if (c->max_utts < 1 || c->max_utts > 64) return fail(MVB_ERR_ARG, "max_utts out of range");
-  if (c->max_new < 1 || c->max_new > c->block_size) return fail(MVB_ERR_ARG, "max_new out of range");
-  if (c->kv_dtype != MVB_KV_BF16 && c->kv_dtype != MVB_KV_FP32) return fail(MVB_ERR_ARG, "bad kv_dtype");
-  if ((size_t)c->intermediate * 8 > 48 * 1024 - 256) return fail(MVB_ERR_UNSUPPORTED, "intermediate too large for the staging buffer");
+  if (!c) return set_error(MVB_ERR_ARG, "null config");
+  if (c->head_dim != 128) return set_error(MVB_ERR_UNSUPPORTED, "head_dim must be 128 (got %d)", c->head_dim);
+  if (c->dim != c->n_head * c->head_dim) return set_error(MVB_ERR_ARG, "dim != n_head*head_dim");
+  if (c->dim % 256 || c->intermediate % 256) return set_error(MVB_ERR_UNSUPPORTED, "dim and intermediate must be multiples of 256");
+  if (c->vocab % 2 || c->vocab > SAMP_PAD) return set_error(MVB_ERR_UNSUPPORTED, "vocab must be even and <= %d", SAMP_PAD);
+  if (c->max_utts < 1 || c->max_utts > 64) return set_error(MVB_ERR_ARG, "max_utts out of range");
+  if (c->max_new < 1 || c->max_new > c->block_size) return set_error(MVB_ERR_ARG, "max_new out of range");
+  if (c->kv_dtype != MVB_KV_BF16 && c->kv_dtype != MVB_KV_FP32) return set_error(MVB_ERR_ARG, "bad kv_dtype");
+  if ((size_t)c->intermediate * 8 > 48 * 1024 - 256) return set_error(MVB_ERR_UNSUPPORTED, "intermediate too large for the staging buffer");
   return MVB_OK;
 }
-
-extern "C" int mvb_abi_version(void) { return MVB_ABI_VERSION; }
-extern "C" const char* mvb_last_error(void) { return g_err.c_str(); }
 
 extern "C" size_t mvb_s1_kv_bytes(const mvb_s1_config* c) {
   if (validate(c)) return 0;
@@ -235,64 +206,41 @@ extern "C" size_t mvb_s1_workspace_bytes(const mvb_s1_config* c) {
   return make_layout(*c).total;
 }
 
-// elements of one layer's dequantised weights: wqkv, wo, w1, w3, w2
-static size_t w4_layer_elems(const mvb_s1_config& c) {
-  const size_t D = c.dim, F = c.intermediate;
-  return 4 * D * D + 3 * D * F;
-}
-
 extern "C" size_t mvb_s1_int4_workspace_bytes(const mvb_s1_config* c) {
   if (validate(c)) return 0;
-  return align_up(make_layout(*c).total) + align_up(w4_layer_elems(*c) * 2);
-}
-
-static int create_engine(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
-                         void* d_kv, void* d_ws, mvb_s1** out, bool int4);
-
-extern "C" int mvb_s1_create(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
-                             void* d_kv, void* d_ws, mvb_s1** out) {
-  return create_engine(cfg, d_arena, arena_bytes, offsets, d_kv, d_ws, out, false);
-}
-
-extern "C" int mvb_s1_create_int4(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
-                                  void* d_kv, void* d_ws, mvb_s1** out) {
-  return create_engine(cfg, d_arena, arena_bytes, offsets, d_kv, d_ws, out, true);
+  return make_layout(*c).total_int4;
 }
 
 static int create_engine(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
                          void* d_kv, void* d_ws, mvb_s1** out, bool int4) {
   if (int e = validate(cfg)) return e;
-  if (!d_arena || !offsets || !d_kv || !d_ws || !out) return fail(MVB_ERR_ARG, "null pointer argument");
-  int dev = 0, major = 0, minor = 0;
-  CK(cudaGetDevice(&dev));
-  CK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-  CK(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
-  if (major != 9 || minor != 0) return fail(MVB_ERR_UNSUPPORTED, "libmvb200 is built for sm_90a only; device is sm_%d%d", major, minor);
-  struct Guard {   // frees the half-built handle on every early return below
-    mvb_s1* h;
-    ~Guard() { if (h) mvb_s1_destroy(h); }
-  } guard{new mvb_s1()};
-  mvb_s1* h = guard.h;
+  if (!d_arena || !offsets || !d_kv || !d_ws || !out) return set_error(MVB_ERR_ARG, "null pointer argument");
+  int dev = 0, n_sm = 0, major = 0, minor = 0;
+  if (int e = current_device(&dev, &n_sm)) return e;
+  MVB_CK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
+  MVB_CK(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
+  if (major != 9 || minor != 0) return set_error(MVB_ERR_UNSUPPORTED, "libmvb200 is built for sm_90a only; device is sm_%d%d", major, minor);
+  Building<mvb_s1> hb(new mvb_s1(), mvb_s1_destroy);
+  mvb_s1* h = hb.get();
   h->cfg = *cfg;
-  CK(cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, dev));
+  h->n_sm = n_sm;
   h->arena = reinterpret_cast<const char*>(d_arena);
   const int n_off = MVB_S1_GLOBAL_TENSORS + cfg->n_layer * MVB_S1_LAYER_TENSORS;
+  if (int e = check_offsets(offsets, n_off, arena_bytes, "weight offset")) return e;
   h->off.assign(offsets, offsets + n_off);
-  for (uint64_t o : h->off)
-    if (o % 16 || o >= arena_bytes) return fail(MVB_ERR_ARG, "weight offset %llu not 16B-aligned or outside the arena", (unsigned long long)o);
   h->kv = reinterpret_cast<char*>(d_kv);
   h->ws = reinterpret_cast<char*>(d_ws);
   h->L = make_layout(*cfg);
   h->int4 = int4;
   if (int4) {
-    h->w4_scratch = h->wsp<__nv_bfloat16>(align_up(h->L.total));
+    h->w4_scratch = h->wsp<__nv_bfloat16>(h->L.w4_scratch);
     const int D = cfg->dim, F = cfg->intermediate;
     const int MK[7][2] = {{0, 0}, {3 * D, D}, {D, D}, {0, 0}, {F, D}, {F, D}, {D, F}};
     for (int l = 0; l < cfg->n_layer; ++l)
       for (int t : {1, 2, 4, 5, 6}) {
         const uint64_t o = h->off[MVB_S1_GLOBAL_TENSORS + l * MVB_S1_LAYER_TENSORS + t];
         if (o + w4_packed_bytes(MK[t][0], MK[t][1]) > arena_bytes)
-          return fail(MVB_ERR_ARG, "int4 packed matrix %d of layer %d runs past the end of the arena", t, l);
+          return set_error(MVB_ERR_ARG, "int4 packed matrix %d of layer %d runs past the end of the arena", t, l);
       }
   }
   S1State& s = h->st;
@@ -328,7 +276,7 @@ static int create_engine(const mvb_s1_config* cfg, const void* d_arena, size_t a
       ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 4], h->tc_w(l, 6), D, F, 128);
     }
     ok = ok && make_tmap_bf16(&h->tmW[(size_t)cfg->n_layer * 5], h->w(4), cfg->vocab, D, 128);
-    if (!ok) return fail(MVB_ERR_CUDA, "cuTensorMapEncodeTiled failed for a weight matrix");
+    if (!ok) return set_error(MVB_ERR_CUDA, "cuTensorMapEncodeTiled failed for a weight matrix");
   }
   if (const char* e = getenv("MVB_PATHC")) h->path_c = atoi(e) != 0;
   if (const char* e = getenv("MVB_PC_TRACE")) h->trace = atoi(e) != 0;
@@ -338,7 +286,7 @@ static int create_engine(const mvb_s1_config* cfg, const void* d_arena, size_t a
   memset(&h->tm_kv, 0, sizeof(h->tm_kv));
   bool kv_ok = cfg->kv_dtype == MVB_KV_FP32;
   if (cfg->kv_dtype == MVB_KV_BF16 && cfg->block_size % 64 == 0) {
-    CK(cudaMemset(h->kv, 0, (size_t)cfg->n_layer * 2 * h->kv_half_bytes()));
+    MVB_CK(cudaMemset(h->kv, 0, (size_t)cfg->n_layer * 2 * h->kv_half_bytes()));
     const uint64_t rows = (uint64_t)cfg->n_layer * 2 * (h->kv_half_bytes() / 256);
     kv_ok = rows < (1ull << 31) && make_tmap_bf16(&h->tm_kv, h->kv, rows, 128, 64);
   }
@@ -374,14 +322,23 @@ static int create_engine(const mvb_s1_config* cfg, const void* d_arena, size_t a
   // Opt-in shared-memory size is a per-device function attribute: set it for the device this handle lives on
   // (a process may hold engines on several GPUs).
 #define MVB_PC_ATTR(FP, NBV)                                                                                        \
-  CK(cudaFuncSetAttribute(k_decode_persistent<FP, NBV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PcCfg<NBV>::SMEM))
+  MVB_CK(cudaFuncSetAttribute(k_decode_persistent<FP, NBV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PcCfg<NBV>::SMEM))
   MVB_PC_ATTR(true, 32); MVB_PC_ATTR(true, 16); MVB_PC_ATTR(false, 32); MVB_PC_ATTR(false, 16);
 #undef MVB_PC_ATTR
-  CK(cudaStreamCreateWithFlags(&h->cap_stream, cudaStreamNonBlocking));
-  CK(cudaMallocHost(&h->h_flags, sizeof(int) * 4 * 64));
-  guard.h = nullptr;
-  *out = h;
+  MVB_CK(cudaStreamCreateWithFlags(&h->cap_stream, cudaStreamNonBlocking));
+  MVB_CK(cudaMallocHost(&h->h_flags, sizeof(int) * 4 * 64));
+  *out = hb.release();
   return MVB_OK;
+}
+
+extern "C" int mvb_s1_create(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
+                             void* d_kv, void* d_ws, mvb_s1** out) {
+  return create_engine(cfg, d_arena, arena_bytes, offsets, d_kv, d_ws, out, false);
+}
+
+extern "C" int mvb_s1_create_int4(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
+                                  void* d_kv, void* d_ws, mvb_s1** out) {
+  return create_engine(cfg, d_arena, arena_bytes, offsets, d_kv, d_ws, out, true);
 }
 
 extern "C" int mvb_s1_destroy(mvb_s1* h) {
@@ -440,7 +397,7 @@ static int launch_body(mvb_s1* h, cudaStream_t s, int n_utts) {
   float* att = h->wsp<float>(h->L.att);
   float* ffn = h->wsp<float>(h->L.ffn);
   float* logits = h->wsp<float>(h->L.logits);
-  CK(launch_pdl(h->pdl, k_embed, dim3(2, n_utts), dim3(256), 0, s, h->st, h->w(0), h->w(1),
+  MVB_CK(launch_pdl(h->pdl, k_embed, dim3(2, n_utts), dim3(256), 0, s, h->st, h->w(0), h->w(1),
                 (const float*)h->wsp<float>(h->L.spk), x, D));
   h->launches++;
   const size_t half = h->kv_half_bytes();
@@ -453,32 +410,32 @@ static int launch_body(mvb_s1* h, cudaStream_t s, int n_utts) {
     p.W = h->lw(l, 1); p.W3 = nullptr; p.x = x; p.ldx = D; p.gain = h->lw(l, 0);
     p.out = qkv; p.ldo = 3 * D; p.M = 3 * D; p.K = D;
     p.kcache = kc; p.vcache = vc; p.H = H; p.S_max = c.block_size; p.D = D; p.kv_fp32 = c.kv_dtype == MVB_KV_FP32;
-    CK(launch_gemv<EPI_QKV>(h, s, n_utts, p, h->int4));
+    MVB_CK(launch_gemv<EPI_QKV>(h, s, n_utts, p, h->int4));
     // attention over [0, pos]
     dim3 ag(H, 2 * n_utts, ATT_SPLITS);
     if (c.kv_dtype == MVB_KV_FP32)
-      CK(launch_pdl(h->pdl, k_attn_decode<true>, ag, dim3(128), 0, s, h->st, (const float*)qkv, (const void*)kc, (const void*)vc,
+      MVB_CK(launch_pdl(h->pdl, k_attn_decode<true>, ag, dim3(128), 0, s, h->st, (const float*)qkv, (const void*)kc, (const void*)vc,
                     h->wsp<float>(h->L.part_o), h->wsp<float>(h->L.part_ml), att, H, c.block_size, D));
     else
-      CK(launch_pdl(h->pdl, k_attn_decode<false>, ag, dim3(128), 0, s, h->st, (const float*)qkv, (const void*)kc, (const void*)vc,
+      MVB_CK(launch_pdl(h->pdl, k_attn_decode<false>, ag, dim3(128), 0, s, h->st, (const float*)qkv, (const void*)kc, (const void*)vc,
                     h->wsp<float>(h->L.part_o), h->wsp<float>(h->L.part_ml), att, H, c.block_size, D));
     h->launches++;
     // wo + residual
     p = GemvP{};
     p.eps = c.norm_eps;
     p.W = h->lw(l, 2); p.x = att; p.ldx = D; p.gain = nullptr; p.out = x; p.ldo = D; p.M = D; p.K = D;
-    CK(launch_gemv<EPI_RESID>(h, s, n_utts, p, h->int4));
+    MVB_CK(launch_gemv<EPI_RESID>(h, s, n_utts, p, h->int4));
     // ffn_norm + silu(w1 x) * w3 x
     p.W = h->lw(l, 4); p.W3 = h->lw(l, 5); p.x = x; p.ldx = D; p.gain = h->lw(l, 3); p.out = ffn; p.ldo = F; p.M = F; p.K = D;
-    CK(launch_gemv<EPI_SWIGLU>(h, s, n_utts, p, h->int4));
+    MVB_CK(launch_gemv<EPI_SWIGLU>(h, s, n_utts, p, h->int4));
     // w2 + residual
     p.W = h->lw(l, 6); p.W3 = nullptr; p.x = ffn; p.ldx = F; p.gain = nullptr; p.out = x; p.ldo = D; p.M = D; p.K = F;
-    CK(launch_gemv<EPI_RESID>(h, s, n_utts, p, h->int4));
+    MVB_CK(launch_gemv<EPI_RESID>(h, s, n_utts, p, h->int4));
   }
   GemvP p{};
   p.eps = c.norm_eps;
   p.W = h->w(4); p.x = x; p.ldx = D; p.gain = h->w(3); p.out = logits; p.ldo = V; p.M = V; p.K = D;
-  CK(launch_gemv<EPI_STORE>(h, s, n_utts, p));
+  MVB_CK(launch_gemv<EPI_STORE>(h, s, n_utts, p));
   return MVB_OK;
 }
 
@@ -510,7 +467,7 @@ static int linear_b(mvb_s1* h, cudaStream_t s, int R, const LinB& a, void* kc = 
   TcGemm g{};
   g.epi = EPI; g.R = R; g.Rpad = (R + 15) / 16 * 16; g.split_lo = 1;   // activations as hi + lo bf16 terms
   g.tmB = tmap_b(h, 2 * g.Rpad, a.K);
-  if (!g.tmB) return fail(MVB_ERR_CUDA, "cuTensorMapEncodeTiled failed for the activation buffer");
+  if (!g.tmB) return set_error(MVB_ERR_CUDA, "cuTensorMapEncodeTiled failed for the activation buffer");
   g.tmW = &h->tmW[a.widx]; g.tmW3 = &h->tmW[a.widx3];
   g.B = h->wsp<__nv_bfloat16>(h->L.b_B);
   g.x = a.x; g.ldx = a.ldx; g.gain = a.gain; g.eps = c.norm_eps;
@@ -520,7 +477,7 @@ static int linear_b(mvb_s1* h, cudaStream_t s, int R, const LinB& a, void* kc = 
   g.scratch = h->wsp<float>(h->L.b_scratch);
   g.tickets = h->wsp<unsigned>(h->L.b_tickets);
   g.n_sm = h->n_sm;
-  CK(tc_gemm(s, g));
+  MVB_CK(tc_gemm(s, g));
   h->launches += 2;   // k_prep_b + k_tc_gemm
   return MVB_OK;
 }
@@ -535,7 +492,7 @@ static int launch_layers_b(mvb_s1* h, cudaStream_t s, int R) {
   float* ffn = h->wsp<float>(h->L.b_ffn);
   k_embed_rows<<<R, 256, 0, s>>>(h->rows, h->w(0), h->w(1), h->wsp<float>(h->L.spk), x, D);
   h->launches++;
-  CK(cudaGetLastError());
+  MVB_CK(cudaGetLastError());
   const size_t half = h->kv_half_bytes();
   for (int l = 0; l < c.n_layer; ++l) {
     char* kc = h->kv + (size_t)l * 2 * half;
@@ -551,7 +508,7 @@ static int launch_layers_b(mvb_s1* h, cudaStream_t s, int R) {
       m.n = 5;
       k_w4_dequant<<<4 * h->n_sm, 256, 0, s>>>(m);
       h->launches++;
-      CK(cudaGetLastError());
+      MVB_CK(cudaGetLastError());
     }
     if (int e = linear_b<G_QKV>(h, s, R, LinB{x, D, h->lw(l, 0), l * 5 + 0, l * 5 + 0, 3 * D, D, qkv, 3 * D}, kc, vc)) return e;
     dim3 ag(H, R, ATT_SPLITS);
@@ -562,7 +519,7 @@ static int launch_layers_b(mvb_s1* h, cudaStream_t s, int R) {
       k_attn_rows<false><<<ag, 128, 0, s>>>(h->rows, qkv, kc, vc, h->wsp<float>(h->L.b_part_o), h->wsp<float>(h->L.b_part_ml),
                                             h->wsp<unsigned>(h->L.b_att_tickets), att, H, c.block_size, D);
     h->launches++;
-    CK(cudaGetLastError());
+    MVB_CK(cudaGetLastError());
     if (int e = linear_b<G_RESID>(h, s, R, LinB{att, D, nullptr, l * 5 + 1, l * 5 + 1, D, D, x, D})) return e;
     if (int e = linear_b<G_SWIGLU>(h, s, R, LinB{x, D, h->lw(l, 3), l * 5 + 2, l * 5 + 3, F, D, ffn, F})) return e;
     if (int e = linear_b<G_RESID>(h, s, R, LinB{ffn, F, nullptr, l * 5 + 4, l * 5 + 4, D, F, x, D})) return e;
@@ -576,7 +533,7 @@ static int launch_body_b(mvb_s1* h, cudaStream_t s, int n_utts) {
   const int R = 2 * n_utts;
   k_rows_decode<<<1, 128, 0, s>>>(h->st, h->rows, n_utts);
   h->launches++;
-  CK(cudaGetLastError());
+  MVB_CK(cudaGetLastError());
   if (int e = launch_layers_b(h, s, R)) return e;
   const int hw = c.n_layer * 5;
   return linear_b<G_STORE>(h, s, R, LinB{h->wsp<float>(h->L.b_x), c.dim, h->w(3), hw, hw, c.vocab, c.dim,
@@ -608,14 +565,14 @@ static int launch_persistent(mvb_s1* h, cudaStream_t s, int n_utts, int n_steps,
   p.trace = (h->trace && h->n_sm <= 160) ? h->wsp<long long>(h->L.c_trace) : nullptr;
   p.st = h->st;
   // launch-time invariants of the kernel: grid-barrier counter, RMSNorm statistics and arg-max slots start from zero
-  CK(cudaMemsetAsync(p.bar, 0, 4, s));
-  CK(cudaMemsetAsync(p.stat, 0, sizeof(float) * (size_t)(2 * c.n_layer + 1) * PC_RPAD, s));
-  CK(cudaMemsetAsync(p.samp_best, 0, sizeof(unsigned long long) * 2 * (PC_RPAD / 2), s));
+  MVB_CK(cudaMemsetAsync(p.bar, 0, 4, s));
+  MVB_CK(cudaMemsetAsync(p.stat, 0, sizeof(float) * (size_t)(2 * c.n_layer + 1) * PC_RPAD, s));
+  MVB_CK(cudaMemsetAsync(p.samp_best, 0, sizeof(unsigned long long) * 2 * (PC_RPAD / 2), s));
   h->launches++;
   const bool fp = p.kv_fp32 != 0, wide = p.R > 8;
   const CUtensorMap* tm = h->tm3;
 #define MVB_PC_LAUNCH(FP, NBV)                                                                                        \
-  CK(launch_pdl(h->pdl, k_decode_persistent<FP, NBV>, dim3(h->n_sm), dim3(PC_THREADS), PcCfg<NBV>::SMEM, s,           \
+  MVB_CK(launch_pdl(h->pdl, k_decode_persistent<FP, NBV>, dim3(h->n_sm), dim3(PC_THREADS), PcCfg<NBV>::SMEM, s,           \
                 tm[0], tm[1], tm[2], tm[3], tm[4], tm[5], h->tm_kv, p))
   if (fp && wide) MVB_PC_LAUNCH(true, 32);
   else if (fp) MVB_PC_LAUNCH(true, 16);
@@ -659,21 +616,15 @@ static int run_body(mvb_s1* h, cudaStream_t s, int n_utts, bool allow_b = true) 
   const int key = n_utts + (use_b ? 1000 : 0);
   auto it = h->graphs.find(key);
   if (it == h->graphs.end()) {
-    cudaGraph_t g;
     const uint64_t before = h->launches;
-    CK(cudaStreamBeginCapture(h->cap_stream, cudaStreamCaptureModeThreadLocal));
-    int e = body(h->cap_stream);
-    cudaError_t ce = cudaStreamEndCapture(h->cap_stream, &g);
+    cudaGraphExec_t ge;
+    const int e = capture_graph(h->cap_stream, &ge, body);
     h->graph_nodes[key] = (int)(h->launches - before);
     h->launches = before;
     if (e) return e;
-    CK(ce);
-    cudaGraphExec_t ge;
-    CK(cudaGraphInstantiate(&ge, g, 0));
-    CK(cudaGraphDestroy(g));
     it = h->graphs.emplace(key, ge).first;
   }
-  CK(cudaGraphLaunch(it->second, s));
+  MVB_CK(cudaGraphLaunch(it->second, s));
   h->launches += h->graph_nodes[key];
   return MVB_OK;
 }
@@ -689,23 +640,27 @@ static SamplingDev to_dev(const mvb_sampling* p) {
   return d;
 }
 
+static int check_slot(const mvb_s1* h, int32_t utt) {   // every caller-supplied utterance slot must be one of the handle's
+  return utt < 0 || utt >= h->cfg.max_utts ? set_error(MVB_ERR_ARG, "utterance slot %d out of range", utt) : MVB_OK;
+}
+
 extern "C" int mvb_s1_set_speaker(mvb_s1* h, int32_t utt, const float* d_spk, void* stream) {
-  if (!h || !d_spk) return fail(MVB_ERR_ARG, "null argument");
-  if (utt < 0 || utt >= h->cfg.max_utts) return fail(MVB_ERR_ARG, "utterance slot %d out of range", utt);
+  if (!h || !d_spk) return set_error(MVB_ERR_ARG, "null argument");
+  if (int e = check_slot(h, utt)) return e;
   cudaStream_t s = (cudaStream_t)stream;
   const int D = h->cfg.dim;
   k_spk_proj<<<(D * 32 + 255) / 256, 256, 0, s>>>(h->w(2), d_spk, h->wsp<float>(h->L.spk) + (size_t)utt * D, D, h->cfg.spk_dim);
   h->launches++;
-  CK(cudaGetLastError());
+  MVB_CK(cudaGetLastError());
   return MVB_OK;
 }
 
 extern "C" int mvb_s1_forward(mvb_s1* h, int32_t utt, const int32_t* d_idx, int32_t S, int32_t pos0, float* d_logits,
                               int32_t all_positions, void* stream) {
-  if (!h || !d_idx) return fail(MVB_ERR_ARG, "null argument");
-  if (utt < 0 || utt >= h->cfg.max_utts) return fail(MVB_ERR_ARG, "utterance slot %d out of range", utt);
+  if (!h || !d_idx) return set_error(MVB_ERR_ARG, "null argument");
+  if (int e = check_slot(h, utt)) return e;
   if (S < 1 || pos0 < 0 || pos0 + S > h->cfg.block_size)
-    return fail(MVB_ERR_ARG, "positions [%d, %d) outside the %d-slot context", pos0, pos0 + S, h->cfg.block_size);
+    return set_error(MVB_ERR_ARG, "positions [%d, %d) outside the %d-slot context", pos0, pos0 + S, h->cfg.block_size);
   cudaStream_t s = (cudaStream_t)stream;
   const int V = h->cfg.vocab;
   const float* lg = h->wsp<float>(h->L.logits) + (size_t)(2 * utt) * V;
@@ -718,7 +673,7 @@ extern "C" int mvb_s1_forward(mvb_s1* h, int32_t utt, const int32_t* d_idx, int3
       const int R = 2 * Sc;
       k_rows_prefill<<<1, 128, 0, s>>>(h->rows, utt, d_idx, S, s0, Sc, pos0);
       h->launches++;
-      CK(cudaGetLastError());
+      MVB_CK(cudaGetLastError());
       if (int e = launch_layers_b(h, s, R)) return e;
       const int hw = c.n_layer * 5;
       float* bx = h->wsp<float>(h->L.b_x);
@@ -726,7 +681,7 @@ extern "C" int mvb_s1_forward(mvb_s1* h, int32_t utt, const int32_t* d_idx, int3
         float* bl = h->wsp<float>(h->L.b_logits);
         if (int e = linear_b<G_STORE>(h, s, R, LinB{bx, c.dim, h->w(3), hw, hw, V, c.dim, bl, V})) return e;
         for (int cc = 0; cc < 2; ++cc)
-          CK(cudaMemcpyAsync(d_logits + ((size_t)cc * S + s0) * V, bl + (size_t)cc * Sc * V, sizeof(float) * (size_t)Sc * V,
+          MVB_CK(cudaMemcpyAsync(d_logits + ((size_t)cc * S + s0) * V, bl + (size_t)cc * Sc * V, sizeof(float) * (size_t)Sc * V,
                              cudaMemcpyDeviceToDevice, s));
       }
       if (s0 + Sc == S) {
@@ -734,34 +689,34 @@ extern "C" int mvb_s1_forward(mvb_s1* h, int32_t utt, const int32_t* d_idx, int3
         float* last = h->wsp<float>(h->L.b_last);
         k_gather_last<<<2, 256, 0, s>>>(bx, last, Sc, c.dim);
         h->launches++;
-        CK(cudaGetLastError());
+        MVB_CK(cudaGetLastError());
         if (int e = linear_b<G_STORE>(h, s, 2, LinB{last, c.dim, h->w(3), hw, hw, V, c.dim,
                                                     h->wsp<float>(h->L.logits) + (size_t)(2 * utt) * V, V})) return e;
         k_set_input<<<1, 32, 0, s>>>(h->st, utt, d_idx, S, S - 1, pos0 + S - 1);
         h->launches++;
-        CK(cudaGetLastError());
+        MVB_CK(cudaGetLastError());
       }
     }
-    if (d_logits && !all_positions) CK(cudaMemcpyAsync(d_logits, lg, sizeof(float) * 2 * V, cudaMemcpyDeviceToDevice, s));
+    if (d_logits && !all_positions) MVB_CK(cudaMemcpyAsync(d_logits, lg, sizeof(float) * 2 * V, cudaMemcpyDeviceToDevice, s));
     return MVB_OK;
   }
   for (int i = 0; i < S; ++i) {
     k_set_input<<<1, 32, 0, s>>>(h->st, utt, d_idx, S, i, pos0 + i);
     h->launches++;
-    CK(cudaGetLastError());
+    MVB_CK(cudaGetLastError());
     if (int e = run_body(h, s, 1, false)) return e;
     if (d_logits && all_positions) {
-      CK(cudaMemcpyAsync(d_logits + (size_t)i * V, lg, sizeof(float) * V, cudaMemcpyDeviceToDevice, s));
-      CK(cudaMemcpyAsync(d_logits + ((size_t)S + i) * V, lg + V, sizeof(float) * V, cudaMemcpyDeviceToDevice, s));
+      MVB_CK(cudaMemcpyAsync(d_logits + (size_t)i * V, lg, sizeof(float) * V, cudaMemcpyDeviceToDevice, s));
+      MVB_CK(cudaMemcpyAsync(d_logits + ((size_t)S + i) * V, lg + V, sizeof(float) * V, cudaMemcpyDeviceToDevice, s));
     }
   }
-  if (d_logits && !all_positions) CK(cudaMemcpyAsync(d_logits, lg, sizeof(float) * 2 * V, cudaMemcpyDeviceToDevice, s));
+  if (d_logits && !all_positions) MVB_CK(cudaMemcpyAsync(d_logits, lg, sizeof(float) * 2 * V, cudaMemcpyDeviceToDevice, s));
   return MVB_OK;
 }
 
 extern "C" int mvb_s1_sample(mvb_s1* h, const float* d_logits, const mvb_sampling* p, const float* d_noise, uint64_t step,
                              int32_t* d_token_out, float* d_probs_out, void* stream) {
-  if (!h || !d_logits || !p || !d_token_out) return fail(MVB_ERR_ARG, "null argument");
+  if (!h || !d_logits || !p || !d_token_out) return set_error(MVB_ERR_ARG, "null argument");
   SampleP sp{};
   sp.logits = d_logits;
   sp.V = h->cfg.vocab;
@@ -773,20 +728,20 @@ extern "C" int mvb_s1_sample(mvb_s1* h, const float* d_logits, const mvb_samplin
   sp.probs_out = d_probs_out;
   k_sample<<<1, SAMP_THREADS, 0, (cudaStream_t)stream>>>(sp, h->st);
   h->launches++;
-  CK(cudaGetLastError());
+  MVB_CK(cudaGetLastError());
   return MVB_OK;
 }
 
 extern "C" int mvb_s1_begin(mvb_s1* h, int32_t utt, int32_t first_token, int32_t pos, const mvb_sampling* p,
                             const float* d_noise, const int32_t* d_forced, void* stream) {
-  if (!h || !p) return fail(MVB_ERR_ARG, "null argument");
-  if (utt < 0 || utt >= h->cfg.max_utts) return fail(MVB_ERR_ARG, "utterance slot %d out of range", utt);
-  if (pos < 0 || pos >= h->cfg.block_size) return fail(MVB_ERR_ARG, "position %d outside the context", pos);
+  if (!h || !p) return set_error(MVB_ERR_ARG, "null argument");
+  if (int e = check_slot(h, utt)) return e;
+  if (pos < 0 || pos >= h->cfg.block_size) return set_error(MVB_ERR_ARG, "position %d outside the context", pos);
   h->h_topk[utt] = p->top_k;
   k_begin<<<1, 32, 0, (cudaStream_t)stream>>>(h->st, utt, first_token, pos, to_dev(p), d_noise, d_forced, first_token >= 0,
                                               h->cfg.max_new);
   h->launches++;
-  CK(cudaGetLastError());
+  MVB_CK(cudaGetLastError());
   return MVB_OK;
 }
 
@@ -808,19 +763,19 @@ __global__ void k_set_done(S1State st, int utt, int done) {
 // until its done flag latches (mvb_s1_poll), after which the host fetches its tokens and may admit another request.
 extern "C" int mvb_s1_admit(mvb_s1* h, int32_t utt, const int32_t* prompt, int32_t T, const float* spk_emb,
                             const mvb_sampling* params, int32_t max_new_tokens, const float* d_noise, void* stream) {
-  if (!h || !prompt || !spk_emb || !params) return fail(MVB_ERR_ARG, "null argument");
+  if (!h || !prompt || !spk_emb || !params) return set_error(MVB_ERR_ARG, "null argument");
   const mvb_s1_config& c = h->cfg;
-  if (utt < 0 || utt >= c.max_utts) return fail(MVB_ERR_ARG, "utterance slot %d out of range", utt);
-  if (T < 1) return fail(MVB_ERR_ARG, "empty prompt");
-  if (max_new_tokens < 1 || max_new_tokens > c.max_new) return fail(MVB_ERR_ARG, "max_new_tokens %d out of range", max_new_tokens);
+  if (int e = check_slot(h, utt)) return e;
+  if (T < 1) return set_error(MVB_ERR_ARG, "empty prompt");
+  if (max_new_tokens < 1 || max_new_tokens > c.max_new) return set_error(MVB_ERR_ARG, "max_new_tokens %d out of range", max_new_tokens);
   const int room = (T + max_new_tokens < c.block_size ? T + max_new_tokens : c.block_size) - T;
-  if (room <= 0) return fail(MVB_ERR_PROMPT_TOO_LONG, "Prompt is too long to generate more tokens");
+  if (room <= 0) return set_error(MVB_ERR_PROMPT_TOO_LONG, "Prompt is too long to generate more tokens");
   cudaStream_t s = (cudaStream_t)stream;
   int* di = h->wsp<int>(h->L.stage_idx) + (size_t)utt * 2 * c.block_size;
   float* d_spk = h->wsp<float>(h->L.stage_spk) + (size_t)utt * c.spk_dim;
-  CK(cudaMemcpyAsync(d_spk, spk_emb, sizeof(float) * c.spk_dim, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(di, prompt, sizeof(int) * T, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(di + T, prompt, sizeof(int) * T, cudaMemcpyHostToDevice, s));
+  MVB_CK(cudaMemcpyAsync(d_spk, spk_emb, sizeof(float) * c.spk_dim, cudaMemcpyHostToDevice, s));
+  MVB_CK(cudaMemcpyAsync(di, prompt, sizeof(int) * T, cudaMemcpyHostToDevice, s));
+  MVB_CK(cudaMemcpyAsync(di + T, prompt, sizeof(int) * T, cudaMemcpyHostToDevice, s));
   if (int e = mvb_s1_set_speaker(h, utt, d_spk, s)) return e;
   if (int e = mvb_s1_begin(h, utt, -1, 0, params, d_noise, nullptr, s)) return e;
   k_set_budget<<<1, 32, 0, s>>>(h->st, utt, room);
@@ -832,29 +787,29 @@ extern "C" int mvb_s1_admit(mvb_s1* h, int32_t utt, const int32_t* prompt, int32
   spp.decode_mode = 1;
   k_sample<<<1, SAMP_THREADS, 0, s>>>(spp, h->st);  // slot_map[0] == utt after the prefill
   h->launches++;
-  CK(cudaGetLastError());
+  MVB_CK(cudaGetLastError());
   return MVB_OK;
 }
 
 // Park a slot: its rows still ride along in the batch (recomputed at a frozen position) but nothing is sampled or
 // appended for it until the next mvb_s1_admit / mvb_s1_begin.
 extern "C" int mvb_s1_release(mvb_s1* h, int32_t utt, void* stream) {
-  if (!h) return fail(MVB_ERR_ARG, "null handle");
-  if (utt < 0 || utt >= h->cfg.max_utts) return fail(MVB_ERR_ARG, "utterance slot %d out of range", utt);
+  if (!h) return set_error(MVB_ERR_ARG, "null handle");
+  if (int e = check_slot(h, utt)) return e;
   k_set_done<<<1, 32, 0, (cudaStream_t)stream>>>(h->st, utt, 1);
   h->launches++;
-  CK(cudaGetLastError());
+  MVB_CK(cudaGetLastError());
   return MVB_OK;
 }
 
 // done flags and generated-token counts of slots [0, n_slots) in one device->host round trip (synchronises `stream`).
 extern "C" int mvb_s1_poll(mvb_s1* h, int32_t n_slots, int32_t* done_out, int32_t* n_gen_out, void* stream) {
-  if (!h || !done_out || !n_gen_out) return fail(MVB_ERR_ARG, "null argument");
-  if (n_slots < 1 || n_slots > h->cfg.max_utts) return fail(MVB_ERR_ARG, "n_slots %d out of range", n_slots);
+  if (!h || !done_out || !n_gen_out) return set_error(MVB_ERR_ARG, "null argument");
+  if (n_slots < 1 || n_slots > h->cfg.max_utts) return set_error(MVB_ERR_ARG, "n_slots %d out of range", n_slots);
   cudaStream_t s = (cudaStream_t)stream;
-  CK(cudaMemcpyAsync(h->h_flags, h->st.done, sizeof(int) * n_slots, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(h->h_flags + 64, h->st.n_gen, sizeof(int) * n_slots, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
+  MVB_CK(cudaMemcpyAsync(h->h_flags, h->st.done, sizeof(int) * n_slots, cudaMemcpyDeviceToHost, s));
+  MVB_CK(cudaMemcpyAsync(h->h_flags + 64, h->st.n_gen, sizeof(int) * n_slots, cudaMemcpyDeviceToHost, s));
+  MVB_CK(cudaStreamSynchronize(s));
   for (int i = 0; i < n_slots; ++i) { done_out[i] = h->h_flags[i]; n_gen_out[i] = h->h_flags[64 + i]; }
   return MVB_OK;
 }
@@ -866,24 +821,24 @@ static int sample_step(mvb_s1* h, cudaStream_t s, int n_utts) {
   sp.decode_mode = 1;
   sp.grid_bar = h->wsp<unsigned>(h->L.c_bar);
   h->launches++;
-  CK(launch_pdl(h->pdl, k_sample, dim3(n_utts), dim3(SAMP_THREADS), 0, s, sp, h->st));
+  MVB_CK(launch_pdl(h->pdl, k_sample, dim3(n_utts), dim3(SAMP_THREADS), 0, s, sp, h->st));
   return MVB_OK;
 }
 
 extern "C" int mvb_s1_decode(mvb_s1* h, int32_t n_utts, int32_t n_steps, void* stream) {
-  if (!h) return fail(MVB_ERR_ARG, "null handle");
-  if (n_utts < 1 || n_utts > h->cfg.max_utts) return fail(MVB_ERR_ARG, "n_utts %d out of range", n_utts);
+  if (!h) return set_error(MVB_ERR_ARG, "null handle");
+  if (n_utts < 1 || n_utts > h->cfg.max_utts) return set_error(MVB_ERR_ARG, "n_utts %d out of range", n_utts);
   if (n_steps < 1) return MVB_OK;
   cudaStream_t s = (cudaStream_t)stream;
   k_identity_slots<<<1, 64, 0, s>>>(h->st, n_utts);
   h->launches++;
-  CK(cudaGetLastError());
+  MVB_CK(cudaGetLastError());
   const bool use_c = use_path_c(h, n_utts);
   if (use_c) {
     // The persistent kernel ACCUMULATES split-K partial logits (red.add); a prefill (mvb_s1_forward) leaves the last
     // position's logits in the same rows, so they must be zero before the first fused step.  Its grid-barrier counter
     // starts from zero at every launch.
-    CK(cudaMemsetAsync(h->wsp<float>(h->L.logits), 0, sizeof(float) * 2 * (size_t)n_utts * h->cfg.vocab, s));
+    MVB_CK(cudaMemsetAsync(h->wsp<float>(h->L.logits), 0, sizeof(float) * 2 * (size_t)n_utts * h->cfg.vocab, s));
     // One launch for the whole burst: the kernel samples on the device (top_k = None only, the stage-1 default of
     // TTS.synthesise) and stays resident across positions.
     bool fused = h->fused && (h->cfg.vocab + h->n_sm - 1) / h->n_sm <= PC_SAMP_OWN && h->cfg.vocab <= SAMP_PAD;
@@ -908,62 +863,64 @@ extern "C" int mvb_s1_decode(mvb_s1* h, int32_t n_utts, int32_t n_steps, void* s
 // fused kernel where mvb_s1_decode would use it (up to 8 utterances), else the per-layer path (tensor-core rows path
 // from 2 utterances up).
 extern "C" int mvb_s1_step_logits(mvb_s1* h, int32_t n_utts, float* d_logits, void* stream) {
-  if (!h || !d_logits) return fail(MVB_ERR_ARG, "null argument");
-  if (n_utts < 1 || n_utts > h->cfg.max_utts) return fail(MVB_ERR_ARG, "n_utts %d out of range", n_utts);
+  if (!h || !d_logits) return set_error(MVB_ERR_ARG, "null argument");
+  if (n_utts < 1 || n_utts > h->cfg.max_utts) return set_error(MVB_ERR_ARG, "n_utts %d out of range", n_utts);
   cudaStream_t s = (cudaStream_t)stream;
   const size_t bytes = sizeof(float) * 2 * (size_t)n_utts * h->cfg.vocab;
   k_identity_slots<<<1, 64, 0, s>>>(h->st, n_utts);
   h->launches++;
-  CK(cudaGetLastError());
+  MVB_CK(cudaGetLastError());
   if (!use_path_c(h, n_utts)) {
     if (int e = run_body(h, s, n_utts)) return e;
-    CK(cudaMemcpyAsync(d_logits, h->wsp<float>(h->L.logits), bytes, cudaMemcpyDeviceToDevice, s));
+    MVB_CK(cudaMemcpyAsync(d_logits, h->wsp<float>(h->L.logits), bytes, cudaMemcpyDeviceToDevice, s));
     return MVB_OK;
   }
-  CK(cudaMemsetAsync(h->wsp<float>(h->L.logits), 0, bytes, s));
-  CK(cudaMemsetAsync(h->wsp<unsigned>(h->L.c_bar), 0, 4, s));
+  MVB_CK(cudaMemsetAsync(h->wsp<float>(h->L.logits), 0, bytes, s));
+  MVB_CK(cudaMemsetAsync(h->wsp<unsigned>(h->L.c_bar), 0, 4, s));
   if (int e = launch_persistent(h, s, n_utts, 1, false)) return e;
-  CK(cudaMemcpyAsync(d_logits, h->wsp<float>(h->L.logits), bytes, cudaMemcpyDeviceToDevice, s));
-  CK(cudaMemsetAsync(h->wsp<float>(h->L.logits), 0, bytes, s));
-  CK(cudaMemsetAsync(h->wsp<unsigned>(h->L.c_bar), 0, 4, s));
+  MVB_CK(cudaMemcpyAsync(d_logits, h->wsp<float>(h->L.logits), bytes, cudaMemcpyDeviceToDevice, s));
+  MVB_CK(cudaMemsetAsync(h->wsp<float>(h->L.logits), 0, bytes, s));
+  MVB_CK(cudaMemsetAsync(h->wsp<unsigned>(h->L.c_bar), 0, 4, s));
   return MVB_OK;
 }
 
 // Debug: copy the persistent kernel's per-CTA phase time stamps (clock64) of the last step to the host.
 extern "C" int mvb_s1_trace_fetch(mvb_s1* h, long long* out, int32_t max_ctas, void* stream) {
-  if (!h || !out) return fail(MVB_ERR_ARG, "null argument");
+  if (!h || !out) return set_error(MVB_ERR_ARG, "null argument");
   const int n = h->n_sm < max_ctas ? h->n_sm : max_ctas;
-  CK(cudaMemcpyAsync(out, h->wsp<long long>(h->L.c_trace), sizeof(long long) * (size_t)n * PC_TRACE_EVENTS, cudaMemcpyDeviceToHost,
+  MVB_CK(cudaMemcpyAsync(out, h->wsp<long long>(h->L.c_trace), sizeof(long long) * (size_t)n * PC_TRACE_EVENTS, cudaMemcpyDeviceToHost,
                      (cudaStream_t)stream));
-  CK(cudaStreamSynchronize((cudaStream_t)stream));
+  MVB_CK(cudaStreamSynchronize((cudaStream_t)stream));
   return n;
 }
 
 extern "C" int mvb_s1_fetch(mvb_s1* h, int32_t utt, int32_t* out_tokens, int32_t cap, int32_t* n_out, int32_t* done,
                             void* stream) {
-  if (!h) return fail(MVB_ERR_ARG, "null handle");
-  if (utt < 0 || utt >= h->cfg.max_utts) return fail(MVB_ERR_ARG, "utterance slot %d out of range", utt);
+  if (!h) return set_error(MVB_ERR_ARG, "null handle");
+  if (int e = check_slot(h, utt)) return e;
   cudaStream_t s = (cudaStream_t)stream;
-  CK(cudaMemcpyAsync(h->h_flags, h->st.n_gen + utt, 4, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(h->h_flags + 1, h->st.done + utt, 4, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
+  MVB_CK(cudaMemcpyAsync(h->h_flags, h->st.n_gen + utt, 4, cudaMemcpyDeviceToHost, s));
+  MVB_CK(cudaMemcpyAsync(h->h_flags + 1, h->st.done + utt, 4, cudaMemcpyDeviceToHost, s));
+  MVB_CK(cudaStreamSynchronize(s));
   const int n = h->h_flags[0];
   if (n_out) *n_out = n;
   if (done) *done = h->h_flags[1];
   if (out_tokens && cap > 0) {
     const int m = n < cap ? n : cap;
-    CK(cudaMemcpyAsync(out_tokens, h->st.gen_tokens + (size_t)utt * h->cfg.max_new, sizeof(int) * m, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
+    MVB_CK(cudaMemcpyAsync(out_tokens, h->st.gen_tokens + (size_t)utt * h->cfg.max_new, sizeof(int) * m, cudaMemcpyDeviceToHost, s));
+    MVB_CK(cudaStreamSynchronize(s));
   }
   return MVB_OK;
 }
 
 // Sampled (pre-teacher-forcing) tokens, for the parity tests.
 extern "C" int mvb_s1_fetch_sampled(mvb_s1* h, int32_t utt, int32_t* out_tokens, int32_t cap, void* stream) {
-  if (!h || !out_tokens) return fail(MVB_ERR_ARG, "null argument");
+  if (!h || !out_tokens) return set_error(MVB_ERR_ARG, "null argument");
+  if (int e = check_slot(h, utt)) return e;
+  if (cap < 0 || cap > h->cfg.max_new) return set_error(MVB_ERR_ARG, "cap %d outside [0, %d]", cap, h->cfg.max_new);
   cudaStream_t s = (cudaStream_t)stream;
-  CK(cudaMemcpyAsync(out_tokens, h->st.sampled_tokens + (size_t)utt * h->cfg.max_new, sizeof(int) * cap, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
+  MVB_CK(cudaMemcpyAsync(out_tokens, h->st.sampled_tokens + (size_t)utt * h->cfg.max_new, sizeof(int) * cap, cudaMemcpyDeviceToHost, s));
+  MVB_CK(cudaStreamSynchronize(s));
   return MVB_OK;
 }
 
@@ -972,18 +929,18 @@ extern "C" int mvb_s1_generate(mvb_s1* h, int32_t n_utts, const int32_t* prompts
                                const float* noise, int32_t noise_on_device, const int32_t* forced, int32_t* out_tokens,
                                int32_t* out_lens, void* stream) {
   if (!h || !prompts || !prompt_lens || !spk_embs || !params || !out_tokens || !out_lens)
-    return fail(MVB_ERR_ARG, "null argument");
+    return set_error(MVB_ERR_ARG, "null argument");
   const mvb_s1_config& c = h->cfg;
-  if (n_utts < 1 || n_utts > c.max_utts) return fail(MVB_ERR_ARG, "n_utts %d exceeds the %d slots", n_utts, c.max_utts);
-  if (max_new_tokens < 1 || max_new_tokens > c.max_new) return fail(MVB_ERR_ARG, "max_new_tokens %d out of range", max_new_tokens);
+  if (n_utts < 1 || n_utts > c.max_utts) return set_error(MVB_ERR_ARG, "n_utts %d exceeds the %d slots", n_utts, c.max_utts);
+  if (max_new_tokens < 1 || max_new_tokens > c.max_new) return set_error(MVB_ERR_ARG, "max_new_tokens %d out of range", max_new_tokens);
   cudaStream_t s = (cudaStream_t)stream;
   // generate(): max_seq = min(T + max_new, block_size); raise if no room (utils:196-204)
   std::vector<int> budget(n_utts);
   for (int i = 0; i < n_utts; ++i) {
     const int T = prompt_lens[i];
-    if (T < 1) return fail(MVB_ERR_ARG, "empty prompt for utterance %d", i);
+    if (T < 1) return set_error(MVB_ERR_ARG, "empty prompt for utterance %d", i);
     const int room = (T + max_new_tokens < c.block_size ? T + max_new_tokens : c.block_size) - T;
-    if (room <= 0) return fail(MVB_ERR_PROMPT_TOO_LONG, "Prompt is too long to generate more tokens");
+    if (room <= 0) return set_error(MVB_ERR_PROMPT_TOO_LONG, "Prompt is too long to generate more tokens");
     budget[i] = room;
   }
   const int V = c.vocab;
@@ -993,18 +950,18 @@ extern "C" int mvb_s1_generate(mvb_s1* h, int32_t n_utts, const int32_t* prompts
   float* d_stage = h->wsp<float>(h->L.stage_noise);
   auto stage_rows = [&](int step0, int rows) -> int {
     for (int i = 0; i < n_utts; ++i)
-      CK(cudaMemcpyAsync(d_stage + (size_t)i * GEN_BURST * V, noise + ((size_t)i * max_new_tokens + step0) * V,
+      MVB_CK(cudaMemcpyAsync(d_stage + (size_t)i * GEN_BURST * V, noise + ((size_t)i * max_new_tokens + step0) * V,
                          sizeof(float) * (size_t)rows * V, cudaMemcpyHostToDevice, s));
     k_set_noise_base<<<1, 64, 0, s>>>(h->st, n_utts, step0);
     h->launches++;
-    CK(cudaGetLastError());
+    MVB_CK(cudaGetLastError());
     return MVB_OK;
   };
   int* d_forced = h->wsp<int>(h->L.stage_forced);
-  if (forced) CK(cudaMemcpyAsync(d_forced, forced, sizeof(int) * (size_t)n_utts * max_new_tokens, cudaMemcpyHostToDevice, s));
+  if (forced) MVB_CK(cudaMemcpyAsync(d_forced, forced, sizeof(int) * (size_t)n_utts * max_new_tokens, cudaMemcpyHostToDevice, s));
   int* d_idx = h->wsp<int>(h->L.stage_idx);
   float* d_spk = h->wsp<float>(h->L.stage_spk);
-  CK(cudaMemcpyAsync(d_spk, spk_embs, sizeof(float) * (size_t)n_utts * c.spk_dim, cudaMemcpyHostToDevice, s));
+  MVB_CK(cudaMemcpyAsync(d_spk, spk_embs, sizeof(float) * (size_t)n_utts * c.spk_dim, cudaMemcpyHostToDevice, s));
   int rc = MVB_OK;
   size_t poff = 0;
   int max_budget = 0;
@@ -1012,8 +969,8 @@ extern "C" int mvb_s1_generate(mvb_s1* h, int32_t n_utts, const int32_t* prompts
     const int T = prompt_lens[i];
     int* di = d_idx + (size_t)i * 2 * c.block_size;
     // prompt.view(1,-1).repeat(2,1): both CFG rows see the same tokens (utils:211)
-    CK(cudaMemcpyAsync(di, prompts + poff, sizeof(int) * T, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(di + T, prompts + poff, sizeof(int) * T, cudaMemcpyHostToDevice, s));
+    MVB_CK(cudaMemcpyAsync(di, prompts + poff, sizeof(int) * T, cudaMemcpyHostToDevice, s));
+    MVB_CK(cudaMemcpyAsync(di + T, prompts + poff, sizeof(int) * T, cudaMemcpyHostToDevice, s));
     poff += T;
     if ((rc = mvb_s1_set_speaker(h, i, d_spk + (size_t)i * c.spk_dim, s))) break;
     mvb_sampling sp = params[i];
@@ -1037,7 +994,7 @@ extern "C" int mvb_s1_generate(mvb_s1* h, int32_t n_utts, const int32_t* prompts
     spp.decode_mode = 1;
     k_sample<<<1, SAMP_THREADS, 0, s>>>(spp, h->st);  // slot_map[0] == i after the prefill
     h->launches++;
-    if (cudaGetLastError() != cudaSuccess) { rc = fail(MVB_ERR_CUDA, "sampler launch failed"); break; }
+    if (cudaGetLastError() != cudaSuccess) { rc = set_error(MVB_ERR_CUDA, "sampler launch failed"); break; }
   }
   // decode_n_tokens: at most budget-1 further steps, all utterances advance together with their own positions;
   // per-utterance budgets and the end of the context are latched on the device (done flag).
@@ -1050,24 +1007,24 @@ extern "C" int mvb_s1_generate(mvb_s1* h, int32_t n_utts, const int32_t* prompts
       remaining -= burst;
       step0 += burst;
       if (rc) break;
-      CK(cudaMemcpyAsync(h->h_flags, h->st.done, sizeof(int) * n_utts, cudaMemcpyDeviceToHost, s));
-      CK(cudaStreamSynchronize(s));
+      MVB_CK(cudaMemcpyAsync(h->h_flags, h->st.done, sizeof(int) * n_utts, cudaMemcpyDeviceToHost, s));
+      MVB_CK(cudaStreamSynchronize(s));
       bool all = true;
       for (int i = 0; i < n_utts; ++i) all = all && h->h_flags[i];
       if (all) break;
     }
   }
   if (rc == MVB_OK) {
-    CK(cudaMemcpyAsync(h->h_flags, h->st.n_gen, sizeof(int) * n_utts, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
+    MVB_CK(cudaMemcpyAsync(h->h_flags, h->st.n_gen, sizeof(int) * n_utts, cudaMemcpyDeviceToHost, s));
+    MVB_CK(cudaStreamSynchronize(s));
     for (int i = 0; i < n_utts; ++i) {
       int n = h->h_flags[i];
       if (n > budget[i]) n = budget[i];
       out_lens[i] = n;
-      CK(cudaMemcpyAsync(out_tokens + (size_t)i * max_new_tokens, h->st.gen_tokens + (size_t)i * c.max_new, sizeof(int) * n,
+      MVB_CK(cudaMemcpyAsync(out_tokens + (size_t)i * max_new_tokens, h->st.gen_tokens + (size_t)i * c.max_new, sizeof(int) * n,
                          cudaMemcpyDeviceToHost, s));
     }
-    CK(cudaStreamSynchronize(s));
+    MVB_CK(cudaStreamSynchronize(s));
   }
   return rc;
 }
@@ -1079,15 +1036,15 @@ extern "C" int mvb_w4_gemv_test(int32_t epi, const void* d_W, const void* d_W3, 
                                 int32_t ldx, int32_t n_utts, const void* d_gain, float eps, float* d_out, int32_t ldo,
                                 void* d_kcache, void* d_vcache, const int32_t* d_slot_map, const int32_t* d_pos, int32_t H,
                                 int32_t S_max, int32_t D, int32_t kv_fp32, void* stream) {
-  if (!d_W || !d_x || !d_out || !d_slot_map || !d_pos) return fail(MVB_ERR_ARG, "null argument");
-  if (epi < EPI_STORE || epi > EPI_QKV) return fail(MVB_ERR_ARG, "bad epilogue %d", epi);
-  if (K < 256 || K % 256 || M < 2 || M % 2 || n_utts < 1 || n_utts > 64) return fail(MVB_ERR_ARG, "bad shape M=%d K=%d n_utts=%d", M, K, n_utts);
-  if ((size_t)2 * K * sizeof(float) > 48 * 1024) return fail(MVB_ERR_UNSUPPORTED, "K=%d exceeds the staging buffer", K);
-  if (epi == EPI_SWIGLU && !d_W3) return fail(MVB_ERR_ARG, "SwiGLU needs W3");
-  if (epi == EPI_QKV && (!d_kcache || !d_vcache || M != 3 * D || D != 128 * H)) return fail(MVB_ERR_ARG, "bad QKV arguments");
+  if (!d_W || !d_x || !d_out || !d_slot_map || !d_pos) return set_error(MVB_ERR_ARG, "null argument");
+  if (epi < EPI_STORE || epi > EPI_QKV) return set_error(MVB_ERR_ARG, "bad epilogue %d", epi);
+  if (K < 256 || K % 256 || M < 2 || M % 2 || n_utts < 1 || n_utts > 64) return set_error(MVB_ERR_ARG, "bad shape M=%d K=%d n_utts=%d", M, K, n_utts);
+  if ((size_t)2 * K * sizeof(float) > 48 * 1024) return set_error(MVB_ERR_UNSUPPORTED, "K=%d exceeds the staging buffer", K);
+  if (epi == EPI_SWIGLU && !d_W3) return set_error(MVB_ERR_ARG, "SwiGLU needs W3");
+  if (epi == EPI_QKV && (!d_kcache || !d_vcache || M != 3 * D || D != 128 * H)) return set_error(MVB_ERR_ARG, "bad QKV arguments");
   mvb_s1 h{};
-  h.n_sm = 132;
-  CK(cudaDeviceGetAttribute(&h.n_sm, cudaDevAttrMultiProcessorCount, 0));
+  int dev = 0;
+  if (int e = current_device(&dev, &h.n_sm)) return e;
   h.st.slot_map = const_cast<int*>(d_slot_map);
   h.st.pos = const_cast<int*>(d_pos);
   GemvP p{};
@@ -1097,27 +1054,27 @@ extern "C" int mvb_w4_gemv_test(int32_t epi, const void* d_W, const void* d_W3, 
   p.kcache = d_kcache; p.vcache = d_vcache; p.H = H; p.S_max = S_max; p.D = D; p.kv_fp32 = kv_fp32;
   cudaStream_t s = (cudaStream_t)stream;
   switch (epi) {
-    case EPI_STORE: CK(launch_gemv<EPI_STORE>(&h, s, n_utts, p, true)); break;
-    case EPI_RESID: CK(launch_gemv<EPI_RESID>(&h, s, n_utts, p, true)); break;
-    case EPI_SWIGLU: CK(launch_gemv<EPI_SWIGLU>(&h, s, n_utts, p, true)); break;
-    default: CK(launch_gemv<EPI_QKV>(&h, s, n_utts, p, true)); break;
+    case EPI_STORE: MVB_CK(launch_gemv<EPI_STORE>(&h, s, n_utts, p, true)); break;
+    case EPI_RESID: MVB_CK(launch_gemv<EPI_RESID>(&h, s, n_utts, p, true)); break;
+    case EPI_SWIGLU: MVB_CK(launch_gemv<EPI_SWIGLU>(&h, s, n_utts, p, true)); break;
+    default: MVB_CK(launch_gemv<EPI_QKV>(&h, s, n_utts, p, true)); break;
   }
-  CK(cudaStreamSynchronize(s));
+  MVB_CK(cudaStreamSynchronize(s));
   return MVB_OK;
 }
 
 extern "C" int mvb_w4_dequant_test(const void* d_W, int32_t M, int32_t K, void* d_out, void* stream) {
-  if (!d_W || !d_out) return fail(MVB_ERR_ARG, "null argument");
-  if (M < 1 || K < 256 || K % 256) return fail(MVB_ERR_ARG, "bad shape M=%d K=%d", M, K);
+  if (!d_W || !d_out) return set_error(MVB_ERR_ARG, "null argument");
+  if (M < 1 || K < 256 || K % 256) return set_error(MVB_ERR_ARG, "bad shape M=%d K=%d", M, K);
   W4Mats m{};
   m.src[0] = reinterpret_cast<const uint8_t*>(d_W);
   m.dst[0] = reinterpret_cast<__nv_bfloat16*>(d_out);
   m.M[0] = M; m.K[0] = K; m.n = 1;
-  int n_sm = 132;
-  CK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, 0));
+  int dev = 0, n_sm = 0;
+  if (int e = current_device(&dev, &n_sm)) return e;
   cudaStream_t s = (cudaStream_t)stream;
   k_w4_dequant<<<4 * n_sm, 256, 0, s>>>(m);
-  CK(cudaGetLastError());
-  CK(cudaStreamSynchronize(s));
+  MVB_CK(cudaGetLastError());
+  MVB_CK(cudaStreamSynchronize(s));
   return MVB_OK;
 }

@@ -8,22 +8,13 @@
 #include <cuda_runtime.h>
 
 #include <cstdlib>
-#include <string>
 #include <vector>
 
-#include "../../include/mvb200.h"
 #include "common.cuh"
+#include "host.cuh"
 #include "tc_gemm_host.cuh"
 
 using namespace mvb;
-namespace mvb { int set_error(int code, const char* fmt, ...); }
-
-#define SCK(expr)                                                                                    \
-  do {                                                                                               \
-    cudaError_t _e = (expr);                                                                         \
-    if (_e != cudaSuccess)                                                                           \
-      return mvb::set_error(MVB_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
-  } while (0)
 
 namespace {
 
@@ -252,40 +243,36 @@ struct mvb_s2 {
   int g_layer(int l, int t) const { return cfg.n_in + 3 + cfg.n_out + l * 7 + t; }
 };
 
-static size_t s2_align(size_t v) { return (v + 255) / 256 * 256; }
+struct S2Layout { size_t x, qkv, att, ffn, logits, spk, B, scratch, tickets, tokens, wte, idx, spk_stage, params, total; };
 
-static int s2_hidden(const mvb_s2_config* c) { return c->hidden; }
-
-static size_t s2_layout(const mvb_s2_config* c, size_t* o_x, size_t* o_qkv, size_t* o_att, size_t* o_ffn, size_t* o_logits, size_t* o_spk,
-                        size_t* o_B, size_t* o_scratch, size_t* o_tickets, size_t* o_tokens, size_t* o_wte, size_t* o_idx = nullptr,
-                        size_t* o_spkst = nullptr, size_t* o_prm = nullptr) {
-  const size_t rows = (size_t)c->max_batch * c->block_size, E = c->n_embd, Hd = s2_hidden(c);
+static S2Layout s2_layout(const mvb_s2_config* c) {
+  const size_t rows = (size_t)c->max_batch * c->block_size, E = c->n_embd, Hd = c->hidden;
   size_t vmax = 0;
   for (int i = 0; i < c->n_out; ++i) vmax = vmax > (size_t)c->vocab_out[i] ? vmax : (size_t)c->vocab_out[i];
-  size_t o = 0;
-  auto take = [&](size_t b) { size_t r = o; o = s2_align(o + b); return r; };
-  *o_x = take(rows * E * 4);
-  *o_qkv = take(rows * 3 * E * 4);
-  *o_att = take(rows * E * 4);
-  *o_ffn = take(rows * Hd * 4);
-  *o_logits = take((size_t)c->n_out * rows * vmax * 4);
-  *o_spk = take((size_t)c->max_batch * E * 4);
-  *o_B = take((size_t)2 * S2_ROWS * (Hd > E ? Hd : E) * 2);
+  S2Layout L;
+  WsBump ws;
+  L.x = ws.take(rows * E * 4);
+  L.qkv = ws.take(rows * 3 * E * 4);
+  L.att = ws.take(rows * E * 4);
+  L.ffn = ws.take(rows * Hd * 4);
+  L.logits = ws.take((size_t)c->n_out * rows * vmax * 4);
+  L.spk = ws.take((size_t)c->max_batch * E * 4);
+  L.B = ws.take((size_t)2 * S2_ROWS * (Hd > E ? Hd : E) * 2);
   size_t sc = 0;
   const size_t mats[5][3] = {{3 * E, E, 1}, {E, E, 1}, {Hd, E, 2}, {E, Hd, 1}, {vmax, E, 1}};
   for (auto& m : mats) {
     GemmPlan g = plan_gemm((int)m[0], (int)m[1], 2 * S2_ROWS, m[2] == 2, GEMM_MAX_SM);
     sc = sc > g.scratch_floats ? sc : g.scratch_floats;
   }
-  *o_scratch = take(sc * 4);
-  *o_tickets = take(256 * 4);
-  *o_tokens = take((size_t)c->n_out * rows * 4);
-  *o_wte = take(16 * sizeof(void*));
-  const size_t a = take((size_t)c->max_batch * c->n_in * c->block_size * 4), b2 = take((size_t)c->max_batch * c->spk_dim * 4), p3 = take(256);
-  if (o_idx) *o_idx = a;
-  if (o_spkst) *o_spkst = b2;
-  if (o_prm) *o_prm = p3;
-  return o;
+  L.scratch = ws.take(sc * 4);
+  L.tickets = ws.take(256 * 4);
+  L.tokens = ws.take((size_t)c->n_out * rows * 4);
+  L.wte = ws.take(16 * sizeof(void*));
+  L.idx = ws.take((size_t)c->max_batch * c->n_in * c->block_size * 4);
+  L.spk_stage = ws.take((size_t)c->max_batch * c->spk_dim * 4);
+  L.params = ws.take(256);
+  L.total = ws.end;
+  return L;
 }
 
 static int s2_validate(const mvb_s2_config* c) {
@@ -302,37 +289,34 @@ static int s2_validate(const mvb_s2_config* c) {
 
 extern "C" size_t mvb_s2_workspace_bytes(const mvb_s2_config* c) {
   if (s2_validate(c)) return 0;
-  size_t a, b, cc, d, e, f, g, h, i, j, k;
-  return s2_layout(c, &a, &b, &cc, &d, &e, &f, &g, &h, &i, &j, &k);
+  return s2_layout(c).total;
 }
 
 extern "C" int mvb_s2_create(const mvb_s2_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets, void* d_ws,
                              mvb_s2** out) {
   if (int e = s2_validate(cfg)) return e;
   if (!d_arena || !offsets || !d_ws || !out) return mvb::set_error(MVB_ERR_ARG, "null pointer argument");
-  mvb_s2* h = new mvb_s2();
+  const int n_off = cfg->n_in + 3 + cfg->n_out + 7 * cfg->n_layer;
+  if (int e = check_offsets(offsets, n_off, arena_bytes, "stage 2: weight offset")) return e;
+  Building<mvb_s2> hb(new mvb_s2(), mvb_s2_destroy);
+  mvb_s2* h = hb.get();
   h->cfg = *cfg;
   h->hidden = cfg->hidden;
   int dev = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, dev);
+  if (int e = current_device(&dev, &h->n_sm)) return e;
   h->arena = reinterpret_cast<const char*>(d_arena);
-  const int n_off = cfg->n_in + 3 + cfg->n_out + 7 * cfg->n_layer;
   h->off.assign(offsets, offsets + n_off);
-  for (uint64_t o : h->off)
-    if (o % 16 || o >= arena_bytes) { delete h; return mvb::set_error(MVB_ERR_ARG, "bad weight offset"); }
   h->ws = reinterpret_cast<char*>(d_ws);
-  size_t ox, oq, oa, of, ol, os, oB, osc, ot, otok, ow, oidx, ospk, oprm;
-  s2_layout(cfg, &ox, &oq, &oa, &of, &ol, &os, &oB, &osc, &ot, &otok, &ow, &oidx, &ospk, &oprm);
-  h->idx_stage = (int*)(h->ws + oidx); h->spk_stage = (float*)(h->ws + ospk); h->params = (S2SampleParams*)(h->ws + oprm);
+  const S2Layout L = s2_layout(cfg);
+  h->idx_stage = (int*)(h->ws + L.idx); h->spk_stage = (float*)(h->ws + L.spk_stage); h->params = (S2SampleParams*)(h->ws + L.params);
   h->use_graph = getenv("MVB_S2_NO_GRAPH") == nullptr;
-  h->x = (float*)(h->ws + ox); h->qkv = (float*)(h->ws + oq); h->att = (float*)(h->ws + oa); h->ffn = (float*)(h->ws + of);
-  h->logits = (float*)(h->ws + ol); h->spk_proj = (float*)(h->ws + os); h->B = (__nv_bfloat16*)(h->ws + oB);
-  h->scratch = (float*)(h->ws + osc); h->tickets = (unsigned*)(h->ws + ot); h->tokens = (int*)(h->ws + otok);
-  h->wte_dev = (const __nv_bfloat16**)(h->ws + ow);
+  h->x = (float*)(h->ws + L.x); h->qkv = (float*)(h->ws + L.qkv); h->att = (float*)(h->ws + L.att); h->ffn = (float*)(h->ws + L.ffn);
+  h->logits = (float*)(h->ws + L.logits); h->spk_proj = (float*)(h->ws + L.spk); h->B = (__nv_bfloat16*)(h->ws + L.B);
+  h->scratch = (float*)(h->ws + L.scratch); h->tickets = (unsigned*)(h->ws + L.tickets); h->tokens = (int*)(h->ws + L.tokens);
+  h->wte_dev = (const __nv_bfloat16**)(h->ws + L.wte);
   std::vector<const __nv_bfloat16*> wte(cfg->n_in);
   for (int i = 0; i < cfg->n_in; ++i) wte[i] = h->w(i);
-  SCK(cudaMemcpy(h->wte_dev, wte.data(), sizeof(void*) * cfg->n_in, cudaMemcpyHostToDevice));
+  MVB_CK(cudaMemcpy(h->wte_dev, wte.data(), sizeof(void*) * cfg->n_in, cudaMemcpyHostToDevice));
   const int E = cfg->n_embd, Hd = h->hidden;
   h->tmW.resize((size_t)cfg->n_layer * 5 + cfg->n_out);
   bool ok = true;
@@ -347,13 +331,11 @@ extern "C" int mvb_s2_create(const mvb_s2_config* cfg, const void* d_arena, size
     ok = ok && make_tmap_bf16(&h->tmW[(size_t)cfg->n_layer * 5 + i], h->w(h->g_head(i)), cfg->vocab_out[i], E, 128);
   ok = ok && make_tmap_bf16(&h->tmB_E, h->B, 2 * S2_ROWS, E, 2 * S2_ROWS);
   ok = ok && make_tmap_bf16(&h->tmB_H, h->B, 2 * S2_ROWS, Hd, 2 * S2_ROWS);
-  if (!ok) { delete h; return mvb::set_error(MVB_ERR_CUDA, "cuTensorMapEncodeTiled failed (stage 2)"); }
+  if (!ok) return mvb::set_error(MVB_ERR_CUDA, "cuTensorMapEncodeTiled failed (stage 2)");
   if (cudaStreamCreateWithFlags(&h->cap_stream, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaMallocHost(&h->h_params, sizeof(S2SampleParams)) != cudaSuccess) {
-    delete h;
+      cudaMallocHost(&h->h_params, sizeof(S2SampleParams)) != cudaSuccess)
     return mvb::set_error(MVB_ERR_CUDA, "stage 2: stream / pinned buffer allocation failed");
-  }
-  *out = h;
+  *out = hb.release();
   return MVB_OK;
 }
 
@@ -381,8 +363,8 @@ extern "C" int mvb_s2_attn_test(const float* d_qkv, int32_t B, int32_t t, int32_
   if (B < 1 || t < 1 || n_head < 1 || E != n_head * (E / n_head) || (E / n_head != 64 && E / n_head != 128))
     return mvb::set_error(MVB_ERR_UNSUPPORTED, "mvb_s2_attn_test: B, t >= 1 and head size E / n_head of 64 or 128 required");
   cudaStream_t s = (cudaStream_t)stream;
-  SCK(launch_s2_attn(s, d_qkv, d_out, B, t, E, n_head));
-  SCK(cudaStreamSynchronize(s));
+  MVB_CK(launch_s2_attn(s, d_qkv, d_out, B, t, E, n_head));
+  MVB_CK(cudaStreamSynchronize(s));
   return MVB_OK;
 }
 
@@ -399,8 +381,8 @@ extern "C" int mvb_s2_sample_test(const float* d_logits, int32_t n_hier, int32_t
   if (n_hier < 1 || n_rows < 1 || V < 1 || V > S2_PAD)
     return mvb::set_error(MVB_ERR_UNSUPPORTED, "mvb_s2_sample_test: n_hier, n_rows >= 1 and 1 <= V <= %d required", S2_PAD);
   cudaStream_t s = (cudaStream_t)stream;
-  SCK(launch_s2_sample(s, d_logits, V, reinterpret_cast<const S2SampleParams*>(d_params), d_noise, d_tokens, n_rows, n_hier));
-  SCK(cudaStreamSynchronize(s));
+  MVB_CK(launch_s2_sample(s, d_logits, V, reinterpret_cast<const S2SampleParams*>(d_params), d_noise, d_tokens, n_rows, n_hier));
+  MVB_CK(cudaStreamSynchronize(s));
   return MVB_OK;
 }
 
@@ -419,7 +401,7 @@ static int s2_linear(mvb_s2* h, cudaStream_t s, int rows, const float* x, int ld
     g.R = rows - r0 < S2_ROWS ? rows - r0 : S2_ROWS;
     g.x = x + (size_t)r0 * ldx;
     g.out = out + (size_t)r0 * ldo;
-    SCK(tc_gemm(s, g));
+    MVB_CK(tc_gemm(s, g));
   }
   return MVB_OK;
 }
@@ -428,16 +410,16 @@ static int s2_linear(mvb_s2* h, cudaStream_t s, int rows, const float* x, int ld
 static int s2_body(mvb_s2* h, cudaStream_t s, int batch, bool has_spk, const float* d_noise) {
   const mvb_s2_config& c = h->cfg;
   const int t = c.block_size, rows = batch * t, E = c.n_embd, Hd = h->hidden;
-  SCK(cudaMemsetAsync(h->tickets, 0, 256 * 4, s));
+  MVB_CK(cudaMemsetAsync(h->tickets, 0, 256 * 4, s));
   if (has_spk) {
     k_s2_spk<<<dim3((E * 32 + 255) / 256, batch), 256, 0, s>>>(h->w(h->g_spk()), h->spk_stage, h->spk_proj, E, c.spk_dim);
-    SCK(cudaGetLastError());
+    MVB_CK(cudaGetLastError());
   }
   k_s2_embed<<<rows, 128, 0, s>>>(h->idx_stage, c.n_in, t, h->wte_dev, h->w(h->g_wpe()), has_spk ? h->spk_proj : nullptr, h->x, E);
-  SCK(cudaGetLastError());
+  MVB_CK(cudaGetLastError());
   for (int l = 0; l < c.n_layer; ++l) {
     if (int e = s2_linear<G_STORE>(h, s, rows, h->x, E, h->w(h->g_layer(l, 0)), l * 5 + 0, l * 5 + 0, 3 * E, E, h->qkv, 3 * E)) return e;
-    SCK(launch_s2_attn(s, h->qkv, h->att, batch, t, E, c.n_head));
+    MVB_CK(launch_s2_attn(s, h->qkv, h->att, batch, t, E, c.n_head));
     if (int e = s2_linear<G_RESID>(h, s, rows, h->att, E, nullptr, l * 5 + 1, l * 5 + 1, E, E, h->x, E)) return e;
     if (int e = s2_linear<G_SWIGLU>(h, s, rows, h->x, E, h->w(h->g_layer(l, 3)), l * 5 + 2, l * 5 + 3, Hd, E, h->ffn, Hd)) return e;
     if (int e = s2_linear<G_RESID>(h, s, rows, h->ffn, Hd, nullptr, l * 5 + 4, l * 5 + 4, E, Hd, h->x, E)) return e;
@@ -447,7 +429,7 @@ static int s2_body(mvb_s2* h, cudaStream_t s, int batch, bool has_spk, const flo
     const int hw = c.n_layer * 5 + i;
     if (int e = s2_linear<G_STORE>(h, s, rows, h->x, E, h->w(h->g_lnf()), hw, hw, vmax, E, h->logits + (size_t)i * rows * vmax, vmax)) return e;
   }
-  SCK(launch_s2_sample(s, h->logits, vmax, h->params, d_noise, h->tokens, rows, c.n_out));
+  MVB_CK(launch_s2_sample(s, h->logits, vmax, h->params, d_noise, h->tokens, rows, c.n_out));
   return MVB_OK;
 }
 
@@ -464,32 +446,26 @@ extern "C" int mvb_s2_forward(mvb_s2* h, int32_t batch, const int32_t* d_idx, co
   const size_t vmax = c.vocab_out[0];
   // inputs -> internal staging buffers: the forward pass itself (~500 small launches: 8 passes of 128 rows per Linear)
   // only touches library memory and is replayed as ONE CUDA graph per (batch, speaker) signature
-  SCK(cudaMemcpyAsync(h->idx_stage, d_idx, sizeof(int) * (size_t)batch * c.n_in * t, cudaMemcpyDeviceToDevice, s));
-  if (d_spk) SCK(cudaMemcpyAsync(h->spk_stage, d_spk, sizeof(float) * (size_t)batch * c.spk_dim, cudaMemcpyDeviceToDevice, s));
-  SCK(cudaStreamSynchronize(s));            // h_params is reused across calls: the previous upload must have been consumed
+  MVB_CK(cudaMemcpyAsync(h->idx_stage, d_idx, sizeof(int) * (size_t)batch * c.n_in * t, cudaMemcpyDeviceToDevice, s));
+  if (d_spk) MVB_CK(cudaMemcpyAsync(h->spk_stage, d_spk, sizeof(float) * (size_t)batch * c.spk_dim, cudaMemcpyDeviceToDevice, s));
+  MVB_CK(cudaStreamSynchronize(s));            // h_params is reused across calls: the previous upload must have been consumed
   h->h_params->temperature = temperature; h->h_params->top_k = top_k; h->h_params->seed = seed;
-  SCK(cudaMemcpyAsync(h->params, h->h_params, sizeof(S2SampleParams), cudaMemcpyHostToDevice, s));
+  MVB_CK(cudaMemcpyAsync(h->params, h->h_params, sizeof(S2SampleParams), cudaMemcpyHostToDevice, s));
   if (h->use_graph && d_noise == nullptr) {
     cudaGraphExec_t& ge = h->graphs[d_spk ? 1 : 0][batch];
     if (!ge) {
-      cudaGraph_t g;
-      SCK(cudaStreamBeginCapture(h->cap_stream, cudaStreamCaptureModeThreadLocal));
-      const int e = s2_body(h, h->cap_stream, batch, d_spk != nullptr, nullptr);
-      const cudaError_t ce = cudaStreamEndCapture(h->cap_stream, &g);
-      if (e) return e;
-      SCK(ce);
-      SCK(cudaGraphInstantiate(&ge, g, 0));
-      SCK(cudaGraphDestroy(g));
+      auto body = [&](cudaStream_t cs) { return s2_body(h, cs, batch, d_spk != nullptr, nullptr); };
+      if (int e = capture_graph(h->cap_stream, &ge, body)) return e;
     }
-    SCK(cudaGraphLaunch(ge, s));
+    MVB_CK(cudaGraphLaunch(ge, s));
   } else {
     if (int e = s2_body(h, s, batch, d_spk != nullptr, d_noise)) return e;
   }
   // tokens [n_out, batch*t] -> caller layout [batch, n_out, t]
   for (int b = 0; b < batch; ++b)
     for (int i = 0; i < c.n_out; ++i)
-      SCK(cudaMemcpyAsync(d_tokens + ((size_t)b * c.n_out + i) * t, h->tokens + (size_t)i * rows + (size_t)b * t, sizeof(int) * t,
+      MVB_CK(cudaMemcpyAsync(d_tokens + ((size_t)b * c.n_out + i) * t, h->tokens + (size_t)i * rows + (size_t)b * t, sizeof(int) * t,
                           cudaMemcpyDeviceToDevice, s));
-  if (d_logits_out) SCK(cudaMemcpyAsync(d_logits_out, h->logits, sizeof(float) * c.n_out * rows * vmax, cudaMemcpyDeviceToDevice, s));
+  if (d_logits_out) MVB_CK(cudaMemcpyAsync(d_logits_out, h->logits, sizeof(float) * c.n_out * rows * vmax, cudaMemcpyDeviceToDevice, s));
   return MVB_OK;
 }

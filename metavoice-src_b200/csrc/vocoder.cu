@@ -11,18 +11,10 @@
 
 #include <vector>
 
-#include "../../include/mvb200.h"
 #include "common.cuh"
+#include "host.cuh"
 
 using namespace mvb;
-namespace mvb { int set_error(int code, const char* fmt, ...); }
-
-#define VCK(expr)                                                                                    \
-  do {                                                                                               \
-    cudaError_t _e = (expr);                                                                         \
-    if (_e != cudaSuccess)                                                                           \
-      return mvb::set_error(MVB_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
-  } while (0)
 
 namespace {
 
@@ -288,25 +280,27 @@ struct mvb_voc {
 //   per ratio: up {w,b}, res.c1 {w,b}, res.c2 {w,b}, res.shortcut {w,b} | conv_out {w,b}
 static int voc_n_tensors(const mvb_voc_config* c) { return c->n_q + 2 + 6 + c->n_ratios * 8 + 2; }
 
-static size_t voc_layout(const mvb_voc_config* c, size_t* oA, size_t* oB, size_t* oC, size_t* oPre, size_t* oH, size_t* oBar, size_t* oBooks) {
-  size_t T = c->max_frames, maxelems = (size_t)c->hidden * c->n_filters / c->n_filters * T;  // placeholder, refined below
+struct VocLayout { size_t A, B, C, pre, h, bar, books, total; };
+
+static VocLayout voc_layout(const mvb_voc_config* c) {
+  const size_t T = c->max_frames;
   int ch = c->n_filters << c->n_ratios;   // 512
-  maxelems = (size_t)ch * T;
-  size_t Tl = T;
+  size_t maxelems = (size_t)ch * T, Tl = T;
   for (int i = 0; i < c->n_ratios; ++i) {
     Tl *= c->ratios[i];
     ch >>= 1;
     if ((size_t)ch * Tl > maxelems) maxelems = (size_t)ch * Tl;
   }
   const size_t top = (size_t)(c->n_filters << c->n_ratios);
-  size_t o = 0;
-  auto take = [&](size_t b) { size_t r = o; o = (o + b + 255) / 256 * 256; return r; };
-  *oA = take(maxelems * 4); *oB = take(maxelems * 4); *oC = take(maxelems * 4);
-  *oPre = take(4 * top * T * 4);
-  *oH = take(2 * top * 4);
-  *oBar = take(256);
-  *oBooks = take(64 * sizeof(void*));
-  return o;
+  VocLayout L;
+  WsBump ws;
+  L.A = ws.take(maxelems * 4); L.B = ws.take(maxelems * 4); L.C = ws.take(maxelems * 4);
+  L.pre = ws.take(4 * top * T * 4);
+  L.h = ws.take(2 * top * 4);
+  L.bar = ws.take(256);
+  L.books = ws.take(64 * sizeof(void*));
+  L.total = ws.end;
+  return L;
 }
 
 static int voc_validate(const mvb_voc_config* c) {
@@ -324,29 +318,27 @@ static int voc_validate(const mvb_voc_config* c) {
 
 extern "C" size_t mvb_voc_workspace_bytes(const mvb_voc_config* c) {
   if (voc_validate(c)) return 0;
-  size_t a, b, cc, d, e, f, g;
-  return voc_layout(c, &a, &b, &cc, &d, &e, &f, &g);
+  return voc_layout(c).total;
 }
 
 extern "C" int mvb_voc_create(const mvb_voc_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets, void* d_ws,
                               mvb_voc** out) {
   if (int e = voc_validate(cfg)) return e;
   if (!d_arena || !offsets || !d_ws || !out) return mvb::set_error(MVB_ERR_ARG, "null pointer argument");
-  mvb_voc* h = new mvb_voc();
+  if (int e = check_offsets(offsets, voc_n_tensors(cfg), arena_bytes, "vocoder: weight offset")) return e;
+  Building<mvb_voc> hb(new mvb_voc(), mvb_voc_destroy);
+  mvb_voc* h = hb.get();
   h->cfg = *cfg;
   h->arena = reinterpret_cast<const char*>(d_arena);
   h->off.assign(offsets, offsets + voc_n_tensors(cfg));
-  for (uint64_t o : h->off)
-    if (o % 16 || o >= arena_bytes) { delete h; return mvb::set_error(MVB_ERR_ARG, "bad weight offset"); }
   h->ws = reinterpret_cast<char*>(d_ws);
-  size_t oA, oB, oC, oP, oH, oBar, oBk;
-  voc_layout(cfg, &oA, &oB, &oC, &oP, &oH, &oBar, &oBk);
-  h->bufA = (float*)(h->ws + oA); h->bufB = (float*)(h->ws + oB); h->bufC = (float*)(h->ws + oC); h->pre = (float*)(h->ws + oP);
-  h->hbuf = (float*)(h->ws + oH); h->bar = (unsigned*)(h->ws + oBar); h->books_dev = (const float**)(h->ws + oBk);
+  const VocLayout L = voc_layout(cfg);
+  h->bufA = (float*)(h->ws + L.A); h->bufB = (float*)(h->ws + L.B); h->bufC = (float*)(h->ws + L.C); h->pre = (float*)(h->ws + L.pre);
+  h->hbuf = (float*)(h->ws + L.h); h->bar = (unsigned*)(h->ws + L.bar); h->books_dev = (const float**)(h->ws + L.books);
   std::vector<const float*> books(cfg->n_q);
   for (int q = 0; q < cfg->n_q; ++q) books[q] = h->w(q);
-  VCK(cudaMemcpy(h->books_dev, books.data(), sizeof(void*) * cfg->n_q, cudaMemcpyHostToDevice));
-  *out = h;
+  MVB_CK(cudaMemcpy(h->books_dev, books.data(), sizeof(void*) * cfg->n_q, cudaMemcpyHostToDevice));
+  *out = hb.release();
   return MVB_OK;
 }
 
@@ -367,7 +359,7 @@ extern "C" int mvb_voc_decode_latent(mvb_voc* h, const int32_t* d_codes, int32_t
   if (!h || !d_codes || !d_latent) return mvb::set_error(MVB_ERR_ARG, "null argument");
   if (T < 1 || T > h->cfg.max_frames) return mvb::set_error(MVB_ERR_ARG, "frame count %d out of range", T);
   k_rvq_decode<<<dim3((T + 31) / 32, 1), 128, 0, (cudaStream_t)stream>>>(d_codes, h->cfg.n_q, T, h->books_dev, h->cfg.hidden, d_latent);
-  VCK(cudaGetLastError());
+  MVB_CK(cudaGetLastError());
   return MVB_OK;
 }
 
@@ -381,19 +373,19 @@ extern "C" int mvb_voc_decode(mvb_voc* h, const int32_t* d_codes, int32_t T, flo
   int ti = c.n_q;
   float *A = h->bufA, *B = h->bufB, *Cc = h->bufC;
   if (int e = mvb_voc_decode_latent(h, d_codes, T, A, stream)) return e;
-  VCK(conv<7>(s, A, c.hidden, T, h->w(ti), h->w(ti + 1), B, top, 0, 0));      // conv_in
+  MVB_CK(conv<7>(s, A, c.hidden, T, h->w(ti), h->w(ti + 1), B, top, 0, 0));      // conv_in
   ti += 2;
   // LSTM: x = B;  layer 0 -> A ; layer 1 (+ skip x) -> Cc
   const size_t lsmem = (size_t)(16 * top + top) * 4;
   static PerDeviceOnce attr;
-  if (attr.pending()) { VCK(cudaFuncSetAttribute(k_lstm_layer, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024)); attr.mark(); }
+  if (attr.pending()) { MVB_CK(cudaFuncSetAttribute(k_lstm_layer, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024)); attr.mark(); }
   const float* lin = B;
   float* louts[2] = {A, Cc};
   for (int l = 0; l < 2; ++l) {
-    VCK(conv<1>(s, lin, top, T, h->w(ti), h->w(ti + 2), h->pre, 4 * top, 0, 0));   // W_ih x + (b_ih + b_hh)
-    VCK(cudaMemsetAsync(h->bar, 0, 4, s));
+    MVB_CK(conv<1>(s, lin, top, T, h->w(ti), h->w(ti + 2), h->pre, 4 * top, 0, 0));   // W_ih x + (b_ih + b_hh)
+    MVB_CK(cudaMemsetAsync(h->bar, 0, 4, s));
     k_lstm_layer<<<top / 4, 128, lsmem, s>>>(h->pre, h->w(ti + 1), top, T, h->hbuf, h->bar, louts[l], l == 1 ? B : nullptr);
-    VCK(cudaGetLastError());
+    MVB_CK(cudaGetLastError());
     lin = louts[l];
     ti += 3;
   }
@@ -405,14 +397,14 @@ extern "C" int mvb_voc_decode(mvb_voc* h, const int32_t* d_codes, int32_t T, flo
     const int r = c.ratios[i], co = ch / 2;
     const size_t smem = (size_t)(16 * 33 + 16 * 32 * 2 * r) * 4;
     k_convtr1d<<<dim3((Tl + 31) / 32, (co + 31) / 32, 1), 256, smem, s>>>(x, ch, Tl, h->w(ti), h->w(ti + 1), f1, co, r);
-    VCK(cudaGetLastError());
+    MVB_CK(cudaGetLastError());
     Tl *= r; ch = co;
     // resnet block: y = shortcut(u) + conv_k1(elu(conv_k3(elu(u))))
-    VCK(conv<3>(s, f1, ch, Tl, h->w(ti + 2), h->w(ti + 3), f2, ch / c.compress, 1, 0));
-    VCK(conv<1>(s, f1, ch, Tl, h->w(ti + 6), h->w(ti + 7), x, ch, 0, 0));
-    VCK(conv<1>(s, f2, ch / c.compress, Tl, h->w(ti + 4), h->w(ti + 5), x, ch, 1, 1));
+    MVB_CK(conv<3>(s, f1, ch, Tl, h->w(ti + 2), h->w(ti + 3), f2, ch / c.compress, 1, 0));
+    MVB_CK(conv<1>(s, f1, ch, Tl, h->w(ti + 6), h->w(ti + 7), x, ch, 0, 0));
+    MVB_CK(conv<1>(s, f2, ch / c.compress, Tl, h->w(ti + 4), h->w(ti + 5), x, ch, 1, 1));
     ti += 8;
   }
-  VCK(conv<7>(s, x, ch, Tl, h->w(ti), h->w(ti + 1), d_wav, 1, 1, 0));
+  MVB_CK(conv<7>(s, x, ch, Tl, h->w(ti), h->w(ti + 1), d_wav, 1, 1, 0));
   return MVB_OK;
 }

@@ -229,6 +229,22 @@ def test_end_of_audio_latch_and_errors(tiny_sd):
     assert torch.isfinite(out).all()
 
 
+def test_fetch_sampled_rejects_a_slice_outside_the_slot(tiny_sd):
+    """mvb_s1_fetch_sampled copies `cap` tokens of slot `utt`: a slot past max_utts or a cap past max_new would read
+    outside that slot's slice of the sampled-token buffer, so both are argument errors."""
+    import ctypes as C
+    from mvb200 import _lib
+    m = _mk(synth.TINY, tiny_sd, "fp32", utts=2, max_new=16)
+    lib, h, st = m._lib, m.handle, m._stream()
+    out = np.zeros(17, dtype=np.int32)
+    dst = out.ctypes.data_as(C.c_void_p)
+    _lib.check(lib.mvb_s1_fetch_sampled(h, 1, dst, 16, st))
+    with pytest.raises(ValueError, match="utterance slot 2"):
+        _lib.check(lib.mvb_s1_fetch_sampled(h, 2, dst, 16, st))
+    with pytest.raises(ValueError, match="cap 17"):
+        _lib.check(lib.mvb_s1_fetch_sampled(h, 0, dst, 17, st))
+
+
 def test_full_size_logits_vs_reference_golden(golden_dir, full_sd):
     """The 1.2 B configuration BASELINE.json quotes, against logits the reference's own Transformer produced in
     fp32 (prefill T=32 and teacher-forced decode steps 1, 8, 64)."""
