@@ -226,6 +226,23 @@ int mvb_mbd_conv_test(int32_t kind, const float* d_x, int32_t Cin, int32_t Tin, 
                       int32_t stride, int32_t dil, int32_t pad, const float* d_gn_stats, const float* d_gn_w,
                       const float* d_gn_b, int32_t groups, const float* d_bias, const float* d_emb, const float* d_resid,
                       float* d_y, int32_t use_tc, void* stream);
+/* Test hooks for the EnCodec decoder and audio post-processing kernels (not part of the drop-in surface):
+ *   mvb_voc_op_test     : one launch of csrc/vocoder.cu exactly as mvb_voc_decode makes it.  op 0: k_conv1d<k>, k = 1 / 3 / 7,
+ *                         d_x [Cin, T] -> d_y [Cout, T], d_w [Cout, Cin, k], d_b [Cout] or NULL, ELU on the input when
+ *                         elu_in, added to d_y when accumulate; op 1: k_convtr1d (ELU fused) at ratio r = k in 1..8,
+ *                         d_x [Cin, T] -> d_y [Cout, T r], d_w [Cin, Cout, 2 r], d_b [Cout]; op 2: k_lstm_layer, H = Cin
+ *                         (H % 32 == 0, its H / 4 CTAs co-resident), d_x = pre [4 H, T], d_w = W_hh [4 H, H], d_skip
+ *                         [H, T] or NULL, d_y [H, T].  Scratch (h exchange, barrier word) is allocated per call.
+ *   mvb_audio_post_test : mvb_audio_post with a workspace of its own, plus the K-weighted signal d_y fp32 [n_samples],
+ *                         the block energies d_energy fp32 [n_blocks + 1] (the last entry: sum of x^2 over the whole
+ *                         signal) and d_res fp32 [3] = {LKFS, gain, compressor flag}; *n_blocks_out (host) = number of
+ *                         complete 400 ms gating blocks.
+ * Both synchronise `stream`. */
+int mvb_voc_op_test(int32_t op, const float* d_x, int32_t Cin, int32_t T, const float* d_w, const float* d_b, int32_t Cout,
+                    int32_t k, int32_t elu_in, int32_t accumulate, const float* d_skip, float* d_y, void* stream);
+int mvb_audio_post_test(const float* d_wav, int32_t n_samples, int32_t sample_rate, float loudness_headroom_db,
+                        int32_t loudness_compressor, int16_t* d_pcm16, float* d_wav_out, float* d_y, float* d_energy,
+                        float* d_res, int32_t* n_blocks_out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Stage 2: the non-causal codebook-expansion model (fam/llm/model.py:195-314 with causal=False) and its sampler
@@ -374,7 +391,12 @@ int mvb_spk_embed(mvb_spk* h, const float* d_wav, int32_t n_samples, const int32
  * audio_write(strategy="loudness", loudness_compressor=True)): BS.1770-4 integrated loudness exactly as
  * torchaudio.functional.loudness computes it (the function audiocraft calls), gain to -loudness_headroom_db LUFS, tanh
  * compressor, clip, PCM16.  d_wav fp32 mono [n_samples]; d_pcm16 int16 [n_samples]; d_wav_out optional fp32 [n_samples];
- * d_lkfs_gain optional fp32 [2] = {measured LKFS, applied linear gain}.  Signals below the 2e-3 RMS floor pass through. */
+ * d_lkfs_gain optional fp32 [2] = {measured LKFS, applied linear gain}.  Edge cases:
+ *   LKFS = -inf: the RMS is below the 2e-3 energy floor; gain 1, no compressor (the signal passes through, clipped).
+ *   LKFS = NaN : the meter is undefined -- a non-finite sample, no complete 400 ms block, or every block below the
+ *                -70 LKFS gate (where torchaudio raises or returns NaN and audiocraft's normalize_loudness fails); gain 1,
+ *                no compressor, NaN samples written as 0.  Callers that mirror the host writer must raise here.
+ * n_samples beyond 15,996 gating blocks returns MVB_ERR_UNSUPPORTED before anything is launched. */
 size_t mvb_audio_post_workspace_bytes(int32_t max_samples);
 int mvb_audio_post(const float* d_wav, int32_t n_samples, int32_t sample_rate, float loudness_headroom_db,
                    int32_t loudness_compressor, void* d_workspace, int16_t* d_pcm16, float* d_wav_out,

@@ -6,8 +6,9 @@
 // The waveform never leaves the device as fp32; the caller gets 16-bit samples (and the measured loudness).
 //
 // The two K-weighting biquads are recursive; they are evaluated in independent chunks, each warmed up over the
-// preceding 4096 samples from a zero state (the slowest pole, the 38 Hz high-pass at 24 kHz, has decayed by e^-40 by
-// then), so the filter runs in ~6 K sequential steps instead of T.
+// preceding 4096 samples from a zero state (the slowest section, the 38 Hz high-pass, is a near-double pole whose impulse
+// response there is 1.0e-14 at 24 kHz and 6e-6 at 48 kHz; tests/test_audio_post_ops_gpu.py), so the filter runs in
+// ~6 K sequential steps instead of T.
 #include <cuda_runtime.h>
 #include <math.h>
 
@@ -60,32 +61,40 @@ __global__ void __launch_bounds__(256) k_block_energy(const float* __restrict__ 
   }
 }
 
-// gating + gain (one thread: <= a few hundred blocks).  out[0] = LKFS, out[1] = linear gain (1 when the signal is
-// below the energy floor, as audiocraft's normalize_loudness leaves it untouched; the compressor is skipped too: out[2] = 0)
+// gating + gain (one thread: <= 16000 blocks).  out[0] = LKFS, out[1] = linear gain, out[2] = 1 when the compressor may
+// run.  Below the energy floor: LKFS = -inf, gain 1, no compressor (audiocraft's normalize_loudness leaves the signal
+// untouched).  Where the meter is undefined -- non-finite input, no complete block, or every block gated (torchaudio
+// returns NaN or raises there, and normalize_loudness fails its finiteness assert) -- LKFS = NaN, gain 1, no compressor,
+// so that no NaN reaches the PCM.
 __global__ void k_loudness_gain(const float* __restrict__ energy, int n_blocks, int T, float headroom_db, float energy_floor,
                                 float* __restrict__ out) {
   if (threadIdx.x != 0) return;
+  out[1] = 1.f; out[2] = 0.f;
   const float rms = sqrtf(energy[n_blocks] / (float)T);
-  if (rms < energy_floor || n_blocks < 1) { out[0] = -INFINITY; out[1] = 1.f; out[2] = 0.f; return; }
+  if (!isfinite(rms)) { out[0] = NAN; return; }
+  if (rms < energy_floor) { out[0] = -INFINITY; return; }
   const float bias = -0.691f, gamma_abs = -70.f;
   float sum = 0.f; int cnt = 0;
   for (int b = 0; b < n_blocks; ++b) {
     const float l = bias + 10.f * log10f(energy[b]);
     if (l > gamma_abs) { sum += energy[b]; ++cnt; }
   }
+  if (cnt == 0) { out[0] = NAN; return; }
   const float gamma_rel = bias + 10.f * log10f(sum / (float)cnt) - 10.f;
   sum = 0.f; cnt = 0;
   for (int b = 0; b < n_blocks; ++b) {
     const float l = bias + 10.f * log10f(energy[b]);
     if (l > gamma_abs && l > gamma_rel) { sum += energy[b]; ++cnt; }
   }
+  if (cnt == 0) { out[0] = NAN; return; }
   const float lkfs = bias + 10.f * log10f(sum / (float)cnt);
   out[0] = lkfs;
   out[1] = powf(10.f, (-headroom_db - lkfs) / 20.f);
   out[2] = 1.f;
 }
 
-// out = clip(tanh(gain * x)) -> PCM16 (round to nearest even, like numpy's round in audio_out.py / torchaudio.save)
+// out = clip(tanh(gain * x)) -> PCM16 (round to nearest even, like numpy's round in audio_out.py / torchaudio.save).
+// A NaN sample is written as 0 (fmaxf would otherwise turn it into -1).
 __global__ void __launch_bounds__(256) k_apply_pcm16(const float* __restrict__ x, int T, const float* __restrict__ g, int compressor,
                                                      short* __restrict__ pcm, float* __restrict__ wav_out) {
   const float gain = g[1];
@@ -93,7 +102,7 @@ __global__ void __launch_bounds__(256) k_apply_pcm16(const float* __restrict__ x
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < T; i += gridDim.x * blockDim.x) {
     float v = gain * x[i];
     if (comp) v = tanhf(v);
-    v = fminf(fmaxf(v, -1.f), 1.f);
+    v = isnan(v) ? 0.f : fminf(fmaxf(v, -1.f), 1.f);
     if (wav_out) wav_out[i] = v;
     pcm[i] = (short)__float2int_rn(v * 32767.f);
   }
@@ -116,6 +125,13 @@ static Biquad highpass(double sr, double f0, double Q) {                      //
 constexpr size_t ENERGY_BYTES = 65536;
 size_t energy_offset(size_t n) { WsBump ws; ws.take(n * 4); return ws.take(ENERGY_BYTES); }
 
+// Gating blocks of 400 ms with 75 % overlap: the number of complete blocks, their length and hop in samples
+int gate_blocks(int n_samples, int sample_rate, int* gate, int* step) {
+  *gate = (int)lround(0.4 * sample_rate);
+  *step = (int)lround(*gate * 0.25);
+  return n_samples >= *gate ? (n_samples - *gate) / *step + 1 : 0;
+}
+
 }  // namespace
 
 extern "C" size_t mvb_audio_post_workspace_bytes(int32_t max_samples) {
@@ -131,8 +147,8 @@ extern "C" int mvb_audio_post(const float* d_wav, int32_t n_samples, int32_t sam
   cudaStream_t s = (cudaStream_t)stream;
   float* y = reinterpret_cast<float*>(d_workspace);
   float* energy = reinterpret_cast<float*>(reinterpret_cast<char*>(d_workspace) + energy_offset(n_samples));
-  const int gate = (int)lround(0.4 * sample_rate), step = (int)lround(gate * 0.25);
-  const int n_blocks = n_samples >= gate ? (n_samples - gate) / step + 1 : 0;
+  int gate, step;
+  const int n_blocks = gate_blocks(n_samples, sample_rate, &gate, &step);
   if (n_blocks + 4 > 16000) return mvb::set_error(MVB_ERR_UNSUPPORTED, "audio_post: signal too long for the workspace");
   float* res = energy + n_blocks + 1;
   const int chunks = (n_samples + KW_CHUNK - 1) / KW_CHUNK;
@@ -147,4 +163,31 @@ extern "C" int mvb_audio_post(const float* d_wav, int32_t n_samples, int32_t sam
   MVB_CK(cudaGetLastError());
   if (d_lkfs_gain) MVB_CK(cudaMemcpyAsync(d_lkfs_gain, res, 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
   return MVB_OK;
+}
+
+extern "C" int mvb_audio_post_test(const float* d_wav, int32_t n_samples, int32_t sample_rate, float loudness_headroom_db,
+                                   int32_t loudness_compressor, int16_t* d_pcm16, float* d_wav_out, float* d_y, float* d_energy,
+                                   float* d_res, int32_t* n_blocks_out, void* stream) {
+  if (!d_y || !d_energy || !d_res || !n_blocks_out) return mvb::set_error(MVB_ERR_ARG, "null argument");
+  if (n_samples < 1 || sample_rate < 8000) return mvb::set_error(MVB_ERR_ARG, "audio_post: bad length / sample rate");
+  cudaStream_t s = (cudaStream_t)stream;
+  const size_t bytes = mvb_audio_post_workspace_bytes(n_samples);
+  char* ws = nullptr;
+  MVB_CK(cudaMalloc(&ws, bytes));
+  int rc = mvb_audio_post(d_wav, n_samples, sample_rate, loudness_headroom_db, loudness_compressor, ws, d_pcm16, d_wav_out,
+                          nullptr, stream);
+  if (rc == MVB_OK) {
+    int gate, step;
+    const int n_blocks = gate_blocks(n_samples, sample_rate, &gate, &step);
+    const float* energy = reinterpret_cast<const float*>(ws + energy_offset(n_samples));
+    cudaError_t e = cudaMemcpyAsync(d_y, ws, (size_t)n_samples * 4, cudaMemcpyDeviceToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_energy, energy, (size_t)(n_blocks + 1) * 4, cudaMemcpyDeviceToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_res, energy + n_blocks + 1, 3 * 4, cudaMemcpyDeviceToDevice, s);
+    if (e != cudaSuccess) rc = mvb::set_error(MVB_ERR_CUDA, "mvb_audio_post_test: %s", cudaGetErrorString(e));
+    *n_blocks_out = n_blocks;
+  }
+  const cudaError_t e = cudaStreamSynchronize(s);   // (also on an error path: the buffer is freed only once unused)
+  if (rc == MVB_OK && e != cudaSuccess) rc = mvb::set_error(MVB_ERR_CUDA, "mvb_audio_post_test: %s", cudaGetErrorString(e));
+  cudaFree(ws);
+  return rc;
 }

@@ -303,12 +303,39 @@ static VocLayout voc_layout(const mvb_voc_config* c) {
   return L;
 }
 
+// k_lstm_layer: W_hh slice [16][H] + h [H] of dynamic shared memory per CTA, under the 100 KB opt-in set below
+constexpr int LSTM_SMEM_LIMIT = 100 * 1024;
+static size_t lstm_smem(int H) { return (size_t)(16 * H + H) * 4; }
+
+static int lstm_set_smem_limit() {
+  static PerDeviceOnce attr;
+  if (attr.pending()) {
+    MVB_CK(cudaFuncSetAttribute(k_lstm_layer, cudaFuncAttributeMaxDynamicSharedMemorySize, LSTM_SMEM_LIMIT));
+    attr.mark();
+  }
+  return MVB_OK;
+}
+
+// The H / 4 CTAs of one LSTM layer meet at a grid-wide barrier every step, so all of them must be resident at once on
+// the current device; a layer that cannot be is rejected instead of launched (it would wait forever).
+static int lstm_check_coresident(int H) {
+  if (int e = lstm_set_smem_limit()) return e;
+  int dev = 0, n_sm = 0, per_sm = 0;
+  if (int e = current_device(&dev, &n_sm)) return e;
+  MVB_CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_lstm_layer, 128, lstm_smem(H)));
+  if (H / 4 > per_sm * n_sm)
+    return mvb::set_error(MVB_ERR_UNSUPPORTED, "LSTM width %d: %d CTAs cannot be co-resident (%d per SM x %d SMs)", H, H / 4,
+                          per_sm, n_sm);
+  return MVB_OK;
+}
+
 static int voc_validate(const mvb_voc_config* c) {
   if (!c) return mvb::set_error(MVB_ERR_ARG, "null config");
   if (c->n_ratios < 1 || c->n_ratios > 8 || c->n_q < 1 || c->n_q > 32) return mvb::set_error(MVB_ERR_ARG, "bad codec shape");
   if (c->hidden > 128) return mvb::set_error(MVB_ERR_UNSUPPORTED, "codebook dim > 128");
   const int top = c->n_filters << c->n_ratios;
-  if (top % 32 || top / 4 > 148) return mvb::set_error(MVB_ERR_UNSUPPORTED, "LSTM width %d unsupported", top);
+  if (top < 32 || top % 32 || lstm_smem(top) > (size_t)LSTM_SMEM_LIMIT)
+    return mvb::set_error(MVB_ERR_UNSUPPORTED, "LSTM width %d unsupported", top);
   for (int i = 0; i < c->n_ratios; ++i)
     if (c->ratios[i] < 1 || c->ratios[i] > 8) return mvb::set_error(MVB_ERR_UNSUPPORTED, "upsampling ratio out of range");
   if (c->kernel != 7 || c->res_kernel != 3 || c->last_kernel != 7) return mvb::set_error(MVB_ERR_UNSUPPORTED, "kernel sizes must be 7/3/7");
@@ -326,6 +353,7 @@ extern "C" int mvb_voc_create(const mvb_voc_config* cfg, const void* d_arena, si
   if (int e = voc_validate(cfg)) return e;
   if (!d_arena || !offsets || !d_ws || !out) return mvb::set_error(MVB_ERR_ARG, "null pointer argument");
   if (int e = check_offsets(offsets, voc_n_tensors(cfg), arena_bytes, "vocoder: weight offset")) return e;
+  if (int e = lstm_check_coresident(cfg->n_filters << cfg->n_ratios)) return e;
   Building<mvb_voc> hb(new mvb_voc(), mvb_voc_destroy);
   mvb_voc* h = hb.get();
   h->cfg = *cfg;
@@ -354,6 +382,21 @@ static cudaError_t conv(cudaStream_t s, const float* x, int Cin, int T, const fl
   return cudaGetLastError();
 }
 
+static cudaError_t convtr(cudaStream_t s, const float* x, int Cin, int T, const float* w, const float* b, float* y, int Cout, int r) {
+  const size_t smem = (size_t)(16 * 33 + 16 * 32 * 2 * r) * 4;
+  k_convtr1d<<<dim3((T + 31) / 32, (Cout + 31) / 32, 1), 256, smem, s>>>(x, Cin, T, w, b, y, Cout, r);
+  return cudaGetLastError();
+}
+
+// One LSTM layer over pre [4H, T]; the caller has checked lstm_check_coresident(H) and set the shared-memory limit.
+static cudaError_t lstm(cudaStream_t s, const float* pre, const float* whh, int H, int T, float* hbuf, unsigned* bar, float* out,
+                        const float* skip) {
+  cudaError_t e = cudaMemsetAsync(bar, 0, 4, s);
+  if (e != cudaSuccess) return e;
+  k_lstm_layer<<<H / 4, 128, lstm_smem(H), s>>>(pre, whh, H, T, hbuf, bar, out, skip);
+  return cudaGetLastError();
+}
+
 // RVQ decode only: the diffusion condition `decode_latent` (and the decoder's input).  d_codes int32 [n_q, T].
 extern "C" int mvb_voc_decode_latent(mvb_voc* h, const int32_t* d_codes, int32_t T, float* d_latent, void* stream) {
   if (!h || !d_codes || !d_latent) return mvb::set_error(MVB_ERR_ARG, "null argument");
@@ -376,16 +419,12 @@ extern "C" int mvb_voc_decode(mvb_voc* h, const int32_t* d_codes, int32_t T, flo
   MVB_CK(conv<7>(s, A, c.hidden, T, h->w(ti), h->w(ti + 1), B, top, 0, 0));      // conv_in
   ti += 2;
   // LSTM: x = B;  layer 0 -> A ; layer 1 (+ skip x) -> Cc
-  const size_t lsmem = (size_t)(16 * top + top) * 4;
-  static PerDeviceOnce attr;
-  if (attr.pending()) { MVB_CK(cudaFuncSetAttribute(k_lstm_layer, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024)); attr.mark(); }
+  if (int e = lstm_set_smem_limit()) return e;
   const float* lin = B;
   float* louts[2] = {A, Cc};
   for (int l = 0; l < 2; ++l) {
     MVB_CK(conv<1>(s, lin, top, T, h->w(ti), h->w(ti + 2), h->pre, 4 * top, 0, 0));   // W_ih x + (b_ih + b_hh)
-    MVB_CK(cudaMemsetAsync(h->bar, 0, 4, s));
-    k_lstm_layer<<<top / 4, 128, lsmem, s>>>(h->pre, h->w(ti + 1), top, T, h->hbuf, h->bar, louts[l], l == 1 ? B : nullptr);
-    MVB_CK(cudaGetLastError());
+    MVB_CK(lstm(s, h->pre, h->w(ti + 1), top, T, h->hbuf, h->bar, louts[l], l == 1 ? B : nullptr));
     lin = louts[l];
     ti += 3;
   }
@@ -395,9 +434,7 @@ extern "C" int mvb_voc_decode(mvb_voc* h, const int32_t* d_codes, int32_t T, flo
   int ch = top, Tl = T;
   for (int i = 0; i < c.n_ratios; ++i) {
     const int r = c.ratios[i], co = ch / 2;
-    const size_t smem = (size_t)(16 * 33 + 16 * 32 * 2 * r) * 4;
-    k_convtr1d<<<dim3((Tl + 31) / 32, (co + 31) / 32, 1), 256, smem, s>>>(x, ch, Tl, h->w(ti), h->w(ti + 1), f1, co, r);
-    MVB_CK(cudaGetLastError());
+    MVB_CK(convtr(s, x, ch, Tl, h->w(ti), h->w(ti + 1), f1, co, r));
     Tl *= r; ch = co;
     // resnet block: y = shortcut(u) + conv_k1(elu(conv_k3(elu(u))))
     MVB_CK(conv<3>(s, f1, ch, Tl, h->w(ti + 2), h->w(ti + 3), f2, ch / c.compress, 1, 0));
@@ -406,5 +443,42 @@ extern "C" int mvb_voc_decode(mvb_voc* h, const int32_t* d_codes, int32_t T, flo
     ti += 8;
   }
   MVB_CK(conv<7>(s, x, ch, Tl, h->w(ti), h->w(ti + 1), d_wav, 1, 1, 0));
+  return MVB_OK;
+}
+
+extern "C" int mvb_voc_op_test(int32_t op, const float* d_x, int32_t Cin, int32_t T, const float* d_w, const float* d_b,
+                               int32_t Cout, int32_t k, int32_t elu_in, int32_t accumulate, const float* d_skip, float* d_y,
+                               void* stream) {
+  if (!d_x || !d_w || !d_y) return mvb::set_error(MVB_ERR_ARG, "null argument");
+  if (Cin < 1 || T < 1) return mvb::set_error(MVB_ERR_ARG, "mvb_voc_op_test: bad shape");
+  cudaStream_t s = (cudaStream_t)stream;
+  if (op == 0) {
+    if (Cout < 1) return mvb::set_error(MVB_ERR_ARG, "mvb_voc_op_test: bad shape");
+    if (k == 1) MVB_CK(conv<1>(s, d_x, Cin, T, d_w, d_b, d_y, Cout, elu_in, accumulate));
+    else if (k == 3) MVB_CK(conv<3>(s, d_x, Cin, T, d_w, d_b, d_y, Cout, elu_in, accumulate));
+    else if (k == 7) MVB_CK(conv<7>(s, d_x, Cin, T, d_w, d_b, d_y, Cout, elu_in, accumulate));
+    else return mvb::set_error(MVB_ERR_UNSUPPORTED, "mvb_voc_op_test: conv kernel size %d", k);
+  } else if (op == 1) {
+    if (Cout < 1 || !d_b) return mvb::set_error(MVB_ERR_ARG, "mvb_voc_op_test: bad shape or null bias");
+    if (k < 1 || k > 8) return mvb::set_error(MVB_ERR_UNSUPPORTED, "mvb_voc_op_test: upsampling ratio %d", k);
+    MVB_CK(convtr(s, d_x, Cin, T, d_w, d_b, d_y, Cout, k));
+  } else if (op == 2) {
+    const int H = Cin;
+    if (H % 32 || lstm_smem(H) > (size_t)LSTM_SMEM_LIMIT) return mvb::set_error(MVB_ERR_UNSUPPORTED, "LSTM width %d unsupported", H);
+    if (int e = lstm_check_coresident(H)) return e;
+    WsBump ws;
+    const size_t o_h = ws.take((size_t)2 * H * 4), o_bar = ws.take(4);
+    char* buf = nullptr;
+    MVB_CK(cudaMalloc(&buf, ws.end));
+    cudaError_t e = lstm(s, d_x, d_w, H, T, reinterpret_cast<float*>(buf + o_h), reinterpret_cast<unsigned*>(buf + o_bar), d_y, d_skip);
+    const cudaError_t es = cudaStreamSynchronize(s);   // (also on an error path: the buffer is freed only once unused)
+    cudaFree(buf);
+    if (e == cudaSuccess) e = es;
+    if (e != cudaSuccess) return mvb::set_error(MVB_ERR_CUDA, "mvb_voc_op_test: %s", cudaGetErrorString(e));
+    return MVB_OK;
+  } else {
+    return mvb::set_error(MVB_ERR_ARG, "mvb_voc_op_test: op %d", op);
+  }
+  MVB_CK(cudaStreamSynchronize(s));
   return MVB_OK;
 }

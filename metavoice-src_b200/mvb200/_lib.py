@@ -125,6 +125,10 @@ SIGNATURES = {
     "mvb_w4_dequant_test": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "mvb_s2_sample_test": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_void_p]),
+    "mvb_voc_op_test": (C.c_int, [C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                  C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "mvb_audio_post_test": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p]),
 }
 ABI_VERSION = 2
 

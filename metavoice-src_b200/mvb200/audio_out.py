@@ -99,10 +99,18 @@ def wav_bytes_on_device(wav: torch.Tensor, sample_rate: int, loudness_headroom_d
     st = C.c_void_p(torch.cuda.current_stream(w.device).cuda_stream)
     _lib.check(lib.mvb_audio_post(w.data_ptr(), n, int(sample_rate), float(loudness_headroom_db), int(bool(loudness_compressor)),
                                   ws[1].data_ptr(), pcm.data_ptr(), None, stats.data_ptr(), st))
+    lk, gain = stats.cpu().tolist()
+    if lk != lk:
+        # The meter is undefined (NaN): raise what audio_write_wav raises for the same input.  The device only reports
+        # NaN for non-finite samples, signals above the floor shorter than one 400 ms block (torchaudio's
+        # `loudness` raises RuntimeError), and signals whose blocks are all gated (NaN loudness: the finiteness assert).
+        assert bool(w.isfinite().all()), "wav contains non-finite samples"
+        if n < round(0.4 * sample_rate):
+            raise RuntimeError(f"loudness: {n} samples are shorter than one 400 ms gating block at {sample_rate} Hz")
+        raise AssertionError(f"loudness is undefined: every 400 ms block of the {n}-sample signal is below -70 LKFS")
     body = pcm.cpu().numpy().astype("<i2").tobytes()
     header = (b"RIFF" + struct.pack("<I", 36 + len(body)) + b"WAVEfmt " +
               struct.pack("<IHHIIHH", 16, 1, 1, sample_rate, sample_rate * 2, 2, 16) + b"data" + struct.pack("<I", len(body)))
     if return_stats:
-        lk, gain = stats.cpu().tolist()
         return header + body, lk, gain
     return header + body
