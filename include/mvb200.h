@@ -317,6 +317,20 @@ int mvb_voc_destroy(mvb_voc* h);
 int mvb_voc_decode_latent(mvb_voc* h, const int32_t* d_codes, int32_t T, float* d_latent, void* stream);
 /* d_codes int32 [n_q, T] -> d_wav fp32 [T * prod(ratios)]  (EncodecModel.decode, one chunk, 24 kHz) */
 int mvb_voc_decode(mvb_voc* h, const int32_t* d_codes, int32_t T, float* d_wav, void* stream);
+/* Batched decode (fam/llm/inference.py:438-517 `_sample_utterance_batch` decodes a batch of utterances): n utterances in
+ * one launch set, the two LSTM layers as one grid-barrier loop over max T_i for all of them.  Utterance i is bit-identical
+ * to mvb_voc_decode / mvb_voc_decode_latent on it alone.  Layout, with off_i = T_0 + ... + T_{i-1}:
+ *   d_codes  int32, utterance i as [n_q, T_i] at n_q off_i;  T: HOST int32 [n];
+ *   d_wav    fp32, utterance i as [T_i prod(ratios)] at off_i prod(ratios);  d_latent fp32 [hidden, T_i] at hidden off_i.
+ * d_batch_ws: a caller workspace of mvb_voc_batch_workspace_bytes(cfg, max_batch, max_total_frames) bytes (the handle's
+ * own workspace is not used), passed with the two capacities it was sized for.  MVB_ERR_ARG, before anything is
+ * launched, unless 1 <= n <= max_batch <= 32, every 8 <= T_i <= max_frames and sum T_i <= max_total_frames.  Calls on one
+ * batch workspace must be ordered (same stream).  mvb_voc_batch_workspace_bytes returns 0 for max_batch > 32. */
+size_t mvb_voc_batch_workspace_bytes(const mvb_voc_config* cfg, int32_t max_batch, int32_t max_total_frames);
+int mvb_voc_decode_batch(mvb_voc* h, int32_t n, const int32_t* d_codes, const int32_t* T, void* d_batch_ws, int32_t max_batch,
+                         int32_t max_total_frames, float* d_wav, void* stream);
+int mvb_voc_decode_latent_batch(mvb_voc* h, int32_t n, const int32_t* d_codes, const int32_t* T, void* d_batch_ws,
+                                int32_t max_batch, int32_t max_total_frames, float* d_latent, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Multi-band-diffusion vocoder (SURVEY.md row a17, second half) == `mbd.tokens_to_wav` (fam/llm/decoders.py:84-85 ->
@@ -401,6 +415,16 @@ size_t mvb_audio_post_workspace_bytes(int32_t max_samples);
 int mvb_audio_post(const float* d_wav, int32_t n_samples, int32_t sample_rate, float loudness_headroom_db,
                    int32_t loudness_compressor, void* d_workspace, int16_t* d_pcm16, float* d_wav_out,
                    float* d_lkfs_gain, void* stream);
+/* mvb_audio_post over n signals with one launch set.  d_wav fp32 and d_pcm16 / d_wav_out: signal i at off_i = n_0 + ... +
+ * n_{i-1} (n_samples: HOST int32 [n]); d_lkfs_gain optional fp32 [n][2].  Signal i's PCM, LKFS and gain are bit-identical to
+ * mvb_audio_post on it alone, edge cases included, and no signal's values affect another's.  d_workspace:
+ * mvb_audio_post_batch_workspace_bytes(max_batch, max_total_samples) bytes, passed with the capacities it was sized for.
+ * MVB_ERR_ARG unless 1 <= n <= max_batch, every n_i >= 1 and sum n_i <= max_total_samples; MVB_ERR_UNSUPPORTED when a
+ * signal exceeds 15,996 gating blocks; both before anything is launched. */
+size_t mvb_audio_post_batch_workspace_bytes(int32_t max_batch, int32_t max_total_samples);
+int mvb_audio_post_batch(const float* d_wav, int32_t n, const int32_t* n_samples, int32_t sample_rate, float loudness_headroom_db,
+                         int32_t loudness_compressor, void* d_workspace, int32_t max_batch, int32_t max_total_samples,
+                         int16_t* d_pcm16, float* d_wav_out, float* d_lkfs_gain, void* stream);
 
 #define MVB_OK 0
 #define MVB_ERR_CUDA 1

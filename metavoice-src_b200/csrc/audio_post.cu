@@ -12,6 +12,8 @@
 #include <cuda_runtime.h>
 #include <math.h>
 
+#include <vector>
+
 #include "common.cuh"
 #include "host.cuh"
 
@@ -24,8 +26,8 @@ struct Biquad { float b0, b1, b2, a1, a2; };   // normalised by a0
 constexpr int KW_CHUNK = 2048, KW_WARM = 4096;
 
 // y = clamp(hp(clamp(shelf(x))))   (torchaudio lfilter clamps each biquad's OUTPUT to [-1, 1], not its state)
-__global__ void __launch_bounds__(128) k_kweight(const float* __restrict__ x, int T, Biquad s, Biquad h, float* __restrict__ y) {
-  const int chunk = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void kweight_chunk(const float* __restrict__ x, int T, const Biquad& s, const Biquad& h, float* __restrict__ y,
+                                              int chunk) {
   const int t0 = chunk * KW_CHUNK;
   if (t0 >= T) return;
   const int start = max(0, t0 - KW_WARM), end = min(T, t0 + KW_CHUNK);
@@ -42,11 +44,15 @@ __global__ void __launch_bounds__(128) k_kweight(const float* __restrict__ x, in
   }
 }
 
+__global__ void __launch_bounds__(128) k_kweight(const float* __restrict__ x, int T, Biquad s, Biquad h, float* __restrict__ y) {
+  kweight_chunk(x, T, s, h, y, blockIdx.x * blockDim.x + threadIdx.x);
+}
+
 // block b: mean of y^2 over [b*step, b*step + gate); block n_blocks: sum of x^2 over the whole signal (energy floor test)
-__global__ void __launch_bounds__(256) k_block_energy(const float* __restrict__ y, const float* __restrict__ x, int T, int gate, int step,
-                                                      int n_blocks, float* __restrict__ energy) {
+__device__ __forceinline__ void block_energy(const float* __restrict__ y, const float* __restrict__ x, int T, int gate, int step,
+                                             int n_blocks, float* __restrict__ energy, int b) {
   __shared__ float red[8];
-  const int b = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const float* src = b < n_blocks ? y + (size_t)b * step : x;
   const int n = b < n_blocks ? gate : T;
   float acc = 0.f;
@@ -61,14 +67,18 @@ __global__ void __launch_bounds__(256) k_block_energy(const float* __restrict__ 
   }
 }
 
+__global__ void __launch_bounds__(256) k_block_energy(const float* __restrict__ y, const float* __restrict__ x, int T, int gate, int step,
+                                                      int n_blocks, float* __restrict__ energy) {
+  block_energy(y, x, T, gate, step, n_blocks, energy, blockIdx.x);
+}
+
 // gating + gain (one thread: <= 16000 blocks).  out[0] = LKFS, out[1] = linear gain, out[2] = 1 when the compressor may
 // run.  Below the energy floor: LKFS = -inf, gain 1, no compressor (audiocraft's normalize_loudness leaves the signal
 // untouched).  Where the meter is undefined -- non-finite input, no complete block, or every block gated (torchaudio
 // returns NaN or raises there, and normalize_loudness fails its finiteness assert) -- LKFS = NaN, gain 1, no compressor,
 // so that no NaN reaches the PCM.
-__global__ void k_loudness_gain(const float* __restrict__ energy, int n_blocks, int T, float headroom_db, float energy_floor,
-                                float* __restrict__ out) {
-  if (threadIdx.x != 0) return;
+__device__ __forceinline__ void loudness_gain(const float* __restrict__ energy, int n_blocks, int T, float headroom_db, float energy_floor,
+                                              float* __restrict__ out) {
   out[1] = 1.f; out[2] = 0.f;
   const float rms = sqrtf(energy[n_blocks] / (float)T);
   if (!isfinite(rms)) { out[0] = NAN; return; }
@@ -93,19 +103,65 @@ __global__ void k_loudness_gain(const float* __restrict__ energy, int n_blocks, 
   out[2] = 1.f;
 }
 
+__global__ void k_loudness_gain(const float* __restrict__ energy, int n_blocks, int T, float headroom_db, float energy_floor,
+                                float* __restrict__ out) {
+  if (threadIdx.x != 0) return;
+  loudness_gain(energy, n_blocks, T, headroom_db, energy_floor, out);
+}
+
 // out = clip(tanh(gain * x)) -> PCM16 (round to nearest even, like numpy's round in audio_out.py / torchaudio.save).
-// A NaN sample is written as 0 (fmaxf would otherwise turn it into -1).
-__global__ void __launch_bounds__(256) k_apply_pcm16(const float* __restrict__ x, int T, const float* __restrict__ g, int compressor,
-                                                     short* __restrict__ pcm, float* __restrict__ wav_out) {
+// A NaN sample is written as 0 (fmaxf would otherwise turn it into -1).  Samples first, first + stride, ...
+__device__ __forceinline__ void apply_pcm16(const float* __restrict__ x, int T, const float* __restrict__ g, int compressor,
+                                            short* __restrict__ pcm, float* __restrict__ wav_out, int first, int stride) {
   const float gain = g[1];
   const bool comp = compressor && g[2] != 0.f;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < T; i += gridDim.x * blockDim.x) {
+  for (int i = first; i < T; i += stride) {
     float v = gain * x[i];
     if (comp) v = tanhf(v);
     v = isnan(v) ? 0.f : fminf(fmaxf(v, -1.f), 1.f);
     if (wav_out) wav_out[i] = v;
     pcm[i] = (short)__float2int_rn(v * 32767.f);
   }
+}
+
+__global__ void __launch_bounds__(256) k_apply_pcm16(const float* __restrict__ x, int T, const float* __restrict__ g, int compressor,
+                                                     short* __restrict__ pcm, float* __restrict__ wav_out) {
+  apply_pcm16(x, T, g, compressor, pcm, wav_out, blockIdx.x * blockDim.x + threadIdx.x, gridDim.x * blockDim.x);
+}
+
+// ---- batched post: n signals concatenated, blockIdx.y (k_loudness_gain_b: blockIdx.x) is the signal -------------------
+// Signal i: samples [off, off + n) of the concatenated wav / PCM / K-weighted buffers, its n_blocks block energies, the
+// whole-signal sum of squares and the 3 result scalars at e_off of the energy area.
+struct PostSeg { int n, off, n_blocks, e_off; };
+
+__global__ void __launch_bounds__(128) k_kweight_b(const float* __restrict__ x, const PostSeg* __restrict__ segs, Biquad s, Biquad h,
+                                                   float* __restrict__ y) {
+  const PostSeg g = segs[blockIdx.y];
+  kweight_chunk(x + g.off, g.n, s, h, y + g.off, blockIdx.x * blockDim.x + threadIdx.x);
+}
+
+__global__ void __launch_bounds__(256) k_block_energy_b(const float* __restrict__ y, const float* __restrict__ x, const PostSeg* __restrict__ segs,
+                                                        int gate, int step, float* __restrict__ energy) {
+  const PostSeg g = segs[blockIdx.y];
+  if ((int)blockIdx.x > g.n_blocks) return;
+  block_energy(y + g.off, x + g.off, g.n, gate, step, g.n_blocks, energy + g.e_off, blockIdx.x);
+}
+
+__global__ void k_loudness_gain_b(float* __restrict__ energy, const PostSeg* __restrict__ segs, float headroom_db,
+                                  float energy_floor, float* __restrict__ lkfs_gain) {
+  if (threadIdx.x != 0) return;
+  const PostSeg g = segs[blockIdx.x];
+  float* res = energy + g.e_off + g.n_blocks + 1;
+  loudness_gain(energy + g.e_off, g.n_blocks, g.n, headroom_db, energy_floor, res);
+  if (lkfs_gain) { lkfs_gain[2 * blockIdx.x] = res[0]; lkfs_gain[2 * blockIdx.x + 1] = res[1]; }
+}
+
+__global__ void __launch_bounds__(256) k_apply_pcm16_b(const float* __restrict__ x, const PostSeg* __restrict__ segs,
+                                                       const float* __restrict__ energy, int compressor, short* __restrict__ pcm,
+                                                       float* __restrict__ wav_out) {
+  const PostSeg g = segs[blockIdx.y];
+  apply_pcm16(x + g.off, g.n, energy + g.e_off + g.n_blocks + 1, compressor, pcm + g.off, wav_out ? wav_out + g.off : nullptr,
+              blockIdx.x * blockDim.x + threadIdx.x, gridDim.x * blockDim.x);
 }
 
 static Biquad treble_shelf(double sr, double gain_db, double f0, double Q) {   // torchaudio.functional.treble_biquad
@@ -162,6 +218,74 @@ extern "C" int mvb_audio_post(const float* d_wav, int32_t n_samples, int32_t sam
   k_apply_pcm16<<<GRID_STRIDE_CTAS * 4, 256, 0, s>>>(d_wav, n_samples, res, loudness_compressor, d_pcm16, d_wav_out);
   MVB_CK(cudaGetLastError());
   if (d_lkfs_gain) MVB_CK(cudaMemcpyAsync(d_lkfs_gain, res, 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  return MVB_OK;
+}
+
+// ---- batched post ----------------------------------------------------------------------------------------------------
+// Workspace: K-weighted copy [max_total_samples] | segment table [max_batch] | energy area.  At >= 8 kHz a gating hop is
+// >= 800 samples, so signal i needs at most n_i / 800 + 1 block energies + 1 sum + 3 results.
+constexpr int POST_MAX_BATCH = 65535;   // grid.y limit
+struct PostBatchLayout { size_t seg, energy, total; };
+
+static PostBatchLayout post_batch_layout(int max_batch, int max_total_samples) {
+  PostBatchLayout L;
+  WsBump ws;
+  ws.take((size_t)max_total_samples * 4);
+  L.seg = ws.take((size_t)max_batch * sizeof(PostSeg));
+  L.energy = ws.take(((size_t)max_total_samples / 800 + 5 * (size_t)max_batch) * 4);
+  L.total = ws.end;
+  return L;
+}
+
+extern "C" size_t mvb_audio_post_batch_workspace_bytes(int32_t max_batch, int32_t max_total_samples) {
+  if (max_batch < 1 || max_batch > POST_MAX_BATCH || max_total_samples < 1) return 0;
+  return post_batch_layout(max_batch, max_total_samples).total;
+}
+
+// mvb_audio_post over n concatenated signals with one launch set; signal i's outputs equal mvb_audio_post's on it alone.
+extern "C" int mvb_audio_post_batch(const float* d_wav, int32_t n, const int32_t* n_samples, int32_t sample_rate,
+                                    float loudness_headroom_db, int32_t loudness_compressor, void* d_workspace, int32_t max_batch,
+                                    int32_t max_total_samples, int16_t* d_pcm16, float* d_wav_out, float* d_lkfs_gain, void* stream) {
+  if (!d_wav || !n_samples || !d_workspace || !d_pcm16) return mvb::set_error(MVB_ERR_ARG, "null argument");
+  if (max_batch < 1 || max_batch > POST_MAX_BATCH || max_total_samples < 1)
+    return mvb::set_error(MVB_ERR_ARG, "audio_post batch: bad capacity (%d signals, %d samples)", max_batch, max_total_samples);
+  if (n < 1 || n > max_batch) return mvb::set_error(MVB_ERR_ARG, "audio_post batch: %d signals, capacity %d", n, max_batch);
+  if (sample_rate < 8000) return mvb::set_error(MVB_ERR_ARG, "audio_post: bad length / sample rate");
+  int gate, step;
+  gate_blocks(1, sample_rate, &gate, &step);
+  std::vector<PostSeg> segs(n);
+  long long total = 0, e_total = 0;
+  int max_n = 0, max_blocks = 0;
+  for (int i = 0; i < n; ++i) {
+    if (n_samples[i] < 1) return mvb::set_error(MVB_ERR_ARG, "audio_post batch: signal %d: bad length %d", i, n_samples[i]);
+    const int nb = gate_blocks(n_samples[i], sample_rate, &gate, &step);
+    if (nb + 4 > 16000) return mvb::set_error(MVB_ERR_UNSUPPORTED, "audio_post: signal %d too long for the workspace", i);
+    segs[i] = PostSeg{n_samples[i], (int)total, nb, (int)e_total};
+    total += n_samples[i];
+    e_total += nb + 4;
+    max_n = max(max_n, n_samples[i]);
+    max_blocks = max(max_blocks, nb);
+  }
+  if (total > max_total_samples)
+    return mvb::set_error(MVB_ERR_ARG, "audio_post batch: %lld samples in all, capacity %d", total, max_total_samples);
+  cudaStream_t s = (cudaStream_t)stream;
+  const PostBatchLayout L = post_batch_layout(max_batch, max_total_samples);
+  char* ws = reinterpret_cast<char*>(d_workspace);
+  float* y = reinterpret_cast<float*>(ws);
+  const PostSeg* d_segs = reinterpret_cast<const PostSeg*>(ws + L.seg);
+  float* energy = reinterpret_cast<float*>(ws + L.energy);
+  MVB_CK(cudaMemcpyAsync(ws + L.seg, segs.data(), n * sizeof(PostSeg), cudaMemcpyHostToDevice, s));
+  const int chunks = (max_n + KW_CHUNK - 1) / KW_CHUNK;
+  k_kweight_b<<<dim3((chunks + 127) / 128, n), 128, 0, s>>>(d_wav, d_segs, treble_shelf(sample_rate, 4.0, 1500.0, 1.0 / sqrt(2.0)),
+                                                          highpass(sample_rate, 38.0, 0.5), y);
+  MVB_CK(cudaGetLastError());
+  k_block_energy_b<<<dim3(max_blocks + 1, n), 256, 0, s>>>(y, d_wav, d_segs, gate, step, energy);
+  MVB_CK(cudaGetLastError());
+  k_loudness_gain_b<<<n, 32, 0, s>>>(energy, d_segs, loudness_headroom_db, 2e-3f, d_lkfs_gain);
+  MVB_CK(cudaGetLastError());
+  const int per_signal = max(1, min(GRID_STRIDE_CTAS * 4, (max_n + 2047) / 2048));
+  k_apply_pcm16_b<<<dim3(per_signal, n), 256, 0, s>>>(d_wav, d_segs, energy, loudness_compressor, d_pcm16, d_wav_out);
+  MVB_CK(cudaGetLastError());
   return MVB_OK;
 }
 

@@ -21,37 +21,45 @@ namespace {
 __device__ __forceinline__ float elu1(float v) { return v > 0.f ? v : expm1f(v); }
 
 // latent[c][t] = sum_q codebook_q[codes[q][t]][c]     (EncodecResidualVectorQuantizer.decode)
-__global__ void __launch_bounds__(128) k_rvq_decode(const int* __restrict__ codes, int n_q, int T, const float* const* __restrict__ books,
-                                                    int dim, float* __restrict__ out) {
+// One tile of 32 frames from t0: codes [n_q, T] -> out [dim, T].
+__device__ __forceinline__ void rvq_tile(const int* __restrict__ codes, int n_q, int T, const float* const* __restrict__ books,
+                                         int dim, float* __restrict__ out, int t0) {
   __shared__ float tile[32][129];
-  const int t0 = blockIdx.x * 32, b = blockIdx.y;
   const int c = threadIdx.x;
   for (int i = 0; i < 32; ++i) {
     const int t = t0 + i;
     float acc = 0.f;
     if (t < T && c < dim)
-      for (int q = 0; q < n_q; ++q) acc += books[q][(size_t)codes[((size_t)b * n_q + q) * T + t] * dim + c];
+      for (int q = 0; q < n_q; ++q) acc += books[q][(size_t)codes[(size_t)q * T + t] * dim + c];
     tile[i][c] = acc;
   }
   __syncthreads();
   for (int idx = threadIdx.x; idx < 32 * dim; idx += 128) {
     const int cc = idx / 32, i = idx - cc * 32;
-    if (t0 + i < T) out[((size_t)b * dim + cc) * T + t0 + i] = tile[i][cc];
+    if (t0 + i < T) out[(size_t)cc * T + t0 + i] = tile[i][cc];
   }
+}
+
+__global__ void __launch_bounds__(128) k_rvq_decode(const int* __restrict__ codes, int n_q, int T, const float* const* __restrict__ books,
+                                                    int dim, float* __restrict__ out) {
+  const int b = blockIdx.y;
+  rvq_tile(codes + (size_t)b * n_q * T, n_q, T, books, dim, out + (size_t)b * dim * T, blockIdx.x * 32);
 }
 
 // Causal Conv1d, stride 1, dilation 1, reflect padding of K-1 samples on the left (EncodecConv1d, causal branch),
 // optional ELU on the input (the nn.ELU() that precedes the conv in the stack) and optional accumulation into y
 // (residual / shortcut sum of EncodecResnetBlock).  Tile: 32 output channels x 256 samples, 16 input channels per pass.
+// One tile of one sequence: xb [Cin, T] -> yb [Cout, T], samples t0 .. t0 + 255, output channels co0 .. co0 + 31.
 template <int K>
-__global__ void __launch_bounds__(256) k_conv1d(const float* __restrict__ x, int Cin, int T, const float* __restrict__ w,
-                                                const float* __restrict__ bias, float* __restrict__ y, int Cout, int elu_in, int accumulate) {
+__device__ __forceinline__ void conv1d_tile(const float* __restrict__ xb, int Cin, int T, const float* __restrict__ w,
+                                            const float* __restrict__ bias, float* __restrict__ yb, int Cout, int elu_in,
+                                            int accumulate, int t0, int co0) {
   constexpr int CI = 16, TT = 256, CO = 32;
   __shared__ float xs[CI][TT + K - 1 + 1];
   __shared__ float ws[CO][CI][K];
-  const int t0 = blockIdx.x * TT, co0 = blockIdx.y * CO, b = blockIdx.z;
   const int tx = threadIdx.x & 63, ty = threadIdx.x >> 6;    // 64 time groups of 4 samples x 4 groups of 8 channels
-  const float* xb = x + (size_t)b * Cin * T;
+  // 128-bit loads and stores need T % 4 == 0 and 16-byte aligned sequence bases (a batched segment may start anywhere)
+  const bool vec = (T & 3) == 0 && ((reinterpret_cast<uintptr_t>(xb) | reinterpret_cast<uintptr_t>(yb)) & 15) == 0;
   float acc[8][4];
 #pragma unroll
   for (int i = 0; i < 8; ++i)
@@ -62,7 +70,6 @@ __global__ void __launch_bounds__(256) k_conv1d(const float* __restrict__ x, int
     // line buffer: samples t0-(K-1) .. t0+TT-1 of 16 channels.  The TT-sample body is streamed with 128-bit loads
     // (rows are 16-byte aligned when T % 4 == 0, which holds for every layer of the decoder: T = frames x 8 x ...);
     // the K-1 halo samples in front are loaded one by one, negative times reflect (x[-j] = x[j]).
-    const bool vec = (T & 3) == 0;
     if (vec) {
       for (int i = threadIdx.x; i < CI * (TT / 4); i += 256) {
         const int ci = i / (TT / 4), q4 = i - ci * (TT / 4);
@@ -114,8 +121,8 @@ __global__ void __launch_bounds__(256) k_conv1d(const float* __restrict__ x, int
     if (co >= Cout) continue;
     const float bv = bias ? bias[co] : 0.f;
     const int tb = t0 + tx * 4;
-    if (((T & 3) == 0) && tb < T) {            // 128-bit coalesced store of the thread's 4 consecutive samples
-      float4* o = reinterpret_cast<float4*>(y + ((size_t)b * Cout + co) * T + tb);
+    if (vec && tb < T) {                       // 128-bit coalesced store of the thread's 4 consecutive samples
+      float4* o = reinterpret_cast<float4*>(yb + (size_t)co * T + tb);
       float4 v = make_float4(acc[i][0] + bv, acc[i][1] + bv, acc[i][2] + bv, acc[i][3] + bv);
       if (accumulate) { const float4 p = *o; v.x += p.x; v.y += p.y; v.z += p.z; v.w += p.w; }
       *o = v;
@@ -125,7 +132,7 @@ __global__ void __launch_bounds__(256) k_conv1d(const float* __restrict__ x, int
     for (int j = 0; j < 4; ++j) {
       const int t = t0 + tx * 4 + j;
       if (t < T) {
-        float* o = y + ((size_t)b * Cout + co) * T + t;
+        float* o = yb + (size_t)co * T + t;
         const float v = acc[i][j] + bv;
         *o = accumulate ? *o + v : v;
       }
@@ -133,18 +140,25 @@ __global__ void __launch_bounds__(256) k_conv1d(const float* __restrict__ x, int
   }
 }
 
+template <int K>
+__global__ void __launch_bounds__(256) k_conv1d(const float* __restrict__ x, int Cin, int T, const float* __restrict__ w,
+                                                const float* __restrict__ bias, float* __restrict__ y, int Cout, int elu_in, int accumulate) {
+  const int b = blockIdx.z;
+  conv1d_tile<K>(x + (size_t)b * Cin * T, Cin, T, w, bias, y + (size_t)b * Cout * T, Cout, elu_in, accumulate, blockIdx.x * 256,
+                 blockIdx.y * 32);
+}
+
 // ConvTranspose1d(k = 2r, stride r) trimmed by r samples on the right (EncodecConvTranspose1d, causal) with the
 // preceding ELU fused:  y[co][t*r + p] = b[co] + sum_ci w[ci][co][p] * e[ci][t] + w[ci][co][p + r] * e[ci][t-1].
-__global__ void __launch_bounds__(256) k_convtr1d(const float* __restrict__ x, int Cin, int T, const float* __restrict__ w,
-                                                  const float* __restrict__ bias, float* __restrict__ y, int Cout, int r) {
+// One tile of one sequence: xb [Cin, T] -> yb [Cout, T r], input frames t0 .. t0 + 31; sm = the dynamic shared memory.
+__device__ __forceinline__ void convtr1d_tile(const float* __restrict__ xb, int Cin, int T, const float* __restrict__ w,
+                                              const float* __restrict__ bias, float* __restrict__ yb, int Cout, int r, int t0,
+                                              int co0, float* sm) {
   constexpr int CI = 16, TI = 32, CO = 32;
-  extern __shared__ float sm[];
   float* xs = sm;                       // [CI][TI + 1]   (index 0 = t0 - 1)
   float* ws = sm + CI * (TI + 1);       // [CI][CO][2r]
-  const int t0 = blockIdx.x * TI, co0 = blockIdx.y * CO, b = blockIdx.z;
   const int ox = threadIdx.x & 63, ty = threadIdx.x >> 6;
   const int n_out = TI * r;             // outputs of this tile
-  const float* xb = x + (size_t)b * Cin * T;
   float acc[8][4];
   int tl[4], pp[4];
 #pragma unroll
@@ -195,9 +209,16 @@ __global__ void __launch_bounds__(256) k_convtr1d(const float* __restrict__ x, i
     for (int j = 0; j < 4; ++j) {
       const int o = ox + 64 * j;
       const int n = t0 * r + o;
-      if (o < n_out && n < To) y[((size_t)b * Cout + co) * To + n] = acc[i][j] + bv;
+      if (o < n_out && n < To) yb[(size_t)co * To + n] = acc[i][j] + bv;
     }
   }
+}
+
+__global__ void __launch_bounds__(256) k_convtr1d(const float* __restrict__ x, int Cin, int T, const float* __restrict__ w,
+                                                  const float* __restrict__ bias, float* __restrict__ y, int Cout, int r) {
+  extern __shared__ float sm[];
+  const int b = blockIdx.z;
+  convtr1d_tile(x + (size_t)b * Cin * T, Cin, T, w, bias, y + (size_t)b * Cout * T * r, Cout, r, blockIdx.x * 32, blockIdx.y * 32, sm);
 }
 
 // One LSTM layer (EncodecLSTM: nn.LSTM, gate order i, f, g, o, zero initial state), persistent over time:
@@ -260,6 +281,130 @@ __global__ void __launch_bounds__(128) k_lstm_layer(const float* __restrict__ pr
   }
 }
 
+// ---- batched decode: B utterances of T_i frames in one launch set ------------------------------------------------------
+// Every activation is concatenated per utterance: a layer with C channels at m samples per frame holds utterance i as a
+// [C, T_i m] block starting at element C off_i m (off_i = T_0 + ... + T_{i-1}).  blockIdx.z is the utterance; tiles past
+// its end return, so every tile computes exactly what the same tile of the single-utterance launch computes.
+constexpr int VOC_MAX_BATCH = 32;
+struct Seg { int T, off; };
+
+__global__ void __launch_bounds__(128) k_rvq_decode_b(const int* __restrict__ codes, int n_q, const Seg* __restrict__ segs,
+                                                      const float* const* __restrict__ books, int dim, float* __restrict__ out) {
+  const Seg g = segs[blockIdx.z];
+  const int t0 = blockIdx.x * 32;
+  if (t0 >= g.T) return;
+  rvq_tile(codes + (size_t)n_q * g.off, n_q, g.T, books, dim, out + (size_t)dim * g.off, t0);
+}
+
+template <int K>
+__global__ void __launch_bounds__(256) k_conv1d_b(const float* __restrict__ x, int Cin, const Seg* __restrict__ segs, int m,
+                                                  const float* __restrict__ w, const float* __restrict__ bias, float* __restrict__ y,
+                                                  int Cout, int elu_in, int accumulate) {
+  const Seg g = segs[blockIdx.z];
+  const int T = g.T * m, t0 = blockIdx.x * 256;
+  if (t0 >= T) return;
+  const size_t off = (size_t)g.off * m;
+  conv1d_tile<K>(x + off * Cin, Cin, T, w, bias, y + off * Cout, Cout, elu_in, accumulate, t0, blockIdx.y * 32);
+}
+
+// input at m samples per frame, output at m r
+__global__ void __launch_bounds__(256) k_convtr1d_b(const float* __restrict__ x, int Cin, const Seg* __restrict__ segs, int m,
+                                                    const float* __restrict__ w, const float* __restrict__ bias, float* __restrict__ y,
+                                                    int Cout, int r) {
+  extern __shared__ float sm[];
+  const Seg g = segs[blockIdx.z];
+  const int T = g.T * m, t0 = blockIdx.x * 32;
+  if (t0 >= T) return;
+  const size_t off = (size_t)g.off * m;
+  convtr1d_tile(x + off * Cin, Cin, T, w, bias, y + off * r * Cout, Cout, r, t0, blockIdx.y * 32, sm);
+}
+
+// k_lstm_layer for n <= 32 sequences at once: one grid barrier per step of the longest sequence instead of one per step of
+// every sequence.  CTA c still owns hidden units [4c, 4c+4) and holds their 16 W_hh rows in shared memory, loaded once;
+// each step it computes those 16 gate rows for every sequence still running (t < T_i) and the finished ones stop writing.
+// Every pre-activation is summed exactly as k_lstm_layer sums it (8 lanes x H/8 consecutive products, then xor-shuffles
+// 4 / 2 / 1), so each sequence is bit-identical to its single-sequence run.  Shared memory rows are padded by one float
+// per H/8 segment: the 8 lanes of a row and the 4 rows of a warp then read 32 different banks.
+// pre: per sequence [4H, T_i] at 4H off_i; out / skip: [H, T_i] at H off_i; hbuf [2][n][H].
+__host__ __device__ constexpr int lstm_b_ld(int H) { return H + 8; }
+
+__global__ void __launch_bounds__(128) k_lstm_layer_b(const float* __restrict__ pre, const float* __restrict__ whh, int H,
+                                                      const Seg* __restrict__ segs, int n, int T_max, float* __restrict__ hbuf,
+                                                      unsigned* bar, float* __restrict__ out, const float* __restrict__ skip) {
+  extern __shared__ float sm[];
+  const int seg = H / 8, ld = lstm_b_ld(H);
+  float* wsm = sm;                 // [16][ld]
+  float* hs = sm + 16 * ld;        // [round_up(n, 4)][ld]
+  __shared__ float gates[VOC_MAX_BATCH][16];
+  __shared__ int Ts[VOC_MAX_BATCH], offs[VOC_MAX_BATCH];
+  const int cta = blockIdx.x, tid = threadIdx.x;
+  const int u0 = cta * 4;
+  const int n4 = (n + 3) & ~3;
+  auto at = [seg](int k) { const int p = k / seg; return p * (seg + 1) + (k - p * seg); };   // padded column of k
+  for (int i = tid; i < 16 * H; i += 128) {
+    const int r = i / H, k = i - r * H;
+    const int grow = (r >> 2) * H + u0 + (r & 3);
+    wsm[r * ld + at(k)] = whh[(size_t)grow * H + k];
+  }
+  if (tid < n) { Ts[tid] = segs[tid].T; offs[tid] = segs[tid].off; }
+  float c_state = 0.f;
+  const int row = tid >> 3, part = tid & 7;      // 16 rows x 8 lanes
+  const int cb = tid >> 2, cu = tid & 3;         // cell update: sequence cb, unit u0 + cu
+  __syncthreads();
+  for (int t = 0; t < T_max; ++t) {
+    if (t > 0) {
+      if (tid == 0) wait_counter(bar, (unsigned)t * gridDim.x);
+      __syncthreads();
+      for (int b = 0; b < n; ++b) {
+        if (t >= Ts[b]) continue;
+        const float* hp = hbuf + ((size_t)((t - 1) & 1) * n + b) * H;
+        for (int k = tid; k < H; k += 128) hs[b * ld + at(k)] = __ldcg(hp + k);
+      }
+    } else {
+      for (int k = tid; k < n4 * ld; k += 128) hs[k] = 0.f;
+    }
+    __syncthreads();
+    const float* wr = wsm + row * ld + part * (seg + 1);
+    for (int b0 = 0; b0 < n; b0 += 4) {
+      // four sequences share each W_hh load; every accumulator is its own sequential fmaf chain
+      float a[4] = {0.f, 0.f, 0.f, 0.f};
+      const float* hh = hs + b0 * ld + part * (seg + 1);
+#pragma unroll 4
+      for (int k = 0; k < seg; ++k) {
+        const float wv = wr[k];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) a[j] = fmaf(wv, hh[j * ld + k], a[j]);
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        a[j] += __shfl_xor_sync(0xffffffffu, a[j], 4);
+        a[j] += __shfl_xor_sync(0xffffffffu, a[j], 2);
+        a[j] += __shfl_xor_sync(0xffffffffu, a[j], 1);
+        const int b = b0 + j;
+        if (part == 0 && b < n && t < Ts[b]) {
+          const int grow = (row >> 2) * H + u0 + (row & 3);
+          gates[b][row] = a[j] + pre[(size_t)offs[b] * 4 * H + (size_t)grow * Ts[b] + t];
+        }
+      }
+    }
+    __syncthreads();
+    if (cb < n && t < Ts[cb]) {
+      const float* gt = gates[cb];
+      const float ig = 1.f / (1.f + expf(-gt[cu]));
+      const float fg = 1.f / (1.f + expf(-gt[4 + cu]));
+      const float gg = tanhf(gt[8 + cu]);
+      const float og = 1.f / (1.f + expf(-gt[12 + cu]));
+      c_state = fg * c_state + ig * gg;
+      const float h = og * tanhf(c_state);
+      hbuf[((size_t)(t & 1) * n + cb) * H + u0 + cu] = h;
+      const size_t o = (size_t)offs[cb] * H + (size_t)(u0 + cu) * Ts[cb] + t;
+      out[o] = skip ? h + skip[o] : h;
+    }
+    __syncthreads();
+    if (tid == 0) red_release_inc(bar);
+  }
+}
+
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -282,8 +427,8 @@ static int voc_n_tensors(const mvb_voc_config* c) { return c->n_q + 2 + 6 + c->n
 
 struct VocLayout { size_t A, B, C, pre, h, bar, books, total; };
 
-static VocLayout voc_layout(const mvb_voc_config* c) {
-  const size_t T = c->max_frames;
+// Elements of the largest decoder activation over T frames (channels x samples, over the upsampling stages).
+static size_t voc_max_elems(const mvb_voc_config* c, size_t T) {
   int ch = c->n_filters << c->n_ratios;   // 512
   size_t maxelems = (size_t)ch * T, Tl = T;
   for (int i = 0; i < c->n_ratios; ++i) {
@@ -291,6 +436,12 @@ static VocLayout voc_layout(const mvb_voc_config* c) {
     ch >>= 1;
     if ((size_t)ch * Tl > maxelems) maxelems = (size_t)ch * Tl;
   }
+  return maxelems;
+}
+
+static VocLayout voc_layout(const mvb_voc_config* c) {
+  const size_t T = c->max_frames;
+  const size_t maxelems = voc_max_elems(c, T);
   const size_t top = (size_t)(c->n_filters << c->n_ratios);
   VocLayout L;
   WsBump ws;
@@ -316,17 +467,39 @@ static int lstm_set_smem_limit() {
   return MVB_OK;
 }
 
+// k_lstm_layer_b: W_hh slice + h of round_up(n, 4) sequences, rows padded to lstm_b_ld(H)
+static size_t lstm_b_smem(int H, int n) { return (size_t)(16 + ((n + 3) & ~3)) * lstm_b_ld(H) * 4; }
+
+static int lstm_b_set_smem_limit() {
+  static PerDeviceOnce attr;
+  if (attr.pending()) {
+    MVB_CK(cudaFuncSetAttribute(k_lstm_layer_b, cudaFuncAttributeMaxDynamicSharedMemorySize, LSTM_SMEM_LIMIT));
+    attr.mark();
+  }
+  return MVB_OK;
+}
+
 // The H / 4 CTAs of one LSTM layer meet at a grid-wide barrier every step, so all of them must be resident at once on
 // the current device; a layer that cannot be is rejected instead of launched (it would wait forever).
-static int lstm_check_coresident(int H) {
-  if (int e = lstm_set_smem_limit()) return e;
+template <class Kernel>
+static int check_coresident(Kernel kernel, int H, size_t smem) {
   int dev = 0, n_sm = 0, per_sm = 0;
   if (int e = current_device(&dev, &n_sm)) return e;
-  MVB_CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_lstm_layer, 128, lstm_smem(H)));
+  MVB_CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, 128, smem));
   if (H / 4 > per_sm * n_sm)
     return mvb::set_error(MVB_ERR_UNSUPPORTED, "LSTM width %d: %d CTAs cannot be co-resident (%d per SM x %d SMs)", H, H / 4,
                           per_sm, n_sm);
   return MVB_OK;
+}
+
+static int lstm_check_coresident(int H) {
+  if (int e = lstm_set_smem_limit()) return e;
+  return check_coresident(k_lstm_layer, H, lstm_smem(H));
+}
+
+static int lstm_b_check_coresident(int H, int n) {
+  if (int e = lstm_b_set_smem_limit()) return e;
+  return check_coresident(k_lstm_layer_b, H, lstm_b_smem(H, n));
 }
 
 static int voc_validate(const mvb_voc_config* c) {
@@ -443,6 +616,129 @@ extern "C" int mvb_voc_decode(mvb_voc* h, const int32_t* d_codes, int32_t T, flo
     ti += 8;
   }
   MVB_CK(conv<7>(s, x, ch, Tl, h->w(ti), h->w(ti + 1), d_wav, 1, 1, 0));
+  return MVB_OK;
+}
+
+// ---- batched decode ------------------------------------------------------------------------------------------------------
+// Batch workspace (caller-owned, separate from the handle's): segment table | three activation buffers | LSTM
+// pre-activations | h exchange [2][max_batch][H] | barrier word, all sized for max_total_frames concatenated frames.
+struct VocBatchLayout { size_t seg, A, B, C, pre, h, bar, total; };
+
+static VocBatchLayout voc_batch_layout(const mvb_voc_config* c, int max_batch, int max_total_frames) {
+  const size_t maxelems = voc_max_elems(c, (size_t)max_total_frames);
+  const size_t top = (size_t)(c->n_filters << c->n_ratios);
+  VocBatchLayout L;
+  WsBump ws;
+  L.seg = ws.take((size_t)VOC_MAX_BATCH * sizeof(Seg));
+  L.A = ws.take(maxelems * 4); L.B = ws.take(maxelems * 4); L.C = ws.take(maxelems * 4);
+  L.pre = ws.take(4 * top * (size_t)max_total_frames * 4);
+  L.h = ws.take(2 * (size_t)max_batch * top * 4);
+  L.bar = ws.take(256);
+  L.total = ws.end;
+  return L;
+}
+
+static int voc_batch_capacity(int max_batch, int max_total_frames) {
+  if (max_batch < 1 || max_batch > VOC_MAX_BATCH)
+    return mvb::set_error(MVB_ERR_ARG, "vocoder batch: max_batch %d out of range [1, %d]", max_batch, VOC_MAX_BATCH);
+  if (max_total_frames < 8) return mvb::set_error(MVB_ERR_ARG, "vocoder batch: max_total_frames %d < 8", max_total_frames);
+  return MVB_OK;
+}
+
+extern "C" size_t mvb_voc_batch_workspace_bytes(const mvb_voc_config* c, int32_t max_batch, int32_t max_total_frames) {
+  if (voc_validate(c) || voc_batch_capacity(max_batch, max_total_frames)) return 0;
+  return voc_batch_layout(c, max_batch, max_total_frames).total;
+}
+
+// Validates a batch (nothing is launched on failure) and uploads its segment table; *T_max = the longest utterance.
+static int voc_batch_begin(const mvb_voc* h, int n, const int32_t* d_codes, const int32_t* T, void* d_ws, int max_batch,
+                           int max_total_frames, const void* d_out, cudaStream_t s, const VocBatchLayout& L, int* T_max) {
+  if (!h || !d_codes || !T || !d_ws || !d_out) return mvb::set_error(MVB_ERR_ARG, "null argument");
+  if (int e = voc_batch_capacity(max_batch, max_total_frames)) return e;
+  if (n < 1 || n > max_batch) return mvb::set_error(MVB_ERR_ARG, "vocoder batch: %d utterances, capacity %d", n, max_batch);
+  Seg segs[VOC_MAX_BATCH];
+  long long total = 0;
+  int tmax = 0;
+  for (int i = 0; i < n; ++i) {
+    if (T[i] < 8 || T[i] > h->cfg.max_frames)
+      return mvb::set_error(MVB_ERR_ARG, "vocoder batch: utterance %d: frame count %d out of range [8, %d]", i, T[i], h->cfg.max_frames);
+    segs[i] = Seg{T[i], (int)total};
+    total += T[i];
+    if (T[i] > tmax) tmax = T[i];
+  }
+  if (total > max_total_frames)
+    return mvb::set_error(MVB_ERR_ARG, "vocoder batch: %lld frames in all, capacity %d", total, max_total_frames);
+  MVB_CK(cudaMemcpyAsync(reinterpret_cast<char*>(d_ws) + L.seg, segs, n * sizeof(Seg), cudaMemcpyHostToDevice, s));
+  *T_max = tmax;
+  return MVB_OK;
+}
+
+template <int K>
+static cudaError_t conv_b(cudaStream_t s, const float* x, int Cin, const Seg* segs, int n, int T_max, int m, const float* w,
+                          const float* b, float* y, int Cout, int elu, int acc) {
+  k_conv1d_b<K><<<dim3((T_max * m + 255) / 256, (Cout + 31) / 32, n), 256, 0, s>>>(x, Cin, segs, m, w, b, y, Cout, elu, acc);
+  return cudaGetLastError();
+}
+
+extern "C" int mvb_voc_decode_latent_batch(mvb_voc* h, int32_t n, const int32_t* d_codes, const int32_t* T, void* d_batch_ws,
+                                           int32_t max_batch, int32_t max_total_frames, float* d_latent, void* stream) {
+  cudaStream_t s = (cudaStream_t)stream;
+  const VocBatchLayout L = h ? voc_batch_layout(&h->cfg, max_batch, max_total_frames) : VocBatchLayout{};
+  int T_max = 0;
+  if (int e = voc_batch_begin(h, n, d_codes, T, d_batch_ws, max_batch, max_total_frames, d_latent, s, L, &T_max)) return e;
+  const Seg* segs = reinterpret_cast<const Seg*>(reinterpret_cast<char*>(d_batch_ws) + L.seg);
+  k_rvq_decode_b<<<dim3((T_max + 31) / 32, 1, n), 128, 0, s>>>(d_codes, h->cfg.n_q, segs, h->books_dev, h->cfg.hidden, d_latent);
+  MVB_CK(cudaGetLastError());
+  return MVB_OK;
+}
+
+// The launch sequence of mvb_voc_decode, each launch over all n utterances.
+extern "C" int mvb_voc_decode_batch(mvb_voc* h, int32_t n, const int32_t* d_codes, const int32_t* T, void* d_batch_ws,
+                                    int32_t max_batch, int32_t max_total_frames, float* d_wav, void* stream) {
+  cudaStream_t s = (cudaStream_t)stream;
+  const VocBatchLayout L = h ? voc_batch_layout(&h->cfg, max_batch, max_total_frames) : VocBatchLayout{};
+  int T_max = 0;
+  if (int e = voc_batch_begin(h, n, d_codes, T, d_batch_ws, max_batch, max_total_frames, d_wav, s, L, &T_max)) return e;
+  const mvb_voc_config& c = h->cfg;
+  const int top = c.n_filters << c.n_ratios;
+  if (int e = lstm_b_check_coresident(top, n)) return e;
+  char* ws = reinterpret_cast<char*>(d_batch_ws);
+  const Seg* segs = reinterpret_cast<const Seg*>(ws + L.seg);
+  float *A = (float*)(ws + L.A), *B = (float*)(ws + L.B), *Cc = (float*)(ws + L.C), *pre = (float*)(ws + L.pre);
+  float* hbuf = (float*)(ws + L.h);
+  unsigned* bar = (unsigned*)(ws + L.bar);
+  int ti = c.n_q;
+  k_rvq_decode_b<<<dim3((T_max + 31) / 32, 1, n), 128, 0, s>>>(d_codes, c.n_q, segs, h->books_dev, c.hidden, A);
+  MVB_CK(cudaGetLastError());
+  MVB_CK(conv_b<7>(s, A, c.hidden, segs, n, T_max, 1, h->w(ti), h->w(ti + 1), B, top, 0, 0));      // conv_in
+  ti += 2;
+  const float* lin = B;
+  float* louts[2] = {A, Cc};
+  for (int l = 0; l < 2; ++l) {
+    MVB_CK(conv_b<1>(s, lin, top, segs, n, T_max, 1, h->w(ti), h->w(ti + 2), pre, 4 * top, 0, 0));
+    MVB_CK(cudaMemsetAsync(bar, 0, 4, s));
+    k_lstm_layer_b<<<top / 4, 128, lstm_b_smem(top, n), s>>>(pre, h->w(ti + 1), top, segs, n, T_max, hbuf, bar, louts[l],
+                                                             l == 1 ? B : nullptr);
+    MVB_CK(cudaGetLastError());
+    lin = louts[l];
+    ti += 3;
+  }
+  float* x = Cc;
+  float* f1 = A;
+  float* f2 = B;
+  int ch = top, m = 1;
+  for (int i = 0; i < c.n_ratios; ++i) {
+    const int r = c.ratios[i], co = ch / 2;
+    const size_t smem = (size_t)(16 * 33 + 16 * 32 * 2 * r) * 4;
+    k_convtr1d_b<<<dim3((T_max * m + 31) / 32, (co + 31) / 32, n), 256, smem, s>>>(x, ch, segs, m, h->w(ti), h->w(ti + 1), f1, co, r);
+    MVB_CK(cudaGetLastError());
+    m *= r; ch = co;
+    MVB_CK(conv_b<3>(s, f1, ch, segs, n, T_max, m, h->w(ti + 2), h->w(ti + 3), f2, ch / c.compress, 1, 0));
+    MVB_CK(conv_b<1>(s, f1, ch, segs, n, T_max, m, h->w(ti + 6), h->w(ti + 7), x, ch, 0, 0));
+    MVB_CK(conv_b<1>(s, f2, ch / c.compress, segs, n, T_max, m, h->w(ti + 4), h->w(ti + 5), x, ch, 1, 1));
+    ti += 8;
+  }
+  MVB_CK(conv_b<7>(s, x, ch, segs, n, T_max, m, h->w(ti), h->w(ti + 1), d_wav, 1, 1, 0));
   return MVB_OK;
 }
 

@@ -92,6 +92,11 @@ SIGNATURES = {
     "mvb_voc_destroy": (C.c_int, [C.c_void_p]),
     "mvb_voc_decode_latent": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "mvb_voc_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "mvb_voc_batch_workspace_bytes": (C.c_size_t, [C.POINTER(VocConfig), C.c_int32, C.c_int32]),
+    "mvb_voc_decode_batch": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.c_int32, C.c_int32,
+                                       C.c_void_p, C.c_void_p]),
+    "mvb_voc_decode_latent_batch": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.c_int32,
+                                              C.c_int32, C.c_void_p, C.c_void_p]),
     "mvb_mbd_workspace_bytes": (C.c_size_t, [C.POINTER(MbdConfig)]),
     "mvb_mbd_create": (C.c_int, [C.POINTER(MbdConfig), C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64), C.c_void_p,
                                  C.POINTER(C.c_void_p)]),
@@ -107,6 +112,9 @@ SIGNATURES = {
     "mvb_audio_post_workspace_bytes": (C.c_size_t, [C.c_int32]),
     "mvb_audio_post": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p, C.c_void_p]),
+    "mvb_audio_post_batch_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32]),
+    "mvb_audio_post_batch": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_int32, C.c_float, C.c_int32, C.c_void_p,
+                                       C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "mvb_linear": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_float,
                              C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
     # test / debug hooks (declared in the header as such)

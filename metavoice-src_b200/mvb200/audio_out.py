@@ -101,16 +101,79 @@ def wav_bytes_on_device(wav: torch.Tensor, sample_rate: int, loudness_headroom_d
                                   ws[1].data_ptr(), pcm.data_ptr(), None, stats.data_ptr(), st))
     lk, gain = stats.cpu().tolist()
     if lk != lk:
-        # The meter is undefined (NaN): raise what audio_write_wav raises for the same input.  The device only reports
-        # NaN for non-finite samples, signals above the floor shorter than one 400 ms block (torchaudio's
-        # `loudness` raises RuntimeError), and signals whose blocks are all gated (NaN loudness: the finiteness assert).
-        assert bool(w.isfinite().all()), "wav contains non-finite samples"
-        if n < round(0.4 * sample_rate):
-            raise RuntimeError(f"loudness: {n} samples are shorter than one 400 ms gating block at {sample_rate} Hz")
-        raise AssertionError(f"loudness is undefined: every 400 ms block of the {n}-sample signal is below -70 LKFS")
+        raise _undefined_meter_error(w, sample_rate)
     body = pcm.cpu().numpy().astype("<i2").tobytes()
-    header = (b"RIFF" + struct.pack("<I", 36 + len(body)) + b"WAVEfmt " +
-              struct.pack("<IHHIIHH", 16, 1, 1, sample_rate, sample_rate * 2, 2, 16) + b"data" + struct.pack("<I", len(body)))
     if return_stats:
-        return header + body, lk, gain
-    return header + body
+        return _wav_header(len(body), sample_rate) + body, lk, gain
+    return _wav_header(len(body), sample_rate) + body
+
+
+def _undefined_meter_error(w: torch.Tensor, sample_rate: int, prefix: str = "") -> Exception:
+    """The meter is undefined (NaN): what audio_write_wav raises for the same input.  The device only reports NaN for
+    non-finite samples, signals above the floor shorter than one 400 ms block (torchaudio's `loudness` raises
+    RuntimeError), and signals whose blocks are all gated (NaN loudness: the finiteness assert)."""
+    n = w.numel()
+    if not bool(w.isfinite().all()):
+        return AssertionError(prefix + "wav contains non-finite samples")
+    if n < round(0.4 * sample_rate):
+        return RuntimeError(prefix + f"loudness: {n} samples are shorter than one 400 ms gating block at {sample_rate} Hz")
+    return AssertionError(prefix + f"loudness is undefined: every 400 ms block of the {n}-sample signal is below -70 LKFS")
+
+
+def _wav_header(n_bytes: int, sample_rate: int) -> bytes:
+    return (b"RIFF" + struct.pack("<I", 36 + n_bytes) + b"WAVEfmt " +
+            struct.pack("<IHHIIHH", 16, 1, 1, sample_rate, sample_rate * 2, 2, 16) + b"data" + struct.pack("<I", n_bytes))
+
+
+_POST_BATCH_WS = {}
+
+
+def _post_batch(wavs, sample_rate: int, loudness_headroom_db: float, loudness_compressor: bool):
+    """The batched on-device post of every signal: ([wav file bytes, or the exception wav_bytes_on_device raises for that
+    signal], LKFS [n], gain [n])."""
+    import ctypes as C
+    from . import _lib
+    lib = _lib.load()
+    ws_ = [w.detach().reshape(-1).to(torch.float32) for w in wavs]
+    dev = ws_[0].device
+    assert all(w.is_cuda and w.device == dev for w in ws_), "wav_bytes_on_device_batch expects device tensors on one device"
+    lens = [w.numel() for w in ws_]
+    n, total = len(ws_), sum(lens)
+    cap = _POST_BATCH_WS.get(dev)
+    if cap is None or cap[0] < n or cap[1] < total:
+        nb, ns = max(n, 32, cap[0] if cap else 0), max(total, 1 << 20, cap[1] if cap else 0)
+        cap = (nb, ns, torch.empty(lib.mvb_audio_post_batch_workspace_bytes(nb, ns), dtype=torch.uint8, device=dev))
+        _POST_BATCH_WS[dev] = cap
+    flat = torch.cat(ws_).contiguous()
+    pcm = torch.empty(total, dtype=torch.int16, device=dev)
+    stats = torch.empty(n, 2, dtype=torch.float32, device=dev)
+    st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    _lib.check(lib.mvb_audio_post_batch(flat.data_ptr(), n, (C.c_int32 * n)(*lens), int(sample_rate), float(loudness_headroom_db),
+                                        int(bool(loudness_compressor)), cap[2].data_ptr(), cap[0], cap[1], pcm.data_ptr(), None,
+                                        stats.data_ptr(), st))
+    stats = stats.cpu()
+    pcm = pcm.cpu().numpy().astype("<i2")
+    out, pos = [], 0
+    for i, (w, k) in enumerate(zip(ws_, lens)):
+        if stats[i, 0] != stats[i, 0]:
+            out.append(_undefined_meter_error(w, sample_rate, f"signal {i}: "))
+        else:
+            body = pcm[pos:pos + k].tobytes()
+            out.append(_wav_header(len(body), sample_rate) + body)
+        pos += k
+    return out, stats[:, 0].tolist(), stats[:, 1].tolist()
+
+
+def wav_bytes_on_device_batch(wavs, sample_rate: int, loudness_headroom_db: float = LOUDNESS_HEADROOM_DB,
+                              loudness_compressor: bool = True):
+    """``[wav_bytes_on_device(w, sample_rate) for w in wavs]`` with one launch set for the whole list (the signals are
+    concatenated on the device).  Signal i's bytes equal ``wav_bytes_on_device(wavs[i], sample_rate)``; for a signal
+    whose loudness is undefined, this raises what ``wav_bytes_on_device`` raises for it, naming the signal's index (the
+    first such signal)."""
+    if not wavs:
+        return []
+    out, _, _ = _post_batch(wavs, sample_rate, loudness_headroom_db, loudness_compressor)
+    for r in out:
+        if isinstance(r, Exception):
+            raise r
+    return out

@@ -20,7 +20,7 @@ import time
 import uuid
 from datetime import datetime
 from pathlib import Path
-from typing import Literal, Optional
+from typing import List, Literal, Optional
 
 import numpy as np
 import torch
@@ -82,10 +82,14 @@ class TTS:
         torch.manual_seed(seed)                                                        # inference.py:69-70
         ck2 = torch.load(f"{self._model_dir}/second_stage.pt", map_location="cpu", weights_only=False)
         tok2 = TrainedBPETokeniser(**ck2["meta"]["tokenizer"])
-        self.llm_second_stage = SecondStage(ck2, device=device, tokenizer=tok2)
+        self.llm_second_stage = SecondStage(ck2, device=device, tokenizer=tok2, max_batch=max_utts)
         if encodec_state_dict is None:
             encodec_state_dict = torch.load(f"{self._model_dir}/encodec_24khz.pt", map_location="cpu", weights_only=False)
-        self.codec = EncodecDecodeEngine(encodec_state_dict, device=device)
+        # synthesise_batch decodes up to max_utts utterances (at most 32) per launch set, 10 s of audio each on average;
+        # longer batches are split
+        codec_batch = min(max_utts, 32)
+        self.codec = EncodecDecodeEngine(encodec_state_dict, device=device, max_batch=codec_batch,
+                                         max_total_frames=codec_batch * 750 if codec_batch > 1 else None)
         # decoders.py:13: MultiBandDiffusion.get_mbd_24khz(bw=6) -- here: {"models", "proc", "settings"} (see mvb200/mbd.py)
         self.mbd = None
         mbd_path = f"{self._model_dir}/multiband_diffusion.pt"
@@ -171,3 +175,63 @@ class TTS:
         dt = time.time() - start
         print(f"\nSaved audio to {path} ({len(chunks)} chunks, {wav.shape[-1] / 24000.0:.1f} s of audio in {dt:.2f} s)")
         return path
+
+    def synthesise_batch(self, texts: List[str], spk_ref_paths: List[str], top_p=0.95, guidance_scale=3.0, temperature=1.0,
+                         seed: Optional[int] = None) -> List[Optional[str]]:
+        """N texts with N speaker references in one batch, one wav file per text, returned in input order (the reference's
+        ``_sample_utterance_batch``, inference.py:438-517): stage 1 as one continuous batch over the ``max_utts`` KV
+        slots, stage 2 in batches of ``max_utts``, the EnCodec decode and the loudness post-processing batched on the
+        device (the diffusion refinement, when loaded, per utterance).  An utterance shorter than 400 ms, or one whose
+        loudness is undefined, gets None and the others are still written (the reference returns None where decoding
+        fails, inference.py:330-336).  ``seed`` fixes the result: request i's stage-1 draws come from a Philox stream
+        seeded with ``seed + i`` (``serving.seeded_noise``) and stage 2 samples with ``seed``."""
+        from .audio_out import LOUDNESS_HEADROOM_DB, _post_batch
+        from .fast_inference_utils import encode_tokens
+        from .serving import ContinuousBatcher, seeded_noise
+        if len(texts) != len(spk_ref_paths):
+            raise ValueError(f"{len(texts)} texts but {len(spk_ref_paths)} speaker references")
+        if not texts:
+            return []
+        texts = [normalize_text(t) for t in texts]
+        embs = {}
+        for p in spk_ref_paths:                                # one embedding per distinct reference (disk-cached for audio)
+            if p not in embs:
+                embs[p] = load_speaker_embedding(p, self.smodel)
+        spk = [embs[p] for p in spk_ref_paths]
+        start = time.time()
+        cb = ContinuousBatcher(self.model)
+        ids = []
+        for i, (t, e) in enumerate(zip(texts, spk)):
+            prompt = encode_tokens(self.tokenizer, t, device="cpu")
+            kw = dict(top_p=top_p, guidance_scale=guidance_scale, temperature=temperature)
+            if seed is not None:
+                noise = seeded_noise(self.model, prompt.numel(), seed + i)
+                kw.update(max_new_tokens=noise.shape[0], noise=noise)
+            ids.append(cb.submit(prompt, e, **kw))
+        toks = cb.run_until_done()
+        extracted = [flattened_interleaved_decode(toks[rid].tolist(), self.END_OF_AUDIO_TOKEN)[1] for rid in ids]
+        codes = self.llm_second_stage.non_causal_sample(
+            texts=texts, encodec_tokens=[torch.tensor(x, dtype=torch.int32).unsqueeze(0) for x in extracted],
+            speaker_embs=torch.stack(spk), batch_size=len(texts), top_k=200, temperature=1.0, seed=seed)
+        # 400 ms = 9600 samples = 30 frames at 320 samples per frame (decoders.py:88-91)
+        ok = [i for i, c in enumerate(codes) if c.shape[-1] * self.codec.upsample >= 9600]
+        wavs = self.codec.decode_batch([codes[i] for i in ok])
+        if self.mbd is not None:
+            wavs = [self.mbd.tokens_to_wav(self.codec.decode_latent(codes[i]), w) for i, w in zip(ok, wavs)]
+        files, _, _ = _post_batch(wavs, 24000, LOUDNESS_HEADROOM_DB, True) if wavs else ([], [], [])
+        paths: List[Optional[str]] = [None] * len(texts)
+        for i in range(len(texts)):
+            if i not in ok:
+                print(f"utterance {i}: wav predicted is shorter than 400ms! ({codes[i].shape[-1]} frames)")
+        for i, f in zip(ok, files):
+            if isinstance(f, Exception):
+                print(f"utterance {i}: post-processing failed: {f}")
+                continue
+            name = f"synth_{datetime.now().strftime('%y-%m-%d--%H-%M-%S')}_{texts[i].replace(' ', '_')[:25]}_{uuid.uuid4()}"
+            path = str(Path(self.output_dir).resolve() / name) + ".wav"
+            with open(path, "wb") as fh:
+                fh.write(f)
+            paths[i] = path
+        dt = time.time() - start
+        print(f"\nSaved {sum(p is not None for p in paths)} of {len(texts)} utterances in {dt:.2f} s")
+        return paths

@@ -63,6 +63,18 @@ def chunk_text(text: str, max_chars: int = MAX_CHARS) -> List[str]:
     return chunks
 
 
+def seeded_noise(model, prompt_len: int, seed: int, max_new_tokens: Optional[int] = None) -> torch.Tensor:
+    """Exp(1) draws [max_new, vocab] on the model's device from torch's Philox generator seeded with ``seed``, for
+    ``ContinuousBatcher.submit(..., max_new_tokens=max_new, noise=...)``.  A request's tokens then depend on its seed
+    alone, not on the slot it is admitted to (the engine's own on-device stream is keyed on the slot).  Returns the
+    draws; their first dimension is the ``max_new`` to submit with."""
+    block = model.config.block_size
+    max_new = block - int(prompt_len) if max_new_tokens is None else int(max_new_tokens)
+    max_new = max(1, min(max_new, model._cfg.max_new))
+    g = torch.Generator(device=model.device).manual_seed(int(seed))
+    return torch.empty((max_new, model.config.vocab_size), dtype=torch.float32, device=model.device).exponential_(1, generator=g)
+
+
 @dataclass
 class _Request:
     rid: int

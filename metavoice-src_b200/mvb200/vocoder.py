@@ -5,7 +5,7 @@ The multi-band diffusion stage is not implemented (unpinned: no source, no weigh
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict
+from typing import Dict, List, Optional
 
 import torch
 
@@ -27,7 +27,11 @@ def _fold(sd, prefix):
 
 
 class EncodecDecodeEngine:
-    def __init__(self, state_dict: Dict[str, torch.Tensor], device="cuda", max_frames: int = 2048, n_q: int = 8):
+    def __init__(self, state_dict: Dict[str, torch.Tensor], device="cuda", max_frames: int = 2048, n_q: int = 8,
+                 max_batch: int = 1, max_total_frames: Optional[int] = None):
+        """``max_batch`` > 1 allocates the workspace of ``decode_batch`` / ``decode_latent_batch`` for up to ``max_batch``
+        (<= 32) utterances and ``max_total_frames`` frames in all (default ``max_batch * max_frames``); larger requests
+        are split into several launch sets."""
         sd = state_dict
         tensors = [sd[f"quantizer.layers.{q}.codebook.embed"].float() for q in range(n_q)]
         cw = lambda p: [_fold(sd, p + ".conv"), sd[p + ".conv.bias"].float()]
@@ -65,6 +69,12 @@ class EncodecDecodeEngine:
             _lib.check(self._lib.mvb_voc_create(C.byref(cfg), self._arena.data_ptr(), self._arena.numel(),
                                                 (C.c_uint64 * len(offs))(*offs), self._ws.data_ptr(), C.byref(h)))
         self._h = h
+        self.max_batch, self.max_total_frames, self._bws = max_batch, max_total_frames or max_batch * max_frames, None
+        if max_batch > 1:
+            bwsb = self._lib.mvb_voc_batch_workspace_bytes(C.byref(cfg), max_batch, self.max_total_frames)
+            if bwsb == 0:
+                _lib.check(_lib.MVB_ERR_ARG)
+            self._bws = torch.zeros(bwsb, dtype=torch.uint8, device=self.device)
         self.upsample = 1
         for r in RATIOS:
             self.upsample *= r
@@ -109,3 +119,51 @@ class EncodecDecodeEngine:
         out = torch.empty(c.shape[1] * self.upsample, dtype=torch.float32, device=self.device)
         _lib.check(self._lib.mvb_voc_decode(self._h, c.data_ptr(), c.shape[1], out.data_ptr(), self._st()))
         return out
+
+    def _groups(self, lens: List[int]) -> List[range]:
+        """Consecutive runs of utterances that fit the batch workspace (<= max_batch of them, <= max_total_frames)."""
+        groups, s0, tot = [], 0, 0
+        for i, t in enumerate(lens):
+            if i > s0 and (i - s0 == self.max_batch or tot + t > self.max_total_frames):
+                groups.append(range(s0, i))
+                s0, tot = i, 0
+            tot += t
+        groups.append(range(s0, len(lens)))
+        return groups
+
+    def _batch(self, fn: str, codes: List[torch.Tensor], rows: int, per_frame: int) -> List[torch.Tensor]:
+        cs = [c.to(self.device, torch.int32).contiguous() for c in codes]
+        lens = [int(c.shape[1]) for c in cs]
+        out = torch.empty(rows * sum(lens) * per_frame, dtype=torch.float32, device=self.device)
+        pos = 0
+        for g in self._groups(lens):
+            flat = torch.cat([cs[i].reshape(-1) for i in g])
+            T = (C.c_int32 * len(g))(*[lens[i] for i in g])
+            _lib.check(getattr(self._lib, fn)(self._h, len(g), flat.data_ptr(), T, self._bws.data_ptr(), self.max_batch,
+                                              self.max_total_frames, out[pos:].data_ptr(), self._st()))
+            pos += rows * per_frame * sum(lens[i] for i in g)
+        res, pos = [], 0
+        for t in lens:
+            n = rows * t * per_frame
+            res.append(out[pos:pos + n].view(rows, t * per_frame) if rows > 1 else out[pos:pos + n])
+            pos += n
+        return res
+
+    @torch.no_grad()
+    def decode_batch(self, codes: List[torch.Tensor]) -> List[torch.Tensor]:
+        """[codes int [n_q, T_i]] -> [waveform fp32 [T_i * 320]], each bit-identical to ``decode(codes[i])``.  One launch set
+        per group of utterances that fits the batch workspace (``max_batch``); with ``max_batch=1`` a loop over ``decode``."""
+        if not codes:
+            return []
+        if self._bws is None:
+            return [self.decode(c) for c in codes]
+        return self._batch("mvb_voc_decode_batch", codes, 1, self.upsample)
+
+    @torch.no_grad()
+    def decode_latent_batch(self, codes: List[torch.Tensor]) -> List[torch.Tensor]:
+        """[codes int [n_q, T_i]] -> [latent [hidden, T_i]], each bit-identical to ``decode_latent(codes[i])``."""
+        if not codes:
+            return []
+        if self._bws is None:
+            return [self.decode_latent(c) for c in codes]
+        return self._batch("mvb_voc_decode_latent_batch", codes, self.cfg.hidden, 1)
