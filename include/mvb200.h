@@ -227,7 +227,8 @@ int mvb_mbd_conv_test(int32_t kind, const float* d_x, int32_t Cin, int32_t Tin, 
                       const float* d_gn_b, int32_t groups, const float* d_bias, const float* d_emb, const float* d_resid,
                       float* d_y, int32_t use_tc, void* stream);
 /* Test hooks for the EnCodec decoder and audio post-processing kernels (not part of the drop-in surface):
- *   mvb_voc_op_test     : one launch of csrc/vocoder.cu exactly as mvb_voc_decode makes it.  op 0: k_conv1d<k>, k = 1 / 3 / 7,
+ *   mvb_voc_op_test     : one launch of a csrc/vocoder.cu kernel with a single segment, through the launch helpers of
+ *                         mvb_voc_decode and mvb_voc_decode_batch (every kernel serves both).  op 0: k_conv1d<k>, k = 1 / 3 / 7,
  *                         d_x [Cin, T] -> d_y [Cout, T], d_w [Cout, Cin, k], d_b [Cout] or NULL, ELU on the input when
  *                         elu_in, added to d_y when accumulate; op 1: k_convtr1d (ELU fused) at ratio r = k in 1..8,
  *                         d_x [Cin, T] -> d_y [Cout, T r], d_w [Cin, Cout, 2 r], d_b [Cout]; op 2: k_lstm_layer, H = Cin
@@ -318,8 +319,9 @@ int mvb_voc_decode_latent(mvb_voc* h, const int32_t* d_codes, int32_t T, float* 
 /* d_codes int32 [n_q, T] -> d_wav fp32 [T * prod(ratios)]  (EncodecModel.decode, one chunk, 24 kHz) */
 int mvb_voc_decode(mvb_voc* h, const int32_t* d_codes, int32_t T, float* d_wav, void* stream);
 /* Batched decode (fam/llm/inference.py:438-517 `_sample_utterance_batch` decodes a batch of utterances): n utterances in
- * one launch set, the two LSTM layers as one grid-barrier loop over max T_i for all of them.  Utterance i is bit-identical
- * to mvb_voc_decode / mvb_voc_decode_latent on it alone.  Layout, with off_i = T_0 + ... + T_{i-1}:
+ * one launch set, the two LSTM layers as one grid-barrier loop over max T_i for all of them.  mvb_voc_decode /
+ * mvb_voc_decode_latent run the same launch sequence over one utterance, and utterance i is bit-identical to them on it
+ * alone.  Layout, with off_i = T_0 + ... + T_{i-1}:
  *   d_codes  int32, utterance i as [n_q, T_i] at n_q off_i;  T: HOST int32 [n];
  *   d_wav    fp32, utterance i as [T_i prod(ratios)] at off_i prod(ratios);  d_latent fp32 [hidden, T_i] at hidden off_i.
  * d_batch_ws: a caller workspace of mvb_voc_batch_workspace_bytes(cfg, max_batch, max_total_frames) bytes (the handle's
@@ -415,9 +417,10 @@ size_t mvb_audio_post_workspace_bytes(int32_t max_samples);
 int mvb_audio_post(const float* d_wav, int32_t n_samples, int32_t sample_rate, float loudness_headroom_db,
                    int32_t loudness_compressor, void* d_workspace, int16_t* d_pcm16, float* d_wav_out,
                    float* d_lkfs_gain, void* stream);
-/* mvb_audio_post over n signals with one launch set.  d_wav fp32 and d_pcm16 / d_wav_out: signal i at off_i = n_0 + ... +
- * n_{i-1} (n_samples: HOST int32 [n]); d_lkfs_gain optional fp32 [n][2].  Signal i's PCM, LKFS and gain are bit-identical to
- * mvb_audio_post on it alone, edge cases included, and no signal's values affect another's.  d_workspace:
+/* mvb_audio_post over n signals with one launch set per 32 signals (mvb_audio_post is the same launch set over one).
+ * d_wav fp32 and d_pcm16 / d_wav_out: signal i at off_i = n_0 + ... + n_{i-1} (n_samples: HOST int32 [n]); d_lkfs_gain
+ * optional fp32 [n][2].  Signal i's PCM, LKFS and gain are bit-identical to mvb_audio_post on it alone, edge cases
+ * included, and no signal's values affect another's.  d_workspace:
  * mvb_audio_post_batch_workspace_bytes(max_batch, max_total_samples) bytes, passed with the capacities it was sized for.
  * MVB_ERR_ARG unless 1 <= n <= max_batch, every n_i >= 1 and sum n_i <= max_total_samples; MVB_ERR_UNSUPPORTED when a
  * signal exceeds 15,996 gating blocks; both before anything is launched. */

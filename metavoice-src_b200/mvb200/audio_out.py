@@ -74,50 +74,28 @@ def read_wav_pcm16(path: str):
 
 
 # ---- on-device variant (SURVEY.md row N2): loudness meter, gain, compressor and PCM16 conversion in libmvb200 -----------
-_POST_WS = {}
-
-
 def wav_bytes_on_device(wav: torch.Tensor, sample_rate: int, loudness_headroom_db: float = LOUDNESS_HEADROOM_DB,
                         loudness_compressor: bool = True, return_stats: bool = False):
     """Device fp32 mono waveform [T] (or [1, T]) -> the bytes of the wav FILE `_save_audio` would have written
     (decoders.py:40-47): only 2 bytes per sample cross the PCIe bus, no temp file (serving.py:96-97 re-reads the file it
     just wrote; a server can return these bytes directly)."""
-    import ctypes as C
-    from . import _lib
-    lib = _lib.load()
-    w = wav.detach().reshape(-1).to(torch.float32).contiguous()
-    assert w.is_cuda, "wav_bytes_on_device expects a device tensor (use audio_write_wav for host tensors)"
-    n = w.numel()
-    key = (w.device, max(n, 1 << 17))
-    ws = _POST_WS.get(w.device)
-    if ws is None or ws[0] < n:
-        cap = max(n, 1 << 20)
-        ws = (cap, torch.empty(lib.mvb_audio_post_workspace_bytes(cap), dtype=torch.uint8, device=w.device))
-        _POST_WS[w.device] = ws
-    pcm = torch.empty(n, dtype=torch.int16, device=w.device)
-    stats = torch.empty(2, dtype=torch.float32, device=w.device)
-    st = C.c_void_p(torch.cuda.current_stream(w.device).cuda_stream)
-    _lib.check(lib.mvb_audio_post(w.data_ptr(), n, int(sample_rate), float(loudness_headroom_db), int(bool(loudness_compressor)),
-                                  ws[1].data_ptr(), pcm.data_ptr(), None, stats.data_ptr(), st))
-    lk, gain = stats.cpu().tolist()
-    if lk != lk:
-        raise _undefined_meter_error(w, sample_rate)
-    body = pcm.cpu().numpy().astype("<i2").tobytes()
-    if return_stats:
-        return _wav_header(len(body), sample_rate) + body, lk, gain
-    return _wav_header(len(body), sample_rate) + body
+    assert wav.is_cuda, "wav_bytes_on_device expects a device tensor (use audio_write_wav for host tensors)"
+    (blob,), (lk,), (gain,) = _post_batch([wav], sample_rate, loudness_headroom_db, loudness_compressor)
+    if isinstance(blob, Exception):
+        raise blob
+    return (blob, lk, gain) if return_stats else blob
 
 
-def _undefined_meter_error(w: torch.Tensor, sample_rate: int, prefix: str = "") -> Exception:
+def _undefined_meter_error(w: torch.Tensor, sample_rate: int) -> Exception:
     """The meter is undefined (NaN): what audio_write_wav raises for the same input.  The device only reports NaN for
     non-finite samples, signals above the floor shorter than one 400 ms block (torchaudio's `loudness` raises
     RuntimeError), and signals whose blocks are all gated (NaN loudness: the finiteness assert)."""
     n = w.numel()
     if not bool(w.isfinite().all()):
-        return AssertionError(prefix + "wav contains non-finite samples")
+        return AssertionError("wav contains non-finite samples")
     if n < round(0.4 * sample_rate):
-        return RuntimeError(prefix + f"loudness: {n} samples are shorter than one 400 ms gating block at {sample_rate} Hz")
-    return AssertionError(prefix + f"loudness is undefined: every 400 ms block of the {n}-sample signal is below -70 LKFS")
+        return RuntimeError(f"loudness: {n} samples are shorter than one 400 ms gating block at {sample_rate} Hz")
+    return AssertionError(f"loudness is undefined: every 400 ms block of the {n}-sample signal is below -70 LKFS")
 
 
 def _wav_header(n_bytes: int, sample_rate: int) -> bytes:
@@ -144,24 +122,24 @@ def _post_batch(wavs, sample_rate: int, loudness_headroom_db: float, loudness_co
         nb, ns = max(n, 32, cap[0] if cap else 0), max(total, 1 << 20, cap[1] if cap else 0)
         cap = (nb, ns, torch.empty(lib.mvb_audio_post_batch_workspace_bytes(nb, ns), dtype=torch.uint8, device=dev))
         _POST_BATCH_WS[dev] = cap
-    flat = torch.cat(ws_).contiguous()
+    flat = torch.cat(ws_) if n > 1 else ws_[0].contiguous()   # one signal (wav_bytes_on_device): no device copy
     pcm = torch.empty(total, dtype=torch.int16, device=dev)
     stats = torch.empty(n, 2, dtype=torch.float32, device=dev)
     st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
     _lib.check(lib.mvb_audio_post_batch(flat.data_ptr(), n, (C.c_int32 * n)(*lens), int(sample_rate), float(loudness_headroom_db),
                                         int(bool(loudness_compressor)), cap[2].data_ptr(), cap[0], cap[1], pcm.data_ptr(), None,
                                         stats.data_ptr(), st))
-    stats = stats.cpu()
-    pcm = pcm.cpu().numpy().astype("<i2")
+    stats = stats.cpu().tolist()
+    pcm = pcm.cpu().numpy().astype("<i2", copy=False)
     out, pos = [], 0
-    for i, (w, k) in enumerate(zip(ws_, lens)):
-        if stats[i, 0] != stats[i, 0]:
-            out.append(_undefined_meter_error(w, sample_rate, f"signal {i}: "))
+    for (lk, _), w, k in zip(stats, ws_, lens):
+        if lk != lk:
+            out.append(_undefined_meter_error(w, sample_rate))
         else:
             body = pcm[pos:pos + k].tobytes()
             out.append(_wav_header(len(body), sample_rate) + body)
         pos += k
-    return out, stats[:, 0].tolist(), stats[:, 1].tolist()
+    return out, [s[0] for s in stats], [s[1] for s in stats]
 
 
 def wav_bytes_on_device_batch(wavs, sample_rate: int, loudness_headroom_db: float = LOUDNESS_HEADROOM_DB,
@@ -173,7 +151,7 @@ def wav_bytes_on_device_batch(wavs, sample_rate: int, loudness_headroom_db: floa
     if not wavs:
         return []
     out, _, _ = _post_batch(wavs, sample_rate, loudness_headroom_db, loudness_compressor)
-    for r in out:
+    for i, r in enumerate(out):
         if isinstance(r, Exception):
-            raise r
+            raise type(r)(f"signal {i}: {r}")
     return out

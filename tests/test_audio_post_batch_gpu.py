@@ -1,5 +1,6 @@
 """GPU: the batched on-device audio post (`mvb_audio_post_batch`, through `audio_out.wav_bytes_on_device_batch`) against
-`mvb_audio_post` / `wav_bytes_on_device` on each signal alone.
+`mvb_audio_post` / `wav_bytes_on_device` on each signal alone, which run the same kernels over a group of one signal: no
+signal of a batch may change another's result.
 
 One mixed batch: a 60 s signal at 24 kHz, a 0.3 s tone, a signal with a NaN, an all-gated 5 Hz rumble, a signal below the
 energy floor and one a sample short of a block, plus ordinary speech-like signals between them.  Every signal's PCM16, LKFS and

@@ -1,9 +1,10 @@
 """GPU: the batched EnCodec decode (`mvb_voc_decode_batch` / `mvb_voc_decode_latent_batch`, through
 `EncodecDecodeEngine.decode_batch` / `decode_latent_batch`) against the single-utterance calls.
 
-Every batched kernel computes each tile exactly as the single-utterance launch does (the batched LSTM sums every gate row in
-the same order), so utterance i of a batch must be bit-identical to `mvb_voc_decode` / `mvb_voc_decode_latent` on it alone,
-for B = 1, 3, 8 and 32 ragged utterances of T_i in {8, 9, 31, 257, 375, 2048 = max_frames} in two orders, with code values 0
+The single-utterance calls launch the same kernels with one segment, and every kernel computes a segment's tiles without
+reading another's (the LSTM sums each gate row in the same order whether it runs one sequence or four per pass), so
+utterance i of a batch must be bit-identical to `mvb_voc_decode` / `mvb_voc_decode_latent` on it alone, for B = 1, 3, 8
+and 32 ragged utterances of T_i in {8, 9, 31, 257, 375, 2048 = max_frames} in two orders, with code values 0
 and 1023 present.  The output buffer is NaN-filled with NaN guards on both sides: the call must write every segment and
 nothing else.  One ragged batch is compared with the float64 oracle port at the whole-decode bound of
 test_vocoder_ops_gpu.py.  Sensitivity: the solo results concatenated with two utterances of different length swapped must

@@ -1,6 +1,6 @@
-"""GPU: the EnCodec decoder kernels of csrc/vocoder.cu one at a time (hook `mvb_voc_op_test`, the launches
-`mvb_voc_decode` makes; `k_rvq_decode` through `mvb_voc_decode_latent`) against float64 references of the same operations
-on the kernels' own fp32 inputs.  u = 2^-23.
+"""GPU: the EnCodec decoder kernels of csrc/vocoder.cu one at a time (hook `mvb_voc_op_test`: each kernel launched with
+a single segment, the kernels single and batched decodes both run; `k_rvq_decode` through `mvb_voc_decode_latent`) against
+float64 references of the same operations on the kernels' own fp32 inputs.  u = 2^-23.
 
 k_rvq_decode   latent[c][t] = sum_q book_q[code[q][t]][c], summed in fp32 in codebook order: bit-identical to that sum.
 k_conv1d<K>    causal conv, reflect left padding x[-j] = x[j], optional ELU on every input sample (halo included), bias,
