@@ -244,6 +244,19 @@ int mvb_voc_op_test(int32_t op, const float* d_x, int32_t Cin, int32_t T, const 
 int mvb_audio_post_test(const float* d_wav, int32_t n_samples, int32_t sample_rate, float loudness_headroom_db,
                         int32_t loudness_compressor, int16_t* d_pcm16, float* d_wav_out, float* d_y, float* d_energy,
                         float* d_res, int32_t* n_blocks_out, void* stream);
+/* Test hook for the EnCodec encoder kernels (not part of the drop-in surface): one launch of a csrc/encoder.cu kernel on
+ * a single segment of T samples of which the first V are valid (1 <= V <= T; samples past V are never read into a
+ * written output), through the launch helpers of mvb_enc_encode.
+ *   op 0: k_conv1d_down<k>, stride k in {2, 4, 5, 8} (ELU on the input fused): d_x [Cin, T] (T % k == 0) -> d_y
+ *         [Cout, T / k], of which the first ceil(V / k) columns are written; d_w [Cout, Cin, 2k], d_b [Cout].
+ *   op 1: k_conv1d<k>, k = 1 / 3 / 7, ELU on the input when elu_in: d_x [Cin, T] -> the first V columns of d_y [Cout, T];
+ *         d_w [Cout, Cin, k], d_b [Cout] or NULL.
+ *   op 2: k_rvq_encode over k codebooks: d_x = embeddings [Cin, T] (Cin <= 128), d_w = codebooks [k, 1024, Cin],
+ *         d_codes int32 [k, T], d_y = the residual after the last codebook [Cin, T] or NULL.  |e|^2 is computed as
+ *         mvb_enc_create computes it, into scratch allocated per call.
+ * Synchronises `stream`. */
+int mvb_enc_op_test(int32_t op, const float* d_x, int32_t Cin, int32_t T, int32_t V, const float* d_w, const float* d_b,
+                    int32_t Cout, int32_t k, int32_t elu_in, float* d_y, int32_t* d_codes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Stage 2: the non-causal codebook-expansion model (fam/llm/model.py:195-314 with causal=False) and its sampler
@@ -333,6 +346,49 @@ int mvb_voc_decode_batch(mvb_voc* h, int32_t n, const int32_t* d_codes, const in
                          int32_t max_total_frames, float* d_wav, void* stream);
 int mvb_voc_decode_latent_batch(mvb_voc* h, int32_t n, const int32_t* d_codes, const int32_t* T, void* d_batch_ws,
                                 int32_t max_batch, int32_t max_total_frames, float* d_latent, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Codec, EnCodec-24 kHz encode path: SEANet encoder (causal conv stack with strided downsampling + 2-layer LSTM) and
+ * the residual vector quantiser's encode, i.e. what `EncodecDecoder.get_tokens` (fam/llm/decoders.py:49-64) and the
+ * fine-tuning loader's `_extract_encodec_tokens` (fam/llm/loaders/training_data.py:98-112) evaluate through
+ * transformers EncodecModel.encode (normalize=False, one chunk).  Same checkpoint as mvb_voc; fp32 arena, weight norm
+ * folded.  An input of L samples gives F = ceil(L / prod(ratios)) frames. */
+typedef struct mvb_enc_config {
+  int32_t n_q;          /* codebooks emitted: floor(bandwidth * 1000 / 750), 8 at 6 kbps */
+  int32_t hidden;       /* codebook / embedding dim 128 (<= 128) */
+  int32_t n_filters;    /* 32 */
+  int32_t n_ratios;     /* 4 */
+  int32_t ratios[8];    /* 8, 5, 4, 2 (EncodecConfig.upsampling_ratios; the encoder downsamples by them in reverse), each 2, 4, 5 or 8 */
+  int32_t kernel, res_kernel, last_kernel; /* 7, 3, 7 */
+  int32_t compress;     /* 2 */
+  int32_t max_frames;   /* workspace capacity of mvb_enc_encode in frames */
+} mvb_enc_config;
+typedef struct mvb_enc mvb_enc;
+
+/* The handle's workspace also holds the codebook pointer table and |e_j|^2 of every codebook row, computed in double and
+ * rounded once to fp32 by mvb_enc_create (which synchronises the device). */
+size_t mvb_enc_workspace_bytes(const mvb_enc_config* cfg);
+/* offsets (host), fp32 tensors: codebooks[n_q] [1024, hidden] | conv_in {w[32,1,7], b} | per level, ratios in reverse
+ * (2, 4, 5, 8 at C = 32, 64, 128, 256): res.block1 {w[C/2,C,3], b}, res.block3 {w[C,C/2,1], b}, res.shortcut {w[C,C,1], b},
+ * down {w[2C,C,2r], b} | lstm layer 0 {w_ih, w_hh, b_ih+b_hh} | lstm layer 1 {..} | conv_out {w[hidden,512,7], b}. */
+int mvb_enc_create(const mvb_enc_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
+                   void* d_workspace, mvb_enc** out);
+int mvb_enc_destroy(mvb_enc* h);
+/* d_wav fp32 [L] (mono, 24 kHz) -> d_codes int32 [n_q, F]; d_emb fp32 [hidden, F] (the encoder output before
+ * quantisation, the layout of mvb_voc_decode_latent) or NULL.  1 <= L <= prod(ratios) * max_frames.  The batch of one of
+ * mvb_enc_encode_batch, on the handle's workspace. */
+int mvb_enc_encode(mvb_enc* h, const float* d_wav, int32_t L, int32_t* d_codes, float* d_emb, void* stream);
+/* Batched encode: n utterances in one launch set, the LSTM as one grid-barrier loop over max F_i.  Utterance i is
+ * bit-identical to mvb_enc_encode on it alone.  Layout, with off_i = F_0 + ... + F_{i-1}:
+ *   d_wav    fp32, utterance i's L_i samples at L_0 + ... + L_{i-1};  L: HOST int32 [n];
+ *   d_codes  int32, utterance i as [n_q, F_i] at n_q off_i (the d_codes layout of mvb_voc_decode_batch);
+ *   d_emb    fp32 [hidden, F_i] at hidden off_i, or NULL.
+ * d_batch_ws: mvb_enc_batch_workspace_bytes(cfg, max_batch, max_total_frames) bytes, passed with the capacities it was
+ * sized for.  MVB_ERR_ARG, before anything is launched, unless 1 <= n <= max_batch <= 32, every
+ * 1 <= L_i <= prod(ratios) * max_frames and sum F_i <= max_total_frames.  Calls on one batch workspace must be ordered. */
+size_t mvb_enc_batch_workspace_bytes(const mvb_enc_config* cfg, int32_t max_batch, int32_t max_total_frames);
+int mvb_enc_encode_batch(mvb_enc* h, int32_t n, const float* d_wav, const int32_t* L, void* d_batch_ws, int32_t max_batch,
+                         int32_t max_total_frames, int32_t* d_codes, float* d_emb, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Multi-band-diffusion vocoder (SURVEY.md row a17, second half) == `mbd.tokens_to_wav` (fam/llm/decoders.py:84-85 ->

@@ -37,6 +37,10 @@ class VocConfig(C.Structure):
                 ("compress", C.c_int32), ("max_frames", C.c_int32)]
 
 
+class EncConfig(C.Structure):
+    _fields_ = VocConfig._fields_
+
+
 class MbdConfig(C.Structure):
     _fields_ = [("n_models", C.c_int32), ("chin", C.c_int32), ("hidden", C.c_int32), ("depth", C.c_int32), ("res_blocks", C.c_int32),
                 ("norm_groups", C.c_int32), ("kernel", C.c_int32), ("stride", C.c_int32), ("growth", C.c_float),
@@ -97,6 +101,14 @@ SIGNATURES = {
                                        C.c_void_p, C.c_void_p]),
     "mvb_voc_decode_latent_batch": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.c_int32,
                                               C.c_int32, C.c_void_p, C.c_void_p]),
+    "mvb_enc_workspace_bytes": (C.c_size_t, [C.POINTER(EncConfig)]),
+    "mvb_enc_create": (C.c_int, [C.POINTER(EncConfig), C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64), C.c_void_p,
+                                 C.POINTER(C.c_void_p)]),
+    "mvb_enc_destroy": (C.c_int, [C.c_void_p]),
+    "mvb_enc_encode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "mvb_enc_batch_workspace_bytes": (C.c_size_t, [C.POINTER(EncConfig), C.c_int32, C.c_int32]),
+    "mvb_enc_encode_batch": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.c_int32, C.c_int32,
+                                       C.c_void_p, C.c_void_p, C.c_void_p]),
     "mvb_mbd_workspace_bytes": (C.c_size_t, [C.POINTER(MbdConfig)]),
     "mvb_mbd_create": (C.c_int, [C.POINTER(MbdConfig), C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64), C.c_void_p,
                                  C.POINTER(C.c_void_p)]),
@@ -134,6 +146,8 @@ SIGNATURES = {
     "mvb_s2_sample_test": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_void_p]),
     "mvb_voc_op_test": (C.c_int, [C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                  C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "mvb_enc_op_test": (C.c_int, [C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
                                   C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "mvb_audio_post_test": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p]),

@@ -55,9 +55,9 @@ def slaney_mel_filterbank(sr: int, n_fft: int, n_mels: int) -> np.ndarray:
     return fb.astype(np.float32)
 
 
-def read_wav(path: str):
-    """PCM16 / PCM32 / float32 RIFF wav -> (float32 mono [-1, 1], sample_rate).  Other containers (mp3, flac) need a
-    decoder that is not part of this engine."""
+def read_wav(path: str, mono: bool = True):
+    """PCM16 / PCM32 / float32 RIFF wav -> (float32 mono [-1, 1], sample_rate); with ``mono=False`` the channels are kept,
+    [channels, n].  Other containers (mp3, flac) need a decoder that is not part of this engine."""
     with open(path, "rb") as f:
         data = f.read()
     if data[:4] != b"RIFF" or data[8:12] != b"WAVE":
@@ -82,6 +82,8 @@ def read_wav(path: str):
         x = np.frombuffer(pcm, dtype="<f4").astype(np.float32)
     else:
         raise NotImplementedError(f"{path}: wav format tag {tag} / {bits} bit")
+    if not mono:
+        return np.ascontiguousarray(x.reshape(-1, ch).T), sr
     if ch > 1:
         x = x.reshape(-1, ch).mean(axis=1)          # librosa.load(mono=True)
     return x, sr

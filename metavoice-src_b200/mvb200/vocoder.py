@@ -167,3 +167,166 @@ class EncodecDecodeEngine:
         if self._bws is None:
             return [self.decode_latent(c) for c in codes]
         return self._batch("mvb_voc_decode_latent_batch", codes, self.cfg.hidden, 1)
+
+
+def _encoder_tensors(sd: Dict[str, torch.Tensor], n_q: int) -> List[torch.Tensor]:
+    """The ``mvb_enc_create`` arena order (include/mvb200.h) from an ``EncodecModel`` state dict."""
+    tensors = [sd[f"quantizer.layers.{q}.codebook.embed"].float() for q in range(n_q)]
+    cw = lambda p: [_fold(sd, p + ".conv"), sd[p + ".conv.bias"].float()]   # noqa: E731
+    tensors += cw("encoder.layers.0")
+    i = 1
+    for _ in RATIOS:                      # encoder.layers: resnet block i, ELU i + 1, strided conv i + 2
+        tensors += cw(f"encoder.layers.{i}.block.1") + cw(f"encoder.layers.{i}.block.3") + \
+            cw(f"encoder.layers.{i}.shortcut") + cw(f"encoder.layers.{i + 2}")
+        i += 3
+    for l in range(2):
+        g = lambda k: sd[f"encoder.layers.{i}.lstm.{k}_l{l}"].float()      # noqa: E731
+        tensors += [g("weight_ih"), g("weight_hh"), g("bias_ih") + g("bias_hh")]
+    tensors += cw(f"encoder.layers.{i + 2}")
+    return tensors
+
+
+class EncodecEncodeEngine:
+    """EnCodec-24 kHz encode path on the device (csrc/encoder.cu): waveform fp32 at 24 kHz -> SEANet encoder -> RVQ codes,
+    i.e. ``EncodecModel.encode(wav, bandwidth)`` of the default 24 kHz config (normalize=False, one chunk) that
+    ``EncodecDecoder.get_tokens`` (fam/llm/decoders.py:49-64) and the fine-tuning loader call.  Reads the same
+    ``facebook/encodec_24khz`` state dict as ``EncodecDecodeEngine``; ``n_q = floor(bandwidth * 1000 / 750)`` (8 at 6 kbps).
+    An input of L samples gives ``ceil(L / 320)`` frames; any L >= 1 up to ``320 * max_frames`` is accepted."""
+
+    def __init__(self, state_dict: Dict[str, torch.Tensor], device="cuda", max_frames: int = 2048, n_q: int = 8,
+                 max_batch: int = 1, max_total_frames: Optional[int] = None):
+        """``max_batch`` > 1 allocates the workspace of ``encode_batch`` for up to ``max_batch`` (<= 32) utterances and
+        ``max_total_frames`` frames in all (default ``max_batch * max_frames``); larger requests are split."""
+        tensors = _encoder_tensors(state_dict, n_q)
+        offs, total = [], 0
+        for t in tensors:
+            offs.append(total)
+            total = (total + t.numel() * 4 + 255) // 256 * 256
+        arena = torch.zeros(total, dtype=torch.uint8)
+        for t, o in zip(tensors, offs):
+            arena[o:o + t.numel() * 4] = t.contiguous().reshape(-1).view(torch.uint8)
+        self.device = torch.device(device)
+        self._arena = arena.to(self.device)
+        cfg = _lib.EncConfig()
+        cfg.n_q, cfg.hidden, cfg.n_filters, cfg.n_ratios = n_q, tensors[0].shape[1], 32, len(RATIOS)
+        for k, r in enumerate(RATIOS):
+            cfg.ratios[k] = r
+        cfg.kernel, cfg.res_kernel, cfg.last_kernel, cfg.compress, cfg.max_frames = 7, 3, 7, 2, max_frames
+        self.cfg, self._lib = cfg, _lib.load()
+        self.hop = 1
+        for r in RATIOS:
+            self.hop *= r
+        wsb = self._lib.mvb_enc_workspace_bytes(C.byref(cfg))
+        if wsb == 0:
+            _lib.check(_lib.MVB_ERR_UNSUPPORTED)
+        self._ws = torch.zeros(wsb, dtype=torch.uint8, device=self.device)
+        h = C.c_void_p()
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.mvb_enc_create(C.byref(cfg), self._arena.data_ptr(), self._arena.numel(),
+                                                (C.c_uint64 * len(offs))(*offs), self._ws.data_ptr(), C.byref(h)))
+        self._h = h
+        self.max_batch, self.max_total_frames, self._bws = max_batch, max_total_frames or max_batch * max_frames, None
+        if max_batch > 1:
+            bwsb = self._lib.mvb_enc_batch_workspace_bytes(C.byref(cfg), max_batch, self.max_total_frames)
+            if bwsb == 0:
+                _lib.check(_lib.MVB_ERR_ARG)
+            self._bws = torch.zeros(bwsb, dtype=torch.uint8, device=self.device)
+        # multiply-adds per output sample of every layer, with the layer's output rate in samples per frame
+        terms, m, k = [(tensors[n_q].numel(), self.hop)], self.hop, n_q + 2
+        for r in reversed(RATIOS):
+            terms += [(tensors[k + 2 * j].numel(), m) for j in range(3)]       # resnet block k3, k1, shortcut
+            m //= r
+            terms.append((tensors[k + 6].numel(), m))                          # strided conv
+            k += 8
+        terms += [(tensors[k + 3 * l].numel() + tensors[k + 3 * l + 1].numel(), 1) for l in range(2)]
+        terms.append((tensors[k + 6].numel(), 1))
+        self._flop_terms = terms
+        self._rvq_macs = n_q * tensors[0].numel()                              # every codebook row meets every frame
+
+    def frames(self, n_samples: int) -> int:
+        return -(-int(n_samples) // self.hop)
+
+    def flops(self, n_samples: int) -> float:
+        """fp32 FLOPs (2 x multiply-adds) of one encode of ``n_samples`` samples, counted from shapes: the conv stack,
+        the LSTM and the codebook search."""
+        F = self.frames(n_samples)
+        return float(sum(2.0 * n * m * F for n, m in self._flop_terms) + 2.0 * self._rvq_macs * F)
+
+    def close(self):
+        if getattr(self, "_h", None) is not None:
+            self._lib.mvb_enc_destroy(self._h)
+            self._h = None
+
+    __del__ = close
+
+    def _st(self):
+        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def _run(self, wav: torch.Tensor, emb: bool):
+        x = wav.to(self.device, torch.float32).contiguous().reshape(-1)
+        F = self.frames(x.numel())
+        codes = torch.empty((self.cfg.n_q, F), dtype=torch.int32, device=self.device)
+        e = torch.empty((self.cfg.hidden, F), dtype=torch.float32, device=self.device) if emb else None
+        _lib.check(self._lib.mvb_enc_encode(self._h, x.data_ptr(), x.numel(), codes.data_ptr(),
+                                            e.data_ptr() if emb else None, self._st()))
+        return codes, e
+
+    @torch.no_grad()
+    def encode(self, wav: torch.Tensor) -> torch.Tensor:
+        """waveform fp32 [L] at 24 kHz -> codes int32 [n_q, ceil(L / 320)] (the layout ``EncodecDecodeEngine.decode`` takes)."""
+        return self._run(wav, False)[0]
+
+    @torch.no_grad()
+    def embed(self, wav: torch.Tensor) -> torch.Tensor:
+        """waveform fp32 [L] -> the encoder output before quantisation, fp32 [128, ceil(L / 320)]."""
+        return self._run(wav, True)[1]
+
+    @torch.no_grad()
+    def encode_mono(self, wav: torch.Tensor) -> torch.Tensor:
+        """[channels, L] -> codes of the channel mean: ``_extract_encodec_tokens`` (fam/llm/loaders/training_data.py:98-112)."""
+        return self.encode(wav.float().mean(dim=0) if wav.dim() == 2 else wav)
+
+    def _groups(self, lens: List[int]) -> List[range]:
+        return EncodecDecodeEngine._groups(self, [self.frames(n) for n in lens])
+
+    @torch.no_grad()
+    def encode_batch(self, wavs: List[torch.Tensor]) -> List[torch.Tensor]:
+        """[waveform fp32 [L_i]] -> [codes int32 [n_q, ceil(L_i / 320)]], each bit-identical to ``encode(wavs[i])``.  One
+        launch set per group of utterances that fits the batch workspace (``max_batch``); with ``max_batch=1`` a loop over
+        ``encode``."""
+        if not wavs:
+            return []
+        if self._bws is None:
+            return [self.encode(w) for w in wavs]
+        xs = [w.to(self.device, torch.float32).contiguous().reshape(-1) for w in wavs]
+        lens = [int(x.numel()) for x in xs]
+        n_q = self.cfg.n_q
+        out = torch.empty(n_q * sum(self.frames(n) for n in lens), dtype=torch.int32, device=self.device)
+        pos = 0
+        for g in self._groups(lens):
+            flat = torch.cat([xs[i] for i in g])
+            L = (C.c_int32 * len(g))(*[lens[i] for i in g])
+            _lib.check(self._lib.mvb_enc_encode_batch(self._h, len(g), flat.data_ptr(), L, self._bws.data_ptr(), self.max_batch,
+                                                      self.max_total_frames, out[pos:].data_ptr(), None, self._st()))
+            pos += n_q * sum(self.frames(lens[i]) for i in g)
+        res, pos = [], 0
+        for n in lens:
+            F = self.frames(n)
+            res.append(out[pos:pos + n_q * F].view(n_q, F))
+            pos += n_q * F
+        return res
+
+
+def get_tokens(engine: EncodecEncodeEngine, audio_path: str) -> List[List[int]]:
+    """``EncodecDecoder.get_tokens`` (fam/llm/decoders.py:49-64): audio file -> codes [n_q][F] as nested lists.
+
+    RIFF/WAVE only (PCM16 / PCM32 / float32); mp3 and flac raise ``NotImplementedError`` as the speaker-reference reader
+    does.  The reference passes the channels as the batch and returns the first one (``tokens[0][0]``), so a
+    multi-channel file gives the codes of its first channel.  A file not at 24 kHz is resampled on the host with the
+    polyphase resampler of the speaker encoder; the reference uses ``julius.resample_frac``, so that path is not pinned.
+    The fine-tuning loader's variant (``_extract_encodec_tokens``, training_data.py:98-112) encodes the channel mean
+    instead: ``engine.encode_mono``."""
+    from .speaker_encoder import read_wav, resample
+    x, sr = read_wav(audio_path, mono=False)
+    x = resample(x[0], sr, 24000)
+    return engine.encode(torch.from_numpy(x)).tolist()
