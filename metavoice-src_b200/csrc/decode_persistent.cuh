@@ -8,8 +8,9 @@
 //     swizzle) into a ring of smem stages, KV-cache tiles via cp.async.bulk into two dedicated (K,V) tile slots -- all
 //     guarded by full/empty mbarriers.  Weights do not depend on activations, so the producer never waits for a grid
 //     barrier: the HBM stream keeps running across phase, layer AND token boundaries (the next token's first weight
-//     tiles land while the grid is still sampling).  While the ring is full it pulls the next PC_PF_AHEAD weight tiles
-//     of its schedule into L2 (cp.async.bulk.prefetch.tensor), so that HBM keeps streaming while the grid synchronises.
+//     tiles land while the grid is still sampling).  It issues no L2 prefetch beyond the ring: on an H100 SXM at 700 W
+//     prefetching 1 to 32 tiles ahead (cp.async.bulk.prefetch.tensor while the ring is full) made batch-1 decode
+//     13-68 % slower.
 //   * warp 1 = MMA WARP: the weight tile [128 rows x 64 k] is the A operand, the staged activation rows (hi + lo bf16
 //     halves, NB rows) the B operand of mma.sync.m16n8k16; fragments come from the 128B-swizzled tiles by ldmatrix and the
 //     hi and lo products accumulate into one fp32 register tile [128 x NB/2].  At the end of a tile the warp parks the
@@ -35,7 +36,6 @@
 namespace mvb {
 
 constexpr int PC_THREADS = 192;      // producer warp + MMA warp + 4 compute warps
-constexpr int PC_PF_AHEAD = 8;       // weight tiles the producer prefetches into L2 ahead of the smem ring
 constexpr int PC_KV_TILE_BYTES = 16384;   // K (or V) tile of one (row, head): 64 bf16 / 32 fp32 positions
 constexpr int PC_RPAD = 16;          // rows of the fp32 activation buffers (8 utterances x 2 CFG rows)
 constexpr int PC_BKB_MAX = 12;       // k-blocks of the activation operand one CTA may own in a phase
@@ -312,12 +312,6 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
   const PcSlice s_qkv = pc_slice(p.m_qkv, cta), s_o = pc_slice(p.m_o, cta), s_w13 = pc_slice(p.m_w13, cta),
                 s_w2 = pc_slice(p.m_w2, cta), s_head = pc_slice(p.m_head, cta);
   const int T1 = p.m_w13.T >> 1;  // w1 tiles; tiles >= T1 belong to w3
-  // Flat view of this CTA's weight-tile schedule of ONE token (layer-major: qkv, wo, w1|w3, w2; then the head)
-  const int nk_q = s_qkv.kb1 - s_qkv.kb0, nk_o = s_o.kb1 - s_o.kb0, nk_f = s_w13.kb1 - s_w13.kb0,
-            nk_2 = s_w2.kb1 - s_w2.kb0, nk_h = s_head.kb1 - s_head.kb0;
-  const int c_q = s_qkv.nt * nk_q, c_o = s_o.nt * nk_o, c_f = s_w13.nt * nk_f, c_2 = s_w2.nt * nk_2;
-  const int per_layer = c_q + c_o + c_f + c_2;
-  const int total_tiles = p.n_layer * per_layer + s_head.nt * nk_h;
 
   // There is no warp 6 (PC_THREADS = 192).  Testing for it anyway makes ptxas place the producer's loop ahead of the
   // compute warps' code; with `warp == 0` alone the loop lands at the end of the kernel, and 8-utterance decode measured
@@ -327,30 +321,8 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
     // The whole warp walks the schedule (warp-uniform control flow and operands); one elected lane issues the TMA /
     // bulk-copy instructions.  Issuing them from a `lane == 0` branch makes the compiler wrap each UTMALDG in an
     // ELECT + 4 x R2UR.BROADCAST + vote loop, which capped one producer at a tile per ~0.25 us.
-    auto prefetch_flat = [&](int n) {      // n: index inside one token's schedule
-      const CUtensorMap* tm;
-      const PcSlice* sl;
-      int nk, layer = 0, m;
-      if (n >= p.n_layer * per_layer) {
-        m = n - p.n_layer * per_layer; tm = &tm_head; sl = &s_head; nk = nk_h;
-      } else {
-        layer = n / per_layer;
-        m = n - layer * per_layer;
-        if (m < c_q) { tm = &tm_qkv; sl = &s_qkv; nk = nk_q; }
-        else if (m < c_q + c_o) { m -= c_q; tm = &tm_o; sl = &s_o; nk = nk_o; }
-        else if (m < c_q + c_o + c_f) { m -= c_q + c_o; tm = &tm_w1; sl = &s_w13; nk = nk_f; }
-        else { m -= c_q + c_o + c_f; tm = &tm_w2; sl = &s_w2; nk = nk_2; }
-      }
-      const int ti = m / nk, kb = sl->kb0 + (m - ti * nk);
-      int t = sl->t0 + ti * sl->G;
-      if (sl == &s_w13 && t >= T1) { t -= T1; tm = &tm_w3; }
-      if (ptx::elect_one()) ptx::tma_prefetch_3d(tm, kb * 64, t * TILE_ROWS, layer);
-      __syncwarp();
-    };
-    const long long total_all = (long long)total_tiles * p.n_steps;
     const uint64_t pol = ptx::policy_evict_first();
     uint32_t slot = 0, kv_ctr = 0;
-    long long issued = 0, pf_next = 0;   // L2 prefetch only while the ring is full
     auto gemm_tiles = [&](const CUtensorMap* tmA, const CUtensorMap* tmB2, int split_t, const PcSlice& sl, int layer) {
       for (int i = 0; i < sl.nt; ++i) {
         const int t = sl.t0 + i * sl.G;
@@ -359,17 +331,7 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
         for (int kb = sl.kb0; kb < sl.kb1; ++kb) {
           const auto [s, ph] = ring_pos(slot, STAGES);
           ++slot;
-          const uint32_t eb = ptx::smem_u32(sh.b_empty + s);
-          if (!ptx::mbar_test_wait(eb, ph ^ 1u)) {
-            // the ring is full: spend the idle time pulling upcoming tiles into L2 (non-blocking probe)
-            if (pf_next <= issued) pf_next = issued + 1;      // never prefetch a tile that is about to be loaded
-            while (pf_next < issued + 1 + PC_PF_AHEAD && pf_next < total_all && !ptx::mbar_test_wait(eb, ph ^ 1u)) {
-              prefetch_flat((int)(pf_next % total_tiles));
-              ++pf_next;
-            }
-          }
-          ptx::mbar_wait(eb, ph ^ 1u);
-          ++issued;
+          ptx::mbar_wait(ptx::smem_u32(sh.b_empty + s), ph ^ 1u);
           if (ptx::elect_one()) {
             const uint32_t full = ptx::smem_u32(sh.b_full + s);
             ptx::mbar_arrive_expect_tx(full, STAGE_BYTES);

@@ -36,18 +36,6 @@ __device__ __forceinline__ uint32_t mbar_try_wait(uint32_t bar, uint32_t parity)
       : "memory");
   return ok;
 }
-// Non-blocking probe (try_wait may suspend the thread for a system-dependent time; test_wait returns at once).
-__device__ __forceinline__ uint32_t mbar_test_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return ok;
-}
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
@@ -79,10 +67,6 @@ __device__ __forceinline__ void tma_load_3d_hint(uint32_t dst, const void* tmap,
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4, %5}], [%2], %6;"
       ::"r"(dst), "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "l"(policy) : "memory");
-}
-// Pull a tile into L2 only (no smem, no barrier).
-__device__ __forceinline__ void tma_prefetch_3d(const void* tmap, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];" ::"l"(tmap), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
 // Contiguous global -> shared copy (no tensor map), completing on `bar`.
 __device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
