@@ -204,7 +204,21 @@ int mvb_linear(const void* d_W, int32_t M, int32_t K, const float* d_x, int32_t 
  *                       d_gn_b [Cin]; optional d_bias, d_emb [Cout], d_resid [Cout, Tout]; d_y fp32 [Cout, Tout], Tout =
  *                       Tin, ceil(Tin / stride), Tin * stride.  use_tc != 0: the tensor-core kernel with the engine's
  *                       weight packing; 0: the CUDA-core kernels.
- * Both synchronise `stream`. */
+ *   mvb_mbd_op_test   : one launch of a non-convolution multi-band-diffusion kernel (csrc/mbd.cu) with the engine's launch
+ *                       configuration, without an mvb_mbd handle.  Inputs d_a .. d_e, output d_out (updated in place
+ *                       where noted), sizes i0 .. i2, scalars f0 .. f4; all tensors fp32.  op 0: GroupNorm statistics
+ *                       of d_a [i0, i1] in i2 groups (1 .. 64), eps f0 -> d_out [i2][mean, rstd]; 1: relu(GroupNorm) in
+ *                       place on d_out [i0, i1], i2 groups, statistics d_a, gain d_b, bias d_c; 2: FIR bank, d_out [i0, i1]
+ *                       = d_a [i1] through each row of d_b [i0, i2] with replicate padding (i0 <= 63); 3: unbiased std
+ *                       of the i0 SplitBands bands of x = d_b [i1] from its low-passed copies d_a [i0 - 1, i1] -> d_out
+ *                       [i0]; 4: band mix, d_out [i1] (+= when i2 != 0) sum_b band_b * (d_c / d_d)[b] + d_e[b] over i0
+ *                       bands of (d_a, d_b) as in op 3 (d_d, d_e may be NULL: scale d_c, shift 0); 5: d_out [i0, i1] +=
+ *                       nearest-interpolated d_a [i0, i2]; 6: d_out [i0, i1] = d_a [i0, i2] cropped to i1 + d_b [i0,
+ *                       i1]; 7: schedule step on d_out [i1] with estimate d_a, noise d_b (never read when f2 <= 0),
+ *                       (a, b, sigma, noise scale, clip) = f0 .. f4; 8: d_out [i1] = Box-Muller normals of Philox stream
+ *                       i2 under `seed`; 9: d_out [i1] = sum of the i0 blocks at d_out + m i2 floats; 10: d_out [i1] =
+ *                       d_a * f0.  The fp64 GroupNorm partials are allocated per call.
+ * All three synchronise `stream`. */
 int mvb_gemm_test(int32_t epi, const void* d_W, const void* d_W3, int32_t M, int32_t K, const float* d_x, int32_t ldx,
                   int32_t R, const void* d_gain, float eps, int32_t split_lo, int32_t ksplit_override, float* d_out,
                   int32_t ldo, void* d_kcache, void* d_vcache, const int32_t* d_row_cache, const int32_t* d_row_pos,
@@ -226,6 +240,9 @@ int mvb_mbd_conv_test(int32_t kind, const float* d_x, int32_t Cin, int32_t Tin, 
                       int32_t stride, int32_t dil, int32_t pad, const float* d_gn_stats, const float* d_gn_w,
                       const float* d_gn_b, int32_t groups, const float* d_bias, const float* d_emb, const float* d_resid,
                       float* d_y, int32_t use_tc, void* stream);
+int mvb_mbd_op_test(int32_t op, const float* d_a, const float* d_b, const float* d_c, const float* d_d, const float* d_e,
+                    float* d_out, int32_t i0, int32_t i1, int32_t i2, float f0, float f1, float f2, float f3, float f4,
+                    uint64_t seed, void* stream);
 /* Test hooks for the EnCodec decoder and audio post-processing kernels (not part of the drop-in surface):
  *   mvb_voc_op_test     : one launch of a csrc/vocoder.cu kernel with a single segment, through the launch helpers of
  *                         mvb_voc_decode and mvb_voc_decode_batch (every kernel serves both).  op 0: k_conv1d<k>, k = 1 / 3 / 7,

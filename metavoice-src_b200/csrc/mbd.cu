@@ -30,6 +30,7 @@ namespace {
 // Two stages so that a 4-group norm still fills the machine: GN_SPLIT CTAs per group write fp64 partial sums, one small CTA
 // adds them in a fixed order (run-to-run deterministic).
 constexpr int GN_SPLIT = 64;
+constexpr float GN_EPS = 1e-5f;   // nn.GroupNorm's default
 __global__ void __launch_bounds__(256) k_gn_partial(const float* __restrict__ x, size_t n, double* __restrict__ part) {
   __shared__ double rs[8], rq[8];
   const int g = blockIdx.x, sp = blockIdx.y, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -274,6 +275,10 @@ __global__ void k_randn(float* __restrict__ out, int T, unsigned long long seed,
 // filters: every thread keeps 4 outputs (t, t+256, t+512, t+768) x 2 filters in registers, so one tap costs 4 conflict-free x
 // reads + 2 broadcast coefficient reads for 8 FMAs (the direct form was 2 shared-memory reads per FMA).
 constexpr int FIR_TT = 1024;
+// dynamic shared memory for L taps (the x window [FIR_TT + L - 1] and two filters [L]); the H100 opt-in maximum of 227 KB
+// bounds L at 19029 taps, far above the 5921 of a 64-band bank at 24 kHz
+constexpr size_t FIR_SMEM_MAX = 227 * 1024;
+static size_t fir_smem_bytes(int L) { return (size_t)(FIR_TT + 3 * (size_t)L) * 4; }
 __global__ void __launch_bounds__(256) k_fir_bank(const float* __restrict__ x, int T, const float* __restrict__ bank, int L, int nf,
                                                   float* __restrict__ low) {
   extern __shared__ float sm[];
@@ -404,6 +409,9 @@ static int mbd_validate(const mvb_mbd_config* c) {
   if (!((c->kernel == 8 && c->stride == 4) || (c->kernel == 4 && c->stride == 2)))
     return mvb::set_error(MVB_ERR_UNSUPPORTED, "mbd: (kernel, stride) must be (8, 4) or (4, 2)");
   if (c->chin != 1) return mvb::set_error(MVB_ERR_UNSUPPORTED, "mbd: mono waveforms only (chin = 1)");
+  // the workspace holds GroupNorm partials for 64 groups and three disjoint 64-float statistics slots ([mean, rstd] per group)
+  if (c->norm_groups < 1 || c->norm_groups > 32)
+    return mvb::set_error(MVB_ERR_ARG, "mbd: norm_groups %d out of range (1 .. 32)", c->norm_groups);
   int h = c->hidden;
   for (int i = 0; i < c->depth; ++i) {
     if (h % c->norm_groups) return mvb::set_error(MVB_ERR_ARG, "mbd: channels must be divisible by norm_groups");
@@ -411,6 +419,9 @@ static int mbd_validate(const mvb_mbd_config* c) {
   }
   if (c->proc_bands < 2 || c->proc_bands > 64 || c->eq_bands < 2 || c->eq_bands > 64 || c->n_calls < 1 || c->n_calls > 1000)
     return mvb::set_error(MVB_ERR_ARG, "mbd: band / call counts out of range");
+  for (int L : {c->proc_taps, c->eq_taps})
+    if (L < 1 || fir_smem_bytes(L) > FIR_SMEM_MAX)
+      return mvb::set_error(MVB_ERR_UNSUPPORTED, "mbd: filter length %d (1 .. %d taps)", L, (int)((FIR_SMEM_MAX / 4 - FIR_TT) / 3));
   if (c->max_samples < c->stride) return mvb::set_error(MVB_ERR_ARG, "mbd: max_samples");
   return MVB_OK;
 }
@@ -565,11 +576,11 @@ static int launch_conv(cudaStream_t s, const ConvP& p, int K, int stride) {
   MVB_CK(cudaGetLastError());
   return MVB_OK;
 }
-static int gn_stats(mvb_mbd* h, cudaStream_t s, const float* x, int C, int T, int groups, float* stats) {
-  double* part = reinterpret_cast<double*>(h->base + h->L.gn_part);
+// part: room for groups x GN_SPLIT fp64 (sum, sum of squares) pairs
+static int gn_stats(cudaStream_t s, double* part, const float* x, int C, int T, int groups, float eps, float* stats) {
   const size_t n = (size_t)(C / groups) * T;
   k_gn_partial<<<dim3(groups, GN_SPLIT), 256, 0, s>>>(x, n, part);
-  k_gn_final<<<groups, 32, 0, s>>>(part, groups, (double)n, 1e-5f, stats);
+  k_gn_final<<<groups, 32, 0, s>>>(part, groups, (double)n, eps, stats);
   MVB_CK(cudaGetLastError());
   return MVB_OK;
 }
@@ -626,11 +637,12 @@ static int launch_conv_tc(mvb_mbd* h, cudaStream_t s, const ConvP& p, int widx, 
 static int res_block(mvb_mbd* h, cudaStream_t s, int base, int C, int T, int dil, const float* x, float* tmp, float* out, float* stats,
                      const float* emb) {
   ConvP p{};
-  if (int e = gn_stats(h, s, x, C, T, h->cfg.norm_groups, stats)) return e;
+  double* part = reinterpret_cast<double*>(h->base + h->L.gn_part);
+  if (int e = gn_stats(s, part, x, C, T, h->cfg.norm_groups, GN_EPS, stats)) return e;
   p.x = x; p.Cin = C; p.Tin = T; p.w = h->w(base + 2); p.bias = h->w(base + 3); p.y = tmp; p.Cout = C; p.Tout = T; p.dil = dil; p.pad = dil;
   p.gn_stats = stats; p.gn_w = h->w(base); p.gn_b = h->w(base + 1); p.groups = h->cfg.norm_groups;
   if (int e = h->tc_of[base + 2] >= 0 ? launch_conv_tc(h, s, p, base + 2, 0, 3, 1) : launch_conv(s, p, 3, 1)) return e;
-  if (int e = gn_stats(h, s, tmp, C, T, h->cfg.norm_groups, stats + 64)) return e;
+  if (int e = gn_stats(s, part, tmp, C, T, h->cfg.norm_groups, GN_EPS, stats + 64)) return e;
   p.x = tmp; p.w = h->w(base + 6); p.bias = h->w(base + 7); p.y = out; p.gn_stats = stats + 64; p.gn_w = h->w(base + 4); p.gn_b = h->w(base + 5);
   p.resid = x; p.emb = emb;
   return h->tc_of[base + 6] >= 0 ? launch_conv_tc(h, s, p, base + 6, 0, 3, 1) : launch_conv(s, p, 3, 1);
@@ -641,6 +653,7 @@ static int unet_forward(mvb_mbd* h, cudaStream_t s, int m, int step, const float
   const mvb_mbd_config& c = h->cfg;
   const MbdWs& L = h->L;
   float* stats = reinterpret_cast<float*>(h->base + L.gn);
+  double* part = reinterpret_cast<double*>(h->base + L.gn_part);
   float* tmp[3] = {reinterpret_cast<float*>(h->base + L.tmp[0]), reinterpret_cast<float*>(h->base + L.tmp[1]), reinterpret_cast<float*>(h->base + L.tmp[2])};
   const int pad_k = (c.kernel - c.stride) / 2, G = c.norm_groups;
   int ti = m * h->per_model;
@@ -654,7 +667,7 @@ static int unet_forward(mvb_mbd* h, cudaStream_t s, int m, int step, const float
     p.x = x; p.Cin = Cin; p.Tin = Tl; p.w = h->w(ti); p.y = tmp[0]; p.Cout = C; p.Tout = To; p.dil = 1; p.pad = pad_k;
     if (int e = h->tc_of[ti] >= 0 ? launch_conv_tc(h, s, p, ti, 1, c.kernel, c.stride) : launch_conv(s, p, c.kernel, c.stride)) return e;
     // norm -> relu -> res_blocks: the first ResBlock input is relu(GN(conv)); materialise it (it is also the residual)
-    if (int e = gn_stats(h, s, tmp[0], C, To, G, stats + 128)) return e;
+    if (int e = gn_stats(s, part, tmp[0], C, To, G, GN_EPS, stats + 128)) return e;
     k_gn_relu_inplace<<<GRID_STRIDE_CTAS * 4, 256, 0, s>>>(tmp[0], C, To, C / G, stats + 128, h->w(ti + 1), h->w(ti + 2));
     MVB_CK(cudaGetLastError());
     ti += 3;
@@ -703,7 +716,7 @@ static int unet_forward(mvb_mbd* h, cudaStream_t s, int m, int step, const float
       float* t = a; a = b; b = t;
     }
     ti += 8 * c.res_blocks;
-    if (int e = gn_stats(h, s, a, C, Tsk, G, stats + 128)) return e;
+    if (int e = gn_stats(s, part, a, C, Tsk, G, GN_EPS, stats + 128)) return e;
     const int Cout = lvl == 0 ? 1 : h->ch[lvl - 1];
     const int To = Tsk * c.stride;
     ConvP p{};
@@ -722,14 +735,25 @@ static int unet_forward(mvb_mbd* h, cudaStream_t s, int m, int step, const float
   return MVB_OK;
 }
 
-static int split_lows(mvb_mbd* h, cudaStream_t s, const float* x, int T, int n_bands, const float* bank, int L, float* low) {
-  const size_t smem = (size_t)(FIR_TT + 3 * L) * 4;
-  static PerDeviceOnce attr;
-  if (attr.pending()) { MVB_CK(cudaFuncSetAttribute(k_fir_bank, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024)); attr.mark(); }
-  if (smem > 64 * 1024) return mvb::set_error(MVB_ERR_UNSUPPORTED, "mbd: filter length %d", L);
+// The n_bands - 1 low-passed copies of x [T] through bank [n_bands - 1, L] into low [n_bands - 1, T].  k_fir_bank is opted
+// into 64 KB of dynamic shared memory (every bank up to 55 bands at 24 kHz), and into more, up to the device's opt-in
+// maximum, the first time a longer filter runs on the device.
+static int split_lows(cudaStream_t s, const float* x, int T, int n_bands, const float* bank, int L, float* low) {
+  const size_t smem = fir_smem_bytes(L);
+  static size_t opted[64] = {};
+  int dev = 0;
+  MVB_CK(cudaGetDevice(&dev));
+  size_t& cur = opted[dev >= 0 && dev < 64 ? dev : 0];
+  if (cur == 0 || smem > cur) {
+    const size_t want = smem > 64 * 1024 ? smem : 64 * 1024;
+    int optin = 0;
+    MVB_CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    if (want > (size_t)optin) return mvb::set_error(MVB_ERR_UNSUPPORTED, "mbd: filter length %d needs %zu B of shared memory", L, smem);
+    MVB_CK(cudaFuncSetAttribute(k_fir_bank, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)want));
+    cur = want;
+  }
   k_fir_bank<<<dim3((T + FIR_TT - 1) / FIR_TT, (n_bands - 1 + 1) / 2), 256, smem, s>>>(x, T, bank, L, n_bands - 1, low);
   MVB_CK(cudaGetLastError());
-  (void)h;
   return MVB_OK;
 }
 
@@ -785,7 +809,7 @@ extern "C" int mvb_mbd_tokens_to_wav(mvb_mbd* h, const float* d_cond, int32_t n_
     // MultiBandProcessor.return_sample: bands * (std / target_std) ** power_std + mean, summed; the band models' outputs are
     // added up in model order (one stream: accumulated in place; several streams: per-model buffers summed after the join)
     const int pb = m * h->per_model + h->per_model - 2;
-    if ((rc = split_lows(h, sm, cur, T, c.proc_bands, h->w(g0), c.proc_taps, low_m)) != MVB_OK) break;
+    if ((rc = split_lows(sm, cur, T, c.proc_bands, h->w(g0), c.proc_taps, low_m)) != MVB_OK) break;
     k_band_mix<<<GRID_STRIDE_CTAS * 2, 256, 0, sm>>>(low_m, cur, T, c.proc_bands, h->w(pb), nullptr, h->w(pb + 1), wav_m, multi ? 0 : 1);
     MVB_CK(cudaGetLastError());
     if (multi) MVB_CK(cudaEventRecord(h->ev_join[m], sm));
@@ -803,8 +827,8 @@ extern "C" int mvb_mbd_tokens_to_wav(mvb_mbd* h, const float* d_cond, int32_t n_
   // re_eq(wav, ref = wav_encodec, eq_bands): out = sum_b band_b(wav) * std(band_b(ref)) / std(band_b(wav))
   float* low_w = low;
   float* low_r = low + (size_t)c.eq_bands * T;
-  if (int e = split_lows(h, s, wav, T, c.eq_bands, h->w(g0 + 1), c.eq_taps, low_w)) return e;
-  if (int e = split_lows(h, s, d_wav_encodec, T, c.eq_bands, h->w(g0 + 1), c.eq_taps, low_r)) return e;
+  if (int e = split_lows(s, wav, T, c.eq_bands, h->w(g0 + 1), c.eq_taps, low_w)) return e;
+  if (int e = split_lows(s, d_wav_encodec, T, c.eq_bands, h->w(g0 + 1), c.eq_taps, low_r)) return e;
   k_band_std<<<c.eq_bands, 256, 0, s>>>(low_w, wav, T, c.eq_bands, stdv);
   MVB_CK(cudaGetLastError());
   k_band_std<<<c.eq_bands, 256, 0, s>>>(low_r, d_wav_encodec, T, c.eq_bands, stdv + 64);
@@ -872,4 +896,75 @@ extern "C" int mvb_mbd_conv_test(int32_t kind, const float* d_x, int32_t Cin, in
   if (rc == MVB_OK && e != cudaSuccess) rc = mvb::set_error(MVB_ERR_CUDA, "mvb_mbd_conv_test: %s", cudaGetErrorString(e));
   cudaFree(buf);
   return rc;
+}
+
+// Test hook: one launch of a non-convolution kernel of mvb_mbd_tokens_to_wav with the engine's launch configuration (for
+// GroupNorm statistics and the FIR bank, through the engine's own gn_stats / split_lows).  Operands by op (see the header):
+// a .. e inputs, out the output (in place for the ops that update a tensor), i0 .. i2 sizes, f0 .. f4 scalars.  The fp64
+// GroupNorm partials are allocated per call.  Synchronises `stream`.
+extern "C" int mvb_mbd_op_test(int32_t op, const float* d_a, const float* d_b, const float* d_c, const float* d_d, const float* d_e,
+                               float* d_out, int32_t i0, int32_t i1, int32_t i2, float f0, float f1, float f2, float f3, float f4,
+                               uint64_t seed, void* stream) {
+  if (!d_out) return mvb::set_error(MVB_ERR_ARG, "null argument");
+  cudaStream_t s = (cudaStream_t)stream;
+  auto need = [](bool ok) { return ok ? MVB_OK : mvb::set_error(MVB_ERR_ARG, "mvb_mbd_op_test: bad operands"); };
+  switch (op) {
+    case 0: {   // GroupNorm statistics of a [i0, i1] into out [i2][mean, rstd], eps f0
+      if (int e = need(d_a && i0 >= 1 && i1 >= 1 && i2 >= 1 && i2 <= 64 && i0 % i2 == 0)) return e;
+      double* part = nullptr;
+      MVB_CK(cudaMalloc(&part, sizeof(double) * 2 * GN_SPLIT * i2));
+      int rc = gn_stats(s, part, d_a, i0, i1, i2, f0, d_out);
+      const cudaError_t ce = cudaStreamSynchronize(s);    // (also on an error path: freed only once nothing can use it)
+      cudaFree(part);
+      if (rc == MVB_OK && ce != cudaSuccess) rc = mvb::set_error(MVB_ERR_CUDA, "mvb_mbd_op_test: %s", cudaGetErrorString(ce));
+      return rc;
+    }
+    case 1:     // out [i0, i1] <- relu(GroupNorm(out)) in place, i2 groups, statistics a, gain b, bias c
+      if (int e = need(d_a && d_b && d_c && i0 >= 1 && i1 >= 1 && i2 >= 1 && i0 % i2 == 0)) return e;
+      k_gn_relu_inplace<<<GRID_STRIDE_CTAS * 4, 256, 0, s>>>(d_out, i0, i1, i0 / i2, d_a, d_b, d_c);
+      break;
+    case 2:     // out [i0, i1] <- the i0 low-passed copies of a [i1] through bank b [i0, i2]
+      if (int e = need(d_a && d_b && i0 >= 1 && i0 <= 63 && i1 >= 1 && i2 >= 1)) return e;
+      if (int e = split_lows(s, d_a, i1, i0 + 1, d_b, i2, d_out)) return e;
+      break;
+    case 3:     // out [i0] <- unbiased std of the i0 bands of x = b [i1] given its low-passed copies a [i0 - 1, i1]
+      if (int e = need(d_a && d_b && i0 >= 2 && i0 <= 64 && i1 >= 2)) return e;
+      k_band_std<<<i0, 256, 0, s>>>(d_a, d_b, i1, i0, d_out);
+      break;
+    case 4:     // out [i1] (+)= sum_b band_b * scale_b + shift_b with scale = c / d (d may be null), shift e (may be null);
+                // i2 != 0 accumulates
+      if (int e = need(d_a && d_b && d_c && i0 >= 2 && i0 <= 64 && i1 >= 1)) return e;
+      k_band_mix<<<GRID_STRIDE_CTAS * 2, 256, 0, s>>>(d_a, d_b, i1, i0, d_c, d_d, d_e, d_out, i2);
+      break;
+    case 5:     // out [i0, i1] += nearest-interpolated a [i0, i2]
+      if (int e = need(d_a && i0 >= 1 && i1 >= 1 && i2 >= 1)) return e;
+      k_add_interp<<<GRID_STRIDE_CTAS * 2, 256, 0, s>>>(d_out, i1, d_a, i2, i0);
+      break;
+    case 6:     // out [i0, i1] <- a [i0, i2] cropped to i1 + b [i0, i1]
+      if (int e = need(d_a && d_b && i0 >= 1 && i1 >= 1 && i2 >= i1)) return e;
+      k_add_crop<<<GRID_STRIDE_CTAS * 2, 256, 0, s>>>(d_a, i2, d_b, i1, i0, d_out);
+      break;
+    case 7:     // one schedule step on out [i1]: estimate a, noise b (may be null when sigma <= 0), a f0, b f1, sigma f2,
+                // noise scale f3, clip f4
+      if (int e = need(d_a && i1 >= 1)) return e;
+      k_sched_step<<<GRID_STRIDE_CTAS * 2, 256, 0, s>>>(d_out, d_a, d_b, f0, f1, f2, f3, f4, i1);
+      break;
+    case 8:     // out [i1] <- standard-normal draws of Philox stream i2 under seed
+      if (int e = need(i1 >= 1)) return e;
+      k_randn<<<GRID_STRIDE_CTAS, 256, 0, s>>>(d_out, i1, seed, (unsigned)i2);
+      break;
+    case 9:     // out [i1] <- sum of the i0 blocks out + m i2 (m = 0 .. i0 - 1), in block order
+      if (int e = need(i0 >= 1 && i1 >= 1 && (i0 == 1 || i2 >= i1))) return e;
+      k_sum_blocks<<<GRID_STRIDE_CTAS * 2, 256, 0, s>>>(d_out, (size_t)i2, i0, i1);
+      break;
+    case 10:    // out [i1] <- a * f0
+      if (int e = need(d_a && i1 >= 1)) return e;
+      k_scale_copy<<<GRID_STRIDE_CTAS, 256, 0, s>>>(d_a, f0, d_out, i1);
+      break;
+    default:
+      return mvb::set_error(MVB_ERR_ARG, "mvb_mbd_op_test: op %d", op);
+  }
+  MVB_CK(cudaGetLastError());
+  MVB_CK(cudaStreamSynchronize(s));
+  return MVB_OK;
 }

@@ -30,7 +30,7 @@ def test_library_exports_every_declared_symbol():
     for name in _declared():
         assert hasattr(lib, name), f"{name} declared in include/mvb200.h but not exported"
     assert set(_declared()) == set(_lib.SIGNATURES), "python binding table out of sync with the header"
-    for hook in ("mvb_gemm_test", "mvb_mbd_conv_test", "mvb_s2_attn_test", "mvb_s2_sample_test", "mvb_voc_op_test",
+    for hook in ("mvb_gemm_test", "mvb_mbd_conv_test", "mvb_mbd_op_test", "mvb_s2_attn_test", "mvb_s2_sample_test", "mvb_voc_op_test",
                  "mvb_audio_post_test"):
         assert hook in _lib.SIGNATURES and hasattr(lib, hook), f"test hook {hook} missing"
     assert lib.mvb_abi_version() == _lib.ABI_VERSION == 2
@@ -46,6 +46,54 @@ def test_config_validation_without_gpu():
     bad = _lib.S1Config(24, 16, 64, 1024, 5632, 2562, 2048, 256, 1e-5, 1, 0, 2048)
     assert lib.mvb_s1_kv_bytes(ctypes.byref(bad)) == 0
     assert b"head_dim" in lib.mvb_last_error()
+
+
+_MBD_VALIDATE = r"""
+import ctypes as C, sys
+sys.path[:0] = [{root!r}, {pkg!r}]
+from mvb200 import _lib
+from mvb200.mbd import MBDSettings, _lowpass_bank, _schedule_table
+lib = _lib.load()
+s, u = MBDSettings(), MBDSettings().unet
+cfg = _lib.MbdConfig(s.n_models, u.chin, u.hidden, u.depth, u.res_blocks, u.norm_groups, u.kernel, u.stride, float(u.growth),
+                     int(u.emb_all_layers), u.codec_dim, u.num_steps, _schedule_table(s.schedule, s.steps()).shape[0],
+                     float(s.schedule.noise_scale), float(s.schedule.clip), s.proc_bands,
+                     _lowpass_bank(s.proc_bands, s.sample_rate).shape[1], s.eq_bands,
+                     _lowpass_bank(s.eq_bands, s.sample_rate).shape[1], 12 * s.sample_rate)
+for field, value in {overrides!r}:
+    setattr(cfg, field, value)
+print(lib.mvb_mbd_workspace_bytes(C.byref(cfg)), lib.mvb_last_error().decode())
+"""
+
+
+@pytest.mark.parametrize("overrides,want_error", [
+    ([("norm_groups", 0)], "norm_groups"),
+    ([("norm_groups", -1)], "norm_groups"),
+    ([("norm_groups", 33), ("hidden", 33 * 4)], "norm_groups"),
+    ([("proc_taps", 0)], "filter length"),
+    ([("eq_taps", 19030)], "filter length"),
+    ([("norm_groups", 32), ("hidden", 32 * 3), ("eq_taps", 19029)], None),
+    ([("proc_bands", 64), ("proc_taps", 5921), ("eq_bands", 64), ("eq_taps", 5921)], None),
+], ids=["groups0", "groups-1", "groups33", "taps0", "taps19030", "groups32-taps19029", "bands64"])
+def test_mbd_config_validation(overrides, want_error):
+    """mvb_mbd_workspace_bytes rejects GroupNorm group counts outside 1 .. 32 (the workspace's statistics slots and
+    partials hold 32 groups; 0 used to divide by zero) and filters longer than k_fir_bank's shared memory can hold
+    (227 KB: 19029 taps), and accepts the limits and a 64-band bank.  Each configuration runs in a child process, so that
+    a crash of the validation cannot take the test session down with it."""
+    import subprocess
+    import sys
+    from mvb200 import _lib
+    if not os.path.isfile(_lib.LIB_PATH):
+        import __graft_entry__ as g
+        g.build()
+    code = _MBD_VALIDATE.format(root=ROOT, pkg=os.path.join(ROOT, "metavoice-src_b200"), overrides=overrides)
+    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=300)
+    assert r.returncode == 0, f"child exited with {r.returncode}: {r.stderr[-2000:]}"
+    nbytes, _, err = r.stdout.strip().partition(" ")
+    if want_error is None:
+        assert int(nbytes) > 0, err
+    else:
+        assert int(nbytes) == 0 and want_error in err, r.stdout
 
 
 def test_missing_library_fails_loudly(monkeypatch):

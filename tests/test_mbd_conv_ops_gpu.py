@@ -196,6 +196,67 @@ def test_channel_padding_and_partial_warps(cin, groups, cout):
     _case(f"transposed {cin}->{cout} (k4 s2)", 2, cin, cout, 4, 2, 1, 1, 150, groups=groups, seed=cin + cout + 2)
 
 
+# ---- CUDA-core kernels the engine runs for narrow inputs (and everywhere under MVB_MBD_NO_TC) -------------------------
+@pytest.mark.parametrize("tin", [1, 7, 145, 3833, 144000])
+def test_level0_encoder_conv_cuda_cores(tin):
+    """The first encoder convolution of every UNet call, Cin = 1 -> 48, k8 s4 (k_mbd_conv<8, 4, 1>, always on the CUDA
+    cores): lengths that are and are not multiples of the stride, up to 6 s."""
+    _case(f"strided 1->48 Tin={tin}", 1, 1, 48, 8, 4, 1, 2, tin, gn=False, use_tc=False, seed=tin)
+
+
+@pytest.mark.parametrize("tf", [1, 12, 375])
+def test_codec_conv_cuda_cores(tf):
+    """conv_codec: K = 1, 128 -> 3072 with bias (k_mbd_conv<1, 1, 4>)."""
+    _case(f"codec 128->3072 Tf={tf}", 0, 128, 3072, 1, 1, 1, 0, tf, gn=False, bias=True, use_tc=False, seed=tf)
+
+
+@pytest.mark.parametrize("cin,cout", [(1, 16), (16, 32), (64, 128), (48, 192)])
+@pytest.mark.parametrize("tin", [1, 129, 3833])
+def test_k4_s2_cuda_cores(cin, cout, tin):
+    """The (k4, s2) UNet on the CUDA cores: k_mbd_conv<4, 2, 2> and k_mbd_convtr<2>, including widths below 32 channels."""
+    _case(f"strided {cin}->{cout} (k4 s2) Tin={tin}", 1, cin, cout, 4, 2, 1, 1, tin, gn=False, use_tc=False, seed=cin + tin)
+    if cin > 1:
+        _case(f"transposed {cout}->{cin} (k4 s2) Tin={tin}", 2, cout, cin, 4, 2, 1, 1, tin, use_tc=False, seed=cout + tin)
+
+
+# ---- GroupNorm statistics from the engine's kernels feeding the convolution ---------------------------------------
+def _gn_stats_hook(x, groups):
+    from mvb200 import _lib as L
+    lib = L.load()
+    out = torch.full((2 * GUARD + 2 * groups,), float("nan"), device="cuda")
+    st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    L.check(lib.mvb_mbd_op_test(0, x.data_ptr(), None, None, None, None, out[GUARD:].data_ptr(), x.shape[0], x.shape[1], groups,
+                                1e-5, 0.0, 0.0, 0.0, 0.0, 0, st))
+    assert torch.isnan(out[:GUARD]).all() and torch.isnan(out[GUARD + 2 * groups:]).all()
+    return out[GUARD:GUARD + 2 * groups].view(groups, 2).contiguous()
+
+
+@pytest.mark.parametrize("lvl", [0, 1, 2, 3])
+@pytest.mark.parametrize("use_tc", [True, False])
+def test_gn_stats_feed_the_resblock_conv(lvl, use_tc):
+    """GroupNorm statistics from k_gn_partial + k_gn_final (mvb_mbd_op_test) feed one ResBlock convolution per level.
+    The reference is the one above with the correctly rounded float64 statistics; the kernel's statistics are within
+    2 u24 of the exact ones (tests/test_mbd_ops_gpu.py), so within 3 u24 (u24 = 2^-24) of the rounded ones: per element
+    the prologue input moves by at most |gain| (|x - mean| d_rstd + (rstd + d_rstd) d_mean), propagated through |W|."""
+    c, t = WIDTHS[lvl], LENGTHS[lvl]
+    d = _make(0, c, c, 3, 1, t, 40 + lvl, True, True, True, True)
+    ref, bound, ynorm = _reference(0, d, 3, 1, 1, 1, use_tc, c)
+    stats, gw, gb = d["gn"]
+    hook = _gn_stats_hook(d["x"], d["groups"])
+    got = _run(0, dict(d, gn=(hook, gw, gb)), c, c, 3, 1, 1, 1, use_tc).double()
+    cpg = c // d["groups"]
+    m = stats[:, 0].double().repeat_interleave(cpg)[:, None]
+    r = stats[:, 1].double().repeat_interleave(cpg)[:, None]
+    em, er = 1.5 * U * m.abs(), 1.5 * U * r
+    df = gw.double().abs()[:, None] * ((d["x"].double() - m).abs() * er + (r + er) * em) * (1 + 4 * U)
+    wd = (d["w"].to(torch.bfloat16) if use_tc else d["w"]).double().abs()
+    bound = bound + _conv(0, df, wd, 1, 1, 1)
+    err = (got - ref).abs()
+    ratio, nw = float((err / bound).max()), float(err.norm() / ynorm)
+    print(f"gn stats -> resblock k3 C={c} T={t} {'tc' if use_tc else 'cuda-core'}: max |err|/bound {ratio:.2e}, normwise {nw:.2e}")
+    assert int((err > bound).sum()) == 0 and nw < NORMWISE
+
+
 def test_fp32_taps_violate_the_bound():
     """Sensitivity: the tensor-core result (bf16 taps) must fail a reference built with the unrounded fp32 taps."""
     kind, cin, cout, K, T = 0, 64, 128, 3, 512
