@@ -176,7 +176,9 @@ uint64_t mvb_s1_launch_count(const mvb_s1* h);
  *   mvb_s1_fetch_sampled : the sampler's own draws for `utt` (they differ from the fed-back tokens of mvb_s1_fetch only
  *                          under teacher forcing), host int32 [cap];
  *   mvb_s1_trace_fetch   : per-CTA clock64 phase stamps of the last persistent-kernel step (MVB_PC_TRACE=1), host
- *                          int64 [max_ctas, 512]; returns the number of CTAs copied. */
+ *                          int64 [max_ctas, 512]; the last 6 entries of a CTA's row are its producer warp's stall cycles
+ *                          of the whole launch per phase (qkv, KV tiles, wo, w1|w3, w2, head); returns the number of CTAs
+ *                          copied. */
 int mvb_s1_fetch_sampled(mvb_s1* h, int32_t utt, int32_t* out_tokens, int32_t cap, void* stream);
 int mvb_s1_trace_fetch(mvb_s1* h, long long* out, int32_t max_ctas, void* stream);
 

@@ -5,9 +5,9 @@
 //   * grid = one CTA per SM; every CTA owns a static slice of every weight matrix:
 //       (K split s = cta % S, row tiles t = cta / S, + groups, ...)  chosen per matrix on the host.
 //   * warp 0 = PRODUCER: walks the whole burst's byte schedule -- weight tiles via TMA (cp.async.bulk.tensor, 128B
-//     swizzle) into a ring of smem stages, KV-cache tiles via cp.async.bulk into two dedicated (K,V) tile slots -- all
-//     guarded by full/empty mbarriers.  Weights do not depend on activations, so the producer never waits for a grid
-//     barrier: the HBM stream keeps running across phase, layer AND token boundaries (the next token's first weight
+//     swizzle) and KV-cache tiles (TMA for the bf16 cache, cp.async.bulk for fp32; K and V one stage each) into ONE
+//     ring of smem stages guarded by full/empty mbarriers.  Weights do not depend on activations, so the producer never
+//     waits for a grid barrier: the HBM stream keeps running across phase, layer AND token boundaries (the next token's first weight
 //     tiles land while the grid is still sampling).  It issues no L2 prefetch beyond the ring: on an H100 SXM at 700 W
 //     prefetching 1 to 32 tiles ahead (cp.async.bulk.prefetch.tensor while the ring is full) made batch-1 decode
 //     13-68 % slower.
@@ -36,12 +36,15 @@
 namespace mvb {
 
 constexpr int PC_THREADS = 192;      // producer warp + MMA warp + 4 compute warps
-constexpr int PC_KV_TILE_BYTES = 16384;   // K (or V) tile of one (row, head): 64 bf16 / 32 fp32 positions
+constexpr int PC_KV_TILE_BYTES = 16384;   // K (or V) tile of one (row, head): 64 bf16 / 32 fp32 positions; one ring stage
 constexpr int PC_RPAD = 16;          // rows of the fp32 activation buffers (8 utterances x 2 CFG rows)
 constexpr int PC_BKB_MAX = 12;       // k-blocks of the activation operand one CTA may own in a phase
-constexpr int PC_NKV_MAX = 4;        // (K tile, V tile) slots: PcCfg::NKV of them are used
+constexpr int PC_MAX_STAGES = 12;    // ring stages PcShared has mbarriers for
 constexpr int PC_MAX_CHUNKS = 64;    // per (row, head): ceil(2048 / 32) in fp32 mode
 constexpr int PC_TRACE_EVENTS = 512;
+// producer stall record (MVB_PC_TRACE): clock64 cycles the producer spent waiting for a free ring stage, summed over the
+// launch per phase of the byte schedule; kept in the last entries of the CTA's trace row (a step stamps ~350 events)
+enum PcStall { PCS_QKV, PCS_KV, PCS_WO, PCS_W13, PCS_W2, PCS_HEAD, PC_STALL_PHASES };
 constexpr int PC_MAX_TILES = 128;    // attention KV tiles one CTA may own per layer
 constexpr int PC_SAMP_OWN = 32;      // vocabulary entries one CTA may own in the fused sampler (ceil(V / grid))
 
@@ -53,8 +56,9 @@ struct AttTile {
 };
 
 struct PcShared {   // small shared state behind the big buffers
-  uint64_t b_full[8], b_empty[8], b_ready, acc_full[2], acc_empty[2], kv_full[PC_NKV_MAX], kv_empty[PC_NKV_MAX], tab_ready;
+  uint64_t b_full[PC_MAX_STAGES], b_empty[PC_MAX_STAGES], b_ready, acc_full[2], acc_empty[2], tab_ready;
   int n_att_tiles;
+  int n_kv_tiles;                    // tiles of the table that are loaded (npos > 0): two ring stages each per layer
   // every CTA's private copy of the decode state of the batch (kept in lock-step: the same deterministic update
   // from the same arg-max in every CTA; only the owner CTA writes it back to global memory)
   int st_pos[PC_RPAD / 2], st_ngen[PC_RPAD / 2], st_done[PC_RPAD / 2], st_tok[PC_RPAD];
@@ -69,6 +73,7 @@ struct PcShared {   // small shared state behind the big buffers
   float ss[PC_RPAD];                 // sum of squares of this CTA's K slice, per row
   float red[8];                      // block reductions (sampler)
   unsigned long long best[4];
+  long long stall[PC_STALL_PHASES];  // producer stall cycles per phase (trace only)
   float own_ke[PC_RPAD / 2][PC_SAMP_OWN];   // sampler: kept exp-values of this CTA's vocabulary entries, per utterance
   int row_nz[PC_RPAD];
   AttTile att_tab[PC_MAX_TILES];
@@ -77,16 +82,19 @@ struct PcShared {   // small shared state behind the big buffers
 template <int NB> struct PcCfg {
   static constexpr int TILE_ROWS = 128;
   static constexpr int STAGE_BYTES = TILE_ROWS * 128;     // [TILE_ROWS x 64 k] bf16
-  // ring depth: what fits in 227 KB next to the activation operand, the KV slots and the accumulator slots
-  static constexpr int STAGES = (NB == 16) ? 7 : 5;
-  static constexpr int NKV = 2;
   static constexpr int B_BYTES = PC_BKB_MAX * NB * 128;
   static constexpr int RH = NB / 2;                       // activation rows carried (hi rows; lo rows follow)
   static constexpr int ACC_LD = TILE_ROWS + 4;            // accumulator slot [RH][ACC_LD] fp32 (pad: conflict-free stores)
-  static constexpr int ACC_BYTES = (2 * RH * ACC_LD * 4 + 1023) / 1024 * 1024;   // two slots (keeps kvbuf 1 KB aligned)
-  static constexpr size_t SMEM = 1024 + (size_t)STAGES * STAGE_BYTES + B_BYTES + ACC_BYTES +
-                                 (size_t)NKV * 2 * PC_KV_TILE_BYTES + sizeof(PcShared) + 64;
+  static constexpr int ACC_BYTES = 2 * RH * ACC_LD * 4;   // two slots
+  // ring depth: every whole stage that fits in 227 KB next to the activation operand, the accumulator slots and PcShared
+  // (the 1024 B align the ring for the 128B swizzle)
+  static constexpr int STAGES = (int)((227 * 1024 - 1024 - B_BYTES - ACC_BYTES - sizeof(PcShared) - 64) / STAGE_BYTES);
+  static constexpr size_t SMEM = 1024 + (size_t)STAGES * STAGE_BYTES + B_BYTES + ACC_BYTES + sizeof(PcShared) + 64;
   static_assert(SMEM <= 227 * 1024, "persistent decode kernel exceeds the 227 KB shared-memory opt-in");
+  static_assert(STAGES <= PC_MAX_STAGES, "PcShared has too few ring mbarriers");
+  static_assert(PC_KV_TILE_BYTES == STAGE_BYTES, "a K or V tile travels as one ring stage");
+  // the fused sampler's scratch (s_key, s_e) lives in the activation operand and the accumulator slots between tokens
+  static_assert(2 * SAMP_PAD * sizeof(float) <= (size_t)B_BYTES + ACC_BYTES, "sampler scratch does not fit");
 };
 
 struct PcMat {     // one weight matrix kind, static decomposition
@@ -122,7 +130,8 @@ struct PcParams {
   size_t kv_half;  // bytes of one layer's K (or V) region
   unsigned* bar;   // grid-wide arrival counter (zero at launch)
   long long kv_rows_half;   // bf16 cache: rows (positions) of one layer's K (or V) region in tm_kv = kv_half / 256
-  long long* trace;  // optional [gridDim][PC_TRACE_EVENTS] clock64 stamps of compute-thread 0 (debug)
+  long long* trace;  // optional (debug): [gridDim][PC_TRACE_EVENTS] clock64 stamps of compute-thread 0 of the last step;
+                     // the last PC_STALL_PHASES entries of a row: the producer's stall cycles of the whole launch
   S1State st;
 };
 
@@ -277,8 +286,7 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
   uint8_t* ring = smem_raw + smem_pad_1024(smem_raw);
   uint8_t* Bop = ring + STAGES * STAGE_BYTES;
   float* accbuf = reinterpret_cast<float*>(Bop + Cfg::B_BYTES);   // [2][RH][ACC_LD]: MMA warp -> epilogue
-  uint8_t* kvbuf = Bop + Cfg::B_BYTES + Cfg::ACC_BYTES;     // [NKV][K tile | V tile]; sampler scratch between tokens
-  PcShared& sh = *reinterpret_cast<PcShared*>(kvbuf + Cfg::NKV * 2 * PC_KV_TILE_BYTES);
+  PcShared& sh = *reinterpret_cast<PcShared*>(Bop + Cfg::B_BYTES + Cfg::ACC_BYTES);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int cta = blockIdx.x, G = gridDim.x;
@@ -295,16 +303,13 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
       ptx::mbar_init(ptx::smem_u32(sh.acc_full + i), 32);     // every lane of the MMA warp after its slot stores
       ptx::mbar_init(ptx::smem_u32(sh.acc_empty + i), 128);   // every compute thread after its slot loads
     }
-    for (int i = 0; i < Cfg::NKV; ++i) {
-      ptx::mbar_init(ptx::smem_u32(sh.kv_full + i), 1);
-      ptx::mbar_init(ptx::smem_u32(sh.kv_empty + i), 1);
-    }
     ptx::mbar_init(ptx::smem_u32(&sh.tab_ready), 1);
     ptx::fence_barrier_init();
   }
   // zero the activation operand once: rows >= R (hi and lo halves) must read as zero forever
   for (int i = tid; i < Cfg::B_BYTES / 16; i += PC_THREADS) reinterpret_cast<uint4*>(Bop)[i] = make_uint4(0, 0, 0, 0);
   if (tid < PC_RPAD) sh.ss[tid] = 0.f;
+  if (tid < PC_STALL_PHASES) sh.stall[tid] = 0;
   ptx::fence_async_smem();
   __syncthreads();
   pdl_launch_dependents();
@@ -321,17 +326,32 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
     // The whole warp walks the schedule (warp-uniform control flow and operands); one elected lane issues the TMA /
     // bulk-copy instructions.  Issuing them from a `lane == 0` branch makes the compiler wrap each UTMALDG in an
     // ELECT + 4 x R2UR.BROADCAST + vote loop, which capped one producer at a tile per ~0.25 us.
+    // The ring is ONE FIFO with two consumers: the MMA warp takes the weight stages, the compute warps' attention the KV
+    // stages.  So the issue order must equal the consumption order: layer l's qkv stages, then its KV tiles, then wo,
+    // w1|w3, w2, then layer l+1.  Issuing a layer's KV tiles ahead of its qkv stages would deadlock: the attention
+    // releases a KV stage only after the qkv multiply, and that multiply would need the ring to wrap past the held stage.
     const uint64_t pol = ptx::policy_evict_first();
-    uint32_t slot = 0, kv_ctr = 0;
-    auto gemm_tiles = [&](const CUtensorMap* tmA, const CUtensorMap* tmB2, int split_t, const PcSlice& sl, int layer) {
+    uint32_t slot = 0;
+    auto acquire = [&](int phase) -> uint32_t {   // the next ring stage, once its consumer has released it
+      const auto [s, ph] = ring_pos(slot, STAGES);
+      ++slot;
+      const uint32_t bar = ptx::smem_u32(sh.b_empty + s);
+      if (p.trace == nullptr) {
+        ptx::mbar_wait(bar, ph ^ 1u);
+      } else {
+        const long long t0 = clock64();
+        ptx::mbar_wait(bar, ph ^ 1u);
+        if (lane == 0) sh.stall[phase] += clock64() - t0;
+      }
+      return s;
+    };
+    auto gemm_tiles = [&](const CUtensorMap* tmA, const CUtensorMap* tmB2, int split_t, const PcSlice& sl, int layer, int phase) {
       for (int i = 0; i < sl.nt; ++i) {
         const int t = sl.t0 + i * sl.G;
         const CUtensorMap* tm = (t < split_t) ? tmA : tmB2;
         const int tt = (t < split_t) ? t : t - split_t;
         for (int kb = sl.kb0; kb < sl.kb1; ++kb) {
-          const auto [s, ph] = ring_pos(slot, STAGES);
-          ++slot;
-          ptx::mbar_wait(ptx::smem_u32(sh.b_empty + s), ph ^ 1u);
+          const uint32_t s = acquire(phase);
           if (ptx::elect_one()) {
             const uint32_t full = ptx::smem_u32(sh.b_full + s);
             ptx::mbar_arrive_expect_tx(full, STAGE_BYTES);
@@ -341,64 +361,50 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
         }
       }
     };
-    // KV tiles [from, to) (in this CTA's table order) of layer l; positions < pos come from earlier steps
-    auto kv_units = [&](int l, int from, int to) {
+    // this CTA's KV tiles of layer l (table order), K then V as two consecutive stages -- they may straddle the ring's
+    // wrap; positions < pos come from earlier steps
+    auto kv_tiles = [&](int l) {
       const char* kbase = p.kv + (size_t)l * 2 * p.kv_half;
-      const char* vbase = kbase + p.kv_half;
       const int n_tiles = sh.n_att_tiles;
-      int idx = 0;
       for (int i = 0; i < n_tiles; ++i) {
         const AttTile e = sh.att_tab[i];
         const int npos = (int)(e.meta & 0xffu);
         if (npos == 0) continue;                 // only the current position: it comes from registers
-        const int my = idx++;
-        if (my < from) continue;
-        if (my >= to) break;
-        const auto [ks, ph] = ring_pos(kv_ctr, Cfg::NKV);
-        ++kv_ctr;
-        ptx::mbar_wait(ptx::smem_u32(sh.kv_empty + ks), ph ^ 1u);
-        if (ptx::elect_one()) {
-          const uint32_t full = ptx::smem_u32(sh.kv_full + ks);
-          uint8_t* dst = kvbuf + (size_t)ks * 2 * PC_KV_TILE_BYTES;
-          if constexpr (!KV_FP32) {
-            // 64 positions x 128 dims as two 128B-swizzled [64 x 64] boxes per operand (conflict-free ldmatrix); rows past
-            // npos are older / zero cache contents and are masked by the consumer
-            const int row = (int)((long long)l * 2 * p.kv_rows_half + (long long)(e.off >> 8));
-            const int rowv = row + (int)p.kv_rows_half;
-            ptx::mbar_arrive_expect_tx(full, 2u * PC_KV_TILE_BYTES);
-            ptx::tma_load_2d(ptx::smem_u32(dst), &tm_kv, full, 0, row);
-            ptx::tma_load_2d(ptx::smem_u32(dst + 8192), &tm_kv, full, 64, row);
-            ptx::tma_load_2d(ptx::smem_u32(dst + PC_KV_TILE_BYTES), &tm_kv, full, 0, rowv);
-            ptx::tma_load_2d(ptx::smem_u32(dst + PC_KV_TILE_BYTES + 8192), &tm_kv, full, 64, rowv);
-          } else {
-            const uint32_t bytes = (uint32_t)npos * 128 * esz;
-            ptx::mbar_arrive_expect_tx(full, 2 * bytes);
-            ptx::bulk_load(ptx::smem_u32(dst), kbase + e.off, bytes, full);
-            ptx::bulk_load(ptx::smem_u32(dst + PC_KV_TILE_BYTES), vbase + e.off, bytes, full);
+        for (int v = 0; v < 2; ++v) {            // K, V
+          const uint32_t s = acquire(PCS_KV);
+          if (ptx::elect_one()) {
+            const uint32_t full = ptx::smem_u32(sh.b_full + s);
+            const uint32_t dst = ptx::smem_u32(ring + (size_t)s * STAGE_BYTES);
+            if constexpr (!KV_FP32) {
+              // 64 positions x 128 dims as two 128B-swizzled [64 x 64] boxes (conflict-free ldmatrix); rows past npos are
+              // older / zero cache contents and are masked by the consumer
+              const int row = (int)((long long)(2 * l + v) * p.kv_rows_half + (long long)(e.off >> 8));
+              ptx::mbar_arrive_expect_tx(full, PC_KV_TILE_BYTES);
+              ptx::tma_load_2d(dst, &tm_kv, full, 0, row);
+              ptx::tma_load_2d(dst + 8192, &tm_kv, full, 64, row);
+            } else {
+              const uint32_t bytes = (uint32_t)npos * 128 * esz;
+              ptx::mbar_arrive_expect_tx(full, bytes);
+              ptx::bulk_load(dst, kbase + (size_t)v * p.kv_half + e.off, bytes, full);
+            }
           }
+          __syncwarp();
         }
-        __syncwarp();
       }
     };
     for (int step = 0; step < p.n_steps; ++step) {
       for (int l = 0; l < p.n_layer; ++l) {
-        if (l == 0) {
-          gemm_tiles(&tm_qkv, &tm_qkv, 1 << 30, s_qkv, 0);   // weights first: they need nothing from the previous token
-          ptx::mbar_wait(ptx::smem_u32(&sh.tab_ready), step & 1u);   // this token's tile table is built
-          kv_units(0, 0, 1 << 30);
-        } else {
-          kv_units(l, Cfg::NKV, 1 << 30);                       // (units beyond the prefetched ones)
-        }
-        gemm_tiles(&tm_o, &tm_o, 1 << 30, s_o, l);
-        gemm_tiles(&tm_w1, &tm_w3, T1, s_w13, l);
-        gemm_tiles(&tm_w2, &tm_w2, 1 << 30, s_w2, l);
-        if (l + 1 < p.n_layer) {
-          kv_units(l + 1, 0, Cfg::NKV);                         // next layer's first KV tiles ride ahead of its QKV GEMM
-          gemm_tiles(&tm_qkv, &tm_qkv, 1 << 30, s_qkv, l + 1);
-        }
+        gemm_tiles(&tm_qkv, &tm_qkv, 1 << 30, s_qkv, l, PCS_QKV);
+        if (l == 0) ptx::mbar_wait(ptx::smem_u32(&sh.tab_ready), step & 1u);   // this token's tile table is built
+        kv_tiles(l);
+        gemm_tiles(&tm_o, &tm_o, 1 << 30, s_o, l, PCS_WO);
+        gemm_tiles(&tm_w1, &tm_w3, T1, s_w13, l, PCS_W13);
+        gemm_tiles(&tm_w2, &tm_w2, 1 << 30, s_w2, l, PCS_W2);
       }
-      gemm_tiles(&tm_head, &tm_head, 1 << 30, s_head, 0);
+      gemm_tiles(&tm_head, &tm_head, 1 << 30, s_head, 0, PCS_HEAD);
     }
+    if (p.trace != nullptr && lane == 0)
+      for (int i = 0; i < PC_STALL_PHASES; ++i) p.trace[(size_t)(cta + 1) * PC_TRACE_EVENTS - PC_STALL_PHASES + i] = sh.stall[i];
   } else if (warp == 1) {
     // =================================== MMA WARP ===================================================
     // The whole warp walks the schedule (waits and counters stay warp-uniform) and multiplies every weight stage of a
@@ -443,9 +449,18 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
         ++tile_ctr;
       }
     };
+    uint32_t kv_stages = 0;
     for (int step = 0; step < p.n_steps; ++step) {
       for (int l = 0; l < p.n_layer; ++l) {
         gemm_phase(s_qkv);
+        if (l == 0) {
+          ptx::mbar_wait(ptx::smem_u32(&sh.tab_ready), step & 1u);   // this token's tile table is built
+          kv_stages = 2u * (uint32_t)sh.n_kv_tiles;
+        }
+        // the layer's K, V stages belong to the attention.  Skipping them without a wait is safe: the next stage this
+        // warp waits for comes after a b_ready that the compute warps publish only once the attention has drained them,
+        // so no b_full barrier is ever waited on a full ring lap ahead of its producer.
+        slot += kv_stages;
         gemm_phase(s_o);
         gemm_phase(s_w13);
         gemm_phase(s_w2);
@@ -456,12 +471,17 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
     // =================================== COMPUTE WARPS ==============================================
     const int ct = tid - 64;            // 0..127
     const int cw = ct >> 5;             // 0..3
-    uint32_t tile_ctr = 0, bar_idx = 0, kv_ctr = 0;
+    uint32_t tile_ctr = 0, bar_idx = 0;
+    uint32_t slot = 0;                  // ring position: advanced past the weight stages, consumed at the KV stages
+    auto n_stages = [](const PcSlice& sl) { return (uint32_t)(sl.nt * (sl.kb1 - sl.kb0)); };
+    const uint32_t st_qkv = n_stages(s_qkv), st_head = n_stages(s_head);
+    const uint32_t st_post = n_stages(s_o) + n_stages(s_w13) + n_stages(s_w2);   // wo, w1|w3, w2: after the attention
+    const uint32_t ring_u32 = ptx::smem_u32(ring);
     const float inv_D = 1.f / (float)p.D;
     pdl_wait();                         // state / x inputs of the previous kernels are visible
     int ev = 0;
     auto stamp = [&]() {
-      if (p.trace != nullptr && ct == 0 && ev < PC_TRACE_EVENTS) p.trace[(size_t)cta * PC_TRACE_EVENTS + ev] = clock64();
+      if (p.trace != nullptr && ct == 0 && ev < PC_TRACE_EVENTS - PC_STALL_PHASES) p.trace[(size_t)cta * PC_TRACE_EVENTS + ev] = clock64();
       ++ev;
     };
 
@@ -659,7 +679,11 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
       // waits for them: the first QKV operand is staged straight from the embedding tables by every CTA.
       if (step > 0 && p.fused) finish_sample(step - 1);
       if (ct == 0) {
-        sh.n_att_tiles = build_att_table(p, sh.st_pos, sh.c_slot, cta, G, ppc, esz, sh.att_tab, sh.row_nz);
+        const int n_tiles = build_att_table(p, sh.st_pos, sh.c_slot, cta, G, ppc, esz, sh.att_tab, sh.row_nz);
+        int n_kv = 0;
+        for (int i = 0; i < n_tiles; ++i) n_kv += (sh.att_tab[i].meta & 0xffu) != 0u;
+        sh.n_att_tiles = n_tiles;
+        sh.n_kv_tiles = n_kv;
         ptx::mbar_arrive(ptx::smem_u32(&sh.tab_ready));   // release: the producer may walk the table
       }
       if (owner) {
@@ -707,6 +731,7 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
 
         // ---- attention over [0, pos] + KV-cache append (fast_model.py:104-113, 220-224)
         zero_slice(p.gu, (size_t)PC_RPAD * 2 * p.F);   // free since the previous layer's w2 phase; ordered by the next arrive
+        slot += st_qkv;
         grid_wait();
         stamp();
         if constexpr (!KV_FP32) {
@@ -765,12 +790,12 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
               sh.cur[ct] = kcur;
               sh.cur[128 + ct] = vcur;
             }
+            const RingPos kp = ring_pos(slot, STAGES), vp = ring_pos(slot + 1, STAGES);   // K, V stages of the tile
             if (npos > 0) {
-              const auto [ks, ph] = ring_pos(kv_ctr, Cfg::NKV);
-              ++kv_ctr;
-              ptx::mbar_wait(ptx::smem_u32(sh.kv_full + ks), ph);
-              const uint32_t kt = ptx::smem_u32(kvbuf + (size_t)ks * 2 * PC_KV_TILE_BYTES);
-              const uint32_t vt = kt + PC_KV_TILE_BYTES;
+              slot += 2;
+              ptx::mbar_wait(ptx::smem_u32(sh.b_full + kp.stage), kp.phase);
+              const uint32_t kt = ring_u32 + kp.stage * STAGE_BYTES;
+              const uint32_t vt = ring_u32 + vp.stage * STAGE_BYTES;
               if (16 * cw < npos) {
                 // ---- scores of positions [16w, 16w+16): A = K rows, B = q (hi, lo) in column 0
                 // four independent accumulator chains (hi / lo terms x even / odd k-steps): the mma latency, not its issue
@@ -797,7 +822,8 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
               } else if (lane < 16) {
                 scv[16 * cw + lane] = -INFINITY;
               }
-              compute_sync();                                    // all 64 scores visible
+              compute_sync();                                    // all 64 scores visible: every read of K is done
+              if (ct == 0) ptx::mbar_arrive(ptx::smem_u32(sh.b_empty + kp.stage));
               // ---- online softmax over the tile (identical in every warp)
               // tile max with ONE redux.sync on an order-preserving integer image of the floats (a 5-step shuffle butterfly
               // is ~150 cycles of dependent latency); the running sum stays per lane and is reduced once per unit
@@ -822,6 +848,7 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
 #pragma unroll
               for (int i = 0; i < 4; ++i) { olo[0][i] = 0.f; olo[1][i] = 0.f; }
               const int n_k4 = (npos + 15) >> 4;
+              ptx::mbar_wait(ptx::smem_u32(sh.b_full + vp.stage), vp.phase);
 #pragma unroll
               for (int k4 = 0; k4 < 4; ++k4) {
                 if (k4 < n_k4) {
@@ -842,8 +869,8 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
 #pragma unroll
               for (int i = 0; i < 4; ++i) { oacc[0][i] += olo[0][i]; oacc[1][i] += olo[1][i]; }
             }
-            if (npos > 0 || has_cur) compute_sync();   // KV tile fully consumed; sh.cur visible
-            if (npos > 0 && ct == 0) ptx::mbar_arrive(ptx::smem_u32(sh.kv_empty + ring_pos(kv_ctr - 1, Cfg::NKV).stage));
+            if (npos > 0 || has_cur) compute_sync();   // V stage fully consumed; sh.cur visible
+            if (npos > 0 && ct == 0) ptx::mbar_arrive(ptx::smem_u32(sh.b_empty + vp.stage));
             if (has_cur) {
               // the current token (its k, v never left the chip): every warp applies the same update to its dims
               float sd = 0.f;
@@ -922,12 +949,13 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
               sh.cur[ct] = kcur;
               sh.cur[128 + ct] = vcur;
             }
+            const RingPos kp = ring_pos(slot, STAGES), vp = ring_pos(slot + 1, STAGES);   // K, V stages of the tile
             if (npos > 0) {
-              const auto [ks, ph] = ring_pos(kv_ctr, Cfg::NKV);
-              ++kv_ctr;
-              ptx::mbar_wait(ptx::smem_u32(sh.kv_full + ks), ph);
-              const uint8_t* kt = kvbuf + (size_t)ks * 2 * PC_KV_TILE_BYTES;
-              const uint8_t* vt = kt + PC_KV_TILE_BYTES;
+              slot += 2;
+              ptx::mbar_wait(ptx::smem_u32(sh.b_full + kp.stage), kp.phase);
+              ptx::mbar_wait(ptx::smem_u32(sh.b_full + vp.stage), vp.phase);
+              const uint8_t* kt = ring + (size_t)kp.stage * STAGE_BYTES;
+              const uint8_t* vt = ring + (size_t)vp.stage * STAGE_BYTES;
               // each half-warp owns positions hw, hw+8, ... (hw = 2 * warp + half); two positions per trip for ILP (four per
               // trip was measured: the extra 32 live registers spill in this 255-register kernel and the phase gets 15-30 %
               // slower).  The trip count is WARP-uniform and out-of-range positions are clamped to position 0 with score -inf
@@ -968,7 +996,10 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
               }
             }
             if (npos > 0 || has_cur) compute_sync();   // KV tile fully consumed; sh.cur visible
-            if (npos > 0 && ct == 0) ptx::mbar_arrive(ptx::smem_u32(sh.kv_empty + ring_pos(kv_ctr - 1, Cfg::NKV).stage));
+            if (npos > 0 && ct == 0) {
+              ptx::mbar_arrive(ptx::smem_u32(sh.b_empty + kp.stage));
+              ptx::mbar_arrive(ptx::smem_u32(sh.b_empty + vp.stage));
+            }
             if (has_cur && hw == 0) {
               float sdot = 0.f;
 #pragma unroll
@@ -1126,7 +1157,9 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
         epilogue(s_w2, p.x, p.D, p.D, 1 << 30, nullptr);
         stamp();
         grid_arrive();
+        slot += st_post;
       }
+      slot += st_head;
       // ---- head: logits += (x * out_norm) . W_out^T   (rows n = batch order; scaled by the final RMSNorm below)
       float* stat_h = p.stat + (size_t)(2 * p.n_layer) * PC_RPAD;
       grid_wait();
@@ -1152,7 +1185,9 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
         // CFG mix, temperature, softmax, top-p over the ASCENDING order (drop cum <= 1-p, never the last), softmax of
         // the kept entries, arg-max of probs / Exp(1).  No sort: entry i's cumulative mass is the sum of e_j over all j
         // ordered before-or-at i; every CTA evaluates it for its own ~V/grid entries against the whole vocabulary.
-        float* s_key = reinterpret_cast<float*>(kvbuf);   // [V] (the KV tile slots are idle between tokens)
+        // scratch [V] each: the activation operand and the accumulator slots (contiguous) are idle from the head epilogue
+        // until this CTA stages the next token's qkv operand; the ring is not, the producer streams that token into it
+        float* s_key = reinterpret_cast<float*>(Bop);
         float* s_e = s_key + SAMP_PAD;
         const int per = (V + G - 1) / G;
         const int i0 = cta * per, n_own = max(0, min(V, i0 + per) - i0);
@@ -1242,6 +1277,8 @@ k_decode_persistent(const __grid_constant__ CUtensorMap tm_qkv, const __grid_con
           }
           compute_sync();                     // s_key / s_e are rewritten for the next utterance
         }
+        // the operand's rows >= R read as zero again
+        for (int i = ct; i < Cfg::B_BYTES / 16; i += 128) reinterpret_cast<uint4*>(Bop)[i] = make_uint4(0, 0, 0, 0);
         stamp();
         grid_arrive();
         grid_wait();                          // every CTA's kept mass is visible; nobody reads the logits any more

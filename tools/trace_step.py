@@ -1,4 +1,5 @@
-"""GPU debug: per-phase time breakdown of the persistent decode kernel (clock64 stamps of every CTA).
+"""GPU debug: per-phase time breakdown of the persistent decode kernel (clock64 stamps of every CTA), and how long the
+producer warp waited for a free ring stage in each phase of its byte schedule.
 Writes gpurun_out/trace_<n>.npy and prints medians per event interval."""
 import ctypes as C
 import os
@@ -31,11 +32,13 @@ for u in range(n):
     spk = synth.synthetic_speaker(seed=u).to(dev).reshape(-1).contiguous()
     _lib.check(lib.mvb_s1_set_speaker(h, u, spk.data_ptr(), st))
     _lib.check(lib.mvb_s1_begin(h, u, 100 + u, L_mid - 30, C.byref(sp), None, None, st))
-_lib.check(lib.mvb_s1_decode(h, n, 30, st))
+N_STEPS, N_STALL = 30, 6
+_lib.check(lib.mvb_s1_decode(h, n, N_STEPS, st))
 torch.cuda.synchronize()
 G = torch.cuda.get_device_properties(dev).multi_processor_count   # one CTA per SM
 buf = np.zeros((G, 512), dtype=np.int64)
 got = lib.mvb_s1_trace_fetch(h, buf.ctypes.data_as(C.c_void_p), G, st)
+stall = buf[:, 512 - N_STALL:]   # the producer stall record: the tail of every CTA's row (saved with the stamps below)
 os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
 np.save(os.path.join(ROOT, "gpurun_out", f"trace_{n}.npy"), buf)
 t = buf[:, :2 + 14 * 24 + 4].astype(np.float64)
@@ -49,3 +52,13 @@ for j, nm in enumerate(names):
     v = per[:, 2:, j]
     print(f"{nm:10s} median {np.median(v):7.2f}  mean {v.mean():7.2f}  p90 {np.percentile(v, 90):7.2f}  max {v.max():7.2f}")
 print("per-layer sum (median CTA):", np.median(per[:, 2:, :].sum(axis=2)))
+# producer blocked on a full ring (waiting for b_empty), summed over the launch; per layer and position (all 24 layers)
+# for the layer phases, per position for the head
+s = stall.astype(np.float64) / 1.9e3
+s[:, :5] /= N_STEPS * d.n_layer
+s[:, 5] /= N_STEPS
+print("producer blocked, us per layer (head: per position):")
+for j, nm in enumerate(["qkv", "kv", "wo", "w13", "w2", "head"]):
+    v = s[:, j]
+    print(f"{'blk.' + nm:10s} median {np.median(v):7.2f}  mean {v.mean():7.2f}  p90 {np.percentile(v, 90):7.2f}  max {v.max():7.2f}")
+print("producer blocked per layer (median CTA):", np.median(s[:, :5].sum(axis=1)))
