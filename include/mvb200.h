@@ -473,9 +473,19 @@ int mvb_spk_destroy(mvb_spk* h);
 int mvb_spk_mel(mvb_spk* h, const float* d_wav, int32_t n_samples, float* d_mel, void* stream);
 /* == SpeakerEncoder.embed_utterance on an already padded waveform: slice_starts (HOST int32 [n_partials]) are the first mel
  * frames of the partial windows (compute_partial_slices, model.py:55-79); d_embed fp32 [256]; d_partials_out optional
- * fp32 [n_partials, 256]. */
+ * fp32 [n_partials, 256].  MVB_ERR_ARG before anything is launched unless 1 <= n_partials <= 1024 and every window lies
+ * in the spectrogram: 0 <= start and start + partial_frames <= 1 + n_samples / hop. */
 int mvb_spk_embed(mvb_spk* h, const float* d_wav, int32_t n_samples, const int32_t* slice_starts, int32_t n_partials,
                   float* d_embed, float* d_partials_out, void* stream);
+/* Test hook for the speaker-encoder kernels (not part of the drop-in surface), through the launch helper of mvb_spk_embed
+ * with the handle's weights and configuration:
+ *   op 0: k_spk_lstm over a caller mel d_in fp32 [n_frames, n_mels] at the windows `starts` (HOST int32 [n_partials],
+ *         checked as mvb_spk_embed checks them) -> d_out fp32 [n_partials, 256]; d_trace optional fp32
+ *         [n_partials][partial_frames][3 layers][h, c][256], the LSTM state after every layer step.
+ *   op 1: k_spk_mean over d_in fp32 [n_partials, 256] -> d_out fp32 [256]; n_frames, starts and d_trace are not used.
+ * Synchronises `stream`. */
+int mvb_spk_op_test(mvb_spk* h, int32_t op, const float* d_in, int32_t n_frames, const int32_t* starts, int32_t n_partials,
+                    float* d_out, float* d_trace, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Audio post-processing on the device (SURVEY.md row N2) == `_save_audio` (fam/llm/decoders.py:40-47 -> audiocraft

@@ -68,8 +68,10 @@ struct SpkW {
 __device__ __forceinline__ float sigm(float v) { return 1.f / (1.f + expf(-v)); }
 
 // One partial window per CTA: 160 steps x 3 layers (torch.nn.LSTM, gate order i, f, g, o), then linear + ReLU + L2 norm.
+// trace (optional, tests only): [n_partials][T][3 layers][h, c][256], the state after every layer step.
 __global__ void __launch_bounds__(SPK_THREADS) k_spk_lstm(const float* __restrict__ mel, const int* __restrict__ starts, int n_frames,
-                                                          int T, int n_mels, SpkW W, float* __restrict__ partial_out) {
+                                                          int T, int n_mels, SpkW W, float* __restrict__ partial_out,
+                                                          float* __restrict__ trace) {
   constexpr int H = 256;
   __shared__ float xin[64];
   __shared__ float hs[3][H];
@@ -113,6 +115,11 @@ __global__ void __launch_bounds__(SPK_THREADS) k_spk_lstm(const float* __restric
       const float hn = og * tanhf(c[l]);
       __syncthreads();               // every warp has finished reading hs[l] / gates
       hs[l][tid] = hn;
+      if (trace) {
+        float* tr = trace + (((size_t)p * T + t) * 3 + l) * 2 * H;
+        tr[tid] = hn;
+        tr[H + tid] = c[l];
+      }
       __syncthreads();
     }
   }
@@ -218,24 +225,69 @@ extern "C" int mvb_spk_mel(mvb_spk* h, const float* d_wav, int32_t n_samples, fl
   return spk_mel(h, d_wav, n_samples, d_mel, (cudaStream_t)stream);
 }
 
+// The windows and the average, for mvb_spk_embed and mvb_spk_op_test alike.  With `starts` (HOST int32 [n_partials]):
+// k_spk_lstm over the windows of d_mel [n_frames, n_mels] -> d_partials [n_partials, 256] (+ d_trace when non-null);
+// with d_embed: k_spk_mean over d_partials -> d_embed [256].  Every window must lie inside the mel: k_spk_lstm reads frames
+// start .. start + partial_frames - 1, and a window past either end is neither in the spectrogram nor a window the
+// reference can form.
+static int spk_check_windows(const mvb_spk* h, int n_frames, const int32_t* starts, int n_partials) {
+  if (n_partials < 1 || n_partials > 1024) return mvb::set_error(MVB_ERR_ARG, "n_partials %d out of range", n_partials);
+  if (!starts) return MVB_OK;
+  for (int i = 0; i < n_partials; ++i)
+    if (starts[i] < 0 || (long long)starts[i] + h->cfg.partial_frames > n_frames)
+      return mvb::set_error(MVB_ERR_ARG, "window %d starts at mel frame %d: %d frames from there do not fit in %d", i, starts[i],
+                            h->cfg.partial_frames, n_frames);
+  return MVB_OK;
+}
+
+static int spk_windows(mvb_spk* h, const float* d_mel, int n_frames, const int32_t* starts, int n_partials, float* d_partials,
+                       float* d_trace, float* d_embed, cudaStream_t s) {
+  if (int e = spk_check_windows(h, n_frames, starts, n_partials)) return e;
+  const mvb_spk_config& c = h->cfg;
+  if (starts) {
+    MVB_CK(cudaMemcpyAsync(h->starts(), starts, sizeof(int) * n_partials, cudaMemcpyHostToDevice, s));
+    SpkW W;
+    for (int l = 0; l < 3; ++l) { W.w_ih[l] = h->w(3 * l); W.w_hh[l] = h->w(3 * l + 1); W.b[l] = h->w(3 * l + 2); }
+    W.lw = h->w(9); W.lb = h->w(10);
+    k_spk_lstm<<<n_partials, SPK_THREADS, 0, s>>>(d_mel, h->starts(), n_frames, c.partial_frames, c.n_mels, W, d_partials, d_trace);
+    MVB_CK(cudaGetLastError());
+  }
+  if (d_embed) {
+    k_spk_mean<<<1, SPK_THREADS, 0, s>>>(d_partials, n_partials, d_embed);
+    MVB_CK(cudaGetLastError());
+  }
+  return MVB_OK;
+}
+
 extern "C" int mvb_spk_embed(mvb_spk* h, const float* d_wav, int32_t n_samples, const int32_t* slice_starts, int32_t n_partials,
                              float* d_embed, float* d_partials_out, void* stream) {
   if (!h || !d_wav || !slice_starts || !d_embed) return mvb::set_error(MVB_ERR_ARG, "null argument");
   if (n_samples < 1 || n_samples > h->cfg.max_samples) return mvb::set_error(MVB_ERR_ARG, "n_samples %d out of range", n_samples);
-  if (n_partials < 1 || n_partials > 1024) return mvb::set_error(MVB_ERR_ARG, "n_partials %d out of range", n_partials);
   cudaStream_t s = (cudaStream_t)stream;
-  const mvb_spk_config& c = h->cfg;
-  const int n_frames = 1 + n_samples / c.hop;
+  const int n_frames = 1 + n_samples / h->cfg.hop;
+  if (int e = spk_check_windows(h, n_frames, slice_starts, n_partials)) return e;   // before anything is launched
   if (int e = spk_mel(h, d_wav, n_samples, h->mel(), s)) return e;
-  MVB_CK(cudaMemcpyAsync(h->starts(), slice_starts, sizeof(int) * n_partials, cudaMemcpyHostToDevice, s));
-  SpkW W;
-  for (int l = 0; l < 3; ++l) { W.w_ih[l] = h->w(3 * l); W.w_hh[l] = h->w(3 * l + 1); W.b[l] = h->w(3 * l + 2); }
-  W.lw = h->w(9); W.lb = h->w(10);
-  k_spk_lstm<<<n_partials, SPK_THREADS, 0, s>>>(h->mel(), h->starts(), n_frames, c.partial_frames, c.n_mels, W, h->partials());
-  MVB_CK(cudaGetLastError());
-  k_spk_mean<<<1, SPK_THREADS, 0, s>>>(h->partials(), n_partials, d_embed);
-  MVB_CK(cudaGetLastError());
+  if (int e = spk_windows(h, h->mel(), n_frames, slice_starts, n_partials, h->partials(), nullptr, d_embed, s)) return e;
   if (d_partials_out)
     MVB_CK(cudaMemcpyAsync(d_partials_out, h->partials(), sizeof(float) * (size_t)n_partials * 256, cudaMemcpyDeviceToDevice, s));
+  return MVB_OK;
+}
+
+extern "C" int mvb_spk_op_test(mvb_spk* h, int32_t op, const float* d_in, int32_t n_frames, const int32_t* starts, int32_t n_partials,
+                               float* d_out, float* d_trace, void* stream) {
+  if (!h || !d_in || !d_out) return mvb::set_error(MVB_ERR_ARG, "null argument");
+  cudaStream_t s = (cudaStream_t)stream;
+  int e;
+  if (op == 0) {
+    if (!starts) return mvb::set_error(MVB_ERR_ARG, "null argument");
+    if (n_frames < 1) return mvb::set_error(MVB_ERR_ARG, "mvb_spk_op_test: n_frames %d", n_frames);
+    e = spk_windows(h, d_in, n_frames, starts, n_partials, d_out, d_trace, nullptr, s);
+  } else if (op == 1) {
+    e = spk_windows(h, nullptr, 0, nullptr, n_partials, const_cast<float*>(d_in), nullptr, d_out, s);
+  } else {
+    return mvb::set_error(MVB_ERR_ARG, "mvb_spk_op_test: op %d", op);
+  }
+  if (e) return e;
+  MVB_CK(cudaStreamSynchronize(s));
   return MVB_OK;
 }

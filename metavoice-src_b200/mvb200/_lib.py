@@ -154,6 +154,8 @@ SIGNATURES = {
                                   C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "mvb_audio_post_test": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p]),
+    "mvb_spk_op_test": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                  C.c_void_p]),
 }
 ABI_VERSION = 2
 

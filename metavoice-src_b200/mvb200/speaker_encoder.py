@@ -147,8 +147,11 @@ class SpeakerEncoder:
         for t, o in zip(tensors, offs):
             arena[o:o + t.numel() * 4] = t.contiguous().reshape(-1).view(torch.uint8)
         self._arena = arena.to(self.device)
+        # embed_utterance pads the waveform to the end of its last partial window, up to one window past the input: the
+        # workspace holds max_seconds of input plus that window
+        self.max_input_samples = int(max_seconds * sampling_rate)
         cfg = _lib.SpkConfig(mel_n_channels, model_hidden_size, model_num_layers, model_embedding_size, n_fft, hop,
-                             partials_n_frames, int(max_seconds * sampling_rate))
+                             partials_n_frames, self.max_input_samples + partials_n_frames * hop)
         self.cfg, self._lib = cfg, _lib.load()
         wsb = self._lib.mvb_spk_workspace_bytes(C.byref(cfg))
         if wsb == 0:
@@ -197,12 +200,12 @@ class SpeakerEncoder:
 
     @torch.no_grad()
     def embed_utterance(self, wav: np.ndarray, return_partials=False, rate=1.3, min_coverage=0.75, numpy: bool = True):
+        if len(wav) > self.max_input_samples:
+            raise ValueError(f"speaker reference longer than {self.max_input_samples / sampling_rate:g} s")
         wav_slices, mel_slices = self.compute_partial_slices(len(wav), rate, min_coverage)
         max_wave_length = wav_slices[-1].stop
         if max_wave_length >= len(wav):
             wav = np.pad(wav, (0, max_wave_length - len(wav)), "constant")
-        if len(wav) > self.cfg.max_samples:
-            raise ValueError(f"speaker reference longer than {self.cfg.max_samples / sampling_rate:.0f} s")
         w = torch.from_numpy(np.ascontiguousarray(wav, dtype=np.float32)).to(self.device)
         starts = np.asarray([s.start for s in mel_slices], dtype=np.int32)
         embed = torch.empty(model_embedding_size, dtype=torch.float32, device=self.device)

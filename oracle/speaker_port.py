@@ -51,14 +51,19 @@ def hann_periodic(n=N_FFT) -> np.ndarray:
     return (0.5 - 0.5 * np.cos(2 * np.pi * np.arange(n) / n)).astype(np.float32)
 
 
-def mel_spectrogram(wav: np.ndarray) -> np.ndarray:
-    """audio.py:10-22: power mel spectrogram (NOT log), [n_frames, 40] fp32, n_frames = 1 + len(wav) // 160."""
+def mel_spectrogram(wav: np.ndarray, dtype=np.float32) -> np.ndarray:
+    """audio.py:10-22: power mel spectrogram (NOT log), [n_frames, 40], n_frames = 1 + len(wav) // 160.  float32: the
+    window and the windowed frames in fp32, as librosa computes them; float64: the float64 periodic Hann window, no
+    rounding before the filterbank (whose fp32 values are librosa's)."""
     y = np.pad(np.asarray(wav, dtype=np.float32), N_FFT // 2)          # center=True, pad_mode="constant" (librosa 0.10)
     n_frames = 1 + (len(y) - N_FFT) // HOP
     idx = np.arange(N_FFT)[None, :] + HOP * np.arange(n_frames)[:, None]
-    frames = y[idx] * hann_periodic()[None, :]
+    if dtype == np.float64:
+        frames = y[idx].astype(np.float64) * (0.5 - 0.5 * np.cos(2 * np.pi * np.arange(N_FFT) / N_FFT))[None, :]
+    else:
+        frames = y[idx] * hann_periodic()[None, :]
     spec = np.abs(np.fft.rfft(frames.astype(np.float64), axis=1)) ** 2
-    return (spec @ mel_filterbank().astype(np.float64).T).astype(np.float32)
+    return (spec @ mel_filterbank().astype(np.float64).T).astype(dtype)
 
 
 def compute_partial_slices(n_samples: int, rate: float = 1.3, min_coverage: float = 0.75):
@@ -79,8 +84,12 @@ def compute_partial_slices(n_samples: int, rate: float = 1.3, min_coverage: floa
 
 
 class SpeakerOracle:
-    def __init__(self, model_state: dict):
-        g = lambda k: model_state[k].float()
+    """dtype: the arithmetic of the network, the average and (float64) the mel front-end; the weights are the
+    checkpoint's fp32 values either way."""
+
+    def __init__(self, model_state: dict, dtype: torch.dtype = torch.float32):
+        self.dtype = dtype
+        g = lambda k: model_state[k].float().to(dtype)
         self.layers = [dict(w_ih=g(f"lstm.weight_ih_l{l}"), w_hh=g(f"lstm.weight_hh_l{l}"), b=g(f"lstm.bias_ih_l{l}") + g(f"lstm.bias_hh_l{l}"))
                        for l in range(3)]
         self.lw, self.lb = g("linear.weight"), g("linear.bias")
@@ -88,11 +97,11 @@ class SpeakerOracle:
     @torch.no_grad()
     def forward(self, mels: torch.Tensor) -> torch.Tensor:
         """mels [P, T, 40] -> L2-normalised embeddings [P, 256] (model.py:50-53; torch.nn.LSTM gate order i, f, g, o)."""
-        x = mels.float()
+        x = mels.to(self.dtype)
         for L in self.layers:
             P, T, _ = x.shape
             H = L["w_hh"].shape[1]
-            h, c = torch.zeros(P, H), torch.zeros(P, H)
+            h, c = torch.zeros(P, H, dtype=self.dtype), torch.zeros(P, H, dtype=self.dtype)
             ys = []
             for t in range(T):
                 gts = x[:, t] @ L["w_ih"].t() + h @ L["w_hh"].t() + L["b"]
@@ -104,11 +113,11 @@ class SpeakerOracle:
         e = torch.relu(x[:, -1] @ self.lw.t() + self.lb)
         return e / torch.norm(e, dim=1, keepdim=True)
 
-    def embed_utterance(self, wav: np.ndarray, rate: float = 1.3, min_coverage: float = 0.75, mel_fn=mel_spectrogram):
+    def embed_utterance(self, wav: np.ndarray, rate: float = 1.3, min_coverage: float = 0.75, mel_fn=None):
         wav_s, mel_s = compute_partial_slices(len(wav), rate, min_coverage)
         if wav_s[-1][1] >= len(wav):
             wav = np.pad(wav, (0, wav_s[-1][1] - len(wav)), "constant")
-        mel = mel_fn(wav)
+        mel = mel_fn(wav) if mel_fn is not None else mel_spectrogram(wav, np.float64 if self.dtype == torch.float64 else np.float32)
         mels = torch.from_numpy(np.array([mel[a:b] for a, b in mel_s]))
         pe = self.forward(mels)
         raw = pe.mean(dim=0)

@@ -31,7 +31,7 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(lib, name), f"{name} declared in include/mvb200.h but not exported"
     assert set(_declared()) == set(_lib.SIGNATURES), "python binding table out of sync with the header"
     for hook in ("mvb_gemm_test", "mvb_mbd_conv_test", "mvb_mbd_op_test", "mvb_s2_attn_test", "mvb_s2_sample_test", "mvb_voc_op_test",
-                 "mvb_audio_post_test"):
+                 "mvb_audio_post_test", "mvb_spk_op_test"):
         assert hook in _lib.SIGNATURES and hasattr(lib, hook), f"test hook {hook} missing"
     assert lib.mvb_abi_version() == _lib.ABI_VERSION == 2
 
@@ -46,6 +46,20 @@ def test_config_validation_without_gpu():
     bad = _lib.S1Config(24, 16, 64, 1024, 5632, 2562, 2048, 256, 1e-5, 1, 0, 2048)
     assert lib.mvb_s1_kv_bytes(ctypes.byref(bad)) == 0
     assert b"head_dim" in lib.mvb_last_error()
+    # speaker encoder: 1..64 mel bands (k_spk_lstm's input buffer), 2..2048-point frames, hop >= 1, and only the
+    # reference's 256-wide 3-layer network
+    def spk(**kw):
+        return _lib.SpkConfig(**{**dict(n_mels=40, hidden=256, n_layers=3, emb=256, n_fft=400, hop=160, partial_frames=160,
+                                        max_samples=16000), **kw})
+
+    assert lib.mvb_spk_workspace_bytes(ctypes.byref(spk())) > 0
+    for kw in (dict(n_mels=64), dict(n_mels=1), dict(n_fft=2), dict(n_fft=2048), dict(hop=1)):
+        assert lib.mvb_spk_workspace_bytes(ctypes.byref(spk(**kw))) > 0, kw
+    for kw, msg in ((dict(n_mels=0), b"front-end"), (dict(n_mels=65), b"front-end"), (dict(n_fft=1), b"front-end"),
+                    (dict(n_fft=2049), b"front-end"), (dict(hop=0), b"front-end"), (dict(hidden=128), b"3 layers"),
+                    (dict(n_layers=2), b"3 layers")):
+        assert lib.mvb_spk_workspace_bytes(ctypes.byref(spk(**kw))) == 0, kw
+        assert msg in lib.mvb_last_error(), (kw, lib.mvb_last_error())
 
 
 _MBD_VALIDATE = r"""

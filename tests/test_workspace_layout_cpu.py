@@ -86,7 +86,9 @@ def test_mbd_workspace_bytes(lib, monkeypatch, env, max_seconds, want):
 
 @pytest.mark.parametrize("max_seconds,want", [(180.0, 3932928), (30.0, 1532928)])
 def test_speaker_workspace_bytes(lib, max_seconds, want):
-    cfg = _lib.SpkConfig(40, 256, 3, 256, 400, 160, 160, int(max_seconds * 16000))   # SpeakerEncoder's configuration
+    # SpeakerEncoder's front end and network at an explicit capacity (SpeakerEncoder(max_seconds=s) itself asks for
+    # s * 16000 samples plus one 160-frame window, the most embed_utterance pads an s-second reference to)
+    cfg = _lib.SpkConfig(40, 256, 3, 256, 400, 160, 160, int(max_seconds * 16000))
     assert lib.mvb_spk_workspace_bytes(C.byref(cfg)) == want
 
 
