@@ -20,7 +20,7 @@
 extern "C" {
 #endif
 
-#define MVB_ABI_VERSION 2
+#define MVB_ABI_VERSION 3
 
 /* KV-cache element type.  bf16 is what the reference stores (fast_model.py:97-102);
  * fp32 is the validation mode used for the <=1e-3 parity gate against the fp32 oracle. */
@@ -40,7 +40,15 @@ typedef struct mvb_s1_config {
   int32_t max_utts;      /* utterance slots; each owns 2 CFG rows {cond, uncond} (fast_model.py:132-134) */
   int32_t kv_dtype;      /* MVB_KV_BF16 | MVB_KV_FP32 */
   int32_t max_new;       /* capacity of the per-utterance generated-token ring (<= block_size) */
+  int32_t options;       /* MVB_S1_* bits below; 0 = the production engine */
 } mvb_s1_config;
+
+/* Stage-1 options: reference and identity paths for tests and tools, fixed at create time.  The workspace and KV sizes
+ * do not depend on them; any other bit is MVB_ERR_ARG. */
+#define MVB_S1_NO_ROWS_PATH    0x1 /* no tensor-core rows path: prefill and batched decode run on the CUDA-core kernels */
+#define MVB_S1_NO_RESIDENT     0x2 /* no resident (persistent) decode kernel: decode runs on the per-layer path */
+#define MVB_S1_UNFUSED_SAMPLER 0x4 /* the resident kernel leaves the logits to k_sample instead of sampling in the kernel */
+#define MVB_S1_TRACE           0x8 /* the resident kernel records per-phase clocks for mvb_s1_trace_fetch */
 
 /* Byte offsets (into one bf16 weight arena) of every stage-1 tensor, row-major [out, in]
  * exactly as stored in first_stage.pt (SURVEY.md App. B).  Built by the checkpoint loader that
@@ -175,7 +183,7 @@ uint64_t mvb_s1_launch_count(const mvb_s1* h);
 /* Test / debug hooks (not part of the drop-in surface; used by tests/ and tools/ only):
  *   mvb_s1_fetch_sampled : the sampler's own draws for `utt` (they differ from the fed-back tokens of mvb_s1_fetch only
  *                          under teacher forcing), host int32 [cap];
- *   mvb_s1_trace_fetch   : per-CTA clock64 phase stamps of the last persistent-kernel step (MVB_PC_TRACE=1), host
+ *   mvb_s1_trace_fetch   : per-CTA clock64 phase stamps of the last persistent-kernel step (MVB_S1_TRACE), host
  *                          int64 [max_ctas, 512]; the last 6 entries of a CTA's row are its producer warp's stall cycles
  *                          of the whole launch per phase (qkv, KV tiles, wo, w1|w3, w2, head); returns the number of CTAs
  *                          copied. */
@@ -292,7 +300,10 @@ typedef struct mvb_s2_config {
   int32_t spk_dim;
   float   norm_eps;
   int32_t max_batch;
+  int32_t options;         /* MVB_S2_* bits below; 0 = the production engine */
 } mvb_s2_config;
+/* Stage-2 option (fixed at create time; the workspace size does not depend on it; any other bit is MVB_ERR_ARG): */
+#define MVB_S2_EAGER 0x1   /* launch the forward pass kernel by kernel instead of replaying a captured CUDA graph */
 typedef struct mvb_s2 mvb_s2;
 
 size_t mvb_s2_workspace_bytes(const mvb_s2_config* cfg);
@@ -426,7 +437,12 @@ typedef struct mvb_mbd_config {
   int32_t proc_bands, proc_taps;   /* MultiBandProcessor: SplitBands(n_bands) and its filter length */
   int32_t eq_bands, eq_taps;       /* re_eq: 32 bands and the filter length */
   int32_t max_samples;     /* workspace capacity (samples at 24 kHz) */
+  int32_t options;         /* MVB_MBD_* bits below; 0 = the production engine */
 } mvb_mbd_config;
+/* MBD options, fixed at create time.  Both change the workspace layout, which mvb_mbd_workspace_bytes computes from the
+ * same config; any other bit is MVB_ERR_ARG. */
+#define MVB_MBD_CUDA_CORES 0x1 /* every convolution on the fp32 CUDA-core kernels (no packed bf16 taps, no tensor cores) */
+#define MVB_MBD_ONE_STREAM 0x2 /* band models back to back on the caller's stream with one activation block */
 typedef struct mvb_mbd mvb_mbd;
 /* fp32 arena tensors (offsets, host): for every band model, in this order
  *   per encoder level: conv.weight [C, Cin, k], norm.weight, norm.bias, res_blocks x {norm1.w, norm1.b, conv1.w [C,C,3], conv1.b,

@@ -13,7 +13,6 @@
 // (julius.SplitBands: windowed-sinc low-pass banks, 629 / 2893 taps) are direct FIR kernels.
 #include <cuda_runtime.h>
 #include <math.h>
-#include <stdlib.h>
 
 #include <vector>
 
@@ -376,7 +375,7 @@ __global__ void k_gn_relu_inplace(float* x, int C, int T, int cpg, const float* 
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------------------------
-// Workspace layout, fixed at create time together with the MVB_MBD_NO_TC / MVB_MBD_STREAMS switches it depends on
+// Workspace layout, a function of the config alone (the MVB_MBD_CUDA_CORES / MVB_MBD_ONE_STREAM options included)
 struct MbdWs {
   size_t cur, est, noise, wav, cond, gn, gn_part, stdv, low, skip[8], tmp[3], xt_hi, xt_lo;   // offsets inside one activation block
   size_t blk, wpack, total;   // block size; the packed taps follow n_blk blocks (one block per concurrently running band model)
@@ -423,6 +422,8 @@ static int mbd_validate(const mvb_mbd_config* c) {
     if (L < 1 || fir_smem_bytes(L) > FIR_SMEM_MAX)
       return mvb::set_error(MVB_ERR_UNSUPPORTED, "mbd: filter length %d (1 .. %d taps)", L, (int)((FIR_SMEM_MAX / 4 - FIR_TT) / 3));
   if (c->max_samples < c->stride) return mvb::set_error(MVB_ERR_ARG, "mbd: max_samples");
+  const int known = MVB_MBD_CUDA_CORES | MVB_MBD_ONE_STREAM;
+  if (c->options & ~known) return mvb::set_error(MVB_ERR_ARG, "mbd: options: undefined bits 0x%x", (unsigned)(c->options & ~known));
   return MVB_OK;
 }
 static int mbd_per_model(const mvb_mbd_config* c) { return c->depth * (3 + 8 * c->res_blocks + 1) + 2 + c->depth * (8 * c->res_blocks + 3) + 2; }
@@ -483,8 +484,7 @@ static MbdWs mbd_layout(const mvb_mbd_config* c) {
   L.xt_hi = ws.take(xt);
   L.xt_lo = ws.take(xt);
   WsBump wp;   // the packed taps of one band model
-  const char* no_tc = getenv("MVB_MBD_NO_TC");
-  L.tc = !(no_tc && no_tc[0] == '1');
+  L.tc = !(c->options & MVB_MBD_CUDA_CORES);
   if (L.tc)
     mbd_for_each_conv(c, [&](int, int cin, int cout, int k, int) {
       if (mbd_tc_eligible(cin)) wp.take((size_t)k * cout * mbd_tc_cpad(cin) * 2);
@@ -492,8 +492,7 @@ static MbdWs mbd_layout(const mvb_mbd_config* c) {
   L.blk = (ws.end + 4095) / 4096 * 4096;
   // The band models are independent until their outputs are summed: each runs on its own stream with its own activation
   // block, so the many sub-wave kernels of one UNet (96-CTA convolutions, 4-CTA reductions) overlap with the other models'.
-  const char* streams = getenv("MVB_MBD_STREAMS");
-  L.n_blk = (!(streams && streams[0] == '0') && c->n_models > 1) ? c->n_models : 1;
+  L.n_blk = (!(c->options & MVB_MBD_ONE_STREAM) && c->n_models > 1) ? c->n_models : 1;
   L.wpack = L.blk * L.n_blk;
   L.total = L.wpack + wp.end * c->n_models + 256;
   return L;

@@ -2,7 +2,6 @@
 // No torch, no CPU fallback: every entry point either runs the CUDA path or fails loudly.
 #include <cuda_runtime.h>
 
-#include <cstdlib>
 #include <cstring>
 #include <map>
 #include <vector>
@@ -123,13 +122,12 @@ struct mvb_s1 {
   std::vector<CUtensorMap> tmW;                       // per layer {wqkv, wo, w1, w3, w2}, then lm_head
   std::map<std::pair<int, int>, CUtensorMap> tmB;     // (NB, K) -> activation buffer map
   bool path_b = true;                                 // tensor-core rows path for batched decode and prefill
-  bool pdl = true;                                    // programmatic dependent launch between body kernels
   RowsDev rows;
   // path C
   bool path_c = true;
   bool pc_ok = false;
   bool trace = false;
-  bool fused = true;                                  // sample inside the persistent kernel (multi-token launches; MVB_PC_FUSED)
+  bool fused = true;                                  // sample inside the persistent kernel (multi-token launches)
   CUtensorMap tm_kv;                                  // bf16 cache: 2-D map over the whole KV arena: [rows = layer, k|v, cache row, head, pos][128]
   CUtensorMap tm3[6];                                 // 3-D (k, row, layer) maps: wqkv, wo, w1, w3, w2, head
   PcMat pm[5];
@@ -192,6 +190,8 @@ static int validate(const mvb_s1_config* c) {
   if (c->max_new < 1 || c->max_new > c->block_size) return set_error(MVB_ERR_ARG, "max_new out of range");
   if (c->kv_dtype != MVB_KV_BF16 && c->kv_dtype != MVB_KV_FP32) return set_error(MVB_ERR_ARG, "bad kv_dtype");
   if ((size_t)c->intermediate * 8 > 48 * 1024 - 256) return set_error(MVB_ERR_UNSUPPORTED, "intermediate too large for the staging buffer");
+  const int known = MVB_S1_NO_ROWS_PATH | MVB_S1_NO_RESIDENT | MVB_S1_UNFUSED_SAMPLER | MVB_S1_TRACE;
+  if (c->options & ~known) return set_error(MVB_ERR_ARG, "options: undefined bits 0x%x", (unsigned)(c->options & ~known));
   return MVB_OK;
 }
 
@@ -259,8 +259,10 @@ static int create_engine(const mvb_s1_config* cfg, const void* d_arena, size_t a
   s.noise_base = h->wsp<int>(h->L.noise_base);
   s.max_new = cfg->max_new;
   s.block_size = cfg->block_size;
-  if (const char* e = getenv("MVB_PATHB")) h->path_b = atoi(e) != 0;
-  if (const char* e = getenv("MVB_PDL")) h->pdl = atoi(e) != 0;
+  h->path_b = !(cfg->options & MVB_S1_NO_ROWS_PATH);
+  h->path_c = !(cfg->options & MVB_S1_NO_RESIDENT);
+  h->fused = !(cfg->options & MVB_S1_UNFUSED_SAMPLER);
+  h->trace = (cfg->options & MVB_S1_TRACE) != 0;
   {
     int* rb = h->wsp<int>(h->L.b_rows);
     h->rows.cache_row = rb; h->rows.pos = rb + RB_MAX; h->rows.tok = rb + 2 * RB_MAX; h->rows.utt = rb + 3 * RB_MAX;
@@ -278,9 +280,6 @@ static int create_engine(const mvb_s1_config* cfg, const void* d_arena, size_t a
     ok = ok && make_tmap_bf16(&h->tmW[(size_t)cfg->n_layer * 5], h->w(4), cfg->vocab, D, 128);
     if (!ok) return set_error(MVB_ERR_CUDA, "cuTensorMapEncodeTiled failed for a weight matrix");
   }
-  if (const char* e = getenv("MVB_PATHC")) h->path_c = atoi(e) != 0;
-  if (const char* e = getenv("MVB_PC_TRACE")) h->trace = atoi(e) != 0;
-  if (const char* e = getenv("MVB_PC_FUSED")) h->fused = atoi(e) != 0;
   // The persistent kernel's bf16-cache attention fetches KV tiles through tm_kv as whole 64-position boxes: positions
   // past the valid ones must hold finite values, and the map must be encodable.  Where it is not, path C is declined.
   memset(&h->tm_kv, 0, sizeof(h->tm_kv));
@@ -362,8 +361,7 @@ static int gemv_grid(int n_items, int n_sm) {
 // Launch with the programmatic-dependent-launch attribute: the kernel may start while its predecessor in the
 // stream drains; it prefetches weights, then griddepcontrol.wait orders it after the predecessor's writes.
 template <typename... KArgs, typename... Args>
-static cudaError_t launch_pdl(bool pdl, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s,
-                              Args... args) {
+static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args... args) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = grid;
   cfg.blockDim = block;
@@ -373,7 +371,7 @@ static cudaError_t launch_pdl(bool pdl, void (*kernel)(KArgs...), dim3 grid, dim
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = pdl ? 1 : 0;
+  cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
 
@@ -384,8 +382,8 @@ static cudaError_t launch_gemv(mvb_s1* h, cudaStream_t s, int n_utts, GemvP p, b
   dim3 grid(gemv_grid(n_items, h->n_sm), n_utts);
   const size_t smem = (size_t)2 * p.K * sizeof(float);
   h->launches++;
-  if (w4) return launch_pdl(h->pdl, k_gemv_w4<EPI>, grid, dim3(256), smem, s, p, h->st);
-  return launch_pdl(h->pdl, k_gemv<EPI>, grid, dim3(256), smem, s, p, h->st);
+  if (w4) return launch_pdl(k_gemv_w4<EPI>, grid, dim3(256), smem, s, p, h->st);
+  return launch_pdl(k_gemv<EPI>, grid, dim3(256), smem, s, p, h->st);
 }
 
 // One forward position for `n_utts` logical utterances: embed -> 24 x (attention, FFN) -> head.
@@ -397,7 +395,7 @@ static int launch_body(mvb_s1* h, cudaStream_t s, int n_utts) {
   float* att = h->wsp<float>(h->L.att);
   float* ffn = h->wsp<float>(h->L.ffn);
   float* logits = h->wsp<float>(h->L.logits);
-  MVB_CK(launch_pdl(h->pdl, k_embed, dim3(2, n_utts), dim3(256), 0, s, h->st, h->w(0), h->w(1),
+  MVB_CK(launch_pdl(k_embed, dim3(2, n_utts), dim3(256), 0, s, h->st, h->w(0), h->w(1),
                 (const float*)h->wsp<float>(h->L.spk), x, D));
   h->launches++;
   const size_t half = h->kv_half_bytes();
@@ -414,10 +412,10 @@ static int launch_body(mvb_s1* h, cudaStream_t s, int n_utts) {
     // attention over [0, pos]
     dim3 ag(H, 2 * n_utts, ATT_SPLITS);
     if (c.kv_dtype == MVB_KV_FP32)
-      MVB_CK(launch_pdl(h->pdl, k_attn_decode<true>, ag, dim3(128), 0, s, h->st, (const float*)qkv, (const void*)kc, (const void*)vc,
+      MVB_CK(launch_pdl(k_attn_decode<true>, ag, dim3(128), 0, s, h->st, (const float*)qkv, (const void*)kc, (const void*)vc,
                     h->wsp<float>(h->L.part_o), h->wsp<float>(h->L.part_ml), att, H, c.block_size, D));
     else
-      MVB_CK(launch_pdl(h->pdl, k_attn_decode<false>, ag, dim3(128), 0, s, h->st, (const float*)qkv, (const void*)kc, (const void*)vc,
+      MVB_CK(launch_pdl(k_attn_decode<false>, ag, dim3(128), 0, s, h->st, (const float*)qkv, (const void*)kc, (const void*)vc,
                     h->wsp<float>(h->L.part_o), h->wsp<float>(h->L.part_ml), att, H, c.block_size, D));
     h->launches++;
     // wo + residual
@@ -572,7 +570,7 @@ static int launch_persistent(mvb_s1* h, cudaStream_t s, int n_utts, int n_steps,
   const bool fp = p.kv_fp32 != 0, wide = p.R > 8;
   const CUtensorMap* tm = h->tm3;
 #define MVB_PC_LAUNCH(FP, NBV)                                                                                        \
-  MVB_CK(launch_pdl(h->pdl, k_decode_persistent<FP, NBV>, dim3(h->n_sm), dim3(PC_THREADS), PcCfg<NBV>::SMEM, s,           \
+  MVB_CK(launch_pdl(k_decode_persistent<FP, NBV>, dim3(h->n_sm), dim3(PC_THREADS), PcCfg<NBV>::SMEM, s,                   \
                 tm[0], tm[1], tm[2], tm[3], tm[4], tm[5], h->tm_kv, p))
   if (fp && wide) MVB_PC_LAUNCH(true, 32);
   else if (fp) MVB_PC_LAUNCH(true, 16);
@@ -821,7 +819,7 @@ static int sample_step(mvb_s1* h, cudaStream_t s, int n_utts) {
   sp.decode_mode = 1;
   sp.grid_bar = h->wsp<unsigned>(h->L.c_bar);
   h->launches++;
-  MVB_CK(launch_pdl(h->pdl, k_sample, dim3(n_utts), dim3(SAMP_THREADS), 0, s, sp, h->st));
+  MVB_CK(launch_pdl(k_sample, dim3(n_utts), dim3(SAMP_THREADS), 0, s, sp, h->st));
   return MVB_OK;
 }
 

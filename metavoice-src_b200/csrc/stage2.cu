@@ -7,7 +7,6 @@
 // the reference); sampling is one CTA per (hierarchy, position).
 #include <cuda_runtime.h>
 
-#include <cstdlib>
 #include <vector>
 
 #include "common.cuh"
@@ -284,6 +283,8 @@ static int s2_validate(const mvb_s2_config* c) {
   for (int i = 0; i < c->n_out; ++i)
     if (c->vocab_out[i] > S2_PAD) return mvb::set_error(MVB_ERR_UNSUPPORTED, "target vocab > %d", S2_PAD);
   if (c->max_batch < 1 || c->max_batch > 64 || c->block_size < 1) return mvb::set_error(MVB_ERR_ARG, "bad batch / block size");
+  if (c->options & ~MVB_S2_EAGER)
+    return mvb::set_error(MVB_ERR_ARG, "options: undefined bits 0x%x", (unsigned)(c->options & ~MVB_S2_EAGER));
   return MVB_OK;
 }
 
@@ -309,7 +310,7 @@ extern "C" int mvb_s2_create(const mvb_s2_config* cfg, const void* d_arena, size
   h->ws = reinterpret_cast<char*>(d_ws);
   const S2Layout L = s2_layout(cfg);
   h->idx_stage = (int*)(h->ws + L.idx); h->spk_stage = (float*)(h->ws + L.spk_stage); h->params = (S2SampleParams*)(h->ws + L.params);
-  h->use_graph = getenv("MVB_S2_NO_GRAPH") == nullptr;
+  h->use_graph = !(cfg->options & MVB_S2_EAGER);
   h->x = (float*)(h->ws + L.x); h->qkv = (float*)(h->ws + L.qkv); h->att = (float*)(h->ws + L.att); h->ffn = (float*)(h->ws + L.ffn);
   h->logits = (float*)(h->ws + L.logits); h->spk_proj = (float*)(h->ws + L.spk); h->B = (__nv_bfloat16*)(h->ws + L.B);
   h->scratch = (float*)(h->ws + L.scratch); h->tickets = (unsigned*)(h->ws + L.tickets); h->tokens = (int*)(h->ws + L.tokens);

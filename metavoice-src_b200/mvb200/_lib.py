@@ -11,13 +11,17 @@ LIB_PATH = os.environ.get("MVB200_LIB") or os.path.join(_HERE, "libmvb200.so")  
 MVB_KV_BF16, MVB_KV_FP32 = 0, 1
 MVB_OK, MVB_ERR_CUDA, MVB_ERR_ARG, MVB_ERR_PROMPT_TOO_LONG, MVB_ERR_UNSUPPORTED = 0, 1, 2, 3, 4
 GLOBAL_TENSORS, LAYER_TENSORS = 5, 7
+# `options` bits of the engine configs (include/mvb200.h): reference and identity paths, fixed at create time
+MVB_S1_NO_ROWS_PATH, MVB_S1_NO_RESIDENT, MVB_S1_UNFUSED_SAMPLER, MVB_S1_TRACE = 0x1, 0x2, 0x4, 0x8
+MVB_S2_EAGER = 0x1
+MVB_MBD_CUDA_CORES, MVB_MBD_ONE_STREAM = 0x1, 0x2
 
 
 class S1Config(C.Structure):
     _fields_ = [("n_layer", C.c_int32), ("n_head", C.c_int32), ("head_dim", C.c_int32), ("dim", C.c_int32),
                 ("intermediate", C.c_int32), ("vocab", C.c_int32), ("block_size", C.c_int32),
                 ("spk_dim", C.c_int32), ("norm_eps", C.c_float), ("max_utts", C.c_int32),
-                ("kv_dtype", C.c_int32), ("max_new", C.c_int32)]
+                ("kv_dtype", C.c_int32), ("max_new", C.c_int32), ("options", C.c_int32)]
 
 
 class Sampling(C.Structure):
@@ -28,7 +32,8 @@ class Sampling(C.Structure):
 class S2Config(C.Structure):
     _fields_ = [("n_layer", C.c_int32), ("n_head", C.c_int32), ("n_embd", C.c_int32), ("hidden", C.c_int32),
                 ("block_size", C.c_int32), ("n_in", C.c_int32), ("vocab_in", C.c_int32 * 8), ("n_out", C.c_int32),
-                ("vocab_out", C.c_int32 * 8), ("spk_dim", C.c_int32), ("norm_eps", C.c_float), ("max_batch", C.c_int32)]
+                ("vocab_out", C.c_int32 * 8), ("spk_dim", C.c_int32), ("norm_eps", C.c_float), ("max_batch", C.c_int32),
+                ("options", C.c_int32)]
 
 
 class VocConfig(C.Structure):
@@ -46,7 +51,7 @@ class MbdConfig(C.Structure):
                 ("norm_groups", C.c_int32), ("kernel", C.c_int32), ("stride", C.c_int32), ("growth", C.c_float),
                 ("emb_all_layers", C.c_int32), ("codec_dim", C.c_int32), ("num_steps", C.c_int32), ("n_calls", C.c_int32),
                 ("noise_scale", C.c_float), ("clip", C.c_float), ("proc_bands", C.c_int32), ("proc_taps", C.c_int32),
-                ("eq_bands", C.c_int32), ("eq_taps", C.c_int32), ("max_samples", C.c_int32)]
+                ("eq_bands", C.c_int32), ("eq_taps", C.c_int32), ("max_samples", C.c_int32), ("options", C.c_int32)]
 
 
 class SpkConfig(C.Structure):
@@ -157,7 +162,7 @@ SIGNATURES = {
     "mvb_spk_op_test": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                   C.c_void_p]),
 }
-ABI_VERSION = 2
+ABI_VERSION = 3
 
 _lib = None
 

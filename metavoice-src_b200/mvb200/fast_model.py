@@ -9,7 +9,7 @@ from __future__ import annotations
 
 import ctypes as C
 from dataclasses import dataclass
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Union
 
 import torch
 
@@ -159,11 +159,16 @@ class Transformer:
         self.spk_cond_mask[0] = 1
 
     def setup_caches(self, max_batch_size: int, max_seq_length: int, kv_dtype: str = "bf16", max_new: Optional[int] = None,
-                     tensor_core_path: Optional[bool] = None):
+                     tensor_core_path: Union[None, bool, str] = None, unfused_sampler: Optional[bool] = None,
+                     trace: Optional[bool] = None):
         """fast_model.py:136-148.  ``max_batch_size`` counts rows: 2 per utterance (CFG pair).
-        ``tensor_core_path`` (test hook): force the tensor-core rows path on/off for prefill and batched decode."""
+        Test / tool hooks, the engine's ``options`` (include/mvb200.h); any of them given creates a new engine:
+          ``tensor_core_path``: True / "BC" = every engine path, False / "" = CUDA-core kernels only, "B" = tensor-core rows
+            path without the resident decode kernel, "C" = resident decode kernel with CUDA-core prefill;
+          ``unfused_sampler``: the resident kernel leaves the logits to k_sample;
+          ``trace``: the resident kernel records per-phase clocks for mvb_s1_trace_fetch."""
         if (self._handle is not None and self.max_seq_length >= max_seq_length and self.max_batch_size >= max_batch_size
-                and kv_dtype == self.kv_dtype and tensor_core_path is None):
+                and kv_dtype == self.kv_dtype and tensor_core_path is None and unfused_sampler is None and trace is None):
             return
         c = self.config
         if max_batch_size % 2:
@@ -174,9 +179,15 @@ class Transformer:
         self.max_seq_length, self.max_batch_size = c.block_size, max_batch_size
         self.max_utts = max_batch_size // 2
         self.kv_dtype = kv_dtype
+        if tensor_core_path is None or isinstance(tensor_core_path, bool):
+            paths = "" if tensor_core_path is False else "BC"
+        else:
+            paths = str(tensor_core_path)
+        options = ((0 if "B" in paths else _lib.MVB_S1_NO_ROWS_PATH) | (0 if "C" in paths else _lib.MVB_S1_NO_RESIDENT) |
+                   (_lib.MVB_S1_UNFUSED_SAMPLER if unfused_sampler else 0) | (_lib.MVB_S1_TRACE if trace else 0))
         cfg = _lib.S1Config(c.n_layer, c.n_head, c.head_dim, c.dim, c.intermediate_size, c.vocab_size, c.block_size,
                             c.speaker_emb_dim, c.norm_eps, self.max_utts,
-                            _lib.MVB_KV_FP32 if kv_dtype == "fp32" else _lib.MVB_KV_BF16, max_new or c.block_size)
+                            _lib.MVB_KV_FP32 if kv_dtype == "fp32" else _lib.MVB_KV_BF16, max_new or c.block_size, options)
         self._cfg = cfg
         int4 = self.quantisation_mode == "int4"
         kvb = self._lib.mvb_s1_kv_bytes(C.byref(cfg))
@@ -188,26 +199,10 @@ class Transformer:
         offs = (C.c_uint64 * len(self._offsets))(*self._offsets)
         h = C.c_void_p()
         torch.cuda.synchronize(self.device)
-        import os
-        # test hook: True/"BC" = all engine paths, False/"" = CUDA-core kernels only, "B" = tensor-core rows path
-        # without the persistent decode kernel, "C" = persistent decode kernel with CUDA-core prefill
-        saved = {k: os.environ.get(k) for k in ("MVB_PATHB", "MVB_PATHC")}
-        if tensor_core_path is not None:
-            paths = ("BC" if tensor_core_path else "") if isinstance(tensor_core_path, bool) else str(tensor_core_path)
-            os.environ["MVB_PATHB"] = "1" if "B" in paths else "0"
-            os.environ["MVB_PATHC"] = "1" if "C" in paths else "0"
-        try:
-            with torch.cuda.device(self.device):
-                create = self._lib.mvb_s1_create_int4 if int4 else self._lib.mvb_s1_create
-                rc = create(C.byref(cfg), self._arena.data_ptr(), self._arena.numel(), offs, self._kv.data_ptr(),
-                            self._ws.data_ptr(), C.byref(h))
-        finally:
-            if tensor_core_path is not None:
-                for k, v in saved.items():
-                    if v is None:
-                        os.environ.pop(k, None)
-                    else:
-                        os.environ[k] = v
+        with torch.cuda.device(self.device):
+            create = self._lib.mvb_s1_create_int4 if int4 else self._lib.mvb_s1_create
+            rc = create(C.byref(cfg), self._arena.data_ptr(), self._arena.numel(), offs, self._kv.data_ptr(),
+                        self._ws.data_ptr(), C.byref(h))
         _lib.check(rc)
         self._handle = h
         self._spk_key = None

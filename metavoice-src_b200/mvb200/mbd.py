@@ -105,7 +105,10 @@ _RES = ["norm1.weight", "norm1.bias", "conv1.weight", "conv1.bias", "norm2.weigh
 
 
 class MultiBandDiffusionEngine:
-    def __init__(self, checkpoint: dict, settings: MBDSettings, device="cuda", max_seconds: float = 12.0):
+    def __init__(self, checkpoint: dict, settings: MBDSettings, device="cuda", max_seconds: float = 12.0,
+                 tensor_cores: bool = True, band_streams: bool = True):
+        """``tensor_cores=False`` (test hook): every convolution on the fp32 CUDA-core kernels; ``band_streams=False``: the
+        band models back to back on the caller's stream instead of one stream each."""
         self.s, self.device = settings, torch.device(device)
         u = settings.unet
         tensors = []
@@ -144,7 +147,8 @@ class MultiBandDiffusionEngine:
         cfg = _lib.MbdConfig(settings.n_models, u.chin, u.hidden, u.depth, u.res_blocks, u.norm_groups, u.kernel, u.stride,
                              float(u.growth), int(u.emb_all_layers), u.codec_dim, u.num_steps, sched.shape[0],
                              float(settings.schedule.noise_scale), float(settings.schedule.clip), settings.proc_bands,
-                             bank_p.shape[1], settings.eq_bands, bank_e.shape[1], int(max_seconds * settings.sample_rate))
+                             bank_p.shape[1], settings.eq_bands, bank_e.shape[1], int(max_seconds * settings.sample_rate),
+                             (0 if tensor_cores else _lib.MVB_MBD_CUDA_CORES) | (0 if band_streams else _lib.MVB_MBD_ONE_STREAM))
         self.cfg, self._lib = cfg, _lib.load()
         wsb = self._lib.mvb_mbd_workspace_bytes(C.byref(cfg))
         if wsb == 0:

@@ -65,8 +65,9 @@ _LAYER = ["ln_1.weight", "attn.c_attn.weight", "attn.c_proj.weight", "ln_2.weigh
 
 
 class SecondStage:
-    def __init__(self, checkpoint: dict, device="cuda", max_batch: int = 1, tokenizer=None):
-        """``checkpoint`` = the second_stage.pt dict (model / model_args / meta), as ``Model._init_model`` reads it."""
+    def __init__(self, checkpoint: dict, device="cuda", max_batch: int = 1, tokenizer=None, cuda_graph: bool = True):
+        """``checkpoint`` = the second_stage.pt dict (model / model_args / meta), as ``Model._init_model`` reads it.
+        ``cuda_graph=False`` (test hook): launch the forward pass kernel by kernel instead of replaying a captured graph."""
         a = checkpoint["model_args"]
         if a.get("causal", True):
             raise ValueError("second-stage checkpoint must be non-causal")
@@ -99,6 +100,7 @@ class SecondStage:
         cfg.spk_dim = sd["speaker_cond_pos.weight"].shape[1]
         cfg.norm_eps = a.get("rmsnorm_eps") or 1e-5
         cfg.max_batch = max_batch
+        cfg.options = 0 if cuda_graph else _lib.MVB_S2_EAGER
         self.cfg, self._lib = cfg, _lib.load()
         wsb = self._lib.mvb_s2_workspace_bytes(C.byref(cfg))
         if wsb == 0:

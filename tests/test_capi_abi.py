@@ -1,7 +1,10 @@
 """CPU: the C-ABI library loads and exports every symbol include/mvb200.h declares (no compute calls)."""
 import ctypes
+import json
 import os
 import re
+import subprocess
+import sys
 
 import pytest
 
@@ -33,7 +36,7 @@ def test_library_exports_every_declared_symbol():
     for hook in ("mvb_gemm_test", "mvb_mbd_conv_test", "mvb_mbd_op_test", "mvb_s2_attn_test", "mvb_s2_sample_test", "mvb_voc_op_test",
                  "mvb_audio_post_test", "mvb_spk_op_test"):
         assert hook in _lib.SIGNATURES and hasattr(lib, hook), f"test hook {hook} missing"
-    assert lib.mvb_abi_version() == _lib.ABI_VERSION == 2
+    assert lib.mvb_abi_version() == _lib.ABI_VERSION == 3
 
 
 def test_config_validation_without_gpu():
@@ -94,8 +97,6 @@ def test_mbd_config_validation(overrides, want_error):
     partials hold 32 groups; 0 used to divide by zero) and filters longer than k_fir_bank's shared memory can hold
     (227 KB: 19029 taps), and accepts the limits and a 64-band bank.  Each configuration runs in a child process, so that
     a crash of the validation cannot take the test session down with it."""
-    import subprocess
-    import sys
     from mvb200 import _lib
     if not os.path.isfile(_lib.LIB_PATH):
         import __graft_entry__ as g
@@ -108,6 +109,75 @@ def test_mbd_config_validation(overrides, want_error):
         assert int(nbytes) > 0, err
     else:
         assert int(nbytes) == 0 and want_error in err, r.stdout
+
+
+def _engine_configs():
+    """Production configurations (options = 0) of the three engines whose config carries `options`: stage 1 at 8
+    utterances, stage 2 at batch 1, MBD at its default settings and 12 s."""
+    from mvb200 import _lib, synth
+    from mvb200.mbd import MBDSettings, _lowpass_bank, _schedule_table
+    d = synth.FULL
+    s1 = _lib.S1Config(d.n_layer, d.n_head, d.head_dim, d.dim, d.intermediate_size, d.vocab_size, d.block_size,
+                       d.speaker_emb_dim, d.norm_eps, 8, _lib.MVB_KV_BF16, d.block_size)
+    e = synth.S2_FULL
+    s2 = _lib.S2Config()
+    s2.n_layer, s2.n_head, s2.n_embd, s2.hidden = e.n_layer, e.n_head, e.n_embd, e.hidden
+    s2.block_size, s2.n_in, s2.n_out = e.block_size, len(e.vocab_sizes), len(e.target_vocab_sizes)
+    for i, v in enumerate(e.vocab_sizes):
+        s2.vocab_in[i] = v
+    for i, v in enumerate(e.target_vocab_sizes):
+        s2.vocab_out[i] = v
+    s2.spk_dim, s2.norm_eps, s2.max_batch = e.speaker_emb_dim, e.rmsnorm_eps, 1
+    s, u = MBDSettings(), MBDSettings().unet
+    mbd = _lib.MbdConfig(s.n_models, u.chin, u.hidden, u.depth, u.res_blocks, u.norm_groups, u.kernel, u.stride, float(u.growth),
+                         int(u.emb_all_layers), u.codec_dim, u.num_steps, _schedule_table(s.schedule, s.steps()).shape[0],
+                         float(s.schedule.noise_scale), float(s.schedule.clip), s.proc_bands,
+                         _lowpass_bank(s.proc_bands, s.sample_rate).shape[1], s.eq_bands,
+                         _lowpass_bank(s.eq_bands, s.sample_rate).shape[1], 12 * s.sample_rate)
+    return s1, s2, mbd
+
+
+def _workspace_sizes():
+    from mvb200 import _lib
+    lib = _lib.load()
+    s1, s2, mbd = (ctypes.byref(c) for c in _engine_configs())
+    return {"s1_kv": lib.mvb_s1_kv_bytes(s1), "s1": lib.mvb_s1_workspace_bytes(s1), "s1_int4": lib.mvb_s1_int4_workspace_bytes(s1),
+            "s2": lib.mvb_s2_workspace_bytes(s2), "mbd": lib.mvb_mbd_workspace_bytes(mbd)}
+
+
+# environment variables that earlier versions of the library read when an engine was created
+_OLD_SWITCHES = {"MVB_PATHB": "0", "MVB_PATHC": "0", "MVB_PC_FUSED": "0", "MVB_PC_TRACE": "1", "MVB_PDL": "0",
+                 "MVB_S2_NO_GRAPH": "1", "MVB_MBD_NO_TC": "1", "MVB_MBD_STREAMS": "0"}
+
+
+def test_workspace_sizes_ignore_the_process_environment():
+    """Engine paths are chosen by the config's `options` alone: in a process whose environment sets every variable an
+    earlier library read, each workspace size equals the one for options = 0.  The MBD workspace used to follow two of
+    them, so a buffer sized under one environment could be too small for the engine created under another."""
+    want = _workspace_sizes()
+    assert all(v > 0 for v in want.values()), want
+    code = (f"import sys; sys.path[:0] = {[ROOT, os.path.join(ROOT, 'metavoice-src_b200'), os.path.join(ROOT, 'tests')]!r}\n"
+            "import json, test_capi_abi as t; print(json.dumps(t._workspace_sizes()))")
+    r = subprocess.run([sys.executable, "-c", code], env={**os.environ, **_OLD_SWITCHES}, capture_output=True, text=True,
+                       timeout=300)
+    assert r.returncode == 0, r.stderr[-2000:]
+    assert json.loads(r.stdout) == want
+
+
+def test_undefined_option_bits_are_rejected():
+    """`options` comes from outside the library: a bit no engine defines makes the workspace query fail and names the
+    field, before any engine could be created with it."""
+    from mvb200 import _lib
+    lib = _lib.load()
+    s1, s2, mbd = _engine_configs()
+    for cfg, fn, bits in ((s1, lib.mvb_s1_workspace_bytes, (0x10, -2 ** 31)), (s2, lib.mvb_s2_workspace_bytes, (0x2, -2 ** 31)),
+                          (mbd, lib.mvb_mbd_workspace_bytes, (0x4, -2 ** 31))):
+        assert fn(ctypes.byref(cfg)) > 0
+        for bit in bits:
+            cfg.options = bit
+            assert fn(ctypes.byref(cfg)) == 0, (fn.__name__, bit)
+            assert b"options" in lib.mvb_last_error(), (fn.__name__, bit, lib.mvb_last_error())
+        cfg.options = 0
 
 
 def test_missing_library_fails_loudly(monkeypatch):

@@ -35,13 +35,13 @@ def test_restatement_invariants():
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("frames", [12, 40])
-def test_mbd_device_vs_restatement(frames, monkeypatch):
-    monkeypatch.setenv("MVB_MBD_NO_TC", "1")        # the fp32 CUDA-core kernels (the tensor-core lowering has its own test below)
+def test_mbd_device_vs_restatement(frames):
     from mvb200.mbd import MBDSettings, MultiBandDiffusionEngine, ScheduleSettings, UnetSettings
     ck = synth.mbd_checkpoint(SMALL, 0)
     settings = MBDSettings(n_models=2, unet=UnetSettings(hidden=16, depth=2, growth=2.0, kernel=8, stride=4, res_blocks=1, norm_groups=4),
                            schedule=ScheduleSettings(), proc_bands=4, eq_bands=8, step_list=[999, 749, 499, 249, 0])
-    eng = MultiBandDiffusionEngine(ck, settings, device="cuda:0", max_seconds=1.0)
+    # the fp32 CUDA-core kernels (the tensor-core lowering has its own test below)
+    eng = MultiBandDiffusionEngine(ck, settings, device="cuda:0", max_seconds=1.0, tensor_cores=False)
     T = frames * 320
     g = torch.Generator().manual_seed(frames)
     cond = torch.randn(128, frames, generator=g)
@@ -67,12 +67,11 @@ def _round_conv_weights_to_bf16(ck):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("kernel,stride,frames,hidden", [(8, 4, 12, 64), (8, 4, 33, 64), (4, 2, 12, 64), (8, 4, 12, 48)])
-def test_mbd_tensor_core_convs_vs_restatement(kernel, stride, frames, hidden, monkeypatch):
+def test_mbd_tensor_core_convs_vs_restatement(kernel, stride, frames, hidden):
     """Input widths >= 32 channels take the tensor-core path (csrc/mbd_tc.cuh): shifted-GEMM Conv1d (dilation 1
     and 2), the strided encoder convolution and the phase-decomposed ConvTranspose1d.  With conv weights representable in
     bf16 the path is exact to fp32 round-off against the fp32 restatement; with arbitrary fp32 weights the only deviation
     is the bf16 rounding of the taps (reported, bounded)."""
-    monkeypatch.delenv("MVB_MBD_NO_TC", raising=False)
     from mvb200.mbd import MBDSettings, MultiBandDiffusionEngine, ScheduleSettings, UnetSettings
     ucfg = dict(hidden=hidden, depth=2, growth=2.0, kernel=kernel, stride=stride, res_blocks=2, norm_groups=4)
     cfg = M.MBDConfig(n_models=2, unet=M.UnetCfg(**ucfg), proc_bands=4, eq_bands=8, step_list=[999, 666, 333, 0])
@@ -96,11 +95,10 @@ def test_mbd_tensor_core_convs_vs_restatement(kernel, stride, frames, hidden, mo
 
 
 @pytest.mark.gpu
-def test_mbd_default_config_vs_restatement(monkeypatch):
+def test_mbd_default_config_vs_restatement():
     """The shipped UNet (default UnetSettings: hidden 48, growth 4, depth 4, widths 48 / 192 / 768 / 3072) end to end:
     workspace sizing (mbd_layout) and layer wiring at those widths, 2 band models, 2 sampler calls, 12 frames
     (3833 samples), bf16-representable taps."""
-    monkeypatch.delenv("MVB_MBD_NO_TC", raising=False)
     from mvb200.mbd import MBDSettings, MultiBandDiffusionEngine
     steps = [999, 499, 0]
     cfg = M.MBDConfig(n_models=2, step_list=steps)

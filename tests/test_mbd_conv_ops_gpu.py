@@ -196,7 +196,7 @@ def test_channel_padding_and_partial_warps(cin, groups, cout):
     _case(f"transposed {cin}->{cout} (k4 s2)", 2, cin, cout, 4, 2, 1, 1, 150, groups=groups, seed=cin + cout + 2)
 
 
-# ---- CUDA-core kernels the engine runs for narrow inputs (and everywhere under MVB_MBD_NO_TC) -------------------------
+# ---- CUDA-core kernels the engine runs for narrow inputs (and everywhere under MVB_MBD_CUDA_CORES) --------------------
 @pytest.mark.parametrize("tin", [1, 7, 145, 3833, 144000])
 def test_level0_encoder_conv_cuda_cores(tin):
     """The first encoder convolution of every UNet call, Cin = 1 -> 48, k8 s4 (k_mbd_conv<8, 4, 1>, always on the CUDA

@@ -529,10 +529,11 @@ def test_randn_distribution():
 
 
 # ---- engine-level identities ----------------------------------------------------------------------------------------
-def _engine(settings, oracle_cfg, seed=0):
+def _engine(settings, oracle_cfg, seed=0, band_streams=True):
     from mvb200 import synth
     from mvb200.mbd import MultiBandDiffusionEngine
-    return MultiBandDiffusionEngine(synth.mbd_checkpoint(oracle_cfg, seed), settings, device="cuda:0", max_seconds=1.0)
+    return MultiBandDiffusionEngine(synth.mbd_checkpoint(oracle_cfg, seed), settings, device="cuda:0", max_seconds=1.0,
+                                    band_streams=band_streams)
 
 
 def _small(n_models=4, proc_bands=4, eq_bands=8):
@@ -552,11 +553,9 @@ def _inputs(frames, T, seed):
     return cond, wav_e, g
 
 
-def test_seeded_noise_equals_supplied_noise(monkeypatch):
+def test_seeded_noise_equals_supplied_noise():
     """tokens_to_wav(seed=s) draws row 0 of band model m from Philox stream m 1024 and row i + 1 from m 1024 + i + 1:
     supplying those rows (from the randn hook) as `noise` gives the same waveform bit for bit."""
-    monkeypatch.delenv("MVB_MBD_STREAMS", raising=False)
-    monkeypatch.delenv("MVB_MBD_NO_TC", raising=False)
     settings, ocfg = _small()
     eng = _engine(settings, ocfg, 3)
     frames, T, seed = 12, 12 * 320 - 7, 2 ** 32 + 99
@@ -571,13 +570,12 @@ def test_seeded_noise_equals_supplied_noise(monkeypatch):
 
 
 @pytest.mark.parametrize("config", ["small", "default"])
-def test_one_stream_equals_four_streams(config, monkeypatch):
-    """MVB_MBD_STREAMS=0 (read at create time) runs the band models one after another on the caller's stream and
-    accumulates their outputs in place with k_band_mix; the default runs them on four streams and adds the blocks with
-    k_sum_blocks afterwards.  Both add in model order, so the waveforms are bitwise equal."""
+def test_one_stream_equals_four_streams(config):
+    """band_streams=False (MVB_MBD_ONE_STREAM, fixed at create time) runs the band models one after another on the
+    caller's stream and accumulates their outputs in place with k_band_mix; the default runs them on four streams and adds
+    the blocks with k_sum_blocks afterwards.  Both add in model order, so the waveforms are bitwise equal."""
     from mvb200.mbd import MBDSettings
     from oracle import mbd_port as M
-    monkeypatch.delenv("MVB_MBD_NO_TC", raising=False)
     if config == "small":
         settings, ocfg = _small()
     else:
@@ -585,9 +583,7 @@ def test_one_stream_equals_four_streams(config, monkeypatch):
         settings, ocfg = MBDSettings(n_models=4, step_list=steps), M.MBDConfig(n_models=4, step_list=steps)
     frames, T = 12, 12 * 320 - 7
     cond, wav_e, g = _inputs(frames, T, 2)
-    monkeypatch.setenv("MVB_MBD_STREAMS", "0")
-    one = _engine(settings, ocfg, 4)
-    monkeypatch.delenv("MVB_MBD_STREAMS")
+    one = _engine(settings, ocfg, 4, band_streams=False)
     four = _engine(settings, ocfg, 4)
     noise = torch.randn(4, one.n_calls, T, generator=g)
     a = one.tokens_to_wav(cond, wav_e, noise=noise).cpu()
@@ -597,16 +593,14 @@ def test_one_stream_equals_four_streams(config, monkeypatch):
     assert torch.isfinite(a).all() and torch.equal(a, b)
 
 
-def test_sixty_four_bands_end_to_end(monkeypatch):
+def test_sixty_four_bands_end_to_end():
     """64 processor and re-EQ bands (5921 taps, more than 64 KB of FIR shared memory) run and match the restatement."""
     from oracle import mbd_port as M
-    monkeypatch.setenv("MVB_MBD_NO_TC", "1")
-    monkeypatch.delenv("MVB_MBD_STREAMS", raising=False)
     settings, ocfg = _small(n_models=2, proc_bands=64, eq_bands=64)
     from mvb200 import synth
     ck = synth.mbd_checkpoint(ocfg, 5)
     from mvb200.mbd import MultiBandDiffusionEngine
-    eng = MultiBandDiffusionEngine(ck, settings, device="cuda:0", max_seconds=1.0)
+    eng = MultiBandDiffusionEngine(ck, settings, device="cuda:0", max_seconds=1.0, tensor_cores=False)
     assert eng.cfg.proc_taps == eng.cfg.eq_taps == 5921
     frames, T = 12, 12 * 320
     cond, wav_e, g = _inputs(frames, T, 6)

@@ -44,7 +44,6 @@ sum of two, so split-K order cannot change it, and mvb_s1_step_logits returns bi
 stage-1 samplers consume (asserted: two calls agree).  The fed token selects the distribution; forced tokens set the
 sequence.  Which body and sampler ran is taken from the launch-count delta."""
 import ctypes as C
-import os
 
 import numpy as np
 import pytest
@@ -289,16 +288,8 @@ class Probe:
               "transformer.h.0.mlp.c_proj.weight": torch.zeros(D, F)}
         sd = {k: v.to(torch.bfloat16) for k, v in sd.items()}
         cfg = ModelArgs(block_size=BLOCK, vocab_size=V, n_layer=1, n_head=H, dim=D, intermediate_size=F)
-        saved = os.environ.get("MVB_PC_FUSED")
-        os.environ["MVB_PC_FUSED"] = "1" if fused else "0"           # read once in mvb_s1_create
-        try:
-            self.m = Transformer.from_state_dict(sd, cfg, device="cuda:0")
-            self.m.setup_caches(2 * utts, BLOCK)
-        finally:
-            if saved is None:
-                os.environ.pop("MVB_PC_FUSED", None)
-            else:
-                os.environ["MVB_PC_FUSED"] = saved
+        self.m = Transformer.from_state_dict(sd, cfg, device="cuda:0")
+        self.m.setup_caches(2 * utts, BLOCK, unfused_sampler=not fused)
         self.fused, self.utts = fused, utts
         self.lib, self.h = self.m._lib, self.m.handle
         self._keep = []

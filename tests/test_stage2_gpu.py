@@ -64,7 +64,7 @@ def test_stage2_batch_and_pipeline_shapes():
     assert torch.equal(out[0][:2], codes[0][0][:, :out[0].shape[1]])
 
 
-def test_stage2_graph_replay_equals_eager_launches(monkeypatch):
+def test_stage2_graph_replay_equals_eager_launches():
     """The forward pass is replayed as one CUDA graph (sampling parameters live in device memory): same seed -> the same
     tokens as the eager launch sequence, for two different seeds / temperatures through the same captured graph."""
     from mvb200.second_stage import SecondStage
@@ -72,9 +72,7 @@ def test_stage2_graph_replay_equals_eager_launches(monkeypatch):
     ck = synth.stage2_checkpoint(d, 1)
     text, cb0, cb1 = synth.synthetic_stage2_input(d, 50)
     graph = SecondStage(ck, device="cuda:0")
-    monkeypatch.setenv("MVB_S2_NO_GRAPH", "1")
-    eager = SecondStage(ck, device="cuda:0")
-    monkeypatch.delenv("MVB_S2_NO_GRAPH")
+    eager = SecondStage(ck, device="cuda:0", cuda_graph=False)
     idx = graph.build_input(text, [cb0, cb1])[None]
     spk = synth.synthetic_speaker(seed=2)[None]
     for seed, temp in ((7, 1.0), (8, 0.7), (7, 1.0)):

@@ -71,17 +71,16 @@ def _mbd_cfg(max_seconds):
                           float(s.schedule.clip), s.proc_bands, taps_p, s.eq_bands, taps_e, int(max_seconds * s.sample_rate))
 
 
-@pytest.mark.parametrize("env,max_seconds,want", [
-    ({}, 30.0, 3849490688), ({}, 12.0, 2317570304),
-    ({"MVB_MBD_NO_TC": "1"}, 30.0, 2560819456),
-    ({"MVB_MBD_STREAMS": "0"}, 30.0, 1928876288),
-], ids=["default-30s", "default-12s", "no_tc", "one_stream"])
-def test_mbd_workspace_bytes(lib, monkeypatch, env, max_seconds, want):
-    monkeypatch.delenv("MVB_MBD_NO_TC", raising=False)
-    monkeypatch.delenv("MVB_MBD_STREAMS", raising=False)
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
-    assert lib.mvb_mbd_workspace_bytes(C.byref(_mbd_cfg(max_seconds))) == want
+@pytest.mark.parametrize("options,max_seconds,want", [
+    (0, 30.0, 3849490688), (0, 12.0, 2317570304),
+    (_lib.MVB_MBD_CUDA_CORES, 30.0, 2560819456),
+    (_lib.MVB_MBD_ONE_STREAM, 30.0, 1928876288),
+    (_lib.MVB_MBD_CUDA_CORES | _lib.MVB_MBD_ONE_STREAM, 30.0, 640205056),
+], ids=["default-30s", "default-12s", "no_tc", "one_stream", "no_tc-one_stream"])
+def test_mbd_workspace_bytes(lib, options, max_seconds, want):
+    cfg = _mbd_cfg(max_seconds)
+    cfg.options = options
+    assert lib.mvb_mbd_workspace_bytes(C.byref(cfg)) == want
 
 
 @pytest.mark.parametrize("max_seconds,want", [(180.0, 3932928), (30.0, 1532928)])

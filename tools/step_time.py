@@ -1,7 +1,7 @@
 """Decode-step time (CUDA events) for several engine configurations in one process.
-Usage: python tools/step_time.py "A1:1,B:8,C:1,C:1:MVB_PC_FUSED=0,C:8" [context_len]
-  A1 = CUDA-core path with PDL, A0 = without, B = tensor-core rows path (from 2 utterances up), C = persistent fused
-  kernel; second field = utterances; optional third field = '+'-separated environment switches read by mvb_s1_create."""
+Usage: python tools/step_time.py "A:1,B:8,C:1,C:1:unfused,C:8" [context_len]
+  A = CUDA-core path, B = tensor-core rows path (from 2 utterances up), C = persistent fused kernel; second field =
+  utterances; optional third field `unfused`: the persistent kernel leaves the logits to k_sample."""
 import ctypes as C
 import json
 import os
@@ -16,7 +16,7 @@ import bench  # noqa: E402
 from mvb200 import _lib, synth  # noqa: E402
 from mvb200.fast_model import ModelArgs, Transformer, pack_arena  # noqa: E402
 
-spec = sys.argv[1] if len(sys.argv) > 1 else "A1:1,A0:1,B:8"
+spec = sys.argv[1] if len(sys.argv) > 1 else "A:1,B:8"
 L_mid = int(sys.argv[2]) if len(sys.argv) > 2 else 423
 dev = torch.device("cuda:0")
 torch.cuda.set_device(dev)
@@ -29,14 +29,11 @@ res = []
 for item in spec.split(","):
     parts = item.split(":")
     kind, n = parts[0], int(parts[1])
-    extra = dict(kv.split("=") for kv in parts[2].split("+")) if len(parts) > 2 and parts[2] else {}
-    os.environ.pop("MVB_PC_FUSED", None)
-    os.environ.update(extra)
-    os.environ["MVB_PDL"] = "0" if kind.endswith("0") else "1"
-    os.environ["MVB_PATHB"] = "1" if kind[0] in "BC" else "0"
-    os.environ["MVB_PATHC"] = "1" if kind[0] == "C" else "0"
+    if kind not in ("A", "B", "C") or parts[2:] not in ([], ["unfused"]):
+        raise SystemExit(f"bad configuration {item!r}: expected A|B|C:<utterances>[:unfused]")
     m = Transformer(cfg, arena, offsets, device=dev)
-    m.setup_caches(2 * n, cfg.block_size, kv_dtype="bf16")
+    m.setup_caches(2 * n, cfg.block_size, kv_dtype="bf16", tensor_core_path={"A": "", "B": "B", "C": "BC"}[kind],
+                   unfused_sampler=parts[2:] == ["unfused"])
     lib, h, st = m._lib, m.handle, m._stream()
     for u in range(n):
         sp = _lib.Sampling(3.0, 1.0, 0.95, 0, 9999, 5 + u)

@@ -5,7 +5,6 @@ import ctypes as C
 import os
 import sys
 
-os.environ["MVB_PC_TRACE"] = "1"
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "metavoice-src_b200"))
 import numpy as np  # noqa: E402
@@ -17,15 +16,12 @@ from mvb200.fast_model import ModelArgs, Transformer, pack_arena  # noqa: E402
 
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 1
 L_mid = int(sys.argv[2]) if len(sys.argv) > 2 else 423
-for kv in (sys.argv[3].split("+") if len(sys.argv) > 3 and sys.argv[3] else []):   # e.g. MVB_PDL=0
-    k, v = kv.split("=")
-    os.environ[k] = v
 dev = torch.device("cuda:0"); torch.cuda.set_device(dev)
 d = synth.FULL
 cfg = ModelArgs.from_name("metavoice-1B")
 arena, offsets = pack_arena(synth.stage1_state_dict(d, 0), d.n_layer)
 m = Transformer(cfg, arena.to(dev), offsets, device=dev)
-m.setup_caches(2 * n, cfg.block_size, kv_dtype="bf16")
+m.setup_caches(2 * n, cfg.block_size, kv_dtype="bf16", trace=True)
 lib, h, st = m._lib, m.handle, m._stream()
 for u in range(n):
     sp = _lib.Sampling(3.0, 1.0, 0.95, 0, 9999, 5 + u)
