@@ -177,6 +177,20 @@ size_t mvb_s1_int4_workspace_bytes(const mvb_s1_config* cfg);
 int mvb_s1_create_int4(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
                        void* d_kv, void* d_workspace, mvb_s1** out);
 
+/* Weight-only int8 engine (quantisation_mode="int8", fast_inference_utils.py:283-296).  Same offset table as mvb_s1_create,
+ * but the entry of EVERY Linear weight -- wqkv, wo, w1, w3, w2 of every layer, speaker_cond_pos and lm_head -- points at an
+ * INT8 MATRIX [M, K]: int8 q [M][K] row-major, then at the next 256-byte boundary bf16 [M] row scales s (produced only by
+ * mvb200/quantize.py:pack_int8_matrix; the quantiser is the reference's dynamically_quantize_per_channel(w.float(), -128,
+ * 127) with the scales cast to bf16).  Every kernel computes y_j = s_j * sum_k x_k q_jk: fp32 sums over the exact integer
+ * weights, the scale applied once per output after the whole sum (and after any split-K reduction).  Embeddings and norms
+ * are bf16.  Decode always runs the per-layer CUDA-core path through the int8 GEMV (never the persistent kernel, never the
+ * tensor-core rows path); prefill runs the tensor-core GEMM over one layer's q at a time, widened to bf16 into the scratch
+ * the int4 engine uses, and lm_head's q widened once at create: mvb_s1_int8_workspace_bytes = the int4 workspace + vocab x
+ * dim bf16.  Every other mvb_s1_* call accepts the handle. */
+size_t mvb_s1_int8_workspace_bytes(const mvb_s1_config* cfg);
+int mvb_s1_create_int8(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
+                       void* d_kv, void* d_workspace, mvb_s1** out);
+
 /* Kernel launches issued by this handle since creation (bench.py "gpu_launches"). */
 uint64_t mvb_s1_launch_count(const mvb_s1* h);
 
@@ -246,6 +260,23 @@ int mvb_w4_gemv_test(int32_t epi, const void* d_W, const void* d_W3, int32_t M, 
                      const int32_t* d_slot_map, const int32_t* d_pos, int32_t H, int32_t S_max, int32_t D, int32_t kv_fp32,
                      void* stream);
 int mvb_w4_dequant_test(const void* d_W, int32_t M, int32_t K, void* d_out, void* stream);
+/* Test hooks for the int8 kernels (not part of the drop-in surface):
+ *   mvb_w8_gemv_test  : the int8 GEMV (csrc/gemv_w8.cuh k_gemv_w8) as the int8 engine's decode launches it; the arguments
+ *                       of mvb_w4_gemv_test with d_W / d_W3 int8 matrices [M, K].
+ *   mvb_w8_gemm_test  : mvb_gemm_test's operator with the row-scale epilogue of the int8 engine: d_W (d_W3) bf16 [M, K]
+ *                       holding q, d_scale (d_scale3 for SwiGLU) bf16 [M]; out = epilogue(s_j * (f(x) . W_j)).
+ *   mvb_w8_widen_test : k_w8_widen of one int8 matrix into d_out bf16 row-major [M, K] (q exactly).
+ * All three synchronise `stream`. */
+int mvb_w8_gemv_test(int32_t epi, const void* d_W, const void* d_W3, int32_t M, int32_t K, const float* d_x, int32_t ldx,
+                     int32_t n_utts, const void* d_gain, float eps, float* d_out, int32_t ldo, void* d_kcache, void* d_vcache,
+                     const int32_t* d_slot_map, const int32_t* d_pos, int32_t H, int32_t S_max, int32_t D, int32_t kv_fp32,
+                     void* stream);
+int mvb_w8_gemm_test(int32_t epi, const void* d_W, const void* d_W3, const void* d_scale, const void* d_scale3, int32_t M,
+                     int32_t K, const float* d_x, int32_t ldx, int32_t R, const void* d_gain, float eps, int32_t split_lo,
+                     int32_t ksplit_override, float* d_out, int32_t ldo, void* d_kcache, void* d_vcache,
+                     const int32_t* d_row_cache, const int32_t* d_row_pos, int32_t H, int32_t S_max, int32_t D,
+                     int32_t kv_fp32, void* stream);
+int mvb_w8_widen_test(const void* d_W, int32_t M, int32_t K, void* d_out, void* stream);
 int mvb_mbd_conv_test(int32_t kind, const float* d_x, int32_t Cin, int32_t Tin, const float* d_w, int32_t Cout, int32_t K,
                       int32_t stride, int32_t dil, int32_t pad, const float* d_gn_stats, const float* d_gn_w,
                       const float* d_gn_b, int32_t groups, const float* d_bias, const float* d_emb, const float* d_resid,

@@ -83,8 +83,7 @@ __device__ __forceinline__ void l2_prefetch(const void* p, size_t bytes) {
 // Memory pipeline: the weights do not depend on the previous kernel, so before griddepcontrol.wait every warp asks L2 for
 // all the rows (and their scale / zero pairs) it will stream, one bulk prefetch per item and lane: the whole matrix is in
 // flight while the previous kernel drains and the activations are staged, and the main loop then reads L2.
-// The prologue and the epilogues are k_gemv's (stage1_kernels.cuh) except for the shared-memory permutation: a fix to
-// one belongs in the other.
+// The prologue and the epilogues are k_gemv's (gemv_prologue / gemv_epilogue, stage1_kernels.cuh) over the w4_perm layout.
 template <int EPI>
 __global__ void __launch_bounds__(256, 2) k_gemv_w4(GemvP p, S1State st) {
   extern __shared__ float xs[];  // [2][K] in the w4_perm layout
@@ -117,45 +116,7 @@ __global__ void __launch_bounds__(256, 2) k_gemv_w4(GemvP p, S1State st) {
   pdl_wait();  // activations written by the previous kernel are now visible
 
   const int u = st.slot_map[blockIdx.y];
-  const int r0 = 2 * u;
-  {
-    // == k_gemv's prologue (stage1_kernels.cuh) with w4_perm in place of xs_perm
-    const float* x0 = p.x + (size_t)r0 * p.ldx;
-    const float* x1 = x0 + p.ldx;
-    float s0 = 0.f, s1 = 0.f;
-    for (int k = tid; k < K; k += 256) {
-      const float a = x0[k], b = x1[k];
-      s0 = fmaf(a, a, s0);
-      s1 = fmaf(b, b, s1);
-      const int pk = w4_perm(k, K);
-      xs[pk] = a;
-      xs[K + pk] = b;
-    }
-    if (p.gain != nullptr) {
-      s0 = warp_sum(s0);
-      s1 = warp_sum(s1);
-      if (lane == 0) {
-        red[warp] = s0;
-        red[8 + warp] = s1;
-      }
-      __syncthreads();
-      float t0 = 0.f, t1 = 0.f;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        t0 += red[i];
-        t1 += red[8 + i];
-      }
-      const float rs0 = rsqrtf(t0 / (float)K + p.eps);
-      const float rs1 = rsqrtf(t1 / (float)K + p.eps);
-      for (int k = tid; k < K; k += 256) {
-        const float g = bf16_to_f32(p.gain[k]);
-        const int pk = w4_perm(k, K);
-        xs[pk] = (xs[pk] * rs0) * g;
-        xs[K + pk] = (xs[K + pk] * rs1) * g;
-      }
-    }
-    __syncthreads();
-  }
+  gemv_prologue(p, 2 * u, xs, red, [K](int k) { return w4_perm(k, K); });
 
   const int KF = K >> 9;               // full 512-wide tiles
   const bool tail = (K & 511) != 0;    // one trailing 256-wide tile
@@ -205,48 +166,7 @@ __global__ void __launch_bounds__(256, 2) k_gemv_w4(GemvP p, S1State st) {
     a01 = warp_sum(a01);
     a10 = warp_sum(a10);
     a11 = warp_sum(a11);
-    if (lane == 0) {   // == k_gemv's epilogues (stage1_kernels.cuh)
-      float* o0 = p.out + (size_t)r0 * p.ldo;
-      float* o1 = o0 + p.ldo;
-      if (EPI == EPI_SWIGLU) {
-        o0[item] = (a00 / (1.f + expf(-a00))) * a10;
-        o1[item] = (a01 / (1.f + expf(-a01))) * a11;
-      } else {
-        const int c = 2 * item;
-        if (EPI == EPI_RESID) {
-          o0[c] += a00;
-          o1[c] += a01;
-          o0[c + 1] += a10;
-          o1[c + 1] += a11;
-        } else {
-          o0[c] = a00;
-          o1[c] = a01;
-          o0[c + 1] = a10;
-          o1[c + 1] = a11;
-        }
-        if (EPI == EPI_QKV && c >= p.D) {
-          // scatter k / v of the current token into the cache at input_pos (fast_model.py:111-112), as k_gemv does
-          const int which = (c - p.D) / p.D;  // 0 = k, 1 = v
-          const int cc = (c - p.D) - which * p.D;
-          const int head = cc >> 7, d = cc & 127;
-          const int pos = st.pos[u];
-          const size_t e0 = (((size_t)r0 * p.H + head) * p.S_max + pos) * 128 + d;
-          const size_t e1 = e0 + (size_t)p.H * p.S_max * 128;
-          void* base = which ? p.vcache : p.kcache;
-          if (p.kv_fp32) {
-            float* kvp = reinterpret_cast<float*>(base);
-            kvp[e0] = a00;
-            kvp[e0 + 1] = a10;
-            kvp[e1] = a01;
-            kvp[e1 + 1] = a11;
-          } else {
-            __nv_bfloat16* kvp = reinterpret_cast<__nv_bfloat16*>(base);
-            *reinterpret_cast<__nv_bfloat162*>(kvp + e0) = __floats2bfloat162_rn(a00, a10);
-            *reinterpret_cast<__nv_bfloat162*>(kvp + e1) = __floats2bfloat162_rn(a01, a11);
-          }
-        }
-      }
-    }
+    if (lane == 0) gemv_epilogue<EPI>(p, st, u, item, a00, a01, a10, a11);
   }
 }
 

@@ -7,29 +7,36 @@ using namespace mvb;
 
 namespace mvb {
 
-template <int EPI, int NC>
+template <int EPI, int NC, bool SCALED>
 static cudaError_t launch_tc_gemm_nc(cudaStream_t s, const CUtensorMap& tA, const CUtensorMap& tA3, const CUtensorMap& tB,
                                      const GemmP& p, const GemmPlan& g) {
   static PerDeviceOnce attr_set;
   if (attr_set.pending()) {
-    cudaError_t e = cudaFuncSetAttribute(k_tc_gemm<EPI, NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(k_tc_gemm<EPI, NC, SCALED>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) return e;
     attr_set.mark();
   }
-  k_tc_gemm<EPI, NC><<<dim3(g.tiles, g.ksplit), GEMM_THREADS, g.smem_bytes, s>>>(tA, tA3, tB, p);
+  k_tc_gemm<EPI, NC, SCALED><<<dim3(g.tiles, g.ksplit), GEMM_THREADS, g.smem_bytes, s>>>(tA, tA3, tB, p);
   return cudaGetLastError();
 }
 
 // The accumulator size is a template parameter (registers): the smallest of 16 / 32 / 64 / 128 columns that holds Rpad.
+template <int EPI, bool SCALED>
+static cudaError_t launch_tc_gemm_sc(cudaStream_t s, const CUtensorMap& tA, const CUtensorMap& tA3, const CUtensorMap& tB,
+                                     const GemmP& p, const GemmPlan& g) {
+  if (p.Rpad <= 16) return launch_tc_gemm_nc<EPI, 2, SCALED>(s, tA, tA3, tB, p, g);
+  if (p.Rpad <= 32) return launch_tc_gemm_nc<EPI, 4, SCALED>(s, tA, tA3, tB, p, g);
+  if (p.Rpad <= 64) return launch_tc_gemm_nc<EPI, 8, SCALED>(s, tA, tA3, tB, p, g);
+  return launch_tc_gemm_nc<EPI, 16, SCALED>(s, tA, tA3, tB, p, g);
+}
+
 template <int EPI>
 static cudaError_t launch_tc_gemm(cudaStream_t s, const CUtensorMap& tA, const CUtensorMap& tA3, const CUtensorMap& tB,
                                   GemmP p, const GemmPlan& g) {
   p.ksplit = g.ksplit;
   p.stages = g.stages;
-  if (p.Rpad <= 16) return launch_tc_gemm_nc<EPI, 2>(s, tA, tA3, tB, p, g);
-  if (p.Rpad <= 32) return launch_tc_gemm_nc<EPI, 4>(s, tA, tA3, tB, p, g);
-  if (p.Rpad <= 64) return launch_tc_gemm_nc<EPI, 8>(s, tA, tA3, tB, p, g);
-  return launch_tc_gemm_nc<EPI, 16>(s, tA, tA3, tB, p, g);
+  if (p.scale != nullptr) return launch_tc_gemm_sc<EPI, true>(s, tA, tA3, tB, p, g);
+  return launch_tc_gemm_sc<EPI, false>(s, tA, tA3, tB, p, g);
 }
 
 cudaError_t tc_gemm(cudaStream_t s, const TcGemm& a) {
@@ -43,6 +50,7 @@ cudaError_t tc_gemm(cudaStream_t s, const TcGemm& a) {
   p.scratch = a.scratch; p.tickets = a.tickets; p.out = a.out; p.ldo = a.ldo;
   p.kcache = a.kcache; p.vcache = a.vcache; p.row_cache = a.row_cache; p.row_pos = a.row_pos;
   p.H = a.H; p.S_max = a.S_max; p.D = a.D; p.kv_fp32 = a.kv_fp32 ? 1 : 0;
+  p.scale = a.scale; p.scale3 = a.scale3;
   const GemmPlan g = plan_gemm(a.M, a.K, NB, a.epi == G_SWIGLU, a.n_sm, a.ksplit);
   const CUtensorMap& tA3 = a.epi == G_SWIGLU ? *a.tmW3 : *a.tmW;
   switch (a.epi) {
@@ -112,10 +120,12 @@ extern "C" int mvb_linear(const void* d_W, int32_t M, int32_t K, const float* d_
   return run_gemm(a, d_W, nullptr, (cudaStream_t)stream);
 }
 
-extern "C" int mvb_gemm_test(int32_t epi, const void* d_W, const void* d_W3, int32_t M, int32_t K, const float* d_x, int32_t ldx,
-                             int32_t R, const void* d_gain, float eps, int32_t split_lo, int32_t ksplit_override, float* d_out,
-                             int32_t ldo, void* d_kcache, void* d_vcache, const int32_t* d_row_cache, const int32_t* d_row_pos,
-                             int32_t H, int32_t S_max, int32_t D, int32_t kv_fp32, void* stream) {
+namespace {
+
+int gemm_test(int32_t epi, const void* d_W, const void* d_W3, const void* d_scale, const void* d_scale3, int32_t M, int32_t K,
+              const float* d_x, int32_t ldx, int32_t R, const void* d_gain, float eps, int32_t split_lo, int32_t ksplit_override,
+              float* d_out, int32_t ldo, void* d_kcache, void* d_vcache, const int32_t* d_row_cache, const int32_t* d_row_pos,
+              int32_t H, int32_t S_max, int32_t D, int32_t kv_fp32, void* stream) {
   if (!d_W || !d_x || !d_out) return mvb::set_error(MVB_ERR_ARG, "null argument");
   if (epi < G_STORE || epi > G_QKV) return mvb::set_error(MVB_ERR_ARG, "mvb_gemm_test: epilogue %d", epi);
   if (K % 64 || R < 1 || R > 128 || M < 1 || ldo < M || ldx < K)
@@ -134,5 +144,26 @@ extern "C" int mvb_gemm_test(int32_t epi, const void* d_W, const void* d_W3, int
   a.out = d_out; a.ldo = ldo;
   a.kcache = d_kcache; a.vcache = d_vcache; a.row_cache = d_row_cache; a.row_pos = d_row_pos;
   a.H = H; a.S_max = S_max; a.D = D; a.kv_fp32 = kv_fp32;
+  a.scale = reinterpret_cast<const __nv_bfloat16*>(d_scale); a.scale3 = reinterpret_cast<const __nv_bfloat16*>(d_scale3);
   return run_gemm(a, d_W, d_W3, (cudaStream_t)stream);
+}
+
+}  // namespace
+
+extern "C" int mvb_gemm_test(int32_t epi, const void* d_W, const void* d_W3, int32_t M, int32_t K, const float* d_x, int32_t ldx,
+                             int32_t R, const void* d_gain, float eps, int32_t split_lo, int32_t ksplit_override, float* d_out,
+                             int32_t ldo, void* d_kcache, void* d_vcache, const int32_t* d_row_cache, const int32_t* d_row_pos,
+                             int32_t H, int32_t S_max, int32_t D, int32_t kv_fp32, void* stream) {
+  return gemm_test(epi, d_W, d_W3, nullptr, nullptr, M, K, d_x, ldx, R, d_gain, eps, split_lo, ksplit_override, d_out, ldo,
+                   d_kcache, d_vcache, d_row_cache, d_row_pos, H, S_max, D, kv_fp32, stream);
+}
+
+extern "C" int mvb_w8_gemm_test(int32_t epi, const void* d_W, const void* d_W3, const void* d_scale, const void* d_scale3,
+                                int32_t M, int32_t K, const float* d_x, int32_t ldx, int32_t R, const void* d_gain, float eps,
+                                int32_t split_lo, int32_t ksplit_override, float* d_out, int32_t ldo, void* d_kcache,
+                                void* d_vcache, const int32_t* d_row_cache, const int32_t* d_row_pos, int32_t H, int32_t S_max,
+                                int32_t D, int32_t kv_fp32, void* stream) {
+  if (!d_scale || (epi == G_SWIGLU && !d_scale3)) return mvb::set_error(MVB_ERR_ARG, "mvb_w8_gemm_test: null row scales");
+  return gemm_test(epi, d_W, d_W3, d_scale, d_scale3, M, K, d_x, ldx, R, d_gain, eps, split_lo, ksplit_override, d_out, ldo,
+                   d_kcache, d_vcache, d_row_cache, d_row_pos, H, S_max, D, kv_fp32, stream);
 }

@@ -11,6 +11,7 @@
 #include "tc_gemm_host.cuh"
 #include "decode_persistent.cuh"
 #include "gemv_w4.cuh"
+#include "gemv_w8.cuh"
 
 using namespace mvb;
 
@@ -23,18 +24,31 @@ struct WsLayout {
   // path C (persistent decode kernel)
   size_t c_x, c_qkv, c_gu, c_part_o, c_part_ml, c_bar, c_trace, c_stat, c_samp_part, c_samp_best;
   size_t total;
-  // an int4 engine's workspace continues with the dequantised-layer scratch
-  size_t w4_scratch, total_int4;
+  // an int4 or int8 engine's workspace continues with the one-layer bf16 weight scratch; an int8 engine's then with
+  // lm_head's widened q
+  size_t layer_scratch, total_int4, w8_head, total_int8;
 };
 
 constexpr int RB_MAX = 128;        // rows per tensor-core pass: 64-token prefill chunk x 2 CFG rows, or 64 utterances
 constexpr int PREFILL_CHUNK = 64;
 constexpr int GEN_BURST = 32;       // decode steps between two host polls of the done flags in mvb_s1_generate
 
-// elements of one layer's dequantised weights: wqkv, wo, w1, w3, w2
-static size_t w4_layer_elems(const mvb_s1_config& c) {
+// elements of one layer's bf16 weight scratch: wqkv, wo, w1, w3, w2
+static size_t layer_scratch_elems(const mvb_s1_config& c) {
   const size_t D = c.dim, F = c.intermediate;
   return 4 * D * D + 3 * D * F;
+}
+
+// Storage format of the Linear weights of an engine's arena (include/mvb200.h): bf16 (mvb_s1_create), int4 packed
+// matrices for the five layer matrices (mvb_s1_create_int4), int8 matrices for every Linear (mvb_s1_create_int8).
+enum class WFmt { BF16, INT4, INT8 };
+
+struct Mk { int M, K; };
+// [M, K] of layer tensor t (1 wqkv, 2 wo, 4 w1, 5 w3, 6 w2; {0, 0} for the norms)
+static Mk layer_mk(const mvb_s1_config& c, int t) {
+  const int D = c.dim, F = c.intermediate;
+  const Mk mk[7] = {{0, 0}, {3 * D, D}, {D, D}, {0, 0}, {F, D}, {F, D}, {D, F}};
+  return mk[t];
 }
 
 static WsLayout make_layout(const mvb_s1_config& c) {
@@ -99,8 +113,10 @@ static WsLayout make_layout(const mvb_s1_config& c) {
   L.c_samp_part = ws.take((size_t)(PC_RPAD / 2) * 256 * 4);
   L.c_samp_best = ws.take((size_t)2 * (PC_RPAD / 2) * 8);
   L.total = ws.end;
-  L.w4_scratch = ws.take(w4_layer_elems(c) * 2);
+  L.layer_scratch = ws.take(layer_scratch_elems(c) * 2);
   L.total_int4 = ws.end;
+  L.w8_head = ws.take((size_t)c.vocab * c.dim * 2);
+  L.total_int8 = ws.end;
   return L;
 }
 
@@ -133,23 +149,36 @@ struct mvb_s1 {
   PcMat pm[5];
   std::vector<int> h_topk;                            // top_k of every utterance slot as installed by mvb_s1_begin
   size_t layer_stride_elems = 0;
-  // int4 engine (mvb_s1_create_int4): wqkv / wo / w1 / w3 / w2 are packed matrices; path A streams them through
-  // k_gemv_w4, path B dequantises one layer at a time into w4_scratch (bf16 [wqkv | wo | w1 | w3 | w2]).
-  bool int4 = false;
-  __nv_bfloat16* w4_scratch = nullptr;
+  // int4 engine: wqkv / wo / w1 / w3 / w2 are packed matrices; path A streams them through k_gemv_w4, path B dequantises
+  // one layer at a time into layer_scratch (bf16 [wqkv | wo | w1 | w3 | w2]).
+  // int8 engine: every Linear is an int8 matrix; path A streams them through k_gemv_w8, path B widens one layer's q at a
+  // time into layer_scratch (lm_head's once, at create, into w8_head) and k_tc_gemm applies the row scales.
+  WFmt fmt = WFmt::BF16;
+  __nv_bfloat16* layer_scratch = nullptr;
+  __nv_bfloat16* w8_head = nullptr;
 
   template <typename T>
   T* wsp(size_t o) const { return reinterpret_cast<T*>(ws + o); }
   const __nv_bfloat16* w(int i) const { return reinterpret_cast<const __nv_bfloat16*>(arena + off[i]); }
   const __nv_bfloat16* lw(int layer, int t) const { return w(MVB_S1_GLOBAL_TENSORS + layer * MVB_S1_LAYER_TENSORS + t); }
   // The one weight-source accessor of the tensor-core path: the bf16 matrix t (1 wqkv, 2 wo, 4 w1, 5 w3, 6 w2) of a layer,
-  // i.e. the arena tensor, or for an int4 engine its slot in the dequantised-layer scratch (filled by k_w4_dequant).
+  // i.e. the arena tensor, or for an int4 / int8 engine its slot in the layer scratch (k_w4_dequant / k_w8_widen fill it).
   const __nv_bfloat16* tc_w(int layer, int t) const {
-    if (!int4) return lw(layer, t);
+    if (fmt == WFmt::BF16) return lw(layer, t);
     const size_t D = cfg.dim, F = cfg.intermediate;
     const size_t at[7] = {0, 0, 3 * D * D, 0, 4 * D * D, 4 * D * D + F * D, 4 * D * D + 2 * F * D};
-    return w4_scratch + at[t];
+    return layer_scratch + at[t];
   }
+  // Row scales of the tensor-core path: those of arena tensor i ([M, K]) for an int8 engine, else none.
+  const __nv_bfloat16* tc_scale(int i, int M, int K) const {
+    if (fmt != WFmt::INT8) return nullptr;
+    return reinterpret_cast<const __nv_bfloat16*>(arena + off[i] + w8_scale_offset(M, K));
+  }
+  const __nv_bfloat16* tc_lscale(int layer, int t) const {
+    const Mk mk = layer_mk(cfg, t);
+    return tc_scale(MVB_S1_GLOBAL_TENSORS + layer * MVB_S1_LAYER_TENSORS + t, mk.M, mk.K);
+  }
+  const __nv_bfloat16* head_scale() const { return tc_scale(4, cfg.vocab, cfg.dim); }
   size_t kv_elem() const { return cfg.kv_dtype == MVB_KV_FP32 ? 4 : 2; }
   size_t kv_half_bytes() const {
     return (size_t)2 * cfg.max_utts * cfg.n_head * cfg.block_size * cfg.head_dim * kv_elem();
@@ -211,8 +240,13 @@ extern "C" size_t mvb_s1_int4_workspace_bytes(const mvb_s1_config* c) {
   return make_layout(*c).total_int4;
 }
 
+extern "C" size_t mvb_s1_int8_workspace_bytes(const mvb_s1_config* c) {
+  if (validate(c)) return 0;
+  return make_layout(*c).total_int8;
+}
+
 static int create_engine(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
-                         void* d_kv, void* d_ws, mvb_s1** out, bool int4) {
+                         void* d_kv, void* d_ws, mvb_s1** out, WFmt fmt) {
   if (int e = validate(cfg)) return e;
   if (!d_arena || !offsets || !d_kv || !d_ws || !out) return set_error(MVB_ERR_ARG, "null pointer argument");
   int dev = 0, n_sm = 0, major = 0, minor = 0;
@@ -231,17 +265,30 @@ static int create_engine(const mvb_s1_config* cfg, const void* d_arena, size_t a
   h->kv = reinterpret_cast<char*>(d_kv);
   h->ws = reinterpret_cast<char*>(d_ws);
   h->L = make_layout(*cfg);
-  h->int4 = int4;
-  if (int4) {
-    h->w4_scratch = h->wsp<__nv_bfloat16>(h->L.w4_scratch);
-    const int D = cfg->dim, F = cfg->intermediate;
-    const int MK[7][2] = {{0, 0}, {3 * D, D}, {D, D}, {0, 0}, {F, D}, {F, D}, {D, F}};
+  h->fmt = fmt;
+  if (fmt != WFmt::BF16) {
+    h->layer_scratch = h->wsp<__nv_bfloat16>(h->L.layer_scratch);
+    const bool w8 = fmt == WFmt::INT8;
     for (int l = 0; l < cfg->n_layer; ++l)
       for (int t : {1, 2, 4, 5, 6}) {
         const uint64_t o = h->off[MVB_S1_GLOBAL_TENSORS + l * MVB_S1_LAYER_TENSORS + t];
-        if (o + w4_packed_bytes(MK[t][0], MK[t][1]) > arena_bytes)
-          return set_error(MVB_ERR_ARG, "int4 packed matrix %d of layer %d runs past the end of the arena", t, l);
+        const Mk mk = layer_mk(*cfg, t);
+        if (o + (w8 ? w8_matrix_bytes(mk.M, mk.K) : w4_packed_bytes(mk.M, mk.K)) > arena_bytes)
+          return set_error(MVB_ERR_ARG, "%s matrix %d of layer %d runs past the end of the arena", w8 ? "int8" : "int4 packed", t, l);
       }
+    if (w8) {
+      if (h->off[2] + w8_matrix_bytes(cfg->dim, cfg->spk_dim) > arena_bytes || h->off[4] + w8_matrix_bytes(cfg->vocab, cfg->dim) > arena_bytes)
+        return set_error(MVB_ERR_ARG, "int8 matrix speaker_cond_pos or lm_head runs past the end of the arena");
+      // lm_head's q, widened once: the head GEMM of every prefill chunk reads it from here
+      h->w8_head = h->wsp<__nv_bfloat16>(h->L.w8_head);
+      W8Mats m{};
+      m.src[0] = reinterpret_cast<const uint8_t*>(h->w(4));
+      m.dst[0] = h->w8_head;
+      m.M[0] = cfg->vocab; m.K[0] = cfg->dim; m.n = 1;
+      k_w8_widen<<<4 * n_sm, 256>>>(m);
+      MVB_CK(cudaGetLastError());
+      MVB_CK(cudaStreamSynchronize(0));
+    }
   }
   S1State& s = h->st;
   s.slot_map = h->wsp<int>(h->L.slot_map);
@@ -277,7 +324,7 @@ static int create_engine(const mvb_s1_config* cfg, const void* d_arena, size_t a
       ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 3], h->tc_w(l, 5), F, D, 128);
       ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 4], h->tc_w(l, 6), D, F, 128);
     }
-    ok = ok && make_tmap_bf16(&h->tmW[(size_t)cfg->n_layer * 5], h->w(4), cfg->vocab, D, 128);
+    ok = ok && make_tmap_bf16(&h->tmW[(size_t)cfg->n_layer * 5], fmt == WFmt::INT8 ? h->w8_head : h->w(4), cfg->vocab, D, 128);
     if (!ok) return set_error(MVB_ERR_CUDA, "cuTensorMapEncodeTiled failed for a weight matrix");
   }
   // The persistent kernel's bf16-cache attention fetches KV tiles through tm_kv as whole 64-position boxes: positions
@@ -293,7 +340,7 @@ static int create_engine(const mvb_s1_config* cfg, const void* d_arena, size_t a
   {
     // persistent decode kernel: needs a uniform layer stride (true for arenas packed in checkpoint order)
     const int D = cfg->dim, F = cfg->intermediate, V = cfg->vocab;
-    bool ok = cfg->n_layer >= 1 && !int4 && kv_ok;   // an int4 engine never uses path C
+    bool ok = cfg->n_layer >= 1 && fmt == WFmt::BF16 && kv_ok;   // an int4 or int8 engine never uses path C
     const int o0 = MVB_S1_GLOBAL_TENSORS;
     uint64_t stride = cfg->n_layer > 1 ? h->off[o0 + MVB_S1_LAYER_TENSORS] - h->off[o0] : 2 * (uint64_t)(4 * D * D + 3 * D * F + 2 * D);
     for (int l = 1; l < cfg->n_layer && ok; ++l)
@@ -332,12 +379,17 @@ static int create_engine(const mvb_s1_config* cfg, const void* d_arena, size_t a
 
 extern "C" int mvb_s1_create(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
                              void* d_kv, void* d_ws, mvb_s1** out) {
-  return create_engine(cfg, d_arena, arena_bytes, offsets, d_kv, d_ws, out, false);
+  return create_engine(cfg, d_arena, arena_bytes, offsets, d_kv, d_ws, out, WFmt::BF16);
 }
 
 extern "C" int mvb_s1_create_int4(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
                                   void* d_kv, void* d_ws, mvb_s1** out) {
-  return create_engine(cfg, d_arena, arena_bytes, offsets, d_kv, d_ws, out, true);
+  return create_engine(cfg, d_arena, arena_bytes, offsets, d_kv, d_ws, out, WFmt::INT4);
+}
+
+extern "C" int mvb_s1_create_int8(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
+                                  void* d_kv, void* d_ws, mvb_s1** out) {
+  return create_engine(cfg, d_arena, arena_bytes, offsets, d_kv, d_ws, out, WFmt::INT8);
 }
 
 extern "C" int mvb_s1_destroy(mvb_s1* h) {
@@ -375,14 +427,16 @@ static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
 
-// w4: p.W / p.W3 are int4 packed matrices (k_gemv_w4), else bf16 (k_gemv); both take one item per warp.
+// p.W / p.W3 are matrices of format `fmt`: bf16 (k_gemv), int4 packed (k_gemv_w4) or int8 (k_gemv_w8); all three take one
+// item per warp.
 template <int EPI>
-static cudaError_t launch_gemv(mvb_s1* h, cudaStream_t s, int n_utts, GemvP p, bool w4 = false) {
+static cudaError_t launch_gemv(mvb_s1* h, cudaStream_t s, int n_utts, GemvP p, WFmt fmt) {
   const int n_items = (EPI == EPI_SWIGLU) ? p.M : p.M / 2;
   dim3 grid(gemv_grid(n_items, h->n_sm), n_utts);
   const size_t smem = (size_t)2 * p.K * sizeof(float);
   h->launches++;
-  if (w4) return launch_pdl(k_gemv_w4<EPI>, grid, dim3(256), smem, s, p, h->st);
+  if (fmt == WFmt::INT4) return launch_pdl(k_gemv_w4<EPI>, grid, dim3(256), smem, s, p, h->st);
+  if (fmt == WFmt::INT8) return launch_pdl(k_gemv_w8<EPI>, grid, dim3(256), smem, s, p, h->st);
   return launch_pdl(k_gemv<EPI>, grid, dim3(256), smem, s, p, h->st);
 }
 
@@ -408,7 +462,7 @@ static int launch_body(mvb_s1* h, cudaStream_t s, int n_utts) {
     p.W = h->lw(l, 1); p.W3 = nullptr; p.x = x; p.ldx = D; p.gain = h->lw(l, 0);
     p.out = qkv; p.ldo = 3 * D; p.M = 3 * D; p.K = D;
     p.kcache = kc; p.vcache = vc; p.H = H; p.S_max = c.block_size; p.D = D; p.kv_fp32 = c.kv_dtype == MVB_KV_FP32;
-    MVB_CK(launch_gemv<EPI_QKV>(h, s, n_utts, p, h->int4));
+    MVB_CK(launch_gemv<EPI_QKV>(h, s, n_utts, p, h->fmt));
     // attention over [0, pos]
     dim3 ag(H, 2 * n_utts, ATT_SPLITS);
     if (c.kv_dtype == MVB_KV_FP32)
@@ -422,18 +476,18 @@ static int launch_body(mvb_s1* h, cudaStream_t s, int n_utts) {
     p = GemvP{};
     p.eps = c.norm_eps;
     p.W = h->lw(l, 2); p.x = att; p.ldx = D; p.gain = nullptr; p.out = x; p.ldo = D; p.M = D; p.K = D;
-    MVB_CK(launch_gemv<EPI_RESID>(h, s, n_utts, p, h->int4));
+    MVB_CK(launch_gemv<EPI_RESID>(h, s, n_utts, p, h->fmt));
     // ffn_norm + silu(w1 x) * w3 x
     p.W = h->lw(l, 4); p.W3 = h->lw(l, 5); p.x = x; p.ldx = D; p.gain = h->lw(l, 3); p.out = ffn; p.ldo = F; p.M = F; p.K = D;
-    MVB_CK(launch_gemv<EPI_SWIGLU>(h, s, n_utts, p, h->int4));
+    MVB_CK(launch_gemv<EPI_SWIGLU>(h, s, n_utts, p, h->fmt));
     // w2 + residual
     p.W = h->lw(l, 6); p.W3 = nullptr; p.x = ffn; p.ldx = F; p.gain = nullptr; p.out = x; p.ldo = D; p.M = D; p.K = F;
-    MVB_CK(launch_gemv<EPI_RESID>(h, s, n_utts, p, h->int4));
+    MVB_CK(launch_gemv<EPI_RESID>(h, s, n_utts, p, h->fmt));
   }
   GemvP p{};
   p.eps = c.norm_eps;
   p.W = h->w(4); p.x = x; p.ldx = D; p.gain = h->w(3); p.out = logits; p.ldo = V; p.M = V; p.K = D;
-  MVB_CK(launch_gemv<EPI_STORE>(h, s, n_utts, p));
+  MVB_CK(launch_gemv<EPI_STORE>(h, s, n_utts, p, h->fmt == WFmt::INT8 ? WFmt::INT8 : WFmt::BF16));   // int4: lm_head is bf16
   return MVB_OK;
 }
 
@@ -457,6 +511,8 @@ struct LinB {
   int widx, widx3;                                     // tensor-map indices of W (and W3 for SwiGLU)
   int M, K;
   float* out; int ldo;
+  const __nv_bfloat16* scale = nullptr;                // int8 engine: row scales of W (and W3)
+  const __nv_bfloat16* scale3 = nullptr;
 };
 
 template <int EPI>
@@ -475,6 +531,7 @@ static int linear_b(mvb_s1* h, cudaStream_t s, int R, const LinB& a, void* kc = 
   g.scratch = h->wsp<float>(h->L.b_scratch);
   g.tickets = h->wsp<unsigned>(h->L.b_tickets);
   g.n_sm = h->n_sm;
+  g.scale = a.scale; g.scale3 = a.scale3;
   MVB_CK(tc_gemm(s, g));
   h->launches += 2;   // k_prep_b + k_tc_gemm
   return MVB_OK;
@@ -495,20 +552,26 @@ static int launch_layers_b(mvb_s1* h, cudaStream_t s, int R) {
   for (int l = 0; l < c.n_layer; ++l) {
     char* kc = h->kv + (size_t)l * 2 * half;
     char* vc = kc + half;
-    if (h->int4) {   // this layer's W_deq -> the scratch the tensor maps of every layer point at
-      W4Mats m{};
-      const int MK[5][3] = {{1, 3 * D, D}, {2, D, D}, {4, F, D}, {5, F, D}, {6, D, F}};
+    if (h->fmt != WFmt::BF16) {   // this layer's W_deq (int4) or q (int8) -> the scratch the tensor maps of every layer point at
+      W4Mats m{};   // == W8Mats
+      const int ts[5] = {1, 2, 4, 5, 6};
       for (int i = 0; i < 5; ++i) {
-        m.src[i] = reinterpret_cast<const uint8_t*>(h->lw(l, MK[i][0]));
-        m.dst[i] = const_cast<__nv_bfloat16*>(h->tc_w(l, MK[i][0]));
-        m.M[i] = MK[i][1]; m.K[i] = MK[i][2];
+        const Mk mk = layer_mk(c, ts[i]);
+        m.src[i] = reinterpret_cast<const uint8_t*>(h->lw(l, ts[i]));
+        m.dst[i] = const_cast<__nv_bfloat16*>(h->tc_w(l, ts[i]));
+        m.M[i] = mk.M; m.K[i] = mk.K;
       }
       m.n = 5;
-      k_w4_dequant<<<4 * h->n_sm, 256, 0, s>>>(m);
+      if (h->fmt == WFmt::INT4) {
+        k_w4_dequant<<<4 * h->n_sm, 256, 0, s>>>(m);
+      } else {
+        k_w8_widen<<<4 * h->n_sm, 256, 0, s>>>(m);
+      }
       h->launches++;
       MVB_CK(cudaGetLastError());
     }
-    if (int e = linear_b<G_QKV>(h, s, R, LinB{x, D, h->lw(l, 0), l * 5 + 0, l * 5 + 0, 3 * D, D, qkv, 3 * D}, kc, vc)) return e;
+    if (int e = linear_b<G_QKV>(h, s, R, LinB{x, D, h->lw(l, 0), l * 5 + 0, l * 5 + 0, 3 * D, D, qkv, 3 * D, h->tc_lscale(l, 1)},
+                                kc, vc)) return e;
     dim3 ag(H, R, ATT_SPLITS);
     if (c.kv_dtype == MVB_KV_FP32)
       k_attn_rows<true><<<ag, 128, 0, s>>>(h->rows, qkv, kc, vc, h->wsp<float>(h->L.b_part_o), h->wsp<float>(h->L.b_part_ml),
@@ -518,9 +581,10 @@ static int launch_layers_b(mvb_s1* h, cudaStream_t s, int R) {
                                             h->wsp<unsigned>(h->L.b_att_tickets), att, H, c.block_size, D);
     h->launches++;
     MVB_CK(cudaGetLastError());
-    if (int e = linear_b<G_RESID>(h, s, R, LinB{att, D, nullptr, l * 5 + 1, l * 5 + 1, D, D, x, D})) return e;
-    if (int e = linear_b<G_SWIGLU>(h, s, R, LinB{x, D, h->lw(l, 3), l * 5 + 2, l * 5 + 3, F, D, ffn, F})) return e;
-    if (int e = linear_b<G_RESID>(h, s, R, LinB{ffn, F, nullptr, l * 5 + 4, l * 5 + 4, D, F, x, D})) return e;
+    if (int e = linear_b<G_RESID>(h, s, R, LinB{att, D, nullptr, l * 5 + 1, l * 5 + 1, D, D, x, D, h->tc_lscale(l, 2)})) return e;
+    if (int e = linear_b<G_SWIGLU>(h, s, R, LinB{x, D, h->lw(l, 3), l * 5 + 2, l * 5 + 3, F, D, ffn, F, h->tc_lscale(l, 4),
+                                                  h->tc_lscale(l, 5)})) return e;
+    if (int e = linear_b<G_RESID>(h, s, R, LinB{ffn, F, nullptr, l * 5 + 4, l * 5 + 4, D, F, x, D, h->tc_lscale(l, 6)})) return e;
   }
   return MVB_OK;
 }
@@ -535,7 +599,7 @@ static int launch_body_b(mvb_s1* h, cudaStream_t s, int n_utts) {
   if (int e = launch_layers_b(h, s, R)) return e;
   const int hw = c.n_layer * 5;
   return linear_b<G_STORE>(h, s, R, LinB{h->wsp<float>(h->L.b_x), c.dim, h->w(3), hw, hw, c.vocab, c.dim,
-                                         h->wsp<float>(h->L.logits), c.vocab});
+                                         h->wsp<float>(h->L.logits), c.vocab, h->head_scale()});
 }
 
 
@@ -609,7 +673,7 @@ static int run_body(mvb_s1* h, cudaStream_t s, int n_utts, bool allow_b = true) 
   // Path A (CUDA-core GEMV) streams the weights once per utterance; from 2 utterances up the tensor-core
   // rows path streams them once per step for the whole batch.  slot_map must be the identity for path B
   // (its logits rows are batch-ordered), which mvb_s1_decode guarantees.
-  const bool use_b = allow_b && h->path_b && !h->int4 && n_utts >= 2;   // int4 decode: always path A
+  const bool use_b = allow_b && h->path_b && h->fmt == WFmt::BF16 && n_utts >= 2;   // int4 / int8 decode: always path A
   auto body = [&](cudaStream_t st) { return use_b ? launch_body_b(h, st, n_utts) : launch_body(h, st, n_utts); };
   const int key = n_utts + (use_b ? 1000 : 0);
   auto it = h->graphs.find(key);
@@ -647,7 +711,12 @@ extern "C" int mvb_s1_set_speaker(mvb_s1* h, int32_t utt, const float* d_spk, vo
   if (int e = check_slot(h, utt)) return e;
   cudaStream_t s = (cudaStream_t)stream;
   const int D = h->cfg.dim;
-  k_spk_proj<<<(D * 32 + 255) / 256, 256, 0, s>>>(h->w(2), d_spk, h->wsp<float>(h->L.spk) + (size_t)utt * D, D, h->cfg.spk_dim);
+  float* out = h->wsp<float>(h->L.spk) + (size_t)utt * D;
+  if (h->fmt == WFmt::INT8)
+    k_spk_proj<int8_t><<<(D * 32 + 255) / 256, 256, 0, s>>>(reinterpret_cast<const int8_t*>(h->w(2)), d_spk, out, D, h->cfg.spk_dim,
+                                                            h->tc_scale(2, D, h->cfg.spk_dim));
+  else
+    k_spk_proj<__nv_bfloat16><<<(D * 32 + 255) / 256, 256, 0, s>>>(h->w(2), d_spk, out, D, h->cfg.spk_dim, nullptr);
   h->launches++;
   MVB_CK(cudaGetLastError());
   return MVB_OK;
@@ -677,7 +746,7 @@ extern "C" int mvb_s1_forward(mvb_s1* h, int32_t utt, const int32_t* d_idx, int3
       float* bx = h->wsp<float>(h->L.b_x);
       if (d_logits && all_positions) {
         float* bl = h->wsp<float>(h->L.b_logits);
-        if (int e = linear_b<G_STORE>(h, s, R, LinB{bx, c.dim, h->w(3), hw, hw, V, c.dim, bl, V})) return e;
+        if (int e = linear_b<G_STORE>(h, s, R, LinB{bx, c.dim, h->w(3), hw, hw, V, c.dim, bl, V, h->head_scale()})) return e;
         for (int cc = 0; cc < 2; ++cc)
           MVB_CK(cudaMemcpyAsync(d_logits + ((size_t)cc * S + s0) * V, bl + (size_t)cc * Sc * V, sizeof(float) * (size_t)Sc * V,
                              cudaMemcpyDeviceToDevice, s));
@@ -689,7 +758,7 @@ extern "C" int mvb_s1_forward(mvb_s1* h, int32_t utt, const int32_t* d_idx, int3
         h->launches++;
         MVB_CK(cudaGetLastError());
         if (int e = linear_b<G_STORE>(h, s, 2, LinB{last, c.dim, h->w(3), hw, hw, V, c.dim,
-                                                    h->wsp<float>(h->L.logits) + (size_t)(2 * utt) * V, V})) return e;
+                                                    h->wsp<float>(h->L.logits) + (size_t)(2 * utt) * V, V, h->head_scale()})) return e;
         k_set_input<<<1, 32, 0, s>>>(h->st, utt, d_idx, S, S - 1, pos0 + S - 1);
         h->launches++;
         MVB_CK(cudaGetLastError());
@@ -1028,12 +1097,12 @@ extern "C" int mvb_s1_generate(mvb_s1* h, int32_t n_utts, const int32_t* prompts
 }
 
 // ------------------------------------------------------------------------------------------------
-// Test hooks of the int4 kernels (include/mvb200.h): k_gemv_w4<epi> exactly as path A launches it, over a caller-built
-// decode state (slot map and positions), and k_w4_dequant on one packed matrix.
-extern "C" int mvb_w4_gemv_test(int32_t epi, const void* d_W, const void* d_W3, int32_t M, int32_t K, const float* d_x,
-                                int32_t ldx, int32_t n_utts, const void* d_gain, float eps, float* d_out, int32_t ldo,
-                                void* d_kcache, void* d_vcache, const int32_t* d_slot_map, const int32_t* d_pos, int32_t H,
-                                int32_t S_max, int32_t D, int32_t kv_fp32, void* stream) {
+// Test hooks of the int4 and int8 kernels (include/mvb200.h): k_gemv_w4<epi> / k_gemv_w8<epi> exactly as path A launches
+// them, over a caller-built decode state (slot map and positions), k_w4_dequant / k_w8_widen on one matrix.
+static int quant_gemv_test(WFmt fmt, int32_t epi, const void* d_W, const void* d_W3, int32_t M, int32_t K, const float* d_x,
+                           int32_t ldx, int32_t n_utts, const void* d_gain, float eps, float* d_out, int32_t ldo,
+                           void* d_kcache, void* d_vcache, const int32_t* d_slot_map, const int32_t* d_pos, int32_t H,
+                           int32_t S_max, int32_t D, int32_t kv_fp32, void* stream) {
   if (!d_W || !d_x || !d_out || !d_slot_map || !d_pos) return set_error(MVB_ERR_ARG, "null argument");
   if (epi < EPI_STORE || epi > EPI_QKV) return set_error(MVB_ERR_ARG, "bad epilogue %d", epi);
   if (K < 256 || K % 256 || M < 2 || M % 2 || n_utts < 1 || n_utts > 64) return set_error(MVB_ERR_ARG, "bad shape M=%d K=%d n_utts=%d", M, K, n_utts);
@@ -1052,13 +1121,29 @@ extern "C" int mvb_w4_gemv_test(int32_t epi, const void* d_W, const void* d_W3, 
   p.kcache = d_kcache; p.vcache = d_vcache; p.H = H; p.S_max = S_max; p.D = D; p.kv_fp32 = kv_fp32;
   cudaStream_t s = (cudaStream_t)stream;
   switch (epi) {
-    case EPI_STORE: MVB_CK(launch_gemv<EPI_STORE>(&h, s, n_utts, p, true)); break;
-    case EPI_RESID: MVB_CK(launch_gemv<EPI_RESID>(&h, s, n_utts, p, true)); break;
-    case EPI_SWIGLU: MVB_CK(launch_gemv<EPI_SWIGLU>(&h, s, n_utts, p, true)); break;
-    default: MVB_CK(launch_gemv<EPI_QKV>(&h, s, n_utts, p, true)); break;
+    case EPI_STORE: MVB_CK(launch_gemv<EPI_STORE>(&h, s, n_utts, p, fmt)); break;
+    case EPI_RESID: MVB_CK(launch_gemv<EPI_RESID>(&h, s, n_utts, p, fmt)); break;
+    case EPI_SWIGLU: MVB_CK(launch_gemv<EPI_SWIGLU>(&h, s, n_utts, p, fmt)); break;
+    default: MVB_CK(launch_gemv<EPI_QKV>(&h, s, n_utts, p, fmt)); break;
   }
   MVB_CK(cudaStreamSynchronize(s));
   return MVB_OK;
+}
+
+extern "C" int mvb_w4_gemv_test(int32_t epi, const void* d_W, const void* d_W3, int32_t M, int32_t K, const float* d_x,
+                                int32_t ldx, int32_t n_utts, const void* d_gain, float eps, float* d_out, int32_t ldo,
+                                void* d_kcache, void* d_vcache, const int32_t* d_slot_map, const int32_t* d_pos, int32_t H,
+                                int32_t S_max, int32_t D, int32_t kv_fp32, void* stream) {
+  return quant_gemv_test(WFmt::INT4, epi, d_W, d_W3, M, K, d_x, ldx, n_utts, d_gain, eps, d_out, ldo, d_kcache, d_vcache,
+                         d_slot_map, d_pos, H, S_max, D, kv_fp32, stream);
+}
+
+extern "C" int mvb_w8_gemv_test(int32_t epi, const void* d_W, const void* d_W3, int32_t M, int32_t K, const float* d_x,
+                                int32_t ldx, int32_t n_utts, const void* d_gain, float eps, float* d_out, int32_t ldo,
+                                void* d_kcache, void* d_vcache, const int32_t* d_slot_map, const int32_t* d_pos, int32_t H,
+                                int32_t S_max, int32_t D, int32_t kv_fp32, void* stream) {
+  return quant_gemv_test(WFmt::INT8, epi, d_W, d_W3, M, K, d_x, ldx, n_utts, d_gain, eps, d_out, ldo, d_kcache, d_vcache,
+                         d_slot_map, d_pos, H, S_max, D, kv_fp32, stream);
 }
 
 extern "C" int mvb_w4_dequant_test(const void* d_W, int32_t M, int32_t K, void* d_out, void* stream) {
@@ -1072,6 +1157,22 @@ extern "C" int mvb_w4_dequant_test(const void* d_W, int32_t M, int32_t K, void* 
   if (int e = current_device(&dev, &n_sm)) return e;
   cudaStream_t s = (cudaStream_t)stream;
   k_w4_dequant<<<4 * n_sm, 256, 0, s>>>(m);
+  MVB_CK(cudaGetLastError());
+  MVB_CK(cudaStreamSynchronize(s));
+  return MVB_OK;
+}
+
+extern "C" int mvb_w8_widen_test(const void* d_W, int32_t M, int32_t K, void* d_out, void* stream) {
+  if (!d_W || !d_out) return set_error(MVB_ERR_ARG, "null argument");
+  if (M < 1 || K < 256 || K % 256) return set_error(MVB_ERR_ARG, "bad shape M=%d K=%d", M, K);
+  W8Mats m{};
+  m.src[0] = reinterpret_cast<const uint8_t*>(d_W);
+  m.dst[0] = reinterpret_cast<__nv_bfloat16*>(d_out);
+  m.M[0] = M; m.K[0] = K; m.n = 1;
+  int dev = 0, n_sm = 0;
+  if (int e = current_device(&dev, &n_sm)) return e;
+  cudaStream_t s = (cudaStream_t)stream;
+  k_w8_widen<<<4 * n_sm, 256, 0, s>>>(m);
   MVB_CK(cudaGetLastError());
   MVB_CK(cudaStreamSynchronize(s));
   return MVB_OK;

@@ -5,6 +5,8 @@
 // Row convention: utterance slot u owns activation rows 2u (speaker-conditioned) and 2u+1
 // (unconditioned) -- the CFG pair of fam/llm/fast_model.py:132-134.
 #pragma once
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace mvb {
@@ -36,14 +38,20 @@ struct S1State {
 };
 
 // ---------------------------------------------------------------------------------------------
-// spk_proj[u] = W_spk . spk_emb   (fast_model.py:155 speaker_cond_pos, hoisted out of the step)
-__global__ void __launch_bounds__(256) k_spk_proj(const __nv_bfloat16* __restrict__ W, const float* __restrict__ spk,
-                                                  float* __restrict__ out, int D, int SD) {
+// spk_proj[u] = W_spk . spk_emb   (fast_model.py:155 speaker_cond_pos, hoisted out of the step).  TW = __nv_bfloat16, or
+// int8_t for an int8 engine, whose bf16 row scales (`scale`) multiply each output once after the sum.
+__device__ __forceinline__ float w_to_f32(__nv_bfloat16 w) { return bf16_to_f32(w); }
+__device__ __forceinline__ float w_to_f32(int8_t w) { return (float)w; }
+
+template <typename TW>
+__global__ void __launch_bounds__(256) k_spk_proj(const TW* __restrict__ W, const float* __restrict__ spk,
+                                                  float* __restrict__ out, int D, int SD, const __nv_bfloat16* __restrict__ scale) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (warp >= D) return;
   float acc = 0.f;
-  for (int k = lane; k < SD; k += 32) acc = fmaf(bf16_to_f32(W[(size_t)warp * SD + k]), spk[k], acc);
+  for (int k = lane; k < SD; k += 32) acc = fmaf(w_to_f32(W[(size_t)warp * SD + k]), spk[k], acc);
   acc = warp_sum(acc);
+  if constexpr (!std::is_same<TW, __nv_bfloat16>::value) acc *= bf16_to_f32(scale[warp]);
   if (lane == 0) out[warp] = acc;
 }
 
@@ -145,7 +153,97 @@ __device__ __forceinline__ void gemv_rows(const GemvP& p, int item, int lane, co
   }
 }
 
-// k_gemv_w4 (gemv_w4.cuh) repeats this prologue and these epilogues over int4 weights: a fix to one belongs in the other.
+// Prologue of the GEMV kernels (k_gemv, k_gemv_w4, k_gemv_w8): stage the two activation rows r0, r0 + 1 of p.x into
+// xs [2][K] at perm(k), RMS-normalised (fp32 statistics, then the bf16 gain) when p.gain is set.  Ends with __syncthreads.
+template <typename Perm>
+__device__ __forceinline__ void gemv_prologue(const GemvP& p, int r0, float* xs, float* red, Perm perm) {
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int K = p.K;
+  const float* x0 = p.x + (size_t)r0 * p.ldx;
+  const float* x1 = x0 + p.ldx;
+  float s0 = 0.f, s1 = 0.f;
+  for (int k = tid; k < K; k += 256) {
+    const float a = x0[k], b = x1[k];
+    s0 = fmaf(a, a, s0);
+    s1 = fmaf(b, b, s1);
+    const int pk = perm(k);
+    xs[pk] = a;
+    xs[K + pk] = b;
+  }
+  if (p.gain != nullptr) {
+    s0 = warp_sum(s0);
+    s1 = warp_sum(s1);
+    if (lane == 0) {
+      red[warp] = s0;
+      red[8 + warp] = s1;
+    }
+    __syncthreads();
+    float t0 = 0.f, t1 = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      t0 += red[i];
+      t1 += red[8 + i];
+    }
+    const float rs0 = rsqrtf(t0 / (float)K + p.eps);
+    const float rs1 = rsqrtf(t1 / (float)K + p.eps);
+    for (int k = tid; k < K; k += 256) {
+      const float g = bf16_to_f32(p.gain[k]);
+      const int pk = perm(k);
+      xs[pk] = (xs[pk] * rs0) * g;
+      xs[K + pk] = (xs[K + pk] * rs1) * g;
+    }
+  }
+  __syncthreads();
+}
+
+// Epilogue of the GEMV kernels for one item of slot u: a<weight row><activation row>, weight rows 2 item, 2 item + 1
+// (EPI_SWIGLU: a0* = w1 row item, a1* = w3 row item).
+template <int EPI>
+__device__ __forceinline__ void gemv_epilogue(const GemvP& p, const S1State& st, int u, int item, float a00, float a01,
+                                              float a10, float a11) {
+  const int r0 = 2 * u;
+  float* o0 = p.out + (size_t)r0 * p.ldo;
+  float* o1 = o0 + p.ldo;
+  if (EPI == EPI_SWIGLU) {
+    o0[item] = (a00 / (1.f + expf(-a00))) * a10;
+    o1[item] = (a01 / (1.f + expf(-a01))) * a11;
+  } else {
+    const int j = 2 * item;
+    if (EPI == EPI_RESID) {
+      o0[j] += a00;
+      o1[j] += a01;
+      o0[j + 1] += a10;
+      o1[j + 1] += a11;
+    } else {
+      o0[j] = a00;
+      o1[j] = a01;
+      o0[j + 1] = a10;
+      o1[j + 1] = a11;
+    }
+    if (EPI == EPI_QKV && j >= p.D) {
+      // scatter k / v of the current token into the cache at input_pos (fast_model.py:111-112)
+      const int which = (j - p.D) / p.D;  // 0 = k, 1 = v
+      const int jj = (j - p.D) - which * p.D;
+      const int head = jj >> 7, d = jj & 127;
+      const int pos = st.pos[u];
+      const size_t e0 = (((size_t)r0 * p.H + head) * p.S_max + pos) * 128 + d;
+      const size_t e1 = e0 + (size_t)p.H * p.S_max * 128;
+      void* base = which ? p.vcache : p.kcache;
+      if (p.kv_fp32) {
+        float* c = reinterpret_cast<float*>(base);
+        c[e0] = a00;
+        c[e0 + 1] = a10;
+        c[e1] = a01;
+        c[e1 + 1] = a11;
+      } else {
+        __nv_bfloat16* c = reinterpret_cast<__nv_bfloat16*>(base);
+        *reinterpret_cast<__nv_bfloat162*>(c + e0) = __floats2bfloat162_rn(a00, a10);
+        *reinterpret_cast<__nv_bfloat162*>(c + e1) = __floats2bfloat162_rn(a01, a11);
+      }
+    }
+  }
+}
+
 template <int EPI>
 __global__ void __launch_bounds__(256, 2) k_gemv(GemvP p, S1State st) {
   extern __shared__ float xs[];  // [2][K] permuted
@@ -159,45 +257,7 @@ __global__ void __launch_bounds__(256, 2) k_gemv(GemvP p, S1State st) {
   pdl_wait();  // activations written by the previous kernel are now visible
 
   const int u = st.slot_map[blockIdx.y];
-  const int r0 = 2 * u;
-  // ---- prologue: stage (and normalise) the two activation rows
-  {
-    const float* x0 = p.x + (size_t)r0 * p.ldx;
-    const float* x1 = x0 + p.ldx;
-    float s0 = 0.f, s1 = 0.f;
-    for (int k = tid; k < K; k += 256) {
-      const float a = x0[k], b = x1[k];
-      s0 = fmaf(a, a, s0);
-      s1 = fmaf(b, b, s1);
-      const int pk = xs_perm(k);
-      xs[pk] = a;
-      xs[K + pk] = b;
-    }
-    if (p.gain != nullptr) {
-      s0 = warp_sum(s0);
-      s1 = warp_sum(s1);
-      if (lane == 0) {
-        red[warp] = s0;
-        red[8 + warp] = s1;
-      }
-      __syncthreads();
-      float t0 = 0.f, t1 = 0.f;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        t0 += red[i];
-        t1 += red[8 + i];
-      }
-      const float rs0 = rsqrtf(t0 / (float)K + p.eps);
-      const float rs1 = rsqrtf(t1 / (float)K + p.eps);
-      for (int k = tid; k < K; k += 256) {
-        const float g = bf16_to_f32(p.gain[k]);
-        const int pk = xs_perm(k);
-        xs[pk] = (xs[pk] * rs0) * g;
-        xs[K + pk] = (xs[K + pk] * rs1) * g;
-      }
-    }
-    __syncthreads();
-  }
+  gemv_prologue(p, 2 * u, xs, red, [](int k) { return xs_perm(k); });
 
   // ---- main: each warp streams two weight rows at a time
   for (int item = blockIdx.x * 8 + warp; item < n_items; item += nwarps) {
@@ -221,48 +281,7 @@ __global__ void __launch_bounds__(256, 2) k_gemv(GemvP p, S1State st) {
     a01 = warp_sum(a01);
     a10 = warp_sum(a10);
     a11 = warp_sum(a11);
-    if (lane == 0) {
-      float* o0 = p.out + (size_t)r0 * p.ldo;
-      float* o1 = o0 + p.ldo;
-      if (EPI == EPI_SWIGLU) {
-        o0[item] = (a00 / (1.f + expf(-a00))) * a10;
-        o1[item] = (a01 / (1.f + expf(-a01))) * a11;
-      } else {
-        const int j = 2 * item;
-        if (EPI == EPI_RESID) {
-          o0[j] += a00;
-          o1[j] += a01;
-          o0[j + 1] += a10;
-          o1[j + 1] += a11;
-        } else {
-          o0[j] = a00;
-          o1[j] = a01;
-          o0[j + 1] = a10;
-          o1[j + 1] = a11;
-        }
-        if (EPI == EPI_QKV && j >= p.D) {
-          // scatter k / v of the current token into the cache at input_pos (fast_model.py:111-112)
-          const int which = (j - p.D) / p.D;  // 0 = k, 1 = v
-          const int jj = (j - p.D) - which * p.D;
-          const int head = jj >> 7, d = jj & 127;
-          const int pos = st.pos[u];
-          const size_t e0 = (((size_t)r0 * p.H + head) * p.S_max + pos) * 128 + d;
-          const size_t e1 = e0 + (size_t)p.H * p.S_max * 128;
-          void* base = which ? p.vcache : p.kcache;
-          if (p.kv_fp32) {
-            float* c = reinterpret_cast<float*>(base);
-            c[e0] = a00;
-            c[e0 + 1] = a10;
-            c[e1] = a01;
-            c[e1 + 1] = a11;
-          } else {
-            __nv_bfloat16* c = reinterpret_cast<__nv_bfloat16*>(base);
-            *reinterpret_cast<__nv_bfloat162*>(c + e0) = __floats2bfloat162_rn(a00, a10);
-            *reinterpret_cast<__nv_bfloat162*>(c + e1) = __floats2bfloat162_rn(a01, a11);
-          }
-        }
-      }
-    }
+    if (lane == 0) gemv_epilogue<EPI>(p, st, u, item, a00, a01, a10, a11);
   }
 }
 

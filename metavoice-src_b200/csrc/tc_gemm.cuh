@@ -38,12 +38,19 @@ struct GemmP {
   const int* row_cache;  // [R] cache row of each activation row
   const int* row_pos;    // [R] cache position of each activation row
   int H, S_max, D, kv_fp32;
+  // int8 weights (the widened q): bf16 [M] row scales of W (and W3), applied once per output after the (split-K) sum
+  const __nv_bfloat16* scale;
+  const __nv_bfloat16* scale3;
 };
 
 constexpr int GEMM_THREADS = 288;
 
-template <int EPI>
+template <int EPI, bool SCALED>
 __device__ __forceinline__ void gemm_apply(const GemmP& p, int n, int j, float y, float y3) {
+  if (SCALED) {
+    y *= bf16_to_f32(p.scale[j]);
+    if (EPI == G_SWIGLU) y3 *= bf16_to_f32(p.scale3[j]);
+  }
   if (EPI == G_STORE) {
     p.out[(size_t)n * p.ldo + j] = y;
   } else if (EPI == G_RESID) {
@@ -66,8 +73,10 @@ __device__ __forceinline__ void gemm_apply(const GemmP& p, int n, int j, float y
   }
 }
 
-// NC = n8 column chunks the accumulator holds (>= Rpad / 8; the chunks past Rpad / 8 are skipped at run time)
-template <int EPI, int NC>
+// NC = n8 column chunks the accumulator holds (>= Rpad / 8; the chunks past Rpad / 8 are skipped at run time).
+// SCALED: int8 weights, p.scale (p.scale3) multiply each output row after the sum; a template flag, so that the bf16
+// instances compile exactly as without it.
+template <int EPI, int NC, bool SCALED>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA3,
           const __grid_constant__ CUtensorMap tmB, const GemmP p) {
@@ -110,7 +119,7 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         const int n = 8 * c + n0 + (e & 1), j = tile * 128 + rl0 + 8 * (e >> 1);
-        if (c < nc && n < p.R && j < p.M) gemm_apply<EPI>(p, n, j, acc[0][c][e], acc[NA - 1][c][e]);
+        if (c < nc && n < p.R && j < p.M) gemm_apply<EPI, SCALED>(p, n, j, acc[0][c][e], acc[NA - 1][c][e]);
       }
     return;
   }
@@ -146,7 +155,7 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
         y += __ldcg(ps + (size_t)n * 128);
         if (NA == 2) y3 += __ldcg(ps + (size_t)(p.Rpad + n) * 128);
       }
-      if (j < p.M) gemm_apply<EPI>(p, n, j, y, y3);
+      if (j < p.M) gemm_apply<EPI, SCALED>(p, n, j, y, y3);
     }
   }
   asm volatile("bar.sync 1, 256;" ::: "memory");

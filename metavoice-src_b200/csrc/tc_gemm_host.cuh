@@ -118,6 +118,8 @@ struct TcGemm {
   unsigned* tickets;                              // [256] split-K counters, zero before the first launch
   int n_sm;                                       // SMs of the device
   int ksplit;                                     // > 0: force the K split (tests)
+  const __nv_bfloat16* scale;                     // int8 weights: bf16 [M] row scales of W, or null
+  const __nv_bfloat16* scale3;                    // G_SWIGLU: those of W3
 };
 cudaError_t tc_gemm(cudaStream_t s, const TcGemm& a);
 

@@ -97,8 +97,8 @@ class Transformer:
 
     def __init__(self, config: ModelArgs, arena: torch.Tensor, offsets: List[int], device="cuda",
                  quantisation_mode: Optional[str] = None):
-        if quantisation_mode not in (None, "int4"):
-            raise NotImplementedError(f"quantisation_mode={quantisation_mode!r} is not implemented (only None and 'int4')")
+        if quantisation_mode not in (None, "int4", "int8"):
+            raise NotImplementedError(f"quantisation_mode={quantisation_mode!r} is not implemented (only None, 'int4' and 'int8')")
         self.config = config
         self.quantisation_mode = quantisation_mode
         self.device = torch.device(device)
@@ -121,14 +121,19 @@ class Transformer:
     @classmethod
     def from_state_dict(cls, state_dict, config: ModelArgs, device="cuda", quantisation_mode: Optional[str] = None):
         """``quantisation_mode="int4"`` quantises wqkv / wo / w1 / w3 / w2 at load (mvb200/quantize.py) and builds an int4
-        engine: decode streams the packed weights through k_gemv_w4, prefill dequantises one layer at a time."""
+        engine: decode streams the packed weights through k_gemv_w4, prefill dequantises one layer at a time.
+        ``quantisation_mode="int8"`` quantises every Linear per output channel at load and builds an int8 engine: decode
+        streams the int8 weights through k_gemv_w8, prefill widens one layer's q at a time and scales the GEMM outputs."""
         if quantisation_mode == "int4":
             from .quantize import pack_arena_int4
             arena, offsets, _ = pack_arena_int4(state_dict, config.n_layer)
+        elif quantisation_mode == "int8":
+            from .quantize import pack_arena_int8
+            arena, offsets, _ = pack_arena_int8(state_dict, config.n_layer)
         elif quantisation_mode is None:
             arena, offsets = pack_arena(state_dict, config.n_layer)
         else:
-            raise NotImplementedError(f"quantisation_mode={quantisation_mode!r} is not implemented (only None and 'int4')")
+            raise NotImplementedError(f"quantisation_mode={quantisation_mode!r} is not implemented (only None, 'int4' and 'int8')")
         return cls(config, arena, offsets, device, quantisation_mode)
 
     @staticmethod
@@ -146,11 +151,22 @@ class Transformer:
         rest = 2 * c.vocab_size * c.dim + c.block_size * c.dim + c.speaker_emb_dim * c.dim + c.dim
         return c.n_layer * per_layer + rest * 2
 
+    @staticmethod
+    def int8_model_size_bytes(c: ModelArgs) -> int:
+        """Bytes of the int8 arena's tensors == the reference's ``model_size`` of its int8 model: int8 weights plus one bf16
+        scale per output row for every Linear (the five layer matrices, speaker_cond_pos, lm_head), bf16 for the rest."""
+        D, F, V = c.dim, c.intermediate_size, c.vocab_size
+        per_layer = 4 * D * D + 3 * D * F + (3 * D + D + 2 * F + D) * 2 + 2 * D * 2
+        linear_rest = c.speaker_emb_dim * D + D * 2 + V * D + V * 2
+        return c.n_layer * per_layer + linear_rest + (V * D + c.block_size * D + D) * 2
+
     def model_size_bytes(self) -> int:
         """Σ numel*itemsize of parameters == the reference's ``model_size`` (utils:348) before caches; for an int4 engine
         the bytes its arena's tensors occupy, so that main()'s bandwidth figure counts the bytes actually read."""
         if self.quantisation_mode == "int4":
             return self.int4_model_size_bytes(self.config)
+        if self.quantisation_mode == "int8":
+            return self.int8_model_size_bytes(self.config)
         return self.bf16_model_size_bytes(self.config)
 
     def setup_spk_cond_mask(self):
@@ -189,9 +205,11 @@ class Transformer:
                             c.speaker_emb_dim, c.norm_eps, self.max_utts,
                             _lib.MVB_KV_FP32 if kv_dtype == "fp32" else _lib.MVB_KV_BF16, max_new or c.block_size, options)
         self._cfg = cfg
-        int4 = self.quantisation_mode == "int4"
+        workspace_bytes, create = {None: (self._lib.mvb_s1_workspace_bytes, self._lib.mvb_s1_create),
+                                   "int4": (self._lib.mvb_s1_int4_workspace_bytes, self._lib.mvb_s1_create_int4),
+                                   "int8": (self._lib.mvb_s1_int8_workspace_bytes, self._lib.mvb_s1_create_int8)}[self.quantisation_mode]
         kvb = self._lib.mvb_s1_kv_bytes(C.byref(cfg))
-        wsb = (self._lib.mvb_s1_int4_workspace_bytes if int4 else self._lib.mvb_s1_workspace_bytes)(C.byref(cfg))
+        wsb = workspace_bytes(C.byref(cfg))
         if kvb == 0 or wsb == 0:
             _lib.check(_lib.MVB_ERR_UNSUPPORTED)
         self._kv = torch.zeros(kvb, dtype=torch.uint8, device=self.device)
@@ -200,7 +218,6 @@ class Transformer:
         h = C.c_void_p()
         torch.cuda.synchronize(self.device)
         with torch.cuda.device(self.device):
-            create = self._lib.mvb_s1_create_int4 if int4 else self._lib.mvb_s1_create
             rc = create(C.byref(cfg), self._arena.data_ptr(), self._arena.numel(), offs, self._kv.data_ptr(),
                         self._ws.data_ptr(), C.byref(h))
         _lib.check(rc)

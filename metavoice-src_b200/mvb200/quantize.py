@@ -1,6 +1,7 @@
-"""Weight-only int4 quantisation of the stage-1 model (``quantisation_mode="int4"``, fast_inference_utils.py:297-306).
+"""Weight-only quantisation of the stage-1 model: int4 (``quantisation_mode="int4"``, fast_inference_utils.py:297-306) and
+int8 (``quantisation_mode="int8"``, fast_inference_utils.py:283-296).
 
-Semantics, defined once here and in include/mvb200.h ("int4 packed matrix"):
+int4 semantics, defined once here and in include/mvb200.h ("int4 packed matrix"):
 
 * Which tensors.  A Linear weight [out, in] is quantised when ``out % 8 == 0`` and ``in % 128 == 0`` (the rule of the
   reference's ``WeightOnlyInt4QuantHandler``, fast_quantize.py:270-299, with groupsize 128).  A Linear with
@@ -19,12 +20,29 @@ Semantics, defined once here and in include/mvb200.h ("int4 packed matrix"):
   (the reference's first rounding, which cancellation against z can make larger than an ulp of the result) plus one ulp of
   the result (tests/test_int4_quant.py).
 * Consequence.  An int4 engine computes the same function as a bf16 engine whose arena holds ``W_deq``.
+
+int8 semantics, defined once here and in include/mvb200.h ("int8 matrix"):
+
+* Which tensors.  Every ``nn.Linear`` of the stage-1 model, as the reference's ``WeightOnlyInt8QuantHandler`` walks
+  ``named_modules()`` (fast_quantize.py:151-170): wqkv, wo, w1, w3, w2 of every layer, speaker_cond_pos and lm_head.
+  Embeddings and norms stay bf16.
+* Quantiser.  The reference quantises the bf16 model, so ``w = fp32(bf16 weight)``; then in fp32
+  ``s32 = clamp(max(|min_row|, max_row) / 127.5, min=FLT_EPSILON)``, ``q = clamp(round_half_even(w / s32), -128, 127)``,
+  and the stored scale is ``s = bf16_rn(s32)``: q is computed with the fp32 scale, the function uses the bf16 one.
+  Bit-identical to the reference's ``dynamically_quantize_per_channel(w.float(), -128, 127, torch.int8)`` with the scales
+  cast to bf16 as ``create_quantized_state_dict`` does (pinned by tests/golden/int8_quant.npz).
+* Function.  ``WeightOnlyInt8Linear.forward`` is ``F.linear(x, q) * s``; every kernel computes ``y_j = s_j sum_k x_k q_jk``
+  with fp32 accumulation over the exact integer weights and the scale applied once per output after the whole sum.
+* Consequence.  Where every scale is a power of two, ``s q`` is exact in bf16 and an int8 engine computes the same function
+  as a bf16 engine whose arena holds ``W' = s q`` (``int8_dequantized_state_dict``).
 """
 from __future__ import annotations
 
 from typing import Dict, List, Tuple
 
 import torch
+
+from .fast_model import _GLOBAL_KEYS, _LAYER_KEYS
 
 GROUP = 128
 N_BIT = 4
@@ -128,11 +146,8 @@ def unpack_matrix(buf: torch.Tensor, M: int, K: int):
     return q, sz[..., 0].contiguous(), sz[..., 1].contiguous()
 
 
-# arena order == include/mvb200.h; which entries are Linear weights, and which of those the engine streams as int4
-_GLOBAL_KEYS = ["transformer.wtes.0.weight", "transformer.wpe.weight", "speaker_cond_pos.weight",
-                "transformer.ln_f.weight", "lm_heads.0.weight"]
-_LAYER_KEYS = ["ln_1.weight", "attn.c_attn.weight", "attn.c_proj.weight", "ln_2.weight",
-               "mlp.swiglu.w1.weight", "mlp.swiglu.w3.weight", "mlp.c_proj.weight"]
+# which entries of the arena (order: fast_model._GLOBAL_KEYS / _LAYER_KEYS) are Linear weights, and which of those the
+# int4 engine streams packed
 _GLOBAL_LINEAR = {2, 4}            # speaker_cond_pos, lm_head
 _LAYER_PACKED = {1, 2, 4, 5, 6}    # wqkv, wo, w1, w3, w2: int4 packed matrices read by k_gemv_w4 / k_w4_dequant
 
@@ -145,12 +160,29 @@ def _keys(n_layer: int) -> List[Tuple[str, bool, bool]]:
     return out
 
 
+def _strip(state_dict: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+    return {(k[len("_orig_mod."):] if k.startswith("_orig_mod.") else k): v for k, v in state_dict.items()}
+
+
+def _place(blobs: List[torch.Tensor]):
+    """uint8 blobs -> (arena, offsets): each blob at the next 256-byte boundary, in order."""
+    offsets: List[int] = []
+    total = 0
+    for b in blobs:
+        offsets.append(total)
+        total = (total + b.numel() + _ALIGN - 1) // _ALIGN * _ALIGN
+    arena = torch.zeros(total, dtype=torch.uint8)
+    for b, o in zip(blobs, offsets):
+        arena[o:o + b.numel()] = b
+    return arena, offsets
+
+
 def pack_arena_int4(state_dict: Dict[str, torch.Tensor], n_layer: int):
     """Checkpoint state dict -> (uint8 arena, byte offsets, bytes the arena's tensors occupy without padding).
     Per layer wqkv / wo / w1 / w3 / w2 become int4 packed matrices (the offset points at the nibble block); a quantised
     Linear the engine does not stream in int4 (speaker_cond_pos, and lm_head when its out % 8 == 0) is stored as W_deq in
     bf16, so it computes what the reference's int4 Linear computes; everything else is the bf16 tensor."""
-    sd = {(k[len("_orig_mod."):] if k.startswith("_orig_mod.") else k): v for k, v in state_dict.items()}
+    sd = _strip(state_dict)
     blobs: List[torch.Tensor] = []
     payload = 0
     for k, linear, packed in _keys(n_layer):
@@ -169,23 +201,94 @@ def pack_arena_int4(state_dict: Dict[str, torch.Tensor], n_layer: int):
             raise ValueError(f"{k}: the int4 engine streams this matrix packed, but out % 8 != 0")
         blobs.append(t.contiguous().reshape(-1).view(torch.uint8))
         payload += t.numel() * 2
-    offsets: List[int] = []
-    total = 0
-    for b in blobs:
-        offsets.append(total)
-        total = (total + b.numel() + _ALIGN - 1) // _ALIGN * _ALIGN
-    arena = torch.zeros(total, dtype=torch.uint8)
-    for b, o in zip(blobs, offsets):
-        arena[o:o + b.numel()] = b
+    arena, offsets = _place(blobs)
     return arena, offsets, payload
 
 
 def dequantized_state_dict(state_dict: Dict[str, torch.Tensor], n_layer: int) -> Dict[str, torch.Tensor]:
     """The checkpoint with every quantised Linear replaced by W_deq (bf16): the bf16 model an int4 engine equals."""
-    sd = {(k[len("_orig_mod."):] if k.startswith("_orig_mod.") else k): v for k, v in state_dict.items()}
+    sd = _strip(state_dict)
     out = dict(sd)
     for k, linear, _ in _keys(n_layer):
         t = sd[k]
         if linear and is_quantised(t.shape[0], t.shape[1], k):
             out[k] = dequantize(*group_quantize(t.to(torch.bfloat16)))
+    return out
+
+
+# ---- weight-only int8 -------------------------------------------------------------------------------------------------
+_FLT_EPS = torch.finfo(torch.float32).eps
+
+
+def quantize_per_channel(w: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """w [M, K] -> (q int8 [M, K], s bf16 [M]): the reference's dynamically_quantize_per_channel(bf16 w -> fp32, -128, 127)
+    with the scales cast to bf16 (fast_quantize.py:38-67, 160-162)."""
+    wf = w.detach().to("cpu", torch.bfloat16).float()
+    if torch.isnan(wf).any():
+        raise ValueError("cannot quantise a weight holding NaN")
+    lo, hi = torch.aminmax(wf, dim=1)
+    amax = torch.maximum(-torch.clamp(lo, max=0.0), torch.clamp(hi, min=0.0))
+    s32 = torch.clamp(amax / 127.5, min=_FLT_EPS)
+    q = torch.clamp(torch.round(wf / s32[:, None]), -128, 127).to(torch.int8)
+    return q, s32.to(torch.bfloat16)
+
+
+def dequantize_int8(q: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
+    """W' = bf16_rn(s q), bf16 [M, K] (s q is exact in fp32: 8 + 8 significant bits)."""
+    return (q.float() * s.float()[:, None]).to(torch.bfloat16)
+
+
+def int8_matrix_bytes(M: int, K: int) -> int:
+    """Bytes of one int8 matrix: int8 [M, K] padded to 256 bytes, then bf16 [M] scales."""
+    return (M * K + _ALIGN - 1) // _ALIGN * _ALIGN + 2 * M
+
+
+def pack_int8_matrix(q: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
+    """The int8 matrix of include/mvb200.h: int8 [M][K] row-major, then at the next 256-byte boundary bf16 [M] scales."""
+    M, K = q.shape
+    buf = torch.zeros(int8_matrix_bytes(M, K), dtype=torch.uint8)
+    buf[:M * K] = q.contiguous().reshape(-1).view(torch.uint8)
+    so = (M * K + _ALIGN - 1) // _ALIGN * _ALIGN
+    buf[so:] = s.contiguous().view(torch.uint8)
+    return buf
+
+
+def unpack_int8_matrix(buf: torch.Tensor, M: int, K: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Inverse of pack_int8_matrix: (q, s)."""
+    so = (M * K + _ALIGN - 1) // _ALIGN * _ALIGN
+    q = buf[:M * K].clone().view(torch.int8).reshape(M, K)
+    return q, buf[so:so + 2 * M].clone().view(torch.bfloat16)
+
+
+def pack_arena_int8(state_dict: Dict[str, torch.Tensor], n_layer: int):
+    """Checkpoint state dict -> (uint8 arena, byte offsets, payload bytes).  Every Linear weight is an int8 matrix (its
+    offset points at the int8 block); embeddings and norms are the bf16 tensors.  The payload is the reference's
+    ``model_size`` of the int8 model: int8 weights plus bf16 scales plus the bf16 tensors."""
+    sd = _strip(state_dict)
+    blobs: List[torch.Tensor] = []
+    payload = 0
+    for k, linear, _ in _keys(n_layer):
+        if k not in sd:
+            raise KeyError(f"checkpoint is missing {k}")
+        t = sd[k].detach()
+        if linear:
+            q, s = quantize_per_channel(t)
+            blobs.append(pack_int8_matrix(q, s))
+            payload += q.numel() + 2 * s.numel()
+        else:
+            t = t.to(torch.bfloat16)
+            blobs.append(t.contiguous().reshape(-1).view(torch.uint8))
+            payload += t.numel() * 2
+    arena, offsets = _place(blobs)
+    return arena, offsets, payload
+
+
+def int8_dequantized_state_dict(state_dict: Dict[str, torch.Tensor], n_layer: int) -> Dict[str, torch.Tensor]:
+    """The checkpoint with every Linear replaced by bf16_rn(s q): the bf16 model an int8 engine equals when every scale is
+    a power of two (and approximates to the rounding of s q otherwise)."""
+    sd = _strip(state_dict)
+    out = dict(sd)
+    for k, linear, _ in _keys(n_layer):
+        if linear:
+            out[k] = dequantize_int8(*quantize_per_channel(sd[k]))
     return out
