@@ -534,6 +534,49 @@ int mvb_spk_embed(mvb_spk* h, const float* d_wav, int32_t n_samples, const int32
 int mvb_spk_op_test(mvb_spk* h, int32_t op, const float* d_in, int32_t n_frames, const int32_t* starts, int32_t n_partials,
                     float* d_out, float* d_trace, void* stream);
 
+/* Batched speaker front-end: a file's waveform -> 16 kHz (mvb_resample_batch) -> silence trimmed (mvb_spk_trim_batch) ->
+ * embedded (mvb_spk_embed_batch).  Each call takes up to MVB_SPK_MAX_BATCH signals with their lengths in HOST arrays,
+ * validates everything before anything is launched (MVB_ERR_ARG / MVB_ERR_UNSUPPORTED, outputs untouched) and launches
+ * one kernel per stage for the whole batch; signal i is computed exactly as it is alone.  "Packed" means signal i's
+ * samples start at n_0 + ... + n_{i-1}. */
+#define MVB_SPK_MAX_BATCH 32
+/* Longest filter the resampler takes: 20 max(up, down) + 1 <= 16384 taps, i.e. max(up, down) <= 819 after reduction.
+ * Every standard rate from 8 to 96 kHz to 16 kHz fits (11.025 kHz: 640/441, 12,801 taps). */
+#define MVB_RESAMPLE_MAX_TAPS 16384
+/* == scipy.signal.resample_poly(x, up, down) with its defaults, per signal, in fp32 (fp32 products and sums).  up / down
+ * are reduced by their gcd.  The caller designs the filter in float64,
+ *   h = firwin(n_taps, 1 / max(up, down), window=("kaiser", 5.0)) * up,   n_taps = 20 max(up, down) + 1,
+ * and passes it in polyphase order: d_taps fp32 [up][P], P = ceil(n_taps / up), d_taps[r][q] = h[r + q up] (0 past the
+ * end).  Output j of a signal of n_in samples is sum_q h[r + q up] x[m - q] over 0 <= m - q < n_in, with
+ * t = j down + (n_taps - 1) / 2 (scipy's delay compensation), r = t mod up, m = t div up: q ascending, one fmaf chain
+ * from 0.  d_in packed fp32 with n_in (HOST int32 [n], each >= 1) -> d_out packed fp32, n_out_i = ceil(n_in_i up / down).
+ * When up == down the signals are copied (no kernel); d_taps and n_taps are then not read.  MVB_ERR_UNSUPPORTED when the
+ * filter would exceed MVB_RESAMPLE_MAX_TAPS; MVB_ERR_ARG for n_taps != 20 max(up, down) + 1. */
+int mvb_resample_batch(int32_t n, const float* d_in, const int32_t* n_in, int32_t up, int32_t down, const float* d_taps,
+                       int32_t n_taps, float* d_out, void* stream);
+/* Bytes of the batch workspace of mvb_spk_trim_batch / mvb_spk_embed_batch for at most max_batch (<= 32) signals of
+ * max_total_samples (<= INT32_MAX) 16 kHz samples in all; 0 on an invalid argument.  It holds max_batch +
+ * max_total_samples / hop mel frames, as many windows, and the trim's RMS frames.  Calls on one workspace must be ordered. */
+size_t mvb_spk_batch_workspace_bytes(const mvb_spk_config* cfg, int32_t max_batch, int64_t max_total_samples);
+/* == trim_silence / librosa.effects.trim(y, top_db) per signal: frames of 2048 samples centered every 512 (zero padded),
+ * RMS in fp32, ref = the signal's loudest frame; kept are the frames with 20 log10(max(rms, 1e-10) / ref) > -top_db,
+ * evaluated as max(rms, 1e-10) / ref > 10^(-top_db / 20) with the threshold rounded to fp32 once.
+ * d_wav packed fp32 with n_samples (HOST int32 [n], each >= 1, sum <= max_total_samples) -> d_spans int32 [n][2]:
+ * {first kept frame * 512, min(n_i, (last kept frame + 1) * 512)}, {0, 0} when nothing is kept (an all-zero signal).
+ * top_db must be finite and > 0. */
+int mvb_spk_trim_batch(mvb_spk* h, int32_t n, const float* d_wav, const int32_t* n_samples, float top_db, void* d_batch_ws,
+                       int32_t max_batch, int64_t max_total_samples, int32_t* d_spans, void* stream);
+/* Batched SpeakerEncoder.embed_utterance: utterance i is the n_wav_i (>= 0) samples at d_wav + wav_off_i (HOST int64 [n],
+ * so trimmed spans are read in place), zero-extended to max(n_wav_i, (last start + partial_frames) * hop) samples as
+ * embed_utterance pads it; that length must be <= max_samples, and the padded lengths sum to <= max_total_samples.
+ * Its n_partials_i (HOST int32 [n], >= 1) window starts follow those of utterance i - 1 in `starts` (HOST int32, flat),
+ * each >= 0; at most max_batch + max_total_samples / hop windows in all.  d_embed fp32 [n, 256]; d_partials_out
+ * optional fp32 [sum n_partials, 256] in the same order.  Utterance i is bit-identical to mvb_spk_embed on its padded
+ * waveform alone: one k_spk_mel launch over all utterances, one k_spk_lstm over all windows, one k_spk_mean. */
+int mvb_spk_embed_batch(mvb_spk* h, int32_t n, const float* d_wav, const int64_t* wav_off, const int32_t* n_wav,
+                        const int32_t* starts, const int32_t* n_partials, void* d_batch_ws, int32_t max_batch,
+                        int64_t max_total_samples, float* d_embed, float* d_partials_out, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Audio post-processing on the device (SURVEY.md row N2) == `_save_audio` (fam/llm/decoders.py:40-47 -> audiocraft
  * audio_write(strategy="loudness", loudness_compressor=True)): BS.1770-4 integrated loudness exactly as

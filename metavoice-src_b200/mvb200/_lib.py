@@ -15,6 +15,7 @@ GLOBAL_TENSORS, LAYER_TENSORS = 5, 7
 MVB_S1_NO_ROWS_PATH, MVB_S1_NO_RESIDENT, MVB_S1_UNFUSED_SAMPLER, MVB_S1_TRACE = 0x1, 0x2, 0x4, 0x8
 MVB_S2_EAGER = 0x1
 MVB_MBD_CUDA_CORES, MVB_MBD_ONE_STREAM = 0x1, 0x2
+SPK_MAX_BATCH, RESAMPLE_MAX_TAPS = 32, 16384      # MVB_SPK_MAX_BATCH, MVB_RESAMPLE_MAX_TAPS
 
 
 class S1Config(C.Structure):
@@ -129,6 +130,13 @@ SIGNATURES = {
     "mvb_spk_destroy": (C.c_int, [C.c_void_p]),
     "mvb_spk_mel": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "mvb_spk_embed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "mvb_resample_batch": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
+                                     C.c_void_p]),
+    "mvb_spk_batch_workspace_bytes": (C.c_size_t, [C.POINTER(SpkConfig), C.c_int32, C.c_int64]),
+    "mvb_spk_trim_batch": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_int32, C.c_int64,
+                                     C.c_void_p, C.c_void_p]),
+    "mvb_spk_embed_batch": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "mvb_audio_post_workspace_bytes": (C.c_size_t, [C.c_int32]),
     "mvb_audio_post": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p, C.c_void_p]),

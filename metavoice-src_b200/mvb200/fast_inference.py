@@ -176,6 +176,19 @@ class TTS:
         print(f"\nSaved audio to {path} ({len(chunks)} chunks, {wav.shape[-1] / 24000.0:.1f} s of audio in {dt:.2f} s)")
         return path
 
+    def embed_speakers(self, spk_ref_paths: List[str]) -> torch.Tensor:
+        """One speaker embedding per reference -> fp32 [n, 256] on the CPU in input order: ``.pt`` / ``.npy`` files load
+        as ``synthesise`` loads them, and every audio file goes through ``get_cached_embeddings`` (the same disk cache,
+        with all misses embedded in one batched front-end pass on the device).  A serving loop can embed the
+        references of a batch this way and pass the embeddings on as ``.pt`` files."""
+        from .speaker_encoder import get_cached_embeddings
+        audio = [p for p in spk_ref_paths if not p.endswith((".pt", ".npy"))]
+        if audio and self.smodel is None:
+            raise FileNotFoundError("speaker_encoder.pt not found in the model directory: pass a precomputed embedding (.pt / .npy)")
+        rows = dict(zip(audio, get_cached_embeddings(audio, self.smodel))) if audio else {}
+        out = [rows[p].reshape(1, -1).float() if p in rows else load_speaker_embedding(p) for p in spk_ref_paths]
+        return torch.cat(out) if out else torch.empty((0, 256))
+
     def synthesise_batch(self, texts: List[str], spk_ref_paths: List[str], top_p=0.95, guidance_scale=3.0, temperature=1.0,
                          seed: Optional[int] = None) -> List[Optional[str]]:
         """N texts with N speaker references in one batch, one wav file per text, returned in input order (the reference's

@@ -3,8 +3,11 @@
 Same constructor keywords, ``embed_utterance`` / ``embed_utterance_from_file`` / ``compute_partial_slices`` contract and
 ``speaker_encoder.pt`` layout (``{"model_state": {lstm.*, linear.*}}``, model.py:45-46).  The mel front-end, the 3-layer
 LSTM, the projection and the partial-window averaging run on the device (csrc/speaker.cu); reading / resampling /
-trimming the reference file stays on the host (the reference uses librosa for those: librosa.load at 16 kHz +
-librosa.effects.trim(top_db=20), model.py:112-113 -- restated here with scipy's polyphase resampler, not pinned).
+trimming the reference file stays on the host in ``embed_utterance_from_file`` (the reference uses librosa for those:
+librosa.load at 16 kHz + librosa.effects.trim(top_db=20), model.py:112-113 -- restated here with scipy's polyphase
+resampler, not pinned).  ``embed_files`` runs the whole front-end for a batch of files on the device: the same polyphase
+filter in fp32 (``mvb_resample_batch``), the same trim (``mvb_spk_trim_batch``) and one embedding launch set
+(``mvb_spk_embed_batch``).
 """
 from __future__ import annotations
 
@@ -12,7 +15,8 @@ import ctypes as C
 import hashlib
 import os
 import struct
-from typing import Dict, Optional, Union
+from math import gcd
+from typing import Dict, List, Optional, Sequence, Union
 
 import numpy as np
 import torch
@@ -98,6 +102,30 @@ def resample(x: np.ndarray, sr_in: int, sr_out: int) -> np.ndarray:
     return resample_poly(x.astype(np.float64), sr_out // g, sr_in // g).astype(np.float32)
 
 
+def resample_ratio(sr_in: int, sr_out: int):
+    """(up, down) = (sr_out, sr_in) reduced by their gcd, as resample_poly reduces them."""
+    g = gcd(sr_in, sr_out)
+    return sr_out // g, sr_in // g
+
+
+def resample_taps(up: int, down: int) -> np.ndarray:
+    """float64 filter of scipy.signal.resample_poly(x, up, down) with its defaults: a Kaiser(5) windowed sinc of
+    20 max(up, down) + 1 taps at cutoff 1 / max(up, down), times up."""
+    from scipy.signal import firwin
+    m = max(up, down)
+    return firwin(20 * m + 1, 1.0 / m, window=("kaiser", 5.0)) * up
+
+
+def polyphase(h: np.ndarray, up: int) -> np.ndarray:
+    """h -> [up, ceil(len(h) / up)] with row r = h[r], h[r + up], ... (zero past the end): mvb_resample_batch's order."""
+    P = -(-h.size // up)
+    return np.concatenate([h, np.zeros(up * P - h.size, h.dtype)]).reshape(P, up).T.copy()
+
+
+def resampled_length(n: int, up: int, down: int) -> int:
+    return -(-n * up // down)
+
+
 def trim_silence(y: np.ndarray, top_db: float = 20.0, frame_length: int = 2048, hop_length: int = 512) -> np.ndarray:
     """librosa.effects.trim(y, top_db): keep the span between the first and last frame whose RMS is within top_db of the
     loudest frame (centered frames, zero padded)."""
@@ -162,6 +190,11 @@ class SpeakerEncoder:
             _lib.check(self._lib.mvb_spk_create(C.byref(cfg), self._arena.data_ptr(), self._arena.numel(),
                                                 (C.c_uint64 * len(offs))(*offs), self._ws.data_ptr(), C.byref(h)))
         self._h = h
+        # batch front-end: filters per (up, down) on the device, and a workspace for MVB_SPK_MAX_BATCH utterances of up
+        # to twice the longest single one, allocated on first use
+        self._taps: Dict[tuple, torch.Tensor] = {}
+        self.batch_max, self.batch_samples = _lib.SPK_MAX_BATCH, 2 * cfg.max_samples
+        self._batch_ws: Optional[torch.Tensor] = None
         if verbose:
             print(f"Loaded the speaker embedding model on {self.device.type}.")
 
@@ -220,6 +253,131 @@ class SpeakerEncoder:
             return embed_o, partials_o, wav_slices
         return embed_o
 
+    def _batch_workspace(self) -> torch.Tensor:
+        if self._batch_ws is None:
+            nb = self._lib.mvb_spk_batch_workspace_bytes(C.byref(self.cfg), self.batch_max, self.batch_samples)
+            if nb == 0:
+                _lib.check(_lib.MVB_ERR_ARG)
+            self._batch_ws = torch.empty(nb, dtype=torch.uint8, device=self.device)
+        return self._batch_ws
+
+    def _groups(self, lengths: Sequence[int]) -> List[List[int]]:
+        """Consecutive runs of indices that fit one batch call: at most batch_max of them, batch_samples in all."""
+        groups, cur, tot = [], [], 0
+        for i, n in enumerate(lengths):
+            if cur and (len(cur) == self.batch_max or tot + n > self.batch_samples):
+                groups.append(cur)
+                cur, tot = [], 0
+            cur.append(i)
+            tot += n
+        return groups + [cur] if cur else groups
+
+    def _embed_device(self, buf: torch.Tensor, offs: Sequence[int], lens: Sequence[int], rate, min_coverage):
+        """Utterance i = the lens[i] 16 kHz samples of the device buffer buf at offs[i] -> embeddings [n, 256] and
+        partials [sum windows, 256] on the device, and each utterance's wav slices."""
+        for n in lens:
+            if n > self.max_input_samples:
+                raise ValueError(f"speaker reference longer than {self.max_input_samples / sampling_rate:g} s")
+        plans = [self.compute_partial_slices(n, rate, min_coverage) for n in lens]
+        padded = [max(n, ws[-1].stop) for n, (ws, _) in zip(lens, plans)]
+        n_win = [len(ms) for _, ms in plans]
+        first_win = np.concatenate([[0], np.cumsum(n_win)]).astype(np.int64)
+        embeds = torch.empty((len(lens), model_embedding_size), dtype=torch.float32, device=self.device)
+        partials = torch.empty((int(first_win[-1]), model_embedding_size), dtype=torch.float32, device=self.device)
+        ws = self._batch_workspace()
+        for g in self._groups(padded):
+            starts = np.ascontiguousarray(np.concatenate([[s.start for s in plans[i][1]] for i in g]), dtype=np.int32)
+            off = np.ascontiguousarray([offs[i] for i in g], dtype=np.int64)
+            nw = np.ascontiguousarray([lens[i] for i in g], dtype=np.int32)
+            npart = np.ascontiguousarray([n_win[i] for i in g], dtype=np.int32)
+            ptr = lambda a: a.ctypes.data_as(C.c_void_p)
+            _lib.check(self._lib.mvb_spk_embed_batch(
+                self._h, len(g), buf.data_ptr(), ptr(off), ptr(nw), ptr(starts), ptr(npart), ws.data_ptr(), self.batch_max,
+                self.batch_samples, embeds[g[0]].data_ptr(), partials[int(first_win[g[0]])].data_ptr(), self._st()))
+        return embeds, partials, first_win, [ws_ for ws_, _ in plans]
+
+    @torch.no_grad()
+    def embed_utterance_batch(self, wavs: Sequence[np.ndarray], rate=1.3, min_coverage=0.75, return_partials=False):
+        """embed_utterance over a list of 16 kHz waveforms: fp32 [n, 256], row i bit-identical to embed_utterance(wavs[i]);
+        with return_partials also each utterance's partial embeddings and wav slices."""
+        lens = [len(w) for w in wavs]
+        host = np.concatenate([np.asarray(w, dtype=np.float32).reshape(-1) for w in wavs] + [np.zeros(1, np.float32)])
+        buf = torch.from_numpy(host).to(self.device)
+        offs = np.concatenate([[0], np.cumsum(lens)[:-1]]).tolist()
+        embeds, partials, first, slices = self._embed_device(buf, offs, lens, rate, min_coverage)
+        embeds = embeds.cpu().numpy()
+        if not return_partials:
+            return embeds
+        partials = partials.cpu().numpy()
+        return embeds, [partials[first[i]:first[i + 1]] for i in range(len(lens))], slices
+
+    def _resample_filter(self, up: int, down: int) -> torch.Tensor:
+        if (up, down) not in self._taps:
+            self._taps[(up, down)] = torch.from_numpy(polyphase(resample_taps(up, down), up).astype(np.float32)).to(self.device)
+        return self._taps[(up, down)]
+
+    @torch.no_grad()
+    def embed_files(self, paths: Sequence[str], min_seconds: float = 30.0) -> torch.Tensor:
+        """embed_utterance_from_file for a list of RIFF/WAVE files with the front-end on the device: each file is read and
+        mixed to mono on the host, resampled to 16 kHz (one launch per input rate and 32 files), trimmed and embedded in
+        batches.  Returns fp32 [n, 256] on the device in input order.  A file shorter than ``min_seconds`` (the 30 s of
+        check_audio_file), at a rate whose resampling filter exceeds MVB_RESAMPLE_MAX_TAPS, or longer than max_seconds
+        once resampled (before trimming) raises an error that names it, before anything runs on the device."""
+        sigs = []
+        for p in paths:
+            x, sr = read_wav(p)
+            if x.size / sr < min_seconds:
+                raise Exception(f"{p}: The audio file is too short. Please provide an audio file that is at least "
+                                f"{min_seconds} seconds long to proceed.")
+            up, down = resample_ratio(sr, sampling_rate)
+            if up != down and 20 * max(up, down) + 1 > _lib.RESAMPLE_MAX_TAPS:
+                raise ValueError(f"{p}: resampling {sr} Hz to {sampling_rate} Hz ({up}/{down}) needs a filter longer than "
+                                 f"{_lib.RESAMPLE_MAX_TAPS} taps")
+            n16 = resampled_length(x.size, up, down)
+            if n16 > self.max_input_samples:
+                raise ValueError(f"{p}: speaker reference longer than {self.max_input_samples / sampling_rate:g} s")
+            sigs.append((x, up, down, n16))
+        if not sigs:
+            return torch.empty((0, model_embedding_size), dtype=torch.float32, device=self.device)
+        # the 16 kHz buffer holds the files grouped by rate, so that each rate's outputs are packed
+        order = sorted(range(len(sigs)), key=lambda i: (sigs[i][1], sigs[i][2]))
+        lens = [sigs[i][3] for i in order]
+        offs = np.concatenate([[0], np.cumsum(lens)[:-1]]).astype(np.int64).tolist()
+        buf = torch.empty(sum(lens), dtype=torch.float32, device=self.device)
+        k = 0
+        while k < len(order):
+            _, up, down, _ = sigs[order[k]]
+            e = k
+            while e < len(order) and sigs[order[e]][1:3] == (up, down):
+                e += 1
+            host = np.concatenate([sigs[i][0] for i in order[k:e]])
+            if up == down:
+                buf[offs[k]:offs[k] + host.size].copy_(torch.from_numpy(host))
+            else:
+                x = torch.from_numpy(host).to(self.device)
+                taps = self._resample_filter(up, down)
+                n_in = [sigs[i][0].size for i in order[k:e]]
+                x_off = np.concatenate([[0], np.cumsum(n_in)]).astype(np.int64)
+                for c in range(0, e - k, self.batch_max):
+                    chunk = np.ascontiguousarray(n_in[c:c + self.batch_max], dtype=np.int32)
+                    _lib.check(self._lib.mvb_resample_batch(
+                        len(chunk), x[int(x_off[c]):].data_ptr(), chunk.ctypes.data_as(C.c_void_p), up, down, taps.data_ptr(),
+                        20 * max(up, down) + 1, buf[offs[k + c]:].data_ptr(), self._st()))
+            k = e
+        spans = torch.empty((len(lens), 2), dtype=torch.int32, device=self.device)
+        ws = self._batch_workspace()
+        for g in self._groups(lens):
+            n = np.ascontiguousarray([lens[i] for i in g], dtype=np.int32)
+            _lib.check(self._lib.mvb_spk_trim_batch(self._h, len(g), buf[offs[g[0]]:].data_ptr(), n.ctypes.data_as(C.c_void_p),
+                                                    20.0, ws.data_ptr(), self.batch_max, self.batch_samples,
+                                                    spans[g[0]].data_ptr(), self._st()))
+        spans = spans.cpu().numpy()                           # one copy: compute_partial_slices needs the trimmed lengths
+        embeds, _, _, _ = self._embed_device(buf, [o + int(b) for o, (b, _) in zip(offs, spans)],
+                                             [int(e - b) for b, e in spans], 1.3, 0.75)
+        out = torch.empty_like(embeds)
+        out[torch.as_tensor(order, device=self.device)] = embeds
+        return out
+
     def embed_utterance_from_file(self, fpath: str, numpy: bool) -> torch.Tensor:
         wav, sr = read_wav(fpath)                             # librosa.load(fpath, sr=16000)
         wav = trim_silence(resample(wav, sr, sampling_rate), top_db=20)
@@ -233,16 +391,44 @@ def check_audio_file(path: str, threshold_s: float = 30.0):
         raise Exception(f"The audio file is too short. Please provide an audio file that is at least {threshold_s} seconds long to proceed.")
 
 
+def _embedding_cache_path(local_file_path: str) -> str:
+    name = "embedding_" + hashlib.md5(local_file_path.encode("utf-8")).hexdigest() + ".pt"
+    os.makedirs(os.path.expanduser("~/.cache/fam/"), exist_ok=True)
+    return os.path.expanduser(f"~/.cache/fam/{name}")
+
+
 def get_cached_embedding(local_file_path: str, spkemb_model: SpeakerEncoder) -> torch.Tensor:
     """fam/llm/inference.py:419-435: disk cache ~/.cache/fam/embedding_<md5(path)>.pt keyed by the path string."""
     if not os.path.exists(local_file_path):
         raise FileNotFoundError(f"File {local_file_path} not found!")
-    name = "embedding_" + hashlib.md5(local_file_path.encode("utf-8")).hexdigest() + ".pt"
-    os.makedirs(os.path.expanduser("~/.cache/fam/"), exist_ok=True)
-    cache_path = os.path.expanduser(f"~/.cache/fam/{name}")
+    cache_path = _embedding_cache_path(local_file_path)
     if not os.path.exists(cache_path):
         spk_emb = spkemb_model.embed_utterance_from_file(local_file_path, numpy=False).unsqueeze(0).cpu()
         torch.save(spk_emb, cache_path)
     else:
         spk_emb = torch.load(cache_path, map_location="cpu")
     return spk_emb
+
+
+def get_cached_embeddings(paths: Sequence[str], spkemb_model: SpeakerEncoder) -> torch.Tensor:
+    """get_cached_embedding for a list of files -> fp32 [n, 256] on the CPU in input order, with the same cache files:
+    hits are read from disk, and every miss is embedded in one SpeakerEncoder.embed_files call and written back."""
+    for p in paths:
+        if not os.path.exists(p):
+            raise FileNotFoundError(f"File {p} not found!")
+    out: Dict[str, torch.Tensor] = {}
+    misses = []
+    for p in paths:
+        if p in out or p in misses:
+            continue
+        cache_path = _embedding_cache_path(p)
+        if os.path.exists(cache_path):
+            out[p] = torch.load(cache_path, map_location="cpu").reshape(1, -1)
+        else:
+            misses.append(p)
+    if misses:
+        embeds = spkemb_model.embed_files(misses).cpu()
+        for p, e in zip(misses, embeds):
+            out[p] = e.unsqueeze(0).clone()
+            torch.save(out[p], _embedding_cache_path(p))
+    return torch.cat([out[p] for p in paths]).float() if paths else torch.empty((0, model_embedding_size))
