@@ -111,6 +111,7 @@ def _post_batch(wavs, sample_rate: int, loudness_headroom_db: float, loudness_co
     signal], LKFS [n], gain [n])."""
     import ctypes as C
     from . import _lib
+    from ._engine import current_stream
     lib = _lib.load()
     ws_ = [w.detach().reshape(-1).to(torch.float32) for w in wavs]
     dev = ws_[0].device
@@ -125,10 +126,9 @@ def _post_batch(wavs, sample_rate: int, loudness_headroom_db: float, loudness_co
     flat = torch.cat(ws_) if n > 1 else ws_[0].contiguous()   # one signal (wav_bytes_on_device): no device copy
     pcm = torch.empty(total, dtype=torch.int16, device=dev)
     stats = torch.empty(n, 2, dtype=torch.float32, device=dev)
-    st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
     _lib.check(lib.mvb_audio_post_batch(flat.data_ptr(), n, (C.c_int32 * n)(*lens), int(sample_rate), float(loudness_headroom_db),
                                         int(bool(loudness_compressor)), cap[2].data_ptr(), cap[0], cap[1], pcm.data_ptr(), None,
-                                        stats.data_ptr(), st))
+                                        stats.data_ptr(), current_stream(dev)))
     stats = stats.cpu().tolist()
     pcm = pcm.cpu().numpy().astype("<i2", copy=False)
     out, pos = [], 0

@@ -7,15 +7,13 @@ Same names and call signatures as the reference (``ModelArgs``, ``Transformer.fr
 """
 from __future__ import annotations
 
-import ctypes as C
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Union
 
 import torch
 
 from . import _lib
-
-_ALIGN = 256  # byte alignment of every tensor inside the weight arena (TMA needs >= 128)
+from ._engine import Engine, pack_arena_bytes
 
 
 def find_multiple(n: int, k: int) -> int:
@@ -70,18 +68,10 @@ def pack_arena(state_dict: Dict[str, torch.Tensor], n_layer: int):
     keys = list(_GLOBAL_KEYS)
     for i in range(n_layer):
         keys += [f"transformer.h.{i}.{k}" for k in _LAYER_KEYS]
-    offsets: List[int] = []
-    total = 0
     for k in keys:
         if k not in sd:
             raise KeyError(f"checkpoint is missing {k}")
-        offsets.append(total)
-        total = (total + sd[k].numel() * 2 + _ALIGN - 1) // _ALIGN * _ALIGN
-    arena = torch.zeros(total, dtype=torch.uint8)
-    for k, o in zip(keys, offsets):
-        t = sd[k].detach().to(torch.bfloat16).contiguous().reshape(-1)
-        arena[o:o + t.numel() * 2] = t.view(torch.uint8)
-    return arena, offsets
+    return pack_arena_bytes([sd[k].to(torch.bfloat16) for k in keys])
 
 
 class KVCache:
@@ -92,21 +82,16 @@ class KVCache:
         self.k_cache, self.v_cache = k_cache, v_cache
 
 
-class Transformer:
+class Transformer(Engine):
     """Mirror of fam/llm/fast_model.py:116-167 backed by an ``mvb_s1`` engine handle."""
 
     def __init__(self, config: ModelArgs, arena: torch.Tensor, offsets: List[int], device="cuda",
                  quantisation_mode: Optional[str] = None):
         if quantisation_mode not in (None, "int4", "int8"):
             raise NotImplementedError(f"quantisation_mode={quantisation_mode!r} is not implemented (only None, 'int4' and 'int8')")
+        super().__init__(device, arena, offsets)
         self.config = config
         self.quantisation_mode = quantisation_mode
-        self.device = torch.device(device)
-        self._lib = _lib.load()
-        self._arena = arena.to(self.device) if arena.device != self.device else arena
-        self._offsets = list(offsets)
-        self._handle = None
-        self._kv = self._ws = None
         self.max_batch_size = -1
         self.max_seq_length = -1
         self.max_utts = 0
@@ -183,7 +168,7 @@ class Transformer:
             path without the resident decode kernel, "C" = resident decode kernel with CUDA-core prefill;
           ``unfused_sampler``: the resident kernel leaves the logits to k_sample;
           ``trace``: the resident kernel records per-phase clocks for mvb_s1_trace_fetch."""
-        if (self._handle is not None and self.max_seq_length >= max_seq_length and self.max_batch_size >= max_batch_size
+        if (self._h is not None and self.max_seq_length >= max_seq_length and self.max_batch_size >= max_batch_size
                 and kv_dtype == self.kv_dtype and tensor_core_path is None and unfused_sampler is None and trace is None):
             return
         c = self.config
@@ -208,42 +193,22 @@ class Transformer:
         workspace_bytes, create = {None: (self._lib.mvb_s1_workspace_bytes, self._lib.mvb_s1_create),
                                    "int4": (self._lib.mvb_s1_int4_workspace_bytes, self._lib.mvb_s1_create_int4),
                                    "int8": (self._lib.mvb_s1_int8_workspace_bytes, self._lib.mvb_s1_create_int8)}[self.quantisation_mode]
-        kvb = self._lib.mvb_s1_kv_bytes(C.byref(cfg))
-        wsb = workspace_bytes(C.byref(cfg))
-        if kvb == 0 or wsb == 0:
-            _lib.check(_lib.MVB_ERR_UNSUPPORTED)
-        self._kv = torch.zeros(kvb, dtype=torch.uint8, device=self.device)
-        self._ws = torch.zeros(wsb, dtype=torch.uint8, device=self.device)
-        offs = (C.c_uint64 * len(self._offsets))(*self._offsets)
-        h = C.c_void_p()
-        torch.cuda.synchronize(self.device)
-        with torch.cuda.device(self.device):
-            rc = create(C.byref(cfg), self._arena.data_ptr(), self._arena.numel(), offs, self._kv.data_ptr(),
-                        self._ws.data_ptr(), C.byref(h))
-        _lib.check(rc)
-        self._handle = h
+        self._create(create, self._lib.mvb_s1_destroy, cfg, self._lib.mvb_s1_kv_bytes, workspace_bytes)
         self._spk_key = None
-
-    def close(self):
-        if self._handle is not None:
-            self._lib.mvb_s1_destroy(self._handle)
-            self._handle = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     # ---- helpers --------------------------------------------------------------------------------
     @property
     def handle(self):
-        if self._handle is None:
+        if self._h is None:
             raise RuntimeError("call setup_caches() first")
-        return self._handle
+        return self._h
 
-    def _stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+    @property
+    def _kv(self):
+        """The KV cache: the first device buffer the handle is created over."""
+        return self._ws[0]
+
+    _stream = Engine._st
 
     def set_speaker(self, utt: int, spk_emb: torch.Tensor):
         e = spk_emb.detach().reshape(-1).to(device=self.device, dtype=torch.float32).contiguous()

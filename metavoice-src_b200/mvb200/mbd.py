@@ -5,7 +5,6 @@ follows audiocraft's module names (``models`` = one ``DiffusionUnet`` state dict
 ``MultiBandProcessor`` statistics)."""
 from __future__ import annotations
 
-import ctypes as C
 import math
 from dataclasses import dataclass, field
 from typing import List, Optional
@@ -13,6 +12,7 @@ from typing import List, Optional
 import torch
 
 from . import _lib
+from ._engine import Engine, pack_arena_bytes
 
 
 @dataclass
@@ -104,12 +104,12 @@ def _schedule_table(s: ScheduleSettings, steps: List[int]) -> torch.Tensor:
 _RES = ["norm1.weight", "norm1.bias", "conv1.weight", "conv1.bias", "norm2.weight", "norm2.bias", "conv2.weight", "conv2.bias"]
 
 
-class MultiBandDiffusionEngine:
+class MultiBandDiffusionEngine(Engine):
     def __init__(self, checkpoint: dict, settings: MBDSettings, device="cuda", max_seconds: float = 12.0,
                  tensor_cores: bool = True, band_streams: bool = True):
         """``tensor_cores=False`` (test hook): every convolution on the fp32 CUDA-core kernels; ``band_streams=False``: the
         band models back to back on the caller's stream instead of one stream each."""
-        self.s, self.device = settings, torch.device(device)
+        self.s = settings
         u = settings.unet
         tensors = []
         for sd, pr in zip(checkpoint["models"], checkpoint["proc"]):
@@ -136,29 +136,14 @@ class MultiBandDiffusionEngine:
         bank_e = _lowpass_bank(settings.eq_bands, settings.sample_rate)
         sched = _schedule_table(settings.schedule, settings.steps())
         tensors += [bank_p, bank_e, sched]
-        offs, total = [], 0
-        for t in tensors:
-            offs.append(total)
-            total = (total + t.numel() * 4 + 255) // 256 * 256
-        arena = torch.zeros(total, dtype=torch.uint8)
-        for t, o in zip(tensors, offs):
-            arena[o:o + t.numel() * 4] = t.contiguous().reshape(-1).view(torch.uint8)
-        self._arena = arena.to(self.device)
+        super().__init__(device, *pack_arena_bytes(tensors))
         cfg = _lib.MbdConfig(settings.n_models, u.chin, u.hidden, u.depth, u.res_blocks, u.norm_groups, u.kernel, u.stride,
                              float(u.growth), int(u.emb_all_layers), u.codec_dim, u.num_steps, sched.shape[0],
                              float(settings.schedule.noise_scale), float(settings.schedule.clip), settings.proc_bands,
                              bank_p.shape[1], settings.eq_bands, bank_e.shape[1], int(max_seconds * settings.sample_rate),
                              (0 if tensor_cores else _lib.MVB_MBD_CUDA_CORES) | (0 if band_streams else _lib.MVB_MBD_ONE_STREAM))
-        self.cfg, self._lib = cfg, _lib.load()
-        wsb = self._lib.mvb_mbd_workspace_bytes(C.byref(cfg))
-        if wsb == 0:
-            _lib.check(_lib.MVB_ERR_UNSUPPORTED)
-        self._ws = torch.zeros(wsb, dtype=torch.uint8, device=self.device)
-        h = C.c_void_p()
-        with torch.cuda.device(self.device):
-            _lib.check(self._lib.mvb_mbd_create(C.byref(cfg), self._arena.data_ptr(), self._arena.numel(),
-                                                (C.c_uint64 * len(offs))(*offs), self._ws.data_ptr(), C.byref(h)))
-        self._h = h
+        self.cfg = cfg
+        self._create(self._lib.mvb_mbd_create, self._lib.mvb_mbd_destroy, cfg, self._lib.mvb_mbd_workspace_bytes)
         self.n_calls = sched.shape[0]
 
     def flops(self, n_samples: int, n_frames: int) -> float:
@@ -174,13 +159,6 @@ class MultiBandDiffusionEngine:
         per += 2.0 * u.codec_dim * ch[-1] * n_frames
         return per * self.s.n_models * (len(self.s.steps()) - 1)
 
-    def close(self):
-        if getattr(self, "_h", None) is not None:
-            self._lib.mvb_mbd_destroy(self._h)
-            self._h = None
-
-    __del__ = close
-
     @torch.no_grad()
     def tokens_to_wav(self, cond: torch.Tensor, wav_encodec: torch.Tensor, noise: Optional[torch.Tensor] = None, seed: int = 0) -> torch.Tensor:
         """cond fp32 [codec_dim, T_frames] (``decode_latent``), wav_encodec fp32 [T] (codec decode) -> refined wav fp32 [T].
@@ -192,7 +170,7 @@ class MultiBandDiffusionEngine:
             nz = noise.to(self.device, torch.float32).contiguous()
             assert nz.shape == (self.s.n_models, self.n_calls, w.numel()), nz.shape
         out = torch.empty_like(w)
-        st = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
         _lib.check(self._lib.mvb_mbd_tokens_to_wav(self._h, c.data_ptr(), c.shape[1], w.data_ptr(), w.numel(),
-                                                   None if nz is None else nz.data_ptr(), int(seed) & (2**64 - 1), out.data_ptr(), st))
+                                                   None if nz is None else nz.data_ptr(), int(seed) & (2**64 - 1), out.data_ptr(),
+                                                   self._st()))
         return out

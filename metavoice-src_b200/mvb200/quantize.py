@@ -42,11 +42,11 @@ from typing import Dict, List, Tuple
 
 import torch
 
+from ._engine import align_up, pack_arena_bytes
 from .fast_model import _GLOBAL_KEYS, _LAYER_KEYS
 
 GROUP = 128
 N_BIT = 4
-_ALIGN = 256
 
 
 def is_quantised(out_features: int, in_features: int, name: str = "") -> bool:
@@ -121,7 +121,7 @@ def unpack_nibbles(p: torch.Tensor) -> torch.Tensor:
 
 def packed_bytes(M: int, K: int) -> int:
     """Bytes of one packed matrix: the nibble block padded to 256 bytes, then the (scale, zero) block."""
-    return (M * K // 2 + _ALIGN - 1) // _ALIGN * _ALIGN + M * (K // GROUP) * 4
+    return align_up(M * K // 2) + M * (K // GROUP) * 4
 
 
 def pack_matrix(q: torch.Tensor, s: torch.Tensor, z: torch.Tensor) -> torch.Tensor:
@@ -132,7 +132,7 @@ def pack_matrix(q: torch.Tensor, s: torch.Tensor, z: torch.Tensor) -> torch.Tens
     nb = M * K // 2
     buf[:nb] = pack_nibbles(q).reshape(-1)
     sz = torch.stack([s, z], dim=-1).contiguous().reshape(-1)
-    so = (nb + _ALIGN - 1) // _ALIGN * _ALIGN
+    so = align_up(nb)
     buf[so:] = sz.view(torch.uint8)
     return buf
 
@@ -140,7 +140,7 @@ def pack_matrix(q: torch.Tensor, s: torch.Tensor, z: torch.Tensor) -> torch.Tens
 def unpack_matrix(buf: torch.Tensor, M: int, K: int):
     """Inverse of pack_matrix: (q, scales, zeros)."""
     nb = M * K // 2
-    so = (nb + _ALIGN - 1) // _ALIGN * _ALIGN
+    so = align_up(nb)
     q = unpack_nibbles(buf[:nb].reshape(M, K // 2))
     sz = buf[so:so + M * (K // GROUP) * 4].clone().view(torch.bfloat16).reshape(M, K // GROUP, 2)
     return q, sz[..., 0].contiguous(), sz[..., 1].contiguous()
@@ -162,19 +162,6 @@ def _keys(n_layer: int) -> List[Tuple[str, bool, bool]]:
 
 def _strip(state_dict: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
     return {(k[len("_orig_mod."):] if k.startswith("_orig_mod.") else k): v for k, v in state_dict.items()}
-
-
-def _place(blobs: List[torch.Tensor]):
-    """uint8 blobs -> (arena, offsets): each blob at the next 256-byte boundary, in order."""
-    offsets: List[int] = []
-    total = 0
-    for b in blobs:
-        offsets.append(total)
-        total = (total + b.numel() + _ALIGN - 1) // _ALIGN * _ALIGN
-    arena = torch.zeros(total, dtype=torch.uint8)
-    for b, o in zip(blobs, offsets):
-        arena[o:o + b.numel()] = b
-    return arena, offsets
 
 
 def pack_arena_int4(state_dict: Dict[str, torch.Tensor], n_layer: int):
@@ -199,9 +186,9 @@ def pack_arena_int4(state_dict: Dict[str, torch.Tensor], n_layer: int):
             t = dequantize(q, s, z)
         elif packed:
             raise ValueError(f"{k}: the int4 engine streams this matrix packed, but out % 8 != 0")
-        blobs.append(t.contiguous().reshape(-1).view(torch.uint8))
+        blobs.append(t)
         payload += t.numel() * 2
-    arena, offsets = _place(blobs)
+    arena, offsets = pack_arena_bytes(blobs)
     return arena, offsets, payload
 
 
@@ -240,7 +227,7 @@ def dequantize_int8(q: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
 
 def int8_matrix_bytes(M: int, K: int) -> int:
     """Bytes of one int8 matrix: int8 [M, K] padded to 256 bytes, then bf16 [M] scales."""
-    return (M * K + _ALIGN - 1) // _ALIGN * _ALIGN + 2 * M
+    return align_up(M * K) + 2 * M
 
 
 def pack_int8_matrix(q: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
@@ -248,14 +235,14 @@ def pack_int8_matrix(q: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
     M, K = q.shape
     buf = torch.zeros(int8_matrix_bytes(M, K), dtype=torch.uint8)
     buf[:M * K] = q.contiguous().reshape(-1).view(torch.uint8)
-    so = (M * K + _ALIGN - 1) // _ALIGN * _ALIGN
+    so = align_up(M * K)
     buf[so:] = s.contiguous().view(torch.uint8)
     return buf
 
 
 def unpack_int8_matrix(buf: torch.Tensor, M: int, K: int) -> Tuple[torch.Tensor, torch.Tensor]:
     """Inverse of pack_int8_matrix: (q, s)."""
-    so = (M * K + _ALIGN - 1) // _ALIGN * _ALIGN
+    so = align_up(M * K)
     q = buf[:M * K].clone().view(torch.int8).reshape(M, K)
     return q, buf[so:so + 2 * M].clone().view(torch.bfloat16)
 
@@ -277,9 +264,9 @@ def pack_arena_int8(state_dict: Dict[str, torch.Tensor], n_layer: int):
             payload += q.numel() + 2 * s.numel()
         else:
             t = t.to(torch.bfloat16)
-            blobs.append(t.contiguous().reshape(-1).view(torch.uint8))
+            blobs.append(t)
             payload += t.numel() * 2
-    arena, offsets = _place(blobs)
+    arena, offsets = pack_arena_bytes(blobs)
     return arena, offsets, payload
 
 

@@ -7,12 +7,12 @@ Token adapters (integer bucketing, SURVEY.md rows a12/a16) stay on the host exac
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import List, Optional, Sequence
 
 import torch
 
 from . import _lib
+from ._engine import Engine, pack_arena_bytes
 
 PAD = 1024  # _encodec_codes_pad_token (inference.py:125)
 
@@ -64,7 +64,7 @@ _LAYER = ["ln_1.weight", "attn.c_attn.weight", "attn.c_proj.weight", "ln_2.weigh
           "mlp.swiglu.w3.weight", "mlp.c_proj.weight"]
 
 
-class SecondStage:
+class SecondStage(Engine):
     def __init__(self, checkpoint: dict, device="cuda", max_batch: int = 1, tokenizer=None, cuda_graph: bool = True):
         """``checkpoint`` = the second_stage.pt dict (model / model_args / meta), as ``Model._init_model`` reads it.
         ``cuda_graph=False`` (test hook): launch the forward pass kernel by kernel instead of replaying a captured graph."""
@@ -77,18 +77,10 @@ class SecondStage:
             # model.py:104-107: the reference itself refuses a non-causal model with spk_emb_on_text=False
             raise NotImplementedError("spk_emb_on_text=False is not supported for the non-causal second stage (model.py:104-107)")
         sd = {(k[len("_orig_mod."):] if k.startswith("_orig_mod.") else k): v for k, v in checkpoint["model"].items()}
-        self.args, self.device = a, torch.device(device)
+        self.args = a
         self.n_in, self.n_out = len(a["vocab_sizes"]), len(a["target_vocab_sizes"])
         keys = _GLOBAL(self.n_in, self.n_out) + [f"transformer.h.{l}.{k}" for l in range(a["n_layer"]) for k in _LAYER]
-        offs, total = [], 0
-        for k in keys:
-            offs.append(total)
-            total = (total + sd[k].numel() * 2 + 255) // 256 * 256
-        arena = torch.zeros(total, dtype=torch.uint8)
-        for k, o in zip(keys, offs):
-            t = sd[k].detach().to(torch.bfloat16).contiguous().reshape(-1)
-            arena[o:o + t.numel() * 2] = t.view(torch.uint8)
-        self._arena = arena.to(self.device)
+        super().__init__(device, *pack_arena_bytes([sd[k].to(torch.bfloat16) for k in keys]))
         hidden = sd["transformer.h.0.mlp.swiglu.w1.weight"].shape[0]
         cfg = _lib.S2Config()
         cfg.n_layer, cfg.n_head, cfg.n_embd, cfg.hidden = a["n_layer"], a["n_head"], a["n_embd"], hidden
@@ -101,25 +93,10 @@ class SecondStage:
         cfg.norm_eps = a.get("rmsnorm_eps") or 1e-5
         cfg.max_batch = max_batch
         cfg.options = 0 if cuda_graph else _lib.MVB_S2_EAGER
-        self.cfg, self._lib = cfg, _lib.load()
-        wsb = self._lib.mvb_s2_workspace_bytes(C.byref(cfg))
-        if wsb == 0:
-            _lib.check(_lib.MVB_ERR_UNSUPPORTED)
-        self._ws = torch.zeros(wsb, dtype=torch.uint8, device=self.device)
-        h = C.c_void_p()
-        with torch.cuda.device(self.device):
-            _lib.check(self._lib.mvb_s2_create(C.byref(cfg), self._arena.data_ptr(), self._arena.numel(),
-                                               (C.c_uint64 * len(offs))(*offs), self._ws.data_ptr(), C.byref(h)))
-        self._h = h
+        self.cfg = cfg
+        self._create(self._lib.mvb_s2_create, self._lib.mvb_s2_destroy, cfg, self._lib.mvb_s2_workspace_bytes)
         self.tokenizer = tokenizer
         self.block_size = a["block_size"]
-
-    def close(self):
-        if getattr(self, "_h", None) is not None:
-            self._lib.mvb_s2_destroy(self._h)
-            self._h = None
-
-    __del__ = close
 
     # inference.py:283-301
     def build_input(self, text_ids: Sequence[int], codes: Sequence[Sequence[int]]) -> torch.Tensor:
@@ -138,10 +115,9 @@ class SecondStage:
         out = torch.empty((b, self.n_out, self.block_size), dtype=torch.int32, device=self.device)
         lg = torch.empty((self.n_out, b * self.block_size, V), dtype=torch.float32, device=self.device) if return_logits else None
         nz = None if noise is None else noise.to(self.device, torch.float32).contiguous()
-        st = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
         _lib.check(self._lib.mvb_s2_forward(self._h, b, idx_d.data_ptr(), None if spk_d is None else spk_d.data_ptr(),
                                             float(temperature), int(top_k or 0), None if nz is None else nz.data_ptr(),
-                                            int(seed), out.data_ptr(), None if lg is None else lg.data_ptr(), st))
+                                            int(seed), out.data_ptr(), None if lg is None else lg.data_ptr(), self._st()))
         return (out, lg) if return_logits else out
 
     @torch.no_grad()

@@ -22,6 +22,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from ._engine import Engine, pack_arena_bytes, split_runs
 
 mel_window_length = 25
 mel_window_step = 10
@@ -145,14 +146,13 @@ def trim_silence(y: np.ndarray, top_db: float = 20.0, frame_length: int = 2048, 
     return y[keep[0] * hop_length:min(y.size, (keep[-1] + 1) * hop_length)]
 
 
-class SpeakerEncoder:
+class SpeakerEncoder(Engine):
     """model.py:21-117 with the arithmetic in libmvb200."""
 
     def __init__(self, weights_fpath: Optional[str] = None, device: Optional[Union[str, torch.device]] = None, verbose: bool = True,
                  eval: bool = False, model_state: Optional[Dict[str, torch.Tensor]] = None, max_seconds: float = 180.0):
         if device is None:
             device = "cuda"
-        self.device = torch.device(device)
         if model_state is None:
             model_state = torch.load(weights_fpath, map_location="cpu", weights_only=False)["model_state"]
         g = lambda k: model_state[k].detach().float().contiguous()
@@ -167,29 +167,14 @@ class SpeakerEncoder:
                     torch.from_numpy((0.5 - 0.5 * np.cos(2 * np.pi * i / n_fft)).astype(np.float32)),     # periodic Hann
                     torch.from_numpy(np.cos(2 * np.pi * i / n_fft).astype(np.float32)),
                     torch.from_numpy((-np.sin(2 * np.pi * i / n_fft)).astype(np.float32))]
-        offs, total = [], 0
-        for t in tensors:
-            offs.append(total)
-            total = (total + t.numel() * 4 + 255) // 256 * 256
-        arena = torch.zeros(total, dtype=torch.uint8)
-        for t, o in zip(tensors, offs):
-            arena[o:o + t.numel() * 4] = t.contiguous().reshape(-1).view(torch.uint8)
-        self._arena = arena.to(self.device)
+        super().__init__(device, *pack_arena_bytes(tensors))
         # embed_utterance pads the waveform to the end of its last partial window, up to one window past the input: the
         # workspace holds max_seconds of input plus that window
         self.max_input_samples = int(max_seconds * sampling_rate)
         cfg = _lib.SpkConfig(mel_n_channels, model_hidden_size, model_num_layers, model_embedding_size, n_fft, hop,
                              partials_n_frames, self.max_input_samples + partials_n_frames * hop)
-        self.cfg, self._lib = cfg, _lib.load()
-        wsb = self._lib.mvb_spk_workspace_bytes(C.byref(cfg))
-        if wsb == 0:
-            _lib.check(_lib.MVB_ERR_UNSUPPORTED)
-        self._ws = torch.zeros(wsb, dtype=torch.uint8, device=self.device)
-        h = C.c_void_p()
-        with torch.cuda.device(self.device):
-            _lib.check(self._lib.mvb_spk_create(C.byref(cfg), self._arena.data_ptr(), self._arena.numel(),
-                                                (C.c_uint64 * len(offs))(*offs), self._ws.data_ptr(), C.byref(h)))
-        self._h = h
+        self.cfg = cfg
+        self._create(self._lib.mvb_spk_create, self._lib.mvb_spk_destroy, cfg, self._lib.mvb_spk_workspace_bytes)
         # batch front-end: filters per (up, down) on the device, and a workspace for MVB_SPK_MAX_BATCH utterances of up
         # to twice the longest single one, allocated on first use
         self._taps: Dict[tuple, torch.Tensor] = {}
@@ -197,16 +182,6 @@ class SpeakerEncoder:
         self._batch_ws: Optional[torch.Tensor] = None
         if verbose:
             print(f"Loaded the speaker embedding model on {self.device.type}.")
-
-    def close(self):
-        if getattr(self, "_h", None) is not None:
-            self._lib.mvb_spk_destroy(self._h)
-            self._h = None
-
-    __del__ = close
-
-    def _st(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
     @staticmethod
     def compute_partial_slices(n_samples: int, rate, min_coverage):
@@ -255,22 +230,13 @@ class SpeakerEncoder:
 
     def _batch_workspace(self) -> torch.Tensor:
         if self._batch_ws is None:
-            nb = self._lib.mvb_spk_batch_workspace_bytes(C.byref(self.cfg), self.batch_max, self.batch_samples)
-            if nb == 0:
-                _lib.check(_lib.MVB_ERR_ARG)
-            self._batch_ws = torch.empty(nb, dtype=torch.uint8, device=self.device)
+            self._batch_ws = self._batch_workspace_of(
+                self._lib.mvb_spk_batch_workspace_bytes(C.byref(self.cfg), self.batch_max, self.batch_samples), zeroed=False)
         return self._batch_ws
 
-    def _groups(self, lengths: Sequence[int]) -> List[List[int]]:
+    def _groups(self, lengths: Sequence[int]) -> List[range]:
         """Consecutive runs of indices that fit one batch call: at most batch_max of them, batch_samples in all."""
-        groups, cur, tot = [], [], 0
-        for i, n in enumerate(lengths):
-            if cur and (len(cur) == self.batch_max or tot + n > self.batch_samples):
-                groups.append(cur)
-                cur, tot = [], 0
-            cur.append(i)
-            tot += n
-        return groups + [cur] if cur else groups
+        return split_runs(lengths, self.batch_max, self.batch_samples)
 
     def _embed_device(self, buf: torch.Tensor, offs: Sequence[int], lens: Sequence[int], rate, min_coverage):
         """Utterance i = the lens[i] 16 kHz samples of the device buffer buf at offs[i] -> embeddings [n, 256] and

@@ -10,6 +10,7 @@ from typing import Dict, List, Optional
 import torch
 
 from . import _lib
+from ._engine import Engine, pack_arena_bytes, split_runs
 
 RATIOS = (8, 5, 4, 2)
 
@@ -26,7 +27,7 @@ def _fold(sd, prefix):
     return v * (g.float() / n)
 
 
-class EncodecDecodeEngine:
+class EncodecDecodeEngine(Engine):
     def __init__(self, state_dict: Dict[str, torch.Tensor], device="cuda", max_frames: int = 2048, n_q: int = 8,
                  max_batch: int = 1, max_total_frames: Optional[int] = None):
         """``max_batch`` > 1 allocates the workspace of ``decode_batch`` / ``decode_latent_batch`` for up to ``max_batch``
@@ -45,36 +46,18 @@ class EncodecDecodeEngine:
                 cw(f"decoder.layers.{i + 1}.block.3") + cw(f"decoder.layers.{i + 1}.shortcut")
             i += 3
         tensors += cw(f"decoder.layers.{i}")
-        offs, total = [], 0
-        for t in tensors:
-            offs.append(total)
-            total = (total + t.numel() * 4 + 255) // 256 * 256
-        arena = torch.zeros(total, dtype=torch.uint8)
-        for t, o in zip(tensors, offs):
-            arena[o:o + t.numel() * 4] = t.contiguous().reshape(-1).view(torch.uint8)
-        self.device = torch.device(device)
-        self._arena = arena.to(self.device)
+        super().__init__(device, *pack_arena_bytes(tensors))
         cfg = _lib.VocConfig()
         cfg.n_q, cfg.hidden, cfg.n_filters, cfg.n_ratios = n_q, tensors[0].shape[1], 32, len(RATIOS)
         for k, r in enumerate(RATIOS):
             cfg.ratios[k] = r
         cfg.kernel, cfg.res_kernel, cfg.last_kernel, cfg.compress, cfg.max_frames = 7, 3, 7, 2, max_frames
-        self.cfg, self._lib = cfg, _lib.load()
-        wsb = self._lib.mvb_voc_workspace_bytes(C.byref(cfg))
-        if wsb == 0:
-            _lib.check(_lib.MVB_ERR_UNSUPPORTED)
-        self._ws = torch.zeros(wsb, dtype=torch.uint8, device=self.device)
-        h = C.c_void_p()
-        with torch.cuda.device(self.device):
-            _lib.check(self._lib.mvb_voc_create(C.byref(cfg), self._arena.data_ptr(), self._arena.numel(),
-                                                (C.c_uint64 * len(offs))(*offs), self._ws.data_ptr(), C.byref(h)))
-        self._h = h
+        self.cfg = cfg
+        self._create(self._lib.mvb_voc_create, self._lib.mvb_voc_destroy, cfg, self._lib.mvb_voc_workspace_bytes)
         self.max_batch, self.max_total_frames, self._bws = max_batch, max_total_frames or max_batch * max_frames, None
         if max_batch > 1:
-            bwsb = self._lib.mvb_voc_batch_workspace_bytes(C.byref(cfg), max_batch, self.max_total_frames)
-            if bwsb == 0:
-                _lib.check(_lib.MVB_ERR_ARG)
-            self._bws = torch.zeros(bwsb, dtype=torch.uint8, device=self.device)
+            self._bws = self._batch_workspace_of(
+                self._lib.mvb_voc_batch_workspace_bytes(C.byref(cfg), max_batch, self.max_total_frames))
         self.upsample = 1
         for r in RATIOS:
             self.upsample *= r
@@ -94,16 +77,6 @@ class EncodecDecodeEngine:
         """fp32 FLOPs (2 x multiply-adds) of one SEANet decode of ``n_frames`` code frames."""
         return float(sum(2.0 * n * m * n_frames for n, m in self._flop_terms))
 
-    def close(self):
-        if getattr(self, "_h", None) is not None:
-            self._lib.mvb_voc_destroy(self._h)
-            self._h = None
-
-    __del__ = close
-
-    def _st(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-
     @torch.no_grad()
     def decode_latent(self, codes: torch.Tensor) -> torch.Tensor:
         """codes int [n_q, T] -> [hidden, T] (the MBD condition, audiocraft ``get_condition``)."""
@@ -120,23 +93,12 @@ class EncodecDecodeEngine:
         _lib.check(self._lib.mvb_voc_decode(self._h, c.data_ptr(), c.shape[1], out.data_ptr(), self._st()))
         return out
 
-    def _groups(self, lens: List[int]) -> List[range]:
-        """Consecutive runs of utterances that fit the batch workspace (<= max_batch of them, <= max_total_frames)."""
-        groups, s0, tot = [], 0, 0
-        for i, t in enumerate(lens):
-            if i > s0 and (i - s0 == self.max_batch or tot + t > self.max_total_frames):
-                groups.append(range(s0, i))
-                s0, tot = i, 0
-            tot += t
-        groups.append(range(s0, len(lens)))
-        return groups
-
     def _batch(self, fn: str, codes: List[torch.Tensor], rows: int, per_frame: int) -> List[torch.Tensor]:
         cs = [c.to(self.device, torch.int32).contiguous() for c in codes]
         lens = [int(c.shape[1]) for c in cs]
         out = torch.empty(rows * sum(lens) * per_frame, dtype=torch.float32, device=self.device)
         pos = 0
-        for g in self._groups(lens):
+        for g in split_runs(lens, self.max_batch, self.max_total_frames):
             flat = torch.cat([cs[i].reshape(-1) for i in g])
             T = (C.c_int32 * len(g))(*[lens[i] for i in g])
             _lib.check(getattr(self._lib, fn)(self._h, len(g), flat.data_ptr(), T, self._bws.data_ptr(), self.max_batch,
@@ -186,7 +148,7 @@ def _encoder_tensors(sd: Dict[str, torch.Tensor], n_q: int) -> List[torch.Tensor
     return tensors
 
 
-class EncodecEncodeEngine:
+class EncodecEncodeEngine(Engine):
     """EnCodec-24 kHz encode path on the device (csrc/encoder.cu): waveform fp32 at 24 kHz -> SEANet encoder -> RVQ codes,
     i.e. ``EncodecModel.encode(wav, bandwidth)`` of the default 24 kHz config (normalize=False, one chunk) that
     ``EncodecDecoder.get_tokens`` (fam/llm/decoders.py:49-64) and the fine-tuning loader call.  Reads the same
@@ -198,39 +160,21 @@ class EncodecEncodeEngine:
         """``max_batch`` > 1 allocates the workspace of ``encode_batch`` for up to ``max_batch`` (<= 32) utterances and
         ``max_total_frames`` frames in all (default ``max_batch * max_frames``); larger requests are split."""
         tensors = _encoder_tensors(state_dict, n_q)
-        offs, total = [], 0
-        for t in tensors:
-            offs.append(total)
-            total = (total + t.numel() * 4 + 255) // 256 * 256
-        arena = torch.zeros(total, dtype=torch.uint8)
-        for t, o in zip(tensors, offs):
-            arena[o:o + t.numel() * 4] = t.contiguous().reshape(-1).view(torch.uint8)
-        self.device = torch.device(device)
-        self._arena = arena.to(self.device)
+        super().__init__(device, *pack_arena_bytes(tensors))
         cfg = _lib.EncConfig()
         cfg.n_q, cfg.hidden, cfg.n_filters, cfg.n_ratios = n_q, tensors[0].shape[1], 32, len(RATIOS)
         for k, r in enumerate(RATIOS):
             cfg.ratios[k] = r
         cfg.kernel, cfg.res_kernel, cfg.last_kernel, cfg.compress, cfg.max_frames = 7, 3, 7, 2, max_frames
-        self.cfg, self._lib = cfg, _lib.load()
+        self.cfg = cfg
         self.hop = 1
         for r in RATIOS:
             self.hop *= r
-        wsb = self._lib.mvb_enc_workspace_bytes(C.byref(cfg))
-        if wsb == 0:
-            _lib.check(_lib.MVB_ERR_UNSUPPORTED)
-        self._ws = torch.zeros(wsb, dtype=torch.uint8, device=self.device)
-        h = C.c_void_p()
-        with torch.cuda.device(self.device):
-            _lib.check(self._lib.mvb_enc_create(C.byref(cfg), self._arena.data_ptr(), self._arena.numel(),
-                                                (C.c_uint64 * len(offs))(*offs), self._ws.data_ptr(), C.byref(h)))
-        self._h = h
+        self._create(self._lib.mvb_enc_create, self._lib.mvb_enc_destroy, cfg, self._lib.mvb_enc_workspace_bytes)
         self.max_batch, self.max_total_frames, self._bws = max_batch, max_total_frames or max_batch * max_frames, None
         if max_batch > 1:
-            bwsb = self._lib.mvb_enc_batch_workspace_bytes(C.byref(cfg), max_batch, self.max_total_frames)
-            if bwsb == 0:
-                _lib.check(_lib.MVB_ERR_ARG)
-            self._bws = torch.zeros(bwsb, dtype=torch.uint8, device=self.device)
+            self._bws = self._batch_workspace_of(
+                self._lib.mvb_enc_batch_workspace_bytes(C.byref(cfg), max_batch, self.max_total_frames))
         # multiply-adds per output sample of every layer, with the layer's output rate in samples per frame
         terms, m, k = [(tensors[n_q].numel(), self.hop)], self.hop, n_q + 2
         for r in reversed(RATIOS):
@@ -251,16 +195,6 @@ class EncodecEncodeEngine:
         the LSTM and the codebook search."""
         F = self.frames(n_samples)
         return float(sum(2.0 * n * m * F for n, m in self._flop_terms) + 2.0 * self._rvq_macs * F)
-
-    def close(self):
-        if getattr(self, "_h", None) is not None:
-            self._lib.mvb_enc_destroy(self._h)
-            self._h = None
-
-    __del__ = close
-
-    def _st(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
     def _run(self, wav: torch.Tensor, emb: bool):
         x = wav.to(self.device, torch.float32).contiguous().reshape(-1)
@@ -286,9 +220,6 @@ class EncodecEncodeEngine:
         """[channels, L] -> codes of the channel mean: ``_extract_encodec_tokens`` (fam/llm/loaders/training_data.py:98-112)."""
         return self.encode(wav.float().mean(dim=0) if wav.dim() == 2 else wav)
 
-    def _groups(self, lens: List[int]) -> List[range]:
-        return EncodecDecodeEngine._groups(self, [self.frames(n) for n in lens])
-
     @torch.no_grad()
     def encode_batch(self, wavs: List[torch.Tensor]) -> List[torch.Tensor]:
         """[waveform fp32 [L_i]] -> [codes int32 [n_q, ceil(L_i / 320)]], each bit-identical to ``encode(wavs[i])``.  One
@@ -303,7 +234,7 @@ class EncodecEncodeEngine:
         n_q = self.cfg.n_q
         out = torch.empty(n_q * sum(self.frames(n) for n in lens), dtype=torch.int32, device=self.device)
         pos = 0
-        for g in self._groups(lens):
+        for g in split_runs([self.frames(n) for n in lens], self.max_batch, self.max_total_frames):
             flat = torch.cat([xs[i] for i in g])
             L = (C.c_int32 * len(g))(*[lens[i] for i in g])
             _lib.check(self._lib.mvb_enc_encode_batch(self._h, len(g), flat.data_ptr(), L, self._bws.data_ptr(), self.max_batch,
