@@ -363,6 +363,15 @@ int mvb_s2_attn_test(const float* d_qkv, int32_t B, int32_t t, int32_t E, int32_
  * Allocates nothing; synchronises `stream`. */
 int mvb_s2_sample_test(const float* d_logits, int32_t n_hier, int32_t n_rows, int32_t V, const void* d_params,
                        const float* d_noise, int32_t* d_tokens, void* stream);
+/* Test hook (not part of the drop-in surface): the stage-2 front end (k_s2_spk, then k_s2_embed, launched as
+ * mvb_s2_forward launches them) without an mvb_s2 handle.  d_idx int32 [B, n_in, t]; d_wte DEVICE array of n_in bf16
+ * table pointers ([vocab_h, E] each); d_wpe bf16 [>= t, E]; d_W_spk bf16 [E, spk_dim]; d_spk fp32 [B, spk_dim] or NULL
+ * (no speaker term; d_W_spk and d_spk_proj are then not read); d_spk_proj fp32 [B, E] = W_spk . spk[b];
+ * d_x fp32 [B * t, E] = sum_h wte_h[idx[b, h, i]] + wpe[i] (+ spk_proj[b]).  MVB_ERR_ARG for a null pointer, B, t, E or
+ * spk_dim < 1, or n_in outside 1..8.  Allocates nothing; synchronises `stream`. */
+int mvb_s2_embed_test(const int32_t* d_idx, int32_t B, int32_t n_in, int32_t t, const void* d_wte, const void* d_wpe,
+                      const void* d_W_spk, const float* d_spk, int32_t spk_dim, int32_t E, float* d_spk_proj, float* d_x,
+                      void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Vocoder, EnCodec-24 kHz decode path: RVQ decode (the diffusion condition `decode_latent`) and the SEANet decoder

@@ -351,6 +351,34 @@ extern "C" int mvb_s2_destroy(mvb_s2* h) {
   return MVB_OK;
 }
 
+// Launches the front end exactly as s2_body does: the speaker projection spk_proj[b] = W_spk . spk[b] (when spk is
+// non-null), then x[b*t + i] = sum_h wte_h[idx[b, h, i]] + wpe[i] (+ spk_proj[b]).
+static cudaError_t launch_s2_embed(cudaStream_t s, const int* idx, int B, int n_in, int t, const __nv_bfloat16* const* wte,
+                                   const __nv_bfloat16* wpe, const __nv_bfloat16* W_spk, const float* spk, int SD, int E,
+                                   float* spk_proj, float* x) {
+  if (spk) {
+    k_s2_spk<<<dim3((E * 32 + 255) / 256, B), 256, 0, s>>>(W_spk, spk, spk_proj, E, SD);
+    if (cudaError_t e = cudaGetLastError()) return e;
+  }
+  k_s2_embed<<<B * t, 128, 0, s>>>(idx, n_in, t, wte, wpe, spk ? spk_proj : nullptr, x, E);
+  return cudaGetLastError();
+}
+
+extern "C" int mvb_s2_embed_test(const int32_t* d_idx, int32_t B, int32_t n_in, int32_t t, const void* d_wte, const void* d_wpe,
+                                 const void* d_W_spk, const float* d_spk, int32_t spk_dim, int32_t E, float* d_spk_proj, float* d_x,
+                                 void* stream) {
+  if (!d_idx || !d_wte || !d_wpe || !d_x || (d_spk && (!d_W_spk || !d_spk_proj)))
+    return mvb::set_error(MVB_ERR_ARG, "mvb_s2_embed_test: null argument");
+  if (B < 1 || t < 1 || E < 1 || spk_dim < 1 || n_in < 1 || n_in > 8)
+    return mvb::set_error(MVB_ERR_ARG, "mvb_s2_embed_test: B, t, E, spk_dim >= 1 and 1 <= n_in <= 8 required");
+  cudaStream_t s = (cudaStream_t)stream;
+  MVB_CK(launch_s2_embed(s, d_idx, B, n_in, t, reinterpret_cast<const __nv_bfloat16* const*>(d_wte),
+                         reinterpret_cast<const __nv_bfloat16*>(d_wpe), reinterpret_cast<const __nv_bfloat16*>(d_W_spk), d_spk,
+                         spk_dim, E, d_spk_proj, d_x));
+  MVB_CK(cudaStreamSynchronize(s));
+  return MVB_OK;
+}
+
 // Launches the bidirectional attention of one layer exactly as s2_body does.
 static cudaError_t launch_s2_attn(cudaStream_t s, const float* qkv, float* out, int batch, int t, int E, int n_head) {
   const dim3 ag((t + 31) / 32, n_head, batch);
@@ -412,12 +440,8 @@ static int s2_body(mvb_s2* h, cudaStream_t s, int batch, bool has_spk, const flo
   const mvb_s2_config& c = h->cfg;
   const int t = c.block_size, rows = batch * t, E = c.n_embd, Hd = h->hidden;
   MVB_CK(cudaMemsetAsync(h->tickets, 0, 256 * 4, s));
-  if (has_spk) {
-    k_s2_spk<<<dim3((E * 32 + 255) / 256, batch), 256, 0, s>>>(h->w(h->g_spk()), h->spk_stage, h->spk_proj, E, c.spk_dim);
-    MVB_CK(cudaGetLastError());
-  }
-  k_s2_embed<<<rows, 128, 0, s>>>(h->idx_stage, c.n_in, t, h->wte_dev, h->w(h->g_wpe()), has_spk ? h->spk_proj : nullptr, h->x, E);
-  MVB_CK(cudaGetLastError());
+  MVB_CK(launch_s2_embed(s, h->idx_stage, batch, c.n_in, t, h->wte_dev, h->w(h->g_wpe()), h->w(h->g_spk()),
+                         has_spk ? h->spk_stage : nullptr, c.spk_dim, E, h->spk_proj, h->x));
   for (int l = 0; l < c.n_layer; ++l) {
     if (int e = s2_linear<G_STORE>(h, s, rows, h->x, E, h->w(h->g_layer(l, 0)), l * 5 + 0, l * 5 + 0, 3 * E, E, h->qkv, 3 * E)) return e;
     MVB_CK(launch_s2_attn(s, h->qkv, h->att, batch, t, E, c.n_head));

@@ -58,8 +58,8 @@ def build_input(text_ids: Sequence[int], cb0: Sequence[int], cb1: Sequence[int],
 
 
 class Stage2Oracle:
-    def __init__(self, sd: Dict[str, torch.Tensor], n_head: int, eps: float, dtype=torch.float32):
-        cv = lambda t: t.to(dtype).contiguous()
+    def __init__(self, sd: Dict[str, torch.Tensor], n_head: int, eps: float, dtype=torch.float32, device="cpu"):
+        cv = lambda t: t.to(device=device, dtype=dtype).contiguous()
         self.n_head, self.eps = n_head, eps
         self.wtes = []
         while f"transformer.wtes.{len(self.wtes)}.weight" in sd:
@@ -85,9 +85,10 @@ class Stage2Oracle:
     def forward(self, idx: torch.Tensor, spk: Optional[torch.Tensor]) -> List[torch.Tensor]:
         """idx int64 [b, 2, t]; spk [b, 1, spk_dim] -> list of 6 logits [b, t, V_target] (model.py:232-311)."""
         b, nh_in, t = idx.shape
-        x = sum(w[idx[:, i]] for i, w in enumerate(self.wtes)) + self.wpe[torch.arange(t)]
+        idx = idx.to(self.wpe.device)
+        x = sum(w[idx[:, i]] for i, w in enumerate(self.wtes)) + self.wpe[:t]
         if spk is not None:
-            x = x + spk.to(x.dtype) @ self.w_spk.t()                      # spk_emb_on_text=True: all positions
+            x = x + spk.to(x) @ self.w_spk.t()                         # spk_emb_on_text=True: all positions
         E = x.shape[-1]
         hs = E // self.n_head
         for L in self.layers:
