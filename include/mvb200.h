@@ -144,6 +144,34 @@ int mvb_s1_admit(mvb_s1* h, int32_t utt, const int32_t* prompt, int32_t T, const
 int mvb_s1_release(mvb_s1* h, int32_t utt, void* stream);
 int mvb_s1_poll(mvb_s1* h, int32_t n_slots, int32_t* done_out, int32_t* n_gen_out, void* stream);
 
+/* Prompt guidance: the reference's guidance_scale = (s, p) of _sample_batch (fam/llm/mixins/causal.py:89-105, 224-262;
+ * inference.py:438-560), logits = (s + p - 1) cond + (1 - s) uncond_speaker + (1 - p) uncond_prompt, with the fast path's
+ * temperature / top-k / top-p / Exp(1) tail after the mix.  A guided utterance owns two slots: its own (`utt`, rows
+ * cond and uncond speaker) and a companion whose speaker-on row is the uncond-prompt row (its other row is computed and
+ * ignored).  The forward passes see two ordinary slots; the sampler of the primary reads the three rows, does the
+ * bookkeeping of both slots and feeds the companion `fed > end_of_audio ? end_of_text_token : fed` (causal.py:262).
+ * Guided slots are sampled by k_sample, never by the resident kernel's fused sampler.
+ *   mvb_s1_admit_guided  == mvb_s1_admit for slot `utt` (params->guidance_scale = s) plus companion slot `companion`,
+ *                        prefilled with the prompt's tokens > params->end_of_audio replaced by end_of_text_token, under
+ *                        the same speaker.  The first token is sampled from the three rows of the last prompt position.
+ *                        p == 1 is exactly mvb_s1_admit (no companion is touched).
+ *   mvb_s1_sample_guided == mvb_s1_sample over three rows: d_logits fp32 [3, vocab] = {cond, uncond speaker, uncond
+ *                        prompt}; p == 1 reads rows 0 and 1 only and equals mvb_s1_sample.
+ * MVB_ERR_ARG, before anything is launched, unless both scales are finite and >= 1 (the reference asserts s >= 1 and
+ * p >= 1), `companion` != `utt` and both are slots of the handle, and end_of_text_token is in the vocabulary; T and
+ * max_new_tokens are checked as mvb_s1_admit checks them.  mvb_s1_poll reports the companion done whenever the primary
+ * is.  The link is dissolved on both sides (a former companion is parked) when mvb_s1_poll or mvb_s1_fetch reads the
+ * primary's done flag set, when the primary is released, or when either slot is admitted or begun again; after that the
+ * old companion is an ordinary free slot and unguided bursts sample in the resident kernel again.  While a link lives,
+ * mvb_s1_decode returns MVB_ERR_ARG when one of its slots is inside [0, n_utts) and the other is not.  s and p are
+ * passed as fp32: for a scale fp32 cannot represent exactly, a mix coefficient can differ from the reference's (formed
+ * from Python doubles) by one fp32 ulp. */
+int mvb_s1_admit_guided(mvb_s1* h, int32_t utt, int32_t companion, const int32_t* prompt, int32_t T,
+                        const float* spk_emb, const mvb_sampling* params, float prompt_guidance_scale,
+                        int32_t end_of_text_token, int32_t max_new_tokens, const float* d_noise, void* stream);
+int mvb_s1_sample_guided(mvb_s1* h, const float* d_logits, const mvb_sampling* p, float prompt_guidance_scale,
+                         const float* d_noise, uint64_t step, int32_t* d_token_out, float* d_probs_out, void* stream);
+
 /* Install per-utterance decode state after prefill: first token, sampling params, optional device
  * noise [max_new, vocab] / forced-token [max_new] buffers (NULL = none). */
 int mvb_s1_begin(mvb_s1* h, int32_t utt, int32_t first_token, int32_t pos, const mvb_sampling* p,

@@ -2,6 +2,7 @@
 // No torch, no CPU fallback: every entry point either runs the CUDA path or fails loudly.
 #include <cuda_runtime.h>
 
+#include <cmath>
 #include <cstring>
 #include <map>
 #include <vector>
@@ -148,6 +149,7 @@ struct mvb_s1 {
   CUtensorMap tm3[6];                                 // 3-D (k, row, layer) maps: wqkv, wo, w1, w3, w2, head
   PcMat pm[5];
   std::vector<int> h_topk;                            // top_k of every utterance slot as installed by mvb_s1_begin
+  std::vector<int> h_link;                            // SamplingDev::link of every slot as installed by mvb_s1_admit_guided
   size_t layer_stride_elems = 0;
   // int4 engine: wqkv / wo / w1 / w3 / w2 are packed matrices; path A streams them through k_gemv_w4, path B dequantises
   // one layer at a time into layer_scratch (bf16 [wqkv | wo | w1 | w3 | w2]).
@@ -337,6 +339,7 @@ static int create_engine(const mvb_s1_config* cfg, const void* d_arena, size_t a
     kv_ok = rows < (1ull << 31) && make_tmap_bf16(&h->tm_kv, h->kv, rows, 128, 64);
   }
   h->h_topk.assign(cfg->max_utts, 0);
+  h->h_link.assign(cfg->max_utts, 0);
   {
     // persistent decode kernel: needs a uniform layer stride (true for arenas packed in checkpoint order)
     const int D = cfg->dim, F = cfg->intermediate, V = cfg->vocab;
@@ -698,6 +701,7 @@ static SamplingDev to_dev(const mvb_sampling* p) {
   d.top_p = p->top_p;
   d.top_k = p->top_k;
   d.end_of_audio = p->end_of_audio;
+  d.link = 0;
   d.seed = p->seed;
   return d;
 }
@@ -781,14 +785,15 @@ extern "C" int mvb_s1_forward(mvb_s1* h, int32_t utt, const int32_t* d_idx, int3
   return MVB_OK;
 }
 
-extern "C" int mvb_s1_sample(mvb_s1* h, const float* d_logits, const mvb_sampling* p, const float* d_noise, uint64_t step,
-                             int32_t* d_token_out, float* d_probs_out, void* stream) {
-  if (!h || !d_logits || !p || !d_token_out) return set_error(MVB_ERR_ARG, "null argument");
+// k_sample in API mode; prompt_guidance > 1 mixes the three rows of d_logits [3, V], anything else the two of [2, V].
+static int sample_api(mvb_s1* h, const float* d_logits, const mvb_sampling* p, float prompt_guidance, const float* d_noise,
+                      uint64_t step, int32_t* d_token_out, float* d_probs_out, void* stream) {
   SampleP sp{};
   sp.logits = d_logits;
   sp.V = h->cfg.vocab;
   sp.decode_mode = 0;
   sp.sp = to_dev(p);
+  sp.prompt_guidance = prompt_guidance;
   sp.noise = d_noise;
   sp.step = step;
   sp.token_out = d_token_out;
@@ -799,11 +804,61 @@ extern "C" int mvb_s1_sample(mvb_s1* h, const float* d_logits, const mvb_samplin
   return MVB_OK;
 }
 
+extern "C" int mvb_s1_sample(mvb_s1* h, const float* d_logits, const mvb_sampling* p, const float* d_noise, uint64_t step,
+                             int32_t* d_token_out, float* d_probs_out, void* stream) {
+  if (!h || !d_logits || !p || !d_token_out) return set_error(MVB_ERR_ARG, "null argument");
+  return sample_api(h, d_logits, p, 1.0f, d_noise, step, d_token_out, d_probs_out, stream);
+}
+
+// The reference asserts both guidance scales (causal.py:87-88): finite and >= 1.
+static int check_guidance(float s, float pg) {
+  if (!std::isfinite(s) || !std::isfinite(pg) || s < 1.0f || pg < 1.0f)
+    return set_error(MVB_ERR_ARG, "guidance_scale (%g, %g): both scales must be finite and >= 1", (double)s, (double)pg);
+  return MVB_OK;
+}
+
+extern "C" int mvb_s1_sample_guided(mvb_s1* h, const float* d_logits, const mvb_sampling* p, float prompt_guidance_scale,
+                                    const float* d_noise, uint64_t step, int32_t* d_token_out, float* d_probs_out, void* stream) {
+  if (!h || !d_logits || !p || !d_token_out) return set_error(MVB_ERR_ARG, "null argument");
+  if (int e = check_guidance(p->guidance_scale, prompt_guidance_scale)) return e;
+  return sample_api(h, d_logits, p, prompt_guidance_scale, d_noise, step, d_token_out, d_probs_out, stream);
+}
+
+// Prompt-guidance link of a primary u and its companion c (SamplingDev::link); the companion's entry takes p and
+// end_of_text.  k_unlink dissolves a link on both sides and parks the former companion.
+__global__ void k_link(S1State st, int u, int c, float prompt_guidance, int end_of_text) {
+  if (threadIdx.x == 0) {
+    st.samp[u].link = c + 1;
+    st.samp[c].link = -(u + 1);
+    st.samp[c].guidance = prompt_guidance;
+    st.samp[c].end_of_audio = end_of_text;
+  }
+}
+__global__ void k_unlink(S1State st, int a, int b, int companion) {
+  if (threadIdx.x == 0) {
+    st.samp[a].link = 0;
+    st.samp[b].link = 0;
+    st.done[companion] = 1;
+  }
+}
+
+static int unlink_slot(mvb_s1* h, int utt, cudaStream_t s) {
+  const int l = h->h_link[utt];
+  if (l == 0) return MVB_OK;
+  const int partner = l > 0 ? l - 1 : -l - 1;
+  k_unlink<<<1, 32, 0, s>>>(h->st, utt, partner, l > 0 ? partner : utt);
+  h->launches++;
+  MVB_CK(cudaGetLastError());
+  h->h_link[utt] = h->h_link[partner] = 0;
+  return MVB_OK;
+}
+
 extern "C" int mvb_s1_begin(mvb_s1* h, int32_t utt, int32_t first_token, int32_t pos, const mvb_sampling* p,
                             const float* d_noise, const int32_t* d_forced, void* stream) {
   if (!h || !p) return set_error(MVB_ERR_ARG, "null argument");
   if (int e = check_slot(h, utt)) return e;
   if (pos < 0 || pos >= h->cfg.block_size) return set_error(MVB_ERR_ARG, "position %d outside the context", pos);
+  if (int e = unlink_slot(h, utt, (cudaStream_t)stream)) return e;
   h->h_topk[utt] = p->top_k;
   k_begin<<<1, 32, 0, (cudaStream_t)stream>>>(h->st, utt, first_token, pos, to_dev(p), d_noise, d_forced, first_token >= 0,
                                               h->cfg.max_new);
@@ -828,16 +883,20 @@ __global__ void k_set_done(S1State st, int utt, int done) {
 // mvb_s1_admit == the per-utterance prologue of generate() (utils:196-212): budget check, prompt / speaker upload,
 // prefill, first token sampled from the last prompt position.  The slot then rides along in every mvb_s1_decode burst
 // until its done flag latches (mvb_s1_poll), after which the host fetches its tokens and may admit another request.
-extern "C" int mvb_s1_admit(mvb_s1* h, int32_t utt, const int32_t* prompt, int32_t T, const float* spk_emb,
-                            const mvb_sampling* params, int32_t max_new_tokens, const float* d_noise, void* stream) {
-  if (!h || !prompt || !spk_emb || !params) return set_error(MVB_ERR_ARG, "null argument");
+// Argument checks of an admission: the prompt length and token budget (generate(): utils:196-204) -> *room.
+static int admit_room(const mvb_s1* h, int32_t T, int32_t max_new_tokens, int* room) {
   const mvb_s1_config& c = h->cfg;
-  if (int e = check_slot(h, utt)) return e;
   if (T < 1) return set_error(MVB_ERR_ARG, "empty prompt");
   if (max_new_tokens < 1 || max_new_tokens > c.max_new) return set_error(MVB_ERR_ARG, "max_new_tokens %d out of range", max_new_tokens);
-  const int room = (T + max_new_tokens < c.block_size ? T + max_new_tokens : c.block_size) - T;
-  if (room <= 0) return set_error(MVB_ERR_PROMPT_TOO_LONG, "Prompt is too long to generate more tokens");
-  cudaStream_t s = (cudaStream_t)stream;
+  *room = (T + max_new_tokens < c.block_size ? T + max_new_tokens : c.block_size) - T;
+  if (*room <= 0) return set_error(MVB_ERR_PROMPT_TOO_LONG, "Prompt is too long to generate more tokens");
+  return MVB_OK;
+}
+
+// Prompt / speaker upload, decode state and prefill of slot `utt`: everything of an admission but the first sample.
+static int admit_prefill(mvb_s1* h, int32_t utt, const int32_t* prompt, int32_t T, const float* spk_emb,
+                         const mvb_sampling* params, int room, const float* d_noise, cudaStream_t s) {
+  const mvb_s1_config& c = h->cfg;
   int* di = h->wsp<int>(h->L.stage_idx) + (size_t)utt * 2 * c.block_size;
   float* d_spk = h->wsp<float>(h->L.stage_spk) + (size_t)utt * c.spk_dim;
   MVB_CK(cudaMemcpyAsync(d_spk, spk_emb, sizeof(float) * c.spk_dim, cudaMemcpyHostToDevice, s));
@@ -847,15 +906,60 @@ extern "C" int mvb_s1_admit(mvb_s1* h, int32_t utt, const int32_t* prompt, int32
   if (int e = mvb_s1_begin(h, utt, -1, 0, params, d_noise, nullptr, s)) return e;
   k_set_budget<<<1, 32, 0, s>>>(h->st, utt, room);
   h->launches++;
-  if (int e = mvb_s1_forward(h, utt, di, T, 0, nullptr, 0, s)) return e;
+  return mvb_s1_forward(h, utt, di, T, 0, nullptr, 0, s);
+}
+
+// The first token of the slot prefilled last (slot_map[0] == that slot after the prefill), in decode mode.
+static int admit_sample(mvb_s1* h, cudaStream_t s) {
   SampleP spp{};
   spp.logits = h->wsp<float>(h->L.logits);
-  spp.V = c.vocab;
+  spp.V = h->cfg.vocab;
   spp.decode_mode = 1;
-  k_sample<<<1, SAMP_THREADS, 0, s>>>(spp, h->st);  // slot_map[0] == utt after the prefill
+  k_sample<<<1, SAMP_THREADS, 0, s>>>(spp, h->st);
   h->launches++;
   MVB_CK(cudaGetLastError());
   return MVB_OK;
+}
+
+extern "C" int mvb_s1_admit(mvb_s1* h, int32_t utt, const int32_t* prompt, int32_t T, const float* spk_emb,
+                            const mvb_sampling* params, int32_t max_new_tokens, const float* d_noise, void* stream) {
+  if (!h || !prompt || !spk_emb || !params) return set_error(MVB_ERR_ARG, "null argument");
+  if (int e = check_slot(h, utt)) return e;
+  int room = 0;
+  if (int e = admit_room(h, T, max_new_tokens, &room)) return e;
+  cudaStream_t s = (cudaStream_t)stream;
+  if (int e = admit_prefill(h, utt, prompt, T, spk_emb, params, room, d_noise, s)) return e;
+  return admit_sample(h, s);
+}
+
+// Prompt guidance (_sample_batch with guidance_scale = (s, p), causal.py:224-262): the companion slot is prefilled with
+// the prompt's text tokens replaced by end_of_text under the same speaker, the primary as mvb_s1_admit does, then the
+// link is installed and the first token is sampled from the three rows.  p == 1 is mvb_s1_admit: no companion.
+extern "C" int mvb_s1_admit_guided(mvb_s1* h, int32_t utt, int32_t companion, const int32_t* prompt, int32_t T,
+                                   const float* spk_emb, const mvb_sampling* params, float prompt_guidance_scale,
+                                   int32_t end_of_text_token, int32_t max_new_tokens, const float* d_noise, void* stream) {
+  if (!h || !prompt || !spk_emb || !params) return set_error(MVB_ERR_ARG, "null argument");
+  if (int e = check_slot(h, utt)) return e;
+  if (int e = check_slot(h, companion)) return e;
+  if (companion == utt) return set_error(MVB_ERR_ARG, "companion slot %d is the utterance's own slot", companion);
+  if (int e = check_guidance(params->guidance_scale, prompt_guidance_scale)) return e;
+  if (end_of_text_token < 0 || end_of_text_token >= h->cfg.vocab)
+    return set_error(MVB_ERR_ARG, "end_of_text_token %d outside the vocabulary", end_of_text_token);
+  int room = 0;
+  if (int e = admit_room(h, T, max_new_tokens, &room)) return e;
+  if (prompt_guidance_scale == 1.0f) return mvb_s1_admit(h, utt, prompt, T, spk_emb, params, max_new_tokens, d_noise, stream);
+  cudaStream_t s = (cudaStream_t)stream;
+  std::vector<int32_t> uncond(prompt, prompt + T);   // causal.py:259-262
+  for (int32_t& t : uncond)
+    if (t > params->end_of_audio) t = end_of_text_token;
+  if (int e = admit_prefill(h, companion, uncond.data(), T, spk_emb, params, room, nullptr, s)) return e;
+  if (int e = admit_prefill(h, utt, prompt, T, spk_emb, params, room, d_noise, s)) return e;
+  k_link<<<1, 32, 0, s>>>(h->st, utt, companion, prompt_guidance_scale, end_of_text_token);
+  h->launches++;
+  MVB_CK(cudaGetLastError());
+  h->h_link[utt] = companion + 1;
+  h->h_link[companion] = -(utt + 1);
+  return admit_sample(h, s);
 }
 
 // Park a slot: its rows still ride along in the batch (recomputed at a frozen position) but nothing is sampled or
@@ -866,7 +970,15 @@ extern "C" int mvb_s1_release(mvb_s1* h, int32_t utt, void* stream) {
   k_set_done<<<1, 32, 0, (cudaStream_t)stream>>>(h->st, utt, 1);
   h->launches++;
   MVB_CK(cudaGetLastError());
+  if (h->h_link[utt] > 0) return unlink_slot(h, utt, (cudaStream_t)stream);   // a guided primary parks its companion too
   return MVB_OK;
+}
+
+// A guided primary whose done flag the host has read has finished for good (only an admission or mvb_s1_begin clears the
+// flag): its link is dissolved here, so that later bursts may leave the old companion out and sample unguided slots in
+// the resident kernel again.
+static int unlink_finished(mvb_s1* h, int32_t utt, int done, cudaStream_t s) {
+  return (done && h->h_link[utt] > 0) ? unlink_slot(h, utt, s) : MVB_OK;
 }
 
 // done flags and generated-token counts of slots [0, n_slots) in one device->host round trip (synchronises `stream`).
@@ -878,6 +990,8 @@ extern "C" int mvb_s1_poll(mvb_s1* h, int32_t n_slots, int32_t* done_out, int32_
   MVB_CK(cudaMemcpyAsync(h->h_flags + 64, h->st.n_gen, sizeof(int) * n_slots, cudaMemcpyDeviceToHost, s));
   MVB_CK(cudaStreamSynchronize(s));
   for (int i = 0; i < n_slots; ++i) { done_out[i] = h->h_flags[i]; n_gen_out[i] = h->h_flags[64 + i]; }
+  for (int i = 0; i < n_slots; ++i)
+    if (int e = unlink_finished(h, i, done_out[i], s)) return e;
   return MVB_OK;
 }
 
@@ -895,6 +1009,11 @@ static int sample_step(mvb_s1* h, cudaStream_t s, int n_utts) {
 extern "C" int mvb_s1_decode(mvb_s1* h, int32_t n_utts, int32_t n_steps, void* stream) {
   if (!h) return set_error(MVB_ERR_ARG, "null handle");
   if (n_utts < 1 || n_utts > h->cfg.max_utts) return set_error(MVB_ERR_ARG, "n_utts %d out of range", n_utts);
+  for (int u = 0; u < n_utts; ++u) {   // a guided primary samples from its companion's rows: both must be decoded
+    const int l = h->h_link[u], partner = l > 0 ? l - 1 : -l - 1;
+    if (l != 0 && partner >= n_utts)
+      return set_error(MVB_ERR_ARG, "slot %d is linked to slot %d outside the %d decoded slots", u, partner, n_utts);
+  }
   if (n_steps < 1) return MVB_OK;
   cudaStream_t s = (cudaStream_t)stream;
   k_identity_slots<<<1, 64, 0, s>>>(h->st, n_utts);
@@ -909,7 +1028,7 @@ extern "C" int mvb_s1_decode(mvb_s1* h, int32_t n_utts, int32_t n_steps, void* s
     // One launch for the whole burst: the kernel samples on the device (top_k = None only, the stage-1 default of
     // TTS.synthesise) and stays resident across positions.
     bool fused = h->fused && (h->cfg.vocab + h->n_sm - 1) / h->n_sm <= PC_SAMP_OWN && h->cfg.vocab <= SAMP_PAD;
-    for (int u = 0; u < n_utts; ++u) fused = fused && h->h_topk[u] <= 0;
+    for (int u = 0; u < n_utts; ++u) fused = fused && h->h_topk[u] <= 0 && h->h_link[u] == 0;   // top-k and guided: k_sample
     if (fused) return launch_persistent(h, s, n_utts, n_steps, true);
   }
   for (int i = 0; i < n_steps; ++i) {
@@ -969,15 +1088,15 @@ extern "C" int mvb_s1_fetch(mvb_s1* h, int32_t utt, int32_t* out_tokens, int32_t
   MVB_CK(cudaMemcpyAsync(h->h_flags, h->st.n_gen + utt, 4, cudaMemcpyDeviceToHost, s));
   MVB_CK(cudaMemcpyAsync(h->h_flags + 1, h->st.done + utt, 4, cudaMemcpyDeviceToHost, s));
   MVB_CK(cudaStreamSynchronize(s));
-  const int n = h->h_flags[0];
+  const int n = h->h_flags[0], finished = h->h_flags[1];
   if (n_out) *n_out = n;
-  if (done) *done = h->h_flags[1];
+  if (done) *done = finished;
   if (out_tokens && cap > 0) {
     const int m = n < cap ? n : cap;
     MVB_CK(cudaMemcpyAsync(out_tokens, h->st.gen_tokens + (size_t)utt * h->cfg.max_new, sizeof(int) * m, cudaMemcpyDeviceToHost, s));
     MVB_CK(cudaStreamSynchronize(s));
   }
-  return MVB_OK;
+  return unlink_finished(h, utt, finished, s);
 }
 
 // Sampled (pre-teacher-forcing) tokens, for the parity tests.

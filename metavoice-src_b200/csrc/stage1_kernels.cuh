@@ -17,8 +17,13 @@ namespace mvb {
 struct SamplingDev {
   float guidance, temperature, top_p;
   int top_k, end_of_audio;
+  // Prompt-guidance link (mvb_s1_admit_guided), in what would otherwise be padding: 0 = none, c + 1 on a guided primary
+  // whose companion slot is c, -(u + 1) on the companion of primary u.  A companion's entry is not otherwise used for
+  // sampling, so it carries the primary's prompt guidance scale p in `guidance` and end_of_text in `end_of_audio`.
+  int link;
   unsigned long long seed;
 };
+static_assert(sizeof(SamplingDev) == 32, "SamplingDev is part of the pinned workspace layout");
 
 struct S1State {
   int* slot_map;        // [max_utts] logical batch index -> utterance slot
@@ -502,15 +507,22 @@ __global__ void k_gather_last(const float* __restrict__ x, float* __restrict__ d
 // softmax, argmax(p / Exp(1))     (fast_inference_utils.py:61-120).  One CTA per utterance.
 // `decode_mode` additionally performs the loop bookkeeping of decode_n_tokens / generate
 // (utils:160-172, 212-226): append, feed back, bump position, latch end-of-audio.
+//
+// Prompt guidance (mixins/causal.py:89-105, 224-262): a guided primary u with companion slot c mixes three rows,
+// cond 2u, uncond-speaker 2u + 1 and uncond-prompt 2c, as (s + p - 1) cond + (1 - s) uncond_spk + (1 - p) uncond_prompt,
+// then runs the same tail.  In decode mode the primary also does the companion's bookkeeping (the companion is fed
+// `fed > end_of_audio ? end_of_text : fed`, causal.py:262) and hands back all four of its rows zeroed; the companion's
+// own CTA does nothing.
 constexpr int SAMP_THREADS = 1024;
 constexpr int SAMP_PAD = 4096;
 
 struct SampleP {
-  const float* logits;  // [rows, V] (decode mode: engine logits buffer) or [2, V] (API mode)
+  const float* logits;  // [rows, V] (decode mode: engine logits buffer) or [2, V] / guided [3, V] (API mode)
   int V;
   int decode_mode;
   // API mode
   SamplingDev sp;
+  float prompt_guidance;  // > 1: logits are [3, V] = {cond, uncond speaker, uncond prompt}
   const float* noise;
   unsigned long long step;
   int* token_out;
@@ -534,30 +546,64 @@ __global__ void __launch_bounds__(SAMP_THREADS) k_sample(SampleP p, S1State st) 
   const float* noise = p.noise;
   unsigned long long step = p.step;
   const float* lc = p.logits;
+  const float* lp = nullptr;     // uncond-prompt row of a guided utterance
+  float pg = p.prompt_guidance;
+  int comp = -1, eot = 0;        // decode mode: companion slot of a guided primary and its end_of_text token
   if (p.decode_mode) {
     u = st.slot_map[blockIdx.x];
     lc = p.logits + (size_t)(2 * u) * V;
+    const int link = st.samp[u].link;
+    if (link < 0) return;        // a companion: its primary reads, zeroes and advances its rows
+    comp = link - 1;
     if (st.done[u]) {
       // a finished utterance still rides along in the batch (its rows are recomputed at a frozen position): hand its
       // logits rows back zeroed so the persistent kernel's red.add accumulation starts from zero every step
       float* z = const_cast<float*>(lc);
       for (int v = tid; v < 2 * V; v += SAMP_THREADS) z[v] = 0.f;
+      if (comp >= 0) {   // and so are its companion's
+        z = const_cast<float*>(p.logits) + (size_t)(2 * comp) * V;
+        for (int v = tid; v < 2 * V; v += SAMP_THREADS) z[v] = 0.f;
+      }
       return;
     }
     sp = st.samp[u];
     step = (unsigned long long)st.n_gen[u];
     noise = st.noise[u] ? st.noise[u] + (size_t)(st.n_gen[u] - st.noise_base[u]) * V : nullptr;
+    if (comp >= 0) {
+      const SamplingDev cs = st.samp[comp];
+      pg = cs.guidance;
+      eot = cs.end_of_audio;
+      lp = p.logits + (size_t)(2 * comp) * V;
+    }
+  } else if (pg > 1.0f) {
+    lp = lc + 2 * V;
   }
   const float* lu = lc + V;
 
   // -- CFG mix and temperature, with torch's rounding order (utils:116, :92)
-  const float g = sp.guidance, omg = __fsub_rn(1.0f, sp.guidance);
   const float tdiv = fmaxf(sp.temperature, 1e-5f);
-  for (int v = tid; v < SAMP_PAD; v += SAMP_THREADS) {
-    float k = INFINITY;
-    if (v < V) k = __fdiv_rn(__fadd_rn(__fmul_rn(g, lc[v]), __fmul_rn(omg, lu[v])), tdiv);
-    key[v] = k;
-    sid[v] = (unsigned short)v;
+  if (lp == nullptr) {
+    const float g = sp.guidance, omg = __fsub_rn(1.0f, sp.guidance);
+    for (int v = tid; v < SAMP_PAD; v += SAMP_THREADS) {
+      float k = INFINITY;
+      if (v < V) k = __fdiv_rn(__fadd_rn(__fmul_rn(g, lc[v]), __fmul_rn(omg, lu[v])), tdiv);
+      key[v] = k;
+      sid[v] = (unsigned short)v;
+    }
+  } else {
+    // causal.py:100-104 with Python-float coefficients: each formed in double and rounded once to fp32, as torch does
+    // for a Python scalar times an fp32 tensor; then ((base c + (1-s) u) + (1-p) up).  s and p arrive through the C ABI
+    // already rounded to fp32, so for a scale fp32 cannot represent (3.1) a coefficient can differ from torch's by one
+    // fp32 ulp; dyadic scales (3, 1.5, 2.5, ...) give torch's coefficients exactly.
+    const double s = sp.guidance, pd = pg;
+    const float cb = __double2float_rn(s + pd - 1.0), cs = __double2float_rn(1.0 - s), cp = __double2float_rn(1.0 - pd);
+    for (int v = tid; v < SAMP_PAD; v += SAMP_THREADS) {
+      float k = INFINITY;
+      if (v < V)
+        k = __fdiv_rn(__fadd_rn(__fadd_rn(__fmul_rn(cb, lc[v]), __fmul_rn(cs, lu[v])), __fmul_rn(cp, lp[v])), tdiv);
+      key[v] = k;
+      sid[v] = (unsigned short)v;
+    }
   }
   __syncthreads();
   if (p.decode_mode) {
@@ -565,6 +611,10 @@ __global__ void __launch_bounds__(SAMP_THREADS) k_sample(SampleP p, S1State st) 
     // (after the barrier: every thread has consumed its logits by now)
     float* z = const_cast<float*>(lc);
     for (int v = tid; v < 2 * V; v += SAMP_THREADS) z[v] = 0.f;
+    if (comp >= 0) {
+      z = const_cast<float*>(lp);
+      for (int v = tid; v < 2 * V; v += SAMP_THREADS) z[v] = 0.f;
+    }
   }
 
   // -- ascending bitonic sort of (logit, index); padding (+inf) sinks to the end
@@ -722,6 +772,16 @@ __global__ void __launch_bounds__(SAMP_THREADS) k_sample(SampleP p, S1State st) 
         if (!stop) st.pos[u] = np;
         st.n_gen[u] = n + 1;
         if (stop) st.done[u] = 1;
+        if (comp >= 0) {   // the companion follows the primary's positions; text tokens reach it as end_of_text
+          const int fc = fed > sp.end_of_audio ? eot : fed;
+          st.sampled_tokens[(size_t)comp * st.max_new + n] = tok;
+          st.gen_tokens[(size_t)comp * st.max_new + n] = fc;
+          st.row_tok[2 * comp] = fc;
+          st.row_tok[2 * comp + 1] = fc;
+          if (!stop) st.pos[comp] = np;
+          st.n_gen[comp] = n + 1;
+          if (stop) st.done[comp] = 1;
+        }
       }
     }
   }

@@ -85,6 +85,10 @@ SIGNATURES = {
                                C.c_void_p, C.c_void_p]),
     "mvb_s1_release": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p]),
     "mvb_s1_poll": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "mvb_s1_admit_guided": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(Sampling),
+                                      C.c_float, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "mvb_s1_sample_guided": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(Sampling), C.c_float, C.c_void_p, C.c_uint64, C.c_void_p,
+                                       C.c_void_p, C.c_void_p]),
     "mvb_s1_step_logits": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "mvb_s1_launch_count": (C.c_uint64, [C.c_void_p]),
     "mvb_s1_int4_workspace_bytes": (C.c_size_t, [C.POINTER(S1Config)]),

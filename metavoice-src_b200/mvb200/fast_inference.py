@@ -25,7 +25,7 @@ from typing import List, Literal, Optional
 import numpy as np
 import torch
 
-from .fast_inference_utils import build_model, main
+from .fast_inference_utils import build_model, main, split_guidance
 from .second_stage import SecondStage, flattened_interleaved_decode
 from .tokenise import TrainedBPETokeniser
 from .vocoder import EncodecDecodeEngine
@@ -110,7 +110,16 @@ class TTS:
             from .speaker_encoder import SpeakerEncoder
             self.smodel = SpeakerEncoder(weights_fpath=spk_ckpt, device=device, eval=True, verbose=False)
 
+    def _check_guidance(self, guidance_scale) -> None:
+        """``guidance_scale`` is a float or the reference's ``(s, p)`` (inference.py:646-647).  With p > 1 every text is
+        decoded on two KV slots (its own and the prompt-guidance companion), which a one-slot engine does not have."""
+        _, p = split_guidance(guidance_scale, self.tokenizer.eot_token)
+        if p is not None and self.model.max_utts < 2:
+            raise ValueError(f"guidance_scale={tuple(guidance_scale)!r} (prompt guidance) decodes each text on two KV slots; "
+                             "create the TTS with max_utts=2 or more")
+
     def synthesise(self, text: str, spk_ref_path: str, top_p=0.95, guidance_scale=3.0, temperature=1.0) -> str:
+        self._check_guidance(guidance_scale)
         text = normalize_text(text)
         spk_emb = load_speaker_embedding(spk_ref_path, self.smodel)
         start = time.time()
@@ -150,6 +159,7 @@ class TTS:
         vocoder, and the waveforms are concatenated into one file."""
         from .fast_inference_utils import encode_tokens
         from .serving import ContinuousBatcher, chunk_text
+        self._check_guidance(guidance_scale)
         chunks = chunk_text(normalize_text(text), max_chars)
         if not chunks:
             raise ValueError("empty text")
@@ -157,7 +167,7 @@ class TTS:
         start = time.time()
         cb = ContinuousBatcher(self.model)
         ids = [cb.submit(encode_tokens(self.tokenizer, c, device="cpu"), spk_emb, top_p=top_p, guidance_scale=guidance_scale,
-                         temperature=temperature) for c in chunks]
+                         temperature=temperature, end_of_text_token=self.tokenizer.eot_token) for c in chunks]
         toks = cb.run_until_done()
         wavs = []
         for c, rid in zip(chunks, ids):
@@ -203,6 +213,7 @@ class TTS:
         from .serving import ContinuousBatcher, seeded_noise
         if len(texts) != len(spk_ref_paths):
             raise ValueError(f"{len(texts)} texts but {len(spk_ref_paths)} speaker references")
+        self._check_guidance(guidance_scale)
         if not texts:
             return []
         texts = [normalize_text(t) for t in texts]
@@ -216,7 +227,8 @@ class TTS:
         ids = []
         for i, (t, e) in enumerate(zip(texts, spk)):
             prompt = encode_tokens(self.tokenizer, t, device="cpu")
-            kw = dict(top_p=top_p, guidance_scale=guidance_scale, temperature=temperature)
+            kw = dict(top_p=top_p, guidance_scale=guidance_scale, temperature=temperature,
+                      end_of_text_token=self.tokenizer.eot_token)
             if seed is not None:
                 noise = seeded_noise(self.model, prompt.numel(), seed + i)
                 kw.update(max_new_tokens=noise.shape[0], noise=noise)

@@ -8,6 +8,7 @@ checkpoint (the reference needs 30-120 s, README.md:98).
 from __future__ import annotations
 
 import ctypes as C
+import math
 import time
 import warnings
 from pathlib import Path
@@ -36,13 +37,40 @@ def _sampling_struct(guidance_scale, temperature, top_p=None, top_k=None, end_of
                          int(end_of_audio_token), int(seed) & (2**64 - 1))
 
 
+def split_guidance(guidance_scale, end_of_text_token: Optional[int] = None, *, need_eot: bool = True
+                   ) -> Tuple[float, Optional[float]]:
+    """``guidance_scale`` as the fast path's scalar g, or as the reference's pair ``(s, p)`` of speaker and prompt guidance
+    (mixins/causal.py:89-105) -> ``(s, p)`` with ``p = None`` when there is no prompt guidance: a scalar, or ``p == 1``,
+    which is the scalar ``s`` exactly.  A pair must have finite scales >= 1 (the reference asserts both), and ``p > 1``
+    needs ``end_of_text_token`` (unless ``need_eot`` is False): the uncond-prompt row sees every text token as
+    end-of-text (causal.py:259-262)."""
+    if not isinstance(guidance_scale, (tuple, list)):
+        return guidance_scale, None
+    if len(guidance_scale) != 2:
+        raise ValueError(f"guidance_scale must be a float or a pair (speaker, prompt), got {guidance_scale!r}")
+    s, p = (_f(v) for v in guidance_scale)
+    if not (math.isfinite(s) and math.isfinite(p) and s >= 1 and p >= 1):
+        raise ValueError(f"guidance_scale {(s, p)}: both scales must be finite and >= 1")
+    if p == 1:
+        return s, None
+    if need_eot and end_of_text_token is None:
+        raise ValueError("prompt guidance (guidance_scale=(s, p) with p > 1) needs end_of_text_token=")
+    return s, p
+
+
 # ---- fast_inference_utils.py:107-120 --------------------------------------------------------------
 def sample(logits: torch.Tensor, guidance_scale, temperature, top_p=None, top_k=None, *, model: Transformer = None,
            q: Optional[torch.Tensor] = None):
     """logits [2, S, V] -> (idx_next int32 [1], probs [V]).  The Exp(1) noise ``q`` is drawn with torch's
     generator exactly where the reference draws it (``multinomial_sample_one_no_sync``, utils:61-65) unless
-    supplied, then everything else runs in one CUDA kernel."""
+    supplied, then everything else runs in one CUDA kernel.  ``guidance_scale=(s, p)`` with p > 1 takes logits
+    [3, S, V] = {cond, uncond speaker, uncond prompt} and mixes them as the reference's ``_sample_next_token``
+    (mixins/causal.py:89-105); ``(s, 1.0)`` is ``s``."""
     model = model or sample.default_model
+    s, p = split_guidance(guidance_scale, need_eot=False)
+    rows = 2 if p is None else 3
+    if logits.shape[0] < rows:
+        raise ValueError(f"logits have {logits.shape[0]} rows; guidance_scale={guidance_scale!r} needs {rows}")
     lg = logits[:, -1].to(torch.float32).contiguous()
     V = lg.shape[-1]
     if q is None:
@@ -50,9 +78,13 @@ def sample(logits: torch.Tensor, guidance_scale, temperature, top_p=None, top_k=
     q = q.to(device=lg.device, dtype=torch.float32).contiguous()
     tok = torch.empty(1, dtype=torch.int32, device=lg.device)
     probs = torch.empty(V, dtype=torch.float32, device=lg.device)
-    sp = _sampling_struct(guidance_scale, temperature, top_p, top_k)
-    _lib.check(model._lib.mvb_s1_sample(model.handle, lg.data_ptr(), C.byref(sp), q.data_ptr(), 0, tok.data_ptr(),
-                                        probs.data_ptr(), model._stream()))
+    sp = _sampling_struct(s, temperature, top_p, top_k)
+    if p is None:
+        _lib.check(model._lib.mvb_s1_sample(model.handle, lg.data_ptr(), C.byref(sp), q.data_ptr(), 0, tok.data_ptr(),
+                                            probs.data_ptr(), model._stream()))
+    else:
+        _lib.check(model._lib.mvb_s1_sample_guided(model.handle, lg.data_ptr(), C.byref(sp), p, q.data_ptr(), 0,
+                                                   tok.data_ptr(), probs.data_ptr(), model._stream()))
     return tok, probs
 
 
@@ -131,7 +163,7 @@ def draw_reference_noise(n_utts: int, n_steps: int, vocab: int, device, rng: str
 def generate_batch(model: Transformer, prompts, spk_embs: torch.Tensor, *, max_new_tokens: Optional[int] = None,
                    end_of_audio_token: int = 2048, noise=None, forced=None, seed: Optional[int] = None,
                    guidance_scale=3.0, temperature=1.0, top_p=None, top_k=None, return_sampled: bool = False,
-                   rng: Optional[str] = None):
+                   rng: Optional[str] = None, end_of_text_token: Optional[int] = None):
     """N independent utterances decoded together with per-utterance positions (the batching semantics of
     fam/llm/mixins/causal.py:179-287, numerically equal to running each utterance alone).  Goes through the
     HOST-buffer plugin call ``mvb_s1_generate``: prompts/speakers are copied host->device and the tokens
@@ -140,8 +172,20 @@ def generate_batch(model: Transformer, prompts, spk_embs: torch.Tensor, *, max_n
     Randomness: ``noise`` (explicit Exp(1) draws) > ``seed`` (on-device Philox stream keyed by it) > ``rng``.
     With neither ``noise`` nor ``seed`` the draws come from torch's global generator exactly where the reference
     takes them (``rng="torch"``, see ``draw_reference_noise``); ``rng="philox"`` selects the on-device stream keyed
-    from torch's generator instead (no noise buffer, used by the throughput benchmark)."""
+    from torch's generator instead (no noise buffer, used by the throughput benchmark).
+
+    Prompt guidance: ``guidance_scale=(s, p)`` with p > 1 is the reference's three-row CFG (mixins/causal.py:89-105,
+    224-262) and needs ``end_of_text_token``; each utterance i then takes slot i plus companion slot n + i, so the engine
+    needs 2 n slots, and the loop runs through ``mvb_s1_admit_guided`` / ``mvb_s1_decode`` / ``mvb_s1_poll``.
+    ``(s, 1.0)`` is ``s``."""
     n = len(prompts)
+    s_g, p_g = split_guidance(guidance_scale, end_of_text_token)
+    if p_g is not None:
+        if 2 * n > model.max_utts:
+            raise ValueError(f"{n} prompt-guided utterances need {2 * n} slots; setup_caches set up {model.max_utts}")
+        if forced is not None:
+            raise ValueError("teacher forcing is not available with prompt guidance")
+    guidance_scale = s_g
     if n > model.max_utts:
         raise ValueError(f"{n} utterances exceed the {model.max_utts} slots set up by setup_caches")
     lens = np.asarray([int(p.numel()) for p in prompts], dtype=np.int32)
@@ -174,6 +218,12 @@ def generate_batch(model: Transformer, prompts, spk_embs: torch.Tensor, *, max_n
     if fc is not None:
         assert fc.shape == (n, max_new), fc.shape
     vp = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)
+    if p_g is not None:
+        if nz is not None:
+            d_noise = torch.from_numpy(nz).to(model.device)
+        offs = np.concatenate([[0], np.cumsum(lens)])
+        return _generate_guided(model, [flat[offs[i]:offs[i + 1]] for i in range(n)], spk, params, p_g, int(end_of_text_token),
+                                max_new, d_noise, return_sampled)
     noise_arg, on_dev = (C.c_void_p(d_noise.data_ptr()), 1) if d_noise is not None else (vp(nz), 0)
     _lib.check(model._lib.mvb_s1_generate(model.handle, n, vp(flat), vp(lens), vp(spk), params, max_new, noise_arg, on_dev,
                                           vp(fc), vp(out), vp(out_lens), model._stream()))
@@ -187,6 +237,38 @@ def generate_batch(model: Transformer, prompts, spk_embs: torch.Tensor, *, max_n
         _lib.check(model._lib.mvb_s1_fetch_sampled(model.handle, i, vp(buf), int(out_lens[i]), model._stream()))
         sampled.append(torch.from_numpy(buf))
     return fed, sampled
+
+
+def _generate_guided(model: Transformer, prompts, spk: np.ndarray, params, prompt_guidance: float, end_of_text_token: int,
+                     max_new: int, d_noise: Optional[torch.Tensor], return_sampled: bool):
+    """generate_batch's prompt-guided loop: utterance i in slot i with companion slot n + i, decoded in bursts until every
+    done flag latches.  ``d_noise``: DEVICE Exp(1) draws [n, max_new, vocab] or None (on-device Philox)."""
+    lib, h, st = model._lib, model.handle, model._stream()
+    n = len(prompts)
+    vp = lambda a: a.ctypes.data_as(C.c_void_p)
+    for i in range(n):
+        pr = np.ascontiguousarray(prompts[i], dtype=np.int32)
+        sv = np.ascontiguousarray(spk[i], dtype=np.float32)
+        dn = None if d_noise is None else C.c_void_p(d_noise[i].data_ptr())
+        _lib.check(lib.mvb_s1_admit_guided(h, i, n + i, vp(pr), int(pr.size), vp(sv), C.byref(params[i]), prompt_guidance,
+                                           end_of_text_token, max_new, dn, st))
+    done = np.zeros(2 * n, dtype=np.int32)
+    n_gen = np.zeros(2 * n, dtype=np.int32)
+    while True:
+        _lib.check(lib.mvb_s1_poll(h, 2 * n, vp(done), vp(n_gen), st))
+        if done[:n].all():
+            break
+        _lib.check(lib.mvb_s1_decode(h, 2 * n, 32, st))
+    fed, sampled = [], []
+    for i in range(n):
+        buf = np.zeros(int(n_gen[i]), dtype=np.int32)
+        _lib.check(lib.mvb_s1_fetch(h, i, vp(buf), int(buf.size), None, None, st))
+        fed.append(torch.from_numpy(buf))
+        if return_sampled:
+            sb = np.zeros(int(n_gen[i]), dtype=np.int32)
+            _lib.check(lib.mvb_s1_fetch_sampled(h, i, vp(sb), int(sb.size), st))
+            sampled.append(torch.from_numpy(sb))
+    return (fed, sampled) if return_sampled else fed
 
 
 def encode_tokens(tokenizer, text: str, device="cuda") -> torch.Tensor:
@@ -254,7 +336,7 @@ def main(*, model, tokenizer, model_size, prompt: str, guidance_scale, temperatu
     device_sync(device)
     t0 = time.perf_counter()
     y = generate(model, encoded, spk_emb, temperature=temperature, top_k=top_k, top_p=top_p,
-                 guidance_scale=guidance_scale)
+                 guidance_scale=guidance_scale, end_of_text_token=getattr(tokenizer, "eot_token", None))
     device_sync(device)
     t = time.perf_counter() - t0
     tokens_generated = y.size(0) - prompt_length

@@ -23,7 +23,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .fast_inference_utils import _sampling_struct
+from .fast_inference_utils import _sampling_struct, split_guidance
 
 MAX_CHARS = 220  # fam/llm/inference.py:537
 
@@ -84,19 +84,25 @@ class _Request:
     max_new: int
     seed: int
     noise: Optional[torch.Tensor] = None
+    prompt_guidance: Optional[float] = None      # p > 1 of guidance_scale = (s, p): the request needs a companion slot
+    end_of_text: int = 0
     slot: int = -1
+    companion: int = -1
     tokens: Optional[torch.Tensor] = None
 
 
 @dataclass
 class ContinuousBatcher:
-    """Admit-between-bursts scheduler over one ``mvb200.fast_model.Transformer`` (``setup_caches(2 * slots, ...)``)."""
+    """Admit-between-bursts scheduler over one ``mvb200.fast_model.Transformer`` (``setup_caches(2 * slots, ...)``).
+    A prompt-guided request (``guidance_scale=(s, p)``, p > 1) occupies two slots, its own and a companion, from
+    admission until it finishes; requests are admitted in submission order."""
     model: object
     burst: int = 32
     _next: int = 0
     _pending: Deque[_Request] = field(default_factory=deque)
     _active: Dict[int, _Request] = field(default_factory=dict)   # slot -> request
     _done: Dict[int, torch.Tensor] = field(default_factory=dict)
+    _companions: Dict[int, int] = field(default_factory=dict)   # companion slot -> its request's slot
 
     def __post_init__(self):
         self.slots = self.model.max_utts
@@ -107,7 +113,13 @@ class ContinuousBatcher:
     # ---- client side -----------------------------------------------------------------------------
     def submit(self, prompt: torch.Tensor, spk_emb: torch.Tensor, *, max_new_tokens: Optional[int] = None,
                guidance_scale=3.0, temperature=1.0, top_p=0.95, top_k=None, end_of_audio_token: int = 2048,
-               seed: Optional[int] = None, noise: Optional[torch.Tensor] = None) -> int:
+               seed: Optional[int] = None, noise: Optional[torch.Tensor] = None,
+               end_of_text_token: Optional[int] = None) -> int:
+        """``guidance_scale``: a float, or the reference's ``(s, p)``; p > 1 needs ``end_of_text_token`` and two free
+        slots at admission, and ``(s, 1.0)`` is ``s``."""
+        s_g, p_g = split_guidance(guidance_scale, end_of_text_token)
+        if p_g is not None and self.slots < 2:
+            raise ValueError(f"a prompt-guided request needs 2 slots; setup_caches set up {self.slots}")
         T = int(prompt.numel())
         block = self.model.config.block_size
         max_new = block - T if max_new_tokens is None else int(max_new_tokens)
@@ -120,8 +132,9 @@ class ContinuousBatcher:
         self._next += 1
         self._pending.append(_Request(rid, prompt.detach().cpu().numpy().astype(np.int32).reshape(-1),
                                       np.ascontiguousarray(spk_emb.detach().to("cpu", torch.float32).numpy().reshape(-1)),
-                                      dict(guidance_scale=guidance_scale, temperature=temperature, top_p=top_p, top_k=top_k,
-                                           end_of_audio_token=end_of_audio_token), max_new, seed, noise))
+                                      dict(guidance_scale=s_g, temperature=temperature, top_p=top_p, top_k=top_k,
+                                           end_of_audio_token=end_of_audio_token), max_new, seed, noise, p_g,
+                                      int(end_of_text_token) if p_g is not None else 0))
         return rid
 
     @property
@@ -131,8 +144,8 @@ class ContinuousBatcher:
     # ---- engine side -----------------------------------------------------------------------------
     def _admit(self):
         lib, h, st = self.model._lib, self.model.handle, self.model._stream()
-        free = [s for s in range(self.slots) if s not in self._active]
-        while self._pending and free:
+        free = [s for s in range(self.slots) if s not in self._active and s not in self._companions]
+        while self._pending and len(free) >= (1 if self._pending[0].prompt_guidance is None else 2):
             r = self._pending.popleft()
             r.slot = free.pop(0)
             sp = _sampling_struct(seed=r.seed, **r.sampling)
@@ -141,8 +154,15 @@ class ContinuousBatcher:
                 r.noise = r.noise.to(self.model.device, torch.float32).contiguous()     # keep alive while the slot is active
                 assert r.noise.shape == (r.max_new, self.model.config.vocab_size)
                 d_noise = C.c_void_p(r.noise.data_ptr())
-            _lib.check(lib.mvb_s1_admit(h, r.slot, r.prompt.ctypes.data_as(C.c_void_p), int(r.prompt.size),
-                                        r.spk.ctypes.data_as(C.c_void_p), C.byref(sp), r.max_new, d_noise, st))
+            if r.prompt_guidance is None:
+                _lib.check(lib.mvb_s1_admit(h, r.slot, r.prompt.ctypes.data_as(C.c_void_p), int(r.prompt.size),
+                                            r.spk.ctypes.data_as(C.c_void_p), C.byref(sp), r.max_new, d_noise, st))
+            else:
+                r.companion = free.pop(0)
+                _lib.check(lib.mvb_s1_admit_guided(h, r.slot, r.companion, r.prompt.ctypes.data_as(C.c_void_p),
+                                                   int(r.prompt.size), r.spk.ctypes.data_as(C.c_void_p), C.byref(sp),
+                                                   r.prompt_guidance, r.end_of_text, r.max_new, d_noise, st))
+                self._companions[r.companion] = r.slot
             self._active[r.slot] = r
 
     def step(self) -> List[int]:
@@ -152,7 +172,7 @@ class ContinuousBatcher:
         if not self._active:
             return []
         lib, h, st = self.model._lib, self.model.handle, self.model._stream()
-        n_slots = max(self._active) + 1
+        n_slots = max([*self._active, *self._companions]) + 1
         _lib.check(lib.mvb_s1_decode(h, n_slots, self.burst, st))
         done = np.zeros(n_slots, dtype=np.int32)
         n_gen = np.zeros(n_slots, dtype=np.int32)
@@ -161,6 +181,7 @@ class ContinuousBatcher:
         for s in list(self._active):
             if done[s]:
                 r = self._active.pop(s)
+                self._companions.pop(r.companion, None)     # the engine parked it with its request
                 buf = np.zeros(int(n_gen[s]), dtype=np.int32)
                 n, d = C.c_int32(0), C.c_int32(0)
                 _lib.check(lib.mvb_s1_fetch(h, s, buf.ctypes.data_as(C.c_void_p), int(buf.size), C.byref(n), C.byref(d), st))
