@@ -593,8 +593,8 @@ __global__ void __launch_bounds__(SAMP_THREADS) k_sample(SampleP p, S1State st) 
   } else {
     // causal.py:100-104 with Python-float coefficients: each formed in double and rounded once to fp32, as torch does
     // for a Python scalar times an fp32 tensor; then ((base c + (1-s) u) + (1-p) up).  s and p arrive through the C ABI
-    // already rounded to fp32, so for a scale fp32 cannot represent (3.1) a coefficient can differ from torch's by one
-    // fp32 ulp; dyadic scales (3, 1.5, 2.5, ...) give torch's coefficients exactly.
+    // already rounded to fp32, so for a scale fp32 cannot represent a coefficient can differ from torch's by half an ulp
+    // of that scale plus its own rounding (1 ulp at (3.1, 1.7), 3 ulps of 1 - s at s = 1.1); dyadic scales are exact.
     const double s = sp.guidance, pd = pg;
     const float cb = __double2float_rn(s + pd - 1.0), cs = __double2float_rn(1.0 - s), cp = __double2float_rn(1.0 - pd);
     for (int v = tid; v < SAMP_PAD; v += SAMP_THREADS) {

@@ -209,7 +209,7 @@ def token_ok(tok, k, q, sampler, philox=False, **kw):
     return (*judge(tok, q, variants), nb)
 
 
-def check_api_draw(tok, probs, k, q, top_p, top_k, label):
+def check_api_draw(tok, probs, k, q, top_p, top_k, label, philox=False):
     """k_sample API mode: kept set, probabilities and token.  Returns (worst |err|/bound, n_band, near_tie)."""
     V = k.size
     r = reference(k, top_p=top_p, top_k=top_k, q=q)
@@ -229,7 +229,7 @@ def check_api_draw(tok, probs, k, q, top_p, top_k, label):
     bound = beta * r2["p"] + 2.0 ** -125
     bad = np.nonzero(err > bound)[0]
     assert bad.size == 0, f"{label}: probs over the bound at {bad[:8].tolist()} (max ratio {float((err / bound).max()):.2e})"
-    ok, near, nb = token_ok(int(tok), k, q, "k_sample", top_p=top_p, top_k=top_k)
+    ok, near, nb = token_ok(int(tok), k, q, "k_sample", philox, top_p=top_p, top_k=top_k)
     assert ok, f"{label}: token {int(tok)} vs float64 {r['token']} (not a certified near-tie)"
     return float((err / bound).max()), nb, near
 
@@ -257,9 +257,10 @@ def _n_sm():
 
 
 class Probe:
-    """The probe model of the module docstring at vocabulary V for `utts` utterance slots."""
+    """The probe model of the module docstring at vocabulary V for `utts` utterance slots; tc and mode are
+    setup_caches' tensor_core_path and from_state_dict's quantisation_mode."""
 
-    def __init__(self, V, utts, fused=True, seed=0):
+    def __init__(self, V, utts, fused=True, seed=0, tc=None, mode=None):
         from mvb200.fast_model import ModelArgs, Transformer
         self.V = V
         rng = np.random.default_rng(seed + V)
@@ -288,8 +289,8 @@ class Probe:
               "transformer.h.0.mlp.c_proj.weight": torch.zeros(D, F)}
         sd = {k: v.to(torch.bfloat16) for k, v in sd.items()}
         cfg = ModelArgs(block_size=BLOCK, vocab_size=V, n_layer=1, n_head=H, dim=D, intermediate_size=F)
-        self.m = Transformer.from_state_dict(sd, cfg, device="cuda:0")
-        self.m.setup_caches(2 * utts, BLOCK, unfused_sampler=not fused)
+        self.m = Transformer.from_state_dict(sd, cfg, device="cuda:0", quantisation_mode=mode)
+        self.m.setup_caches(2 * utts, BLOCK, tensor_core_path=tc, unfused_sampler=not fused)
         self.fused, self.utts = fused, utts
         self.lib, self.h = self.m._lib, self.m.handle
         self._keep = []
