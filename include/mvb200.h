@@ -347,28 +347,47 @@ int mvb_enc_op_test(int32_t op, const float* d_x, int32_t Cin, int32_t T, int32_
 /* ------------------------------------------------------------------------------------------------
  * Stage 2: the non-causal codebook-expansion model (fam/llm/model.py:195-314 with causal=False) and its sampler
  * (fam/llm/mixins/non_causal.py:15-67).  Shapes come from second_stage.pt["model_args"] (inference.py:124-128).
- * Supported: norm_type "rmsnorm", nonlinearity "swiglu", bias False, head size 64 or 128 (anything else fails loudly). */
+ * Supported: every GPTConfig (model.py:26-46) the reference's non-causal GPT builds with a speaker projection --
+ * norm_type "rmsnorm" or "layernorm", nonlinearity_type "swiglu" or "gelu", bias True or False (mvb_s2_arch) -- with
+ * head size 64 or 128 and equal target vocabularies (anything else fails loudly). */
 typedef struct mvb_s2_config {
   int32_t n_layer, n_head, n_embd;
-  int32_t hidden;          /* SwiGLU width (layers.py:51-53) */
+  int32_t hidden;          /* MLP width: SwiGLU's (layers.py:51-53), or 4 n_embd for GELU (layers.py:46) */
   int32_t block_size;      /* sequence length t of the single non-causal pass (non_causal.py:31) */
   int32_t n_in;            /* input hierarchies (2) */
   int32_t vocab_in[8];
   int32_t n_out;           /* predicted hierarchies (6) */
   int32_t vocab_out[8];
   int32_t spk_dim;
-  float   norm_eps;
+  float   norm_eps;        /* RMSNorm eps; LayerNorm always uses 1e-5 (layers.py:17) */
   int32_t max_batch;
   int32_t options;         /* MVB_S2_* bits below; 0 = the production engine */
 } mvb_s2_config;
 /* Stage-2 option (fixed at create time; the workspace size does not depend on it; any other bit is MVB_ERR_ARG): */
 #define MVB_S2_EAGER 0x1   /* launch the forward pass kernel by kernel instead of replaying a captured CUDA graph */
 typedef struct mvb_s2 mvb_s2;
+/* Stage-2 architecture (GPTConfig.norm_type, nonlinearity_type, bias); all zero = rmsnorm, swiglu, no bias.  A field
+ * outside its values is MVB_ERR_ARG naming it. */
+typedef struct mvb_s2_arch {
+  int32_t norm;            /* MVB_S2_NORM_*: ln_1, ln_2 and ln_f */
+  int32_t mlp;             /* MVB_S2_MLP_* */
+  int32_t bias;            /* 1: biases on c_attn, attn.c_proj, the MLP Linears and (LayerNorm) ln_1, ln_2, ln_f */
+} mvb_s2_arch;
+#define MVB_S2_NORM_RMS    0   /* RMSNorm(eps = norm_eps), layers.py:20-30 */
+#define MVB_S2_NORM_LAYER  1   /* LayerNorm(eps = 1e-5), with a beta when bias, layers.py:8-17 */
+#define MVB_S2_MLP_SWIGLU  0   /* c_proj(silu(w1 x) * (w3 x)) */
+#define MVB_S2_MLP_GELU    1   /* c_proj(GELU(c_fc x)), exact erf GELU (nn.GELU()) */
 
 size_t mvb_s2_workspace_bytes(const mvb_s2_config* cfg);
-/* offsets (host): wte[n_in], wpe, speaker_cond_pos, ln_f, lm_heads[n_out], then per layer
- * {ln_1, attn.c_attn, attn.c_proj, ln_2, mlp.swiglu.w1, mlp.swiglu.w3, mlp.c_proj}; bf16 arena as for stage 1.
- * d_workspace must be zero-filled.  Replaces Model._init_model (inference.py:102-141). */
+/* offsets (host), bf16 arena as for stage 1: wte[n_in], wpe, speaker_cond_pos, ln_f, lm_heads[n_out], then per layer
+ * {ln_1, attn.c_attn, attn.c_proj, ln_2, mlp.swiglu.w1, mlp.swiglu.w3, mlp.c_proj} (GELU: {ln_1, attn.c_attn,
+ * attn.c_proj, ln_2, mlp.c_fc, mlp.c_proj}); then, when arch->bias: ln_f.bias (LayerNorm only), and per layer
+ * {ln_1.bias (LayerNorm only), attn.c_attn.bias, attn.c_proj.bias, ln_2.bias (LayerNorm only), mlp.c_fc.bias |
+ * mlp.swiglu.w1.bias, mlp.swiglu.w3.bias, mlp.c_proj.bias}.  speaker_cond_pos and lm_heads never have a bias.
+ * arch NULL = all zero.  d_workspace must be zero-filled; its size does not depend on arch.  Replaces Model._init_model
+ * (inference.py:102-141).  mvb_s2_create == mvb_s2_create_ex with arch NULL. */
+int mvb_s2_create_ex(const mvb_s2_config* cfg, const mvb_s2_arch* arch, const void* d_arena, size_t arena_bytes,
+                     const uint64_t* offsets, void* d_workspace, mvb_s2** out);
 int mvb_s2_create(const mvb_s2_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
                   void* d_workspace, mvb_s2** out);
 int mvb_s2_destroy(mvb_s2* h);
@@ -400,6 +419,14 @@ int mvb_s2_sample_test(const float* d_logits, int32_t n_hier, int32_t n_rows, in
 int mvb_s2_embed_test(const int32_t* d_idx, int32_t B, int32_t n_in, int32_t t, const void* d_wte, const void* d_wpe,
                       const void* d_W_spk, const float* d_spk, int32_t spk_dim, int32_t E, float* d_spk_proj, float* d_x,
                       void* stream);
+/* Test hook (not part of the drop-in surface): mvb_gemm_test's operator with the stage-2 prologues and epilogues.
+ * out[R, M] (+)= epilogue(f(x) . W^T + bias): norm 0 none, 1 RMSNorm (gain, eps), 2 LayerNorm (gain, optional beta,
+ * eps); epi 0 store, 1 residual add, 2 SwiGLU silu(x W^T + bias) * (x W3^T + bias3), 4 GELU (exact erf).  d_bias,
+ * d_bias3 bf16 [M] or NULL (d_bias3 is required by SwiGLU with a bias).  ksplit_override > 0 forces the K split.
+ * Synchronises `stream`. */
+int mvb_s2_linear_test(int32_t epi, int32_t norm, const void* d_W, const void* d_W3, const void* d_bias, const void* d_bias3,
+                       int32_t M, int32_t K, const float* d_x, int32_t ldx, int32_t R, const void* d_gain, const void* d_beta,
+                       float eps, int32_t split_lo, int32_t ksplit_override, float* d_out, int32_t ldo, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Vocoder, EnCodec-24 kHz decode path: RVQ decode (the diffusion condition `decode_latent`) and the SEANet decoder

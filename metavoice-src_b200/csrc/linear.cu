@@ -7,42 +7,56 @@ using namespace mvb;
 
 namespace mvb {
 
-template <int EPI, int NC, bool SCALED>
+template <int EPI, int NC, bool SCALED, bool BIASED>
 static cudaError_t launch_tc_gemm_nc(cudaStream_t s, const CUtensorMap& tA, const CUtensorMap& tA3, const CUtensorMap& tB,
                                      const GemmP& p, const GemmPlan& g) {
   static PerDeviceOnce attr_set;
   if (attr_set.pending()) {
-    cudaError_t e = cudaFuncSetAttribute(k_tc_gemm<EPI, NC, SCALED>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(k_tc_gemm<EPI, NC, SCALED, BIASED>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) return e;
     attr_set.mark();
   }
-  k_tc_gemm<EPI, NC, SCALED><<<dim3(g.tiles, g.ksplit), GEMM_THREADS, g.smem_bytes, s>>>(tA, tA3, tB, p);
+  k_tc_gemm<EPI, NC, SCALED, BIASED><<<dim3(g.tiles, g.ksplit), GEMM_THREADS, g.smem_bytes, s>>>(tA, tA3, tB, p);
   return cudaGetLastError();
 }
 
 // The accumulator size is a template parameter (registers): the smallest of 16 / 32 / 64 / 128 columns that holds Rpad.
-template <int EPI, bool SCALED>
+template <int EPI, bool SCALED, bool BIASED>
 static cudaError_t launch_tc_gemm_sc(cudaStream_t s, const CUtensorMap& tA, const CUtensorMap& tA3, const CUtensorMap& tB,
                                      const GemmP& p, const GemmPlan& g) {
-  if (p.Rpad <= 16) return launch_tc_gemm_nc<EPI, 2, SCALED>(s, tA, tA3, tB, p, g);
-  if (p.Rpad <= 32) return launch_tc_gemm_nc<EPI, 4, SCALED>(s, tA, tA3, tB, p, g);
-  if (p.Rpad <= 64) return launch_tc_gemm_nc<EPI, 8, SCALED>(s, tA, tA3, tB, p, g);
-  return launch_tc_gemm_nc<EPI, 16, SCALED>(s, tA, tA3, tB, p, g);
+  if (p.Rpad <= 16) return launch_tc_gemm_nc<EPI, 2, SCALED, BIASED>(s, tA, tA3, tB, p, g);
+  if (p.Rpad <= 32) return launch_tc_gemm_nc<EPI, 4, SCALED, BIASED>(s, tA, tA3, tB, p, g);
+  if (p.Rpad <= 64) return launch_tc_gemm_nc<EPI, 8, SCALED, BIASED>(s, tA, tA3, tB, p, g);
+  return launch_tc_gemm_nc<EPI, 16, SCALED, BIASED>(s, tA, tA3, tB, p, g);
 }
 
+// Instances: int8 row scales on every epilogue but G_GELU, Linear biases on every epilogue but G_QKV, never both (they
+// share GemmP's per-row vector slots).
 template <int EPI>
 static cudaError_t launch_tc_gemm(cudaStream_t s, const CUtensorMap& tA, const CUtensorMap& tA3, const CUtensorMap& tB,
-                                  GemmP p, const GemmPlan& g) {
+                                  GemmP p, const GemmPlan& g, bool scaled, bool biased) {
   p.ksplit = g.ksplit;
   p.stages = g.stages;
-  if (p.scale != nullptr) return launch_tc_gemm_sc<EPI, true>(s, tA, tA3, tB, p, g);
-  return launch_tc_gemm_sc<EPI, false>(s, tA, tA3, tB, p, g);
+  if constexpr (EPI != G_GELU) {
+    if (scaled) return launch_tc_gemm_sc<EPI, true, false>(s, tA, tA3, tB, p, g);
+  }
+  if constexpr (EPI != G_QKV) {
+    if (biased) return launch_tc_gemm_sc<EPI, false, true>(s, tA, tA3, tB, p, g);
+  }
+  if (scaled || biased) return cudaErrorInvalidValue;
+  return launch_tc_gemm_sc<EPI, false, false>(s, tA, tA3, tB, p, g);
 }
 
 cudaError_t tc_gemm(cudaStream_t s, const TcGemm& a) {
   if (a.Rpad < 16 || a.Rpad > 128 || a.Rpad % 16) return cudaErrorInvalidValue;
+  const bool scaled = a.scale != nullptr, biased = a.bias != nullptr;
+  if ((a.layer_norm && a.gain == nullptr) || (scaled && biased) || (a.epi == G_SWIGLU && biased && a.bias3 == nullptr))
+    return cudaErrorInvalidValue;
   const int NB = a.Rpad * (a.split_lo ? 2 : 1);
-  k_prep_b<<<a.Rpad, 256, 0, s>>>(a.x, a.ldx, a.gain, a.eps, a.K, a.Rpad, a.R, a.split_lo ? 1 : 0, a.B);
+  if (a.layer_norm)
+    k_prep_b<true><<<a.Rpad, 256, 0, s>>>(a.x, a.ldx, a.gain, a.beta, a.eps, a.K, a.Rpad, a.R, a.split_lo ? 1 : 0, a.B);
+  else
+    k_prep_b<false><<<a.Rpad, 256, 0, s>>>(a.x, a.ldx, a.gain, nullptr, a.eps, a.K, a.Rpad, a.R, a.split_lo ? 1 : 0, a.B);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   GemmP p{};
@@ -50,14 +64,16 @@ cudaError_t tc_gemm(cudaStream_t s, const TcGemm& a) {
   p.scratch = a.scratch; p.tickets = a.tickets; p.out = a.out; p.ldo = a.ldo;
   p.kcache = a.kcache; p.vcache = a.vcache; p.row_cache = a.row_cache; p.row_pos = a.row_pos;
   p.H = a.H; p.S_max = a.S_max; p.D = a.D; p.kv_fp32 = a.kv_fp32 ? 1 : 0;
-  p.scale = a.scale; p.scale3 = a.scale3;
+  if (scaled) { p.scale = a.scale; p.scale3 = a.scale3; }
+  if (biased) { p.bias = a.bias; p.bias3 = a.bias3; }
   const GemmPlan g = plan_gemm(a.M, a.K, NB, a.epi == G_SWIGLU, a.n_sm, a.ksplit);
   const CUtensorMap& tA3 = a.epi == G_SWIGLU ? *a.tmW3 : *a.tmW;
   switch (a.epi) {
-    case G_STORE: return launch_tc_gemm<G_STORE>(s, *a.tmW, tA3, *a.tmB, p, g);
-    case G_RESID: return launch_tc_gemm<G_RESID>(s, *a.tmW, tA3, *a.tmB, p, g);
-    case G_SWIGLU: return launch_tc_gemm<G_SWIGLU>(s, *a.tmW, tA3, *a.tmB, p, g);
-    default: return launch_tc_gemm<G_QKV>(s, *a.tmW, tA3, *a.tmB, p, g);
+    case G_STORE: return launch_tc_gemm<G_STORE>(s, *a.tmW, tA3, *a.tmB, p, g, scaled, biased);
+    case G_RESID: return launch_tc_gemm<G_RESID>(s, *a.tmW, tA3, *a.tmB, p, g, scaled, biased);
+    case G_SWIGLU: return launch_tc_gemm<G_SWIGLU>(s, *a.tmW, tA3, *a.tmB, p, g, scaled, biased);
+    case G_GELU: return launch_tc_gemm<G_GELU>(s, *a.tmW, tA3, *a.tmB, p, g, scaled, biased);
+    default: return launch_tc_gemm<G_QKV>(s, *a.tmW, tA3, *a.tmB, p, g, scaled, biased);
   }
 }
 
@@ -166,4 +182,29 @@ extern "C" int mvb_w8_gemm_test(int32_t epi, const void* d_W, const void* d_W3, 
   if (!d_scale || (epi == G_SWIGLU && !d_scale3)) return mvb::set_error(MVB_ERR_ARG, "mvb_w8_gemm_test: null row scales");
   return gemm_test(epi, d_W, d_W3, d_scale, d_scale3, M, K, d_x, ldx, R, d_gain, eps, split_lo, ksplit_override, d_out, ldo,
                    d_kcache, d_vcache, d_row_cache, d_row_pos, H, S_max, D, kv_fp32, stream);
+}
+
+extern "C" int mvb_s2_linear_test(int32_t epi, int32_t norm, const void* d_W, const void* d_W3, const void* d_bias,
+                                  const void* d_bias3, int32_t M, int32_t K, const float* d_x, int32_t ldx, int32_t R,
+                                  const void* d_gain, const void* d_beta, float eps, int32_t split_lo, int32_t ksplit_override,
+                                  float* d_out, int32_t ldo, void* stream) {
+  if (!d_W || !d_x || !d_out) return mvb::set_error(MVB_ERR_ARG, "null argument");
+  if (epi != G_STORE && epi != G_RESID && epi != G_SWIGLU && epi != G_GELU)
+    return mvb::set_error(MVB_ERR_ARG, "mvb_s2_linear_test: epilogue %d", epi);
+  if (norm < 0 || norm > 2) return mvb::set_error(MVB_ERR_ARG, "mvb_s2_linear_test: norm %d", norm);
+  if ((norm != 0) != (d_gain != nullptr) || (d_beta && norm != 2))
+    return mvb::set_error(MVB_ERR_ARG, "mvb_s2_linear_test: a norm takes a gain (and only LayerNorm a beta)");
+  if (K % 64 || R < 1 || R > 128 || M < 1 || ldo < M || ldx < K)
+    return mvb::set_error(MVB_ERR_UNSUPPORTED, "mvb_s2_linear_test: K %% 64 == 0, 1 <= R <= 128, ldo >= M, ldx >= K required");
+  if (epi == G_SWIGLU && (!d_W3 || (d_bias && !d_bias3)))
+    return mvb::set_error(MVB_ERR_ARG, "mvb_s2_linear_test: SwiGLU needs W3 (and bias3 with a bias)");
+  TcGemm a{};
+  a.epi = epi;
+  a.x = d_x; a.ldx = ldx; a.gain = reinterpret_cast<const __nv_bfloat16*>(d_gain); a.eps = eps;
+  a.layer_norm = norm == 2; a.beta = reinterpret_cast<const __nv_bfloat16*>(d_beta);
+  a.M = M; a.K = K; a.R = R; a.split_lo = split_lo; a.ksplit = ksplit_override;
+  a.out = d_out; a.ldo = ldo;
+  a.bias = reinterpret_cast<const __nv_bfloat16*>(d_bias);
+  a.bias3 = epi == G_SWIGLU ? reinterpret_cast<const __nv_bfloat16*>(d_bias3) : nullptr;
+  return run_gemm(a, d_W, d_W3, (cudaStream_t)stream);
 }

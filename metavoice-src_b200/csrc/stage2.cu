@@ -212,8 +212,15 @@ __global__ void __launch_bounds__(256) k_s2_sample(const float* __restrict__ log
 
 }  // namespace
 
+// Per-layer norm parameters and Linear biases (null when the architecture has none).
+struct S2LayerP {
+  const __nv_bfloat16 *g1, *b1, *g2, *b2;                // ln_1 / ln_2 gain and (LayerNorm with bias) beta
+  const __nv_bfloat16 *qkv_b, *o_b, *fc_b, *fc3_b, *proj_b;   // c_attn, attn.c_proj, c_fc | w1, w3, mlp.c_proj
+};
+
 struct mvb_s2 {
   mvb_s2_config cfg;
+  mvb_s2_arch arch{};
   int n_sm = 132, hidden = 0;
   const char* arena = nullptr;
   std::vector<uint64_t> off;
@@ -231,16 +238,36 @@ struct mvb_s2 {
   cudaStream_t cap_stream = nullptr;
   cudaGraphExec_t graphs[2][65] = {};   // [has speaker][batch]
   const __nv_bfloat16** wte_dev;
-  std::vector<CUtensorMap> tmW;   // per layer {c_attn, c_proj, w1, w3, mlp.c_proj}, then heads
+  std::vector<CUtensorMap> tmW;   // per layer {c_attn, c_proj, w1 | c_fc, w3 (GELU: c_fc again), mlp.c_proj}, then heads
   CUtensorMap tmB_E, tmB_H;
+  std::vector<S2LayerP> lp;
+  const __nv_bfloat16* lnf_b = nullptr;
   const __nv_bfloat16* w(int i) const { return reinterpret_cast<const __nv_bfloat16*>(arena + off[i]); }
+  bool gelu() const { return arch.mlp == MVB_S2_MLP_GELU; }
   // arena order: wte[n_in], wpe, spk_proj, ln_f, heads[n_out], then per layer {ln_1, c_attn, c_proj, ln_2, w1, w3, c_proj}
+  // (GELU: {ln_1, c_attn, c_proj, ln_2, c_fc, c_proj}), then the biases (s2_offset_count)
   int g_wpe() const { return cfg.n_in; }
   int g_spk() const { return cfg.n_in + 1; }
   int g_lnf() const { return cfg.n_in + 2; }
   int g_head(int i) const { return cfg.n_in + 3 + i; }
-  int g_layer(int l, int t) const { return cfg.n_in + 3 + cfg.n_out + l * 7 + t; }
+  int g_layer(int l, int t) const { return cfg.n_in + 3 + cfg.n_out + l * (gelu() ? 6 : 7) + t; }
 };
+
+// Tensors in the offset list: the weights, then, with bias, ln_f.bias (LayerNorm) and per layer {ln_1.bias (LayerNorm),
+// c_attn.bias, attn.c_proj.bias, ln_2.bias (LayerNorm), w1.bias, w3.bias | c_fc.bias, mlp.c_proj.bias}.
+static int s2_offset_count(const mvb_s2_config* c, const mvb_s2_arch& a) {
+  const bool ln = a.norm == MVB_S2_NORM_LAYER, gelu = a.mlp == MVB_S2_MLP_GELU;
+  int n = c->n_in + 3 + c->n_out + c->n_layer * (gelu ? 6 : 7);
+  if (a.bias) n += (ln ? 1 : 0) + c->n_layer * ((ln ? 2 : 0) + 3 + (gelu ? 1 : 2));
+  return n;
+}
+
+static int s2_validate_arch(const mvb_s2_arch& a) {
+  if (a.norm != MVB_S2_NORM_RMS && a.norm != MVB_S2_NORM_LAYER) return mvb::set_error(MVB_ERR_ARG, "arch.norm: undefined value %d", a.norm);
+  if (a.mlp != MVB_S2_MLP_SWIGLU && a.mlp != MVB_S2_MLP_GELU) return mvb::set_error(MVB_ERR_ARG, "arch.mlp: undefined value %d", a.mlp);
+  if (a.bias != 0 && a.bias != 1) return mvb::set_error(MVB_ERR_ARG, "arch.bias: undefined value %d", a.bias);
+  return MVB_OK;
+}
 
 struct S2Layout { size_t x, qkv, att, ffn, logits, spk, B, scratch, tickets, tokens, wte, idx, spk_stage, params, total; };
 
@@ -293,15 +320,19 @@ extern "C" size_t mvb_s2_workspace_bytes(const mvb_s2_config* c) {
   return s2_layout(c).total;
 }
 
-extern "C" int mvb_s2_create(const mvb_s2_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets, void* d_ws,
-                             mvb_s2** out) {
+extern "C" int mvb_s2_create_ex(const mvb_s2_config* cfg, const mvb_s2_arch* arch, const void* d_arena, size_t arena_bytes,
+                                const uint64_t* offsets, void* d_ws, mvb_s2** out) {
   if (int e = s2_validate(cfg)) return e;
-  if (!d_arena || !offsets || !d_ws || !out) return mvb::set_error(MVB_ERR_ARG, "null pointer argument");
-  const int n_off = cfg->n_in + 3 + cfg->n_out + 7 * cfg->n_layer;
+  const mvb_s2_arch a = arch ? *arch : mvb_s2_arch{};
+  if (int e = s2_validate_arch(a)) return e;
+  if (!offsets) return mvb::set_error(MVB_ERR_ARG, "null pointer argument");
+  const int n_off = s2_offset_count(cfg, a);
   if (int e = check_offsets(offsets, n_off, arena_bytes, "stage 2: weight offset")) return e;
+  if (!d_arena || !d_ws || !out) return mvb::set_error(MVB_ERR_ARG, "null pointer argument");
   Building<mvb_s2> hb(new mvb_s2(), mvb_s2_destroy);
   mvb_s2* h = hb.get();
   h->cfg = *cfg;
+  h->arch = a;
   h->hidden = cfg->hidden;
   int dev = 0;
   if (int e = current_device(&dev, &h->n_sm)) return e;
@@ -319,14 +350,31 @@ extern "C" int mvb_s2_create(const mvb_s2_config* cfg, const void* d_arena, size
   for (int i = 0; i < cfg->n_in; ++i) wte[i] = h->w(i);
   MVB_CK(cudaMemcpy(h->wte_dev, wte.data(), sizeof(void*) * cfg->n_in, cudaMemcpyHostToDevice));
   const int E = cfg->n_embd, Hd = h->hidden;
+  const bool ln = a.norm == MVB_S2_NORM_LAYER, gelu = h->gelu();
+  int nb = s2_offset_count(cfg, mvb_s2_arch{a.norm, a.mlp, 0});    // first bias slot
+  auto bias_slot = [&](bool present) { return present && a.bias ? h->w(nb++) : nullptr; };
+  h->lnf_b = bias_slot(ln);
+  h->lp.resize(cfg->n_layer);
+  for (int l = 0; l < cfg->n_layer; ++l) {
+    S2LayerP& p = h->lp[l];
+    p.g1 = h->w(h->g_layer(l, 0));
+    p.g2 = h->w(h->g_layer(l, 3));
+    p.b1 = bias_slot(ln);
+    p.qkv_b = bias_slot(true);
+    p.o_b = bias_slot(true);
+    p.b2 = bias_slot(ln);
+    p.fc_b = bias_slot(true);
+    p.fc3_b = bias_slot(!gelu);
+    p.proj_b = bias_slot(true);
+  }
   h->tmW.resize((size_t)cfg->n_layer * 5 + cfg->n_out);
   bool ok = true;
   for (int l = 0; l < cfg->n_layer && ok; ++l) {
     ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 0], h->w(h->g_layer(l, 1)), 3 * E, E, 128);
     ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 1], h->w(h->g_layer(l, 2)), E, E, 128);
     ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 2], h->w(h->g_layer(l, 4)), Hd, E, 128);
-    ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 3], h->w(h->g_layer(l, 5)), Hd, E, 128);
-    ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 4], h->w(h->g_layer(l, 6)), E, Hd, 128);
+    ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 3], h->w(h->g_layer(l, gelu ? 4 : 5)), Hd, E, 128);
+    ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 4], h->w(h->g_layer(l, gelu ? 5 : 6)), E, Hd, 128);
   }
   for (int i = 0; i < cfg->n_out && ok; ++i)
     ok = ok && make_tmap_bf16(&h->tmW[(size_t)cfg->n_layer * 5 + i], h->w(h->g_head(i)), cfg->vocab_out[i], E, 128);
@@ -338,6 +386,11 @@ extern "C" int mvb_s2_create(const mvb_s2_config* cfg, const void* d_arena, size
     return mvb::set_error(MVB_ERR_CUDA, "stage 2: stream / pinned buffer allocation failed");
   *out = hb.release();
   return MVB_OK;
+}
+
+extern "C" int mvb_s2_create(const mvb_s2_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets, void* d_ws,
+                             mvb_s2** out) {
+  return mvb_s2_create_ex(cfg, nullptr, d_arena, arena_bytes, offsets, d_ws, out);
 }
 
 extern "C" int mvb_s2_destroy(mvb_s2* h) {
@@ -415,15 +468,21 @@ extern "C" int mvb_s2_sample_test(const float* d_logits, int32_t n_hier, int32_t
   return MVB_OK;
 }
 
-// y[rows, M] (+)= f(x)[rows, K] . W^T in passes of 128 rows through the tensor-core GEMM
+// y[rows, M] (+)= f(x)[rows, K] . W^T (+ bias) in passes of 128 rows through the tensor-core GEMM; f = the arch's norm
+// (gain, beta) when gain != null.  LayerNorm's eps is 1e-5 (layers/layers.py:17), RMSNorm's the config's.
 template <int EPI>
-static int s2_linear(mvb_s2* h, cudaStream_t s, int rows, const float* x, int ldx, const __nv_bfloat16* gain, int widx, int widx3, int M, int K,
-                     float* out, int ldo) {
+static int s2_linear(mvb_s2* h, cudaStream_t s, int rows, const float* x, int ldx, const __nv_bfloat16* gain,
+                     const __nv_bfloat16* beta, int widx, int widx3, const __nv_bfloat16* bias, const __nv_bfloat16* bias3, int M,
+                     int K, float* out, int ldo) {
   TcGemm g{};
   g.epi = EPI; g.Rpad = S2_ROWS; g.split_lo = 1;
   g.tmW = &h->tmW[widx]; g.tmW3 = &h->tmW[widx3];
   g.B = h->B; g.tmB = (K == h->cfg.n_embd) ? &h->tmB_E : &h->tmB_H;
-  g.ldx = ldx; g.gain = gain; g.eps = h->cfg.norm_eps;
+  g.ldx = ldx; g.gain = gain;
+  g.layer_norm = gain != nullptr && h->arch.norm == MVB_S2_NORM_LAYER;
+  g.beta = g.layer_norm ? beta : nullptr;
+  g.eps = g.layer_norm ? 1e-5f : h->cfg.norm_eps;
+  g.bias = bias; g.bias3 = bias3;
   g.M = M; g.K = K; g.ldo = ldo;
   g.scratch = h->scratch; g.tickets = h->tickets; g.n_sm = h->n_sm;
   for (int r0 = 0; r0 < rows; r0 += S2_ROWS) {
@@ -443,16 +502,22 @@ static int s2_body(mvb_s2* h, cudaStream_t s, int batch, bool has_spk, const flo
   MVB_CK(launch_s2_embed(s, h->idx_stage, batch, c.n_in, t, h->wte_dev, h->w(h->g_wpe()), h->w(h->g_spk()),
                          has_spk ? h->spk_stage : nullptr, c.spk_dim, E, h->spk_proj, h->x));
   for (int l = 0; l < c.n_layer; ++l) {
-    if (int e = s2_linear<G_STORE>(h, s, rows, h->x, E, h->w(h->g_layer(l, 0)), l * 5 + 0, l * 5 + 0, 3 * E, E, h->qkv, 3 * E)) return e;
+    const S2LayerP& p = h->lp[l];
+    if (int e = s2_linear<G_STORE>(h, s, rows, h->x, E, p.g1, p.b1, l * 5 + 0, l * 5 + 0, p.qkv_b, nullptr, 3 * E, E, h->qkv, 3 * E)) return e;
     MVB_CK(launch_s2_attn(s, h->qkv, h->att, batch, t, E, c.n_head));
-    if (int e = s2_linear<G_RESID>(h, s, rows, h->att, E, nullptr, l * 5 + 1, l * 5 + 1, E, E, h->x, E)) return e;
-    if (int e = s2_linear<G_SWIGLU>(h, s, rows, h->x, E, h->w(h->g_layer(l, 3)), l * 5 + 2, l * 5 + 3, Hd, E, h->ffn, Hd)) return e;
-    if (int e = s2_linear<G_RESID>(h, s, rows, h->ffn, Hd, nullptr, l * 5 + 4, l * 5 + 4, E, Hd, h->x, E)) return e;
+    if (int e = s2_linear<G_RESID>(h, s, rows, h->att, E, nullptr, nullptr, l * 5 + 1, l * 5 + 1, p.o_b, nullptr, E, E, h->x, E)) return e;
+    if (h->gelu()) {
+      if (int e = s2_linear<G_GELU>(h, s, rows, h->x, E, p.g2, p.b2, l * 5 + 2, l * 5 + 2, p.fc_b, nullptr, Hd, E, h->ffn, Hd)) return e;
+    } else {
+      if (int e = s2_linear<G_SWIGLU>(h, s, rows, h->x, E, p.g2, p.b2, l * 5 + 2, l * 5 + 3, p.fc_b, p.fc3_b, Hd, E, h->ffn, Hd)) return e;
+    }
+    if (int e = s2_linear<G_RESID>(h, s, rows, h->ffn, Hd, nullptr, nullptr, l * 5 + 4, l * 5 + 4, p.proj_b, nullptr, E, Hd, h->x, E)) return e;
   }
   const int vmax = c.vocab_out[0];
   for (int i = 0; i < c.n_out; ++i) {
     const int hw = c.n_layer * 5 + i;
-    if (int e = s2_linear<G_STORE>(h, s, rows, h->x, E, h->w(h->g_lnf()), hw, hw, vmax, E, h->logits + (size_t)i * rows * vmax, vmax)) return e;
+    if (int e = s2_linear<G_STORE>(h, s, rows, h->x, E, h->w(h->g_lnf()), h->lnf_b, hw, hw, nullptr, nullptr, vmax, E,
+                                   h->logits + (size_t)i * rows * vmax, vmax)) return e;
   }
   MVB_CK(launch_s2_sample(s, h->logits, vmax, h->params, d_noise, h->tokens, rows, c.n_out));
   return MVB_OK;

@@ -38,18 +38,24 @@ struct GemmP {
   const int* row_cache;  // [R] cache row of each activation row
   const int* row_pos;    // [R] cache position of each activation row
   int H, S_max, D, kv_fp32;
-  // int8 weights (the widened q): bf16 [M] row scales of W (and W3), applied once per output after the (split-K) sum
-  const __nv_bfloat16* scale;
-  const __nv_bfloat16* scale3;
+  // bf16 [M] per-row vectors of W (and W3), applied once per output after the (split-K) sum: the row scales of int8
+  // weights (the widened q, SCALED) or the Linear biases (stage 2 with bias=True, BIASED).  No instance uses both, so
+  // they share the slots: a larger GemmP costs the existing instances registers.
+  union { const __nv_bfloat16* scale; const __nv_bfloat16* bias; };
+  union { const __nv_bfloat16* scale3; const __nv_bfloat16* bias3; };
 };
 
 constexpr int GEMM_THREADS = 288;
 
-template <int EPI, bool SCALED>
+template <int EPI, bool SCALED, bool BIASED>
 __device__ __forceinline__ void gemm_apply(const GemmP& p, int n, int j, float y, float y3) {
   if (SCALED) {
     y *= bf16_to_f32(p.scale[j]);
     if (EPI == G_SWIGLU) y3 *= bf16_to_f32(p.scale3[j]);
+  }
+  if (BIASED) {
+    y += bf16_to_f32(p.bias[j]);
+    if (EPI == G_SWIGLU) y3 += bf16_to_f32(p.bias3[j]);
   }
   if (EPI == G_STORE) {
     p.out[(size_t)n * p.ldo + j] = y;
@@ -57,6 +63,8 @@ __device__ __forceinline__ void gemm_apply(const GemmP& p, int n, int j, float y
     p.out[(size_t)n * p.ldo + j] += y;
   } else if (EPI == G_SWIGLU) {
     p.out[(size_t)n * p.ldo + j] = (y / (1.f + expf(-y))) * y3;
+  } else if (EPI == G_GELU) {   // nn.GELU(approximate='none'): the exact erf form
+    p.out[(size_t)n * p.ldo + j] = 0.5f * y * (1.f + erff(y * (float)M_SQRT1_2));
   } else {
     p.out[(size_t)n * p.ldo + j] = y;
     if (j >= p.D) {
@@ -74,9 +82,10 @@ __device__ __forceinline__ void gemm_apply(const GemmP& p, int n, int j, float y
 }
 
 // NC = n8 column chunks the accumulator holds (>= Rpad / 8; the chunks past Rpad / 8 are skipped at run time).
-// SCALED: int8 weights, p.scale (p.scale3) multiply each output row after the sum; a template flag, so that the bf16
-// instances compile exactly as without it.
-template <int EPI, int NC, bool SCALED>
+// SCALED: int8 weights, p.scale (p.scale3) multiply each output row after the sum; BIASED: p.bias (p.bias3) are added to
+// it.  Both are template flags, so that the unscaled bias-free instances compile exactly as without them; no instance has
+// both.
+template <int EPI, int NC, bool SCALED, bool BIASED>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA3,
           const __grid_constant__ CUtensorMap tmB, const GemmP p) {
@@ -119,7 +128,7 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         const int n = 8 * c + n0 + (e & 1), j = tile * 128 + rl0 + 8 * (e >> 1);
-        if (c < nc && n < p.R && j < p.M) gemm_apply<EPI, SCALED>(p, n, j, acc[0][c][e], acc[NA - 1][c][e]);
+        if (c < nc && n < p.R && j < p.M) gemm_apply<EPI, SCALED, BIASED>(p, n, j, acc[0][c][e], acc[NA - 1][c][e]);
       }
     return;
   }
@@ -155,7 +164,7 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
         y += __ldcg(ps + (size_t)n * 128);
         if (NA == 2) y3 += __ldcg(ps + (size_t)(p.Rpad + n) * 128);
       }
-      if (j < p.M) gemm_apply<EPI, SCALED>(p, n, j, y, y3);
+      if (j < p.M) gemm_apply<EPI, SCALED, BIASED>(p, n, j, y, y3);
     }
   }
   asm volatile("bar.sync 1, 256;" ::: "memory");
@@ -168,10 +177,15 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
   }
 }
 
-// B-operand preparation: one CTA per activation row.  Optional RMSNorm (fast_model.py:250-261: fp32
-// statistics, then gain), then the exact two-term bf16 split x = hi + lo.
+// B-operand preparation: one CTA per activation row.  Optional norm, then the exact two-term bf16 split x = hi + lo.
+//   LAYER = false: RMSNorm when gain != null (fast_model.py:250-261: fp32 statistics, then gain), else none.
+//   LAYER = true : LayerNorm (layers/layers.py:8-17, F.layer_norm): fp32 mean, then the biased variance as a second pass
+//                  over the centred row, (x - mean) * rsqrt(var + eps) * gain (+ beta when non-null); gain is required.
+// A template flag, so that the RMS / no-norm instance stage 1 uses compiles exactly as without it.
+template <bool LAYER>
 static __global__ void __launch_bounds__(256) k_prep_b(const float* __restrict__ x, int ldx, const __nv_bfloat16* __restrict__ gain,
-                                                float eps, int K, int Rpad, int R, int split_lo, __nv_bfloat16* __restrict__ B) {
+                                                const __nv_bfloat16* __restrict__ beta, float eps, int K, int Rpad, int R,
+                                                int split_lo, __nv_bfloat16* __restrict__ B) {
   __shared__ float red[8];
   const int n = blockIdx.x, tid = threadIdx.x;
   if (n >= R) {  // padding rows [R, Rpad) of the B operand must read as zero
@@ -183,6 +197,38 @@ static __global__ void __launch_bounds__(256) k_prep_b(const float* __restrict__
     return;
   }
   const float* xr = x + (size_t)n * ldx;
+  if (LAYER) {
+    float s = 0.f;
+    for (int k = tid; k < K; k += 256) s += xr[k];
+    s = warp_sum(s);
+    if ((tid & 31) == 0) red[tid >> 5] = s;
+    __syncthreads();
+    float t = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) t += red[i];
+    const float mean = t / (float)K;
+    __syncthreads();                       // every thread has read red before it is reused
+    float ss = 0.f;
+    for (int k = tid; k < K; k += 256) {
+      const float d = xr[k] - mean;
+      ss = fmaf(d, d, ss);
+    }
+    ss = warp_sum(ss);
+    if ((tid & 31) == 0) red[tid >> 5] = ss;
+    __syncthreads();
+    t = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) t += red[i];
+    const float rs = rsqrtf(t / (float)K + eps);
+    for (int k = tid; k < K; k += 256) {
+      float v = ((xr[k] - mean) * rs) * bf16_to_f32(gain[k]);
+      if (beta != nullptr) v += bf16_to_f32(beta[k]);
+      const __nv_bfloat16 h = __float2bfloat16_rn(v);
+      B[(size_t)n * K + k] = h;
+      if (split_lo) B[(size_t)(Rpad + n) * K + k] = lo_term(v, h);
+    }
+    return;
+  }
   float rs = 1.f;
   if (gain != nullptr) {
     float ss = 0.f;

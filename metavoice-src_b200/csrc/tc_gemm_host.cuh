@@ -7,7 +7,7 @@
 
 namespace mvb {
 
-enum { G_STORE = 0, G_RESID = 1, G_SWIGLU = 2, G_QKV = 3 };
+enum { G_STORE = 0, G_RESID = 1, G_SWIGLU = 2, G_QKV = 3, G_GELU = 4 };
 
 constexpr int GEMM_A_BYTES = 128 * 64 * 2;  // one 128-row x 64-k bf16 tile
 // SM count the engine workspaces size the split-K scratch for.  plan_gemm never plans for more SMs, so the reserved
@@ -98,16 +98,18 @@ static inline GemmPlan plan_gemm(int M, int K, int NB, bool swiglu, int n_sm, in
   return g;
 }
 
-// One projection on the tensor cores: k_prep_b stages the R input rows (optional RMSNorm, then the bf16 hi / lo split)
-// in B, then k_tc_gemm computes out[n, j] (+)= f(x)[n, :] . W[j, :] with epilogue `epi`.
+// One projection on the tensor cores: k_prep_b stages the R input rows (optional RMSNorm or LayerNorm, then the bf16
+// hi / lo split) in B, then k_tc_gemm computes out[n, j] (+)= f(x)[n, :] . W[j, :] (+ bias[j]) with epilogue `epi`.
 struct TcGemm {
-  int epi;                                        // G_STORE / G_RESID / G_SWIGLU / G_QKV
+  int epi;                                        // G_STORE / G_RESID / G_SWIGLU / G_QKV / G_GELU
   const CUtensorMap* tmW;                         // weight [M, K], 128-row boxes
   const CUtensorMap* tmW3;                        // G_SWIGLU: the second weight (silu(x W^T) * (x W3^T))
   __nv_bfloat16* B;                               // activation operand [Rpad * (1 + split_lo), K]
   const CUtensorMap* tmB;                         // map over B with one box of all its rows
   const float* x; int ldx;                        // input rows
-  const __nv_bfloat16* gain; float eps;           // RMSNorm gain, or null
+  const __nv_bfloat16* gain; float eps;           // RMSNorm (LayerNorm when layer_norm) gain, or null: no norm
+  int layer_norm;                                 // with gain: LayerNorm, (x - mean) * rstd * gain (+ beta)
+  const __nv_bfloat16* beta;                      // LayerNorm bias, or null
   int M, K;
   int R, Rpad, split_lo;                          // rows, rows reserved in B (multiple of 16, <= 128), lo terms carried
   float* out; int ldo;
@@ -120,6 +122,8 @@ struct TcGemm {
   int ksplit;                                     // > 0: force the K split (tests)
   const __nv_bfloat16* scale;                     // int8 weights: bf16 [M] row scales of W, or null
   const __nv_bfloat16* scale3;                    // G_SWIGLU: those of W3
+  const __nv_bfloat16* bias;                      // bf16 [M] Linear bias of W, or null (never with scale or G_QKV)
+  const __nv_bfloat16* bias3;                     // G_SWIGLU with bias: that of W3
 };
 cudaError_t tc_gemm(cudaStream_t s, const TcGemm& a);
 

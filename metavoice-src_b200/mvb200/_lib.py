@@ -14,6 +14,8 @@ GLOBAL_TENSORS, LAYER_TENSORS = 5, 7
 # `options` bits of the engine configs (include/mvb200.h): reference and identity paths, fixed at create time
 MVB_S1_NO_ROWS_PATH, MVB_S1_NO_RESIDENT, MVB_S1_UNFUSED_SAMPLER, MVB_S1_TRACE = 0x1, 0x2, 0x4, 0x8
 MVB_S2_EAGER = 0x1
+MVB_S2_NORM_RMS, MVB_S2_NORM_LAYER = 0, 1          # mvb_s2_arch.norm
+MVB_S2_MLP_SWIGLU, MVB_S2_MLP_GELU = 0, 1          # mvb_s2_arch.mlp
 MVB_MBD_CUDA_CORES, MVB_MBD_ONE_STREAM = 0x1, 0x2
 SPK_MAX_BATCH, RESAMPLE_MAX_TAPS = 32, 16384      # MVB_SPK_MAX_BATCH, MVB_RESAMPLE_MAX_TAPS
 
@@ -35,6 +37,10 @@ class S2Config(C.Structure):
                 ("block_size", C.c_int32), ("n_in", C.c_int32), ("vocab_in", C.c_int32 * 8), ("n_out", C.c_int32),
                 ("vocab_out", C.c_int32 * 8), ("spk_dim", C.c_int32), ("norm_eps", C.c_float), ("max_batch", C.c_int32),
                 ("options", C.c_int32)]
+
+
+class S2Arch(C.Structure):
+    _fields_ = [("norm", C.c_int32), ("mlp", C.c_int32), ("bias", C.c_int32)]
 
 
 class VocConfig(C.Structure):
@@ -100,6 +106,8 @@ SIGNATURES = {
     "mvb_s2_workspace_bytes": (C.c_size_t, [C.POINTER(S2Config)]),
     "mvb_s2_create": (C.c_int, [C.POINTER(S2Config), C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64), C.c_void_p,
                                 C.POINTER(C.c_void_p)]),
+    "mvb_s2_create_ex": (C.c_int, [C.POINTER(S2Config), C.POINTER(S2Arch), C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64),
+                                   C.c_void_p, C.POINTER(C.c_void_p)]),
     "mvb_s2_destroy": (C.c_int, [C.c_void_p]),
     "mvb_s2_forward": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_float, C.c_int32, C.c_void_p,
                                  C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -178,6 +186,9 @@ SIGNATURES = {
                                      C.c_void_p]),
     "mvb_s2_embed_test": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                     C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "mvb_s2_linear_test": (C.c_int, [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                     C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_float, C.c_int32, C.c_int32,
+                                     C.c_void_p, C.c_int32, C.c_void_p]),
     "mvb_voc_op_test": (C.c_int, [C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                   C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "mvb_enc_op_test": (C.c_int, [C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,

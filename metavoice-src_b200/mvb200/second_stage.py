@@ -7,7 +7,8 @@ Token adapters (integer bucketing, SURVEY.md rows a12/a16) stay on the host exac
 """
 from __future__ import annotations
 
-from typing import List, Optional, Sequence
+import ctypes as C
+from typing import List, Optional, Sequence, Tuple
 
 import torch
 
@@ -60,8 +61,37 @@ def build_stage2_input(text_ids: Sequence[int], codes: Sequence[Sequence[int]], 
 _GLOBAL = lambda n_in, n_out: ([f"transformer.wtes.{i}.weight" for i in range(n_in)] +
                                ["transformer.wpe.weight", "speaker_cond_pos.weight", "transformer.ln_f.weight"] +
                                [f"lm_heads.{i}.weight" for i in range(n_out)])
-_LAYER = ["ln_1.weight", "attn.c_attn.weight", "attn.c_proj.weight", "ln_2.weight", "mlp.swiglu.w1.weight",
-          "mlp.swiglu.w3.weight", "mlp.c_proj.weight"]
+_NORMS = {"rmsnorm": _lib.MVB_S2_NORM_RMS, "layernorm": _lib.MVB_S2_NORM_LAYER}
+_MLPS = {"swiglu": _lib.MVB_S2_MLP_SWIGLU, "gelu": _lib.MVB_S2_MLP_GELU}
+
+
+def stage2_arch(model_args: dict) -> Tuple[str, str, bool]:
+    """(norm_type, nonlinearity_type, bias) of a second-stage ``model_args``, a missing key meaning GPTConfig's default
+    (model.py:36-43: bias=True, norm_type="layernorm", nonlinearity_type="gelu"), as ``GPTConfig(**model_args)`` reads
+    it.  A value libmvb200 does not build raises NotImplementedError naming it."""
+    norm = model_args.get("norm_type", "layernorm")
+    mlp = model_args.get("nonlinearity_type", "gelu")
+    bias = model_args.get("bias", True)
+    if norm not in _NORMS:
+        raise NotImplementedError(f"libmvb200 stage 2: norm_type {norm!r} is not supported (rmsnorm, layernorm)")
+    if mlp not in _MLPS:
+        raise NotImplementedError(f"libmvb200 stage 2: nonlinearity_type {mlp!r} is not supported (swiglu, gelu)")
+    if bias not in (True, False):
+        raise NotImplementedError(f"libmvb200 stage 2: bias {bias!r} is not supported (True, False)")
+    return norm, mlp, bool(bias)
+
+
+def stage2_keys(n_in: int, n_out: int, n_layer: int, norm: str, mlp: str, bias: bool) -> List[str]:
+    """State-dict keys in the order of mvb_s2_create_ex's offset list (include/mvb200.h)."""
+    ffn = ["mlp.c_fc"] if mlp == "gelu" else ["mlp.swiglu.w1", "mlp.swiglu.w3"]
+    layer = ["ln_1", "attn.c_attn", "attn.c_proj", "ln_2"] + ffn + ["mlp.c_proj"]
+    keys = _GLOBAL(n_in, n_out) + [f"transformer.h.{l}.{k}.weight" for l in range(n_layer) for k in layer]
+    if bias:
+        ln = norm == "layernorm"
+        keys += ["transformer.ln_f.bias"] if ln else []
+        with_bias = [k for k in layer if ln or not k.startswith("ln_")]
+        keys += [f"transformer.h.{l}.{k}.bias" for l in range(n_layer) for k in with_bias]
+    return keys
 
 
 class SecondStage(Engine):
@@ -71,17 +101,16 @@ class SecondStage(Engine):
         a = checkpoint["model_args"]
         if a.get("causal", True):
             raise ValueError("second-stage checkpoint must be non-causal")
-        if a.get("norm_type") != "rmsnorm" or a.get("nonlinearity_type") != "swiglu" or a.get("bias", False):
-            raise NotImplementedError("libmvb200 stage 2 supports rmsnorm + swiglu + bias=False checkpoints")
+        norm, mlp, bias = stage2_arch(a)
         if not a.get("spk_emb_on_text", True):
             # model.py:104-107: the reference itself refuses a non-causal model with spk_emb_on_text=False
             raise NotImplementedError("spk_emb_on_text=False is not supported for the non-causal second stage (model.py:104-107)")
         sd = {(k[len("_orig_mod."):] if k.startswith("_orig_mod.") else k): v for k, v in checkpoint["model"].items()}
         self.args = a
         self.n_in, self.n_out = len(a["vocab_sizes"]), len(a["target_vocab_sizes"])
-        keys = _GLOBAL(self.n_in, self.n_out) + [f"transformer.h.{l}.{k}" for l in range(a["n_layer"]) for k in _LAYER]
+        keys = stage2_keys(self.n_in, self.n_out, a["n_layer"], norm, mlp, bias)
         super().__init__(device, *pack_arena_bytes([sd[k].to(torch.bfloat16) for k in keys]))
-        hidden = sd["transformer.h.0.mlp.swiglu.w1.weight"].shape[0]
+        hidden = sd["transformer.h.0.mlp.c_fc.weight" if mlp == "gelu" else "transformer.h.0.mlp.swiglu.w1.weight"].shape[0]
         cfg = _lib.S2Config()
         cfg.n_layer, cfg.n_head, cfg.n_embd, cfg.hidden = a["n_layer"], a["n_head"], a["n_embd"], hidden
         cfg.block_size, cfg.n_in, cfg.n_out = a["block_size"], self.n_in, self.n_out
@@ -90,11 +119,13 @@ class SecondStage(Engine):
         for i, v in enumerate(a["target_vocab_sizes"]):
             cfg.vocab_out[i] = v
         cfg.spk_dim = sd["speaker_cond_pos.weight"].shape[1]
-        cfg.norm_eps = a.get("rmsnorm_eps") or 1e-5
+        cfg.norm_eps = a.get("rmsnorm_eps") or 1e-5     # RMSNorm only: LayerNorm's eps is 1e-5 in the library
         cfg.max_batch = max_batch
         cfg.options = 0 if cuda_graph else _lib.MVB_S2_EAGER
         self.cfg = cfg
-        self._create(self._lib.mvb_s2_create, self._lib.mvb_s2_destroy, cfg, self._lib.mvb_s2_workspace_bytes)
+        self.arch = _lib.S2Arch(_NORMS[norm], _MLPS[mlp], int(bias))
+        create = lambda cfg_p, *rest: self._lib.mvb_s2_create_ex(cfg_p, C.byref(self.arch), *rest)   # noqa: E731
+        self._create(create, self._lib.mvb_s2_destroy, cfg, self._lib.mvb_s2_workspace_bytes)
         self.tokenizer = tokenizer
         self.block_size = a["block_size"]
 

@@ -185,7 +185,8 @@ def dims_as_dict(d: Stage1Dims) -> dict:
 class Stage2Dims:
     """Shape of the non-causal codebook-expansion model (fam/llm/model.py:26-46 GPTConfig, causal=False).
     The real values live in second_stage.pt["model_args"] (not available offline); these defaults give the
-    "~10 Mn parameters" of README.md:164 and are only used for synthetic checkpoints."""
+    "~10 Mn parameters" of README.md:164 and are only used for synthetic checkpoints.  norm_type, nonlinearity_type
+    and bias select the architecture (GPTConfig's own defaults are "layernorm", "gelu", True)."""
 
     n_layer: int = 6
     n_head: int = 6
@@ -196,9 +197,14 @@ class Stage2Dims:
     speaker_emb_dim: int = 256
     rmsnorm_eps: float = 1e-5
     swiglu_multiple_of: int = 256
+    norm_type: str = "rmsnorm"
+    nonlinearity_type: str = "swiglu"
+    bias: bool = False
 
     @property
     def hidden(self) -> int:
+        if self.nonlinearity_type == "gelu":
+            return 4 * self.n_embd           # fam/llm/layers/layers.py:46
         h = int(2 * 4 * self.n_embd / 3)    # fam/llm/layers/layers.py:51-52
         m = self.swiglu_multiple_of
         return m * ((h + m - 1) // m)
@@ -209,15 +215,18 @@ S2_TINY = Stage2Dims(n_layer=2, n_head=2, n_embd=128, block_size=256)
 
 
 def stage2_model_args(d: Stage2Dims) -> dict:
-    return dict(n_layer=d.n_layer, n_head=d.n_head, n_embd=d.n_embd, block_size=d.block_size, bias=False,
+    return dict(n_layer=d.n_layer, n_head=d.n_head, n_embd=d.n_embd, block_size=d.block_size, bias=d.bias,
                 vocab_sizes=list(d.vocab_sizes), target_vocab_sizes=list(d.target_vocab_sizes), causal=False,
-                norm_type="rmsnorm", rmsnorm_eps=d.rmsnorm_eps, nonlinearity_type="swiglu",
+                norm_type=d.norm_type, rmsnorm_eps=d.rmsnorm_eps, nonlinearity_type=d.nonlinearity_type,
                 swiglu_multiple_of=d.swiglu_multiple_of, attn_kernel_type="torch_attn", spk_emb_on_text=True, dropout=0.0)
 
 
 def stage2_state_dict(d: Stage2Dims, seed: int = 1) -> Dict[str, torch.Tensor]:
-    """bf16 state dict with the slow-path GPT key names (fam/llm/model.py:118-146)."""
+    """bf16 state dict with the slow-path GPT key names (fam/llm/model.py:118-146).  The default architecture's tensors
+    are drawn first, in a fixed order (GELU: c_fc in place of w1, no w3); then, with bias, LayerNorm betas 0.1 N(0, 1)
+    and Linear biases 0.02 N(0, 1), non-zero so that a dropped bias changes the output."""
     gen = torch.Generator().manual_seed(seed)
+    gelu, ln = d.nonlinearity_type == "gelu", d.norm_type == "layernorm"
     e, hd = d.n_embd, d.hidden
     proj_std = 0.02 / math.sqrt(2 * d.n_layer)
     gain = lambda: (1.0 + 0.1 * torch.empty(e).normal_(generator=gen)).to(torch.bfloat16)
@@ -231,13 +240,34 @@ def stage2_state_dict(d: Stage2Dims, seed: int = 1) -> Dict[str, torch.Tensor]:
         sd[p + "ln_2.weight"] = gain()
         sd[p + "attn.c_attn.weight"] = _normal(gen, (3 * e, e), 0.02)
         sd[p + "attn.c_proj.weight"] = _normal(gen, (e, e), proj_std)
-        sd[p + "mlp.swiglu.w1.weight"] = _normal(gen, (hd, e), 0.02)
-        sd[p + "mlp.swiglu.w3.weight"] = _normal(gen, (hd, e), 0.02)
+        if gelu:
+            sd[p + "mlp.c_fc.weight"] = _normal(gen, (hd, e), 0.02)
+        else:
+            sd[p + "mlp.swiglu.w1.weight"] = _normal(gen, (hd, e), 0.02)
+            sd[p + "mlp.swiglu.w3.weight"] = _normal(gen, (hd, e), 0.02)
         sd[p + "mlp.c_proj.weight"] = _normal(gen, (e, hd), proj_std)
     sd["transformer.ln_f.weight"] = gain()
     sd["speaker_cond_pos.weight"] = _normal(gen, (e, d.speaker_emb_dim), 0.02)
     for i, v in enumerate(d.target_vocab_sizes):
         sd[f"lm_heads.{i}.weight"] = _normal(gen, (v, e), 0.05)
+    if d.bias:
+        beta = lambda: _normal(gen, (e,), 0.1)      # noqa: E731
+        lin = lambda n: _normal(gen, (n,), 0.02)    # noqa: E731
+        if ln:
+            sd["transformer.ln_f.bias"] = beta()
+        for i in range(d.n_layer):
+            p = f"transformer.h.{i}."
+            if ln:
+                sd[p + "ln_1.bias"] = beta()
+                sd[p + "ln_2.bias"] = beta()
+            sd[p + "attn.c_attn.bias"] = lin(3 * e)
+            sd[p + "attn.c_proj.bias"] = lin(e)
+            if gelu:
+                sd[p + "mlp.c_fc.bias"] = lin(hd)
+            else:
+                sd[p + "mlp.swiglu.w1.bias"] = lin(hd)
+                sd[p + "mlp.swiglu.w3.bias"] = lin(hd)
+            sd[p + "mlp.c_proj.bias"] = lin(e)
     return sd
 
 
