@@ -88,6 +88,31 @@ int mvb_s1_create(const mvb_s1_config* cfg, const void* d_arena, size_t arena_by
                   const uint64_t* offsets, void* d_kv, void* d_workspace, mvb_s1** out);
 int mvb_s1_destroy(mvb_s1* h);
 
+/* Stage-1 architecture: the GPTConfig fields (fam/llm/model.py:26-46) norm_type, nonlinearity_type and bias of the
+ * reference's causal GPT (model.py:195-314, layers/attn.py, layers/combined.py, layers/layers.py), served by its slow
+ * path fam.llm.inference (inference.py:102-156).  All zero = rmsnorm, swiglu, no bias: the production engine.  A field
+ * outside its values is MVB_ERR_ARG naming it. */
+typedef struct mvb_s1_arch {
+  int32_t norm;            /* MVB_S1_NORM_*: ln_1, ln_2 and ln_f */
+  int32_t mlp;             /* MVB_S1_MLP_* */
+  int32_t bias;            /* 1: biases on attn.c_attn (k and v are cached with theirs), attn.c_proj, every MLP Linear and
+                            * (LayerNorm) ln_1, ln_2, ln_f; speaker_cond_pos and the head (tied to wtes.0) never have one */
+} mvb_s1_arch;
+#define MVB_S1_NORM_RMS    0   /* RMSNorm(eps = norm_eps), layers.py:20-30 */
+#define MVB_S1_NORM_LAYER  1   /* LayerNorm(eps = 1e-5), with a beta when bias, layers.py:8-17 */
+#define MVB_S1_MLP_SWIGLU  0   /* c_proj(silu(w1 x) * (w3 x)) */
+#define MVB_S1_MLP_GELU    1   /* c_proj(GELU(c_fc x)), exact erf GELU (nn.GELU()); cfg->intermediate = 4 dim */
+/* mvb_s1_create with an architecture; mvb_s1_create == mvb_s1_create_ex with arch NULL (all zero).  The offset list is
+ * mvb_s1_create's (MVB_S1_GLOBAL_TENSORS, then per layer {ln_1, attn.c_attn, attn.c_proj, ln_2, mlp.swiglu.w1,
+ * mlp.swiglu.w3, mlp.c_proj}; GELU: {ln_1, attn.c_attn, attn.c_proj, ln_2, mlp.c_fc, mlp.c_proj}); then, when
+ * arch->bias: ln_f.bias (LayerNorm only), and per layer {ln_1.bias (LayerNorm only), attn.c_attn.bias, attn.c_proj.bias,
+ * ln_2.bias (LayerNorm only), mlp.c_fc.bias | mlp.swiglu.w1.bias, mlp.swiglu.w3.bias, mlp.c_proj.bias}, all bf16.  The
+ * KV and workspace sizes do not depend on arch.  Any architecture but the production one decodes one utterance on the
+ * CUDA-core GEMVs and a batch on the tensor-core rows path (MVB_S1_NO_ROWS_PATH: everything on the GEMVs), never in the
+ * resident decode kernel, and prefills on the tensor cores. */
+int mvb_s1_create_ex(const mvb_s1_config* cfg, const mvb_s1_arch* arch, const void* d_arena, size_t arena_bytes,
+                     const uint64_t* offsets, void* d_kv, void* d_workspace, mvb_s1** out);
+
 /* Hoisted speaker conditioning: spk_proj[utt] = W_spk * spk_emb (fast_model.py:152-157 recomputes it
  * every step; it only changes per utterance).  d_spk_emb: fp32 [spk_dim] on device. */
 int mvb_s1_set_speaker(mvb_s1* h, int32_t utt, const float* d_spk_emb, void* stream);
@@ -305,6 +330,23 @@ int mvb_w8_gemm_test(int32_t epi, const void* d_W, const void* d_W3, const void*
                      const int32_t* d_row_cache, const int32_t* d_row_pos, int32_t H, int32_t S_max, int32_t D,
                      int32_t kv_fp32, void* stream);
 int mvb_w8_widen_test(const void* d_W, int32_t M, int32_t K, void* d_out, void* stream);
+/* Test hook for the projections of a non-production stage-1 architecture (not part of the drop-in surface):
+ *   path 0: k_gemv as path A launches it, for utterances u in [0, n_utts): rows 2 s, 2 s + 1 (s = d_slot_map[u]) of d_x
+ *           fp32 [*, ldx] and d_out [*, ldo]; out = epilogue(f(x) . W^T + bias); norm 0 none, 1 RMSNorm (d_gain, eps),
+ *           2 LayerNorm (d_gain, optional d_beta, eps); epi 0 store, 1 residual add, 2 SwiGLU silu(x W^T + bias) *
+ *           (x W3^T + bias3), 3 QKV plus the K / V thirds (with their bias) scattered to d_kcache / d_vcache
+ *           [rows][H][S_max][128] at position d_pos[s] (D = 128 H, M = 3 D), 4 GELU (exact erf).  d_bias, d_bias3 bf16
+ *           [M] or NULL.  K % 256 == 0, 2 K floats <= 96 KB.
+ *   path 1: the QKV epilogue of k_tc_gemm (epi must be 3) over R = 2 n_utts activation rows n of d_x / d_out, row n
+ *           scattering to cache row 2 s + (n & 1) at position d_pos[s], s = d_slot_map[n >> 1]; the norm as above (the
+ *           k_prep_b prologue), the bias added once per output after the split-K sum; ksplit_override > 0 forces the K
+ *           split.  K % 64 == 0.  Row scratch is allocated per call.
+ * Synchronises `stream`. */
+int mvb_s1_arch_gemv_test(int32_t path, int32_t epi, int32_t norm, const void* d_W, const void* d_W3, const void* d_bias,
+                          const void* d_bias3, int32_t M, int32_t K, const float* d_x, int32_t ldx, int32_t n_utts,
+                          const void* d_gain, const void* d_beta, float eps, float* d_out, int32_t ldo, void* d_kcache,
+                          void* d_vcache, const int32_t* d_slot_map, const int32_t* d_pos, int32_t H, int32_t S_max,
+                          int32_t D, int32_t kv_fp32, int32_t ksplit_override, void* stream);
 int mvb_mbd_conv_test(int32_t kind, const float* d_x, int32_t Cin, int32_t Tin, const float* d_w, int32_t Cout, int32_t K,
                       int32_t stride, int32_t dil, int32_t pad, const float* d_gn_stats, const float* d_gn_w,
                       const float* d_gn_b, int32_t groups, const float* d_bias, const float* d_emb, const float* d_resid,

@@ -30,8 +30,8 @@ static cudaError_t launch_tc_gemm_sc(cudaStream_t s, const CUtensorMap& tA, cons
   return launch_tc_gemm_nc<EPI, 16, SCALED, BIASED>(s, tA, tA3, tB, p, g);
 }
 
-// Instances: int8 row scales on every epilogue but G_GELU, Linear biases on every epilogue but G_QKV, never both (they
-// share GemmP's per-row vector slots).
+// Instances: int8 row scales on every epilogue but G_GELU, Linear biases on every epilogue, never both (they share
+// GemmP's per-row vector slots).
 template <int EPI>
 static cudaError_t launch_tc_gemm(cudaStream_t s, const CUtensorMap& tA, const CUtensorMap& tA3, const CUtensorMap& tB,
                                   GemmP p, const GemmPlan& g, bool scaled, bool biased) {
@@ -40,9 +40,7 @@ static cudaError_t launch_tc_gemm(cudaStream_t s, const CUtensorMap& tA, const C
   if constexpr (EPI != G_GELU) {
     if (scaled) return launch_tc_gemm_sc<EPI, true, false>(s, tA, tA3, tB, p, g);
   }
-  if constexpr (EPI != G_QKV) {
-    if (biased) return launch_tc_gemm_sc<EPI, false, true>(s, tA, tA3, tB, p, g);
-  }
+  if (biased) return launch_tc_gemm_sc<EPI, false, true>(s, tA, tA3, tB, p, g);
   if (scaled || biased) return cudaErrorInvalidValue;
   return launch_tc_gemm_sc<EPI, false, false>(s, tA, tA3, tB, p, g);
 }
@@ -122,6 +120,12 @@ int run_gemm(TcGemm a, const void* d_W, const void* d_W3, cudaStream_t s) {
 }
 
 }  // namespace
+
+namespace mvb {
+int tc_gemm_test(const TcGemm& a, const void* d_W, const void* d_W3, void* stream) {
+  return run_gemm(a, d_W, d_W3, (cudaStream_t)stream);
+}
+}  // namespace mvb
 
 extern "C" int mvb_linear(const void* d_W, int32_t M, int32_t K, const float* d_x, int32_t ldx, int32_t R,
                           const void* d_gain, float eps, int32_t split_lo, int32_t ksplit_override, float* d_out,

@@ -121,8 +121,17 @@ static WsLayout make_layout(const mvb_s1_config& c) {
   return L;
 }
 
+// Per-layer norm parameters and Linear biases of a non-production architecture (null where it has none).
+struct S1LayerP {
+  const __nv_bfloat16 *g1, *b1, *g2, *b2;                   // ln_1 / ln_2 gain and (LayerNorm with bias) beta
+  const __nv_bfloat16 *qkv_b, *o_b, *fc_b, *fc3_b, *proj_b;  // c_attn, attn.c_proj, c_fc | w1, w3, mlp.c_proj
+};
+
 struct mvb_s1 {
   mvb_s1_config cfg;
+  mvb_s1_arch arch{};                                 // all zero: the production architecture (rmsnorm, swiglu, no bias)
+  std::vector<S1LayerP> lp;
+  const __nv_bfloat16* lnf_b = nullptr;               // ln_f beta (LayerNorm with bias)
   int n_sm = 132;
   const char* arena = nullptr;
   std::vector<uint64_t> off;
@@ -162,7 +171,17 @@ struct mvb_s1 {
   template <typename T>
   T* wsp(size_t o) const { return reinterpret_cast<T*>(ws + o); }
   const __nv_bfloat16* w(int i) const { return reinterpret_cast<const __nv_bfloat16*>(arena + off[i]); }
-  const __nv_bfloat16* lw(int layer, int t) const { return w(MVB_S1_GLOBAL_TENSORS + layer * MVB_S1_LAYER_TENSORS + t); }
+  bool gelu() const { return arch.mlp == MVB_S1_MLP_GELU; }
+  bool layer_norm() const { return arch.norm == MVB_S1_NORM_LAYER; }
+  bool production_arch() const { return arch.norm == MVB_S1_NORM_RMS && arch.mlp == MVB_S1_MLP_SWIGLU && !arch.bias; }
+  // eps of ln_1 / ln_2 / ln_f: LayerNorm's is fixed at 1e-5 (layers/layers.py:17), RMSNorm's is the config's
+  float norm_eps() const { return layer_norm() ? 1e-5f : cfg.norm_eps; }
+  // arena tensor t of a layer (0 ln_1, 1 wqkv, 2 wo, 3 ln_2, 4 w1 | c_fc, 5 w3, 6 w2 = mlp.c_proj); a GELU layer has six
+  // tensors and no w3
+  const __nv_bfloat16* lw(int layer, int t) const {
+    const bool g = gelu();
+    return w(MVB_S1_GLOBAL_TENSORS + layer * (g ? 6 : MVB_S1_LAYER_TENSORS) + (g && t == 6 ? 5 : t));
+  }
   // The one weight-source accessor of the tensor-core path: the bf16 matrix t (1 wqkv, 2 wo, 4 w1, 5 w3, 6 w2) of a layer,
   // i.e. the arena tensor, or for an int4 / int8 engine its slot in the layer scratch (k_w4_dequant / k_w8_widen fill it).
   const __nv_bfloat16* tc_w(int layer, int t) const {
@@ -211,6 +230,12 @@ static PcMat plan_pc(int M, int K, int ctas, int tile_rows) {
   return best;
 }
 
+// Largest K of a path-A GEMV: its two staged fp32 activation rows (2 K floats) must fit in the opt-in shared memory of
+// two co-resident CTAs.  The int4 and int8 GEMVs, and every kernel of the resident decode kernel's engine, keep the
+// default 48 KB (quant_staging_ok, pc_ok).
+constexpr size_t GEMV_MAX_SMEM = 96 * 1024;
+static bool default_staging_ok(const mvb_s1_config& c) { return (size_t)c.intermediate * 8 <= 48 * 1024 - 256; }
+
 static int validate(const mvb_s1_config* c) {
   if (!c) return set_error(MVB_ERR_ARG, "null config");
   if (c->head_dim != 128) return set_error(MVB_ERR_UNSUPPORTED, "head_dim must be 128 (got %d)", c->head_dim);
@@ -220,7 +245,7 @@ static int validate(const mvb_s1_config* c) {
   if (c->max_utts < 1 || c->max_utts > 64) return set_error(MVB_ERR_ARG, "max_utts out of range");
   if (c->max_new < 1 || c->max_new > c->block_size) return set_error(MVB_ERR_ARG, "max_new out of range");
   if (c->kv_dtype != MVB_KV_BF16 && c->kv_dtype != MVB_KV_FP32) return set_error(MVB_ERR_ARG, "bad kv_dtype");
-  if ((size_t)c->intermediate * 8 > 48 * 1024 - 256) return set_error(MVB_ERR_UNSUPPORTED, "intermediate too large for the staging buffer");
+  if ((size_t)c->intermediate * 8 > GEMV_MAX_SMEM) return set_error(MVB_ERR_UNSUPPORTED, "intermediate too large for the staging buffer");
   const int known = MVB_S1_NO_ROWS_PATH | MVB_S1_NO_RESIDENT | MVB_S1_UNFUSED_SAMPLER | MVB_S1_TRACE;
   if (c->options & ~known) return set_error(MVB_ERR_ARG, "options: undefined bits 0x%x", (unsigned)(c->options & ~known));
   return MVB_OK;
@@ -237,20 +262,50 @@ extern "C" size_t mvb_s1_workspace_bytes(const mvb_s1_config* c) {
   return make_layout(*c).total;
 }
 
+// The int4 / int8 GEMVs stage their activations in the default 48 KB of shared memory.
+static int quant_staging_ok(const mvb_s1_config* c) {
+  if (!default_staging_ok(*c)) return set_error(MVB_ERR_UNSUPPORTED, "intermediate too large for the staging buffer");
+  return MVB_OK;
+}
+
 extern "C" size_t mvb_s1_int4_workspace_bytes(const mvb_s1_config* c) {
-  if (validate(c)) return 0;
+  if (validate(c) || quant_staging_ok(c)) return 0;
   return make_layout(*c).total_int4;
 }
 
 extern "C" size_t mvb_s1_int8_workspace_bytes(const mvb_s1_config* c) {
-  if (validate(c)) return 0;
+  if (validate(c) || quant_staging_ok(c)) return 0;
   return make_layout(*c).total_int8;
 }
 
-static int create_engine(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
-                         void* d_kv, void* d_ws, mvb_s1** out, WFmt fmt) {
+// Tensors in the offset list: the weights (GELU: six per layer), then, with bias, ln_f.bias (LayerNorm) and per layer
+// {ln_1.bias (LayerNorm), c_attn.bias, attn.c_proj.bias, ln_2.bias (LayerNorm), w1.bias, w3.bias | c_fc.bias,
+// mlp.c_proj.bias}.
+static int s1_offset_count(const mvb_s1_config* c, const mvb_s1_arch& a) {
+  const bool ln = a.norm == MVB_S1_NORM_LAYER, gelu = a.mlp == MVB_S1_MLP_GELU;
+  int n = MVB_S1_GLOBAL_TENSORS + c->n_layer * (gelu ? 6 : MVB_S1_LAYER_TENSORS);
+  if (a.bias) n += (ln ? 1 : 0) + c->n_layer * ((ln ? 2 : 0) + 3 + (gelu ? 1 : 2));
+  return n;
+}
+
+static int s1_validate_arch(const mvb_s1_arch& a) {
+  if (a.norm != MVB_S1_NORM_RMS && a.norm != MVB_S1_NORM_LAYER) return set_error(MVB_ERR_ARG, "arch.norm: undefined value %d", a.norm);
+  if (a.mlp != MVB_S1_MLP_SWIGLU && a.mlp != MVB_S1_MLP_GELU) return set_error(MVB_ERR_ARG, "arch.mlp: undefined value %d", a.mlp);
+  if (a.bias != 0 && a.bias != 1) return set_error(MVB_ERR_ARG, "arch.bias: undefined value %d", a.bias);
+  return MVB_OK;
+}
+
+static int create_engine(const mvb_s1_config* cfg, const mvb_s1_arch* arch, const void* d_arena, size_t arena_bytes,
+                         const uint64_t* offsets, void* d_kv, void* d_ws, mvb_s1** out, WFmt fmt) {
   if (int e = validate(cfg)) return e;
-  if (!d_arena || !offsets || !d_kv || !d_ws || !out) return set_error(MVB_ERR_ARG, "null pointer argument");
+  if (fmt != WFmt::BF16)
+    if (int e = quant_staging_ok(cfg)) return e;
+  const mvb_s1_arch a = arch ? *arch : mvb_s1_arch{};
+  if (int e = s1_validate_arch(a)) return e;
+  if (!offsets) return set_error(MVB_ERR_ARG, "null pointer argument");
+  const int n_off = s1_offset_count(cfg, a);
+  if (int e = check_offsets(offsets, n_off, arena_bytes, "weight offset")) return e;
+  if (!d_arena || !d_kv || !d_ws || !out) return set_error(MVB_ERR_ARG, "null pointer argument");
   int dev = 0, n_sm = 0, major = 0, minor = 0;
   if (int e = current_device(&dev, &n_sm)) return e;
   MVB_CK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
@@ -259,11 +314,29 @@ static int create_engine(const mvb_s1_config* cfg, const void* d_arena, size_t a
   Building<mvb_s1> hb(new mvb_s1(), mvb_s1_destroy);
   mvb_s1* h = hb.get();
   h->cfg = *cfg;
+  h->arch = a;
   h->n_sm = n_sm;
   h->arena = reinterpret_cast<const char*>(d_arena);
-  const int n_off = MVB_S1_GLOBAL_TENSORS + cfg->n_layer * MVB_S1_LAYER_TENSORS;
-  if (int e = check_offsets(offsets, n_off, arena_bytes, "weight offset")) return e;
   h->off.assign(offsets, offsets + n_off);
+  if (!h->production_arch()) {
+    const bool ln = h->layer_norm(), gelu = h->gelu();
+    int nb = s1_offset_count(cfg, mvb_s1_arch{a.norm, a.mlp, 0});    // first bias slot
+    auto bias_slot = [&](bool present) { return present && a.bias ? h->w(nb++) : nullptr; };
+    h->lnf_b = bias_slot(ln);
+    h->lp.resize(cfg->n_layer);
+    for (int l = 0; l < cfg->n_layer; ++l) {
+      S1LayerP& p = h->lp[l];
+      p.g1 = h->lw(l, 0);
+      p.g2 = h->lw(l, 3);
+      p.b1 = bias_slot(ln);
+      p.qkv_b = bias_slot(true);
+      p.o_b = bias_slot(true);
+      p.b2 = bias_slot(ln);
+      p.fc_b = bias_slot(true);
+      p.fc3_b = bias_slot(!gelu);
+      p.proj_b = bias_slot(true);
+    }
+  }
   h->kv = reinterpret_cast<char*>(d_kv);
   h->ws = reinterpret_cast<char*>(d_ws);
   h->L = make_layout(*cfg);
@@ -323,7 +396,7 @@ static int create_engine(const mvb_s1_config* cfg, const void* d_arena, size_t a
       ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 0], h->tc_w(l, 1), 3 * D, D, 128);
       ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 1], h->tc_w(l, 2), D, D, 128);
       ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 2], h->tc_w(l, 4), F, D, 128);
-      ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 3], h->tc_w(l, 5), F, D, 128);
+      ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 3], h->tc_w(l, h->gelu() ? 4 : 5), F, D, 128);   // GELU: c_fc again
       ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 4], h->tc_w(l, 6), D, F, 128);
     }
     ok = ok && make_tmap_bf16(&h->tmW[(size_t)cfg->n_layer * 5], fmt == WFmt::INT8 ? h->w8_head : h->w(4), cfg->vocab, D, 128);
@@ -343,7 +416,8 @@ static int create_engine(const mvb_s1_config* cfg, const void* d_arena, size_t a
   {
     // persistent decode kernel: needs a uniform layer stride (true for arenas packed in checkpoint order)
     const int D = cfg->dim, F = cfg->intermediate, V = cfg->vocab;
-    bool ok = cfg->n_layer >= 1 && fmt == WFmt::BF16 && kv_ok;   // an int4 or int8 engine never uses path C
+    // an int4 or int8 engine, and any architecture but the production one, never uses path C
+    bool ok = cfg->n_layer >= 1 && fmt == WFmt::BF16 && kv_ok && h->production_arch() && default_staging_ok(*cfg);
     const int o0 = MVB_S1_GLOBAL_TENSORS;
     uint64_t stride = cfg->n_layer > 1 ? h->off[o0 + MVB_S1_LAYER_TENSORS] - h->off[o0] : 2 * (uint64_t)(4 * D * D + 3 * D * F + 2 * D);
     for (int l = 1; l < cfg->n_layer && ok; ++l)
@@ -380,19 +454,24 @@ static int create_engine(const mvb_s1_config* cfg, const void* d_arena, size_t a
   return MVB_OK;
 }
 
+extern "C" int mvb_s1_create_ex(const mvb_s1_config* cfg, const mvb_s1_arch* arch, const void* d_arena, size_t arena_bytes,
+                                const uint64_t* offsets, void* d_kv, void* d_ws, mvb_s1** out) {
+  return create_engine(cfg, arch, d_arena, arena_bytes, offsets, d_kv, d_ws, out, WFmt::BF16);
+}
+
 extern "C" int mvb_s1_create(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
                              void* d_kv, void* d_ws, mvb_s1** out) {
-  return create_engine(cfg, d_arena, arena_bytes, offsets, d_kv, d_ws, out, WFmt::BF16);
+  return mvb_s1_create_ex(cfg, nullptr, d_arena, arena_bytes, offsets, d_kv, d_ws, out);
 }
 
 extern "C" int mvb_s1_create_int4(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
                                   void* d_kv, void* d_ws, mvb_s1** out) {
-  return create_engine(cfg, d_arena, arena_bytes, offsets, d_kv, d_ws, out, WFmt::INT4);
+  return create_engine(cfg, nullptr, d_arena, arena_bytes, offsets, d_kv, d_ws, out, WFmt::INT4);
 }
 
 extern "C" int mvb_s1_create_int8(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
                                   void* d_kv, void* d_ws, mvb_s1** out) {
-  return create_engine(cfg, d_arena, arena_bytes, offsets, d_kv, d_ws, out, WFmt::INT8);
+  return create_engine(cfg, nullptr, d_arena, arena_bytes, offsets, d_kv, d_ws, out, WFmt::INT8);
 }
 
 extern "C" int mvb_s1_destroy(mvb_s1* h) {
@@ -431,16 +510,83 @@ static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 }
 
 // p.W / p.W3 are matrices of format `fmt`: bf16 (k_gemv), int4 packed (k_gemv_w4) or int8 (k_gemv_w8); all three take one
-// item per warp.
-template <int EPI>
+// item per warp.  LAYER (LayerNorm prologue) and BIASED (Linear biases) exist for bf16 only.  A K whose staging rows need
+// more than the default 48 KB of shared memory (a GELU c_proj, K = 4 dim) opts the bf16 instance in first.
+template <int EPI, bool LAYER = false, bool BIASED = false>
 static cudaError_t launch_gemv(mvb_s1* h, cudaStream_t s, int n_utts, GemvP p, WFmt fmt) {
   const int n_items = (EPI == EPI_SWIGLU) ? p.M : p.M / 2;
   dim3 grid(gemv_grid(n_items, h->n_sm), n_utts);
   const size_t smem = (size_t)2 * p.K * sizeof(float);
   h->launches++;
-  if (fmt == WFmt::INT4) return launch_pdl(k_gemv_w4<EPI>, grid, dim3(256), smem, s, p, h->st);
-  if (fmt == WFmt::INT8) return launch_pdl(k_gemv_w8<EPI>, grid, dim3(256), smem, s, p, h->st);
-  return launch_pdl(k_gemv<EPI>, grid, dim3(256), smem, s, p, h->st);
+  if constexpr (!LAYER && !BIASED && EPI != EPI_GELU) {
+    if (fmt == WFmt::INT4) return launch_pdl(k_gemv_w4<EPI>, grid, dim3(256), smem, s, p, h->st);
+    if (fmt == WFmt::INT8) return launch_pdl(k_gemv_w8<EPI>, grid, dim3(256), smem, s, p, h->st);
+  }
+  if (fmt != WFmt::BF16) return cudaErrorInvalidValue;
+  if (smem > 48 * 1024) {
+    if (smem > GEMV_MAX_SMEM) return cudaErrorInvalidValue;
+    const cudaError_t e = cudaFuncSetAttribute(k_gemv<EPI, LAYER, BIASED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+  }
+  return launch_pdl(k_gemv<EPI, LAYER, BIASED>, grid, dim3(256), smem, s, p, h->st);
+}
+
+// k_gemv of a non-production architecture: the LayerNorm prologue when `layer` (p.gain set), the biased epilogue when
+// p.bias is set.
+template <int EPI>
+static cudaError_t launch_gemv_arch(mvb_s1* h, cudaStream_t s, int n_utts, const GemvP& p, bool layer) {
+  const bool biased = p.bias != nullptr;
+  if (layer) {
+    if (biased) return launch_gemv<EPI, true, true>(h, s, n_utts, p, WFmt::BF16);
+    return launch_gemv<EPI, true, false>(h, s, n_utts, p, WFmt::BF16);
+  }
+  if (biased) return launch_gemv<EPI, false, true>(h, s, n_utts, p, WFmt::BF16);
+  return launch_gemv<EPI, false, false>(h, s, n_utts, p, WFmt::BF16);
+}
+
+// Path A for one position of a non-production architecture (layers/combined.py:38-50 per layer, model.py:303 ln_f, the
+// tied head model.py:137-143): ln_1 -> c_attn (+ bias) + cache scatter, attention, c_proj (+ bias) + residual, ln_2 ->
+// SwiGLU or GELU MLP (+ biases), mlp.c_proj (+ bias) + residual; the norms are RMSNorm or LayerNorm (eps 1e-5, beta).
+static int launch_layers_arch(mvb_s1* h, cudaStream_t s, int n_utts, float* x, float* qkv, float* att, float* ffn) {
+  const mvb_s1_config& c = h->cfg;
+  const int D = c.dim, F = c.intermediate, H = c.n_head;
+  const bool ln = h->layer_norm();
+  const size_t half = h->kv_half_bytes();
+  for (int l = 0; l < c.n_layer; ++l) {
+    const S1LayerP& lp = h->lp[l];
+    char* kc = h->kv + (size_t)l * 2 * half;
+    char* vc = kc + half;
+    GemvP p{};
+    p.eps = h->norm_eps();
+    p.W = h->lw(l, 1); p.x = x; p.ldx = D; p.gain = lp.g1; p.beta = lp.b1; p.bias = lp.qkv_b;
+    p.out = qkv; p.ldo = 3 * D; p.M = 3 * D; p.K = D;
+    p.kcache = kc; p.vcache = vc; p.H = H; p.S_max = c.block_size; p.D = D; p.kv_fp32 = c.kv_dtype == MVB_KV_FP32;
+    MVB_CK(launch_gemv_arch<EPI_QKV>(h, s, n_utts, p, ln));
+    dim3 ag(H, 2 * n_utts, ATT_SPLITS);
+    if (c.kv_dtype == MVB_KV_FP32)
+      MVB_CK(launch_pdl(k_attn_decode<true>, ag, dim3(128), 0, s, h->st, (const float*)qkv, (const void*)kc, (const void*)vc,
+                    h->wsp<float>(h->L.part_o), h->wsp<float>(h->L.part_ml), att, H, c.block_size, D));
+    else
+      MVB_CK(launch_pdl(k_attn_decode<false>, ag, dim3(128), 0, s, h->st, (const float*)qkv, (const void*)kc, (const void*)vc,
+                    h->wsp<float>(h->L.part_o), h->wsp<float>(h->L.part_ml), att, H, c.block_size, D));
+    h->launches++;
+    p = GemvP{};
+    p.eps = h->norm_eps();
+    p.W = h->lw(l, 2); p.x = att; p.ldx = D; p.bias = lp.o_b; p.out = x; p.ldo = D; p.M = D; p.K = D;
+    MVB_CK(launch_gemv_arch<EPI_RESID>(h, s, n_utts, p, false));
+    p.W = h->lw(l, 4); p.x = x; p.ldx = D; p.gain = lp.g2; p.beta = lp.b2; p.bias = lp.fc_b; p.out = ffn; p.ldo = F; p.M = F;
+    p.K = D;
+    if (h->gelu()) {
+      MVB_CK(launch_gemv_arch<EPI_GELU>(h, s, n_utts, p, ln));
+    } else {
+      p.W3 = h->lw(l, 5); p.bias3 = lp.fc3_b;
+      MVB_CK(launch_gemv_arch<EPI_SWIGLU>(h, s, n_utts, p, ln));
+    }
+    p = GemvP{};
+    p.W = h->lw(l, 6); p.x = ffn; p.ldx = F; p.bias = lp.proj_b; p.out = x; p.ldo = D; p.M = D; p.K = F;
+    MVB_CK(launch_gemv_arch<EPI_RESID>(h, s, n_utts, p, false));
+  }
+  return MVB_OK;
 }
 
 // One forward position for `n_utts` logical utterances: embed -> 24 x (attention, FFN) -> head.
@@ -455,6 +601,14 @@ static int launch_body(mvb_s1* h, cudaStream_t s, int n_utts) {
   MVB_CK(launch_pdl(k_embed, dim3(2, n_utts), dim3(256), 0, s, h->st, h->w(0), h->w(1),
                 (const float*)h->wsp<float>(h->L.spk), x, D));
   h->launches++;
+  if (!h->production_arch()) {
+    if (int e = launch_layers_arch(h, s, n_utts, x, qkv, att, ffn)) return e;
+    GemvP p{};
+    p.eps = h->norm_eps();
+    p.W = h->w(4); p.x = x; p.ldx = D; p.gain = h->w(3); p.beta = h->lnf_b; p.out = logits; p.ldo = V; p.M = V; p.K = D;
+    MVB_CK(launch_gemv_arch<EPI_STORE>(h, s, n_utts, p, h->layer_norm()));
+    return MVB_OK;
+  }
   const size_t half = h->kv_half_bytes();
   for (int l = 0; l < c.n_layer; ++l) {
     char* kc = h->kv + (size_t)l * 2 * half;
@@ -510,12 +664,15 @@ static const CUtensorMap* tmap_b(mvb_s1* h, int NB, int K) {
 }
 
 struct LinB {
-  const float* x; int ldx; const __nv_bfloat16* gain;  // input rows (+ optional RMSNorm gain)
+  const float* x; int ldx; const __nv_bfloat16* gain;  // input rows (+ optional norm gain: the architecture's norm)
   int widx, widx3;                                     // tensor-map indices of W (and W3 for SwiGLU)
   int M, K;
   float* out; int ldo;
   const __nv_bfloat16* scale = nullptr;                // int8 engine: row scales of W (and W3)
   const __nv_bfloat16* scale3 = nullptr;
+  const __nv_bfloat16* beta = nullptr;                 // LayerNorm with bias: the norm's beta
+  const __nv_bfloat16* bias = nullptr;                 // Linear biases of W (and W3)
+  const __nv_bfloat16* bias3 = nullptr;
 };
 
 template <int EPI>
@@ -528,6 +685,9 @@ static int linear_b(mvb_s1* h, cudaStream_t s, int R, const LinB& a, void* kc = 
   g.tmW = &h->tmW[a.widx]; g.tmW3 = &h->tmW[a.widx3];
   g.B = h->wsp<__nv_bfloat16>(h->L.b_B);
   g.x = a.x; g.ldx = a.ldx; g.gain = a.gain; g.eps = c.norm_eps;
+  if (a.gain != nullptr && h->layer_norm()) {   // LayerNorm (layers/layers.py:8-17): eps 1e-5, optional beta
+    g.layer_norm = 1; g.beta = a.beta; g.eps = 1e-5f;
+  }
   g.M = a.M; g.K = a.K; g.out = a.out; g.ldo = a.ldo;
   g.kcache = kc; g.vcache = vc; g.row_cache = h->rows.cache_row; g.row_pos = h->rows.pos;
   g.H = c.n_head; g.S_max = c.block_size; g.D = c.dim; g.kv_fp32 = c.kv_dtype == MVB_KV_FP32;
@@ -535,9 +695,55 @@ static int linear_b(mvb_s1* h, cudaStream_t s, int R, const LinB& a, void* kc = 
   g.tickets = h->wsp<unsigned>(h->L.b_tickets);
   g.n_sm = h->n_sm;
   g.scale = a.scale; g.scale3 = a.scale3;
+  g.bias = a.bias; g.bias3 = a.bias3;
   MVB_CK(tc_gemm(s, g));
   h->launches += 2;   // k_prep_b + k_tc_gemm
   return MVB_OK;
+}
+
+static int attn_rows(mvb_s1* h, cudaStream_t s, int R, const float* qkv, const void* kc, const void* vc, float* att) {
+  const mvb_s1_config& c = h->cfg;
+  const int D = c.dim, H = c.n_head;
+  dim3 ag(H, R, ATT_SPLITS);
+  if (c.kv_dtype == MVB_KV_FP32)
+    k_attn_rows<true><<<ag, 128, 0, s>>>(h->rows, qkv, kc, vc, h->wsp<float>(h->L.b_part_o), h->wsp<float>(h->L.b_part_ml),
+                                         h->wsp<unsigned>(h->L.b_att_tickets), att, H, c.block_size, D);
+  else
+    k_attn_rows<false><<<ag, 128, 0, s>>>(h->rows, qkv, kc, vc, h->wsp<float>(h->L.b_part_o), h->wsp<float>(h->L.b_part_ml),
+                                          h->wsp<unsigned>(h->L.b_att_tickets), att, H, c.block_size, D);
+  h->launches++;
+  MVB_CK(cudaGetLastError());
+  return MVB_OK;
+}
+
+// One layer of a non-production architecture on the tensor cores: the projections of launch_layers_arch with the
+// LayerNorm prologue of k_prep_b<true> and the BIASED / G_GELU epilogues of k_tc_gemm.
+static int layer_b_arch(mvb_s1* h, cudaStream_t s, int R, int l, float* x, float* qkv, float* att, float* ffn, void* kc,
+                        void* vc) {
+  const int D = h->cfg.dim, F = h->cfg.intermediate;
+  const S1LayerP& p = h->lp[l];
+  LinB a{x, D, p.g1, l * 5 + 0, l * 5 + 0, 3 * D, D, qkv, 3 * D};
+  a.beta = p.b1; a.bias = p.qkv_b;
+  if (int e = linear_b<G_QKV>(h, s, R, a, kc, vc)) return e;
+  if (int e = attn_rows(h, s, R, qkv, kc, vc, att)) return e;
+  a = LinB{att, D, nullptr, l * 5 + 1, l * 5 + 1, D, D, x, D};
+  a.bias = p.o_b;
+  if (int e = linear_b<G_RESID>(h, s, R, a)) return e;
+  a = LinB{x, D, p.g2, l * 5 + 2, l * 5 + 3, F, D, ffn, F};
+  a.beta = p.b2; a.bias = p.fc_b; a.bias3 = p.fc3_b;
+  if (int e = h->gelu() ? linear_b<G_GELU>(h, s, R, a) : linear_b<G_SWIGLU>(h, s, R, a)) return e;
+  a = LinB{ffn, F, nullptr, l * 5 + 4, l * 5 + 4, D, F, x, D};
+  a.bias = p.proj_b;
+  return linear_b<G_RESID>(h, s, R, a);
+}
+
+// The final norm and the head of path B over R rows of x: y = ln_f(x) . lm_head^T into out [R, vocab].
+static int head_b(mvb_s1* h, cudaStream_t s, int R, const float* x, float* out) {
+  const mvb_s1_config& c = h->cfg;
+  const int hw = c.n_layer * 5;
+  LinB a{x, c.dim, h->w(3), hw, hw, c.vocab, c.dim, out, c.vocab, h->head_scale()};
+  a.beta = h->lnf_b;
+  return linear_b<G_STORE>(h, s, R, a);
 }
 
 // embed + all layers for the R rows described by h->rows (already filled on the device)
@@ -573,6 +779,10 @@ static int launch_layers_b(mvb_s1* h, cudaStream_t s, int R) {
       h->launches++;
       MVB_CK(cudaGetLastError());
     }
+    if (!h->production_arch()) {   // the layer of a non-production architecture (path A's launch_layers_arch)
+      if (int e = layer_b_arch(h, s, R, l, x, qkv, att, ffn, kc, vc)) return e;
+      continue;
+    }
     if (int e = linear_b<G_QKV>(h, s, R, LinB{x, D, h->lw(l, 0), l * 5 + 0, l * 5 + 0, 3 * D, D, qkv, 3 * D, h->tc_lscale(l, 1)},
                                 kc, vc)) return e;
     dim3 ag(H, R, ATT_SPLITS);
@@ -594,15 +804,12 @@ static int launch_layers_b(mvb_s1* h, cudaStream_t s, int R) {
 
 // batched decode position: rows from the decode state, logits land in the sampler's buffer
 static int launch_body_b(mvb_s1* h, cudaStream_t s, int n_utts) {
-  const mvb_s1_config& c = h->cfg;
   const int R = 2 * n_utts;
   k_rows_decode<<<1, 128, 0, s>>>(h->st, h->rows, n_utts);
   h->launches++;
   MVB_CK(cudaGetLastError());
   if (int e = launch_layers_b(h, s, R)) return e;
-  const int hw = c.n_layer * 5;
-  return linear_b<G_STORE>(h, s, R, LinB{h->wsp<float>(h->L.b_x), c.dim, h->w(3), hw, hw, c.vocab, c.dim,
-                                         h->wsp<float>(h->L.logits), c.vocab, h->head_scale()});
+  return head_b(h, s, R, h->wsp<float>(h->L.b_x), h->wsp<float>(h->L.logits));
 }
 
 
@@ -746,11 +953,10 @@ extern "C" int mvb_s1_forward(mvb_s1* h, int32_t utt, const int32_t* d_idx, int3
       h->launches++;
       MVB_CK(cudaGetLastError());
       if (int e = launch_layers_b(h, s, R)) return e;
-      const int hw = c.n_layer * 5;
       float* bx = h->wsp<float>(h->L.b_x);
       if (d_logits && all_positions) {
         float* bl = h->wsp<float>(h->L.b_logits);
-        if (int e = linear_b<G_STORE>(h, s, R, LinB{bx, c.dim, h->w(3), hw, hw, V, c.dim, bl, V, h->head_scale()})) return e;
+        if (int e = head_b(h, s, R, bx, bl)) return e;
         for (int cc = 0; cc < 2; ++cc)
           MVB_CK(cudaMemcpyAsync(d_logits + ((size_t)cc * S + s0) * V, bl + (size_t)cc * Sc * V, sizeof(float) * (size_t)Sc * V,
                              cudaMemcpyDeviceToDevice, s));
@@ -761,8 +967,7 @@ extern "C" int mvb_s1_forward(mvb_s1* h, int32_t utt, const int32_t* d_idx, int3
         k_gather_last<<<2, 256, 0, s>>>(bx, last, Sc, c.dim);
         h->launches++;
         MVB_CK(cudaGetLastError());
-        if (int e = linear_b<G_STORE>(h, s, 2, LinB{last, c.dim, h->w(3), hw, hw, V, c.dim,
-                                                    h->wsp<float>(h->L.logits) + (size_t)(2 * utt) * V, V, h->head_scale()})) return e;
+        if (int e = head_b(h, s, 2, last, h->wsp<float>(h->L.logits) + (size_t)(2 * utt) * V)) return e;
         k_set_input<<<1, 32, 0, s>>>(h->st, utt, d_idx, S, S - 1, pos0 + S - 1);
         h->launches++;
         MVB_CK(cudaGetLastError());
@@ -1293,6 +1498,87 @@ extern "C" int mvb_w8_widen_test(const void* d_W, int32_t M, int32_t K, void* d_
   cudaStream_t s = (cudaStream_t)stream;
   k_w8_widen<<<4 * n_sm, 256, 0, s>>>(m);
   MVB_CK(cudaGetLastError());
+  MVB_CK(cudaStreamSynchronize(s));
+  return MVB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Test hook of the non-production architectures' projections (include/mvb200.h): k_gemv with any norm, bias and epilogue
+// exactly as path A launches it, or the BIASED QKV k_tc_gemm of path B with a forced K split.
+// Rows of a tensor-core QKV test: activation row n -> cache row 2 s + (n & 1) at position pos[s], s = slot_map[n >> 1].
+__global__ void k_rows_of_slots(const int* __restrict__ slot_map, const int* __restrict__ pos, int n_utts,
+                                int* __restrict__ row_cache, int* __restrict__ row_pos) {
+  const int n = threadIdx.x;
+  if (n < 2 * n_utts) {
+    const int s = slot_map[n >> 1];
+    row_cache[n] = 2 * s + (n & 1);
+    row_pos[n] = pos[s];
+  }
+}
+
+extern "C" int mvb_s1_arch_gemv_test(int32_t path, int32_t epi, int32_t norm, const void* d_W, const void* d_W3,
+                                     const void* d_bias, const void* d_bias3, int32_t M, int32_t K, const float* d_x,
+                                     int32_t ldx, int32_t n_utts, const void* d_gain, const void* d_beta, float eps,
+                                     float* d_out, int32_t ldo, void* d_kcache, void* d_vcache, const int32_t* d_slot_map,
+                                     const int32_t* d_pos, int32_t H, int32_t S_max, int32_t D, int32_t kv_fp32,
+                                     int32_t ksplit_override, void* stream) {
+  if (!d_W || !d_x || !d_out || !d_slot_map || !d_pos) return set_error(MVB_ERR_ARG, "null argument");
+  if (path != 0 && path != 1) return set_error(MVB_ERR_ARG, "mvb_s1_arch_gemv_test: path %d", path);
+  if (epi < EPI_STORE || epi > EPI_GELU) return set_error(MVB_ERR_ARG, "mvb_s1_arch_gemv_test: epilogue %d", epi);
+  if (norm < 0 || norm > 2) return set_error(MVB_ERR_ARG, "mvb_s1_arch_gemv_test: norm %d", norm);
+  if ((norm != 0) != (d_gain != nullptr) || (d_beta && norm != 2))
+    return set_error(MVB_ERR_ARG, "mvb_s1_arch_gemv_test: a norm takes a gain (and only LayerNorm a beta)");
+  if (n_utts < 1 || n_utts > 64) return set_error(MVB_ERR_ARG, "mvb_s1_arch_gemv_test: n_utts %d", n_utts);
+  if (epi == EPI_SWIGLU && (!d_W3 || (d_bias && !d_bias3)))
+    return set_error(MVB_ERR_ARG, "mvb_s1_arch_gemv_test: SwiGLU needs W3 (and bias3 with a bias)");
+  if (epi == EPI_QKV && (!d_kcache || !d_vcache || M != 3 * D || D != 128 * H || S_max < 1))
+    return set_error(MVB_ERR_ARG, "mvb_s1_arch_gemv_test: QKV needs both caches, D == 128 H, M == 3 D, S_max >= 1");
+  if (ldo < M || ldx < K) return set_error(MVB_ERR_ARG, "mvb_s1_arch_gemv_test: ldo >= M and ldx >= K required");
+  cudaStream_t s = (cudaStream_t)stream;
+  if (path == 1) {
+    if (epi != EPI_QKV) return set_error(MVB_ERR_ARG, "mvb_s1_arch_gemv_test: path 1 is the QKV GEMM");
+    if (K % 64 || 2 * n_utts > RB_MAX) return set_error(MVB_ERR_UNSUPPORTED, "mvb_s1_arch_gemv_test: K %% 64 == 0, 2 n_utts <= 128");
+    int* rows = nullptr;
+    MVB_CK(cudaMalloc(&rows, sizeof(int) * 2 * RB_MAX));
+    k_rows_of_slots<<<1, RB_MAX, 0, s>>>(d_slot_map, d_pos, n_utts, rows, rows + RB_MAX);
+    TcGemm a{};
+    a.epi = G_QKV;
+    a.x = d_x; a.ldx = ldx; a.gain = reinterpret_cast<const __nv_bfloat16*>(d_gain); a.eps = eps;
+    a.layer_norm = norm == 2; a.beta = reinterpret_cast<const __nv_bfloat16*>(d_beta);
+    a.M = M; a.K = K; a.R = 2 * n_utts; a.split_lo = 1; a.ksplit = ksplit_override;
+    a.out = d_out; a.ldo = ldo;
+    a.kcache = d_kcache; a.vcache = d_vcache; a.row_cache = rows; a.row_pos = rows + RB_MAX;
+    a.H = H; a.S_max = S_max; a.D = D; a.kv_fp32 = kv_fp32;
+    a.bias = reinterpret_cast<const __nv_bfloat16*>(d_bias);
+    const cudaError_t le = cudaGetLastError();
+    const int rc = le == cudaSuccess ? tc_gemm_test(a, d_W, nullptr, stream)
+                                     : set_error(MVB_ERR_CUDA, "k_rows_of_slots: %s", cudaGetErrorString(le));
+    cudaFree(rows);
+    return rc;
+  }
+  if (K < 256 || K % 256 || M < 2 || M % 2 || (size_t)2 * K * sizeof(float) > GEMV_MAX_SMEM)
+    return set_error(MVB_ERR_UNSUPPORTED, "mvb_s1_arch_gemv_test: bad GEMV shape M=%d K=%d", M, K);
+  mvb_s1 h{};
+  int dev = 0;
+  if (int e = current_device(&dev, &h.n_sm)) return e;
+  h.st.slot_map = const_cast<int*>(d_slot_map);
+  h.st.pos = const_cast<int*>(d_pos);
+  GemvP p{};
+  p.W = reinterpret_cast<const __nv_bfloat16*>(d_W); p.W3 = reinterpret_cast<const __nv_bfloat16*>(d_W3);
+  p.x = d_x; p.ldx = ldx; p.gain = reinterpret_cast<const __nv_bfloat16*>(d_gain); p.eps = eps;
+  p.beta = reinterpret_cast<const __nv_bfloat16*>(d_beta);
+  p.bias = reinterpret_cast<const __nv_bfloat16*>(d_bias);
+  p.bias3 = epi == EPI_SWIGLU ? reinterpret_cast<const __nv_bfloat16*>(d_bias3) : nullptr;
+  p.out = d_out; p.ldo = ldo; p.M = M; p.K = K;
+  p.kcache = d_kcache; p.vcache = d_vcache; p.H = H; p.S_max = S_max; p.D = D; p.kv_fp32 = kv_fp32;
+  const bool ln = norm == 2;
+  switch (epi) {
+    case EPI_STORE: MVB_CK(launch_gemv_arch<EPI_STORE>(&h, s, n_utts, p, ln)); break;
+    case EPI_RESID: MVB_CK(launch_gemv_arch<EPI_RESID>(&h, s, n_utts, p, ln)); break;
+    case EPI_SWIGLU: MVB_CK(launch_gemv_arch<EPI_SWIGLU>(&h, s, n_utts, p, ln)); break;
+    case EPI_QKV: MVB_CK(launch_gemv_arch<EPI_QKV>(&h, s, n_utts, p, ln)); break;
+    default: MVB_CK(launch_gemv_arch<EPI_GELU>(&h, s, n_utts, p, ln)); break;
+  }
   MVB_CK(cudaStreamSynchronize(s));
   return MVB_OK;
 }

@@ -122,7 +122,11 @@ __global__ void __launch_bounds__(256) k_embed(S1State st, const __nv_bfloat16* 
 //   EPI_RESID  : wo / w2 projection + residual add             (fast_model.py:226,179-180, 247)
 //   EPI_SWIGLU : silu(w1 x) * (w3 x)                           (fast_model.py:230-237)
 //   EPI_STORE  : final norm + LM head                          (fast_model.py:161-163)
-enum { EPI_STORE = 0, EPI_RESID = 1, EPI_SWIGLU = 2, EPI_QKV = 3 };
+//   EPI_GELU   : GELU(c_fc x), exact erf                       (layers/layers.py:45-48, 63-65: nn.GELU())
+// The other GPTConfig architectures (model.py:26-46) add a LayerNorm prologue (k_gemv's LAYER flag) and the Linear
+// biases of c_attn, attn.c_proj and the MLP (BIASED; attn.py:61-64, layers.py:37-53); the int4 / int8 GEMVs never take
+// either.
+enum { EPI_STORE = 0, EPI_RESID = 1, EPI_SWIGLU = 2, EPI_QKV = 3, EPI_GELU = 4 };
 
 struct GemvP {
   const __nv_bfloat16* W;
@@ -138,7 +142,14 @@ struct GemvP {
   void* kcache;
   void* vcache;
   int H, S_max, D, kv_fp32;
+  // k_gemv only: LayerNorm beta [K] or null (LAYER), Linear biases of W (and W3) [M] (BIASED)
+  const __nv_bfloat16* beta;
+  const __nv_bfloat16* bias;
+  const __nv_bfloat16* bias3;
 };
+
+// nn.GELU(approximate='none'), as k_tc_gemm's G_GELU epilogue computes it
+__device__ __forceinline__ float gelu_erf(float y) { return 0.5f * y * (1.f + erff(y * (float)M_SQRT1_2)); }
 
 // Position of activation k inside the conflict-free shared-memory layout: a lane's eight
 // consecutive k values are split into two float4 that sit 128 floats apart.
@@ -160,12 +171,78 @@ __device__ __forceinline__ void gemv_rows(const GemvP& p, int item, int lane, co
 
 // Prologue of the GEMV kernels (k_gemv, k_gemv_w4, k_gemv_w8): stage the two activation rows r0, r0 + 1 of p.x into
 // xs [2][K] at perm(k), RMS-normalised (fp32 statistics, then the bf16 gain) when p.gain is set.  Ends with __syncthreads.
-template <typename Perm>
+// LAYER (k_gemv only): LayerNorm instead (layers/layers.py:8-17, F.layer_norm with eps p.eps), the arithmetic of
+// k_prep_b<true>: fp32 mean, then the biased variance as a second pass over the centred row, then
+// ((x - mean) * rsqrt(var + eps)) * gain (+ beta when p.beta is set); p.gain is required.
+template <bool LAYER = false, typename Perm>
 __device__ __forceinline__ void gemv_prologue(const GemvP& p, int r0, float* xs, float* red, Perm perm) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int K = p.K;
   const float* x0 = p.x + (size_t)r0 * p.ldx;
   const float* x1 = x0 + p.ldx;
+  if constexpr (LAYER) {
+    float s0 = 0.f, s1 = 0.f;
+    for (int k = tid; k < K; k += 256) {
+      const float a = x0[k], b = x1[k];
+      s0 += a;
+      s1 += b;
+      const int pk = perm(k);
+      xs[pk] = a;
+      xs[K + pk] = b;
+    }
+    s0 = warp_sum(s0);
+    s1 = warp_sum(s1);
+    if (lane == 0) {
+      red[warp] = s0;
+      red[8 + warp] = s1;
+    }
+    __syncthreads();
+    float t0 = 0.f, t1 = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      t0 += red[i];
+      t1 += red[8 + i];
+    }
+    const float m0 = t0 / (float)K, m1 = t1 / (float)K;
+    __syncthreads();                       // every thread has read red before it is reused
+    float q0 = 0.f, q1 = 0.f;
+    for (int k = tid; k < K; k += 256) {   // this thread's own staged entries
+      const int pk = perm(k);
+      const float d0 = xs[pk] - m0, d1 = xs[K + pk] - m1;
+      q0 = fmaf(d0, d0, q0);
+      q1 = fmaf(d1, d1, q1);
+    }
+    q0 = warp_sum(q0);
+    q1 = warp_sum(q1);
+    if (lane == 0) {
+      red[warp] = q0;
+      red[8 + warp] = q1;
+    }
+    __syncthreads();
+    t0 = 0.f;
+    t1 = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      t0 += red[i];
+      t1 += red[8 + i];
+    }
+    const float rs0 = rsqrtf(t0 / (float)K + p.eps);
+    const float rs1 = rsqrtf(t1 / (float)K + p.eps);
+    for (int k = tid; k < K; k += 256) {
+      const float g = bf16_to_f32(p.gain[k]);
+      const int pk = perm(k);
+      float v0 = ((xs[pk] - m0) * rs0) * g, v1 = ((xs[K + pk] - m1) * rs1) * g;
+      if (p.beta != nullptr) {
+        const float be = bf16_to_f32(p.beta[k]);
+        v0 += be;
+        v1 += be;
+      }
+      xs[pk] = v0;
+      xs[K + pk] = v1;
+    }
+    __syncthreads();
+    return;
+  }
   float s0 = 0.f, s1 = 0.f;
   for (int k = tid; k < K; k += 256) {
     const float a = x0[k], b = x1[k];
@@ -202,16 +279,31 @@ __device__ __forceinline__ void gemv_prologue(const GemvP& p, int r0, float* xs,
 }
 
 // Epilogue of the GEMV kernels for one item of slot u: a<weight row><activation row>, weight rows 2 item, 2 item + 1
-// (EPI_SWIGLU: a0* = w1 row item, a1* = w3 row item).
-template <int EPI>
+// (EPI_SWIGLU: a0* = w1 row item, a1* = w3 row item).  BIASED (k_gemv only): the Linear biases are added to the sums
+// first, so the QKV scatter stores k and v with their bias (before a bf16 cache rounds them).
+template <int EPI, bool BIASED = false>
 __device__ __forceinline__ void gemv_epilogue(const GemvP& p, const S1State& st, int u, int item, float a00, float a01,
                                               float a10, float a11) {
   const int r0 = 2 * u;
   float* o0 = p.out + (size_t)r0 * p.ldo;
   float* o1 = o0 + p.ldo;
+  if constexpr (BIASED) {
+    const float b0 = bf16_to_f32(p.bias[EPI == EPI_SWIGLU ? item : 2 * item]);
+    const float b1 = bf16_to_f32(EPI == EPI_SWIGLU ? p.bias3[item] : p.bias[2 * item + 1]);
+    a00 += b0;
+    a01 += b0;
+    a10 += b1;
+    a11 += b1;
+  }
   if (EPI == EPI_SWIGLU) {
     o0[item] = (a00 / (1.f + expf(-a00))) * a10;
     o1[item] = (a01 / (1.f + expf(-a01))) * a11;
+  } else if (EPI == EPI_GELU) {
+    const int j = 2 * item;
+    o0[j] = gelu_erf(a00);
+    o1[j] = gelu_erf(a01);
+    o0[j + 1] = gelu_erf(a10);
+    o1[j + 1] = gelu_erf(a11);
   } else {
     const int j = 2 * item;
     if (EPI == EPI_RESID) {
@@ -249,7 +341,7 @@ __device__ __forceinline__ void gemv_epilogue(const GemvP& p, const S1State& st,
   }
 }
 
-template <int EPI>
+template <int EPI, bool LAYER = false, bool BIASED = false>
 __global__ void __launch_bounds__(256, 2) k_gemv(GemvP p, S1State st) {
   extern __shared__ float xs[];  // [2][K] permuted
   __shared__ float red[16];
@@ -262,7 +354,7 @@ __global__ void __launch_bounds__(256, 2) k_gemv(GemvP p, S1State st) {
   pdl_wait();  // activations written by the previous kernel are now visible
 
   const int u = st.slot_map[blockIdx.y];
-  gemv_prologue(p, 2 * u, xs, red, [](int k) { return xs_perm(k); });
+  gemv_prologue<LAYER>(p, 2 * u, xs, red, [](int k) { return xs_perm(k); });
 
   // ---- main: each warp streams two weight rows at a time
   for (int item = blockIdx.x * 8 + warp; item < n_items; item += nwarps) {
@@ -286,7 +378,7 @@ __global__ void __launch_bounds__(256, 2) k_gemv(GemvP p, S1State st) {
     a01 = warp_sum(a01);
     a10 = warp_sum(a10);
     a11 = warp_sum(a11);
-    if (lane == 0) gemv_epilogue<EPI>(p, st, u, item, a00, a01, a10, a11);
+    if (lane == 0) gemv_epilogue<EPI, BIASED>(p, st, u, item, a00, a01, a10, a11);
   }
 }
 

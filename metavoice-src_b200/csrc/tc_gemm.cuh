@@ -39,7 +39,7 @@ struct GemmP {
   const int* row_pos;    // [R] cache position of each activation row
   int H, S_max, D, kv_fp32;
   // bf16 [M] per-row vectors of W (and W3), applied once per output after the (split-K) sum: the row scales of int8
-  // weights (the widened q, SCALED) or the Linear biases (stage 2 with bias=True, BIASED).  No instance uses both, so
+  // weights (the widened q, SCALED) or the Linear biases (GPTConfig bias=True, BIASED).  No instance uses both, so
   // they share the slots: a larger GemmP costs the existing instances registers.
   union { const __nv_bfloat16* scale; const __nv_bfloat16* bias; };
   union { const __nv_bfloat16* scale3; const __nv_bfloat16* bias3; };

@@ -122,9 +122,12 @@ struct TcGemm {
   int ksplit;                                     // > 0: force the K split (tests)
   const __nv_bfloat16* scale;                     // int8 weights: bf16 [M] row scales of W, or null
   const __nv_bfloat16* scale3;                    // G_SWIGLU: those of W3
-  const __nv_bfloat16* bias;                      // bf16 [M] Linear bias of W, or null (never with scale or G_QKV)
+  const __nv_bfloat16* bias;                      // bf16 [M] Linear bias of W, or null (never with scale)
   const __nv_bfloat16* bias3;                     // G_SWIGLU with bias: that of W3
 };
 cudaError_t tc_gemm(cudaStream_t s, const TcGemm& a);
+// Test hooks: tc_gemm over `a` with the B buffer, split-K scratch and tickets of mvb_linear (a.Rpad, a.B, a.scratch,
+// a.tickets, a.n_sm and the tensor maps are filled in); W3 is G_SWIGLU's second weight.  Synchronises `stream`.
+int tc_gemm_test(const TcGemm& a, const void* d_W, const void* d_W3, void* stream);
 
 }  // namespace mvb

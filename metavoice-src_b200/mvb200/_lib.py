@@ -16,6 +16,8 @@ MVB_S1_NO_ROWS_PATH, MVB_S1_NO_RESIDENT, MVB_S1_UNFUSED_SAMPLER, MVB_S1_TRACE = 
 MVB_S2_EAGER = 0x1
 MVB_S2_NORM_RMS, MVB_S2_NORM_LAYER = 0, 1          # mvb_s2_arch.norm
 MVB_S2_MLP_SWIGLU, MVB_S2_MLP_GELU = 0, 1          # mvb_s2_arch.mlp
+MVB_S1_NORM_RMS, MVB_S1_NORM_LAYER = 0, 1          # mvb_s1_arch.norm
+MVB_S1_MLP_SWIGLU, MVB_S1_MLP_GELU = 0, 1          # mvb_s1_arch.mlp
 MVB_MBD_CUDA_CORES, MVB_MBD_ONE_STREAM = 0x1, 0x2
 SPK_MAX_BATCH, RESAMPLE_MAX_TAPS = 32, 16384      # MVB_SPK_MAX_BATCH, MVB_RESAMPLE_MAX_TAPS
 
@@ -37,6 +39,10 @@ class S2Config(C.Structure):
                 ("block_size", C.c_int32), ("n_in", C.c_int32), ("vocab_in", C.c_int32 * 8), ("n_out", C.c_int32),
                 ("vocab_out", C.c_int32 * 8), ("spk_dim", C.c_int32), ("norm_eps", C.c_float), ("max_batch", C.c_int32),
                 ("options", C.c_int32)]
+
+
+class S1Arch(C.Structure):
+    _fields_ = [("norm", C.c_int32), ("mlp", C.c_int32), ("bias", C.c_int32)]
 
 
 class S2Arch(C.Structure):
@@ -72,6 +78,8 @@ SIGNATURES = {
     "mvb_last_error": (C.c_char_p, []),
     "mvb_s1_kv_bytes": (C.c_size_t, [C.POINTER(S1Config)]),
     "mvb_s1_workspace_bytes": (C.c_size_t, [C.POINTER(S1Config)]),
+    "mvb_s1_create_ex": (C.c_int, [C.POINTER(S1Config), C.POINTER(S1Arch), C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64),
+                                   C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]),
     "mvb_s1_create": (C.c_int, [C.POINTER(S1Config), C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64), C.c_void_p,
                                 C.c_void_p, C.POINTER(C.c_void_p)]),
     "mvb_s1_destroy": (C.c_int, [C.c_void_p]),
@@ -182,6 +190,10 @@ SIGNATURES = {
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                    C.c_void_p]),
     "mvb_w8_widen_test": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "mvb_s1_arch_gemv_test": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                        C.c_float, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     "mvb_s2_sample_test": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_void_p]),
     "mvb_s2_embed_test": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -12,7 +12,7 @@ import math
 import time
 import warnings
 from pathlib import Path
-from typing import Optional, Tuple
+from typing import Dict, Optional, Tuple
 
 import numpy as np
 import torch
@@ -276,6 +276,39 @@ def encode_tokens(tokenizer, text: str, device="cuda") -> torch.Tensor:
 
 
 # ---- fast_inference_utils.py:236-321 ---------------------------------------------------------------
+_ARCH_VALUES = {"norm_type": ("rmsnorm", "layernorm"), "nonlinearity_type": ("swiglu", "gelu"), "bias": (False, True)}
+_PRODUCTION_ARCH = {"norm_type": "rmsnorm", "nonlinearity_type": "swiglu", "bias": False}
+
+
+def stage1_arch(model_args: dict, state_dict: Dict[str, torch.Tensor]) -> Tuple[str, str, bool]:
+    """(norm_type, nonlinearity_type, bias) of a first-stage checkpoint, the GPTConfig fields (model.py:36-43) the
+    reference's slow path builds ``GPT(GPTConfig(**model_args))`` from (inference.py:102-156).
+
+    A key present in ``model_args`` is taken as it is.  A missing key means what the fast path has always assumed
+    (rmsnorm, swiglu, no bias), not GPTConfig's own default (layernorm, gelu, bias): checkpoints the reference writes
+    always carry all three keys (finetune.py).  A state dict that contradicts an assumed value -- ``mlp.c_fc`` weights
+    without ``nonlinearity_type``, any ``.bias`` tensor without ``bias`` -- raises ValueError naming the missing key.
+    What the engine does not build raises NotImplementedError naming the key: an unknown value, spk_emb_on_text=False,
+    more than one input hierarchy."""
+    arch = {}
+    for key, values in _ARCH_VALUES.items():
+        v = model_args.get(key, _PRODUCTION_ARCH[key])
+        if not any(v is x or (type(v) is type(x) and v == x) for x in values):
+            raise NotImplementedError(f"model_args[{key!r}] = {v!r} is not supported (one of {values})")
+        arch[key] = v
+    if "nonlinearity_type" not in model_args and any(k.endswith(".mlp.c_fc.weight") for k in state_dict):
+        raise ValueError("model_args has no 'nonlinearity_type' but the state dict holds mlp.c_fc weights (a GELU MLP): "
+                         "set nonlinearity_type")
+    if "bias" not in model_args and any(k.endswith(".bias") for k in state_dict):
+        raise ValueError("model_args has no 'bias' but the state dict holds .bias tensors: set bias")
+    if model_args.get("spk_emb_on_text", True) is not True:
+        raise NotImplementedError("model_args['spk_emb_on_text'] = False is not supported (speaker on text tokens only)")
+    if len(model_args.get("vocab_sizes") or [None]) > 1:
+        raise NotImplementedError(f"model_args['vocab_sizes'] = {model_args['vocab_sizes']!r}: more than one input "
+                                  "hierarchy is not supported")
+    return arch["norm_type"], arch["nonlinearity_type"], arch["bias"]
+
+
 def _load_model(checkpoint_path, spk_emb_ckpt_path, device, precision, quantisation_mode=None, n_head: int = None):
     if quantisation_mode is not None:
         if quantisation_mode not in ("int4", "int8"):
@@ -286,13 +319,21 @@ def _load_model(checkpoint_path, spk_emb_ckpt_path, device, precision, quantisat
     sd = checkpoint["model"]
     args = checkpoint.get("model_args", {})
     sd0 = {(k[len("_orig_mod."):] if k.startswith("_orig_mod.") else k): v for k, v in sd.items()}
+    norm_type, nonlinearity_type, bias = stage1_arch(args, sd0)
+    if quantisation_mode is not None and (norm_type, nonlinearity_type, bias) != ("rmsnorm", "swiglu", False):
+        # before any weight is read (the checkpoint is memory-mapped)
+        raise NotImplementedError(f"quantisation_mode={quantisation_mode!r} is implemented for the production architecture "
+                                  f"only; model_args['norm_type', 'nonlinearity_type', 'bias'] = "
+                                  f"{(norm_type, nonlinearity_type, bias)!r}")
     vocab, dim = sd0["transformer.wtes.0.weight"].shape
     n_layer = args.get("n_layer") or sum(1 for k in sd0 if k.endswith(".ln_1.weight"))
     n_head = n_head or args.get("n_head") or dim // 128
+    mlp_in = "mlp.c_fc" if nonlinearity_type == "gelu" else "mlp.swiglu.w1"
     config = ModelArgs(block_size=sd0["transformer.wpe.weight"].shape[0], vocab_size=vocab, n_layer=n_layer,
                        n_head=n_head, dim=dim, speaker_emb_dim=sd0["speaker_cond_pos.weight"].shape[1],
-                       intermediate_size=sd0["transformer.h.0.mlp.swiglu.w1.weight"].shape[0],
-                       norm_eps=args.get("rmsnorm_eps") or 1e-5)
+                       intermediate_size=sd0[f"transformer.h.0.{mlp_in}.weight"].shape[0],
+                       norm_eps=args.get("rmsnorm_eps") or 1e-5,
+                       norm_type=norm_type, nonlinearity_type=nonlinearity_type, bias=bias)
     if quantisation_mode == "int8":   # measured: 0.84x the bf16 decode rate at batch 1 on an H100 (DESIGN.md section 8)
         warnings.warn("int8 quantisation is slower than bf16/fp16 for undebugged reasons! Please set optimisation_mode to "
                       "`None` or to `int4`.")

@@ -7,6 +7,7 @@ Same names and call signatures as the reference (``ModelArgs``, ``Transformer.fr
 """
 from __future__ import annotations
 
+import ctypes as C
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Union
 
@@ -34,13 +35,25 @@ class ModelArgs:
     head_dim: int = 64
     norm_eps: float = 1e-5
     dtype: torch.dtype = torch.bfloat16
+    # GPTConfig's architecture fields (fam/llm/model.py:36-43); the defaults are the production model's, which is the
+    # only architecture the reference's fast path builds.  Any other runs on the engine's per-layer paths.
+    norm_type: str = "rmsnorm"
+    nonlinearity_type: str = "swiglu"
+    bias: bool = False
 
     def __post_init__(self):
         if self.n_local_heads == -1:
             self.n_local_heads = self.n_head
         if self.intermediate_size is None:
-            self.intermediate_size = find_multiple(int(2 * 4 * self.dim / 3), 256)
+            if self.nonlinearity_type == "gelu":
+                self.intermediate_size = 4 * self.dim                   # layers/layers.py:46
+            else:
+                self.intermediate_size = find_multiple(int(2 * 4 * self.dim / 3), 256)
         self.head_dim = self.dim // self.n_head
+
+    @property
+    def production_arch(self) -> bool:
+        return (self.norm_type, self.nonlinearity_type, self.bias) == ("rmsnorm", "swiglu", False)
 
     @classmethod
     def from_name(cls, name: str):
@@ -61,13 +74,31 @@ _LAYER_KEYS = ["ln_1.weight", "attn.c_attn.weight", "attn.c_proj.weight", "ln_2.
                "mlp.swiglu.w1.weight", "mlp.swiglu.w3.weight", "mlp.c_proj.weight"]
 
 
-def pack_arena(state_dict: Dict[str, torch.Tensor], n_layer: int):
+_NORMS = {"rmsnorm": _lib.MVB_S1_NORM_RMS, "layernorm": _lib.MVB_S1_NORM_LAYER}
+_MLPS = {"swiglu": _lib.MVB_S1_MLP_SWIGLU, "gelu": _lib.MVB_S1_MLP_GELU}
+
+
+def stage1_keys(n_layer: int, norm_type: str = "rmsnorm", nonlinearity_type: str = "swiglu", bias: bool = False) -> List[str]:
+    """State-dict keys in the order of mvb_s1_create_ex's offset list (include/mvb200.h): the production list, GELU's
+    ``mlp.c_fc`` in place of the two SwiGLU matrices, then the biases (LayerNorm betas only for LayerNorm)."""
+    ffn = ["mlp.c_fc"] if nonlinearity_type == "gelu" else ["mlp.swiglu.w1", "mlp.swiglu.w3"]
+    layer = ["ln_1", "attn.c_attn", "attn.c_proj", "ln_2"] + ffn + ["mlp.c_proj"]
+    keys = list(_GLOBAL_KEYS) + [f"transformer.h.{i}.{k}.weight" for i in range(n_layer) for k in layer]
+    if bias:
+        ln = norm_type == "layernorm"
+        keys += ["transformer.ln_f.bias"] if ln else []
+        with_bias = [k for k in layer if ln or not k.startswith("ln_")]
+        keys += [f"transformer.h.{i}.{k}.bias" for i in range(n_layer) for k in with_bias]
+    return keys
+
+
+def pack_arena(state_dict: Dict[str, torch.Tensor], n_layer: int, config: Optional["ModelArgs"] = None):
     """Checkpoint state dict -> one contiguous bf16 byte arena (CPU) + byte offsets.
-    Replaces the module construction of ``_load_model`` (fast_inference_utils.py:236-281)."""
+    Replaces the module construction of ``_load_model`` (fast_inference_utils.py:236-281).  ``config`` selects the
+    architecture's tensors (default: the production model's)."""
     sd = {(k[len("_orig_mod."):] if k.startswith("_orig_mod.") else k): v for k, v in state_dict.items()}
-    keys = list(_GLOBAL_KEYS)
-    for i in range(n_layer):
-        keys += [f"transformer.h.{i}.{k}" for k in _LAYER_KEYS]
+    c = config or ModelArgs(n_layer=n_layer)
+    keys = stage1_keys(n_layer, c.norm_type, c.nonlinearity_type, c.bias)
     for k in keys:
         if k not in sd:
             raise KeyError(f"checkpoint is missing {k}")
@@ -89,6 +120,9 @@ class Transformer(Engine):
                  quantisation_mode: Optional[str] = None):
         if quantisation_mode not in (None, "int4", "int8"):
             raise NotImplementedError(f"quantisation_mode={quantisation_mode!r} is not implemented (only None, 'int4' and 'int8')")
+        if quantisation_mode is not None and not config.production_arch:
+            raise NotImplementedError(f"quantisation_mode={quantisation_mode!r} is implemented for the production architecture "
+                                      "(rmsnorm, swiglu, no bias) only")
         super().__init__(device, arena, offsets)
         self.config = config
         self.quantisation_mode = quantisation_mode
@@ -108,7 +142,12 @@ class Transformer(Engine):
         """``quantisation_mode="int4"`` quantises wqkv / wo / w1 / w3 / w2 at load (mvb200/quantize.py) and builds an int4
         engine: decode streams the packed weights through k_gemv_w4, prefill dequantises one layer at a time.
         ``quantisation_mode="int8"`` quantises every Linear per output channel at load and builds an int8 engine: decode
-        streams the int8 weights through k_gemv_w8, prefill widens one layer's q at a time and scales the GEMM outputs."""
+        streams the int8 weights through k_gemv_w8, prefill widens one layer's q at a time and scales the GEMM outputs.
+        ``config``'s norm_type / nonlinearity_type / bias select the architecture (mvb_s1_create_ex); only the production
+        one takes a quantisation mode."""
+        if quantisation_mode is not None and not config.production_arch:
+            raise NotImplementedError(f"quantisation_mode={quantisation_mode!r} is implemented for the production architecture "
+                                      "(rmsnorm, swiglu, no bias) only")
         if quantisation_mode == "int4":
             from .quantize import pack_arena_int4
             arena, offsets, _ = pack_arena_int4(state_dict, config.n_layer)
@@ -116,15 +155,20 @@ class Transformer(Engine):
             from .quantize import pack_arena_int8
             arena, offsets, _ = pack_arena_int8(state_dict, config.n_layer)
         elif quantisation_mode is None:
-            arena, offsets = pack_arena(state_dict, config.n_layer)
+            arena, offsets = pack_arena(state_dict, config.n_layer, config)
         else:
             raise NotImplementedError(f"quantisation_mode={quantisation_mode!r} is not implemented (only None, 'int4' and 'int8')")
         return cls(config, arena, offsets, device, quantisation_mode)
 
     @staticmethod
     def bf16_model_size_bytes(c: ModelArgs) -> int:
-        per_layer = 4 * c.dim * c.dim + 3 * c.dim * c.intermediate_size + 2 * c.dim
+        n_mlp = 2 if c.nonlinearity_type == "gelu" else 3
+        per_layer = 4 * c.dim * c.dim + n_mlp * c.dim * c.intermediate_size + 2 * c.dim
+        if c.bias:   # c_attn, attn.c_proj, the MLP Linears, and the LayerNorm betas
+            per_layer += 4 * c.dim + (n_mlp - 1) * c.intermediate_size + (2 * c.dim if c.norm_type == "layernorm" else 0)
         n = c.n_layer * per_layer + 2 * c.vocab_size * c.dim + c.block_size * c.dim + c.speaker_emb_dim * c.dim + c.dim
+        if c.bias and c.norm_type == "layernorm":
+            n += c.dim
         return n * 2
 
     @staticmethod
@@ -193,6 +237,9 @@ class Transformer(Engine):
         workspace_bytes, create = {None: (self._lib.mvb_s1_workspace_bytes, self._lib.mvb_s1_create),
                                    "int4": (self._lib.mvb_s1_int4_workspace_bytes, self._lib.mvb_s1_create_int4),
                                    "int8": (self._lib.mvb_s1_int8_workspace_bytes, self._lib.mvb_s1_create_int8)}[self.quantisation_mode]
+        if not c.production_arch:
+            self._arch = _lib.S1Arch(_NORMS[c.norm_type], _MLPS[c.nonlinearity_type], int(c.bias))
+            create = lambda cfg_p, *rest: self._lib.mvb_s1_create_ex(cfg_p, C.byref(self._arch), *rest)   # noqa: E731
         self._create(create, self._lib.mvb_s1_destroy, cfg, self._lib.mvb_s1_kv_bytes, workspace_bytes)
         self._spk_key = None
 

@@ -24,7 +24,8 @@ import torch
 
 @dataclass
 class Stage1Dims:
-    """Shape parameters of the stage-1 causal LM (fam/llm/fast_model.py:52-94)."""
+    """Shape parameters of the stage-1 causal LM (fam/llm/fast_model.py:52-94).  norm_type, nonlinearity_type and bias
+    select the architecture of the reference's causal ``GPT`` (model.py:26-46); the defaults are the production model's."""
 
     n_layer: int = 24
     n_head: int = 16
@@ -34,8 +35,13 @@ class Stage1Dims:
     speaker_emb_dim: int = 256
     norm_eps: float = 1e-5
     intermediate_size: Optional[int] = None
+    norm_type: str = "rmsnorm"
+    nonlinearity_type: str = "swiglu"
+    bias: bool = False
 
     def __post_init__(self):
+        if self.intermediate_size is None and self.nonlinearity_type == "gelu":
+            self.intermediate_size = 4 * self.dim        # fam/llm/layers/layers.py:46
         if self.intermediate_size is None:
             # fam/llm/fast_model.py:69-72: find_multiple(int(2*4*dim/3), 256)
             n_hidden = int(2 * 4 * self.dim / 3)
@@ -47,8 +53,12 @@ class Stage1Dims:
 
     def n_params(self) -> int:
         d, f, v = self.dim, self.intermediate_size, self.vocab_size
-        per_layer = 3 * d * d + d * d + 3 * d * f + 2 * d
-        return self.n_layer * per_layer + 2 * v * d + self.block_size * d + self.speaker_emb_dim * d + d
+        n_mlp = 2 if self.nonlinearity_type == "gelu" else 3
+        ln_beta = self.bias and self.norm_type == "layernorm"
+        per_layer = 3 * d * d + d * d + n_mlp * d * f + 2 * d
+        if self.bias:
+            per_layer += 4 * d + (n_mlp - 1) * f + (2 * d if ln_beta else 0)
+        return self.n_layer * per_layer + 2 * v * d + self.block_size * d + self.speaker_emb_dim * d + d + (d if ln_beta else 0)
 
 
 FULL = Stage1Dims()
@@ -69,9 +79,13 @@ def stage1_state_dict(dims: Stage1Dims, seed: int = 0, tie_head: bool = False) -
     reference's all-ones so that the gain path is actually exercised by parity tests.
     The LM head is drawn independently by default (the reference loads it as a separate
     tensor, fast_inference_utils.py:252) so head and embedding mistakes cannot cancel.
+    A GELU MLP draws ``mlp.c_fc`` where SwiGLU draws w1 and has no w3; with ``dims.bias``, LayerNorm betas 0.1 N(0, 1)
+    and Linear biases 0.02 N(0, 1) are drawn after every other tensor, non-zero so that a dropped bias changes the
+    output.  The default architecture draws exactly the tensors it always has.
     """
     gen = torch.Generator().manual_seed(seed)
     d, f, v = dims.dim, dims.intermediate_size, dims.vocab_size
+    gelu, ln = dims.nonlinearity_type == "gelu", dims.norm_type == "layernorm"
     proj_std = 0.02 / math.sqrt(2 * dims.n_layer)
     sd: Dict[str, torch.Tensor] = {}
     sd["transformer.wtes.0.weight"] = _normal(gen, (v, d), 0.02)
@@ -83,14 +97,35 @@ def stage1_state_dict(dims: Stage1Dims, seed: int = 0, tie_head: bool = False) -
         sd[p + "attn.c_attn.weight"] = _normal(gen, (3 * d, d), 0.02)
         sd[p + "attn.c_proj.weight"] = _normal(gen, (d, d), proj_std)
         sd[p + "ln_2.weight"] = (1.0 + 0.1 * torch.empty(d).normal_(generator=gen)).to(torch.bfloat16)
-        sd[p + "mlp.swiglu.w1.weight"] = _normal(gen, (f, d), 0.02)
-        sd[p + "mlp.swiglu.w3.weight"] = _normal(gen, (f, d), 0.02)
+        if gelu:
+            sd[p + "mlp.c_fc.weight"] = _normal(gen, (f, d), 0.02)
+        else:
+            sd[p + "mlp.swiglu.w1.weight"] = _normal(gen, (f, d), 0.02)
+            sd[p + "mlp.swiglu.w3.weight"] = _normal(gen, (f, d), 0.02)
         sd[p + "mlp.c_proj.weight"] = _normal(gen, (d, f), proj_std)
     sd["transformer.ln_f.weight"] = (1.0 + 0.1 * torch.empty(d).normal_(generator=gen)).to(torch.bfloat16)
     if tie_head:
         sd["lm_heads.0.weight"] = sd["transformer.wtes.0.weight"]
     else:
         sd["lm_heads.0.weight"] = _normal(gen, (v, d), 0.02)
+    if dims.bias:
+        beta = lambda: _normal(gen, (d,), 0.1)      # noqa: E731
+        lin = lambda n: _normal(gen, (n,), 0.02)    # noqa: E731
+        if ln:
+            sd["transformer.ln_f.bias"] = beta()
+        for i in range(dims.n_layer):
+            p = f"transformer.h.{i}."
+            if ln:
+                sd[p + "ln_1.bias"] = beta()
+                sd[p + "ln_2.bias"] = beta()
+            sd[p + "attn.c_attn.bias"] = lin(3 * d)
+            sd[p + "attn.c_proj.bias"] = lin(d)
+            if gelu:
+                sd[p + "mlp.c_fc.bias"] = lin(f)
+            else:
+                sd[p + "mlp.swiglu.w1.bias"] = lin(f)
+                sd[p + "mlp.swiglu.w3.bias"] = lin(f)
+            sd[p + "mlp.c_proj.bias"] = lin(d)
     return sd
 
 
@@ -129,28 +164,32 @@ def synthetic_tokenizer_meta(n_text_tokens: int = 512, offset: int = 2049) -> di
     )
 
 
-def stage1_checkpoint(dims: Stage1Dims, seed: int = 0) -> dict:
-    """Full ``first_stage.pt`` container (SURVEY.md App. B)."""
-    model_args = dict(
+def stage1_model_args(dims: Stage1Dims) -> dict:
+    """``first_stage.pt["model_args"]``: the GPTConfig (fam/llm/model.py:26-46) the reference builds the model from."""
+    return dict(
         n_layer=dims.n_layer,
         n_head=dims.n_head,
         n_embd=dims.dim,
         block_size=dims.block_size,
-        bias=False,
+        bias=dims.bias,
         vocab_sizes=[dims.vocab_size],
         causal=True,
         target_vocab_sizes=None,
-        norm_type="rmsnorm",
+        norm_type=dims.norm_type,
         rmsnorm_eps=dims.norm_eps,
-        nonlinearity_type="swiglu",
+        nonlinearity_type=dims.nonlinearity_type,
         attn_kernel_type="torch_attn",
         spk_emb_on_text=True,
         swiglu_multiple_of=256,
         dropout=0.0,
     )
+
+
+def stage1_checkpoint(dims: Stage1Dims, seed: int = 0, tie_head: bool = False) -> dict:
+    """Full ``first_stage.pt`` container (SURVEY.md App. B)."""
     return dict(
-        model=stage1_state_dict(dims, seed),
-        model_args=model_args,
+        model=stage1_state_dict(dims, seed, tie_head=tie_head),
+        model_args=stage1_model_args(dims),
         config=dict(causal=True),
         meta=dict(tokenizer=synthetic_tokenizer_meta(), speaker_cond=True, speaker_emb_size=dims.speaker_emb_dim),
         iter_num=0,
