@@ -267,6 +267,13 @@ int mvb_linear(const void* d_W, int32_t M, int32_t K, const float* d_x, int32_t 
                const void* d_gain, float eps, int32_t split_lo, int32_t ksplit_override, float* d_out,
                int32_t ldo, int32_t accumulate, void* stream);
 
+/* Test hook (not part of the drop-in surface): cap the SM count the library plans for.  While n > 0, every engine
+ * create and test hook reads the device's SM count as min(real, n), so the persistent decode kernel's grid, its K
+ * splits, attention units and fused-sampler choice, and every split-K GEMM plan are those of a part with n SMs.  The
+ * cap never raises the count (those kernels need every CTA co-resident).  n = 0 removes it; n < 0 is MVB_ERR_ARG.
+ * A handle keeps the count it was created with.  Process-wide; no device setting is touched. */
+int mvb_test_set_sm_limit(int32_t n);
+
 /* Test hooks for the op-level tests of two tensor-core kernels (not part of the drop-in surface):
  *   mvb_gemm_test     : mvb_linear's operator with any epilogue of the weight-streaming GEMM (csrc/tc_gemm.cuh):
  *                       epi 0 store, 1 residual add, 2 SwiGLU  out = silu(x W^T) * (x W3^T)  (d_W3 bf16 [M, K]),

@@ -1,4 +1,5 @@
 // Definitions of the shared host helpers (host.cuh) and of the library-wide C ABI entry points.
+#include <atomic>
 #include <cstdarg>
 #include <cstdio>
 #include <string>
@@ -29,10 +30,22 @@ int check_offsets(const uint64_t* off, size_t n, size_t arena_bytes, const char*
   return MVB_OK;
 }
 
+// SM cap of mvb_test_set_sm_limit (0: none).  It only ever lowers the count: the persistent kernel and the split-K
+// GEMM need every CTA of their grid co-resident, which a count above the device's own would break.
+static std::atomic<int> g_sm_limit{0};
+
 int current_device(int* dev, int* n_sm) {
   MVB_CK(cudaGetDevice(dev));
   MVB_CK(cudaDeviceGetAttribute(n_sm, cudaDevAttrMultiProcessorCount, *dev));
+  const int cap = g_sm_limit.load();
+  if (cap > 0 && cap < *n_sm) *n_sm = cap;
   return MVB_OK;
 }
 
 }  // namespace mvb
+
+extern "C" int mvb_test_set_sm_limit(int32_t n) {
+  if (n < 0) return mvb::set_error(MVB_ERR_ARG, "mvb_test_set_sm_limit: n = %d must be >= 0", n);
+  mvb::g_sm_limit.store(n);
+  return MVB_OK;
+}

@@ -863,7 +863,9 @@ static int launch_persistent(mvb_s1* h, cudaStream_t s, int n_utts, int n_steps,
 // so the batch has at most R H Z units of at most ceil(TT / Z) tiles each.  Units are dealt round-robin over the G CTAs,
 // so no CTA owns more than ceil(R H Z / G) units, i.e. ceil(R H Z / G) * ceil(TT / Z) tiles, whatever the positions.
 // The same Z bounds the split count that indexes the PC_MAX_CHUNKS partial slots of every (row, head).
-// At block_size 2048, H = 16 on 132 SMs the worst case (fp32 cache, 8 utterances: Z = 1, TT = 64) is exactly 128.
+// The bound is derived for G = n_sm, so which batches reach PC_MAX_TILES depends on the part.  At block_size 2048, H = 16
+// it is reached (exactly 128 tiles) by fp32 KV with 8 utterances at 132 SMs, fp32 with 1 utterance at 16, fp32 with 4 at
+// 64, bf16 with 8 at 64 and bf16 with 1 at 8; a batch one past such an edge goes to the per-layer path.
 static bool pc_att_fits(const mvb_s1* h, int n_utts) {
   const int R = 2 * n_utts, H = h->cfg.n_head, G = h->n_sm;
   const int ppc = PC_KV_TILE_BYTES / (128 * (int)h->kv_elem());
@@ -874,9 +876,11 @@ static bool pc_att_fits(const mvb_s1* h, int n_utts) {
   return Z <= PC_MAX_CHUNKS && units_per_cta * ((TT + Z - 1) / Z) <= PC_MAX_TILES;
 }
 
-// The persistent decode kernel serves the batch (else the per-layer path does).
+// The persistent decode kernel serves the batch (else the per-layer path does).  CTA 2b alone writes batch entry b's
+// x rows and decode state back (decode_persistent.cuh, `owner`), so CTA 2 (n_utts - 1) must exist: pc_att_fits does not
+// imply it at a short block_size or a small width.
 static bool use_path_c(const mvb_s1* h, int n_utts) {
-  return h->path_c && h->pc_ok && 2 * n_utts <= PC_RPAD && pc_att_fits(h, n_utts);
+  return h->path_c && h->pc_ok && 2 * n_utts <= PC_RPAD && 2 * n_utts - 1 <= h->n_sm && pc_att_fits(h, n_utts);
 }
 
 static int run_body(mvb_s1* h, cudaStream_t s, int n_utts, bool allow_b = true) {

@@ -209,6 +209,7 @@ SIGNATURES = {
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p]),
     "mvb_spk_op_test": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                   C.c_void_p]),
+    "mvb_test_set_sm_limit": (C.c_int, [C.c_int32]),
 }
 ABI_VERSION = 3
 

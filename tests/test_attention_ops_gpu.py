@@ -105,19 +105,20 @@ def _n_sm():
     return torch.cuda.get_device_properties(0).multi_processor_count
 
 
-def _pc_fits(n_utts, H, kv):
+def _pc_fits(n_utts, H, kv, n_sm=None):
     """Mirror of pc_att_fits (stage1_engine.cu): the persistent kernel's per-CTA attention tile table (<= 128 tiles) and
-    split count (<= 64) hold for n_utts utterances at every position of the 2048-slot context on this part."""
-    G, R = _n_sm(), 2 * n_utts
-    TT = BLOCK // (32 if kv == "fp32" else 64)
-    Z = min(max(1, G // (R * H)), TT)
-    return Z <= 64 and -(-R * H * Z // G) * -(-TT // Z) <= 128
+    split count (<= 64) hold for n_utts utterances at every position of the 2048-slot context on a part with n_sm SMs
+    (default: this one)."""
+    from test_sm_count_cpu import att_fits
+    return att_fits(n_sm or _n_sm(), n_utts, H, kv, BLOCK)
 
 
 def expected_body(p, n_utts):
-    """The body mvb_s1_step_logits / mvb_s1_decode runs for n_utts utterances of probe p: the persistent kernel where its
-    tile table fits, else the per-layer path (tensor-core rows path from 2 utterances up)."""
-    if p.body == "C" and not _pc_fits(n_utts, p.H, p.kv):
+    """The body mvb_s1_step_logits / mvb_s1_decode runs for n_utts utterances of probe p: the persistent kernel where the
+    host's rule (use_path_c, mirrored in test_sm_count_cpu.py) takes the batch, else the per-layer path (tensor-core rows
+    path from 2 utterances up)."""
+    from test_sm_count_cpu import path_c
+    if p.body == "C" and not path_c((p.D, p.H, 256, p.V), p.n_sm, n_utts, p.kv, BLOCK):
         return "B" if n_utts >= 2 else "A"
     return p.body
 
@@ -143,9 +144,11 @@ def softmax_eps(s, A, n_resc, n_acc, kappa, rho_p):
 # ---------------------------------------------------------------------------------------------------------------------
 # stage-1 probe model
 class Probe:
-    def __init__(self, H, form, utts, seed=0, n_layer=1):
+    def __init__(self, H, form, utts, seed=0, n_layer=1, n_sm=None):
+        """n_sm: the SM count the engine is planned for (default: this device's)."""
         from mvb200.fast_model import ModelArgs, Transformer
         kv, tc, body = FORMS[form]
+        self.n_sm = n_sm or _n_sm()
         self.H, self.D, self.form, self.body, self.kv = H, 128 * H, form, body, kv
         D = self.D
         self.V = 512 if D <= 256 else 2562
@@ -425,9 +428,14 @@ def test_persistent_tile_table_at_capacity(probes):
 def test_split_merge_above_four_splits(probes):
     """H = 2, one utterance: zmax = n_sm / 4, so long rows are cut into more than 4 splits and the wo staging takes its
     nch > 4 merge branch (fp32: up to 64 tiles -> min(zmax, 64) splits)."""
-    n_sm = torch.cuda.get_device_properties(0).multi_processor_count
+    split_merge(probes)
+
+
+def split_merge(probes):
+    """test_split_merge_above_four_splits on the SM count the probes are planned for."""
     for form, ppc in (("C-fp32", 32), ("C-mma", 64)):
         p = probes(2, form, 8)
+        n_sm = p.n_sm
         for L in (1000, 2048):
             tt = (L + ppc - 1) // ppc
             zr = min(n_sm // 4, tt)
@@ -519,10 +527,17 @@ def test_fused_burst_reads_back_its_own_appends(probes, form, first, last, n_utt
     + eps)):  r b + |n1| r^2 sum(|z| b) / D, plus 2^-15 |n1| for the layer-1 QKV (hi/lo staging, 256-term fp32 sum of
     squares, rsqrtf) and 2^-8 |n1| for the bf16 rounding.  No other cache byte changes.  With the fp32 cache, a reference
     that misses the entry appended one step earlier (a stale read) must violate the bound."""
-    from mvb200 import _lib
     p = probes(2, form, 8, n_layer=2)
     if expected_body(p, n_utts) != "C":
         pytest.skip(f"on {_n_sm()} SMs the persistent kernel does not take this batch")
+    fused_burst(probes, form, first, last, n_utts)
+
+
+def fused_burst(probes, form, first, last, n_utts):
+    """test_fused_burst_reads_back_its_own_appends on the SM count the probes are planned for; path C must take the
+    batch with the fused sampler."""
+    from mvb200 import _lib
+    p = probes(2, form, 8, n_layer=2)
     n_steps, D = last - first + 1, p.D
     g = torch.Generator(device="cuda").manual_seed(first + n_utts)
     toks = torch.randint(0, p.V, (n_utts, n_steps), generator=torch.Generator().manual_seed(first + n_utts))

@@ -134,7 +134,7 @@ def plan_pc(M, K, ctas, tile_rows=128):
         cost = tiles_per * (2 * kb_per + 5) + 4 * kb_per
         if best is None or cost < best[0]:
             best = (cost, S)
-    return best[1]
+    return best[1] if best else 0     # 0: no split fits (the host then declines path C)
 
 
 def plan_gemm_ksplit(M, K, n_sm):
@@ -148,29 +148,31 @@ def plan_gemm_ksplit(M, K, n_sm):
     return min(ks, 16)
 
 
-def n_split(body, mat):
-    """K splits whose fp32 partials are added for one output element (0 on path A)."""
+def n_split(body, mat, n_sm=None):
+    """K splits whose fp32 partials are added for one output element (0 on path A), planned for n_sm SMs (default:
+    this device's count)."""
     M, K = MATS[mat]
+    n_sm = n_sm or _n_sm()
     if body == "C":
-        return plan_pc(M, K, _n_sm())
+        return plan_pc(M, K, n_sm)
     if body == "B":
-        return plan_gemm_ksplit(M // 2 if mat == "w13" else M, K, _n_sm())   # the SwiGLU instance tiles w1 and w3 together
+        return plan_gemm_ksplit(M // 2 if mat == "w13" else M, K, n_sm)   # the SwiGLU instance tiles w1 and w3 together
     return 0
 
 
-def gamma(body, mat):
+def gamma(body, mat, n_sm=None):
     """gamma of the module docstring: MMAs of the longest split (ceil(KB / S) k-blocks, hi and lo) + the split adds + 1."""
     K = MATS[mat][1]
     if body == "A":
         return (K / 32 + 5 + 1) * U
-    S = n_split(body, mat)
+    S = n_split(body, mat, n_sm)
     return (18 * 4 * 2 * -(-(K // 64) // S) + S + 1) * U
 
 
-def split0_cols(mat):
+def split0_cols(mat, n_sm=None):
     """The columns of split 0 of path C's plan (pc_slice: kb1 = KB / S for split 0)."""
     M, K = MATS[mat]
-    return 64 * ((K // 64) // plan_pc(M, K, _n_sm()))
+    return 64 * ((K // 64) // plan_pc(M, K, n_sm or _n_sm()))
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -219,9 +221,10 @@ class Arena:
 
 
 class Engine:
-    def __init__(self, arena, form):
+    def __init__(self, arena, form, n_sm=None):
+        """n_sm: the SM count the engine is planned for (default: this device's)."""
         from mvb200.fast_model import ModelArgs, Transformer
-        self.form = form
+        self.form, self.n_sm = form, n_sm or _n_sm()
         self.kv, tc, self.body, self.utts = FORMS[form]
         cfg = ModelArgs(block_size=BLOCK, vocab_size=V, n_layer=NL, n_head=H, dim=D, intermediate_size=F)
         self.m = Transformer(cfg, arena.buf, arena.offsets, device="cuda:0")
@@ -289,8 +292,8 @@ def linear(W, nh, s):
     return (nh @ W.t()) * s, (nh.abs() @ W.abs().t()) * s
 
 
-def lin_bound(body, mat, y, A):
-    return (gamma(body, mat) + TAU[body]) * A + 2 * U * y.abs() + 1e-30
+def lin_bound(body, mat, y, A, n_sm=None):
+    return (gamma(body, mat, n_sm) + TAU[body]) * A + 2 * U * y.abs() + 1e-30
 
 
 def rs64(x):
@@ -357,7 +360,7 @@ def appended(e, n, poss, l):
 def kv_bound(e, y, A, i):
     """reference and bound of the appended k (i = 0) or v (i = 1) from the QKV reference y, A [R, 3D]."""
     sl = slice((i + 1) * D, (i + 2) * D)
-    ref, b = y[:, sl], lin_bound(e.body, "qkv", y[:, sl], A[:, sl])
+    ref, b = y[:, sl], lin_bound(e.body, "qkv", y[:, sl], A[:, sl], e.n_sm)
     if e.kv == "bf16":
         b = b + BF16_U * (ref.abs() + b)
     return ref, b
@@ -514,7 +517,7 @@ def run_probe(a, e, probe, l):
                 r, w = check_kv(e, label, kv_got, y, A)
                 worst, nw = max(worst, r), max(nw, w)
                 if sens_case and body == "C" and probe == "qkv":
-                    c = split0_cols("qkv")
+                    c = split0_cols("qkv", e.n_sm)
                     y_d = linear(Wqkv[:, c:], nh[:, c:], s)[0]
                     sens["qkv without split 0"] = sum(
                         n_over(kv_got[i], y_d[:, (i + 1) * D:(i + 2) * D], kv_bound(e, y, A, i)[1]) for i in range(2))
@@ -522,29 +525,30 @@ def run_probe(a, e, probe, l):
                     v = kv_got[1]
                     op = v if body == "A" else hilo(v.float())[0]
                     yo, Ao = linear(Wo, op, 1.0)
-                    b = gamma(body, "o") * Ao + (n_split(body, "o") + 1) * U * x.abs() + 1e-30
+                    b = gamma(body, "o", e.n_sm) * Ao + (n_split(body, "o", e.n_sm) + 1) * U * x.abs() + 1e-30
                     yh = recover(a, lg, x)
                     r, w = assess(label + " y", yh, yo, obs_bound(body, x, yo, b), mask)
                     worst, nw = max(worst, r), max(nw, w)
             elif probe == "ffn":
                 check_cache_rest(e, n, poss, l)
                 yh = recover(a, lg, x)
-                yr, b, parts = _ffn_ref(body, x, g2, W1, W3, W2)
+                yr, b, parts = _ffn_ref(body, x, g2, W1, W3, W2, n_sm=e.n_sm)
                 r, w = assess(label + " y", yh, yr, obs_bound(body, x, yr, b), mask)
                 worst, nw = max(worst, r), max(nw, w)
                 if sens_case:
                     bo = obs_bound(body, x, yr, b)
-                    sens["u scaled by rs, g not"] = n_over(yh, _ffn_ref(body, x, g2, W1, W3, W2, g_unscaled=True)[0], bo, mask)
-                    sens["ln_1 gain in the FFN"] = n_over(yh, _ffn_ref(body, x, g1, W1, W3, W2)[0], bo, mask)
+                    sens["u scaled by rs, g not"] = n_over(yh, _ffn_ref(body, x, g2, W1, W3, W2, g_unscaled=True, n_sm=e.n_sm)[0],
+                                                           bo, mask)
+                    sens["ln_1 gain in the FFN"] = n_over(yh, _ffn_ref(body, x, g1, W1, W3, W2, n_sm=e.n_sm)[0], bo, mask)
                     if body == "C":
-                        c = split0_cols("w2")
+                        c = split0_cols("w2", e.n_sm)
                         h = parts["h"]
                         sens["w2 without split 0"] = n_over(yh, h[:, c:] @ W2[:, c:].t(), bo, mask)
             else:   # head
                 check_cache_rest(e, n, poss, l)
                 nh, hi, s = operand(x, gf, body)
                 y, A = linear(Wh, nh, s)
-                b = lin_bound(body, "head", y, A)
+                b = lin_bound(body, "head", y, A, e.n_sm)
                 r, w = assess(label + " logits", lg, y, b)
                 worst, nw = max(worst, r), max(nw, w)
                 if sens_case:
@@ -554,7 +558,7 @@ def run_probe(a, e, probe, l):
                     if body != "A":
                         sens["head operand hi only"] = n_over(lg[:1], linear(Wh, hi, s)[0][:1], b[:1])
                     if body == "C":
-                        c = split0_cols("head")
+                        c = split0_cols("head", e.n_sm)
                         sens["head without split 0"] = n_over(lg, linear(Wh[:, c:], nh[:, c:], s)[0], b)
     finally:
         case.clear()
@@ -564,12 +568,12 @@ def run_probe(a, e, probe, l):
     return worst, nw, sens
 
 
-def _ffn_ref(body, x, gain, W1, W3, W2, g_unscaled=False):
+def _ffn_ref(body, x, gain, W1, W3, W2, g_unscaled=False, n_sm=None):
     """float64 FFN of the module docstring: (y, elementwise bound before the observation chain, parts)."""
     nh, _, s = operand(x, gain, body)
     G, AG = linear(W1, nh, s)
     Uu, AU = linear(W3, nh, s)
-    gam, tau = gamma(body, "w13"), TAU[body]
+    gam, tau = gamma(body, "w13", n_sm), TAU[body]
     eg = (gam + tau) * AG + 2.0 ** -21 * G.abs()
     eu = (gam + tau) * AU + 2.0 ** -21 * Uu.abs()
     if g_unscaled:
@@ -581,7 +585,8 @@ def _ffn_ref(body, x, gain, W1, W3, W2, g_unscaled=False):
     if body != "A":
         eh = eh + HILO * (h.abs() + eh)
     y = h @ W2.t()
-    b = gamma(body, "w2") * ((h.abs() + eh) @ W2.abs().t()) + eh @ W2.abs().t() + (n_split(body, "w2") + 1) * U * x.abs()
+    b = (gamma(body, "w2", n_sm) * ((h.abs() + eh) @ W2.abs().t()) + eh @ W2.abs().t()
+         + (n_split(body, "w2", n_sm) + 1) * U * x.abs())
     return y, b + 1e-30, {"h": h}
 
 
@@ -637,8 +642,8 @@ def _run_mixed(a, e, case, label, n, g1, Wqkv, Wo, mask, sens):
         m, em = torch.stack(mean), torch.stack(em)
         eop = em + (0.0 if body == "A" else HILO * (m.abs() + em))
         yo = m @ Wo.t()
-        b = (gamma(body, "o") * ((m.abs() + eop) @ Wo.abs().t()) + eop @ Wo.abs().t()
-             + (n_split(body, "o") + 1) * U * x.abs() + 1e-30)
+        b = (gamma(body, "o", e.n_sm) * ((m.abs() + eop) @ Wo.abs().t()) + eop @ Wo.abs().t()
+             + (n_split(body, "o", e.n_sm) + 1) * U * x.abs() + 1e-30)
         yh = recover(a, lg, x)
         r, w = assess(f"{label} launch {it} y", yh, yo, obs_bound(body, x, yo, b), mask)
         worst, nw = max(worst, r), max(nw, w)

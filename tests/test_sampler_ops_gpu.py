@@ -260,9 +260,10 @@ class Probe:
     """The probe model of the module docstring at vocabulary V for `utts` utterance slots; tc and mode are
     setup_caches' tensor_core_path and from_state_dict's quantisation_mode."""
 
-    def __init__(self, V, utts, fused=True, seed=0, tc=None, mode=None):
+    def __init__(self, V, utts, fused=True, seed=0, tc=None, mode=None, n_sm=None):
+        """n_sm: the SM count the engine is planned for (default: this device's)."""
         from mvb200.fast_model import ModelArgs, Transformer
-        self.V = V
+        self.V, self.n_sm = V, n_sm or _n_sm()
         rng = np.random.default_rng(seed + V)
         tok = np.zeros((V, D), np.float32)
         tok[np.arange(V), np.arange(V) % N_COL] = 1.0
@@ -335,12 +336,9 @@ class Probe:
 
     def body(self, n, top_k_any=False):
         """(sampler, per-step launches) mvb_s1_decode must run for n utterances, and whether it is one fused launch."""
-        R = 2 * n
-        TT = BLOCK // 64
-        Z = min(max(1, _n_sm() // (R * H)), TT)
-        path_c = R <= 16 and Z <= 64 and -(-R * H * Z // _n_sm()) * -(-TT // Z) <= 128
-        if path_c:
-            if self.fused and not top_k_any and -(-self.V // _n_sm()) <= 32:
+        from test_sm_count_cpu import fused_ok, path_c
+        if path_c((D, H, F, self.V), self.n_sm, n, "bf16", BLOCK):
+            if self.fused and not top_k_any and fused_ok(self.n_sm, self.V):
                 return "fused"
             return "C+k_sample"
         return "B+k_sample" if n >= 2 else "A+k_sample"
@@ -587,7 +585,12 @@ def test_decode_burst_supplied_noise(probes, V, n, fused, top_k):
     """A 40-step mvb_s1_decode burst, every slot with its own guidance / temperature / top_p (and top_k > 0 on even
     slots, which forces k_sample), forced tokens, supplied noise: every draw against the float64 reference.  The body
     (one fused launch; persistent + k_sample per step; path B + k_sample) is asserted from the launch count."""
-    p = probes(V, 12 if n > 8 else 8, fused)
+    burst_supplied_noise(probes(V, 12 if n > 8 else 8, fused), n, top_k)
+
+
+def burst_supplied_noise(p, n, top_k):
+    """test_decode_burst_supplied_noise on probe p; returns the sampler that ran."""
+    V, fused = p.V, p.fused
     rng = np.random.default_rng(V + n + (top_k or 0))
     n_steps = 40
     slots = _slots(n, V, n_steps, rng, top_k)
@@ -595,9 +598,10 @@ def test_decode_burst_supplied_noise(probes, V, n, fused, top_k):
     table = p.table(n, np.concatenate([s["fed"] for s in slots]))
     sampled, noises, body = run_decode(p, slots, n_steps, seed=V + n)
     if fused and top_k is None and n <= 8:
-        assert body == "fused" or -(-V // _n_sm()) > 32
+        assert body == "fused" or -(-V // p.n_sm) > 32
     draws, near, nb = check_decode(p, slots, sampled, noises, table, body, f"V={V} n={n}")
-    print(f"decode V={V}, {n} utterances [{body}]: {draws} draws, {near} certified near-ties, {nb} band entries")
+    print(f"decode V={V}, {n} utterances [{body}] on {p.n_sm} SMs: {draws} draws, {near} certified near-ties, {nb} band entries")
+    return body
 
 
 def test_decode_eoa_latch_leaves_other_slots_alone(probes):
@@ -681,7 +685,11 @@ def test_decode_flat_tie_order_exact(probes, fused):
     """V = 4096, every logit equal, top_p = 0.5: the kept set is exactly 2048 ... 4095 in the fused ranking and in
     k_sample's sort.  Designed noise puts the smallest q on 2047 / 2048 / 4095 / 0: the tokens must be 2048, 2048,
     4095, 3000, 2049, 4095, and the remaining steps the argmin of q over 2048 ... 4095."""
-    p = probes(4096, 8, fused)
+    flat_tie_order(probes(4096, 8, fused))
+
+
+def flat_tie_order(p):
+    """test_decode_flat_tie_order_exact on probe p (V = 4096); returns the sampler that ran."""
     n_steps = 12
     slot = dict(g=3.0, T=1.0, top_p=0.5, fed=np.zeros(n_steps + 1, int), design=_flat_design)
     p.set_speakers([0.0])
@@ -689,10 +697,11 @@ def test_decode_flat_tie_order_exact(probes, fused):
     lg = table[0]
     assert np.all(lg == lg[0, 0]), "the flat column does not give equal logits"
     sampled, noises, body = run_decode(p, [slot], n_steps, seed=3)
-    assert body == ("fused" if fused else "C+k_sample")
+    assert body == ("fused" if p.fused and -(-4096 // p.n_sm) <= 32 else "C+k_sample")
     want = [2048 + int(np.argmin(noises[0][i, 2048:])) for i in range(n_steps)]
     assert want[:6] == [2048, 2048, 4095, 3000, 2049, 4095]
     assert sampled[0].tolist() == want
+    return body
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -179,9 +179,12 @@ class Model:
 
 
 class Eng:
-    def __init__(self, model, fmt, kv, tc, utts):
+    def __init__(self, model, fmt, kv, tc, utts, n_sm=None):
+        """n_sm: the SM count the engine is planned for (default: this device's)."""
         from mvb200.fast_model import ModelArgs, Transformer
+        from test_decode_linear_ops_gpu import _n_sm
         self.model, self.fmt, self.kv, self.tc, self.utts = model, fmt, kv, tc, utts
+        self.n_sm = n_sm or _n_sm()
         arena, self.offsets = model.arenas[fmt]
         cfg = ModelArgs(block_size=BLOCK, vocab_size=V, n_layer=NL, n_head=H, dim=D, intermediate_size=F)
         self.m = Transformer(cfg, arena, self.offsets, device="cuda:0", quantisation_mode=None if fmt == "bf16" else fmt)
@@ -382,7 +385,14 @@ def body_rows(n, tc, tu, ps):
 
 @pytest.mark.parametrize("body", list(BODIES))
 def test_embedding_bit_exact(model, engines, body):
-    kv, tc_path, utts, counts, xbuf = BODIES[body]
+    embedding_bit_exact(model, engines, body)
+
+
+def embedding_bit_exact(model, engines, body, counts=None):
+    """test_embedding_bit_exact on the engines `engines` returns (their SM count may be capped), for the utterance
+    counts `counts` (default: the body's own) that the body takes on that count."""
+    kv, tc_path, utts, own, xbuf = BODIES[body]
+    counts = counts or own
     e = engines("bf16", kv, tc_path, utts)
     e.m._kv.zero_()
     sp = e.sl("spk", torch.float32).view(utts, D).clone()
@@ -405,21 +415,26 @@ def test_embedding_bit_exact(model, engines, body):
             pm = [max(p - 1, 0) for p in rows[1]]
             sel = torch.tensor(rows[1], device="cuda") > 0
             caught(f"{body}: position row pos - 1", float((got != x_rows(model, sp, rows[0], pm, rows[2], rows[3]))[sel].float().mean()), BIT_SENS)
-    print(f"embedding, body {body} ({LAUNCHES[body[0]]} launches), n_utts {list(counts)}: bit exact")
+    print(f"embedding, body {body} ({LAUNCHES[body[0]]} launches), n_utts {list(counts)}, {e.n_sm} SMs: bit exact")
 
 
 # ---------------------------------------------------------------------------------------------------------------------
 # 3. the persistent kernel's staged layer-0 operand
 @pytest.mark.parametrize("kv", ["fp32", "bf16"])
 def test_staged_operand(model, engines, kv):
-    from test_decode_linear_ops_gpu import _n_sm
+    staged_operand(model, engines, kv)
+
+
+def staged_operand(model, engines, kv, counts=(1, 4, 5, 8)):
+    """test_staged_operand on the engines `engines` returns, with the qkv K split planned for their SM count, for the
+    utterance counts `counts` (path C must take each)."""
     e = engines("bf16", kv, "BC", MAXU)
     o_g, o_w = e.offsets[5], e.offsets[5 + 1]
     g1 = e.arena[o_g:o_g + 2 * D].view(torch.bfloat16)
     Wqkv = e.arena[o_w:o_w + 2 * 3 * D * D].view(torch.bfloat16).view(3 * D, D)
     gen = torch.Generator(device="cuda").manual_seed(5)
     gain = (1 + 0.1 * torch.randn(D, generator=gen, device="cuda")).to(torch.bfloat16)
-    depth = 8 + 5 + 8 + plan_pc(3 * D, D, _n_sm()) + 2
+    depth = 8 + 5 + 8 + plan_pc(3 * D, D, e.n_sm) + 2
     sp = e.sl("spk", torch.float32).view(MAXU, D).clone()
     worst = 0.0
     sens = {"speaker dropped": [], "other row's token": [], "position row pos + 1": []}
@@ -427,7 +442,7 @@ def test_staged_operand(model, engines, kv):
         g1.copy_(gain)
         Wqkv[D:2 * D] = torch.eye(D, device="cuda").to(torch.bfloat16)
         torch.cuda.synchronize()
-        for n in (1, 4, 5, 8):
+        for n in counts:
             e.m._kv.zero_()
             tc, tu, ps = design(n, 100 + n)
             begin(e, n, tc, tu, ps)
@@ -439,7 +454,7 @@ def test_staged_operand(model, engines, kv):
             def ref(xx):
                 nh, _, s = operand(xx.double(), gain, "C")
                 y, A = nh * s, nh.abs() * s
-                b = lin_bound("C", "qkv", y, A) + tau_ss(depth) * A
+                b = lin_bound("C", "qkv", y, A, e.n_sm) + tau_ss(depth) * A
                 if kv == "bf16":
                     b = b + BF16_U * (y.abs() + b)
                 return y, b
@@ -458,7 +473,7 @@ def test_staged_operand(model, engines, kv):
         torch.cuda.synchronize()
     for name, v in sens.items():
         caught(f"staged operand kv {kv}: {name}", float(torch.cat([t.flatten() for t in v]).double().mean()), BOUND_SENS)
-    print(f"staged layer-0 operand, path C kv {kv}, n_utts 1 4 5 8: max |err|/bound {worst:.2e}")
+    print(f"staged layer-0 operand, path C kv {kv}, n_utts {list(counts)}, {e.n_sm} SMs: max |err|/bound {worst:.2e}")
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -504,7 +519,7 @@ def head_ref(e, x, body):
     sc = 1.0 if s is None else s[None, :]
     y = (nh @ W.t()) * rs * sc
     A = (nh.abs() @ W.abs().t()) * rs * sc
-    b = lin_bound(body, "head", y, A) + tau_ss(SS_DEPTH_AB) * A
+    b = lin_bound(body, "head", y, A, e.n_sm) + tau_ss(SS_DEPTH_AB) * A
     if s is not None:
         b = b + U * y.abs()
     return y, b
@@ -601,6 +616,11 @@ PREFILL_ENGINES = [("bf16", "bf16"), ("bf16", "fp32"), ("int8", "fp32"), ("int8"
 
 @pytest.mark.parametrize("fmt,kv", PREFILL_ENGINES, ids=[f"{f}-{k}" for f, k in PREFILL_ENGINES])
 def test_prefill(model, engines, fmt, kv):
+    prefill_cases(engines, fmt, kv, PREFILL)
+
+
+def prefill_cases(engines, fmt, kv, cases):
+    """test_prefill for the (S, pos0) cases on the engines `engines` returns (their SM count may be capped)."""
     e = engines(fmt, kv, "BC", MAXU)
     gen = torch.Generator(device="cuda").manual_seed(3)
     e.m._kv.view(e.dt).copy_(torch.randn(e.m._kv.numel() // e.cache.element_size(), generator=gen, device="cuda"))
@@ -609,14 +629,14 @@ def test_prefill(model, engines, fmt, kv):
     sens = {}
     try:
         for utt in (0, MAXU - 1):
-            for i, (S, pos0) in enumerate(PREFILL):
+            for i, (S, pos0) in enumerate(cases):
                 sens_case = sens if (utt == MAXU - 1 and (S, pos0) in ((70, 1000), (129, 0))) else None
                 worst = max(worst, run_prefill(e, utt, S, pos0, 1000 * utt + i, sens_case))
     finally:
         e.before = None
     for name, v in sens.items():
         caught(f"prefill {fmt}/{kv}: {name}", float(torch.cat(v).double().mean()), BOUND_SENS)
-    print(f"prefill {fmt} engine, kv {kv}: {len(PREFILL)} cases x slots 0, {MAXU - 1}: max |err|/bound {worst:.2e}; "
+    print(f"prefill {fmt} engine, kv {kv}, {e.n_sm} SMs: {len(cases)} cases x slots 0, {MAXU - 1}: max |err|/bound {worst:.2e}; "
           f"peak device memory {torch.cuda.max_memory_allocated() / 2 ** 30:.2f} GiB")
 
 

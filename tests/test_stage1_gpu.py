@@ -377,6 +377,12 @@ def test_persistent_kernel_logits_full_bf16_kv_vs_reference_golden(golden_dir, f
     then teacher-forced positions through mvb_s1_step_logits, against the reference's fp32 logits.  A bf16 cache
     cannot meet 1e-3 (SURVEY.md D8): the bound is the reference's OWN bf16-vs-fp32 gap at the same step.
     The bf16 cache's attention runs on mma.sync over TMA-swizzled tiles."""
+    full_bf16_kv_golden(golden_dir, full_arena, attention)
+
+
+def full_bf16_kv_golden(golden_dir, full_arena, attention="mma"):
+    """test_persistent_kernel_logits_full_bf16_kv_vs_reference_golden; the engine plans for the SM count in effect when
+    it is created."""
     g = _golden(golden_dir, "stage1_full")
     m = _mk_full(full_arena, "bf16")
     steps = [int(s) for s in g["steps"]]
