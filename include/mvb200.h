@@ -302,7 +302,10 @@ int mvb_test_set_sm_limit(int32_t n);
  *                       (a, b, sigma, noise scale, clip) = f0 .. f4; 8: d_out [i1] = Box-Muller normals of Philox stream
  *                       i2 under `seed`; 9: d_out [i1] = sum of the i0 blocks at d_out + m i2 floats; 10: d_out [i1] =
  *                       d_a * f0.  The fp64 GroupNorm partials are allocated per call.
- * All three synchronise `stream`. */
+ *   mvb_mbd_unet_test : one UNet evaluation of mvb_mbd_tokens_to_wav on handle h: band model `model`, at the step of
+ *                       schedule row `call`, in that model's workspace block, d_est [n_samples] <- UNet(d_cur [n_samples],
+ *                       step, d_cond [codec_dim, n_frames]); the argument checks of mvb_mbd_tokens_to_wav.
+ * All four synchronise `stream`. */
 int mvb_gemm_test(int32_t epi, const void* d_W, const void* d_W3, int32_t M, int32_t K, const float* d_x, int32_t ldx,
                   int32_t R, const void* d_gain, float eps, int32_t split_lo, int32_t ksplit_override, float* d_out,
                   int32_t ldo, void* d_kcache, void* d_vcache, const int32_t* d_row_cache, const int32_t* d_row_pos,
@@ -361,6 +364,9 @@ int mvb_mbd_conv_test(int32_t kind, const float* d_x, int32_t Cin, int32_t Tin, 
 int mvb_mbd_op_test(int32_t op, const float* d_a, const float* d_b, const float* d_c, const float* d_d, const float* d_e,
                     float* d_out, int32_t i0, int32_t i1, int32_t i2, float f0, float f1, float f2, float f3, float f4,
                     uint64_t seed, void* stream);
+struct mvb_mbd;
+int mvb_mbd_unet_test(struct mvb_mbd* h, int32_t model, int32_t call, const float* d_cur, int32_t n_samples, const float* d_cond,
+                      int32_t n_frames, float* d_est, void* stream);
 /* Test hooks for the EnCodec decoder and audio post-processing kernels (not part of the drop-in surface):
  *   mvb_voc_op_test     : one launch of a csrc/vocoder.cu kernel with a single segment, through the launch helpers of
  *                         mvb_voc_decode and mvb_voc_decode_batch (every kernel serves both).  op 0: k_conv1d<k>, k = 1 / 3 / 7,
@@ -602,7 +608,10 @@ int mvb_mbd_create(const mvb_mbd_config* cfg, const void* d_arena, size_t arena_
 int mvb_mbd_destroy(mvb_mbd* h);
 /* d_cond fp32 [codec_dim, n_frames] (mvb_voc_decode_latent), d_wav_encodec fp32 [n_samples] (mvb_voc_decode),
  * d_noise fp32 [n_models, n_calls, n_samples] standard-normal draws (row 0 = initial sample, row i = the draw added after
- * call i - 1 ... see oracle/mbd_port.py) or NULL for on-device Philox (seed); d_wav_out fp32 [n_samples]. */
+ * call i - 1 ... see oracle/mbd_port.py) or NULL for on-device Philox (seed); d_wav_out fp32 [n_samples].
+ * MVB_ERR_ARG, before anything is enqueued, unless 16 stride <= n_samples <= max_samples and 1 <= n_frames <=
+ * min(max_samples / 320 + 8, 2 Tl): the workspace holds the projected condition for max_samples / 320 + 8 frames, and the
+ * condition may be at most 2x longer than the bottleneck, Tl = n_samples divided depth times by stride, rounded up. */
 int mvb_mbd_tokens_to_wav(mvb_mbd* h, const float* d_cond, int32_t n_frames, const float* d_wav_encodec, int32_t n_samples,
                           const float* d_noise, uint64_t seed, float* d_wav_out, void* stream);
 

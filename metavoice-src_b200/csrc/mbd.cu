@@ -693,7 +693,6 @@ static int unet_forward(mvb_mbd* h, cudaStream_t s, int m, int step, const float
     ConvP p{};
     p.x = d_cond; p.Cin = c.codec_dim; p.Tin = Tf; p.w = h->w(ti); p.bias = h->w(ti + 1); p.y = cemb; p.Cout = Cb; p.Tout = Tf; p.dil = 1; p.pad = 0;
     if (int e = launch_conv(s, p, 1, 1)) return e;
-    if (Tf > 2 * Tl) return mvb::set_error(MVB_ERR_ARG, "mbd: condition is downsampled by >= 2 (%d vs %d)", Tf, Tl);
     MVB_CK(cudaMemcpyAsync(z, x, sizeof(float) * (size_t)Cb * Tl, cudaMemcpyDeviceToDevice, s));
     k_add_interp<<<GRID_STRIDE_CTAS * 2, 256, 0, s>>>(z, Tl, cemb, Tf, Cb);
     MVB_CK(cudaGetLastError());
@@ -756,12 +755,30 @@ static int split_lows(cudaStream_t s, const float* x, int T, int n_bands, const 
   return MVB_OK;
 }
 
+// The shape checks of one UNet call, made before anything is enqueued.  The codec condition is projected into L.cond,
+// which holds max_samples / 320 + 8 frames, and then interpolated onto the bottleneck, which may downsample it at most
+// 2x (the restatement's assert): n_frames <= 2 Tl, Tl = n_samples divided depth times by the stride, rounded up.
+static int mbd_check_shape(const mvb_mbd_config& c, int32_t n_frames, int32_t n_samples) {
+  if (n_samples < 16 * c.stride || n_samples > c.max_samples) return mvb::set_error(MVB_ERR_ARG, "mbd: n_samples %d out of range", n_samples);
+  if (n_frames < 1) return mvb::set_error(MVB_ERR_ARG, "mbd: n_frames %d", n_frames);
+  const int cap = c.max_samples / 320 + 8;
+  if (n_frames > cap)
+    return mvb::set_error(MVB_ERR_ARG, "mbd: n_frames %d exceeds the condition capacity %d (max_samples %d)", n_frames, cap, c.max_samples);
+  int tl = n_samples;
+  for (int i = 0; i < c.depth; ++i) tl = (tl + c.stride - 1) / c.stride;
+  if (n_frames > 2 * tl)
+    return mvb::set_error(MVB_ERR_ARG, "mbd: n_frames %d is more than twice the bottleneck length %d of %d samples", n_frames, tl,
+                          n_samples);
+  return MVB_OK;
+}
+
+// Every shape check (mbd_check_shape: n_samples, and n_frames against the L.cond capacity and the bottleneck) runs before
+// the first copy, launch or stream fork.
 extern "C" int mvb_mbd_tokens_to_wav(mvb_mbd* h, const float* d_cond, int32_t n_frames, const float* d_wav_encodec, int32_t n_samples,
                                      const float* d_noise, uint64_t seed, float* d_wav_out, void* stream) {
   if (!h || !d_cond || !d_wav_encodec || !d_wav_out) return mvb::set_error(MVB_ERR_ARG, "null argument");
   const mvb_mbd_config& c = h->cfg;
-  if (n_samples < 16 * c.stride || n_samples > c.max_samples) return mvb::set_error(MVB_ERR_ARG, "mbd: n_samples %d out of range", n_samples);
-  if (n_frames < 1) return mvb::set_error(MVB_ERR_ARG, "mbd: n_frames");
+  if (int e = mbd_check_shape(c, n_frames, n_samples)) return e;
   cudaStream_t s = (cudaStream_t)stream;
   const MbdWs& L = h->L;
   const int T = n_samples;
@@ -835,6 +852,28 @@ extern "C" int mvb_mbd_tokens_to_wav(mvb_mbd* h, const float* d_cond, int32_t n_
   k_band_mix<<<GRID_STRIDE_CTAS * 2, 256, 0, s>>>(low_w, wav, T, c.eq_bands, stdv + 64, stdv, nullptr, d_wav_out, 0);
   MVB_CK(cudaGetLastError());
   return MVB_OK;
+}
+
+// Test hook: the unet_forward of tokens_to_wav for band model `model` at the step of schedule row `call`, in that model's
+// activation block (block 0 under MVB_MBD_ONE_STREAM), on `stream`: d_est [n_samples] <- UNet(d_cur, step, d_cond).
+// The shape checks of tokens_to_wav.  Synchronises `stream`.
+extern "C" int mvb_mbd_unet_test(mvb_mbd* h, int32_t model, int32_t call, const float* d_cur, int32_t n_samples, const float* d_cond,
+                                 int32_t n_frames, float* d_est, void* stream) {
+  if (!h || !d_cur || !d_cond || !d_est) return mvb::set_error(MVB_ERR_ARG, "null argument");
+  const mvb_mbd_config& c = h->cfg;
+  if (model < 0 || model >= c.n_models || call < 0 || call >= c.n_calls)
+    return mvb::set_error(MVB_ERR_ARG, "mvb_mbd_unet_test: model %d / call %d out of range", model, call);
+  if (int e = mbd_check_shape(c, n_frames, n_samples)) return e;
+  cudaStream_t s = (cudaStream_t)stream;
+  float row[4];
+  MVB_CK(cudaMemcpyAsync(row, h->w(c.n_models * h->per_model + 2) + 4 * (size_t)call, sizeof(row), cudaMemcpyDeviceToHost, s));
+  MVB_CK(cudaStreamSynchronize(s));
+  h->base = h->ws + (h->L.n_blk > 1 ? (size_t)model * h->L.blk : 0);
+  int rc = unet_forward(h, s, model, (int)row[3], d_cur, n_samples, d_cond, n_frames, d_est);
+  h->base = h->ws;
+  const cudaError_t e = cudaStreamSynchronize(s);
+  if (rc == MVB_OK && e != cudaSuccess) rc = mvb::set_error(MVB_ERR_CUDA, "mvb_mbd_unet_test: %s", cudaGetErrorString(e));
+  return rc;
 }
 
 // Test hook: one convolution of the kinds unet_forward runs, outside any mvb_mbd handle, with the taps packed by

@@ -177,6 +177,8 @@ SIGNATURES = {
     "mvb_mbd_op_test": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
                                   C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_uint64,
                                   C.c_void_p]),
+    "mvb_mbd_unet_test": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
+                                    C.c_void_p]),
     "mvb_s2_attn_test": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "mvb_w4_gemv_test": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32,
                                    C.c_void_p, C.c_float, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,

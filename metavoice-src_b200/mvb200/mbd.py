@@ -159,10 +159,25 @@ class MultiBandDiffusionEngine(Engine):
         per += 2.0 * u.codec_dim * ch[-1] * n_frames
         return per * self.s.n_models * (len(self.s.steps()) - 1)
 
+    def check_shape(self, n_frames: int, n_samples: int) -> None:
+        """The library's shape checks of ``tokens_to_wav``, as ValueError before anything reaches the device: n_samples
+        within 16 x stride .. the workspace capacity, and at most the frames the workspace's condition buffer holds
+        (capacity / 320 + 8), and at most twice the UNet bottleneck length."""
+        u, cap = self.s.unet, self.cfg.max_samples
+        if not 16 * u.stride <= n_samples <= cap:
+            raise ValueError(f"mbd: n_samples {n_samples} out of range ({16 * u.stride} .. {cap})")
+        tl = n_samples
+        for _ in range(u.depth):
+            tl = -(-tl // u.stride)
+        limit = min(cap // 320 + 8, 2 * tl)
+        if not 1 <= n_frames <= limit:
+            raise ValueError(f"mbd: n_frames {n_frames} out of range (1 .. {limit} for {n_samples} samples)")
+
     @torch.no_grad()
     def tokens_to_wav(self, cond: torch.Tensor, wav_encodec: torch.Tensor, noise: Optional[torch.Tensor] = None, seed: int = 0) -> torch.Tensor:
         """cond fp32 [codec_dim, T_frames] (``decode_latent``), wav_encodec fp32 [T] (codec decode) -> refined wav fp32 [T].
         ``noise`` [n_models, n_calls, T]: the standard-normal draws of the sampler (parity tests); else on-device Philox."""
+        self.check_shape(cond.shape[1], wav_encodec.numel())
         c = cond.to(self.device, torch.float32).contiguous()
         w = wav_encodec.to(self.device, torch.float32).reshape(-1).contiguous()
         nz = None

@@ -33,7 +33,7 @@ def test_library_exports_every_declared_symbol():
     for name in _declared():
         assert hasattr(lib, name), f"{name} declared in include/mvb200.h but not exported"
     assert set(_declared()) == set(_lib.SIGNATURES), "python binding table out of sync with the header"
-    for hook in ("mvb_gemm_test", "mvb_mbd_conv_test", "mvb_mbd_op_test", "mvb_s2_attn_test", "mvb_s2_sample_test", "mvb_s2_embed_test",
+    for hook in ("mvb_gemm_test", "mvb_mbd_conv_test", "mvb_mbd_op_test", "mvb_mbd_unet_test", "mvb_s2_attn_test", "mvb_s2_sample_test", "mvb_s2_embed_test",
                  "mvb_voc_op_test",
                  "mvb_audio_post_test", "mvb_spk_op_test"):
         assert hook in _lib.SIGNATURES and hasattr(lib, hook), f"test hook {hook} missing"
