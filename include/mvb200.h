@@ -244,6 +244,26 @@ size_t mvb_s1_int8_workspace_bytes(const mvb_s1_config* cfg);
 int mvb_s1_create_int8(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
                        void* d_kv, void* d_workspace, mvb_s1** out);
 
+/* Weight-only fp8 engine (quantisation_mode="fp8"; an extension, the reference has no fp8 mode).  Same offset table and
+ * Linear weights as mvb_s1_create_int8, but each entry points at an FP8 MATRIX [M, K] (M even, K % 256 == 0): the int8
+ * matrix layout -- M * K one-byte codes, then at the next 256-byte boundary bf16 [M] row scales s -- whose codes are
+ * float8 e4m3fn values q in a fragment-native order (produced only by mvb200/quantize.py:pack_fp8_matrix):
+ *   rows [0, M16), M16 = M & ~15, in 16-row blocks b, each block's K in 32-wide chunks c; chunk c of block b is 512 bytes
+ *   at (b * K / 32 + c) * 512, in which lane l = 4 g + t (g = l / 4, t = l % 4) owns bytes [16 l, 16 l + 16): word 2 s + h
+ *   (s, h in {0, 1}) holds the codes of (row g, k0), (row g + 8, k0), (row g, k0 + 1), (row g + 8, k0 + 1), k0 = 16 s +
+ *   8 h + 2 t within the chunk -- the bf16 A fragment of mma.m16n8k16 for k-step s once each pair is widened;
+ *   rows [M16, M) after them, row-major.
+ * Quantiser, per output row j: s_j = bf16(max(amax_j / 448, FLT_EPSILON)), q_jk = e4m3(clamp(w_jk / s_j, -448, 448)) with
+ * round-to-nearest-even; NaN or Inf weights are rejected.  Every kernel computes y_j = s_j * sum_k x_k q_jk: fp32 sums over
+ * the exact e4m3 values, the scale applied once per output after the whole sum.  Decode of 1 to 8 slots runs the
+ * per-layer path through the tensor-core fp8 GEMV, which reads every weight once per step for all of them; prefill and a
+ * decode of more than 8 slots run the tensor-core GEMM over one layer's q at a time, widened to bf16 as the int8 engine
+ * does.  Never the persistent kernel.  mvb_s1_fp8_workspace_bytes = the int8 workspace + dim x spk_dim bf16
+ * (speaker_cond_pos's q, widened once at create).  Every other mvb_s1_* call accepts the handle. */
+size_t mvb_s1_fp8_workspace_bytes(const mvb_s1_config* cfg);
+int mvb_s1_create_fp8(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
+                      void* d_kv, void* d_workspace, mvb_s1** out);
+
 /* Kernel launches issued by this handle since creation (bench.py "gpu_launches"). */
 uint64_t mvb_s1_launch_count(const mvb_s1* h);
 
@@ -340,6 +360,17 @@ int mvb_w8_gemm_test(int32_t epi, const void* d_W, const void* d_W3, const void*
                      const int32_t* d_row_cache, const int32_t* d_row_pos, int32_t H, int32_t S_max, int32_t D,
                      int32_t kv_fp32, void* stream);
 int mvb_w8_widen_test(const void* d_W, int32_t M, int32_t K, void* d_out, void* stream);
+/* Test hooks for the fp8 kernels (not part of the drop-in surface):
+ *   mvb_f8_gemv_test  : the fp8 GEMV (csrc/gemv_f8.cuh k_gemv_f8) as the fp8 engine's decode launches it, for any n_utts
+ *                       in [1, 64] (one launch row per 8); the arguments of mvb_w4_gemv_test with d_W / d_W3 fp8 matrices
+ *                       [M, K], any K % 256 == 0 and an even ldx.
+ *   mvb_f8_widen_test : k_f8_widen of one fp8 matrix into d_out bf16 row-major [M, K] (q exactly).
+ * Both synchronise `stream`. */
+int mvb_f8_gemv_test(int32_t epi, const void* d_W, const void* d_W3, int32_t M, int32_t K, const float* d_x, int32_t ldx,
+                     int32_t n_utts, const void* d_gain, float eps, float* d_out, int32_t ldo, void* d_kcache, void* d_vcache,
+                     const int32_t* d_slot_map, const int32_t* d_pos, int32_t H, int32_t S_max, int32_t D, int32_t kv_fp32,
+                     void* stream);
+int mvb_f8_widen_test(const void* d_W, int32_t M, int32_t K, void* d_out, void* stream);
 /* Test hook for the projections of a non-production stage-1 architecture (not part of the drop-in surface):
  *   path 0: k_gemv as path A launches it, for utterances u in [0, n_utts): rows 2 s, 2 s + 1 (s = d_slot_map[u]) of d_x
  *           fp32 [*, ldx] and d_out [*, ldo]; out = epilogue(f(x) . W^T + bias); norm 0 none, 1 RMSNorm (d_gain, eps),

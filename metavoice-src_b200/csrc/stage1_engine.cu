@@ -13,6 +13,7 @@
 #include "decode_persistent.cuh"
 #include "gemv_w4.cuh"
 #include "gemv_w8.cuh"
+#include "gemv_f8.cuh"
 
 using namespace mvb;
 
@@ -25,9 +26,9 @@ struct WsLayout {
   // path C (persistent decode kernel)
   size_t c_x, c_qkv, c_gu, c_part_o, c_part_ml, c_bar, c_trace, c_stat, c_samp_part, c_samp_best;
   size_t total;
-  // an int4 or int8 engine's workspace continues with the one-layer bf16 weight scratch; an int8 engine's then with
-  // lm_head's widened q
-  size_t layer_scratch, total_int4, w8_head, total_int8;
+  // an int4, int8 or fp8 engine's workspace continues with the one-layer bf16 weight scratch; an int8 or fp8 engine's
+  // then with lm_head's widened q; an fp8 engine's then with speaker_cond_pos's widened q
+  size_t layer_scratch, total_int4, w8_head, total_int8, f8_spk, total_fp8;
 };
 
 constexpr int RB_MAX = 128;        // rows per tensor-core pass: 64-token prefill chunk x 2 CFG rows, or 64 utterances
@@ -41,8 +42,9 @@ static size_t layer_scratch_elems(const mvb_s1_config& c) {
 }
 
 // Storage format of the Linear weights of an engine's arena (include/mvb200.h): bf16 (mvb_s1_create), int4 packed
-// matrices for the five layer matrices (mvb_s1_create_int4), int8 matrices for every Linear (mvb_s1_create_int8).
-enum class WFmt { BF16, INT4, INT8 };
+// matrices for the five layer matrices (mvb_s1_create_int4), int8 matrices for every Linear (mvb_s1_create_int8), fp8
+// matrices for every Linear (mvb_s1_create_fp8).
+enum class WFmt { BF16, INT4, INT8, FP8 };
 
 struct Mk { int M, K; };
 // [M, K] of layer tensor t (1 wqkv, 2 wo, 4 w1, 5 w3, 6 w2; {0, 0} for the norms)
@@ -118,6 +120,8 @@ static WsLayout make_layout(const mvb_s1_config& c) {
   L.total_int4 = ws.end;
   L.w8_head = ws.take((size_t)c.vocab * c.dim * 2);
   L.total_int8 = ws.end;
+  L.f8_spk = ws.take((size_t)c.dim * c.spk_dim * 2);
+  L.total_fp8 = ws.end;
   return L;
 }
 
@@ -164,9 +168,13 @@ struct mvb_s1 {
   // one layer at a time into layer_scratch (bf16 [wqkv | wo | w1 | w3 | w2]).
   // int8 engine: every Linear is an int8 matrix; path A streams them through k_gemv_w8, path B widens one layer's q at a
   // time into layer_scratch (lm_head's once, at create, into w8_head) and k_tc_gemm applies the row scales.
+  // fp8 engine: every Linear is an fp8 matrix; path A streams them through k_gemv_f8 for up to F8_MAX_UTTS slots at once,
+  // path B widens them as the int8 engine does (k_f8_widen), speaker_cond_pos's once at create into f8_spk.
   WFmt fmt = WFmt::BF16;
   __nv_bfloat16* layer_scratch = nullptr;
   __nv_bfloat16* w8_head = nullptr;
+  __nv_bfloat16* f8_spk = nullptr;
+  bool row_scaled() const { return fmt == WFmt::INT8 || fmt == WFmt::FP8; }   // int8 / fp8 matrices with row scales
 
   template <typename T>
   T* wsp(size_t o) const { return reinterpret_cast<T*>(ws + o); }
@@ -183,16 +191,17 @@ struct mvb_s1 {
     return w(MVB_S1_GLOBAL_TENSORS + layer * (g ? 6 : MVB_S1_LAYER_TENSORS) + (g && t == 6 ? 5 : t));
   }
   // The one weight-source accessor of the tensor-core path: the bf16 matrix t (1 wqkv, 2 wo, 4 w1, 5 w3, 6 w2) of a layer,
-  // i.e. the arena tensor, or for an int4 / int8 engine its slot in the layer scratch (k_w4_dequant / k_w8_widen fill it).
+  // i.e. the arena tensor, or for an int4 / int8 / fp8 engine its slot in the layer scratch (k_w4_dequant / k_w8_widen /
+  // k_f8_widen fill it).
   const __nv_bfloat16* tc_w(int layer, int t) const {
     if (fmt == WFmt::BF16) return lw(layer, t);
     const size_t D = cfg.dim, F = cfg.intermediate;
     const size_t at[7] = {0, 0, 3 * D * D, 0, 4 * D * D, 4 * D * D + F * D, 4 * D * D + 2 * F * D};
     return layer_scratch + at[t];
   }
-  // Row scales of the tensor-core path: those of arena tensor i ([M, K]) for an int8 engine, else none.
+  // Row scales of the tensor-core path: those of arena tensor i ([M, K]) for an int8 or fp8 engine, else none.
   const __nv_bfloat16* tc_scale(int i, int M, int K) const {
-    if (fmt != WFmt::INT8) return nullptr;
+    if (!row_scaled()) return nullptr;
     return reinterpret_cast<const __nv_bfloat16*>(arena + off[i] + w8_scale_offset(M, K));
   }
   const __nv_bfloat16* tc_lscale(int layer, int t) const {
@@ -278,6 +287,11 @@ extern "C" size_t mvb_s1_int8_workspace_bytes(const mvb_s1_config* c) {
   return make_layout(*c).total_int8;
 }
 
+extern "C" size_t mvb_s1_fp8_workspace_bytes(const mvb_s1_config* c) {
+  if (validate(c) || quant_staging_ok(c)) return 0;
+  return make_layout(*c).total_fp8;
+}
+
 // Tensors in the offset list: the weights (GELU: six per layer), then, with bias, ln_f.bias (LayerNorm) and per layer
 // {ln_1.bias (LayerNorm), c_attn.bias, attn.c_proj.bias, ln_2.bias (LayerNorm), w1.bias, w3.bias | c_fc.bias,
 // mlp.c_proj.bias}.
@@ -343,24 +357,34 @@ static int create_engine(const mvb_s1_config* cfg, const mvb_s1_arch* arch, cons
   h->fmt = fmt;
   if (fmt != WFmt::BF16) {
     h->layer_scratch = h->wsp<__nv_bfloat16>(h->L.layer_scratch);
-    const bool w8 = fmt == WFmt::INT8;
+    const bool w8 = h->row_scaled();   // int8 and fp8 matrices share one layout (include/mvb200.h)
+    const char* kind = fmt == WFmt::INT8 ? "int8" : fmt == WFmt::FP8 ? "fp8" : "int4 packed";
     for (int l = 0; l < cfg->n_layer; ++l)
       for (int t : {1, 2, 4, 5, 6}) {
         const uint64_t o = h->off[MVB_S1_GLOBAL_TENSORS + l * MVB_S1_LAYER_TENSORS + t];
         const Mk mk = layer_mk(*cfg, t);
         if (o + (w8 ? w8_matrix_bytes(mk.M, mk.K) : w4_packed_bytes(mk.M, mk.K)) > arena_bytes)
-          return set_error(MVB_ERR_ARG, "%s matrix %d of layer %d runs past the end of the arena", w8 ? "int8" : "int4 packed", t, l);
+          return set_error(MVB_ERR_ARG, "%s matrix %d of layer %d runs past the end of the arena", kind, t, l);
       }
     if (w8) {
       if (h->off[2] + w8_matrix_bytes(cfg->dim, cfg->spk_dim) > arena_bytes || h->off[4] + w8_matrix_bytes(cfg->vocab, cfg->dim) > arena_bytes)
-        return set_error(MVB_ERR_ARG, "int8 matrix speaker_cond_pos or lm_head runs past the end of the arena");
-      // lm_head's q, widened once: the head GEMM of every prefill chunk reads it from here
+        return set_error(MVB_ERR_ARG, "%s matrix speaker_cond_pos or lm_head runs past the end of the arena", kind);
+      // lm_head's q, widened once: the head GEMM of every prefill chunk reads it from here; an fp8 engine's
+      // speaker_cond_pos q too, for k_spk_proj
       h->w8_head = h->wsp<__nv_bfloat16>(h->L.w8_head);
       W8Mats m{};
       m.src[0] = reinterpret_cast<const uint8_t*>(h->w(4));
       m.dst[0] = h->w8_head;
       m.M[0] = cfg->vocab; m.K[0] = cfg->dim; m.n = 1;
-      k_w8_widen<<<4 * n_sm, 256>>>(m);
+      if (fmt == WFmt::FP8) {
+        h->f8_spk = h->wsp<__nv_bfloat16>(h->L.f8_spk);
+        m.src[1] = reinterpret_cast<const uint8_t*>(h->w(2));
+        m.dst[1] = h->f8_spk;
+        m.M[1] = cfg->dim; m.K[1] = cfg->spk_dim; m.n = 2;
+        k_f8_widen<<<4 * n_sm, 256>>>(m);
+      } else {
+        k_w8_widen<<<4 * n_sm, 256>>>(m);
+      }
       MVB_CK(cudaGetLastError());
       MVB_CK(cudaStreamSynchronize(0));
     }
@@ -399,7 +423,7 @@ static int create_engine(const mvb_s1_config* cfg, const mvb_s1_arch* arch, cons
       ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 3], h->tc_w(l, h->gelu() ? 4 : 5), F, D, 128);   // GELU: c_fc again
       ok = ok && make_tmap_bf16(&h->tmW[l * 5 + 4], h->tc_w(l, 6), D, F, 128);
     }
-    ok = ok && make_tmap_bf16(&h->tmW[(size_t)cfg->n_layer * 5], fmt == WFmt::INT8 ? h->w8_head : h->w(4), cfg->vocab, D, 128);
+    ok = ok && make_tmap_bf16(&h->tmW[(size_t)cfg->n_layer * 5], h->row_scaled() ? h->w8_head : h->w(4), cfg->vocab, D, 128);
     if (!ok) return set_error(MVB_ERR_CUDA, "cuTensorMapEncodeTiled failed for a weight matrix");
   }
   // The persistent kernel's bf16-cache attention fetches KV tiles through tm_kv as whole 64-position boxes: positions
@@ -416,7 +440,7 @@ static int create_engine(const mvb_s1_config* cfg, const mvb_s1_arch* arch, cons
   {
     // persistent decode kernel: needs a uniform layer stride (true for arenas packed in checkpoint order)
     const int D = cfg->dim, F = cfg->intermediate, V = cfg->vocab;
-    // an int4 or int8 engine, and any architecture but the production one, never uses path C
+    // an int4, int8 or fp8 engine, and any architecture but the production one, never uses path C
     bool ok = cfg->n_layer >= 1 && fmt == WFmt::BF16 && kv_ok && h->production_arch() && default_staging_ok(*cfg);
     const int o0 = MVB_S1_GLOBAL_TENSORS;
     uint64_t stride = cfg->n_layer > 1 ? h->off[o0 + MVB_S1_LAYER_TENSORS] - h->off[o0] : 2 * (uint64_t)(4 * D * D + 3 * D * F + 2 * D);
@@ -474,6 +498,11 @@ extern "C" int mvb_s1_create_int8(const mvb_s1_config* cfg, const void* d_arena,
   return create_engine(cfg, nullptr, d_arena, arena_bytes, offsets, d_kv, d_ws, out, WFmt::INT8);
 }
 
+extern "C" int mvb_s1_create_fp8(const mvb_s1_config* cfg, const void* d_arena, size_t arena_bytes, const uint64_t* offsets,
+                                 void* d_kv, void* d_ws, mvb_s1** out) {
+  return create_engine(cfg, nullptr, d_arena, arena_bytes, offsets, d_kv, d_ws, out, WFmt::FP8);
+}
+
 extern "C" int mvb_s1_destroy(mvb_s1* h) {
   if (!h) return MVB_OK;
   for (auto& kv : h->graphs) cudaGraphExecDestroy(kv.second);
@@ -509,11 +538,25 @@ static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
 
-// p.W / p.W3 are matrices of format `fmt`: bf16 (k_gemv), int4 packed (k_gemv_w4) or int8 (k_gemv_w8); all three take one
-// item per warp.  LAYER (LayerNorm prologue) and BIASED (Linear biases) exist for bf16 only.  A K whose staging rows need
-// more than the default 48 KB of shared memory (a GELU c_proj, K = 4 dim) opts the bf16 instance in first.
+// k_gemv_f8 over batch entries [0, n_utts): one launch row of up to F8_MAX_UTTS slots (gridDim.y > 1 only for a larger
+// batch on an engine without the rows path), one n8 block of MMA columns up to 4 slots, two above.
+template <int EPI>
+static cudaError_t launch_gemv_f8(mvb_s1* h, cudaStream_t s, int n_utts, const GemvP& p) {
+  const dim3 grid(f8_gemv_ctas((p.M + 15) / 16, h->n_sm), (n_utts + F8_MAX_UTTS - 1) / F8_MAX_UTTS);
+  h->launches++;
+  if (n_utts > F8_MAX_UTTS / 2) return launch_pdl(k_gemv_f8<EPI, 2>, grid, dim3(256), 0, s, p, h->st, n_utts);
+  return launch_pdl(k_gemv_f8<EPI, 1>, grid, dim3(256), 0, s, p, h->st, n_utts);
+}
+
+// p.W / p.W3 are matrices of format `fmt`: bf16 (k_gemv), int4 packed (k_gemv_w4), int8 (k_gemv_w8) or fp8 (k_gemv_f8);
+// the first three take one item per warp and one utterance per launch row.  LAYER (LayerNorm prologue) and BIASED (Linear
+// biases) exist for bf16 only.  A K whose staging rows need more than the default 48 KB of shared memory (a GELU c_proj,
+// K = 4 dim) opts the bf16 instance in first.
 template <int EPI, bool LAYER = false, bool BIASED = false>
 static cudaError_t launch_gemv(mvb_s1* h, cudaStream_t s, int n_utts, GemvP p, WFmt fmt) {
+  if constexpr (!LAYER && !BIASED && EPI != EPI_GELU) {
+    if (fmt == WFmt::FP8) return launch_gemv_f8<EPI>(h, s, n_utts, p);
+  }
   const int n_items = (EPI == EPI_SWIGLU) ? p.M : p.M / 2;
   dim3 grid(gemv_grid(n_items, h->n_sm), n_utts);
   const size_t smem = (size_t)2 * p.K * sizeof(float);
@@ -644,7 +687,7 @@ static int launch_body(mvb_s1* h, cudaStream_t s, int n_utts) {
   GemvP p{};
   p.eps = c.norm_eps;
   p.W = h->w(4); p.x = x; p.ldx = D; p.gain = h->w(3); p.out = logits; p.ldo = V; p.M = V; p.K = D;
-  MVB_CK(launch_gemv<EPI_STORE>(h, s, n_utts, p, h->fmt == WFmt::INT8 ? WFmt::INT8 : WFmt::BF16));   // int4: lm_head is bf16
+  MVB_CK(launch_gemv<EPI_STORE>(h, s, n_utts, p, h->fmt == WFmt::INT4 ? WFmt::BF16 : h->fmt));   // int4: lm_head is bf16
   return MVB_OK;
 }
 
@@ -668,7 +711,7 @@ struct LinB {
   int widx, widx3;                                     // tensor-map indices of W (and W3 for SwiGLU)
   int M, K;
   float* out; int ldo;
-  const __nv_bfloat16* scale = nullptr;                // int8 engine: row scales of W (and W3)
+  const __nv_bfloat16* scale = nullptr;                // int8 / fp8 engine: row scales of W (and W3)
   const __nv_bfloat16* scale3 = nullptr;
   const __nv_bfloat16* beta = nullptr;                 // LayerNorm with bias: the norm's beta
   const __nv_bfloat16* bias = nullptr;                 // Linear biases of W (and W3)
@@ -761,7 +804,7 @@ static int launch_layers_b(mvb_s1* h, cudaStream_t s, int R) {
   for (int l = 0; l < c.n_layer; ++l) {
     char* kc = h->kv + (size_t)l * 2 * half;
     char* vc = kc + half;
-    if (h->fmt != WFmt::BF16) {   // this layer's W_deq (int4) or q (int8) -> the scratch the tensor maps of every layer point at
+    if (h->fmt != WFmt::BF16) {   // this layer's W_deq (int4) or q (int8, fp8) -> the scratch the tensor maps of every layer point at
       W4Mats m{};   // == W8Mats
       const int ts[5] = {1, 2, 4, 5, 6};
       for (int i = 0; i < 5; ++i) {
@@ -773,6 +816,8 @@ static int launch_layers_b(mvb_s1* h, cudaStream_t s, int R) {
       m.n = 5;
       if (h->fmt == WFmt::INT4) {
         k_w4_dequant<<<4 * h->n_sm, 256, 0, s>>>(m);
+      } else if (h->fmt == WFmt::FP8) {
+        k_f8_widen<<<4 * h->n_sm, 256, 0, s>>>(m);
       } else {
         k_w8_widen<<<4 * h->n_sm, 256, 0, s>>>(m);
       }
@@ -886,8 +931,11 @@ static bool use_path_c(const mvb_s1* h, int n_utts) {
 static int run_body(mvb_s1* h, cudaStream_t s, int n_utts, bool allow_b = true) {
   // Path A (CUDA-core GEMV) streams the weights once per utterance; from 2 utterances up the tensor-core
   // rows path streams them once per step for the whole batch.  slot_map must be the identity for path B
-  // (its logits rows are batch-ordered), which mvb_s1_decode guarantees.
-  const bool use_b = allow_b && h->path_b && h->fmt == WFmt::BF16 && n_utts >= 2;   // int4 / int8 decode: always path A
+  // (its logits rows are batch-ordered), which mvb_s1_decode guarantees.  int4 / int8 decode: always path A.  fp8
+  // decode: path A, whose k_gemv_f8 reads the weights once per step for up to F8_MAX_UTTS slots; a larger batch takes
+  // path B, since one k_gemv_f8 launch row holds at most F8_MAX_UTTS slots (two n8 MMA blocks).
+  const bool use_b = allow_b && h->path_b &&
+                     ((h->fmt == WFmt::BF16 && n_utts >= 2) || (h->fmt == WFmt::FP8 && n_utts > F8_MAX_UTTS));
   auto body = [&](cudaStream_t st) { return use_b ? launch_body_b(h, st, n_utts) : launch_body(h, st, n_utts); };
   const int key = n_utts + (use_b ? 1000 : 0);
   auto it = h->graphs.find(key);
@@ -927,7 +975,10 @@ extern "C" int mvb_s1_set_speaker(mvb_s1* h, int32_t utt, const float* d_spk, vo
   cudaStream_t s = (cudaStream_t)stream;
   const int D = h->cfg.dim;
   float* out = h->wsp<float>(h->L.spk) + (size_t)utt * D;
-  if (h->fmt == WFmt::INT8)
+  if (h->fmt == WFmt::FP8)
+    k_spk_proj<__nv_bfloat16><<<(D * 32 + 255) / 256, 256, 0, s>>>(h->f8_spk, d_spk, out, D, h->cfg.spk_dim,
+                                                                    h->tc_scale(2, D, h->cfg.spk_dim));
+  else if (h->fmt == WFmt::INT8)
     k_spk_proj<int8_t><<<(D * 32 + 255) / 256, 256, 0, s>>>(reinterpret_cast<const int8_t*>(h->w(2)), d_spk, out, D, h->cfg.spk_dim,
                                                             h->tc_scale(2, D, h->cfg.spk_dim));
   else
@@ -1425,8 +1476,9 @@ extern "C" int mvb_s1_generate(mvb_s1* h, int32_t n_utts, const int32_t* prompts
 }
 
 // ------------------------------------------------------------------------------------------------
-// Test hooks of the int4 and int8 kernels (include/mvb200.h): k_gemv_w4<epi> / k_gemv_w8<epi> exactly as path A launches
-// them, over a caller-built decode state (slot map and positions), k_w4_dequant / k_w8_widen on one matrix.
+// Test hooks of the int4, int8 and fp8 kernels (include/mvb200.h): k_gemv_w4<epi> / k_gemv_w8<epi> / k_gemv_f8<epi>
+// exactly as path A launches them, over a caller-built decode state (slot map and positions), k_w4_dequant / k_w8_widen /
+// k_f8_widen on one matrix.
 static int quant_gemv_test(WFmt fmt, int32_t epi, const void* d_W, const void* d_W3, int32_t M, int32_t K, const float* d_x,
                            int32_t ldx, int32_t n_utts, const void* d_gain, float eps, float* d_out, int32_t ldo,
                            void* d_kcache, void* d_vcache, const int32_t* d_slot_map, const int32_t* d_pos, int32_t H,
@@ -1434,7 +1486,9 @@ static int quant_gemv_test(WFmt fmt, int32_t epi, const void* d_W, const void* d
   if (!d_W || !d_x || !d_out || !d_slot_map || !d_pos) return set_error(MVB_ERR_ARG, "null argument");
   if (epi < EPI_STORE || epi > EPI_QKV) return set_error(MVB_ERR_ARG, "bad epilogue %d", epi);
   if (K < 256 || K % 256 || M < 2 || M % 2 || n_utts < 1 || n_utts > 64) return set_error(MVB_ERR_ARG, "bad shape M=%d K=%d n_utts=%d", M, K, n_utts);
-  if ((size_t)2 * K * sizeof(float) > 48 * 1024) return set_error(MVB_ERR_UNSUPPORTED, "K=%d exceeds the staging buffer", K);
+  if (fmt != WFmt::FP8 && (size_t)2 * K * sizeof(float) > 48 * 1024)
+    return set_error(MVB_ERR_UNSUPPORTED, "K=%d exceeds the staging buffer", K);
+  if (fmt == WFmt::FP8 && ldx % 2) return set_error(MVB_ERR_ARG, "ldx=%d must be even", ldx);
   if (epi == EPI_SWIGLU && !d_W3) return set_error(MVB_ERR_ARG, "SwiGLU needs W3");
   if (epi == EPI_QKV && (!d_kcache || !d_vcache || M != 3 * D || D != 128 * H)) return set_error(MVB_ERR_ARG, "bad QKV arguments");
   mvb_s1 h{};
@@ -1474,6 +1528,14 @@ extern "C" int mvb_w8_gemv_test(int32_t epi, const void* d_W, const void* d_W3, 
                          d_slot_map, d_pos, H, S_max, D, kv_fp32, stream);
 }
 
+extern "C" int mvb_f8_gemv_test(int32_t epi, const void* d_W, const void* d_W3, int32_t M, int32_t K, const float* d_x,
+                                int32_t ldx, int32_t n_utts, const void* d_gain, float eps, float* d_out, int32_t ldo,
+                                void* d_kcache, void* d_vcache, const int32_t* d_slot_map, const int32_t* d_pos, int32_t H,
+                                int32_t S_max, int32_t D, int32_t kv_fp32, void* stream) {
+  return quant_gemv_test(WFmt::FP8, epi, d_W, d_W3, M, K, d_x, ldx, n_utts, d_gain, eps, d_out, ldo, d_kcache, d_vcache,
+                         d_slot_map, d_pos, H, S_max, D, kv_fp32, stream);
+}
+
 extern "C" int mvb_w4_dequant_test(const void* d_W, int32_t M, int32_t K, void* d_out, void* stream) {
   if (!d_W || !d_out) return set_error(MVB_ERR_ARG, "null argument");
   if (M < 1 || K < 256 || K % 256) return set_error(MVB_ERR_ARG, "bad shape M=%d K=%d", M, K);
@@ -1501,6 +1563,22 @@ extern "C" int mvb_w8_widen_test(const void* d_W, int32_t M, int32_t K, void* d_
   if (int e = current_device(&dev, &n_sm)) return e;
   cudaStream_t s = (cudaStream_t)stream;
   k_w8_widen<<<4 * n_sm, 256, 0, s>>>(m);
+  MVB_CK(cudaGetLastError());
+  MVB_CK(cudaStreamSynchronize(s));
+  return MVB_OK;
+}
+
+extern "C" int mvb_f8_widen_test(const void* d_W, int32_t M, int32_t K, void* d_out, void* stream) {
+  if (!d_W || !d_out) return set_error(MVB_ERR_ARG, "null argument");
+  if (M < 2 || M % 2 || K < 256 || K % 256) return set_error(MVB_ERR_ARG, "bad shape M=%d K=%d", M, K);
+  W4Mats m{};
+  m.src[0] = reinterpret_cast<const uint8_t*>(d_W);
+  m.dst[0] = reinterpret_cast<__nv_bfloat16*>(d_out);
+  m.M[0] = M; m.K[0] = K; m.n = 1;
+  int dev = 0, n_sm = 0;
+  if (int e = current_device(&dev, &n_sm)) return e;
+  cudaStream_t s = (cudaStream_t)stream;
+  k_f8_widen<<<4 * n_sm, 256, 0, s>>>(m);
   MVB_CK(cudaGetLastError());
   MVB_CK(cudaStreamSynchronize(s));
   return MVB_OK;

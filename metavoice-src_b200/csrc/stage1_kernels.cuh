@@ -44,7 +44,8 @@ struct S1State {
 
 // ---------------------------------------------------------------------------------------------
 // spk_proj[u] = W_spk . spk_emb   (fast_model.py:155 speaker_cond_pos, hoisted out of the step).  TW = __nv_bfloat16, or
-// int8_t for an int8 engine, whose bf16 row scales (`scale`) multiply each output once after the sum.
+// int8_t for an int8 engine.  bf16 row scales (`scale`: an int8 engine's, or an fp8 engine's over its widened q) multiply
+// each output once after the sum; a bf16 engine passes none.
 __device__ __forceinline__ float w_to_f32(__nv_bfloat16 w) { return bf16_to_f32(w); }
 __device__ __forceinline__ float w_to_f32(int8_t w) { return (float)w; }
 
@@ -56,7 +57,7 @@ __global__ void __launch_bounds__(256) k_spk_proj(const TW* __restrict__ W, cons
   float acc = 0.f;
   for (int k = lane; k < SD; k += 32) acc = fmaf(w_to_f32(W[(size_t)warp * SD + k]), spk[k], acc);
   acc = warp_sum(acc);
-  if constexpr (!std::is_same<TW, __nv_bfloat16>::value) acc *= bf16_to_f32(scale[warp]);
+  if (scale != nullptr) acc *= bf16_to_f32(scale[warp]);
   if (lane == 0) out[warp] = acc;
 }
 

@@ -111,6 +111,9 @@ SIGNATURES = {
     "mvb_s1_int8_workspace_bytes": (C.c_size_t, [C.POINTER(S1Config)]),
     "mvb_s1_create_int8": (C.c_int, [C.POINTER(S1Config), C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64), C.c_void_p,
                                      C.c_void_p, C.POINTER(C.c_void_p)]),
+    "mvb_s1_fp8_workspace_bytes": (C.c_size_t, [C.POINTER(S1Config)]),
+    "mvb_s1_create_fp8": (C.c_int, [C.POINTER(S1Config), C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64), C.c_void_p,
+                                    C.c_void_p, C.POINTER(C.c_void_p)]),
     "mvb_s2_workspace_bytes": (C.c_size_t, [C.POINTER(S2Config)]),
     "mvb_s2_create": (C.c_int, [C.POINTER(S2Config), C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64), C.c_void_p,
                                 C.POINTER(C.c_void_p)]),
@@ -192,6 +195,10 @@ SIGNATURES = {
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                    C.c_void_p]),
     "mvb_w8_widen_test": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "mvb_f8_gemv_test": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32,
+                                   C.c_void_p, C.c_float, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                   C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
+    "mvb_f8_widen_test": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "mvb_s1_arch_gemv_test": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                         C.c_float, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

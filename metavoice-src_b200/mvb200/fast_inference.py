@@ -68,7 +68,7 @@ class TTS:
     END_OF_AUDIO_TOKEN = 1024
 
     def __init__(self, model_name: str = "metavoiceio/metavoice-1B-v0.1", *, seed: int = 1337, output_dir: str = "outputs",
-                 quantisation_mode: Optional[Literal["int4", "int8"]] = None, first_stage_path: Optional[str] = None,
+                 quantisation_mode: Optional[Literal["int4", "int8", "fp8"]] = None, first_stage_path: Optional[str] = None,
                  telemetry_origin: Optional[str] = None, encodec_state_dict=None, device: str = "cuda", max_utts: int = 1,
                  mbd_checkpoint: Optional[dict] = None, mbd_settings=None):
         self._device = device

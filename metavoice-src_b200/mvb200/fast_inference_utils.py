@@ -311,10 +311,11 @@ def stage1_arch(model_args: dict, state_dict: Dict[str, torch.Tensor]) -> Tuple[
 
 def _load_model(checkpoint_path, spk_emb_ckpt_path, device, precision, quantisation_mode=None, n_head: int = None):
     if quantisation_mode is not None:
-        if quantisation_mode not in ("int4", "int8"):
-            raise Exception(f"Invalid quantisation mode {quantisation_mode}! Must be either 'int4' or 'int8'!")
-        if quantisation_mode == "int8" and torch.device(device).type != "cuda":
-            raise NotImplementedError("int8 weight-only quantisation runs on the CUDA engine only; there is no CPU engine")
+        if quantisation_mode not in ("int4", "int8", "fp8"):
+            raise Exception(f"Invalid quantisation mode {quantisation_mode}! Must be one of 'int4', 'int8' or 'fp8'!")
+        if quantisation_mode in ("int8", "fp8") and torch.device(device).type != "cuda":
+            raise NotImplementedError(f"{quantisation_mode} weight-only quantisation runs on the CUDA engine only; there is no "
+                                      "CPU engine")
     checkpoint = torch.load(str(checkpoint_path), mmap=True, weights_only=False)
     sd = checkpoint["model"]
     args = checkpoint.get("model_args", {})

@@ -118,8 +118,9 @@ class Transformer(Engine):
 
     def __init__(self, config: ModelArgs, arena: torch.Tensor, offsets: List[int], device="cuda",
                  quantisation_mode: Optional[str] = None):
-        if quantisation_mode not in (None, "int4", "int8"):
-            raise NotImplementedError(f"quantisation_mode={quantisation_mode!r} is not implemented (only None, 'int4' and 'int8')")
+        if quantisation_mode not in (None, "int4", "int8", "fp8"):
+            raise NotImplementedError(f"quantisation_mode={quantisation_mode!r} is not implemented (only None, 'int4', 'int8' "
+                                      "and 'fp8')")
         if quantisation_mode is not None and not config.production_arch:
             raise NotImplementedError(f"quantisation_mode={quantisation_mode!r} is implemented for the production architecture "
                                       "(rmsnorm, swiglu, no bias) only")
@@ -143,6 +144,9 @@ class Transformer(Engine):
         engine: decode streams the packed weights through k_gemv_w4, prefill dequantises one layer at a time.
         ``quantisation_mode="int8"`` quantises every Linear per output channel at load and builds an int8 engine: decode
         streams the int8 weights through k_gemv_w8, prefill widens one layer's q at a time and scales the GEMM outputs.
+        ``quantisation_mode="fp8"`` quantises every Linear to e4m3 per output channel at load and builds an fp8 engine:
+        decode of up to 8 utterances reads the weights once per step for all of them through k_gemv_f8, prefill (and a
+        larger decode batch) widens one layer's q at a time as int8 does.
         ``config``'s norm_type / nonlinearity_type / bias select the architecture (mvb_s1_create_ex); only the production
         one takes a quantisation mode."""
         if quantisation_mode is not None and not config.production_arch:
@@ -154,10 +158,14 @@ class Transformer(Engine):
         elif quantisation_mode == "int8":
             from .quantize import pack_arena_int8
             arena, offsets, _ = pack_arena_int8(state_dict, config.n_layer)
+        elif quantisation_mode == "fp8":
+            from .quantize import pack_arena_fp8
+            arena, offsets, _ = pack_arena_fp8(state_dict, config.n_layer)
         elif quantisation_mode is None:
             arena, offsets = pack_arena(state_dict, config.n_layer, config)
         else:
-            raise NotImplementedError(f"quantisation_mode={quantisation_mode!r} is not implemented (only None, 'int4' and 'int8')")
+            raise NotImplementedError(f"quantisation_mode={quantisation_mode!r} is not implemented (only None, 'int4', 'int8' "
+                                      "and 'fp8')")
         return cls(config, arena, offsets, device, quantisation_mode)
 
     @staticmethod
@@ -194,7 +202,7 @@ class Transformer(Engine):
         the bytes its arena's tensors occupy, so that main()'s bandwidth figure counts the bytes actually read."""
         if self.quantisation_mode == "int4":
             return self.int4_model_size_bytes(self.config)
-        if self.quantisation_mode == "int8":
+        if self.quantisation_mode in ("int8", "fp8"):   # one byte per weight plus one bf16 scale per row, either way
             return self.int8_model_size_bytes(self.config)
         return self.bf16_model_size_bytes(self.config)
 
@@ -236,7 +244,8 @@ class Transformer(Engine):
         self._cfg = cfg
         workspace_bytes, create = {None: (self._lib.mvb_s1_workspace_bytes, self._lib.mvb_s1_create),
                                    "int4": (self._lib.mvb_s1_int4_workspace_bytes, self._lib.mvb_s1_create_int4),
-                                   "int8": (self._lib.mvb_s1_int8_workspace_bytes, self._lib.mvb_s1_create_int8)}[self.quantisation_mode]
+                                   "int8": (self._lib.mvb_s1_int8_workspace_bytes, self._lib.mvb_s1_create_int8),
+                                   "fp8": (self._lib.mvb_s1_fp8_workspace_bytes, self._lib.mvb_s1_create_fp8)}[self.quantisation_mode]
         if not c.production_arch:
             self._arch = _lib.S1Arch(_NORMS[c.norm_type], _MLPS[c.nonlinearity_type], int(c.bias))
             create = lambda cfg_p, *rest: self._lib.mvb_s1_create_ex(cfg_p, C.byref(self._arch), *rest)   # noqa: E731

@@ -35,6 +35,20 @@ int8 semantics, defined once here and in include/mvb200.h ("int8 matrix"):
   with fp32 accumulation over the exact integer weights and the scale applied once per output after the whole sum.
 * Consequence.  Where every scale is a power of two, ``s q`` is exact in bf16 and an int8 engine computes the same function
   as a bf16 engine whose arena holds ``W' = s q`` (``int8_dequantized_state_dict``).
+
+fp8 semantics (``quantisation_mode="fp8"``, an extension: the reference has no fp8 mode), defined once here and in
+include/mvb200.h ("fp8 matrix"):
+
+* Which tensors.  Those int8 quantises: every ``nn.Linear``.
+* Quantiser, per output row j of ``w = fp32(bf16 weight)``: ``s_j = bf16(max(amax_j / 448, FLT_EPSILON))`` and
+  ``q_jk = float8_e4m3fn(clamp(w_jk / fp32(s_j), -448, 448))`` (round to nearest even).  Dividing by the rounded scale
+  keeps q consistent with the scale stored; the clamp is needed because torch's cast does not saturate (500 -> NaN) and a
+  scale rounded down can put |w / s| above 448.  NaN or Inf weights are rejected.
+* Function.  ``y_j = s_j sum_k x_k q_jk``: fp32 sums over the exact e4m3 values, the scale applied once per output.
+* Layout.  The int8 matrix layout with the codes in a fragment-native order (``pack_fp8_matrix``), so that the decode GEMV
+  loads each lane's tensor-core operand with one 128-bit load.
+* Consequence.  Where every scale is a power of two, ``s q`` is exact in bf16 and an fp8 engine computes the same function
+  as a bf16 engine whose arena holds ``W' = s q`` (``fp8_dequantized_state_dict``).
 """
 from __future__ import annotations
 
@@ -278,4 +292,101 @@ def int8_dequantized_state_dict(state_dict: Dict[str, torch.Tensor], n_layer: in
     for k, linear, _ in _keys(n_layer):
         if linear:
             out[k] = dequantize_int8(*quantize_per_channel(sd[k]))
+    return out
+
+
+# ---- weight-only fp8 (e4m3) -------------------------------------------------------------------------------------------
+E4M3_MAX = 448.0
+
+
+def quantize_fp8_per_channel(w: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """w [M, K] -> (q float8_e4m3fn [M, K], s bf16 [M]): s = bf16(max(amax / 448, FLT_EPSILON)) per row, q =
+    e4m3(clamp(w / s, -448, 448))."""
+    wf = w.detach().to("cpu", torch.bfloat16).float()
+    if not torch.isfinite(wf).all():
+        raise ValueError("cannot quantise a weight holding NaN or Inf")
+    amax = wf.abs().amax(dim=1)
+    s = torch.clamp(amax / E4M3_MAX, min=_FLT_EPS).to(torch.bfloat16)
+    q = torch.clamp(wf / s.float()[:, None], -E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn)
+    return q, s
+
+
+def dequantize_fp8(q: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
+    """W' = bf16_rn(s q), bf16 [M, K] (s q is exact in fp32: 8 + 4 significant bits)."""
+    return (q.float() * s.float()[:, None]).to(torch.bfloat16)
+
+
+# Fragment-native order of the codes of a 16-row block (include/mvb200.h, "fp8 matrix"): the block [16, K] viewed as
+# (row >> 3, row & 7, k >> 5, k >> 4 & 1, k >> 3 & 1, k >> 1 & 3, k & 1) -> (chunk, lane = (row & 7, k >> 1 & 3),
+# word = (k >> 4 & 1, k >> 3 & 1), byte = (k & 1, row >> 3)).
+_F8_PERM = (0, 3, 2, 6, 4, 5, 7, 1)
+_F8_UNPERM = (0, 7, 2, 1, 4, 5, 3, 6)
+
+
+def pack_fp8_codes(q: torch.Tensor) -> torch.Tensor:
+    """q float8_e4m3fn [M, K] -> uint8 [M * K]: rows [0, M & ~15) in the fragment-native order, the rest row-major."""
+    M, K = q.shape
+    if M % 2 or K % 256:
+        raise ValueError(f"an fp8 matrix needs an even M and K % 256 == 0 (got {M} x {K})")
+    u = q.contiguous().view(torch.uint8)
+    M16 = M // 16 * 16
+    blocks = u[:M16].reshape(M16 // 16, 2, 8, K // 32, 2, 2, 4, 2).permute(*_F8_PERM).reshape(-1)
+    return torch.cat([blocks, u[M16:].reshape(-1)])
+
+
+def unpack_fp8_codes(codes: torch.Tensor, M: int, K: int) -> torch.Tensor:
+    """Inverse of pack_fp8_codes: uint8 [M * K] -> float8_e4m3fn [M, K]."""
+    M16 = M // 16 * 16
+    blocks = codes[:M16 * K].reshape(M16 // 16, K // 32, 8, 4, 2, 2, 2, 2).permute(*_F8_UNPERM).reshape(M16, K)
+    return torch.cat([blocks, codes[M16 * K:M * K].reshape(M - M16, K)]).contiguous().view(torch.float8_e4m3fn)
+
+
+def pack_fp8_matrix(q: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
+    """The fp8 matrix of include/mvb200.h: the codes of pack_fp8_codes, then at the next 256-byte boundary bf16 [M]
+    scales (the int8 matrix layout, int8_matrix_bytes(M, K) bytes)."""
+    M, K = q.shape
+    buf = torch.zeros(int8_matrix_bytes(M, K), dtype=torch.uint8)
+    buf[:M * K] = pack_fp8_codes(q)
+    so = align_up(M * K)
+    buf[so:] = s.contiguous().view(torch.uint8)
+    return buf
+
+
+def unpack_fp8_matrix(buf: torch.Tensor, M: int, K: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Inverse of pack_fp8_matrix: (q, s)."""
+    so = align_up(M * K)
+    return unpack_fp8_codes(buf[:M * K], M, K), buf[so:so + 2 * M].clone().view(torch.bfloat16)
+
+
+def pack_arena_fp8(state_dict: Dict[str, torch.Tensor], n_layer: int):
+    """Checkpoint state dict -> (uint8 arena, byte offsets, payload bytes).  Every Linear weight is an fp8 matrix (its
+    offset points at the code block); embeddings and norms are the bf16 tensors.  The payload counts one byte per weight,
+    the bf16 scales and the bf16 tensors, as for int8."""
+    sd = _strip(state_dict)
+    blobs: List[torch.Tensor] = []
+    payload = 0
+    for k, linear, _ in _keys(n_layer):
+        if k not in sd:
+            raise KeyError(f"checkpoint is missing {k}")
+        t = sd[k].detach()
+        if linear:
+            q, s = quantize_fp8_per_channel(t)
+            blobs.append(pack_fp8_matrix(q, s))
+            payload += q.numel() + 2 * s.numel()
+        else:
+            t = t.to(torch.bfloat16)
+            blobs.append(t)
+            payload += t.numel() * 2
+    arena, offsets = pack_arena_bytes(blobs)
+    return arena, offsets, payload
+
+
+def fp8_dequantized_state_dict(state_dict: Dict[str, torch.Tensor], n_layer: int) -> Dict[str, torch.Tensor]:
+    """The checkpoint with every Linear replaced by bf16_rn(s q): the bf16 model an fp8 engine equals when every scale is
+    a power of two (and approximates to the rounding of s q otherwise)."""
+    sd = _strip(state_dict)
+    out = dict(sd)
+    for k, linear, _ in _keys(n_layer):
+        if linear:
+            out[k] = dequantize_fp8(*quantize_fp8_per_channel(sd[k]))
     return out
