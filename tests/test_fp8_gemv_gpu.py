@@ -14,7 +14,11 @@ reference's to rsqrtf's error, 2^-21 relative) and the fp32 gain product rounds 
 
 Sensitivity.  References built with each row's scale taken from its neighbour, with the subnormal codes flushed to zero,
 and with the two CFG rows of a slot swapped must violate the bound.  Batch independence: every slot's outputs at 8 slots
-are bit-identical to the same slot run alone."""
+are bit-identical to the same slot run alone.
+
+SM counts.  The grid (f8_gemv_ctas) depends on the SM count: the float64 cases rerun with the grid planned for 114, 78,
+60, 54 and 16 SMs, where CTAs own 2 or 3 of wo's and w2's 16-row blocks and lm_head's ragged tail block is a CTA's third
+from 80 SMs down (a Python mirror of the deal asserts which)."""
 import ctypes as C
 import functools
 
@@ -183,6 +187,44 @@ def test_gemv_f8(epi, M, K, n_utts):
             for r in (2 * s, 2 * s + 1):
                 assert torch.equal(kc[r, :, p].view(view), out[r, D:2 * D].reshape(H, 128).to(dt).view(view)), "K cache"
                 assert torch.equal(vc[r, :, p].view(view), out[r, 2 * D:3 * D].reshape(H, 128).to(dt).view(view)), "V cache"
+
+
+def f8_gemv_ctas(n_blocks, n_sm, ipc=3):
+    """Mirror of f8_gemv_ctas (csrc/gemv_f8.cuh): one 16-row block per SM where there are enough, never more than F8_IPC
+    = 3 per CTA."""
+    return max(-(-n_blocks // ipc), min(n_blocks, n_sm))
+
+
+def n_mine(n_blocks, n_sm):
+    """Blocks CTA x owns (x, x + G, x + 2 G, ...) for every CTA of the launch, as k_gemv_f8 deals them."""
+    G = f8_gemv_ctas(n_blocks, n_sm)
+    return [(n_blocks - 1 - x) // G + 1 for x in range(G)]
+
+
+# the capped counts of tests/test_sm_count_gpu.py that change k_gemv_f8's grid at production width: at 132 SMs wo / w2
+# (128 blocks) give every CTA one block and lm_head's ragged tail (block 160) is its CTA's second
+F8_SM = [114, 78, 60, 54, 16]
+
+
+@pytest.mark.parametrize("G", F8_SM)
+def test_gemv_f8_at_sm_counts(G):
+    """test_gemv_f8's float64 cases (every production matrix and epilogue, NB = 1 and 2) with the grid planned for G SMs
+    (mvb_test_set_sm_limit): wo / w2 at 2 or 3 blocks per CTA, and lm_head's tail block as a CTA's third (i = 2) from
+    G = 78 down."""
+    from test_sm_count_gpu import sm_limit
+    with sm_limit(G) as g:
+        if g != G:
+            pytest.skip(f"this device has fewer than {G} SMs")
+        blocks = n_mine(2048 // 16, G)
+        assert max(blocks) in (2, 3), (G, sorted(set(blocks)))
+        tail_cta_ctas = f8_gemv_ctas(-(-2562 // 16), G)
+        tail_i = 160 // tail_cta_ctas
+        assert tail_i == (2 if G <= 80 else 1), (G, tail_i)
+        print(f"G={G}: wo / w2 blocks per CTA {sorted(set(blocks))} on {len(blocks)} CTAs; lm_head tail block is "
+              f"i = {tail_i} of CTA {160 % tail_cta_ctas} of {tail_cta_ctas}")
+        for epi, M, K in CASES:
+            for n in (1, 5, 8):
+                test_gemv_f8(epi, M, K, n)
 
 
 @pytest.mark.parametrize("epi,M,K", CASES)

@@ -7,9 +7,13 @@ this device's own count.  The limit is set only inside `sm_limit` and always cle
   path choice  1-layer production-width and tiny engines, every G, n_utts 1 .. 8, fp32 / bf16 KV, block_size 256 /
                2048: the body mvb_s1_decode runs (from the launch count) equals the mirror of test_sm_count_cpu.py
                (pc_ok, pc_att_fits, the owner guard 2 n_utts - 1 <= G, the fused-sampler condition).
-  path A       k_gemv (bf16, and the LayerNorm architecture), k_gemv_w8, k_gemv_w4: decode logits bit-identical to the
-               uncapped engine.  A warp's products and their order depend only on its item, not on how many warps the
-               grid has (gemv_grid only changes how many items a warp takes).
+  path A       k_gemv (bf16, and the LayerNorm architecture), k_gemv_w8, k_gemv_w4, k_gemv_f8: decode logits
+               bit-identical to the uncapped engine.  A warp's products and their order depend only on its item, not on
+               how many warps the grid has (gemv_grid only changes how many items a warp takes); a k_gemv_f8 block's sum
+               does not depend on which CTA owns it (f8_gemv_ctas only changes how many blocks a CTA takes);
+  fp8          test_fp8_gemv_gpu.py's float64 GEMV cases at G = 114, 78, 60, 54, 16, where a CTA owns 2 or 3 of wo's and
+               w2's 16-row blocks and (from G = 80 down) lm_head's ragged tail block is a CTA's third (a mirror of
+               f8_gemv_ctas); fp8 decode takes the widened rows path only above 8 slots, at every G;
   path C / B   the projection probes of test_decode_linear_ops_gpu.py (every phase at l* = 0, 12, 23, fp32 and bf16
                forms of the persistent kernel at every G for the batches path C takes there; path B's tensor-core rows
                path at G = 114, 60, 16) with that module's float64 references and bounds, the K splits from the
@@ -151,7 +155,8 @@ def test_path_choice_tiny_model():
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-PATH_A = {"bf16": dict(), "layernorm": dict(norm="layernorm"), "int8": dict(mode="int8"), "int4": dict(mode="int4")}
+PATH_A = {"bf16": dict(), "layernorm": dict(norm="layernorm"), "int8": dict(mode="int8"), "int4": dict(mode="int4"),
+          "fp8": dict(mode="fp8")}
 
 
 @pytest.mark.parametrize("fmt", list(PATH_A))
@@ -188,6 +193,28 @@ def test_path_a_bit_identical(fmt):
         for r, got in zip(ref, logits(G)):
             assert torch.equal(r.view(torch.int32), got.view(torch.int32)), f"{fmt}: G={G} differs from the uncapped engine"
     print(f"path A {fmt}: logits at G = {counts(SM_COUNTS)} bit-identical to the uncapped engine")
+
+
+def test_fp8_rows_path_only_above_8_slots():
+    """A 1-layer production-width fp8 engine with the rows path enabled decodes 1 .. 8 slots on path A (one k_gemv_f8
+    launch row) and 9 .. 12 on path B (which widens the layer first: one launch more than bf16's path B), at every G."""
+    from mvb200 import _lib
+    sd = _state_dict(FULL)
+    want = {"A": DECODE_LAUNCHES["A"], "B": DECODE_LAUNCHES["B"] + 1}
+    for G in counts(SM_COUNTS):
+        with sm_limit(G):
+            m = _engine(sd, FULL, 256, "fp32", 12, mode="fp8")
+            try:
+                for n in range(1, 13):
+                    _begin(m, n, 3)
+                    n0 = _launches(m)
+                    _lib.check(m._lib.mvb_s1_decode(m.handle, n, 1, m._stream()))
+                    torch.cuda.synchronize()
+                    body = "B" if n > 8 else "A"
+                    assert _launches(m) - n0 == want[body], f"fp8 G={G} n={n}: {_launches(m) - n0} launches, not path {body}'s"
+            finally:
+                m.close()
+    print(f"fp8 decode at G = {counts(SM_COUNTS)}: path A at 1 .. 8 slots, path B at 9 .. 12")
 
 
 # ---------------------------------------------------------------------------------------------------------------------

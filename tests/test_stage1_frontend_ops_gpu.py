@@ -1,6 +1,6 @@
 """GPU: the stage-1 front end and the prefill plumbing at production width (metavoice-1B: D = 2048, H = 16, F = 5632,
-V = 2562, speaker dim SD = 256, block_size 2048): the speaker projection k_spk_proj (bf16 and int8), the embedding sum of
-every decode body (k_embed on path A, k_embed_rows on path B, the owner CTA of the persistent kernel on path C), the
+V = 2562, speaker dim SD = 256, block_size 2048): the speaker projection k_spk_proj (bf16, int8 and fp8), the embedding
+sum of every decode body (k_embed on path A, k_embed_rows on path B, the owner CTA of the persistent kernel on path C), the
 layer-0 operand every persistent CTA stages straight from the tables, and mvb_s1_forward's chunk loop (k_rows_prefill,
 k_gather_last, k_set_input, the [2, S, V] all-positions copy, the sampler rows).
 
@@ -8,16 +8,20 @@ PROBE MODEL.  2 layers whose matrices are all zero, so each layer adds exactly 0
 +0, which turns -0 into +0: x is compared as floats).  Token and position tables are random bf16 N(0, 1) with about 0.1 %
 of the entries replaced by +-(64 .. 256); W_spk is random bf16 N(0, 1), the ln_f gain 1 + 0.1 N(0, 1), lm_head bf16
 N(0, 1 / D), speakers fp32 N(0, 1) with a different one in every slot.  The bf16, int8 (quantize.pack_arena_int8:
-every Linear per output channel, so W_spk and lm_head get bf16 row scales that are not powers of two) and int4
+every Linear per output channel, so W_spk and lm_head get bf16 row scales that are not powers of two), int4
 (quantize.pack_arena_int4: the zero layer matrices packed, W_spk stored as its bf16 W_deq, lm_head bf16 since 2562 % 8
-!= 0) engines are built from the same state dict.  The workspace is read through a Python mirror of make_layout
+!= 0) and fp8 (quantize.pack_arena_fp8: e4m3 codes and non-power-of-two bf16 row scales; the engine widens W_spk's and
+lm_head's codes once at create into f8_spk and w8_head) engines are built from the same state dict.  The fp8 speaker
+projection runs k_spk_proj over f8_spk with the arena's row scales: codes written after create are never read, which
+is checked; the quantised workspace tail (layer scratch, w8_head, f8_spk) is mirrored against
+mvb_s1_{int4,int8,fp8}_workspace_bytes and its widened copies compared with the arena's codes.  The workspace is read through a Python mirror of make_layout
 (csrc/stage1_engine.cu), whose end is checked against mvb_s1_workspace_bytes here and the pinned totals of
 tests/test_workspace_layout_cpu.py.
 
 1 SPEAKER PROJECTION (mvb_s1_set_speaker).  Lane l of output row j runs one fma chain over k = l, l + 32, ... (SD / 32
   terms), then a 5-level butterfly adds the lanes: every product passes through at most ceil(SD / 32) + 5 roundings, so
       |y^ - y| <= gamma_(ceil(SD/32)+5) sum_k |W_jk| |spk_k|,    gamma_n = n u / (1 - n u), u = 2^-23.
-  int8: the chain runs over the exact integers q (W = s q), and the bf16 row scale multiplies the sum once: the same
+  int8 / fp8: the chain runs over the exact codes q (W = s q), and the bf16 row scale multiplies the sum once: the same
   gamma times s sum |q| |spk| (to first order; 1.01 gamma is used), + u |y| for the product.  The reference is float64
   of the very weights the engine holds (bf16 W, s q, the int4 arena's W_deq).  The spk slice is NaN-filled first: only
   slot u's D floats may change, and none may stay NaN.  Slots 0, 3, max_utts - 1; a zero speaker (exactly 0 out); a
@@ -44,8 +48,9 @@ tests/test_workspace_layout_cpu.py.
   tests/test_gemm_ops_gpu.py per split, the k-split from plan_gemm_ksplit: R = 2 Sc only changes the column count), + the
   sum of squares of x (k_prep_b and the GEMV prologue: 8-term chains, 5-level butterfly, 8 warp sums, / D, + eps:
   depth 24) and, for int8, u |y| for the row scale.  Lengths S in {1, 2, 63, 64, 65, 128, 129, 2047} at pos0 = 0 and
-  S = 70 at pos0 in {1000, 1977}, into slot 0 and slot max_utts - 1 of an 8-slot engine, for bf16, int8 and int4 with
-  fp32 and bf16 KV; S = 1 takes the one-position path A loop, the rest the 64-token chunks (the launch count shows which),
+  S = 70 at pos0 in {1000, 1977}, into slot 0 and slot max_utts - 1 of an 8-slot engine, for bf16, int8, int4 and fp8
+  with fp32 and bf16 KV (fp8 at S = 1 and on the path A loop: k_gemv_f8's head, the gamma of tests/test_fp8_gemv_gpu.py
+  and its own sum-of-squares depth D / 32 + 12); S = 1 takes the one-position path A loop, the rest the 64-token chunks (the launch count shows which),
   and a CUDA-core-only engine runs the path A loop at S = 2 and 65.  Every call runs with all_positions = 1 into a
   caller buffer between NaN guards (every element written, nothing outside) and with all_positions = 0 (the 2 x V copy
   equals the slot's sampler rows, which must satisfy the bound of the last position).  Afterwards slot_map[0] = utt,
@@ -57,7 +62,7 @@ tests/test_workspace_layout_cpu.py.
 5 SENSITIVITY.  Altered references that must be caught: bit-exact checks must differ on >= 99 % of the affected
   elements (the speaker on the unconditioned row too, slot u - 1's speaker, the speaker rounded to bf16 before the add,
   the position row pos - 1); bounded checks must put >= 50 % of the affected elements over the bound (the int8 speaker
-  projection without its row scale: >= 99 %; prefill: the position row pos0 + s0 + s - 1, the chunk offset s0 dropped
+  projection without its row scale: >= 99 %, int8 / fp8 with each row's scale from its neighbour; prefill: the position row pos0 + s0 + s - 1, the chunk offset s0 dropped
   from the token index, the unconditioned tokens taken from row 0, slot u - 1's speaker, the speaker on both rows, the
   last-position gather from row Sc - 2; staged operand: the speaker dropped, the other row's token, the position row
   pos + 1)."""
@@ -141,13 +146,25 @@ def test_workspace_mirror():
         assert got == want, (name, utts, got, want)
 
 
+def quant_tail(lay, dim=D, inter=F, vocab=V, spk_dim=SPK):
+    """Mirror of make_layout's quantised tail: the one-layer bf16 weight scratch (int4, int8, fp8), lm_head's widened q
+    (int8, fp8: w8_head), speaker_cond_pos's widened q (fp8: f8_spk); name -> (byte offset, bytes), and the totals."""
+    out, off = {}, lay["total"]
+    for name, n in (("layer_scratch", (4 * dim * dim + 3 * dim * inter) * 2), ("w8_head", vocab * dim * 2),
+                    ("f8_spk", dim * spk_dim * 2)):
+        out[name] = (off, n)
+        off = (off + n + 255) // 256 * 256
+        out[{"layer_scratch": "int4", "w8_head": "int8", "f8_spk": "fp8"}[name]] = off
+    return out
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 class Model:
     """The probe state dict, its three device arenas, the tables and the per-slot speakers."""
 
     def __init__(self):
         from mvb200.fast_model import pack_arena
-        from mvb200.quantize import pack_arena_int4, pack_arena_int8
+        from mvb200.quantize import pack_arena_fp8, pack_arena_int4, pack_arena_int8
         g = torch.Generator().manual_seed(0)
 
         def table(rows):
@@ -170,7 +187,8 @@ class Model:
                        p + "mlp.swiglu.w3.weight": torch.zeros(F, D, dtype=bf),
                        p + "mlp.c_proj.weight": torch.zeros(D, F, dtype=bf)})
         self.sd = sd
-        self.arenas = {"bf16": pack_arena(sd, NL), "int8": pack_arena_int8(sd, NL)[:2], "int4": pack_arena_int4(sd, NL)[:2]}
+        self.arenas = {"bf16": pack_arena(sd, NL), "int8": pack_arena_int8(sd, NL)[:2], "int4": pack_arena_int4(sd, NL)[:2],
+                       "fp8": pack_arena_fp8(sd, NL)[:2]}
         self.arenas = {k: (a.cuda(), o) for k, (a, o) in self.arenas.items()}
         self.tok = sd["transformer.wtes.0.weight"].cuda()
         self.pos = sd["transformer.wpe.weight"].cuda()
@@ -209,8 +227,12 @@ class Eng:
 
     def weights(self, name, M, K):
         """float64 (W or q [M, K], row scale [M] or None) of a global Linear as the engine holds it."""
-        if self.fmt == "int8":
-            q = self.tensor(name, (M, K), torch.int8).double()
+        if self.fmt in ("int8", "fp8"):
+            if self.fmt == "int8":
+                q = self.tensor(name, (M, K), torch.int8).double()
+            else:
+                from mvb200.quantize import unpack_fp8_codes
+                q = unpack_fp8_codes(self.tensor(name, (M * K,), torch.uint8).cpu(), M, K).double().cuda()
             s = self.tensor(name, (M,), torch.bfloat16, extra=(M * K + 255) // 256 * 256).double()
             return q, s
         return self.tensor(name, (M, K), torch.bfloat16).double(), None
@@ -279,15 +301,15 @@ def caught(label, frac, need):
 
 # ---------------------------------------------------------------------------------------------------------------------
 # 1. speaker projection
-@pytest.mark.parametrize("fmt", ["bf16", "int8", "int4"])
+@pytest.mark.parametrize("fmt", ["bf16", "int8", "int4", "fp8"])
 def test_speaker_projection(model, engines, fmt):
     e = engines(fmt, "fp32", "BC", MAXU)
     W, s = e.weights("speaker_cond_pos.weight", D, SPK)
-    if fmt == "int8":
-        from mvb200.quantize import quantize_per_channel
-        q0, s0 = quantize_per_channel(model.sd["speaker_cond_pos.weight"])
+    if fmt in ("int8", "fp8"):
+        from mvb200.quantize import quantize_fp8_per_channel, quantize_per_channel
+        q0, s0 = (quantize_per_channel if fmt == "int8" else quantize_fp8_per_channel)(model.sd["speaker_cond_pos.weight"])
         assert torch.equal(W.cpu(), q0.double()) and torch.equal(s.cpu(), s0.double())
-        assert not all(math.log2(v).is_integer() for v in s.abs().tolist()), "int8 row scales are all powers of two"
+        assert not all(math.log2(v).is_integer() for v in s.abs().tolist()), f"{fmt} row scales are all powers of two"
     elif fmt == "int4":
         from mvb200.quantize import dequantize, group_quantize
         wd = dequantize(*group_quantize(model.sd["speaker_cond_pos.weight"]))
@@ -312,15 +334,68 @@ def test_speaker_projection(model, engines, fmt):
             v64 = vec.double()
             y = (W @ v64) * scale
             A = (W.abs() @ v64.abs()) * scale
-            b = 1.01 * gam(-(-SPK // 32) + 5) * A + (U * y.abs() if fmt == "int8" else 0) + 1e-300
+            b = 1.01 * gam(-(-SPK // 32) + 5) * A + (U * y.abs() if s is not None else 0) + 1e-300
             if not vec.any():
                 assert (got[u] == 0).all(), f"{fmt}: a zero speaker projects to nonzero values"
             worst = max(worst, check_bound(f"{fmt} k_spk_proj slot {u}", got[u], y, b))
-            if fmt == "int8" and u == 0:
-                caught("int8 projection without its row scale", float(over(got[u], W @ v64, b).double().mean()), BIT_SENS)
+            if s is not None and u == 0:
+                caught(f"{fmt} projection without its row scale", float(over(got[u], W @ v64, b).double().mean()), BIT_SENS)
+                caught(f"{fmt} projection with each row's scale from its neighbour",
+                       float(over(got[u], (W @ v64) * torch.roll(s, 1), b).double().mean()), BOUND_SENS)
     finally:
         e.set_speakers()
     print(f"k_spk_proj<{'int8_t' if fmt == 'int8' else 'bf16'}> ({fmt} engine): max |err|/bound {worst:.2e}")
+
+
+def test_fp8_speaker_codes_widened_at_create(model, engines):
+    """An fp8 engine projects the speaker through f8_spk, speaker_cond_pos's codes widened once at create: codes written
+    into the arena afterwards are never read (the projection stays bit for bit what it was), while the row scales are
+    read from the arena at every mvb_s1_set_speaker.  So W_spk is part of the engine: change it by creating a new one."""
+    e = engines("fp8", "fp32", "BC", MAXU)
+    o = e.offsets[2]
+    codes = e.arena[o:o + D * SPK]
+    scales = e.arena[o + (D * SPK + 255) // 256 * 256:][:2 * D].view(torch.bfloat16)
+    spk = e.sl("spk", torch.float32).view(MAXU, D)
+    vec = torch.randn(SPK, generator=torch.Generator(device="cuda").manual_seed(12), device="cuda")
+    keep_c, keep_s = codes.clone(), scales.clone()
+    try:
+        e.m.set_speaker(1, vec)
+        torch.cuda.synchronize()
+        before = spk[1].clone()
+        codes.copy_(torch.roll(keep_c, 1))                  # other codes, same scales
+        e.m.set_speaker(1, vec)
+        torch.cuda.synchronize()
+        assert torch.equal(spk[1].view(torch.int32), before.view(torch.int32)), "fp8 k_spk_proj read the arena's codes"
+        codes.copy_(keep_c)
+        scales.mul_(2)                                      # the scales are live: exactly twice the projection
+        e.m.set_speaker(1, vec)
+        torch.cuda.synchronize()
+        assert torch.equal(spk[1], 2 * before), "fp8 k_spk_proj did not apply the arena's row scales"
+    finally:
+        codes.copy_(keep_c)
+        scales.copy_(keep_s)
+        e.set_speakers()
+    print("fp8 speaker projection: codes widened at create, row scales read at every set_speaker")
+
+
+@pytest.mark.parametrize("fmt", ["int8", "fp8"])
+def test_quant_workspace_mirror(model, engines, fmt):
+    """mvb_s1_{int4,int8,fp8}_workspace_bytes end where the mirror's quantised tail does, and the widened copies the
+    engine makes at create hold the arena's codes exactly: lm_head's in w8_head, and for fp8 speaker_cond_pos's in f8_spk."""
+    e = engines(fmt, "fp32", "BC", MAXU)
+    tail = quant_tail(e.lay)
+    for f in ("int4", "int8", "fp8"):
+        got = getattr(e.lib, f"mvb_s1_{f}_workspace_bytes")(C.byref(e.m._cfg))
+        assert got == tail[f], (f, got, tail[f])
+    assert e.ws.numel() >= tail[fmt]
+    names = [("w8_head", "lm_heads.0.weight", V, D)] + ([("f8_spk", "speaker_cond_pos.weight", D, SPK)] if fmt == "fp8" else [])
+    for slot, name, M, K in names:
+        o, n = tail[slot]
+        widened = e.ws[o:o + n].view(torch.bfloat16).view(M, K)
+        q, _ = e.weights(name, M, K)
+        assert torch.equal(widened.double(), q), f"{fmt} {slot}: the widened copy differs from the arena's {name} codes"
+    print(f"{fmt} workspace: int4 / int8 / fp8 totals {tail['int4']} / {tail['int8']} / {tail['fp8']} bytes; "
+          f"{', '.join(n[0] for n in names)} exact")
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -513,13 +588,19 @@ def forward(e, utt, idx, pos0, all_pos):
 
 
 def head_ref(e, x, body):
-    """float64 logits [R, V] and bound of the head over x [R, D] (float32) as body `body` stages it."""
+    """float64 logits [R, V] and bound of the head over x [R, D] (float32) as body `body` stages it.  The fp8 engine's
+    path A head is k_gemv_f8: the gamma of tests/test_fp8_gemv_gpu.py (hi + lo activation terms, RMSNorm) and its sum of
+    squares (a lane's D / 32-term fma chain, 2 shuffles, 8 warp sums, / D, + eps: depth D / 32 + 12)."""
     W, s = e.weights("lm_heads.0.weight", V, D)
     nh, _, rs = operand(x.double(), e.model.gf, body)
     sc = 1.0 if s is None else s[None, :]
     y = (nh @ W.t()) * rs * sc
     A = (nh.abs() @ W.abs().t()) * rs * sc
-    b = lin_bound(body, "head", y, A, e.n_sm) + tau_ss(SS_DEPTH_AB) * A
+    if e.fmt == "fp8" and body == "A":
+        from test_fp8_gemv_gpu import gamma as gamma_f8
+        b = (gamma_f8(D, True) + tau_ss(D // 32 + 12)) * A
+    else:
+        b = lin_bound(body, "head", y, A, e.n_sm) + tau_ss(SS_DEPTH_AB) * A
     if s is not None:
         b = b + U * y.abs()
     return y, b
@@ -611,7 +692,8 @@ def run_prefill(e, utt, S, pos0, seed, sens=None):
     return worst
 
 
-PREFILL_ENGINES = [("bf16", "bf16"), ("bf16", "fp32"), ("int8", "fp32"), ("int8", "bf16"), ("int4", "bf16"), ("int4", "fp32")]
+PREFILL_ENGINES = [("bf16", "bf16"), ("bf16", "fp32"), ("int8", "fp32"), ("int8", "bf16"), ("int4", "bf16"), ("int4", "fp32"),
+                   ("fp8", "fp32"), ("fp8", "bf16")]
 
 
 @pytest.mark.parametrize("fmt,kv", PREFILL_ENGINES, ids=[f"{f}-{k}" for f, k in PREFILL_ENGINES])
@@ -642,7 +724,16 @@ def prefill_cases(engines, fmt, kv, cases):
 
 def test_prefill_path_a(model, engines):
     """tensor_core_path = "": the one-position path A loop at every length."""
-    e = engines("bf16", "fp32", "", 3)
+    prefill_path_a(engines, "bf16")
+
+
+def test_prefill_path_a_fp8(model, engines):
+    """The path A loop of an fp8 engine: k_gemv_f8 for every projection, the head with the bound of k_gemv_f8."""
+    prefill_path_a(engines, "fp8")
+
+
+def prefill_path_a(engines, fmt):
+    e = engines(fmt, "fp32", "", 3)
     e.m._kv.zero_()
     e.before = e.cache.clone()
     worst = 0.0
@@ -651,4 +742,4 @@ def test_prefill_path_a(model, engines):
             worst = max(worst, run_prefill(e, utt, S, pos0, 77 + i))
     finally:
         e.before = None
-    print(f"prefill, path A loop (S = 2, 65): max |err|/bound {worst:.2e}")
+    print(f"prefill {fmt}, path A loop (S = 2, 65): max |err|/bound {worst:.2e}")
