@@ -23,8 +23,10 @@ extern "C" {
 #define MVB_ABI_VERSION 3
 
 /* KV-cache element type.  bf16 is what the reference stores (fast_model.py:97-102);
- * fp32 is the validation mode used for the <=1e-3 parity gate against the fp32 oracle. */
-enum { MVB_KV_BF16 = 0, MVB_KV_FP32 = 1 };
+ * fp32 is the validation mode used for the <=1e-3 parity gate against the fp32 oracle;
+ * fp8 (an extension: the reference has no fp8 cache) stores e4m3 codes with one bf16 scale per head vector, layout and
+ * quantiser at mvb_s1_kv_bytes. */
+enum { MVB_KV_BF16 = 0, MVB_KV_FP32 = 1, MVB_KV_FP8 = 2 };
 
 /* Shape of the stage-1 causal LM: fam/llm/fast_model.py:52-94 (ModelArgs / "metavoice-1B"). */
 typedef struct mvb_s1_config {
@@ -38,7 +40,7 @@ typedef struct mvb_s1_config {
   int32_t spk_dim;       /* 256 */
   float   norm_eps;      /* 1e-5 */
   int32_t max_utts;      /* utterance slots; each owns 2 CFG rows {cond, uncond} (fast_model.py:132-134) */
-  int32_t kv_dtype;      /* MVB_KV_BF16 | MVB_KV_FP32 */
+  int32_t kv_dtype;      /* MVB_KV_BF16 | MVB_KV_FP32 | MVB_KV_FP8 */
   int32_t max_new;       /* capacity of the per-utterance generated-token ring (<= block_size) */
   int32_t options;       /* MVB_S1_* bits below; 0 = the production engine */
 } mvb_s1_config;
@@ -75,7 +77,15 @@ const char* mvb_last_error(void);
 
 /* Sizes the caller must allocate (device memory) before mvb_s1_create.
  * Replaces Transformer.setup_caches (fast_model.py:136-148): KV = n_layer x {K,V} x rows x heads x
- * block_size x head_dim elements. */
+ * block_size x head_dim elements, rows = 2 max_utts, element [layer][K|V][row][head][pos][head_dim].
+ * MVB_KV_FP8: with N = n_layer * 2 * rows * heads * block_size head vectors, bytes [0, 128 N) hold one e4m3 code per
+ * element in that layout, and bytes [128 N, 130 N) one bf16 scale per head vector, [layer][K|V][row][head][pos] (scale
+ * of vector i at byte 128 N + 2 i); mvb_s1_kv_bytes = 130 N (408,944,640 per utterance slot at the production shape,
+ * 0.508x the bf16 cache).  Each vector x (fp32, as the qkv projection produced it) is stored as
+ * s = bf16_rn(max(amax|x| / 448, FLT_EPSILON)), q = e4m3_rn(clamp(x / s, -448, 448)) (mvb200/quantize.py
+ * quantize_kv_fp8); a NaN anywhere in x stores s = NaN (0x7fc0) and every code 0x7f, an infinite element makes s = +inf.
+ * The workspace sizes do not depend on kv_dtype.  An fp8-cache engine never uses the resident decode kernel: one
+ * utterance decodes on the per-layer CUDA-core path. */
 size_t mvb_s1_kv_bytes(const mvb_s1_config* cfg);
 size_t mvb_s1_workspace_bytes(const mvb_s1_config* cfg);
 
@@ -371,6 +381,14 @@ int mvb_f8_gemv_test(int32_t epi, const void* d_W, const void* d_W3, int32_t M, 
                      const int32_t* d_slot_map, const int32_t* d_pos, int32_t H, int32_t S_max, int32_t D, int32_t kv_fp32,
                      void* stream);
 int mvb_f8_widen_test(const void* d_W, int32_t M, int32_t K, void* d_out, void* stream);
+/* Test hook for the fp8 KV cache (not part of the drop-in surface):
+ *   mvb_s1_kv_f8_store_test : k_kv_store_f8 as path B launches it.  Row n in [0, R) of d_qkv fp32 [R, 3 D] (D = 128 H)
+ *                             stores its k and v third, head by head, at cache row d_cache_row[n] (< n_cache_rows),
+ *                             position d_pos[n] (< S_max) of d_codes [K|V][n_cache_rows][H][S_max][128] e4m3 and
+ *                             d_scales [K|V][n_cache_rows][H][S_max] bf16, with the quantiser of mvb_s1_kv_bytes.
+ *                             1 <= R <= 128.  Synchronises `stream`. */
+int mvb_s1_kv_f8_store_test(const float* d_qkv, int32_t R, int32_t H, int32_t n_cache_rows, int32_t S_max,
+                            const int32_t* d_cache_row, const int32_t* d_pos, void* d_codes, void* d_scales, void* stream);
 /* Test hook for the projections of a non-production stage-1 architecture (not part of the drop-in surface):
  *   path 0: k_gemv as path A launches it, for utterances u in [0, n_utts): rows 2 s, 2 s + 1 (s = d_slot_map[u]) of d_x
  *           fp32 [*, ldx] and d_out [*, ldo]; out = epilogue(f(x) . W^T + bias); norm 0 none, 1 RMSNorm (d_gain, eps),

@@ -209,9 +209,18 @@ struct mvb_s1 {
     return tc_scale(MVB_S1_GLOBAL_TENSORS + layer * MVB_S1_LAYER_TENSORS + t, mk.M, mk.K);
   }
   const __nv_bfloat16* head_scale() const { return tc_scale(4, cfg.vocab, cfg.dim); }
-  size_t kv_elem() const { return cfg.kv_dtype == MVB_KV_FP32 ? 4 : 2; }
+  size_t kv_elem() const { return cfg.kv_dtype == MVB_KV_FP32 ? 4 : cfg.kv_dtype == MVB_KV_FP8 ? 1 : 2; }
+  // bytes of one layer's K (or V) elements; an fp8 cache's scales follow all the layers' codes
   size_t kv_half_bytes() const {
     return (size_t)2 * cfg.max_utts * cfg.n_head * cfg.block_size * cfg.head_dim * kv_elem();
+  }
+  bool kv_f8() const { return cfg.kv_dtype == MVB_KV_FP8; }
+  // layer l of an fp8 cache (include/mvb200.h): K / V codes, then K / V scales in the region after every layer's codes
+  KvF8 kv_f8_layer(int l) const {
+    const size_t half = kv_half_bytes(), n_scales = (size_t)2 * cfg.max_utts * cfg.n_head * cfg.block_size;
+    __nv_bfloat16* sc = reinterpret_cast<__nv_bfloat16*>(kv + (size_t)cfg.n_layer * 2 * half) + (size_t)l * 2 * n_scales;
+    uint8_t* kc = reinterpret_cast<uint8_t*>(kv + (size_t)l * 2 * half);
+    return KvF8{kc, kc + half, sc, sc + n_scales};
   }
 };
 
@@ -253,7 +262,8 @@ static int validate(const mvb_s1_config* c) {
   if (c->vocab % 2 || c->vocab > SAMP_PAD) return set_error(MVB_ERR_UNSUPPORTED, "vocab must be even and <= %d", SAMP_PAD);
   if (c->max_utts < 1 || c->max_utts > 64) return set_error(MVB_ERR_ARG, "max_utts out of range");
   if (c->max_new < 1 || c->max_new > c->block_size) return set_error(MVB_ERR_ARG, "max_new out of range");
-  if (c->kv_dtype != MVB_KV_BF16 && c->kv_dtype != MVB_KV_FP32) return set_error(MVB_ERR_ARG, "bad kv_dtype");
+  if (c->kv_dtype != MVB_KV_BF16 && c->kv_dtype != MVB_KV_FP32 && c->kv_dtype != MVB_KV_FP8)
+    return set_error(MVB_ERR_ARG, "bad kv_dtype");
   if ((size_t)c->intermediate * 8 > GEMV_MAX_SMEM) return set_error(MVB_ERR_UNSUPPORTED, "intermediate too large for the staging buffer");
   const int known = MVB_S1_NO_ROWS_PATH | MVB_S1_NO_RESIDENT | MVB_S1_UNFUSED_SAMPLER | MVB_S1_TRACE;
   if (c->options & ~known) return set_error(MVB_ERR_ARG, "options: undefined bits 0x%x", (unsigned)(c->options & ~known));
@@ -262,8 +272,9 @@ static int validate(const mvb_s1_config* c) {
 
 extern "C" size_t mvb_s1_kv_bytes(const mvb_s1_config* c) {
   if (validate(c)) return 0;
-  const size_t esz = c->kv_dtype == MVB_KV_FP32 ? 4 : 2;
-  return (size_t)c->n_layer * 2 * (2 * (size_t)c->max_utts) * c->n_head * c->block_size * c->head_dim * esz;
+  const size_t vecs = (size_t)c->n_layer * 2 * (2 * (size_t)c->max_utts) * c->n_head * c->block_size;   // head vectors
+  if (c->kv_dtype == MVB_KV_FP8) return vecs * c->head_dim + vecs * 2;   // e4m3 codes, then one bf16 scale per vector
+  return vecs * c->head_dim * (c->kv_dtype == MVB_KV_FP32 ? 4 : 2);
 }
 
 extern "C" size_t mvb_s1_workspace_bytes(const mvb_s1_config* c) {
@@ -428,6 +439,7 @@ static int create_engine(const mvb_s1_config* cfg, const mvb_s1_arch* arch, cons
   }
   // The persistent kernel's bf16-cache attention fetches KV tiles through tm_kv as whole 64-position boxes: positions
   // past the valid ones must hold finite values, and the map must be encodable.  Where it is not, path C is declined.
+  // It has no fp8-cache form: an fp8 cache never takes path C (kv_ok stays false).
   memset(&h->tm_kv, 0, sizeof(h->tm_kv));
   bool kv_ok = cfg->kv_dtype == MVB_KV_FP32;
   if (cfg->kv_dtype == MVB_KV_BF16 && cfg->block_size % 64 == 0) {
@@ -587,6 +599,33 @@ static cudaError_t launch_gemv_arch(mvb_s1* h, cudaStream_t s, int n_utts, const
   return launch_gemv<EPI, false, false>(h, s, n_utts, p, WFmt::BF16);
 }
 
+// Attention of path A over layer l: the two CFG rows of n_utts utterances at their decode positions.  An fp8 cache first
+// takes the new k / v from the projection's qkv rows (k_kv_store_f8); a bf16 / fp32 cache got them from its EPI_QKV
+// scatter.
+static int attn_decode(mvb_s1* h, cudaStream_t s, int n_utts, int l, const float* qkv, float* att) {
+  const mvb_s1_config& c = h->cfg;
+  const int D = c.dim, H = c.n_head;
+  float* po = h->wsp<float>(h->L.part_o);
+  float* pm = h->wsp<float>(h->L.part_ml);
+  const dim3 ag(H, 2 * n_utts, ATT_SPLITS);
+  if (h->kv_f8()) {
+    const KvF8 kv = h->kv_f8_layer(l);
+    MVB_CK(launch_pdl(k_kv_store_f8<false>, dim3((4 * n_utts * H + 7) / 8), dim3(256), 0, s, h->st, h->rows, 2 * n_utts, qkv,
+                      kv, H, c.block_size, D));
+    h->launches++;
+    MVB_CK(launch_pdl(k_attn_decode_f8, ag, dim3(128), 0, s, h->st, qkv, kv, po, pm, att, H, c.block_size, D));
+  } else {
+    const char* kc = h->kv + (size_t)l * 2 * h->kv_half_bytes();
+    const void* vc = kc + h->kv_half_bytes();
+    if (c.kv_dtype == MVB_KV_FP32)
+      MVB_CK(launch_pdl(k_attn_decode<true>, ag, dim3(128), 0, s, h->st, qkv, (const void*)kc, vc, po, pm, att, H, c.block_size, D));
+    else
+      MVB_CK(launch_pdl(k_attn_decode<false>, ag, dim3(128), 0, s, h->st, qkv, (const void*)kc, vc, po, pm, att, H, c.block_size, D));
+  }
+  h->launches++;
+  return MVB_OK;
+}
+
 // Path A for one position of a non-production architecture (layers/combined.py:38-50 per layer, model.py:303 ln_f, the
 // tied head model.py:137-143): ln_1 -> c_attn (+ bias) + cache scatter, attention, c_proj (+ bias) + residual, ln_2 ->
 // SwiGLU or GELU MLP (+ biases), mlp.c_proj (+ bias) + residual; the norms are RMSNorm or LayerNorm (eps 1e-5, beta).
@@ -604,15 +643,8 @@ static int launch_layers_arch(mvb_s1* h, cudaStream_t s, int n_utts, float* x, f
     p.W = h->lw(l, 1); p.x = x; p.ldx = D; p.gain = lp.g1; p.beta = lp.b1; p.bias = lp.qkv_b;
     p.out = qkv; p.ldo = 3 * D; p.M = 3 * D; p.K = D;
     p.kcache = kc; p.vcache = vc; p.H = H; p.S_max = c.block_size; p.D = D; p.kv_fp32 = c.kv_dtype == MVB_KV_FP32;
-    MVB_CK(launch_gemv_arch<EPI_QKV>(h, s, n_utts, p, ln));
-    dim3 ag(H, 2 * n_utts, ATT_SPLITS);
-    if (c.kv_dtype == MVB_KV_FP32)
-      MVB_CK(launch_pdl(k_attn_decode<true>, ag, dim3(128), 0, s, h->st, (const float*)qkv, (const void*)kc, (const void*)vc,
-                    h->wsp<float>(h->L.part_o), h->wsp<float>(h->L.part_ml), att, H, c.block_size, D));
-    else
-      MVB_CK(launch_pdl(k_attn_decode<false>, ag, dim3(128), 0, s, h->st, (const float*)qkv, (const void*)kc, (const void*)vc,
-                    h->wsp<float>(h->L.part_o), h->wsp<float>(h->L.part_ml), att, H, c.block_size, D));
-    h->launches++;
+    MVB_CK(h->kv_f8() ? launch_gemv_arch<EPI_STORE>(h, s, n_utts, p, ln) : launch_gemv_arch<EPI_QKV>(h, s, n_utts, p, ln));
+    if (int e = attn_decode(h, s, n_utts, l, qkv, att)) return e;
     p = GemvP{};
     p.eps = h->norm_eps();
     p.W = h->lw(l, 2); p.x = att; p.ldx = D; p.bias = lp.o_b; p.out = x; p.ldo = D; p.M = D; p.K = D;
@@ -658,20 +690,13 @@ static int launch_body(mvb_s1* h, cudaStream_t s, int n_utts) {
     char* vc = kc + half;
     GemvP p{};
     p.eps = c.norm_eps;
-    // attention_norm + wqkv + cache scatter
+    // attention_norm + wqkv + cache scatter (fp8 cache: the qkv rows only)
     p.W = h->lw(l, 1); p.W3 = nullptr; p.x = x; p.ldx = D; p.gain = h->lw(l, 0);
     p.out = qkv; p.ldo = 3 * D; p.M = 3 * D; p.K = D;
     p.kcache = kc; p.vcache = vc; p.H = H; p.S_max = c.block_size; p.D = D; p.kv_fp32 = c.kv_dtype == MVB_KV_FP32;
-    MVB_CK(launch_gemv<EPI_QKV>(h, s, n_utts, p, h->fmt));
+    MVB_CK(h->kv_f8() ? launch_gemv<EPI_STORE>(h, s, n_utts, p, h->fmt) : launch_gemv<EPI_QKV>(h, s, n_utts, p, h->fmt));
     // attention over [0, pos]
-    dim3 ag(H, 2 * n_utts, ATT_SPLITS);
-    if (c.kv_dtype == MVB_KV_FP32)
-      MVB_CK(launch_pdl(k_attn_decode<true>, ag, dim3(128), 0, s, h->st, (const float*)qkv, (const void*)kc, (const void*)vc,
-                    h->wsp<float>(h->L.part_o), h->wsp<float>(h->L.part_ml), att, H, c.block_size, D));
-    else
-      MVB_CK(launch_pdl(k_attn_decode<false>, ag, dim3(128), 0, s, h->st, (const float*)qkv, (const void*)kc, (const void*)vc,
-                    h->wsp<float>(h->L.part_o), h->wsp<float>(h->L.part_ml), att, H, c.block_size, D));
-    h->launches++;
+    if (int e = attn_decode(h, s, n_utts, l, qkv, att)) return e;
     // wo + residual
     p = GemvP{};
     p.eps = c.norm_eps;
@@ -744,16 +769,32 @@ static int linear_b(mvb_s1* h, cudaStream_t s, int R, const LinB& a, void* kc = 
   return MVB_OK;
 }
 
-static int attn_rows(mvb_s1* h, cudaStream_t s, int R, const float* qkv, const void* kc, const void* vc, float* att) {
+// The qkv projection of path B (operands `a`) and the attention of the R rows of h->rows over layer l's cache.  An fp8
+// cache takes the new k / v from the stored qkv rows (G_STORE, then k_kv_store_f8) before the attention reads them: a
+// prefill chunk attends to its own positions.
+static int qkv_attn_rows(mvb_s1* h, cudaStream_t s, int R, int l, const LinB& a, const float* qkv, float* att) {
   const mvb_s1_config& c = h->cfg;
   const int D = c.dim, H = c.n_head;
+  char* kc = h->kv + (size_t)l * 2 * h->kv_half_bytes();
+  char* vc = kc + h->kv_half_bytes();
+  float* po = h->wsp<float>(h->L.b_part_o);
+  float* pm = h->wsp<float>(h->L.b_part_ml);
+  unsigned* tk = h->wsp<unsigned>(h->L.b_att_tickets);
   dim3 ag(H, R, ATT_SPLITS);
-  if (c.kv_dtype == MVB_KV_FP32)
-    k_attn_rows<true><<<ag, 128, 0, s>>>(h->rows, qkv, kc, vc, h->wsp<float>(h->L.b_part_o), h->wsp<float>(h->L.b_part_ml),
-                                         h->wsp<unsigned>(h->L.b_att_tickets), att, H, c.block_size, D);
-  else
-    k_attn_rows<false><<<ag, 128, 0, s>>>(h->rows, qkv, kc, vc, h->wsp<float>(h->L.b_part_o), h->wsp<float>(h->L.b_part_ml),
-                                          h->wsp<unsigned>(h->L.b_att_tickets), att, H, c.block_size, D);
+  if (h->kv_f8()) {
+    if (int e = linear_b<G_STORE>(h, s, R, a)) return e;
+    const KvF8 kv = h->kv_f8_layer(l);
+    k_kv_store_f8<true><<<(2 * R * H + 7) / 8, 256, 0, s>>>(h->st, h->rows, R, qkv, kv, H, c.block_size, D);
+    h->launches++;
+    MVB_CK(cudaGetLastError());
+    k_attn_rows_f8<<<ag, 128, 0, s>>>(h->rows, qkv, kv, po, pm, tk, att, H, c.block_size, D);
+  } else {
+    if (int e = linear_b<G_QKV>(h, s, R, a, kc, vc)) return e;
+    if (c.kv_dtype == MVB_KV_FP32)
+      k_attn_rows<true><<<ag, 128, 0, s>>>(h->rows, qkv, kc, vc, po, pm, tk, att, H, c.block_size, D);
+    else
+      k_attn_rows<false><<<ag, 128, 0, s>>>(h->rows, qkv, kc, vc, po, pm, tk, att, H, c.block_size, D);
+  }
   h->launches++;
   MVB_CK(cudaGetLastError());
   return MVB_OK;
@@ -761,14 +802,12 @@ static int attn_rows(mvb_s1* h, cudaStream_t s, int R, const float* qkv, const v
 
 // One layer of a non-production architecture on the tensor cores: the projections of launch_layers_arch with the
 // LayerNorm prologue of k_prep_b<true> and the BIASED / G_GELU epilogues of k_tc_gemm.
-static int layer_b_arch(mvb_s1* h, cudaStream_t s, int R, int l, float* x, float* qkv, float* att, float* ffn, void* kc,
-                        void* vc) {
+static int layer_b_arch(mvb_s1* h, cudaStream_t s, int R, int l, float* x, float* qkv, float* att, float* ffn) {
   const int D = h->cfg.dim, F = h->cfg.intermediate;
   const S1LayerP& p = h->lp[l];
   LinB a{x, D, p.g1, l * 5 + 0, l * 5 + 0, 3 * D, D, qkv, 3 * D};
   a.beta = p.b1; a.bias = p.qkv_b;
-  if (int e = linear_b<G_QKV>(h, s, R, a, kc, vc)) return e;
-  if (int e = attn_rows(h, s, R, qkv, kc, vc, att)) return e;
+  if (int e = qkv_attn_rows(h, s, R, l, a, qkv, att)) return e;
   a = LinB{att, D, nullptr, l * 5 + 1, l * 5 + 1, D, D, x, D};
   a.bias = p.o_b;
   if (int e = linear_b<G_RESID>(h, s, R, a)) return e;
@@ -792,7 +831,7 @@ static int head_b(mvb_s1* h, cudaStream_t s, int R, const float* x, float* out) 
 // embed + all layers for the R rows described by h->rows (already filled on the device)
 static int launch_layers_b(mvb_s1* h, cudaStream_t s, int R) {
   const mvb_s1_config& c = h->cfg;
-  const int D = c.dim, F = c.intermediate, H = c.n_head;
+  const int D = c.dim, F = c.intermediate;
   float* x = h->wsp<float>(h->L.b_x);
   float* qkv = h->wsp<float>(h->L.b_qkv);
   float* att = h->wsp<float>(h->L.b_att);
@@ -800,10 +839,7 @@ static int launch_layers_b(mvb_s1* h, cudaStream_t s, int R) {
   k_embed_rows<<<R, 256, 0, s>>>(h->rows, h->w(0), h->w(1), h->wsp<float>(h->L.spk), x, D);
   h->launches++;
   MVB_CK(cudaGetLastError());
-  const size_t half = h->kv_half_bytes();
   for (int l = 0; l < c.n_layer; ++l) {
-    char* kc = h->kv + (size_t)l * 2 * half;
-    char* vc = kc + half;
     if (h->fmt != WFmt::BF16) {   // this layer's W_deq (int4) or q (int8, fp8) -> the scratch the tensor maps of every layer point at
       W4Mats m{};   // == W8Mats
       const int ts[5] = {1, 2, 4, 5, 6};
@@ -825,20 +861,11 @@ static int launch_layers_b(mvb_s1* h, cudaStream_t s, int R) {
       MVB_CK(cudaGetLastError());
     }
     if (!h->production_arch()) {   // the layer of a non-production architecture (path A's launch_layers_arch)
-      if (int e = layer_b_arch(h, s, R, l, x, qkv, att, ffn, kc, vc)) return e;
+      if (int e = layer_b_arch(h, s, R, l, x, qkv, att, ffn)) return e;
       continue;
     }
-    if (int e = linear_b<G_QKV>(h, s, R, LinB{x, D, h->lw(l, 0), l * 5 + 0, l * 5 + 0, 3 * D, D, qkv, 3 * D, h->tc_lscale(l, 1)},
-                                kc, vc)) return e;
-    dim3 ag(H, R, ATT_SPLITS);
-    if (c.kv_dtype == MVB_KV_FP32)
-      k_attn_rows<true><<<ag, 128, 0, s>>>(h->rows, qkv, kc, vc, h->wsp<float>(h->L.b_part_o), h->wsp<float>(h->L.b_part_ml),
-                                           h->wsp<unsigned>(h->L.b_att_tickets), att, H, c.block_size, D);
-    else
-      k_attn_rows<false><<<ag, 128, 0, s>>>(h->rows, qkv, kc, vc, h->wsp<float>(h->L.b_part_o), h->wsp<float>(h->L.b_part_ml),
-                                            h->wsp<unsigned>(h->L.b_att_tickets), att, H, c.block_size, D);
-    h->launches++;
-    MVB_CK(cudaGetLastError());
+    if (int e = qkv_attn_rows(h, s, R, l, LinB{x, D, h->lw(l, 0), l * 5 + 0, l * 5 + 0, 3 * D, D, qkv, 3 * D, h->tc_lscale(l, 1)},
+                              qkv, att)) return e;
     if (int e = linear_b<G_RESID>(h, s, R, LinB{att, D, nullptr, l * 5 + 1, l * 5 + 1, D, D, x, D, h->tc_lscale(l, 2)})) return e;
     if (int e = linear_b<G_SWIGLU>(h, s, R, LinB{x, D, h->lw(l, 3), l * 5 + 2, l * 5 + 3, F, D, ffn, F, h->tc_lscale(l, 4),
                                                   h->tc_lscale(l, 5)})) return e;
@@ -1579,6 +1606,28 @@ extern "C" int mvb_f8_widen_test(const void* d_W, int32_t M, int32_t K, void* d_
   if (int e = current_device(&dev, &n_sm)) return e;
   cudaStream_t s = (cudaStream_t)stream;
   k_f8_widen<<<4 * n_sm, 256, 0, s>>>(m);
+  MVB_CK(cudaGetLastError());
+  MVB_CK(cudaStreamSynchronize(s));
+  return MVB_OK;
+}
+
+// Test hook of the fp8 KV store (include/mvb200.h): k_kv_store_f8 as path B launches it, over R caller-described rows.
+extern "C" int mvb_s1_kv_f8_store_test(const float* d_qkv, int32_t R, int32_t H, int32_t n_cache_rows, int32_t S_max,
+                                       const int32_t* d_cache_row, const int32_t* d_pos, void* d_codes, void* d_scales,
+                                       void* stream) {
+  if (!d_qkv || !d_cache_row || !d_pos || !d_codes || !d_scales) return set_error(MVB_ERR_ARG, "null argument");
+  if (R < 1 || R > RB_MAX || H < 1 || n_cache_rows < 1 || S_max < 1)
+    return set_error(MVB_ERR_ARG, "mvb_s1_kv_f8_store_test: R %d (1..%d), H %d, n_cache_rows %d, S_max %d", R, RB_MAX, H,
+                     n_cache_rows, S_max);
+  const size_t n_vec = (size_t)n_cache_rows * H * S_max;
+  uint8_t* codes = reinterpret_cast<uint8_t*>(d_codes);
+  __nv_bfloat16* scales = reinterpret_cast<__nv_bfloat16*>(d_scales);
+  const KvF8 kv{codes, codes + n_vec * 128, scales, scales + n_vec};
+  RowsDev rw{};
+  rw.cache_row = const_cast<int*>(d_cache_row);
+  rw.pos = const_cast<int*>(d_pos);
+  cudaStream_t s = (cudaStream_t)stream;
+  k_kv_store_f8<true><<<(2 * R * H + 7) / 8, 256, 0, s>>>(S1State{}, rw, R, d_qkv, kv, H, S_max, 128 * H);
   MVB_CK(cudaGetLastError());
   MVB_CK(cudaStreamSynchronize(s));
   return MVB_OK;

@@ -7,6 +7,9 @@
 #pragma once
 #include <type_traits>
 
+#include <cuda_fp16.h>
+#include <cuda_fp8.h>
+
 #include "common.cuh"
 
 namespace mvb {
@@ -391,6 +394,16 @@ __global__ void __launch_bounds__(256, 2) k_gemv(GemvP p, S1State st) {
 // Split-KV flash decoding: grid (head, row, split); the last-arriving split merges.
 constexpr int ATT_SPLITS = 8;
 
+// Path B: arbitrary activation rows (batched decode rows or the 2*S rows of a prefill chunk); each row
+// names its cache row and its own position, i.e. causal attention over [0, pos[row]].
+struct RowsDev {
+  int* cache_row;
+  int* pos;
+  int* tok;
+  int* utt;
+  int* cond;
+};
+
 template <bool KV_FP32>
 __device__ __forceinline__ void load8(const void* base, size_t elem, float (&v)[8]) {
   if (KV_FP32) {
@@ -405,13 +418,92 @@ __device__ __forceinline__ void load8(const void* base, size_t elem, float (&v)[
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// fp8 KV cache (MVB_KV_FP8, layout in include/mvb200.h): e4m3 codes where the bf16 cache has its elements, and one bf16
+// scale per (layer, K|V, cache row, head, pos) in a region after all the codes.  Each new 128-element k or v -- the fp32
+// qkv output exactly as the projection produced it -- is stored as
+//   s = bf16_rn(max(amax|x| / 448, FLT_EPSILON)),   q = e4m3_rn(clamp(x / s, -448, 448))
+// (mvb200/quantize.py quantize_kv_fp8); s q is exact in fp32 (8 + 4 significant bits), so attention runs the fp32-cache
+// arithmetic over exact dequantised values.  Non-finite input: a NaN anywhere in x gives s = NaN (bits 0x7fc0) and every
+// code 0x7f; otherwise +-inf makes s = +inf, its own code 0x7f (inf / inf) and every finite element's code a signed zero.
+enum { KVC_BF16 = 0, KVC_FP32 = 1, KVC_FP8 = 2 };   // cache formats, == MVB_KV_*
+
+struct KvF8 {
+  uint8_t* kc;           // this layer's K codes [rows][H][S_max][128]
+  uint8_t* vc;           // V codes
+  __nv_bfloat16* ks;     // K scales [rows][H][S_max]
+  __nv_bfloat16* vs;     // V scales
+};
+
+// e4m3 code of one quotient r = x / s: NaN -> 0x7f, else round to nearest even after the clamp (the hardware cvt)
+__device__ __forceinline__ uint32_t kv_f8_code(float r) {
+  if (r != r) return 0x7fu;
+  return __nv_cvt_float_to_fp8(fminf(fmaxf(r, -448.f), 448.f), __NV_SATFINITE, __NV_E4M3);
+}
+
+// One warp per (activation row n, head, K|V): a float4 per lane, the amax as an unsigned max over |x|'s bit patterns (a NaN
+// sorts above +inf, where fmaxf would drop it), one 128-byte store of codes, one scale store.  ROWS: row n of qkv goes to
+// cache row rw.cache_row[n] at rw.pos[n] (path B: prefill chunks and batched decode); else row n is CFG row n & 1 of slot
+// u = st.slot_map[n >> 1], i.e. qkv / cache row 2u + (n & 1) at st.pos[u] (path A).
+template <bool ROWS>
+__global__ void __launch_bounds__(256) k_kv_store_f8(S1State st, RowsDev rw, int n_rows, const float* __restrict__ qkv,
+                                                     KvF8 kv, int H, int S_max, int D) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (gw >= n_rows * H * 2) return;
+  const int which = gw & 1, h = (gw >> 1) % H, n = (gw >> 1) / H;
+  int row, cache_row, pos;
+  if (ROWS) {
+    row = n;
+    cache_row = rw.cache_row[n];
+    pos = rw.pos[n];
+  } else {
+    const int u = st.slot_map[n >> 1];
+    row = cache_row = 2 * u + (n & 1);
+    pos = st.pos[u];
+  }
+  const float4 x = *reinterpret_cast<const float4*>(qkv + (size_t)row * 3 * D + (size_t)(1 + which) * D + h * 128 + lane * 4);
+  const unsigned m = max(max(__float_as_uint(x.x) & 0x7fffffffu, __float_as_uint(x.y) & 0x7fffffffu),
+                         max(__float_as_uint(x.z) & 0x7fffffffu, __float_as_uint(x.w) & 0x7fffffffu));
+  const unsigned amax = __reduce_max_sync(0xffffffffu, m);
+  uint32_t codes = 0x7f7f7f7fu;
+  __nv_bfloat16 sb = __ushort_as_bfloat16((unsigned short)0x7fc0);
+  if (amax <= 0x7f800000u) {   // no NaN
+    sb = __float2bfloat16_rn(fmaxf(__uint_as_float(amax) / 448.f, 1.1920928955078125e-7f));   // FLT_EPSILON
+    const float s = __bfloat162float(sb);
+    codes = kv_f8_code(x.x / s) | kv_f8_code(x.y / s) << 8 | kv_f8_code(x.z / s) << 16 | kv_f8_code(x.w / s) << 24;
+  }
+  const size_t slot = ((size_t)cache_row * H + h) * S_max + pos;
+  reinterpret_cast<uint32_t*>(which ? kv.vc : kv.kc)[slot * 32 + lane] = codes;
+  if (lane == 0) (which ? kv.vs : kv.ks)[slot] = sb;
+}
+
+// 8 codes of one position (8 bytes per lane: a 128-byte line per half-warp) times the position's scale, exactly
+// (hardware e4m3x2 -> f16x2 conversion, then one fp32 product with 12 significant bits)
+__device__ __forceinline__ void load8_f8(const uint8_t* codes, size_t elem, float scale, float (&v)[8]) {
+  const uint2 w = __ldcg(reinterpret_cast<const uint2*>(codes + elem));
+  const uint32_t wd[2] = {w.x, w.y};
+#pragma unroll
+  for (int j = 0; j < 2; ++j)
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const __half2_raw hr = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(wd[j] >> (16 * i)), __NV_E4M3);
+      const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hr));
+      v[4 * j + 2 * i] = f.x * scale;
+      v[4 * j + 2 * i + 1] = f.y * scale;
+    }
+}
+
 // One (query row, head, KV split): q = query vector (fp32, 128), cache_row/L select the K/V slice,
-// pidx indexes the per-(row, head) partial slots, `ticket` is that pair's arrival counter.
-template <bool KV_FP32>
+// pidx indexes the per-(row, head) partial slots, `ticket` is that pair's arrival counter.  KV: the cache's KVC_* format;
+// kscale / vscale are an fp8 cache's scales (unused otherwise).
+template <int KV>
 __device__ __forceinline__ void attn_core(const float* __restrict__ qvec, const void* kcache, const void* vcache,
                                           int cache_row, int L, int h, int split, int H, int S_max,
                                           float* __restrict__ part_o, float* __restrict__ part_ml, size_t pair,
-                                          unsigned* ticket, float* __restrict__ out_vec) {
+                                          unsigned* ticket, float* __restrict__ out_vec,
+                                          const __nv_bfloat16* kscale = nullptr, const __nv_bfloat16* vscale = nullptr) {
   __shared__ float sm_o[8][128];
   __shared__ float sm_m[8], sm_l[8];
   __shared__ int sm_last;
@@ -427,6 +519,7 @@ __device__ __forceinline__ void attn_core(const float* __restrict__ qvec, const 
     for (int i = 0; i < 8; ++i) q[i] = qvec[sub * 8 + i] * scale;
   }
   const size_t row_base = ((size_t)cache_row * H + h) * S_max * 128 + sub * 8;
+  const size_t scale_base = ((size_t)cache_row * H + h) * S_max;
   float m = -INFINITY, l = 0.f, o[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) o[i] = 0.f;
@@ -437,7 +530,10 @@ __device__ __forceinline__ void attn_core(const float* __restrict__ qvec, const 
     float kv[8];
     float s = 0.f;
     if (valid) {
-      load8<KV_FP32>(kcache, row_base + (size_t)p * 128, kv);
+      if constexpr (KV == KVC_FP8)
+        load8_f8(reinterpret_cast<const uint8_t*>(kcache), row_base + (size_t)p * 128, bf16_to_f32(kscale[scale_base + p]), kv);
+      else
+        load8<KV == KVC_FP32>(kcache, row_base + (size_t)p * 128, kv);
 #pragma unroll
       for (int i = 0; i < 8; ++i) s = fmaf(q[i], kv[i], s);
     }
@@ -446,7 +542,10 @@ __device__ __forceinline__ void attn_core(const float* __restrict__ qvec, const 
     s += __shfl_xor_sync(0xffffffffu, s, 2);
     s += __shfl_xor_sync(0xffffffffu, s, 1);
     if (valid) {
-      load8<KV_FP32>(vcache, row_base + (size_t)p * 128, kv);
+      if constexpr (KV == KVC_FP8)
+        load8_f8(reinterpret_cast<const uint8_t*>(vcache), row_base + (size_t)p * 128, bf16_to_f32(vscale[scale_base + p]), kv);
+      else
+        load8<KV == KVC_FP32>(vcache, row_base + (size_t)p * 128, kv);
       const float mn = fmaxf(m, s);
       const float corr = __expf(m - mn);  // m = -inf on the first visit -> 0
       const float pw = __expf(s - mn);
@@ -524,19 +623,23 @@ __global__ void __launch_bounds__(128) k_attn_decode(S1State st, const float* __
   const int h = blockIdx.x, split = blockIdx.z;
   const int u = st.slot_map[blockIdx.y >> 1];
   const int r = 2 * u + (blockIdx.y & 1);
-  attn_core<KV_FP32>(qkv + (size_t)r * 3 * D + h * 128, kcache, vcache, r, st.pos[u] + 1, h, split, H, S_max, part_o,
-                     part_ml, (size_t)r * H + h, &st.attn_ticket[r * H + h], out + (size_t)r * D + h * 128);
+  attn_core<KV_FP32 ? KVC_FP32 : KVC_BF16>(qkv + (size_t)r * 3 * D + h * 128, kcache, vcache, r, st.pos[u] + 1, h, split, H,
+                                         S_max, part_o, part_ml, (size_t)r * H + h, &st.attn_ticket[r * H + h],
+                                         out + (size_t)r * D + h * 128);
 }
 
-// Path B: arbitrary activation rows (batched decode rows or the 2*S rows of a prefill chunk); each row
-// names its cache row and its own position, i.e. causal attention over [0, pos[row]].
-struct RowsDev {
-  int* cache_row;
-  int* pos;
-  int* tok;
-  int* utt;
-  int* cond;
-};
+// k_attn_decode over an fp8 cache
+__global__ void __launch_bounds__(128) k_attn_decode_f8(S1State st, const float* __restrict__ qkv, KvF8 kv,
+                                                        float* __restrict__ part_o, float* __restrict__ part_ml,
+                                                        float* __restrict__ out, int H, int S_max, int D) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int h = blockIdx.x, split = blockIdx.z;
+  const int u = st.slot_map[blockIdx.y >> 1];
+  const int r = 2 * u + (blockIdx.y & 1);
+  attn_core<KVC_FP8>(qkv + (size_t)r * 3 * D + h * 128, kv.kc, kv.vc, r, st.pos[u] + 1, h, split, H, S_max, part_o, part_ml,
+                    (size_t)r * H + h, &st.attn_ticket[r * H + h], out + (size_t)r * D + h * 128, kv.ks, kv.vs);
+}
 
 template <bool KV_FP32>
 __global__ void __launch_bounds__(128) k_attn_rows(RowsDev rw, const float* __restrict__ qkv, const void* kcache,
@@ -544,8 +647,18 @@ __global__ void __launch_bounds__(128) k_attn_rows(RowsDev rw, const float* __re
                                                    float* __restrict__ part_ml, unsigned* tickets,
                                                    float* __restrict__ out, int H, int S_max, int D) {
   const int h = blockIdx.x, n = blockIdx.y, split = blockIdx.z;
-  attn_core<KV_FP32>(qkv + (size_t)n * 3 * D + h * 128, kcache, vcache, rw.cache_row[n], rw.pos[n] + 1, h, split, H, S_max,
-                     part_o, part_ml, (size_t)n * H + h, &tickets[n * H + h], out + (size_t)n * D + h * 128);
+  attn_core<KV_FP32 ? KVC_FP32 : KVC_BF16>(qkv + (size_t)n * 3 * D + h * 128, kcache, vcache, rw.cache_row[n], rw.pos[n] + 1,
+                                         h, split, H, S_max, part_o, part_ml, (size_t)n * H + h, &tickets[n * H + h],
+                                         out + (size_t)n * D + h * 128);
+}
+
+// k_attn_rows over an fp8 cache
+__global__ void __launch_bounds__(128) k_attn_rows_f8(RowsDev rw, const float* __restrict__ qkv, KvF8 kv,
+                                                      float* __restrict__ part_o, float* __restrict__ part_ml,
+                                                      unsigned* tickets, float* __restrict__ out, int H, int S_max, int D) {
+  const int h = blockIdx.x, n = blockIdx.y, split = blockIdx.z;
+  attn_core<KVC_FP8>(qkv + (size_t)n * 3 * D + h * 128, kv.kc, kv.vc, rw.cache_row[n], rw.pos[n] + 1, h, split, H, S_max,
+                    part_o, part_ml, (size_t)n * H + h, &tickets[n * H + h], out + (size_t)n * D + h * 128, kv.ks, kv.vs);
 }
 
 __global__ void k_rows_decode(S1State st, RowsDev rw, int n_utts) {

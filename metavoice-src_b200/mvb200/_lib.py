@@ -8,7 +8,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("MVB200_LIB") or os.path.join(_HERE, "libmvb200.so")   # override: A/B two builds on one box
 
-MVB_KV_BF16, MVB_KV_FP32 = 0, 1
+MVB_KV_BF16, MVB_KV_FP32, MVB_KV_FP8 = 0, 1, 2
 MVB_OK, MVB_ERR_CUDA, MVB_ERR_ARG, MVB_ERR_PROMPT_TOO_LONG, MVB_ERR_UNSUPPORTED = 0, 1, 2, 3, 4
 GLOBAL_TENSORS, LAYER_TENSORS = 5, 7
 # `options` bits of the engine configs (include/mvb200.h): reference and identity paths, fixed at create time
@@ -199,6 +199,8 @@ SIGNATURES = {
                                    C.c_void_p, C.c_float, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     "mvb_f8_widen_test": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "mvb_s1_kv_f8_store_test": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_void_p]),
     "mvb_s1_arch_gemv_test": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                         C.c_float, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

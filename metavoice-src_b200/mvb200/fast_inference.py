@@ -11,6 +11,8 @@ contract (fast_inference.py:41-50, 111-119, 195).  Differences, all stated where
     checkpoint is available; the DeepFilterNet enhancer (fast_inference.py:158-163) is not implemented (N1);
   * the wav goes through the reference's ``audio_write`` post-processing (loudness normalisation to -14 LUFS, tanh
     compressor, PCM16; decoders.py:40-47) in mvb200/audio_out.py.
+Extension keywords: ``max_utts`` (KV slots of the stage-1 engine, the batch of ``synthesise_batch``) and ``kv_dtype``
+("bf16", the reference's cache; "fp8", e4m3 with one bf16 scale per head vector at half the cache bytes; "fp32").
 """
 from __future__ import annotations
 
@@ -70,7 +72,8 @@ class TTS:
     def __init__(self, model_name: str = "metavoiceio/metavoice-1B-v0.1", *, seed: int = 1337, output_dir: str = "outputs",
                  quantisation_mode: Optional[Literal["int4", "int8", "fp8"]] = None, first_stage_path: Optional[str] = None,
                  telemetry_origin: Optional[str] = None, encodec_state_dict=None, device: str = "cuda", max_utts: int = 1,
-                 mbd_checkpoint: Optional[dict] = None, mbd_settings=None):
+                 mbd_checkpoint: Optional[dict] = None, mbd_settings=None,
+                 kv_dtype: Literal["bf16", "fp32", "fp8"] = "bf16"):
         self._device = device
         self._model_dir = model_name
         if not os.path.isdir(model_name):
@@ -103,7 +106,7 @@ class TTS:
         self.model, self.tokenizer, self.smodel, self.model_size = build_model(
             precision=self.precision, checkpoint_path=Path(self._first_stage_ckpt),
             spk_emb_ckpt_path=Path(f"{self._model_dir}/speaker_encoder.pt"), device=device, compile=True,
-            compile_prefill=True, quantisation_mode=quantisation_mode, max_utts=max_utts)
+            compile_prefill=True, quantisation_mode=quantisation_mode, max_utts=max_utts, kv_dtype=kv_dtype)
         self._seed = seed
         spk_ckpt = f"{self._model_dir}/speaker_encoder.pt"
         if os.path.isfile(spk_ckpt):                                                   # fast_inference_utils.py:314-318

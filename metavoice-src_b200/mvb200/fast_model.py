@@ -74,6 +74,7 @@ _LAYER_KEYS = ["ln_1.weight", "attn.c_attn.weight", "attn.c_proj.weight", "ln_2.
                "mlp.swiglu.w1.weight", "mlp.swiglu.w3.weight", "mlp.c_proj.weight"]
 
 
+_KV_DTYPES = {"bf16": _lib.MVB_KV_BF16, "fp32": _lib.MVB_KV_FP32, "fp8": _lib.MVB_KV_FP8}
 _NORMS = {"rmsnorm": _lib.MVB_S1_NORM_RMS, "layernorm": _lib.MVB_S1_NORM_LAYER}
 _MLPS = {"swiglu": _lib.MVB_S1_MLP_SWIGLU, "gelu": _lib.MVB_S1_MLP_GELU}
 
@@ -215,11 +216,15 @@ class Transformer(Engine):
                      tensor_core_path: Union[None, bool, str] = None, unfused_sampler: Optional[bool] = None,
                      trace: Optional[bool] = None):
         """fast_model.py:136-148.  ``max_batch_size`` counts rows: 2 per utterance (CFG pair).
+        ``kv_dtype``: "bf16" (the reference's cache), "fp32" (validation) or "fp8" (e4m3 codes with one bf16 scale per head
+          vector, half the bytes; mvb200/quantize.py quantize_kv_fp8); any other string is a ValueError.
         Test / tool hooks, the engine's ``options`` (include/mvb200.h); any of them given creates a new engine:
           ``tensor_core_path``: True / "BC" = every engine path, False / "" = CUDA-core kernels only, "B" = tensor-core rows
             path without the resident decode kernel, "C" = resident decode kernel with CUDA-core prefill;
           ``unfused_sampler``: the resident kernel leaves the logits to k_sample;
           ``trace``: the resident kernel records per-phase clocks for mvb_s1_trace_fetch."""
+        if kv_dtype not in _KV_DTYPES:
+            raise ValueError(f"kv_dtype={kv_dtype!r}: expected one of {sorted(_KV_DTYPES)}")
         if (self._h is not None and self.max_seq_length >= max_seq_length and self.max_batch_size >= max_batch_size
                 and kv_dtype == self.kv_dtype and tensor_core_path is None and unfused_sampler is None and trace is None):
             return
@@ -240,7 +245,7 @@ class Transformer(Engine):
                    (_lib.MVB_S1_UNFUSED_SAMPLER if unfused_sampler else 0) | (_lib.MVB_S1_TRACE if trace else 0))
         cfg = _lib.S1Config(c.n_layer, c.n_head, c.head_dim, c.dim, c.intermediate_size, c.vocab_size, c.block_size,
                             c.speaker_emb_dim, c.norm_eps, self.max_utts,
-                            _lib.MVB_KV_FP32 if kv_dtype == "fp32" else _lib.MVB_KV_BF16, max_new or c.block_size, options)
+                            _KV_DTYPES[kv_dtype], max_new or c.block_size, options)
         self._cfg = cfg
         workspace_bytes, create = {None: (self._lib.mvb_s1_workspace_bytes, self._lib.mvb_s1_create),
                                    "int4": (self._lib.mvb_s1_int4_workspace_bytes, self._lib.mvb_s1_create_int4),

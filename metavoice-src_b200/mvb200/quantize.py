@@ -381,6 +381,29 @@ def pack_arena_fp8(state_dict: Dict[str, torch.Tensor], n_layer: int):
     return arena, offsets, payload
 
 
+def quantize_kv_fp8(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The fp8 KV cache's quantiser (``kv_dtype="fp8"``, include/mvb200.h at mvb_s1_kv_bytes): x [..., 128] fp32 head
+    vectors -> (codes float8_e4m3fn [..., 128], scales bf16 [...]) with, per vector,
+    ``s = bf16_rn(max(amax|x| / 448, FLT_EPSILON))`` and ``q = e4m3_rn(clamp(x / s, -448, 448))``: quantize_fp8_per_channel
+    without the bf16 rounding of the input.  Non-finite input has one encoding, which k_kv_store_f8 stores too: a NaN
+    anywhere in x gives s = NaN (bits 0x7fc0) and every code 0x7f; otherwise an infinite element makes s = +inf, its own
+    code 0x7f (inf / inf) and every finite element's a signed zero."""
+    xf = x.detach().to("cpu", torch.float32)
+    nan_row = torch.isnan(xf).any(-1)
+    amax = xf.abs().amax(-1)
+    s = torch.clamp(amax / E4M3_MAX, min=_FLT_EPS).to(torch.bfloat16)
+    r = xf / s.float()[..., None]
+    codes = torch.clamp(r, -E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn).view(torch.uint8)
+    codes = torch.where(torch.isnan(r) | nan_row[..., None], torch.full_like(codes, 0x7F), codes)
+    s = torch.where(nan_row, torch.full_like(s.view(torch.int16), 0x7FC0), s.view(torch.int16)).view(torch.bfloat16)
+    return codes.view(torch.float8_e4m3fn), s
+
+
+def dequantize_kv_fp8(codes: torch.Tensor, scales: torch.Tensor) -> torch.Tensor:
+    """fp32 s q of the fp8 KV cache, exactly (8 + 4 significant bits): codes [..., 128], scales [...]."""
+    return codes.float() * scales.float()[..., None]
+
+
 def fp8_dequantized_state_dict(state_dict: Dict[str, torch.Tensor], n_layer: int) -> Dict[str, torch.Tensor]:
     """The checkpoint with every Linear replaced by bf16_rn(s q): the bf16 model an fp8 engine equals when every scale is
     a power of two (and approximates to the rounding of s q otherwise)."""
