@@ -4,7 +4,7 @@
 //
 // fp8 matrix [M, K] (K % 256 == 0, M even; layout in include/mvb200.h, produced only by mvb200/quantize.py:pack_fp8_matrix):
 //   M * K e4m3 codes in the fragment-native order of f8_code_offset, then at the next 256-byte boundary bf16 [M] row
-//   scales s -- the int8 matrix layout, so the arena checks, k_tc_gemm's SCALED epilogue and W4Mats take it unchanged.
+//   scales s -- the int8 matrix layout, so the arena checks, k_tc_gemm's SCALED epilogue and WidenBatch take it unchanged.
 // Function (every kernel): y_j = s_j * sum_k x_k q_jk -- fp32 sums over the exact e4m3 values, the scale applied once per
 // output after the whole sum.
 #pragma once
@@ -281,7 +281,7 @@ __global__ void __launch_bounds__(256, 1) k_gemv_f8(GemvP p, S1State st, int n_u
 // Widen up to five fp8 matrices (one layer's wqkv, wo, w1, w3, w2, or lm_head / speaker_cond_pos once at create) to bf16
 // row-major [M, K] buffers holding q exactly, undoing the fragment-native order: the operand of the tensor-core GEMM,
 // whose epilogue applies the row scales.  One thread per 16 code bytes: one 128-bit load, eight 32-bit stores.
-__global__ void __launch_bounds__(256) k_f8_widen(W4Mats m) {
+__global__ void __launch_bounds__(256) k_f8_widen(WidenBatch m) {
   const size_t stride = (size_t)gridDim.x * blockDim.x;
 #pragma unroll
   for (int i = 0; i < 5; ++i) {

@@ -65,13 +65,6 @@ __device__ __forceinline__ void w4_dot32(const uint4& va, __nv_bfloat162 sza, co
   }
 }
 
-// Hint: bring [p, p + bytes) into L2 (one bulk request; the range is trimmed to whole 16-byte units inside it).
-__device__ __forceinline__ void l2_prefetch(const void* p, size_t bytes) {
-  const size_t a = reinterpret_cast<size_t>(p), lo = (a + 15) & ~(size_t)15, hi = (a + bytes) & ~(size_t)15;
-  if (hi > lo)
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(lo), "r"((unsigned)(hi - lo)) : "memory");
-}
-
 // ---------------------------------------------------------------------------------------------
 // k_gemv's contract (GemvP, the RMSNorm prologue, the four epilogues, gridDim.y = utterances) over int4 packed weights:
 // p.W (and p.W3 for EPI_SWIGLU) point at packed matrices.  A warp owns one item, as in k_gemv (rows 2i, 2i + 1, or w1 row
@@ -174,14 +167,7 @@ __global__ void __launch_bounds__(256, 2) k_gemv_w4(GemvP p, S1State st) {
 // Dequantise up to five packed matrices (one layer's wqkv, wo, w1, w3, w2) into bf16 row-major [M, K] buffers, the layout
 // of the bf16 arena, for the tensor-core GEMM of the prefill path.  One thread per 32 k of a row: one 128-bit nibble
 // load, one (scale, zero) fetch, four 128-bit stores.
-struct W4Mats {
-  const uint8_t* src[5];
-  __nv_bfloat16* dst[5];
-  int M[5], K[5];
-  int n;
-};
-
-__global__ void __launch_bounds__(256) k_w4_dequant(W4Mats m) {
+__global__ void __launch_bounds__(256) k_w4_dequant(WidenBatch m) {
   const size_t stride = (size_t)gridDim.x * blockDim.x;
 #pragma unroll
   for (int i = 0; i < 5; ++i) {

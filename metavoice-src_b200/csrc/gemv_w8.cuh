@@ -7,7 +7,6 @@
 // per output after the whole sum (== WeightOnlyInt8Linear.forward, F.linear(x, q) * s, fast_quantize.py:196-197).
 #pragma once
 #include "stage1_kernels.cuh"
-#include "gemv_w4.cuh"
 
 namespace mvb {
 
@@ -140,9 +139,7 @@ __global__ void __launch_bounds__(256, 2) k_gemv_w8(GemvP p, S1State st) {
 // Widen up to five int8 matrices (one layer's wqkv, wo, w1, w3, w2, or lm_head once at create) to bf16 row-major [M, K]
 // buffers holding q exactly (|q| <= 128 fits bf16's 8-bit significand), the operand of the tensor-core GEMM, whose
 // epilogue applies the row scales.  One thread per 16 k of a row: one 128-bit load, two 128-bit stores.
-using W8Mats = W4Mats;   // the same batch of up to five (int8 source, bf16 destination, M, K)
-
-__global__ void __launch_bounds__(256) k_w8_widen(W8Mats m) {
+__global__ void __launch_bounds__(256) k_w8_widen(WidenBatch m) {
   const size_t stride = (size_t)gridDim.x * blockDim.x;
 #pragma unroll
   for (int i = 0; i < 5; ++i) {

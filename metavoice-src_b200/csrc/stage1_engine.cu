@@ -125,7 +125,8 @@ static WsLayout make_layout(const mvb_s1_config& c) {
   return L;
 }
 
-// Per-layer norm parameters and Linear biases of a non-production architecture (null where it has none).
+// Per-layer norm parameters and Linear biases, null where the architecture has none (the production one: every beta and
+// bias).
 struct S1LayerP {
   const __nv_bfloat16 *g1, *b1, *g2, *b2;                   // ln_1 / ln_2 gain and (LayerNorm with bias) beta
   const __nv_bfloat16 *qkv_b, *o_b, *fc_b, *fc3_b, *proj_b;  // c_attn, attn.c_proj, c_fc | w1, w3, mlp.c_proj
@@ -164,17 +165,17 @@ struct mvb_s1 {
   std::vector<int> h_topk;                            // top_k of every utterance slot as installed by mvb_s1_begin
   std::vector<int> h_link;                            // SamplingDev::link of every slot as installed by mvb_s1_admit_guided
   size_t layer_stride_elems = 0;
-  // int4 engine: wqkv / wo / w1 / w3 / w2 are packed matrices; path A streams them through k_gemv_w4, path B dequantises
-  // one layer at a time into layer_scratch (bf16 [wqkv | wo | w1 | w3 | w2]).
-  // int8 engine: every Linear is an int8 matrix; path A streams them through k_gemv_w8, path B widens one layer's q at a
-  // time into layer_scratch (lm_head's once, at create, into w8_head) and k_tc_gemm applies the row scales.
-  // fp8 engine: every Linear is an fp8 matrix; path A streams them through k_gemv_f8 for up to F8_MAX_UTTS slots at once,
-  // path B widens them as the int8 engine does (k_f8_widen), speaker_cond_pos's once at create into f8_spk.
+  // int4 engine: wqkv / wo / w1 / w3 / w2 are packed matrices, lm_head stays bf16 (head_fmt).  int8 / fp8 engine: every
+  // Linear is an int8 / fp8 matrix.  Path A streams them through k_gemv_w4 / k_gemv_w8 / k_gemv_f8 (launch_gemv; the fp8
+  // GEMV serves up to F8_MAX_UTTS slots at once); path B widens one layer at a time into layer_scratch (bf16
+  // [wqkv | wo | w1 | w3 | w2]) with `widen`, lm_head's q once at create into w8_head and an fp8 engine's
+  // speaker_cond_pos q into f8_spk, and k_tc_gemm applies the int8 / fp8 row scales.
   WFmt fmt = WFmt::BF16;
   __nv_bfloat16* layer_scratch = nullptr;
   __nv_bfloat16* w8_head = nullptr;
   __nv_bfloat16* f8_spk = nullptr;
   bool row_scaled() const { return fmt == WFmt::INT8 || fmt == WFmt::FP8; }   // int8 / fp8 matrices with row scales
+  WFmt head_fmt() const { return fmt == WFmt::INT4 ? WFmt::BF16 : fmt; }
 
   template <typename T>
   T* wsp(size_t o) const { return reinterpret_cast<T*>(ws + o); }
@@ -320,6 +321,15 @@ static int s1_validate_arch(const mvb_s1_arch& a) {
   return MVB_OK;
 }
 
+// The matrices of m in format fmt (int4 packed, int8 or fp8) -> bf16 operands of the tensor-core GEMM.
+static cudaError_t widen(WFmt fmt, const WidenBatch& m, int n_sm, cudaStream_t s) {
+  if (fmt == WFmt::INT4) k_w4_dequant<<<4 * n_sm, 256, 0, s>>>(m);
+  else if (fmt == WFmt::INT8) k_w8_widen<<<4 * n_sm, 256, 0, s>>>(m);
+  else if (fmt == WFmt::FP8) k_f8_widen<<<4 * n_sm, 256, 0, s>>>(m);
+  else return cudaErrorInvalidValue;
+  return cudaGetLastError();
+}
+
 static int create_engine(const mvb_s1_config* cfg, const mvb_s1_arch* arch, const void* d_arena, size_t arena_bytes,
                          const uint64_t* offsets, void* d_kv, void* d_ws, mvb_s1** out, WFmt fmt) {
   if (int e = validate(cfg)) return e;
@@ -343,7 +353,7 @@ static int create_engine(const mvb_s1_config* cfg, const mvb_s1_arch* arch, cons
   h->n_sm = n_sm;
   h->arena = reinterpret_cast<const char*>(d_arena);
   h->off.assign(offsets, offsets + n_off);
-  if (!h->production_arch()) {
+  {
     const bool ln = h->layer_norm(), gelu = h->gelu();
     int nb = s1_offset_count(cfg, mvb_s1_arch{a.norm, a.mlp, 0});    // first bias slot
     auto bias_slot = [&](bool present) { return present && a.bias ? h->w(nb++) : nullptr; };
@@ -383,7 +393,7 @@ static int create_engine(const mvb_s1_config* cfg, const mvb_s1_arch* arch, cons
       // lm_head's q, widened once: the head GEMM of every prefill chunk reads it from here; an fp8 engine's
       // speaker_cond_pos q too, for k_spk_proj
       h->w8_head = h->wsp<__nv_bfloat16>(h->L.w8_head);
-      W8Mats m{};
+      WidenBatch m{};
       m.src[0] = reinterpret_cast<const uint8_t*>(h->w(4));
       m.dst[0] = h->w8_head;
       m.M[0] = cfg->vocab; m.K[0] = cfg->dim; m.n = 1;
@@ -392,11 +402,8 @@ static int create_engine(const mvb_s1_config* cfg, const mvb_s1_arch* arch, cons
         m.src[1] = reinterpret_cast<const uint8_t*>(h->w(2));
         m.dst[1] = h->f8_spk;
         m.M[1] = cfg->dim; m.K[1] = cfg->spk_dim; m.n = 2;
-        k_f8_widen<<<4 * n_sm, 256>>>(m);
-      } else {
-        k_w8_widen<<<4 * n_sm, 256>>>(m);
       }
-      MVB_CK(cudaGetLastError());
+      MVB_CK(widen(fmt, m, n_sm, 0));
       MVB_CK(cudaStreamSynchronize(0));
     }
   }
@@ -561,42 +568,34 @@ static cudaError_t launch_gemv_f8(mvb_s1* h, cudaStream_t s, int n_utts, const G
 }
 
 // p.W / p.W3 are matrices of format `fmt`: bf16 (k_gemv), int4 packed (k_gemv_w4), int8 (k_gemv_w8) or fp8 (k_gemv_f8);
-// the first three take one item per warp and one utterance per launch row.  LAYER (LayerNorm prologue) and BIASED (Linear
-// biases) exist for bf16 only.  A K whose staging rows need more than the default 48 KB of shared memory (a GELU c_proj,
-// K = 4 dim) opts the bf16 instance in first.
-template <int EPI, bool LAYER = false, bool BIASED = false>
-static cudaError_t launch_gemv(mvb_s1* h, cudaStream_t s, int n_utts, GemvP p, WFmt fmt) {
-  if constexpr (!LAYER && !BIASED && EPI != EPI_GELU) {
-    if (fmt == WFmt::FP8) return launch_gemv_f8<EPI>(h, s, n_utts, p);
-  }
+// the first three take one item per warp and one utterance per launch row.  The LayerNorm prologue (`layer`, p.gain set),
+// the Linear biases (p.bias set) and EPI_GELU exist for bf16 only.  A K whose staging rows need more than the default
+// 48 KB of shared memory (a GELU c_proj, K = 4 dim) opts the bf16 instance in first.
+template <int EPI>
+static cudaError_t launch_gemv(mvb_s1* h, cudaStream_t s, int n_utts, const GemvP& p, WFmt fmt, bool layer) {
+  const bool biased = p.bias != nullptr;
   const int n_items = (EPI == EPI_SWIGLU) ? p.M : p.M / 2;
-  dim3 grid(gemv_grid(n_items, h->n_sm), n_utts);
+  const dim3 grid(gemv_grid(n_items, h->n_sm), n_utts);
   const size_t smem = (size_t)2 * p.K * sizeof(float);
-  h->launches++;
-  if constexpr (!LAYER && !BIASED && EPI != EPI_GELU) {
-    if (fmt == WFmt::INT4) return launch_pdl(k_gemv_w4<EPI>, grid, dim3(256), smem, s, p, h->st);
-    if (fmt == WFmt::INT8) return launch_pdl(k_gemv_w8<EPI>, grid, dim3(256), smem, s, p, h->st);
+  if (fmt != WFmt::BF16) {
+    if constexpr (EPI != EPI_GELU) {
+      if (!layer && !biased) {
+        if (fmt == WFmt::FP8) return launch_gemv_f8<EPI>(h, s, n_utts, p);
+        h->launches++;
+        return launch_pdl(fmt == WFmt::INT4 ? k_gemv_w4<EPI> : k_gemv_w8<EPI>, grid, dim3(256), smem, s, p, h->st);
+      }
+    }
+    return cudaErrorInvalidValue;
   }
-  if (fmt != WFmt::BF16) return cudaErrorInvalidValue;
+  void (*k)(GemvP, S1State) = layer ? (biased ? k_gemv<EPI, true, true> : k_gemv<EPI, true, false>)
+                                    : (biased ? k_gemv<EPI, false, true> : k_gemv<EPI, false, false>);
+  h->launches++;
   if (smem > 48 * 1024) {
     if (smem > GEMV_MAX_SMEM) return cudaErrorInvalidValue;
-    const cudaError_t e = cudaFuncSetAttribute(k_gemv<EPI, LAYER, BIASED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
   }
-  return launch_pdl(k_gemv<EPI, LAYER, BIASED>, grid, dim3(256), smem, s, p, h->st);
-}
-
-// k_gemv of a non-production architecture: the LayerNorm prologue when `layer` (p.gain set), the biased epilogue when
-// p.bias is set.
-template <int EPI>
-static cudaError_t launch_gemv_arch(mvb_s1* h, cudaStream_t s, int n_utts, const GemvP& p, bool layer) {
-  const bool biased = p.bias != nullptr;
-  if (layer) {
-    if (biased) return launch_gemv<EPI, true, true>(h, s, n_utts, p, WFmt::BF16);
-    return launch_gemv<EPI, true, false>(h, s, n_utts, p, WFmt::BF16);
-  }
-  if (biased) return launch_gemv<EPI, false, true>(h, s, n_utts, p, WFmt::BF16);
-  return launch_gemv<EPI, false, false>(h, s, n_utts, p, WFmt::BF16);
+  return launch_pdl(k, grid, dim3(256), smem, s, p, h->st);
 }
 
 // Attention of path A over layer l: the two CFG rows of n_utts utterances at their decode positions.  An fp8 cache first
@@ -626,48 +625,15 @@ static int attn_decode(mvb_s1* h, cudaStream_t s, int n_utts, int l, const float
   return MVB_OK;
 }
 
-// Path A for one position of a non-production architecture (layers/combined.py:38-50 per layer, model.py:303 ln_f, the
-// tied head model.py:137-143): ln_1 -> c_attn (+ bias) + cache scatter, attention, c_proj (+ bias) + residual, ln_2 ->
-// SwiGLU or GELU MLP (+ biases), mlp.c_proj (+ bias) + residual; the norms are RMSNorm or LayerNorm (eps 1e-5, beta).
-static int launch_layers_arch(mvb_s1* h, cudaStream_t s, int n_utts, float* x, float* qkv, float* att, float* ffn) {
-  const mvb_s1_config& c = h->cfg;
-  const int D = c.dim, F = c.intermediate, H = c.n_head;
-  const bool ln = h->layer_norm();
-  const size_t half = h->kv_half_bytes();
-  for (int l = 0; l < c.n_layer; ++l) {
-    const S1LayerP& lp = h->lp[l];
-    char* kc = h->kv + (size_t)l * 2 * half;
-    char* vc = kc + half;
-    GemvP p{};
-    p.eps = h->norm_eps();
-    p.W = h->lw(l, 1); p.x = x; p.ldx = D; p.gain = lp.g1; p.beta = lp.b1; p.bias = lp.qkv_b;
-    p.out = qkv; p.ldo = 3 * D; p.M = 3 * D; p.K = D;
-    p.kcache = kc; p.vcache = vc; p.H = H; p.S_max = c.block_size; p.D = D; p.kv_fp32 = c.kv_dtype == MVB_KV_FP32;
-    MVB_CK(h->kv_f8() ? launch_gemv_arch<EPI_STORE>(h, s, n_utts, p, ln) : launch_gemv_arch<EPI_QKV>(h, s, n_utts, p, ln));
-    if (int e = attn_decode(h, s, n_utts, l, qkv, att)) return e;
-    p = GemvP{};
-    p.eps = h->norm_eps();
-    p.W = h->lw(l, 2); p.x = att; p.ldx = D; p.bias = lp.o_b; p.out = x; p.ldo = D; p.M = D; p.K = D;
-    MVB_CK(launch_gemv_arch<EPI_RESID>(h, s, n_utts, p, false));
-    p.W = h->lw(l, 4); p.x = x; p.ldx = D; p.gain = lp.g2; p.beta = lp.b2; p.bias = lp.fc_b; p.out = ffn; p.ldo = F; p.M = F;
-    p.K = D;
-    if (h->gelu()) {
-      MVB_CK(launch_gemv_arch<EPI_GELU>(h, s, n_utts, p, ln));
-    } else {
-      p.W3 = h->lw(l, 5); p.bias3 = lp.fc3_b;
-      MVB_CK(launch_gemv_arch<EPI_SWIGLU>(h, s, n_utts, p, ln));
-    }
-    p = GemvP{};
-    p.W = h->lw(l, 6); p.x = ffn; p.ldx = F; p.bias = lp.proj_b; p.out = x; p.ldo = D; p.M = D; p.K = F;
-    MVB_CK(launch_gemv_arch<EPI_RESID>(h, s, n_utts, p, false));
-  }
-  return MVB_OK;
-}
-
-// One forward position for `n_utts` logical utterances: embed -> 24 x (attention, FFN) -> head.
+// One forward position for `n_utts` logical utterances (layers/combined.py:38-50 per layer, model.py:303 ln_f, the tied
+// head model.py:137-143): embed, then per layer ln_1 -> c_attn (+ bias) + cache scatter, attention, c_proj (+ bias) +
+// residual, ln_2 -> SwiGLU or GELU MLP (+ biases), mlp.c_proj (+ bias) + residual; then ln_f -> head.  The norms are
+// RMSNorm or LayerNorm (eps 1e-5, beta); the production architecture is RMSNorm, SwiGLU and no bias.
 static int launch_body(mvb_s1* h, cudaStream_t s, int n_utts) {
   const mvb_s1_config& c = h->cfg;
   const int D = c.dim, F = c.intermediate, V = c.vocab, H = c.n_head;
+  const bool ln = h->layer_norm();
+  const float eps = h->norm_eps();
   float* x = h->wsp<float>(h->L.x);
   float* qkv = h->wsp<float>(h->L.qkv);
   float* att = h->wsp<float>(h->L.att);
@@ -676,43 +642,46 @@ static int launch_body(mvb_s1* h, cudaStream_t s, int n_utts) {
   MVB_CK(launch_pdl(k_embed, dim3(2, n_utts), dim3(256), 0, s, h->st, h->w(0), h->w(1),
                 (const float*)h->wsp<float>(h->L.spk), x, D));
   h->launches++;
-  if (!h->production_arch()) {
-    if (int e = launch_layers_arch(h, s, n_utts, x, qkv, att, ffn)) return e;
-    GemvP p{};
-    p.eps = h->norm_eps();
-    p.W = h->w(4); p.x = x; p.ldx = D; p.gain = h->w(3); p.beta = h->lnf_b; p.out = logits; p.ldo = V; p.M = V; p.K = D;
-    MVB_CK(launch_gemv_arch<EPI_STORE>(h, s, n_utts, p, h->layer_norm()));
-    return MVB_OK;
-  }
   const size_t half = h->kv_half_bytes();
   for (int l = 0; l < c.n_layer; ++l) {
+    const S1LayerP& lp = h->lp[l];
     char* kc = h->kv + (size_t)l * 2 * half;
     char* vc = kc + half;
+    // ln_1 + c_attn + cache scatter (fp8 cache: the qkv rows only)
     GemvP p{};
-    p.eps = c.norm_eps;
-    // attention_norm + wqkv + cache scatter (fp8 cache: the qkv rows only)
-    p.W = h->lw(l, 1); p.W3 = nullptr; p.x = x; p.ldx = D; p.gain = h->lw(l, 0);
+    p.eps = eps;
+    p.W = h->lw(l, 1); p.x = x; p.ldx = D; p.gain = lp.g1; p.beta = lp.b1; p.bias = lp.qkv_b;
     p.out = qkv; p.ldo = 3 * D; p.M = 3 * D; p.K = D;
     p.kcache = kc; p.vcache = vc; p.H = H; p.S_max = c.block_size; p.D = D; p.kv_fp32 = c.kv_dtype == MVB_KV_FP32;
-    MVB_CK(h->kv_f8() ? launch_gemv<EPI_STORE>(h, s, n_utts, p, h->fmt) : launch_gemv<EPI_QKV>(h, s, n_utts, p, h->fmt));
+    MVB_CK(h->kv_f8() ? launch_gemv<EPI_STORE>(h, s, n_utts, p, h->fmt, ln) : launch_gemv<EPI_QKV>(h, s, n_utts, p, h->fmt, ln));
     // attention over [0, pos]
     if (int e = attn_decode(h, s, n_utts, l, qkv, att)) return e;
-    // wo + residual
+    // c_proj + residual
     p = GemvP{};
-    p.eps = c.norm_eps;
-    p.W = h->lw(l, 2); p.x = att; p.ldx = D; p.gain = nullptr; p.out = x; p.ldo = D; p.M = D; p.K = D;
-    MVB_CK(launch_gemv<EPI_RESID>(h, s, n_utts, p, h->fmt));
-    // ffn_norm + silu(w1 x) * w3 x
-    p.W = h->lw(l, 4); p.W3 = h->lw(l, 5); p.x = x; p.ldx = D; p.gain = h->lw(l, 3); p.out = ffn; p.ldo = F; p.M = F; p.K = D;
-    MVB_CK(launch_gemv<EPI_SWIGLU>(h, s, n_utts, p, h->fmt));
-    // w2 + residual
-    p.W = h->lw(l, 6); p.W3 = nullptr; p.x = ffn; p.ldx = F; p.gain = nullptr; p.out = x; p.ldo = D; p.M = D; p.K = F;
-    MVB_CK(launch_gemv<EPI_RESID>(h, s, n_utts, p, h->fmt));
+    p.eps = eps;
+    p.W = h->lw(l, 2); p.x = att; p.ldx = D; p.bias = lp.o_b; p.out = x; p.ldo = D; p.M = D; p.K = D;
+    MVB_CK(launch_gemv<EPI_RESID>(h, s, n_utts, p, h->fmt, false));
+    // ln_2 + GELU(c_fc x) or silu(w1 x) * w3 x
+    p = GemvP{};
+    p.eps = eps;
+    p.W = h->lw(l, 4); p.x = x; p.ldx = D; p.gain = lp.g2; p.beta = lp.b2; p.bias = lp.fc_b; p.out = ffn; p.ldo = F; p.M = F;
+    p.K = D;
+    if (h->gelu()) {
+      MVB_CK(launch_gemv<EPI_GELU>(h, s, n_utts, p, h->fmt, ln));
+    } else {
+      p.W3 = h->lw(l, 5); p.bias3 = lp.fc3_b;
+      MVB_CK(launch_gemv<EPI_SWIGLU>(h, s, n_utts, p, h->fmt, ln));
+    }
+    // mlp.c_proj + residual
+    p = GemvP{};
+    p.eps = eps;
+    p.W = h->lw(l, 6); p.x = ffn; p.ldx = F; p.bias = lp.proj_b; p.out = x; p.ldo = D; p.M = D; p.K = F;
+    MVB_CK(launch_gemv<EPI_RESID>(h, s, n_utts, p, h->fmt, false));
   }
   GemvP p{};
-  p.eps = c.norm_eps;
-  p.W = h->w(4); p.x = x; p.ldx = D; p.gain = h->w(3); p.out = logits; p.ldo = V; p.M = V; p.K = D;
-  MVB_CK(launch_gemv<EPI_STORE>(h, s, n_utts, p, h->fmt == WFmt::INT4 ? WFmt::BF16 : h->fmt));   // int4: lm_head is bf16
+  p.eps = eps;
+  p.W = h->w(4); p.x = x; p.ldx = D; p.gain = h->w(3); p.beta = h->lnf_b; p.out = logits; p.ldo = V; p.M = V; p.K = D;
+  MVB_CK(launch_gemv<EPI_STORE>(h, s, n_utts, p, h->head_fmt(), ln));
   return MVB_OK;
 }
 
@@ -800,25 +769,6 @@ static int qkv_attn_rows(mvb_s1* h, cudaStream_t s, int R, int l, const LinB& a,
   return MVB_OK;
 }
 
-// One layer of a non-production architecture on the tensor cores: the projections of launch_layers_arch with the
-// LayerNorm prologue of k_prep_b<true> and the BIASED / G_GELU epilogues of k_tc_gemm.
-static int layer_b_arch(mvb_s1* h, cudaStream_t s, int R, int l, float* x, float* qkv, float* att, float* ffn) {
-  const int D = h->cfg.dim, F = h->cfg.intermediate;
-  const S1LayerP& p = h->lp[l];
-  LinB a{x, D, p.g1, l * 5 + 0, l * 5 + 0, 3 * D, D, qkv, 3 * D};
-  a.beta = p.b1; a.bias = p.qkv_b;
-  if (int e = qkv_attn_rows(h, s, R, l, a, qkv, att)) return e;
-  a = LinB{att, D, nullptr, l * 5 + 1, l * 5 + 1, D, D, x, D};
-  a.bias = p.o_b;
-  if (int e = linear_b<G_RESID>(h, s, R, a)) return e;
-  a = LinB{x, D, p.g2, l * 5 + 2, l * 5 + 3, F, D, ffn, F};
-  a.beta = p.b2; a.bias = p.fc_b; a.bias3 = p.fc3_b;
-  if (int e = h->gelu() ? linear_b<G_GELU>(h, s, R, a) : linear_b<G_SWIGLU>(h, s, R, a)) return e;
-  a = LinB{ffn, F, nullptr, l * 5 + 4, l * 5 + 4, D, F, x, D};
-  a.bias = p.proj_b;
-  return linear_b<G_RESID>(h, s, R, a);
-}
-
 // The final norm and the head of path B over R rows of x: y = ln_f(x) . lm_head^T into out [R, vocab].
 static int head_b(mvb_s1* h, cudaStream_t s, int R, const float* x, float* out) {
   const mvb_s1_config& c = h->cfg;
@@ -828,7 +778,8 @@ static int head_b(mvb_s1* h, cudaStream_t s, int R, const float* x, float* out) 
   return linear_b<G_STORE>(h, s, R, a);
 }
 
-// embed + all layers for the R rows described by h->rows (already filled on the device)
+// embed + all layers for the R rows described by h->rows (already filled on the device): path A's projections with the
+// LayerNorm prologue of k_prep_b<true> and the BIASED / G_GELU / SCALED epilogues of k_tc_gemm.
 static int launch_layers_b(mvb_s1* h, cudaStream_t s, int R) {
   const mvb_s1_config& c = h->cfg;
   const int D = c.dim, F = c.intermediate;
@@ -841,7 +792,7 @@ static int launch_layers_b(mvb_s1* h, cudaStream_t s, int R) {
   MVB_CK(cudaGetLastError());
   for (int l = 0; l < c.n_layer; ++l) {
     if (h->fmt != WFmt::BF16) {   // this layer's W_deq (int4) or q (int8, fp8) -> the scratch the tensor maps of every layer point at
-      W4Mats m{};   // == W8Mats
+      WidenBatch m{};
       const int ts[5] = {1, 2, 4, 5, 6};
       for (int i = 0; i < 5; ++i) {
         const Mk mk = layer_mk(c, ts[i]);
@@ -850,26 +801,22 @@ static int launch_layers_b(mvb_s1* h, cudaStream_t s, int R) {
         m.M[i] = mk.M; m.K[i] = mk.K;
       }
       m.n = 5;
-      if (h->fmt == WFmt::INT4) {
-        k_w4_dequant<<<4 * h->n_sm, 256, 0, s>>>(m);
-      } else if (h->fmt == WFmt::FP8) {
-        k_f8_widen<<<4 * h->n_sm, 256, 0, s>>>(m);
-      } else {
-        k_w8_widen<<<4 * h->n_sm, 256, 0, s>>>(m);
-      }
       h->launches++;
-      MVB_CK(cudaGetLastError());
+      MVB_CK(widen(h->fmt, m, h->n_sm, s));
     }
-    if (!h->production_arch()) {   // the layer of a non-production architecture (path A's launch_layers_arch)
-      if (int e = layer_b_arch(h, s, R, l, x, qkv, att, ffn)) return e;
-      continue;
-    }
-    if (int e = qkv_attn_rows(h, s, R, l, LinB{x, D, h->lw(l, 0), l * 5 + 0, l * 5 + 0, 3 * D, D, qkv, 3 * D, h->tc_lscale(l, 1)},
-                              qkv, att)) return e;
-    if (int e = linear_b<G_RESID>(h, s, R, LinB{att, D, nullptr, l * 5 + 1, l * 5 + 1, D, D, x, D, h->tc_lscale(l, 2)})) return e;
-    if (int e = linear_b<G_SWIGLU>(h, s, R, LinB{x, D, h->lw(l, 3), l * 5 + 2, l * 5 + 3, F, D, ffn, F, h->tc_lscale(l, 4),
-                                                  h->tc_lscale(l, 5)})) return e;
-    if (int e = linear_b<G_RESID>(h, s, R, LinB{ffn, F, nullptr, l * 5 + 4, l * 5 + 4, D, F, x, D, h->tc_lscale(l, 6)})) return e;
+    const S1LayerP& p = h->lp[l];
+    LinB a{x, D, p.g1, l * 5 + 0, l * 5 + 0, 3 * D, D, qkv, 3 * D, h->tc_lscale(l, 1)};
+    a.beta = p.b1; a.bias = p.qkv_b;
+    if (int e = qkv_attn_rows(h, s, R, l, a, qkv, att)) return e;
+    a = LinB{att, D, nullptr, l * 5 + 1, l * 5 + 1, D, D, x, D, h->tc_lscale(l, 2)};
+    a.bias = p.o_b;
+    if (int e = linear_b<G_RESID>(h, s, R, a)) return e;
+    a = LinB{x, D, p.g2, l * 5 + 2, l * 5 + 3, F, D, ffn, F, h->tc_lscale(l, 4), h->tc_lscale(l, 5)};
+    a.beta = p.b2; a.bias = p.fc_b; a.bias3 = p.fc3_b;
+    if (int e = h->gelu() ? linear_b<G_GELU>(h, s, R, a) : linear_b<G_SWIGLU>(h, s, R, a)) return e;
+    a = LinB{ffn, F, nullptr, l * 5 + 4, l * 5 + 4, D, F, x, D, h->tc_lscale(l, 6)};
+    a.bias = p.proj_b;
+    if (int e = linear_b<G_RESID>(h, s, R, a)) return e;
   }
   return MVB_OK;
 }
@@ -1503,9 +1450,38 @@ extern "C" int mvb_s1_generate(mvb_s1* h, int32_t n_utts, const int32_t* prompts
 }
 
 // ------------------------------------------------------------------------------------------------
-// Test hooks of the int4, int8 and fp8 kernels (include/mvb200.h): k_gemv_w4<epi> / k_gemv_w8<epi> / k_gemv_f8<epi>
-// exactly as path A launches them, over a caller-built decode state (slot map and positions), k_w4_dequant / k_w8_widen /
-// k_f8_widen on one matrix.
+// Test hooks of the path-A GEMVs (include/mvb200.h): k_gemv / k_gemv_w4 / k_gemv_w8 / k_gemv_f8 with epilogue epi exactly
+// as path A launches them, over a caller-built decode state (slot map and positions).  The caller checks the arguments.
+static int gemv_test(WFmt fmt, int32_t epi, bool layer, const void* d_W, const void* d_W3, const void* d_bias,
+                     const void* d_bias3, int32_t M, int32_t K, const float* d_x, int32_t ldx, int32_t n_utts,
+                     const void* d_gain, const void* d_beta, float eps, float* d_out, int32_t ldo, void* d_kcache,
+                     void* d_vcache, const int32_t* d_slot_map, const int32_t* d_pos, int32_t H, int32_t S_max, int32_t D,
+                     int32_t kv_fp32, cudaStream_t s) {
+  mvb_s1 h{};
+  int dev = 0;
+  if (int e = current_device(&dev, &h.n_sm)) return e;
+  h.st.slot_map = const_cast<int*>(d_slot_map);
+  h.st.pos = const_cast<int*>(d_pos);
+  GemvP p{};
+  p.W = reinterpret_cast<const __nv_bfloat16*>(d_W); p.W3 = reinterpret_cast<const __nv_bfloat16*>(d_W3);
+  p.x = d_x; p.ldx = ldx; p.gain = reinterpret_cast<const __nv_bfloat16*>(d_gain); p.eps = eps;
+  p.beta = reinterpret_cast<const __nv_bfloat16*>(d_beta);
+  p.bias = reinterpret_cast<const __nv_bfloat16*>(d_bias);
+  p.bias3 = epi == EPI_SWIGLU ? reinterpret_cast<const __nv_bfloat16*>(d_bias3) : nullptr;
+  p.out = d_out; p.ldo = ldo; p.M = M; p.K = K;
+  p.kcache = d_kcache; p.vcache = d_vcache; p.H = H; p.S_max = S_max; p.D = D; p.kv_fp32 = kv_fp32;
+  switch (epi) {
+    case EPI_STORE: MVB_CK(launch_gemv<EPI_STORE>(&h, s, n_utts, p, fmt, layer)); break;
+    case EPI_RESID: MVB_CK(launch_gemv<EPI_RESID>(&h, s, n_utts, p, fmt, layer)); break;
+    case EPI_SWIGLU: MVB_CK(launch_gemv<EPI_SWIGLU>(&h, s, n_utts, p, fmt, layer)); break;
+    case EPI_QKV: MVB_CK(launch_gemv<EPI_QKV>(&h, s, n_utts, p, fmt, layer)); break;
+    default: MVB_CK(launch_gemv<EPI_GELU>(&h, s, n_utts, p, fmt, layer)); break;
+  }
+  MVB_CK(cudaStreamSynchronize(s));
+  return MVB_OK;
+}
+
+// The int4, int8 and fp8 GEMVs.
 static int quant_gemv_test(WFmt fmt, int32_t epi, const void* d_W, const void* d_W3, int32_t M, int32_t K, const float* d_x,
                            int32_t ldx, int32_t n_utts, const void* d_gain, float eps, float* d_out, int32_t ldo,
                            void* d_kcache, void* d_vcache, const int32_t* d_slot_map, const int32_t* d_pos, int32_t H,
@@ -1518,25 +1494,8 @@ static int quant_gemv_test(WFmt fmt, int32_t epi, const void* d_W, const void* d
   if (fmt == WFmt::FP8 && ldx % 2) return set_error(MVB_ERR_ARG, "ldx=%d must be even", ldx);
   if (epi == EPI_SWIGLU && !d_W3) return set_error(MVB_ERR_ARG, "SwiGLU needs W3");
   if (epi == EPI_QKV && (!d_kcache || !d_vcache || M != 3 * D || D != 128 * H)) return set_error(MVB_ERR_ARG, "bad QKV arguments");
-  mvb_s1 h{};
-  int dev = 0;
-  if (int e = current_device(&dev, &h.n_sm)) return e;
-  h.st.slot_map = const_cast<int*>(d_slot_map);
-  h.st.pos = const_cast<int*>(d_pos);
-  GemvP p{};
-  p.W = reinterpret_cast<const __nv_bfloat16*>(d_W); p.W3 = reinterpret_cast<const __nv_bfloat16*>(d_W3);
-  p.x = d_x; p.ldx = ldx; p.gain = reinterpret_cast<const __nv_bfloat16*>(d_gain); p.eps = eps;
-  p.out = d_out; p.ldo = ldo; p.M = M; p.K = K;
-  p.kcache = d_kcache; p.vcache = d_vcache; p.H = H; p.S_max = S_max; p.D = D; p.kv_fp32 = kv_fp32;
-  cudaStream_t s = (cudaStream_t)stream;
-  switch (epi) {
-    case EPI_STORE: MVB_CK(launch_gemv<EPI_STORE>(&h, s, n_utts, p, fmt)); break;
-    case EPI_RESID: MVB_CK(launch_gemv<EPI_RESID>(&h, s, n_utts, p, fmt)); break;
-    case EPI_SWIGLU: MVB_CK(launch_gemv<EPI_SWIGLU>(&h, s, n_utts, p, fmt)); break;
-    default: MVB_CK(launch_gemv<EPI_QKV>(&h, s, n_utts, p, fmt)); break;
-  }
-  MVB_CK(cudaStreamSynchronize(s));
-  return MVB_OK;
+  return gemv_test(fmt, epi, false, d_W, d_W3, nullptr, nullptr, M, K, d_x, ldx, n_utts, d_gain, nullptr, eps, d_out, ldo,
+                   d_kcache, d_vcache, d_slot_map, d_pos, H, S_max, D, kv_fp32, (cudaStream_t)stream);
 }
 
 extern "C" int mvb_w4_gemv_test(int32_t epi, const void* d_W, const void* d_W3, int32_t M, int32_t K, const float* d_x,
@@ -1563,52 +1522,32 @@ extern "C" int mvb_f8_gemv_test(int32_t epi, const void* d_W, const void* d_W3, 
                          d_slot_map, d_pos, H, S_max, D, kv_fp32, stream);
 }
 
-extern "C" int mvb_w4_dequant_test(const void* d_W, int32_t M, int32_t K, void* d_out, void* stream) {
+// k_w4_dequant / k_w8_widen / k_f8_widen on one matrix (an fp8 matrix has an even M).
+static int widen_test(WFmt fmt, const void* d_W, int32_t M, int32_t K, void* d_out, void* stream) {
   if (!d_W || !d_out) return set_error(MVB_ERR_ARG, "null argument");
-  if (M < 1 || K < 256 || K % 256) return set_error(MVB_ERR_ARG, "bad shape M=%d K=%d", M, K);
-  W4Mats m{};
+  if (M < 1 || (fmt == WFmt::FP8 && M % 2) || K < 256 || K % 256) return set_error(MVB_ERR_ARG, "bad shape M=%d K=%d", M, K);
+  WidenBatch m{};
   m.src[0] = reinterpret_cast<const uint8_t*>(d_W);
   m.dst[0] = reinterpret_cast<__nv_bfloat16*>(d_out);
   m.M[0] = M; m.K[0] = K; m.n = 1;
   int dev = 0, n_sm = 0;
   if (int e = current_device(&dev, &n_sm)) return e;
   cudaStream_t s = (cudaStream_t)stream;
-  k_w4_dequant<<<4 * n_sm, 256, 0, s>>>(m);
-  MVB_CK(cudaGetLastError());
+  MVB_CK(widen(fmt, m, n_sm, s));
   MVB_CK(cudaStreamSynchronize(s));
   return MVB_OK;
+}
+
+extern "C" int mvb_w4_dequant_test(const void* d_W, int32_t M, int32_t K, void* d_out, void* stream) {
+  return widen_test(WFmt::INT4, d_W, M, K, d_out, stream);
 }
 
 extern "C" int mvb_w8_widen_test(const void* d_W, int32_t M, int32_t K, void* d_out, void* stream) {
-  if (!d_W || !d_out) return set_error(MVB_ERR_ARG, "null argument");
-  if (M < 1 || K < 256 || K % 256) return set_error(MVB_ERR_ARG, "bad shape M=%d K=%d", M, K);
-  W8Mats m{};
-  m.src[0] = reinterpret_cast<const uint8_t*>(d_W);
-  m.dst[0] = reinterpret_cast<__nv_bfloat16*>(d_out);
-  m.M[0] = M; m.K[0] = K; m.n = 1;
-  int dev = 0, n_sm = 0;
-  if (int e = current_device(&dev, &n_sm)) return e;
-  cudaStream_t s = (cudaStream_t)stream;
-  k_w8_widen<<<4 * n_sm, 256, 0, s>>>(m);
-  MVB_CK(cudaGetLastError());
-  MVB_CK(cudaStreamSynchronize(s));
-  return MVB_OK;
+  return widen_test(WFmt::INT8, d_W, M, K, d_out, stream);
 }
 
 extern "C" int mvb_f8_widen_test(const void* d_W, int32_t M, int32_t K, void* d_out, void* stream) {
-  if (!d_W || !d_out) return set_error(MVB_ERR_ARG, "null argument");
-  if (M < 2 || M % 2 || K < 256 || K % 256) return set_error(MVB_ERR_ARG, "bad shape M=%d K=%d", M, K);
-  W4Mats m{};
-  m.src[0] = reinterpret_cast<const uint8_t*>(d_W);
-  m.dst[0] = reinterpret_cast<__nv_bfloat16*>(d_out);
-  m.M[0] = M; m.K[0] = K; m.n = 1;
-  int dev = 0, n_sm = 0;
-  if (int e = current_device(&dev, &n_sm)) return e;
-  cudaStream_t s = (cudaStream_t)stream;
-  k_f8_widen<<<4 * n_sm, 256, 0, s>>>(m);
-  MVB_CK(cudaGetLastError());
-  MVB_CK(cudaStreamSynchronize(s));
-  return MVB_OK;
+  return widen_test(WFmt::FP8, d_W, M, K, d_out, stream);
 }
 
 // Test hook of the fp8 KV store (include/mvb200.h): k_kv_store_f8 as path B launches it, over R caller-described rows.
@@ -1689,27 +1628,6 @@ extern "C" int mvb_s1_arch_gemv_test(int32_t path, int32_t epi, int32_t norm, co
   }
   if (K < 256 || K % 256 || M < 2 || M % 2 || (size_t)2 * K * sizeof(float) > GEMV_MAX_SMEM)
     return set_error(MVB_ERR_UNSUPPORTED, "mvb_s1_arch_gemv_test: bad GEMV shape M=%d K=%d", M, K);
-  mvb_s1 h{};
-  int dev = 0;
-  if (int e = current_device(&dev, &h.n_sm)) return e;
-  h.st.slot_map = const_cast<int*>(d_slot_map);
-  h.st.pos = const_cast<int*>(d_pos);
-  GemvP p{};
-  p.W = reinterpret_cast<const __nv_bfloat16*>(d_W); p.W3 = reinterpret_cast<const __nv_bfloat16*>(d_W3);
-  p.x = d_x; p.ldx = ldx; p.gain = reinterpret_cast<const __nv_bfloat16*>(d_gain); p.eps = eps;
-  p.beta = reinterpret_cast<const __nv_bfloat16*>(d_beta);
-  p.bias = reinterpret_cast<const __nv_bfloat16*>(d_bias);
-  p.bias3 = epi == EPI_SWIGLU ? reinterpret_cast<const __nv_bfloat16*>(d_bias3) : nullptr;
-  p.out = d_out; p.ldo = ldo; p.M = M; p.K = K;
-  p.kcache = d_kcache; p.vcache = d_vcache; p.H = H; p.S_max = S_max; p.D = D; p.kv_fp32 = kv_fp32;
-  const bool ln = norm == 2;
-  switch (epi) {
-    case EPI_STORE: MVB_CK(launch_gemv_arch<EPI_STORE>(&h, s, n_utts, p, ln)); break;
-    case EPI_RESID: MVB_CK(launch_gemv_arch<EPI_RESID>(&h, s, n_utts, p, ln)); break;
-    case EPI_SWIGLU: MVB_CK(launch_gemv_arch<EPI_SWIGLU>(&h, s, n_utts, p, ln)); break;
-    case EPI_QKV: MVB_CK(launch_gemv_arch<EPI_QKV>(&h, s, n_utts, p, ln)); break;
-    default: MVB_CK(launch_gemv_arch<EPI_GELU>(&h, s, n_utts, p, ln)); break;
-  }
-  MVB_CK(cudaStreamSynchronize(s));
-  return MVB_OK;
+  return gemv_test(WFmt::BF16, epi, norm == 2, d_W, d_W3, d_bias, d_bias3, M, K, d_x, ldx, n_utts, d_gain, d_beta, eps, d_out,
+                   ldo, d_kcache, d_vcache, d_slot_map, d_pos, H, S_max, D, kv_fp32, s);
 }

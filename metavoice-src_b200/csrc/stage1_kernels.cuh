@@ -387,6 +387,24 @@ __global__ void __launch_bounds__(256, 2) k_gemv(GemvP p, S1State st) {
 }
 
 // ---------------------------------------------------------------------------------------------
+// Shared by the int4, int8 and fp8 kernels (gemv_w4.cuh, gemv_w8.cuh, gemv_f8.cuh).
+// Hint: bring [p, p + bytes) into L2 (one bulk request; the range is trimmed to whole 16-byte units inside it).
+__device__ __forceinline__ void l2_prefetch(const void* p, size_t bytes) {
+  const size_t a = reinterpret_cast<size_t>(p), lo = (a + 15) & ~(size_t)15, hi = (a + bytes) & ~(size_t)15;
+  if (hi > lo)
+    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(lo), "r"((unsigned)(hi - lo)) : "memory");
+}
+
+// Up to five quantised matrices (one layer's wqkv, wo, w1, w3, w2, or lm_head / speaker_cond_pos once at create) and their
+// bf16 row-major [M, K] destinations: the batch k_w4_dequant, k_w8_widen and k_f8_widen turn into tensor-core GEMM operands.
+struct WidenBatch {
+  const uint8_t* src[5];
+  __nv_bfloat16* dst[5];
+  int M[5], K[5];
+  int n;
+};
+
+// ---------------------------------------------------------------------------------------------
 // Decode attention: softmax(q K^T / sqrt(128) + causal mask) V over cache slots [0, pos]
 // (fast_model.py:220-224 with the mask row of :148,151).  The reference attends to all 2048 slots
 // through a boolean mask; masked slots carry exactly zero weight, so reading only [0, pos] is

@@ -119,12 +119,7 @@ class Transformer(Engine):
 
     def __init__(self, config: ModelArgs, arena: torch.Tensor, offsets: List[int], device="cuda",
                  quantisation_mode: Optional[str] = None):
-        if quantisation_mode not in (None, "int4", "int8", "fp8"):
-            raise NotImplementedError(f"quantisation_mode={quantisation_mode!r} is not implemented (only None, 'int4', 'int8' "
-                                      "and 'fp8')")
-        if quantisation_mode is not None and not config.production_arch:
-            raise NotImplementedError(f"quantisation_mode={quantisation_mode!r} is implemented for the production architecture "
-                                      "(rmsnorm, swiglu, no bias) only")
+        self._check_mode(config, quantisation_mode)
         super().__init__(device, arena, offsets)
         self.config = config
         self.quantisation_mode = quantisation_mode
@@ -135,6 +130,15 @@ class Transformer(Engine):
         self.kv_dtype = "bf16"
 
     # ---- construction ------------------------------------------------------------------------
+    @staticmethod
+    def _check_mode(config: ModelArgs, quantisation_mode: Optional[str]) -> None:
+        if quantisation_mode not in (None, "int4", "int8", "fp8"):
+            raise NotImplementedError(f"quantisation_mode={quantisation_mode!r} is not implemented (only None, 'int4', 'int8' "
+                                      "and 'fp8')")
+        if quantisation_mode is not None and not config.production_arch:
+            raise NotImplementedError(f"quantisation_mode={quantisation_mode!r} is implemented for the production architecture "
+                                      "(rmsnorm, swiglu, no bias) only")
+
     @classmethod
     def from_name(cls, name: str):
         raise RuntimeError("mvb200.Transformer holds device weights; use Transformer.from_state_dict(...)")
@@ -150,23 +154,11 @@ class Transformer(Engine):
         larger decode batch) widens one layer's q at a time as int8 does.
         ``config``'s norm_type / nonlinearity_type / bias select the architecture (mvb_s1_create_ex); only the production
         one takes a quantisation mode."""
-        if quantisation_mode is not None and not config.production_arch:
-            raise NotImplementedError(f"quantisation_mode={quantisation_mode!r} is implemented for the production architecture "
-                                      "(rmsnorm, swiglu, no bias) only")
-        if quantisation_mode == "int4":
-            from .quantize import pack_arena_int4
-            arena, offsets, _ = pack_arena_int4(state_dict, config.n_layer)
-        elif quantisation_mode == "int8":
-            from .quantize import pack_arena_int8
-            arena, offsets, _ = pack_arena_int8(state_dict, config.n_layer)
-        elif quantisation_mode == "fp8":
-            from .quantize import pack_arena_fp8
-            arena, offsets, _ = pack_arena_fp8(state_dict, config.n_layer)
-        elif quantisation_mode is None:
-            arena, offsets = pack_arena(state_dict, config.n_layer, config)
-        else:
-            raise NotImplementedError(f"quantisation_mode={quantisation_mode!r} is not implemented (only None, 'int4', 'int8' "
-                                      "and 'fp8')")
+        cls._check_mode(config, quantisation_mode)   # before the weights are quantised
+        from . import quantize as Q
+        pack = {None: lambda sd, n: pack_arena(sd, n, config), "int4": Q.pack_arena_int4, "int8": Q.pack_arena_int8,
+                "fp8": Q.pack_arena_fp8}[quantisation_mode]
+        arena, offsets = pack(state_dict, config.n_layer)[:2]
         return cls(config, arena, offsets, device, quantisation_mode)
 
     @staticmethod

@@ -261,10 +261,10 @@ def unpack_int8_matrix(buf: torch.Tensor, M: int, K: int) -> Tuple[torch.Tensor,
     return q, buf[so:so + 2 * M].clone().view(torch.bfloat16)
 
 
-def pack_arena_int8(state_dict: Dict[str, torch.Tensor], n_layer: int):
-    """Checkpoint state dict -> (uint8 arena, byte offsets, payload bytes).  Every Linear weight is an int8 matrix (its
-    offset points at the int8 block); embeddings and norms are the bf16 tensors.  The payload is the reference's
-    ``model_size`` of the int8 model: int8 weights plus bf16 scales plus the bf16 tensors."""
+def _pack_arena_per_channel(state_dict: Dict[str, torch.Tensor], n_layer: int, quantise, pack):
+    """Checkpoint state dict -> (uint8 arena, byte offsets, payload bytes).  Every Linear weight w becomes the one-byte
+    matrix pack(*quantise(w)) (its offset points at the code block); embeddings and norms are the bf16 tensors.  The
+    payload is the reference's ``model_size``: one byte per weight plus the bf16 scales plus the bf16 tensors."""
     sd = _strip(state_dict)
     blobs: List[torch.Tensor] = []
     payload = 0
@@ -273,8 +273,8 @@ def pack_arena_int8(state_dict: Dict[str, torch.Tensor], n_layer: int):
             raise KeyError(f"checkpoint is missing {k}")
         t = sd[k].detach()
         if linear:
-            q, s = quantize_per_channel(t)
-            blobs.append(pack_int8_matrix(q, s))
+            q, s = quantise(t)
+            blobs.append(pack(q, s))
             payload += q.numel() + 2 * s.numel()
         else:
             t = t.to(torch.bfloat16)
@@ -284,15 +284,26 @@ def pack_arena_int8(state_dict: Dict[str, torch.Tensor], n_layer: int):
     return arena, offsets, payload
 
 
-def int8_dequantized_state_dict(state_dict: Dict[str, torch.Tensor], n_layer: int) -> Dict[str, torch.Tensor]:
-    """The checkpoint with every Linear replaced by bf16_rn(s q): the bf16 model an int8 engine equals when every scale is
-    a power of two (and approximates to the rounding of s q otherwise)."""
+def _per_channel_dequantized_state_dict(state_dict: Dict[str, torch.Tensor], n_layer: int, quantise, dequantise):
+    """The checkpoint with every Linear w replaced by dequantise(*quantise(w))."""
     sd = _strip(state_dict)
     out = dict(sd)
     for k, linear, _ in _keys(n_layer):
         if linear:
-            out[k] = dequantize_int8(*quantize_per_channel(sd[k]))
+            out[k] = dequantise(*quantise(sd[k]))
     return out
+
+
+def pack_arena_int8(state_dict: Dict[str, torch.Tensor], n_layer: int):
+    """Checkpoint state dict -> (uint8 arena, byte offsets, payload bytes) with every Linear weight an int8 matrix
+    (_pack_arena_per_channel)."""
+    return _pack_arena_per_channel(state_dict, n_layer, quantize_per_channel, pack_int8_matrix)
+
+
+def int8_dequantized_state_dict(state_dict: Dict[str, torch.Tensor], n_layer: int) -> Dict[str, torch.Tensor]:
+    """The checkpoint with every Linear replaced by bf16_rn(s q): the bf16 model an int8 engine equals when every scale is
+    a power of two (and approximates to the rounding of s q otherwise)."""
+    return _per_channel_dequantized_state_dict(state_dict, n_layer, quantize_per_channel, dequantize_int8)
 
 
 # ---- weight-only fp8 (e4m3) -------------------------------------------------------------------------------------------
@@ -359,26 +370,9 @@ def unpack_fp8_matrix(buf: torch.Tensor, M: int, K: int) -> Tuple[torch.Tensor, 
 
 
 def pack_arena_fp8(state_dict: Dict[str, torch.Tensor], n_layer: int):
-    """Checkpoint state dict -> (uint8 arena, byte offsets, payload bytes).  Every Linear weight is an fp8 matrix (its
-    offset points at the code block); embeddings and norms are the bf16 tensors.  The payload counts one byte per weight,
-    the bf16 scales and the bf16 tensors, as for int8."""
-    sd = _strip(state_dict)
-    blobs: List[torch.Tensor] = []
-    payload = 0
-    for k, linear, _ in _keys(n_layer):
-        if k not in sd:
-            raise KeyError(f"checkpoint is missing {k}")
-        t = sd[k].detach()
-        if linear:
-            q, s = quantize_fp8_per_channel(t)
-            blobs.append(pack_fp8_matrix(q, s))
-            payload += q.numel() + 2 * s.numel()
-        else:
-            t = t.to(torch.bfloat16)
-            blobs.append(t)
-            payload += t.numel() * 2
-    arena, offsets = pack_arena_bytes(blobs)
-    return arena, offsets, payload
+    """Checkpoint state dict -> (uint8 arena, byte offsets, payload bytes) with every Linear weight an fp8 matrix
+    (_pack_arena_per_channel)."""
+    return _pack_arena_per_channel(state_dict, n_layer, quantize_fp8_per_channel, pack_fp8_matrix)
 
 
 def quantize_kv_fp8(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -407,9 +401,4 @@ def dequantize_kv_fp8(codes: torch.Tensor, scales: torch.Tensor) -> torch.Tensor
 def fp8_dequantized_state_dict(state_dict: Dict[str, torch.Tensor], n_layer: int) -> Dict[str, torch.Tensor]:
     """The checkpoint with every Linear replaced by bf16_rn(s q): the bf16 model an fp8 engine equals when every scale is
     a power of two (and approximates to the rounding of s q otherwise)."""
-    sd = _strip(state_dict)
-    out = dict(sd)
-    for k, linear, _ in _keys(n_layer):
-        if linear:
-            out[k] = dequantize_fp8(*quantize_fp8_per_channel(sd[k]))
-    return out
+    return _per_channel_dequantized_state_dict(state_dict, n_layer, quantize_fp8_per_channel, dequantize_fp8)
