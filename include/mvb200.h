@@ -123,6 +123,27 @@ typedef struct mvb_s1_arch {
 int mvb_s1_create_ex(const mvb_s1_config* cfg, const mvb_s1_arch* arch, const void* d_arena, size_t arena_bytes,
                      const uint64_t* offsets, void* d_kv, void* d_workspace, mvb_s1** out);
 
+/* Voices: last-N-block finetunes of the engine's checkpoint (fam/llm/finetune.py trains ln_f and the last
+ * last_n_blocks_to_finetune blocks and freezes the rest) served from one bf16 engine.  Voice 0 is the checkpoint the
+ * engine was created from; every other voice overlays blocks [first_layer, n_layer) and ln_f.
+ *   mvb_s1_add_voice  registers an overlay held in caller-owned device memory d_overlay (like the arena: it must outlive
+ *                     the handle).  `offsets` is a HOST array of byte offsets into it: for each overlaid layer, that
+ *                     layer's tensors in mvb_s1_create_ex's order (its weights; then, when arch->bias, its biases), then
+ *                     ln_f.weight and (LayerNorm with bias) ln_f.bias; n_offsets must be exactly that count.  Offsets
+ *                     are checked as the arena's are (16-byte aligned, inside the overlay).  *voice receives the id
+ *                     (1, 2, ...).  At most MVB_S1_MAX_VOICES voices, voice 0 included: past that, MVB_ERR_ARG.  An
+ *                     int4, int8 or fp8 engine returns MVB_ERR_UNSUPPORTED.
+ *   mvb_s1_set_voice  selects the voice of slot `utt`.  It takes effect at the slot's next admission (mvb_s1_admit,
+ *                     mvb_s1_admit_guided, mvb_s1_generate) or mvb_s1_begin; a prompt-guided companion always takes its
+ *                     primary's voice.  A new handle starts every slot on voice 0.
+ * A decode batch may mix voices; each slot computes exactly what an engine created from its voice's full checkpoint
+ * computes on the same path.  A burst whose slots are all on voice 0 is unchanged (resident decode kernel included);
+ * any other burst runs on the per-layer paths. */
+#define MVB_S1_MAX_VOICES 16
+int mvb_s1_add_voice(mvb_s1* h, const void* d_overlay, size_t overlay_bytes, int32_t first_layer, const uint64_t* offsets,
+                     int32_t n_offsets, int32_t* voice);
+int mvb_s1_set_voice(mvb_s1* h, int32_t utt, int32_t voice);
+
 /* Hoisted speaker conditioning: spk_proj[utt] = W_spk * spk_emb (fast_model.py:152-157 recomputes it
  * every step; it only changes per utterance).  d_spk_emb: fp32 [spk_dim] on device. */
 int mvb_s1_set_speaker(mvb_s1* h, int32_t utt, const float* d_spk_emb, void* stream);

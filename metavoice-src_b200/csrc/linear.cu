@@ -2,6 +2,7 @@
 // operator of the C ABI, y[R, M] (+)= f(x)[R, K] . W[M, K]^T with W in bf16, that tests use to check it in isolation.
 #include "host.cuh"
 #include "tc_gemm.cuh"
+#include "tc_gemm_grp.cuh"
 
 using namespace mvb;
 
@@ -72,6 +73,78 @@ cudaError_t tc_gemm(cudaStream_t s, const TcGemm& a) {
     case G_SWIGLU: return launch_tc_gemm<G_SWIGLU>(s, *a.tmW, tA3, *a.tmB, p, g, scaled, biased);
     case G_GELU: return launch_tc_gemm<G_GELU>(s, *a.tmW, tA3, *a.tmB, p, g, scaled, biased);
     default: return launch_tc_gemm<G_QKV>(s, *a.tmW, tA3, *a.tmB, p, g, scaled, biased);
+  }
+}
+
+template <int EPI, int NC, bool BIASED>
+static cudaError_t launch_grp_nc(cudaStream_t s, const CUtensorMap& tB, const GemmP& p, const GemmGrp& q, const GemmPlan& g,
+                                int units) {
+  static PerDeviceOnce attr_set;
+  if (attr_set.pending()) {
+    cudaError_t e = cudaFuncSetAttribute(k_tc_gemm_grp<EPI, NC, BIASED>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    if (e != cudaSuccess) return e;
+    attr_set.mark();
+  }
+  k_tc_gemm_grp<EPI, NC, BIASED><<<dim3(g.tiles, p.ksplit, units), GEMM_THREADS, g.smem_bytes, s>>>(tB, p, q);
+  return cudaGetLastError();
+}
+
+template <int EPI, bool BIASED>
+static cudaError_t launch_grp(cudaStream_t s, const CUtensorMap& tB, const GemmP& p, const GemmGrp& q, const GemmPlan& g,
+                             int units) {
+  if (p.Rpad <= 16) return launch_grp_nc<EPI, 2, BIASED>(s, tB, p, q, g, units);
+  if (p.Rpad <= 32) return launch_grp_nc<EPI, 4, BIASED>(s, tB, p, q, g, units);
+  if (p.Rpad <= 64) return launch_grp_nc<EPI, 8, BIASED>(s, tB, p, q, g, units);
+  return launch_grp_nc<EPI, 16, BIASED>(s, tB, p, q, g, units);
+}
+
+template <int EPI>
+static cudaError_t launch_grp_b(cudaStream_t s, const CUtensorMap& tB, const GemmP& p, const GemmGrp& q, const GemmPlan& g,
+                                int units, bool biased) {
+  return biased ? launch_grp<EPI, true>(s, tB, p, q, g, units) : launch_grp<EPI, false>(s, tB, p, q, g, units);
+}
+
+cudaError_t tc_gemm_grouped(cudaStream_t s, const TcGemm& a, const TcGemmGrp& g) {
+  if (a.Rpad < 16 || a.Rpad > 128 || a.Rpad % 16 || g.n_units < 1 || g.n_units > GEMM_MAX_GROUPS || !g.row_grp || !g.tickets)
+    return cudaErrorInvalidValue;
+  const bool biased = g.bias[0] != nullptr, normed = g.gain[0] != nullptr;
+  if (a.scale != nullptr || (a.layer_norm && !normed)) return cudaErrorInvalidValue;
+  const int NB = a.Rpad * (a.split_lo ? 2 : 1);
+  PrepGrp pg{};
+  pg.row_grp = g.row_grp;
+  for (int i = 0; i < GEMM_MAX_GROUPS; ++i) { pg.g2u[i] = g.prep_g2u[i]; pg.gain[i] = g.gain[i]; pg.beta[i] = g.beta[i]; }
+  if (a.layer_norm)
+    k_prep_b_grp<true><<<a.Rpad, 256, 0, s>>>(a.x, a.ldx, pg, a.eps, a.K, a.Rpad, a.R, a.split_lo ? 1 : 0, a.B);
+  else
+    k_prep_b_grp<false><<<a.Rpad, 256, 0, s>>>(a.x, a.ldx, pg, a.eps, a.K, a.Rpad, a.R, a.split_lo ? 1 : 0, a.B);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  GemmP p{};
+  p.M = a.M; p.K = a.K; p.NB = NB; p.Rpad = a.Rpad; p.R = a.R; p.split_lo = a.split_lo ? 1 : 0;
+  p.scratch = a.scratch; p.tickets = g.tickets; p.out = a.out; p.ldo = a.ldo;
+  p.kcache = a.kcache; p.vcache = a.vcache; p.row_cache = a.row_cache; p.row_pos = a.row_pos;
+  p.H = a.H; p.S_max = a.S_max; p.D = a.D; p.kv_fp32 = a.kv_fp32 ? 1 : 0;
+  // K split: the units share the SMs (every split of a tile waits for its siblings, so tiles x splits x units CTAs must
+  // be co-resident), and units x splits never exceed the ungrouped launch's splits (its scratch is what is reserved)
+  const bool sw = a.epi == G_SWIGLU;
+  const GemmPlan full = plan_gemm(a.M, a.K, NB, sw, a.n_sm);
+  const int per_unit = a.n_sm / g.n_units > 0 ? a.n_sm / g.n_units : 1;
+  const GemmPlan pl = plan_gemm(a.M, a.K, NB, sw, per_unit);
+  int ks = pl.ksplit < full.ksplit / g.n_units ? pl.ksplit : full.ksplit / g.n_units;
+  if (ks < 1 || pl.tiles > 128) ks = 1;
+  p.ksplit = ks;
+  p.stages = pl.stages;
+  GemmGrp q{};
+  q.row_grp = g.row_grp;
+  for (int i = 0; i < GEMM_MAX_GROUPS; ++i) {
+    q.g2u[i] = g.g2u[i]; q.tmA[i] = g.tmW[i]; q.tmA3[i] = sw ? g.tmW3[i] : g.tmW[i]; q.bias[i] = g.bias[i]; q.bias3[i] = g.bias3[i];
+  }
+  switch (a.epi) {
+    case G_STORE: return launch_grp_b<G_STORE>(s, *a.tmB, p, q, pl, g.n_units, biased);
+    case G_RESID: return launch_grp_b<G_RESID>(s, *a.tmB, p, q, pl, g.n_units, biased);
+    case G_SWIGLU: return launch_grp_b<G_SWIGLU>(s, *a.tmB, p, q, pl, g.n_units, biased);
+    case G_GELU: return launch_grp_b<G_GELU>(s, *a.tmB, p, q, pl, g.n_units, biased);
+    default: return launch_grp_b<G_QKV>(s, *a.tmB, p, q, pl, g.n_units, biased);
   }
 }
 

@@ -3,7 +3,9 @@
 #include <cuda_runtime.h>
 
 #include <cmath>
+#include <algorithm>
 #include <cstring>
+#include <deque>
 #include <map>
 #include <vector>
 
@@ -132,6 +134,46 @@ struct S1LayerP {
   const __nv_bfloat16 *qkv_b, *o_b, *fc_b, *fc3_b, *proj_b;  // c_attn, attn.c_proj, c_fc | w1, w3, mlp.c_proj
 };
 
+// A voice (mvb_s1_add_voice): the tensors of layers [first_layer, n_layer) and ln_f in an overlay; every other tensor is
+// the base checkpoint's.  Voice 0, the base, has first_layer = n_layer + 1, so that it uses the base ln_f too.
+struct S1Voice {
+  int first_layer = 0;
+  std::vector<const __nv_bfloat16*> t;   // 7 per overlaid layer, indexed like mvb_s1::lw's t (GELU: 5 unused)
+  std::vector<S1LayerP> lp;              // per overlaid layer
+  std::vector<CUtensorMap> tmW;          // 5 per overlaid layer, as mvb_s1::tmW
+  const __nv_bfloat16 *lnf_g = nullptr, *lnf_b = nullptr;
+};
+
+// The voice grouping of one batch of decode entries: groups in order of descending first_layer (voice 0 first), each
+// group's entries in batch order.  At any layer the groups still on the base weights are then a prefix of the order.
+struct VoicePlan {
+  int n = 0;                                    // groups
+  int voice[MVB_S1_MAX_VOICES];
+  int start[MVB_S1_MAX_VOICES + 1];             // group g = order[start[g] .. start[g + 1])
+  int grp[64];                                  // voice group of every batch entry
+};
+// Batch entries in group order, by value into k_voice_slots (captured into the step graph).
+struct VoiceOrder {
+  int entry[64];
+  int n;
+};
+// vslots[i] = slot_map[order.entry[i]]: the slot map of the grouped order, whose slices are the voice groups.
+__global__ void k_voice_slots(const int* __restrict__ slot_map, VoiceOrder order, int* __restrict__ vslots) {
+  const int i = threadIdx.x;
+  if (i < order.n) vslots[i] = slot_map[order.entry[i]];
+}
+// Path B with voice groups: row_grp[r] = voice group of decode row r (batch entry r / 2), for k_tc_gemm_grp.
+struct VoiceRows {
+  int grp[64];
+};
+__global__ void k_voice_rows(VoiceRows v, int R, int* __restrict__ row_grp) {
+  const int r = threadIdx.x;
+  if (r < R) row_grp[r] = v.grp[r >> 1];
+}
+
+// Step graphs keyed by a voice grouping are cached up to this many, oldest evicted first (see run_body).
+constexpr int VOICE_GRAPHS_MAX = 32;
+
 struct mvb_s1 {
   mvb_s1_config cfg;
   mvb_s1_arch arch{};                                 // all zero: the production architecture (rmsnorm, swiglu, no bias)
@@ -165,6 +207,19 @@ struct mvb_s1 {
   std::vector<int> h_topk;                            // top_k of every utterance slot as installed by mvb_s1_begin
   std::vector<int> h_link;                            // SamplingDev::link of every slot as installed by mvb_s1_admit_guided
   size_t layer_stride_elems = 0;
+  // voices: [0] is the base; next_voice is what mvb_s1_set_voice selected, slot_voice what the slot was admitted with
+  std::vector<S1Voice> voices;
+  std::vector<int> next_voice, slot_voice;
+  // device buffers of the first mvb_s1_add_voice: [64] k_voice_slots' grouped slot map, then [RB_MAX] k_voice_rows'
+  // row groups; split-K counters of the grouped GEMM; every voice's path-B tensor maps (voice_tm)
+  int* vslots = nullptr;
+  int* row_grp = nullptr;
+  unsigned* vtickets = nullptr;
+  CUtensorMap* d_tm = nullptr;
+  std::map<std::vector<int>, cudaGraphExec_t> vgraphs;   // {use_b, n_utts, voice of every entry} -> step graph
+  std::map<std::vector<int>, int> vgraph_nodes;
+  std::map<std::vector<int>, cudaEvent_t> vgraph_done;   // recorded after each launch of the graph
+  std::deque<std::vector<int>> vgraph_age;            // insertion order of vgraphs' keys
   // int4 engine: wqkv / wo / w1 / w3 / w2 are packed matrices, lm_head stays bf16 (head_fmt).  int8 / fp8 engine: every
   // Linear is an int8 / fp8 matrix.  Path A streams them through k_gemv_w4 / k_gemv_w8 / k_gemv_f8 (launch_gemv; the fp8
   // GEMV serves up to F8_MAX_UTTS slots at once); path B widens one layer at a time into layer_scratch (bf16
@@ -191,6 +246,24 @@ struct mvb_s1 {
     const bool g = gelu();
     return w(MVB_S1_GLOBAL_TENSORS + layer * (g ? 6 : MVB_S1_LAYER_TENSORS) + (g && t == 6 ? 5 : t));
   }
+  // The same for voice v: its overlay's tensor from its first_layer on, the base's below.
+  int first_layer(int v) const { return voices[v].first_layer; }
+  bool overlaid(int v, int layer) const { return layer >= voices[v].first_layer; }
+  const __nv_bfloat16* vlw(int v, int layer, int t) const {
+    return overlaid(v, layer) ? voices[v].t[(size_t)(layer - voices[v].first_layer) * 7 + t] : lw(layer, t);
+  }
+  const S1LayerP& vlp(int v, int layer) const { return overlaid(v, layer) ? voices[v].lp[layer - voices[v].first_layer] : lp[layer]; }
+  // tensor map i (0 wqkv, 1 wo, 2 w1, 3 w3, 4 w2) of a layer of voice v; layer n_layer: lm_head (shared by every voice)
+  const CUtensorMap* vtm(int v, int layer, int i) const {
+    if (layer < cfg.n_layer && overlaid(v, layer)) return &voices[v].tmW[(size_t)(layer - voices[v].first_layer) * 5 + i];
+    return &tmW[(size_t)layer * 5 + (layer < cfg.n_layer ? i : 0)];
+  }
+  // Device copy of vtm(v, layer, i): n_layer * 5 + 1 maps per voice (layer n_layer: lm_head)
+  const CUtensorMap* voice_tm(int v, int layer, int i) const {
+    return d_tm + (size_t)v * (cfg.n_layer * 5 + 1) + (size_t)layer * 5 + (layer < cfg.n_layer ? i : 0);
+  }
+  const __nv_bfloat16* lnf_gain(int v) const { return v ? voices[v].lnf_g : w(3); }
+  const __nv_bfloat16* lnf_beta(int v) const { return v ? voices[v].lnf_b : lnf_b; }
   // The one weight-source accessor of the tensor-core path: the bf16 matrix t (1 wqkv, 2 wo, 4 w1, 5 w3, 6 w2) of a layer,
   // i.e. the arena tensor, or for an int4 / int8 / fp8 engine its slot in the layer scratch (k_w4_dequant / k_w8_widen /
   // k_f8_widen fill it).
@@ -456,6 +529,10 @@ static int create_engine(const mvb_s1_config* cfg, const mvb_s1_arch* arch, cons
   }
   h->h_topk.assign(cfg->max_utts, 0);
   h->h_link.assign(cfg->max_utts, 0);
+  h->voices.resize(1);
+  h->voices[0].first_layer = cfg->n_layer + 1;
+  h->next_voice.assign(cfg->max_utts, 0);
+  h->slot_voice.assign(cfg->max_utts, 0);
   {
     // persistent decode kernel: needs a uniform layer stride (true for arenas packed in checkpoint order)
     const int D = cfg->dim, F = cfg->intermediate, V = cfg->vocab;
@@ -525,6 +602,11 @@ extern "C" int mvb_s1_create_fp8(const mvb_s1_config* cfg, const void* d_arena, 
 extern "C" int mvb_s1_destroy(mvb_s1* h) {
   if (!h) return MVB_OK;
   for (auto& kv : h->graphs) cudaGraphExecDestroy(kv.second);
+  for (auto& kv : h->vgraphs) cudaGraphExecDestroy(kv.second);
+  for (auto& kv : h->vgraph_done) cudaEventDestroy(kv.second);
+  if (h->vslots) cudaFree(h->vslots);
+  if (h->vtickets) cudaFree(h->vtickets);
+  if (h->d_tm) cudaFree(h->d_tm);
   if (h->cap_stream) cudaStreamDestroy(h->cap_stream);
   if (h->h_flags) cudaFreeHost(h->h_flags);
   delete h;
@@ -560,19 +642,22 @@ static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 // k_gemv_f8 over batch entries [0, n_utts): one launch row of up to F8_MAX_UTTS slots (gridDim.y > 1 only for a larger
 // batch on an engine without the rows path), one n8 block of MMA columns up to 4 slots, two above.
 template <int EPI>
-static cudaError_t launch_gemv_f8(mvb_s1* h, cudaStream_t s, int n_utts, const GemvP& p) {
+static cudaError_t launch_gemv_f8(mvb_s1* h, cudaStream_t s, int n_utts, const GemvP& p, const S1State& st) {
   const dim3 grid(f8_gemv_ctas((p.M + 15) / 16, h->n_sm), (n_utts + F8_MAX_UTTS - 1) / F8_MAX_UTTS);
   h->launches++;
-  if (n_utts > F8_MAX_UTTS / 2) return launch_pdl(k_gemv_f8<EPI, 2>, grid, dim3(256), 0, s, p, h->st, n_utts);
-  return launch_pdl(k_gemv_f8<EPI, 1>, grid, dim3(256), 0, s, p, h->st, n_utts);
+  if (n_utts > F8_MAX_UTTS / 2) return launch_pdl(k_gemv_f8<EPI, 2>, grid, dim3(256), 0, s, p, st, n_utts);
+  return launch_pdl(k_gemv_f8<EPI, 1>, grid, dim3(256), 0, s, p, st, n_utts);
 }
 
 // p.W / p.W3 are matrices of format `fmt`: bf16 (k_gemv), int4 packed (k_gemv_w4), int8 (k_gemv_w8) or fp8 (k_gemv_f8);
 // the first three take one item per warp and one utterance per launch row.  The LayerNorm prologue (`layer`, p.gain set),
 // the Linear biases (p.bias set) and EPI_GELU exist for bf16 only.  A K whose staging rows need more than the default
-// 48 KB of shared memory (a GELU c_proj, K = 4 dim) opts the bf16 instance in first.
+// 48 KB of shared memory (a GELU c_proj, K = 4 dim) opts the bf16 instance in first.  `st` (default: the engine's
+// decode state) supplies the slot map: batch entry i is slot st->slot_map[i].
 template <int EPI>
-static cudaError_t launch_gemv(mvb_s1* h, cudaStream_t s, int n_utts, const GemvP& p, WFmt fmt, bool layer) {
+static cudaError_t launch_gemv(mvb_s1* h, cudaStream_t s, int n_utts, const GemvP& p, WFmt fmt, bool layer,
+                               const S1State* st = nullptr) {
+  const S1State& state = st ? *st : h->st;
   const bool biased = p.bias != nullptr;
   const int n_items = (EPI == EPI_SWIGLU) ? p.M : p.M / 2;
   const dim3 grid(gemv_grid(n_items, h->n_sm), n_utts);
@@ -580,9 +665,9 @@ static cudaError_t launch_gemv(mvb_s1* h, cudaStream_t s, int n_utts, const Gemv
   if (fmt != WFmt::BF16) {
     if constexpr (EPI != EPI_GELU) {
       if (!layer && !biased) {
-        if (fmt == WFmt::FP8) return launch_gemv_f8<EPI>(h, s, n_utts, p);
+        if (fmt == WFmt::FP8) return launch_gemv_f8<EPI>(h, s, n_utts, p, state);
         h->launches++;
-        return launch_pdl(fmt == WFmt::INT4 ? k_gemv_w4<EPI> : k_gemv_w8<EPI>, grid, dim3(256), smem, s, p, h->st);
+        return launch_pdl(fmt == WFmt::INT4 ? k_gemv_w4<EPI> : k_gemv_w8<EPI>, grid, dim3(256), smem, s, p, state);
       }
     }
     return cudaErrorInvalidValue;
@@ -595,7 +680,7 @@ static cudaError_t launch_gemv(mvb_s1* h, cudaStream_t s, int n_utts, const Gemv
     const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
   }
-  return launch_pdl(k, grid, dim3(256), smem, s, p, h->st);
+  return launch_pdl(k, grid, dim3(256), smem, s, p, state);
 }
 
 // Attention of path A over layer l: the two CFG rows of n_utts utterances at their decode positions.  An fp8 cache first
@@ -625,11 +710,32 @@ static int attn_decode(mvb_s1* h, cudaStream_t s, int n_utts, int l, const float
   return MVB_OK;
 }
 
+// The weight sets of one layer (l == n_layer: ln_f and the head) over a voice-grouped batch: the leading groups still on
+// the base weights merge into one unit, every later group is a unit of its own.  Without a plan (every entry on voice
+// 0): one unit, the whole batch on the base weights.
+struct VUnit { int lo, hi, voice; };   // entries [lo, hi) of the grouped order
+static int voice_units(const mvb_s1* h, const VoicePlan* vp, int n, int l, VUnit* u) {
+  if (!vp) { u[0] = VUnit{0, n, 0}; return 1; }
+  int g = 0, k = 0;
+  while (g < vp->n && h->first_layer(vp->voice[g]) > l) ++g;
+  if (g > 0) u[k++] = VUnit{0, vp->start[g], 0};
+  for (; g < vp->n; ++g) u[k++] = VUnit{vp->start[g], vp->start[g + 1], vp->voice[g]};
+  return k;
+}
+
+// Path A's decode state for a unit: a slice of the grouped slot map, or the engine's own state for the whole batch.
+static S1State unit_state(const mvb_s1* h, const VUnit& u, int n) {
+  S1State st = h->st;
+  if (u.lo != 0 || u.hi != n) st.slot_map = h->vslots + u.lo;
+  return st;
+}
+
 // One forward position for `n_utts` logical utterances (layers/combined.py:38-50 per layer, model.py:303 ln_f, the tied
 // head model.py:137-143): embed, then per layer ln_1 -> c_attn (+ bias) + cache scatter, attention, c_proj (+ bias) +
 // residual, ln_2 -> SwiGLU or GELU MLP (+ biases), mlp.c_proj (+ bias) + residual; then ln_f -> head.  The norms are
-// RMSNorm or LayerNorm (eps 1e-5, beta); the production architecture is RMSNorm, SwiGLU and no bias.
-static int launch_body(mvb_s1* h, cudaStream_t s, int n_utts) {
+// RMSNorm or LayerNorm (eps 1e-5, beta); the production architecture is RMSNorm, SwiGLU and no bias.  With a voice
+// plan every projection runs once per unit (voice_units) over that unit's slots; the attention runs once for all.
+static int launch_body(mvb_s1* h, cudaStream_t s, int n_utts, const VoicePlan* vp = nullptr) {
   const mvb_s1_config& c = h->cfg;
   const int D = c.dim, F = c.intermediate, V = c.vocab, H = c.n_head;
   const bool ln = h->layer_norm();
@@ -643,45 +749,62 @@ static int launch_body(mvb_s1* h, cudaStream_t s, int n_utts) {
                 (const float*)h->wsp<float>(h->L.spk), x, D));
   h->launches++;
   const size_t half = h->kv_half_bytes();
+  VUnit us[MVB_S1_MAX_VOICES];
   for (int l = 0; l < c.n_layer; ++l) {
-    const S1LayerP& lp = h->lp[l];
     char* kc = h->kv + (size_t)l * 2 * half;
     char* vc = kc + half;
+    const int nu = voice_units(h, vp, n_utts, l, us);
     // ln_1 + c_attn + cache scatter (fp8 cache: the qkv rows only)
-    GemvP p{};
-    p.eps = eps;
-    p.W = h->lw(l, 1); p.x = x; p.ldx = D; p.gain = lp.g1; p.beta = lp.b1; p.bias = lp.qkv_b;
-    p.out = qkv; p.ldo = 3 * D; p.M = 3 * D; p.K = D;
-    p.kcache = kc; p.vcache = vc; p.H = H; p.S_max = c.block_size; p.D = D; p.kv_fp32 = c.kv_dtype == MVB_KV_FP32;
-    MVB_CK(h->kv_f8() ? launch_gemv<EPI_STORE>(h, s, n_utts, p, h->fmt, ln) : launch_gemv<EPI_QKV>(h, s, n_utts, p, h->fmt, ln));
+    for (int i = 0; i < nu; ++i) {
+      const int v = us[i].voice, n = us[i].hi - us[i].lo;
+      const S1LayerP& lp = h->vlp(v, l);
+      const S1State st = unit_state(h, us[i], n_utts);
+      GemvP p{};
+      p.eps = eps;
+      p.W = h->vlw(v, l, 1); p.x = x; p.ldx = D; p.gain = lp.g1; p.beta = lp.b1; p.bias = lp.qkv_b;
+      p.out = qkv; p.ldo = 3 * D; p.M = 3 * D; p.K = D;
+      p.kcache = kc; p.vcache = vc; p.H = H; p.S_max = c.block_size; p.D = D; p.kv_fp32 = c.kv_dtype == MVB_KV_FP32;
+      MVB_CK(h->kv_f8() ? launch_gemv<EPI_STORE>(h, s, n, p, h->fmt, ln, &st) : launch_gemv<EPI_QKV>(h, s, n, p, h->fmt, ln, &st));
+    }
     // attention over [0, pos]
     if (int e = attn_decode(h, s, n_utts, l, qkv, att)) return e;
-    // c_proj + residual
-    p = GemvP{};
-    p.eps = eps;
-    p.W = h->lw(l, 2); p.x = att; p.ldx = D; p.bias = lp.o_b; p.out = x; p.ldo = D; p.M = D; p.K = D;
-    MVB_CK(launch_gemv<EPI_RESID>(h, s, n_utts, p, h->fmt, false));
-    // ln_2 + GELU(c_fc x) or silu(w1 x) * w3 x
-    p = GemvP{};
-    p.eps = eps;
-    p.W = h->lw(l, 4); p.x = x; p.ldx = D; p.gain = lp.g2; p.beta = lp.b2; p.bias = lp.fc_b; p.out = ffn; p.ldo = F; p.M = F;
-    p.K = D;
-    if (h->gelu()) {
-      MVB_CK(launch_gemv<EPI_GELU>(h, s, n_utts, p, h->fmt, ln));
-    } else {
-      p.W3 = h->lw(l, 5); p.bias3 = lp.fc3_b;
-      MVB_CK(launch_gemv<EPI_SWIGLU>(h, s, n_utts, p, h->fmt, ln));
+    for (int i = 0; i < nu; ++i) {
+      const int v = us[i].voice, n = us[i].hi - us[i].lo;
+      const S1LayerP& lp = h->vlp(v, l);
+      const S1State st = unit_state(h, us[i], n_utts);
+      // c_proj + residual
+      GemvP p{};
+      p.eps = eps;
+      p.W = h->vlw(v, l, 2); p.x = att; p.ldx = D; p.bias = lp.o_b; p.out = x; p.ldo = D; p.M = D; p.K = D;
+      MVB_CK(launch_gemv<EPI_RESID>(h, s, n, p, h->fmt, false, &st));
+      // ln_2 + GELU(c_fc x) or silu(w1 x) * w3 x
+      p = GemvP{};
+      p.eps = eps;
+      p.W = h->vlw(v, l, 4); p.x = x; p.ldx = D; p.gain = lp.g2; p.beta = lp.b2; p.bias = lp.fc_b; p.out = ffn; p.ldo = F;
+      p.M = F; p.K = D;
+      if (h->gelu()) {
+        MVB_CK(launch_gemv<EPI_GELU>(h, s, n, p, h->fmt, ln, &st));
+      } else {
+        p.W3 = h->vlw(v, l, 5); p.bias3 = lp.fc3_b;
+        MVB_CK(launch_gemv<EPI_SWIGLU>(h, s, n, p, h->fmt, ln, &st));
+      }
+      // mlp.c_proj + residual
+      p = GemvP{};
+      p.eps = eps;
+      p.W = h->vlw(v, l, 6); p.x = ffn; p.ldx = F; p.bias = lp.proj_b; p.out = x; p.ldo = D; p.M = D; p.K = F;
+      MVB_CK(launch_gemv<EPI_RESID>(h, s, n, p, h->fmt, false, &st));
     }
-    // mlp.c_proj + residual
-    p = GemvP{};
-    p.eps = eps;
-    p.W = h->lw(l, 6); p.x = ffn; p.ldx = F; p.bias = lp.proj_b; p.out = x; p.ldo = D; p.M = D; p.K = F;
-    MVB_CK(launch_gemv<EPI_RESID>(h, s, n_utts, p, h->fmt, false));
   }
-  GemvP p{};
-  p.eps = eps;
-  p.W = h->w(4); p.x = x; p.ldx = D; p.gain = h->w(3); p.beta = h->lnf_b; p.out = logits; p.ldo = V; p.M = V; p.K = D;
-  MVB_CK(launch_gemv<EPI_STORE>(h, s, n_utts, p, h->head_fmt(), ln));
+  const int nu = voice_units(h, vp, n_utts, c.n_layer, us);
+  for (int i = 0; i < nu; ++i) {
+    const int v = us[i].voice;
+    const S1State st = unit_state(h, us[i], n_utts);
+    GemvP p{};
+    p.eps = eps;
+    p.W = h->w(4); p.x = x; p.ldx = D; p.gain = h->lnf_gain(v); p.beta = h->lnf_beta(v); p.out = logits; p.ldo = V; p.M = V;
+    p.K = D;
+    MVB_CK(launch_gemv<EPI_STORE>(h, s, us[i].hi - us[i].lo, p, h->head_fmt(), ln, &st));
+  }
   return MVB_OK;
 }
 
@@ -702,7 +825,7 @@ static const CUtensorMap* tmap_b(mvb_s1* h, int NB, int K) {
 
 struct LinB {
   const float* x; int ldx; const __nv_bfloat16* gain;  // input rows (+ optional norm gain: the architecture's norm)
-  int widx, widx3;                                     // tensor-map indices of W (and W3 for SwiGLU)
+  const CUtensorMap* tmW; const CUtensorMap* tmW3;     // tensor maps of W (and W3 for SwiGLU)
   int M, K;
   float* out; int ldo;
   const __nv_bfloat16* scale = nullptr;                // int8 / fp8 engine: row scales of W (and W3)
@@ -719,7 +842,7 @@ static int linear_b(mvb_s1* h, cudaStream_t s, int R, const LinB& a, void* kc = 
   g.epi = EPI; g.R = R; g.Rpad = (R + 15) / 16 * 16; g.split_lo = 1;   // activations as hi + lo bf16 terms
   g.tmB = tmap_b(h, 2 * g.Rpad, a.K);
   if (!g.tmB) return set_error(MVB_ERR_CUDA, "cuTensorMapEncodeTiled failed for the activation buffer");
-  g.tmW = &h->tmW[a.widx]; g.tmW3 = &h->tmW[a.widx3];
+  g.tmW = a.tmW; g.tmW3 = a.tmW3;
   g.B = h->wsp<__nv_bfloat16>(h->L.b_B);
   g.x = a.x; g.ldx = a.ldx; g.gain = a.gain; g.eps = c.norm_eps;
   if (a.gain != nullptr && h->layer_norm()) {   // LayerNorm (layers/layers.py:8-17): eps 1e-5, optional beta
@@ -738,10 +861,47 @@ static int linear_b(mvb_s1* h, cudaStream_t s, int R, const LinB& a, void* kc = 
   return MVB_OK;
 }
 
-// The qkv projection of path B (operands `a`) and the attention of the R rows of h->rows over layer l's cache.  An fp8
-// cache takes the new k / v from the stored qkv rows (G_STORE, then k_kv_store_f8) before the attention reads them: a
-// prefill chunk attends to its own positions.
-static int qkv_attn_rows(mvb_s1* h, cudaStream_t s, int R, int l, const LinB& a, const float* qkv, float* att) {
+// One projection of a voice-grouped decode batch (rows in batch order, h->row_grp filled by k_voice_rows): unit i of
+// `us` multiplies its rows by its weights (a[i]: tensor maps, norm gain / beta, biases; `dtm[i]` / `dtm3[i]`: the same
+// maps in device memory) in one grouped launch.  One unit is the ungrouped linear_b over every row.
+template <int EPI>
+static int linear_units(mvb_s1* h, cudaStream_t s, int R, const VoicePlan* vp, const VUnit* us, int nu, const LinB* a,
+                        const CUtensorMap* const* dtm, const CUtensorMap* const* dtm3, void* kc = nullptr, void* vc = nullptr) {
+  if (nu == 1) return linear_b<EPI>(h, s, R, a[0], kc, vc);
+  const mvb_s1_config& c = h->cfg;
+  TcGemm g{};
+  g.epi = EPI; g.R = R; g.Rpad = (R + 15) / 16 * 16; g.split_lo = 1;
+  g.tmB = tmap_b(h, 2 * g.Rpad, a[0].K);
+  if (!g.tmB) return set_error(MVB_ERR_CUDA, "cuTensorMapEncodeTiled failed for the activation buffer");
+  g.B = h->wsp<__nv_bfloat16>(h->L.b_B);
+  g.x = a[0].x; g.ldx = a[0].ldx; g.eps = c.norm_eps;
+  if (a[0].gain != nullptr && h->layer_norm()) { g.layer_norm = 1; g.eps = 1e-5f; }
+  g.M = a[0].M; g.K = a[0].K; g.out = a[0].out; g.ldo = a[0].ldo;
+  g.kcache = kc; g.vcache = vc; g.row_cache = h->rows.cache_row; g.row_pos = h->rows.pos;
+  g.H = c.n_head; g.S_max = c.block_size; g.D = c.dim; g.kv_fp32 = c.kv_dtype == MVB_KV_FP32;
+  g.scratch = h->wsp<float>(h->L.b_scratch);
+  g.n_sm = h->n_sm;
+  TcGemmGrp q{};
+  q.row_grp = h->row_grp;
+  q.tickets = h->vtickets;
+  q.n_units = nu;
+  for (int gi = 0; gi < vp->n; ++gi)
+    for (int i = 0; i < nu; ++i)
+      if (vp->start[gi] >= us[i].lo && vp->start[gi] < us[i].hi) q.g2u[gi] = q.prep_g2u[gi] = i;
+  for (int i = 0; i < nu; ++i) {
+    q.tmW[i] = dtm[i]; q.tmW3[i] = dtm3[i]; q.bias[i] = a[i].bias; q.bias3[i] = a[i].bias3;
+    q.gain[i] = a[i].gain; q.beta[i] = a[i].beta;
+  }
+  MVB_CK(tc_gemm_grouped(s, g, q));
+  h->launches += 2;   // k_prep_b_grp + k_tc_gemm_grp
+  return MVB_OK;
+}
+
+// The qkv projection of path B (operands a[i] of each unit) and the attention of the R rows of h->rows over layer l's
+// cache.  An fp8 cache takes the new k / v from the stored qkv rows (G_STORE, then k_kv_store_f8) before the attention
+// reads them: a prefill chunk attends to its own positions.
+static int qkv_attn_rows(mvb_s1* h, cudaStream_t s, int R, int l, const VoicePlan* vp, const VUnit* us, int nu, const LinB* a,
+                         const CUtensorMap* const* dtm, const float* qkv, float* att) {
   const mvb_s1_config& c = h->cfg;
   const int D = c.dim, H = c.n_head;
   char* kc = h->kv + (size_t)l * 2 * h->kv_half_bytes();
@@ -751,14 +911,14 @@ static int qkv_attn_rows(mvb_s1* h, cudaStream_t s, int R, int l, const LinB& a,
   unsigned* tk = h->wsp<unsigned>(h->L.b_att_tickets);
   dim3 ag(H, R, ATT_SPLITS);
   if (h->kv_f8()) {
-    if (int e = linear_b<G_STORE>(h, s, R, a)) return e;
+    if (int e = linear_units<G_STORE>(h, s, R, vp, us, nu, a, dtm, dtm)) return e;
     const KvF8 kv = h->kv_f8_layer(l);
     k_kv_store_f8<true><<<(2 * R * H + 7) / 8, 256, 0, s>>>(h->st, h->rows, R, qkv, kv, H, c.block_size, D);
     h->launches++;
     MVB_CK(cudaGetLastError());
     k_attn_rows_f8<<<ag, 128, 0, s>>>(h->rows, qkv, kv, po, pm, tk, att, H, c.block_size, D);
   } else {
-    if (int e = linear_b<G_QKV>(h, s, R, a, kc, vc)) return e;
+    if (int e = linear_units<G_QKV>(h, s, R, vp, us, nu, a, dtm, dtm, kc, vc)) return e;
     if (c.kv_dtype == MVB_KV_FP32)
       k_attn_rows<true><<<ag, 128, 0, s>>>(h->rows, qkv, kc, vc, po, pm, tk, att, H, c.block_size, D);
     else
@@ -769,18 +929,48 @@ static int qkv_attn_rows(mvb_s1* h, cudaStream_t s, int R, int l, const LinB& a,
   return MVB_OK;
 }
 
-// The final norm and the head of path B over R rows of x: y = ln_f(x) . lm_head^T into out [R, vocab].
-static int head_b(mvb_s1* h, cudaStream_t s, int R, const float* x, float* out) {
+// The final norm and the head of path B over R rows of x: y = ln_f(x) . lm_head^T into out [R, vocab].  A prefill runs on
+// one voice (`voice`); a voice-grouped decode batch (vp) normalises each row with its voice's ln_f and then runs ONE
+// GEMM over every row, since lm_head is shared by every voice.
+static int head_b(mvb_s1* h, cudaStream_t s, int R, const float* x, float* out, int voice = 0, const VoicePlan* vp = nullptr) {
   const mvb_s1_config& c = h->cfg;
-  const int hw = c.n_layer * 5;
-  LinB a{x, c.dim, h->w(3), hw, hw, c.vocab, c.dim, out, c.vocab, h->head_scale()};
-  a.beta = h->lnf_b;
-  return linear_b<G_STORE>(h, s, R, a);
+  if (!vp) {
+    const CUtensorMap* tm = h->vtm(voice, c.n_layer, 0);
+    LinB a{x, c.dim, h->lnf_gain(voice), tm, tm, c.vocab, c.dim, out, c.vocab, h->head_scale()};
+    a.beta = h->lnf_beta(voice);
+    return linear_b<G_STORE>(h, s, R, a);
+  }
+  TcGemm g{};
+  g.epi = G_STORE; g.R = R; g.Rpad = (R + 15) / 16 * 16; g.split_lo = 1;
+  g.tmB = tmap_b(h, 2 * g.Rpad, c.dim);
+  if (!g.tmB) return set_error(MVB_ERR_CUDA, "cuTensorMapEncodeTiled failed for the activation buffer");
+  g.B = h->wsp<__nv_bfloat16>(h->L.b_B);
+  g.x = x; g.ldx = c.dim; g.eps = c.norm_eps;
+  if (h->layer_norm()) { g.layer_norm = 1; g.eps = 1e-5f; }
+  g.M = c.vocab; g.K = c.dim; g.out = out; g.ldo = c.vocab;
+  g.scratch = h->wsp<float>(h->L.b_scratch);
+  g.n_sm = h->n_sm;
+  TcGemmGrp q{};
+  q.row_grp = h->row_grp;
+  q.tickets = h->vtickets;
+  q.n_units = 1;
+  q.tmW[0] = q.tmW3[0] = h->voice_tm(0, c.n_layer, 0);
+  for (int gi = 0; gi < vp->n; ++gi) {
+    q.prep_g2u[gi] = gi;
+    q.gain[gi] = h->lnf_gain(vp->voice[gi]);
+    q.beta[gi] = h->lnf_beta(vp->voice[gi]);
+  }
+  MVB_CK(tc_gemm_grouped(s, g, q));
+  h->launches += 2;
+  return MVB_OK;
 }
 
 // embed + all layers for the R rows described by h->rows (already filled on the device): path A's projections with the
-// LayerNorm prologue of k_prep_b<true> and the BIASED / G_GELU / SCALED epilogues of k_tc_gemm.
-static int launch_layers_b(mvb_s1* h, cudaStream_t s, int R) {
+// LayerNorm prologue of k_prep_b<true> and the BIASED / G_GELU / SCALED epilogues of k_tc_gemm.  A prefill runs on one
+// voice (`voice`).  A voice-grouped decode batch (vp, rows in batch order, row_grp filled) runs each projection as one
+// grouped launch over its units (voice_units): one unit, i.e. every layer below the lowest first_layer in the batch, is
+// the ungrouped launch.
+static int launch_layers_b(mvb_s1* h, cudaStream_t s, int R, int voice = 0, const VoicePlan* vp = nullptr) {
   const mvb_s1_config& c = h->cfg;
   const int D = c.dim, F = c.intermediate;
   float* x = h->wsp<float>(h->L.b_x);
@@ -790,6 +980,9 @@ static int launch_layers_b(mvb_s1* h, cudaStream_t s, int R) {
   k_embed_rows<<<R, 256, 0, s>>>(h->rows, h->w(0), h->w(1), h->wsp<float>(h->L.spk), x, D);
   h->launches++;
   MVB_CK(cudaGetLastError());
+  VUnit us[MVB_S1_MAX_VOICES];
+  LinB qa[MVB_S1_MAX_VOICES], oa[MVB_S1_MAX_VOICES], fa[MVB_S1_MAX_VOICES], pa[MVB_S1_MAX_VOICES];
+  const CUtensorMap* dt[5][MVB_S1_MAX_VOICES];
   for (int l = 0; l < c.n_layer; ++l) {
     if (h->fmt != WFmt::BF16) {   // this layer's W_deq (int4) or q (int8, fp8) -> the scratch the tensor maps of every layer point at
       WidenBatch m{};
@@ -804,31 +997,48 @@ static int launch_layers_b(mvb_s1* h, cudaStream_t s, int R) {
       h->launches++;
       MVB_CK(widen(h->fmt, m, h->n_sm, s));
     }
-    const S1LayerP& p = h->lp[l];
-    LinB a{x, D, p.g1, l * 5 + 0, l * 5 + 0, 3 * D, D, qkv, 3 * D, h->tc_lscale(l, 1)};
-    a.beta = p.b1; a.bias = p.qkv_b;
-    if (int e = qkv_attn_rows(h, s, R, l, a, qkv, att)) return e;
-    a = LinB{att, D, nullptr, l * 5 + 1, l * 5 + 1, D, D, x, D, h->tc_lscale(l, 2)};
-    a.bias = p.o_b;
-    if (int e = linear_b<G_RESID>(h, s, R, a)) return e;
-    a = LinB{x, D, p.g2, l * 5 + 2, l * 5 + 3, F, D, ffn, F, h->tc_lscale(l, 4), h->tc_lscale(l, 5)};
-    a.beta = p.b2; a.bias = p.fc_b; a.bias3 = p.fc3_b;
-    if (int e = h->gelu() ? linear_b<G_GELU>(h, s, R, a) : linear_b<G_SWIGLU>(h, s, R, a)) return e;
-    a = LinB{ffn, F, nullptr, l * 5 + 4, l * 5 + 4, D, F, x, D, h->tc_lscale(l, 6)};
-    a.bias = p.proj_b;
-    if (int e = linear_b<G_RESID>(h, s, R, a)) return e;
+    int nu = 1;
+    if (vp) nu = voice_units(h, vp, R / 2, l, us);
+    else us[0] = VUnit{0, R / 2, voice};
+    for (int i = 0; i < nu; ++i) {
+      const int v = us[i].voice;
+      const S1LayerP& p = h->vlp(v, l);
+      qa[i] = LinB{x, D, p.g1, h->vtm(v, l, 0), h->vtm(v, l, 0), 3 * D, D, qkv, 3 * D, h->tc_lscale(l, 1)};
+      qa[i].beta = p.b1; qa[i].bias = p.qkv_b;
+      oa[i] = LinB{att, D, nullptr, h->vtm(v, l, 1), h->vtm(v, l, 1), D, D, x, D, h->tc_lscale(l, 2)};
+      oa[i].bias = p.o_b;
+      fa[i] = LinB{x, D, p.g2, h->vtm(v, l, 2), h->vtm(v, l, 3), F, D, ffn, F, h->tc_lscale(l, 4), h->tc_lscale(l, 5)};
+      fa[i].beta = p.b2; fa[i].bias = p.fc_b; fa[i].bias3 = p.fc3_b;
+      pa[i] = LinB{ffn, F, nullptr, h->vtm(v, l, 4), h->vtm(v, l, 4), D, F, x, D, h->tc_lscale(l, 6)};
+      pa[i].bias = p.proj_b;
+      for (int t = 0; t < 5; ++t) dt[t][i] = nu > 1 ? h->voice_tm(v, l, t) : nullptr;
+    }
+    if (int e = qkv_attn_rows(h, s, R, l, vp, us, nu, qa, dt[0], qkv, att)) return e;
+    if (int e = linear_units<G_RESID>(h, s, R, vp, us, nu, oa, dt[1], dt[1])) return e;
+    if (int e = h->gelu() ? linear_units<G_GELU>(h, s, R, vp, us, nu, fa, dt[2], dt[2])
+                          : linear_units<G_SWIGLU>(h, s, R, vp, us, nu, fa, dt[2], dt[3]))
+      return e;
+    if (int e = linear_units<G_RESID>(h, s, R, vp, us, nu, pa, dt[4], dt[4])) return e;
   }
   return MVB_OK;
 }
 
-// batched decode position: rows from the decode state, logits land in the sampler's buffer
-static int launch_body_b(mvb_s1* h, cudaStream_t s, int n_utts) {
+// batched decode position: rows from the decode state (batch order), logits land in the sampler's buffer.  With a voice
+// plan, k_voice_rows first records each row's voice group for the grouped launches.
+static int launch_body_b(mvb_s1* h, cudaStream_t s, int n_utts, const VoicePlan* vp = nullptr) {
   const int R = 2 * n_utts;
   k_rows_decode<<<1, 128, 0, s>>>(h->st, h->rows, n_utts);
   h->launches++;
   MVB_CK(cudaGetLastError());
-  if (int e = launch_layers_b(h, s, R)) return e;
-  return head_b(h, s, R, h->wsp<float>(h->L.b_x), h->wsp<float>(h->L.logits));
+  if (vp) {
+    VoiceRows vr{};
+    for (int i = 0; i < n_utts; ++i) vr.grp[i] = vp->grp[i];
+    k_voice_rows<<<1, 128, 0, s>>>(vr, R, h->row_grp);
+    h->launches++;
+    MVB_CK(cudaGetLastError());
+  }
+  if (int e = launch_layers_b(h, s, R, 0, vp)) return e;
+  return head_b(h, s, R, h->wsp<float>(h->L.b_x), h->wsp<float>(h->L.logits), 0, vp);
 }
 
 
@@ -895,14 +1105,61 @@ static bool pc_att_fits(const mvb_s1* h, int n_utts) {
   return Z <= PC_MAX_CHUNKS && units_per_cta * ((TT + Z - 1) / Z) <= PC_MAX_TILES;
 }
 
+// Slots [0, n_utts) are all on voice 0: the only batches the resident decode kernel serves (it walks the base arena
+// with one uniform layer stride).
+static bool all_base_voice(const mvb_s1* h, int n_utts) {
+  for (int u = 0; u < n_utts; ++u)
+    if (h->slot_voice[u] != 0) return false;
+  return true;
+}
+
 // The persistent decode kernel serves the batch (else the per-layer path does).  CTA 2b alone writes batch entry b's
 // x rows and decode state back (decode_persistent.cuh, `owner`), so CTA 2 (n_utts - 1) must exist: pc_att_fits does not
 // imply it at a short block_size or a small width.
 static bool use_path_c(const mvb_s1* h, int n_utts) {
-  return h->path_c && h->pc_ok && 2 * n_utts <= PC_RPAD && 2 * n_utts - 1 <= h->n_sm && pc_att_fits(h, n_utts);
+  return h->path_c && h->pc_ok && 2 * n_utts <= PC_RPAD && 2 * n_utts - 1 <= h->n_sm && pc_att_fits(h, n_utts) &&
+         all_base_voice(h, n_utts);
 }
 
-static int run_body(mvb_s1* h, cudaStream_t s, int n_utts, bool allow_b = true) {
+// The voice plan of a batch: entry i is slot `utt` (a single-entry prefill position) or slot i (decode).  False, and no
+// plan, when every entry is on voice 0.  *order receives the entries in group order, *key the graph key.
+static bool voice_plan(const mvb_s1* h, int n_utts, int utt, bool use_b, VoicePlan* vp, VoiceOrder* order,
+                       std::vector<int>* key) {
+  std::vector<int> ev(n_utts);
+  bool any = false;
+  for (int i = 0; i < n_utts; ++i) {
+    ev[i] = h->slot_voice[utt >= 0 ? utt : i];
+    any = any || ev[i] != 0;
+  }
+  if (!any) return false;
+  std::vector<int> vs(ev.begin(), ev.end());
+  std::sort(vs.begin(), vs.end());
+  vs.erase(std::unique(vs.begin(), vs.end()), vs.end());
+  std::stable_sort(vs.begin(), vs.end(), [&](int a, int b) { return h->first_layer(a) > h->first_layer(b); });
+  vp->n = (int)vs.size();
+  order->n = 0;
+  for (int g = 0; g < vp->n; ++g) {
+    vp->voice[g] = vs[g];
+    vp->start[g] = order->n;
+    for (int i = 0; i < n_utts; ++i)
+      if (ev[i] == vs[g]) {
+        order->entry[order->n++] = i;
+        vp->grp[i] = g;
+      }
+  }
+  vp->start[vp->n] = order->n;
+  key->assign({use_b ? 1 : 0, n_utts});
+  key->insert(key->end(), ev.begin(), ev.end());
+  return true;
+}
+
+// One decode position of n_utts entries through a cached CUDA graph.  Batches whose entries are all on voice 0 are
+// keyed by size and path, as they always were.  Any other batch is keyed by its voice of every entry too, since the
+// grouping is part of the captured launches (path A's slot order and unit sizes, path B's row groups, every unit's
+// weights): at most
+// VOICE_GRAPHS_MAX such graphs are kept, the oldest destroyed first, so a batcher churning through voices holds at most
+// 2 max_utts base graphs + VOICE_GRAPHS_MAX voice graphs, and re-captures (one capture per new grouping) beyond that.
+static int run_body(mvb_s1* h, cudaStream_t s, int n_utts, bool allow_b = true, int utt = -1) {
   // Path A (CUDA-core GEMV) streams the weights once per utterance; from 2 utterances up the tensor-core
   // rows path streams them once per step for the whole batch.  slot_map must be the identity for path B
   // (its logits rows are batch-ordered), which mvb_s1_decode guarantees.  int4 / int8 decode: always path A.  fp8
@@ -910,6 +1167,51 @@ static int run_body(mvb_s1* h, cudaStream_t s, int n_utts, bool allow_b = true) 
   // path B, since one k_gemv_f8 launch row holds at most F8_MAX_UTTS slots (two n8 MMA blocks).
   const bool use_b = allow_b && h->path_b &&
                      ((h->fmt == WFmt::BF16 && n_utts >= 2) || (h->fmt == WFmt::FP8 && n_utts > F8_MAX_UTTS));
+  VoicePlan vp;
+  VoiceOrder order;
+  std::vector<int> vkey;
+  if (voice_plan(h, n_utts, utt, use_b, &vp, &order, &vkey)) {
+    auto body = [&](cudaStream_t st) -> int {
+      if (!use_b) {   // path A's units are slices of the grouped slot map; path B keeps the batch order
+        k_voice_slots<<<1, 64, 0, st>>>(h->st.slot_map, order, h->vslots);
+        h->launches++;
+        MVB_CK(cudaGetLastError());
+      }
+      return use_b ? launch_body_b(h, st, n_utts, &vp) : launch_body(h, st, n_utts, &vp);
+    };
+    auto it = h->vgraphs.find(vkey);
+    if (it == h->vgraphs.end()) {
+      if ((int)h->vgraphs.size() >= VOICE_GRAPHS_MAX) {
+        // the oldest graph's last launch (on whichever stream) must have finished before it is freed
+        const std::vector<int> old = h->vgraph_age.front();
+        h->vgraph_age.pop_front();
+        MVB_CK(cudaEventSynchronize(h->vgraph_done[old]));
+        cudaEventDestroy(h->vgraph_done[old]);
+        cudaGraphExecDestroy(h->vgraphs[old]);
+        h->vgraphs.erase(old);
+        h->vgraph_nodes.erase(old);
+        h->vgraph_done.erase(old);
+      }
+      const uint64_t before = h->launches;
+      cudaGraphExec_t ge;
+      const int e = capture_graph(h->cap_stream, &ge, body);
+      h->vgraph_nodes[vkey] = (int)(h->launches - before);
+      h->launches = before;
+      if (e) return e;
+      cudaEvent_t ev;
+      if (cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) {
+        cudaGraphExecDestroy(ge);
+        return set_error(MVB_ERR_CUDA, "cudaEventCreate failed");
+      }
+      it = h->vgraphs.emplace(vkey, ge).first;
+      h->vgraph_done[vkey] = ev;
+      h->vgraph_age.push_back(vkey);
+    }
+    MVB_CK(cudaGraphLaunch(it->second, s));
+    MVB_CK(cudaEventRecord(h->vgraph_done[vkey], s));
+    h->launches += h->vgraph_nodes[vkey];
+    return MVB_OK;
+  }
   auto body = [&](cudaStream_t st) { return use_b ? launch_body_b(h, st, n_utts) : launch_body(h, st, n_utts); };
   const int key = n_utts + (use_b ? 1000 : 0);
   auto it = h->graphs.find(key);
@@ -943,6 +1245,88 @@ static int check_slot(const mvb_s1* h, int32_t utt) {   // every caller-supplied
   return utt < 0 || utt >= h->cfg.max_utts ? set_error(MVB_ERR_ARG, "utterance slot %d out of range", utt) : MVB_OK;
 }
 
+// ------------------------------------------------------------------------------------------------
+// Voices (include/mvb200.h): overlays of blocks [first_layer, n_layer) and ln_f.
+extern "C" int mvb_s1_add_voice(mvb_s1* h, const void* d_overlay, size_t overlay_bytes, int32_t first_layer,
+                                const uint64_t* offsets, int32_t n_offsets, int32_t* voice) {
+  if (!h || !d_overlay || !offsets || !voice) return set_error(MVB_ERR_ARG, "null argument");
+  if (h->fmt != WFmt::BF16) return set_error(MVB_ERR_UNSUPPORTED, "voices are served by bf16-weight engines only");
+  const mvb_s1_config& c = h->cfg;
+  if (first_layer < 0 || first_layer >= c.n_layer)
+    return set_error(MVB_ERR_ARG, "first_layer %d outside [0, %d)", first_layer, c.n_layer);
+  if ((int)h->voices.size() >= MVB_S1_MAX_VOICES)
+    return set_error(MVB_ERR_ARG, "the engine already holds %d voices (MVB_S1_MAX_VOICES)", MVB_S1_MAX_VOICES);
+  const bool ln = h->layer_norm(), gelu = h->gelu(), bias = h->arch.bias != 0;
+  const int n_w = gelu ? 6 : MVB_S1_LAYER_TENSORS;
+  const int n_b = bias ? (ln ? 2 : 0) + 3 + (gelu ? 1 : 2) : 0;
+  const int n_ov = c.n_layer - first_layer;
+  const int want = n_ov * (n_w + n_b) + 1 + (bias && ln ? 1 : 0);
+  if (n_offsets != want)
+    return set_error(MVB_ERR_ARG, "an overlay from layer %d has %d tensors, got %d offsets", first_layer, want, n_offsets);
+  if (int e = check_offsets(offsets, (size_t)n_offsets, overlay_bytes, "overlay offset")) return e;
+  const char* base = reinterpret_cast<const char*>(d_overlay);
+  auto at = [&](int i) { return reinterpret_cast<const __nv_bfloat16*>(base + offsets[i]); };
+  S1Voice v;
+  v.first_layer = first_layer;
+  v.t.assign((size_t)n_ov * 7, nullptr);
+  v.lp.resize(n_ov);
+  v.tmW.resize((size_t)n_ov * 5);
+  const int D = c.dim, F = c.intermediate;
+  for (int i = 0; i < n_ov; ++i) {
+    const int o = i * (n_w + n_b);
+    for (int t = 0; t < n_w; ++t) v.t[(size_t)i * 7 + (gelu && t == 5 ? 6 : t)] = at(o + t);
+    auto tt = [&](int t) { return v.t[(size_t)i * 7 + t]; };
+    S1LayerP& p = v.lp[i];
+    p = S1LayerP{};
+    p.g1 = tt(0);
+    p.g2 = tt(3);
+    int nb = o + n_w;                                  // this layer's biases, in mvb_s1_create_ex's order
+    auto bias_slot = [&](bool present) { return present && bias ? at(nb++) : nullptr; };
+    p.b1 = bias_slot(ln);
+    p.qkv_b = bias_slot(true);
+    p.o_b = bias_slot(true);
+    p.b2 = bias_slot(ln);
+    p.fc_b = bias_slot(true);
+    p.fc3_b = bias_slot(!gelu);
+    p.proj_b = bias_slot(true);
+    bool ok = make_tmap_bf16(&v.tmW[(size_t)i * 5 + 0], tt(1), 3 * D, D, 128);
+    ok = ok && make_tmap_bf16(&v.tmW[(size_t)i * 5 + 1], tt(2), D, D, 128);
+    ok = ok && make_tmap_bf16(&v.tmW[(size_t)i * 5 + 2], tt(4), F, D, 128);
+    ok = ok && make_tmap_bf16(&v.tmW[(size_t)i * 5 + 3], tt(gelu ? 4 : 5), F, D, 128);   // GELU: c_fc again
+    ok = ok && make_tmap_bf16(&v.tmW[(size_t)i * 5 + 4], tt(6), D, F, 128);
+    if (!ok) return set_error(MVB_ERR_CUDA, "cuTensorMapEncodeTiled failed for a matrix of overlay layer %d", first_layer + i);
+  }
+  const int lf = n_ov * (n_w + n_b);
+  v.lnf_g = at(lf);
+  v.lnf_b = bias && ln ? at(lf + 1) : nullptr;
+  const size_t n_tm = (size_t)c.n_layer * 5 + 1;
+  if (!h->vslots) {
+    MVB_CK(cudaMalloc(&h->vslots, sizeof(int) * (64 + RB_MAX)));
+    h->row_grp = h->vslots + 64;
+    MVB_CK(cudaMalloc(&h->vtickets, sizeof(unsigned) * 256 * GEMM_MAX_GROUPS));
+    MVB_CK(cudaMemset(h->vtickets, 0, sizeof(unsigned) * 256 * GEMM_MAX_GROUPS));
+    MVB_CK(cudaMalloc(&h->d_tm, sizeof(CUtensorMap) * n_tm * MVB_S1_MAX_VOICES));
+    MVB_CK(cudaMemcpy(h->d_tm, h->tmW.data(), sizeof(CUtensorMap) * n_tm, cudaMemcpyHostToDevice));
+  }
+  h->voices.push_back(std::move(v));
+  const int id = (int)h->voices.size() - 1;
+  std::vector<CUtensorMap> tms(n_tm);
+  for (int l = 0; l <= c.n_layer; ++l)
+    for (int i = 0; i < (l < c.n_layer ? 5 : 1); ++i) tms[(size_t)l * 5 + i] = *h->vtm(id, l, i);
+  MVB_CK(cudaMemcpy(h->d_tm + n_tm * id, tms.data(), sizeof(CUtensorMap) * n_tm, cudaMemcpyHostToDevice));
+  *voice = (int32_t)id;
+  return MVB_OK;
+}
+
+extern "C" int mvb_s1_set_voice(mvb_s1* h, int32_t utt, int32_t voice) {
+  if (!h) return set_error(MVB_ERR_ARG, "null handle");
+  if (int e = check_slot(h, utt)) return e;
+  if (voice < 0 || voice >= (int)h->voices.size())
+    return set_error(MVB_ERR_ARG, "voice %d is not registered (%d voices)", voice, (int)h->voices.size());
+  h->next_voice[utt] = voice;
+  return MVB_OK;
+}
+
 extern "C" int mvb_s1_set_speaker(mvb_s1* h, int32_t utt, const float* d_spk, void* stream) {
   if (!h || !d_spk) return set_error(MVB_ERR_ARG, "null argument");
   if (int e = check_slot(h, utt)) return e;
@@ -973,19 +1357,21 @@ extern "C" int mvb_s1_forward(mvb_s1* h, int32_t utt, const int32_t* d_idx, int3
   const float* lg = h->wsp<float>(h->L.logits) + (size_t)(2 * utt) * V;
   if (h->path_b && S >= 2) {
     // Prefill on the tensor cores in chunks of PREFILL_CHUNK tokens: every weight matrix is streamed once per
-    // chunk for all 2*Sc rows (the reference prefill, utils:123-132, does the same with a [2,T] batch).
+    // chunk for all 2*Sc rows (the reference prefill, utils:123-132, does the same with a [2,T] batch).  Every row is
+    // the slot's: it runs with the operands of the slot's voice.
     const mvb_s1_config& c = h->cfg;
+    const int voice = h->slot_voice[utt];
     for (int s0 = 0; s0 < S; s0 += PREFILL_CHUNK) {
       const int Sc = (S - s0) < PREFILL_CHUNK ? (S - s0) : PREFILL_CHUNK;
       const int R = 2 * Sc;
       k_rows_prefill<<<1, 128, 0, s>>>(h->rows, utt, d_idx, S, s0, Sc, pos0);
       h->launches++;
       MVB_CK(cudaGetLastError());
-      if (int e = launch_layers_b(h, s, R)) return e;
+      if (int e = launch_layers_b(h, s, R, voice)) return e;
       float* bx = h->wsp<float>(h->L.b_x);
       if (d_logits && all_positions) {
         float* bl = h->wsp<float>(h->L.b_logits);
-        if (int e = head_b(h, s, R, bx, bl)) return e;
+        if (int e = head_b(h, s, R, bx, bl, voice)) return e;
         for (int cc = 0; cc < 2; ++cc)
           MVB_CK(cudaMemcpyAsync(d_logits + ((size_t)cc * S + s0) * V, bl + (size_t)cc * Sc * V, sizeof(float) * (size_t)Sc * V,
                              cudaMemcpyDeviceToDevice, s));
@@ -996,7 +1382,7 @@ extern "C" int mvb_s1_forward(mvb_s1* h, int32_t utt, const int32_t* d_idx, int3
         k_gather_last<<<2, 256, 0, s>>>(bx, last, Sc, c.dim);
         h->launches++;
         MVB_CK(cudaGetLastError());
-        if (int e = head_b(h, s, 2, last, h->wsp<float>(h->L.logits) + (size_t)(2 * utt) * V)) return e;
+        if (int e = head_b(h, s, 2, last, h->wsp<float>(h->L.logits) + (size_t)(2 * utt) * V, voice)) return e;
         k_set_input<<<1, 32, 0, s>>>(h->st, utt, d_idx, S, S - 1, pos0 + S - 1);
         h->launches++;
         MVB_CK(cudaGetLastError());
@@ -1009,7 +1395,7 @@ extern "C" int mvb_s1_forward(mvb_s1* h, int32_t utt, const int32_t* d_idx, int3
     k_set_input<<<1, 32, 0, s>>>(h->st, utt, d_idx, S, i, pos0 + i);
     h->launches++;
     MVB_CK(cudaGetLastError());
-    if (int e = run_body(h, s, 1, false)) return e;
+    if (int e = run_body(h, s, 1, false, utt)) return e;
     if (d_logits && all_positions) {
       MVB_CK(cudaMemcpyAsync(d_logits + (size_t)i * V, lg, sizeof(float) * V, cudaMemcpyDeviceToDevice, s));
       MVB_CK(cudaMemcpyAsync(d_logits + ((size_t)S + i) * V, lg + V, sizeof(float) * V, cudaMemcpyDeviceToDevice, s));
@@ -1094,6 +1480,7 @@ extern "C" int mvb_s1_begin(mvb_s1* h, int32_t utt, int32_t first_token, int32_t
   if (pos < 0 || pos >= h->cfg.block_size) return set_error(MVB_ERR_ARG, "position %d outside the context", pos);
   if (int e = unlink_slot(h, utt, (cudaStream_t)stream)) return e;
   h->h_topk[utt] = p->top_k;
+  h->slot_voice[utt] = h->next_voice[utt];
   k_begin<<<1, 32, 0, (cudaStream_t)stream>>>(h->st, utt, first_token, pos, to_dev(p), d_noise, d_forced, first_token >= 0,
                                               h->cfg.max_new);
   h->launches++;
@@ -1127,9 +1514,10 @@ static int admit_room(const mvb_s1* h, int32_t T, int32_t max_new_tokens, int* r
   return MVB_OK;
 }
 
-// Prompt / speaker upload, decode state and prefill of slot `utt`: everything of an admission but the first sample.
+// Prompt / speaker upload, decode state and prefill of slot `utt` on voice `voice`: everything of an admission but the
+// first sample.
 static int admit_prefill(mvb_s1* h, int32_t utt, const int32_t* prompt, int32_t T, const float* spk_emb,
-                         const mvb_sampling* params, int room, const float* d_noise, cudaStream_t s) {
+                         const mvb_sampling* params, int room, const float* d_noise, int voice, cudaStream_t s) {
   const mvb_s1_config& c = h->cfg;
   int* di = h->wsp<int>(h->L.stage_idx) + (size_t)utt * 2 * c.block_size;
   float* d_spk = h->wsp<float>(h->L.stage_spk) + (size_t)utt * c.spk_dim;
@@ -1138,6 +1526,7 @@ static int admit_prefill(mvb_s1* h, int32_t utt, const int32_t* prompt, int32_t 
   MVB_CK(cudaMemcpyAsync(di + T, prompt, sizeof(int) * T, cudaMemcpyHostToDevice, s));
   if (int e = mvb_s1_set_speaker(h, utt, d_spk, s)) return e;
   if (int e = mvb_s1_begin(h, utt, -1, 0, params, d_noise, nullptr, s)) return e;
+  h->slot_voice[utt] = voice;
   k_set_budget<<<1, 32, 0, s>>>(h->st, utt, room);
   h->launches++;
   return mvb_s1_forward(h, utt, di, T, 0, nullptr, 0, s);
@@ -1162,7 +1551,7 @@ extern "C" int mvb_s1_admit(mvb_s1* h, int32_t utt, const int32_t* prompt, int32
   int room = 0;
   if (int e = admit_room(h, T, max_new_tokens, &room)) return e;
   cudaStream_t s = (cudaStream_t)stream;
-  if (int e = admit_prefill(h, utt, prompt, T, spk_emb, params, room, d_noise, s)) return e;
+  if (int e = admit_prefill(h, utt, prompt, T, spk_emb, params, room, d_noise, h->next_voice[utt], s)) return e;
   return admit_sample(h, s);
 }
 
@@ -1186,14 +1575,23 @@ extern "C" int mvb_s1_admit_guided(mvb_s1* h, int32_t utt, int32_t companion, co
   std::vector<int32_t> uncond(prompt, prompt + T);   // causal.py:259-262
   for (int32_t& t : uncond)
     if (t > params->end_of_audio) t = end_of_text_token;
-  if (int e = admit_prefill(h, companion, uncond.data(), T, spk_emb, params, room, nullptr, s)) return e;
-  if (int e = admit_prefill(h, utt, prompt, T, spk_emb, params, room, d_noise, s)) return e;
+  // the uncond-prompt row runs through the primary's model: the companion takes the primary's voice
+  if (int e = admit_prefill(h, companion, uncond.data(), T, spk_emb, params, room, nullptr, h->next_voice[utt], s)) return e;
+  if (int e = admit_prefill(h, utt, prompt, T, spk_emb, params, room, d_noise, h->next_voice[utt], s)) return e;
   k_link<<<1, 32, 0, s>>>(h->st, utt, companion, prompt_guidance_scale, end_of_text_token);
   h->launches++;
   MVB_CK(cudaGetLastError());
   h->h_link[utt] = companion + 1;
   h->h_link[companion] = -(utt + 1);
   return admit_sample(h, s);
+}
+
+// A parked or finished slot (and a guided primary's companion) goes back to voice 0: its rows still ride along in the
+// batch, and must not keep a batch of live voice-0 slots off the resident decode kernel or stream an overlay for it.
+static void park_voice(mvb_s1* h, int utt) {
+  h->slot_voice[utt] = 0;
+  const int l = h->h_link[utt];
+  if (l > 0) h->slot_voice[l - 1] = 0;
 }
 
 // Park a slot: its rows still ride along in the batch (recomputed at a frozen position) but nothing is sampled or
@@ -1204,6 +1602,7 @@ extern "C" int mvb_s1_release(mvb_s1* h, int32_t utt, void* stream) {
   k_set_done<<<1, 32, 0, (cudaStream_t)stream>>>(h->st, utt, 1);
   h->launches++;
   MVB_CK(cudaGetLastError());
+  park_voice(h, utt);
   if (h->h_link[utt] > 0) return unlink_slot(h, utt, (cudaStream_t)stream);   // a guided primary parks its companion too
   return MVB_OK;
 }
@@ -1212,6 +1611,7 @@ extern "C" int mvb_s1_release(mvb_s1* h, int32_t utt, void* stream) {
 // flag): its link is dissolved here, so that later bursts may leave the old companion out and sample unguided slots in
 // the resident kernel again.
 static int unlink_finished(mvb_s1* h, int32_t utt, int done, cudaStream_t s) {
+  if (done) park_voice(h, utt);
   return (done && h->h_link[utt] > 0) ? unlink_slot(h, utt, s) : MVB_OK;
 }
 

@@ -126,6 +126,27 @@ struct TcGemm {
   const __nv_bfloat16* bias3;                     // G_SWIGLU with bias: that of W3
 };
 cudaError_t tc_gemm(cudaStream_t s, const TcGemm& a);
+
+// tc_gemm grouped over up to GEMM_MAX_GROUPS units with their own weights (tc_gemm_grp.cuh): `a` gives what every unit
+// shares (rows, epilogue, output, cache, B buffer and its map, scratch, SM count; a.tmW / a.gain / a.beta / a.bias are
+// unused), `g` each row's voice group and, per voice group, its unit of the norm prologue and of the GEMM.  One
+// k_prep_b_grp and one k_tc_gemm_grp launch; the K split is chosen so that tiles x splits x units fit the SMs once and
+// the split-K scratch stays within what a.scratch holds for one ungrouped launch of the same shape.
+constexpr int GEMM_MAX_GROUPS = 16;
+struct TcGemmGrp {
+  const int* row_grp;                                  // [R] voice group of each activation row (device)
+  unsigned* tickets;                                   // [GEMM_MAX_GROUPS * 256] split-K counters, zero before first use
+  int n_units;                                         // GEMM units (distinct weights)
+  int g2u[GEMM_MAX_GROUPS];                            // voice group -> GEMM unit
+  const CUtensorMap* tmW[GEMM_MAX_GROUPS];             // per GEMM unit, maps in DEVICE memory
+  const CUtensorMap* tmW3[GEMM_MAX_GROUPS];
+  const __nv_bfloat16* bias[GEMM_MAX_GROUPS];          // per GEMM unit (all null, or all set)
+  const __nv_bfloat16* bias3[GEMM_MAX_GROUPS];
+  int prep_g2u[GEMM_MAX_GROUPS];                       // voice group -> norm unit
+  const __nv_bfloat16* gain[GEMM_MAX_GROUPS];          // per norm unit (all null: no norm)
+  const __nv_bfloat16* beta[GEMM_MAX_GROUPS];
+};
+cudaError_t tc_gemm_grouped(cudaStream_t s, const TcGemm& a, const TcGemmGrp& g);
 // Test hooks: tc_gemm over `a` with the B buffer, split-K scratch and tickets of mvb_linear (a.Rpad, a.B, a.scratch,
 // a.tickets, a.n_sm and the tensor maps are filled in); W3 is G_SWIGLU's second weight.  Synchronises `stream`.
 int tc_gemm_test(const TcGemm& a, const void* d_W, const void* d_W3, void* stream);

@@ -9,6 +9,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("MVB200_LIB") or os.path.join(_HERE, "libmvb200.so")   # override: A/B two builds on one box
 
 MVB_KV_BF16, MVB_KV_FP32, MVB_KV_FP8 = 0, 1, 2
+MVB_S1_MAX_VOICES = 16                             # voices of one stage-1 engine, the base included
 MVB_OK, MVB_ERR_CUDA, MVB_ERR_ARG, MVB_ERR_PROMPT_TOO_LONG, MVB_ERR_UNSUPPORTED = 0, 1, 2, 3, 4
 GLOBAL_TENSORS, LAYER_TENSORS = 5, 7
 # `options` bits of the engine configs (include/mvb200.h): reference and identity paths, fixed at create time
@@ -105,6 +106,9 @@ SIGNATURES = {
                                        C.c_void_p, C.c_void_p]),
     "mvb_s1_step_logits": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "mvb_s1_launch_count": (C.c_uint64, [C.c_void_p]),
+    "mvb_s1_add_voice": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int32, C.POINTER(C.c_uint64), C.c_int32,
+                                   C.POINTER(C.c_int32)]),
+    "mvb_s1_set_voice": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
     "mvb_s1_int4_workspace_bytes": (C.c_size_t, [C.POINTER(S1Config)]),
     "mvb_s1_create_int4": (C.c_int, [C.POINTER(S1Config), C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64), C.c_void_p,
                                      C.c_void_p, C.POINTER(C.c_void_p)]),

@@ -11,8 +11,10 @@ contract (fast_inference.py:41-50, 111-119, 195).  Differences, all stated where
     checkpoint is available; the DeepFilterNet enhancer (fast_inference.py:158-163) is not implemented (N1);
   * the wav goes through the reference's ``audio_write`` post-processing (loudness normalisation to -14 LUFS, tanh
     compressor, PCM16; decoders.py:40-47) in mvb200/audio_out.py.
-Extension keywords: ``max_utts`` (KV slots of the stage-1 engine, the batch of ``synthesise_batch``) and ``kv_dtype``
-("bf16", the reference's cache; "fp8", e4m3 with one bf16 scale per head vector at half the cache bytes; "fp32").
+Extension keywords: ``max_utts`` (KV slots of the stage-1 engine, the batch of ``synthesise_batch``), ``kv_dtype``
+("bf16", the reference's cache; "fp8", e4m3 with one bf16 scale per head vector at half the cache bytes; "fp32") and
+``voices`` ({name: first_stage.pt} of last-N-block finetunes that fam/llm/finetune.py writes, served by the one stage-1
+engine; ``voice=`` / ``voices=`` of the synthesis calls select them by name, None being the base checkpoint).
 """
 from __future__ import annotations
 
@@ -22,7 +24,7 @@ import time
 import uuid
 from datetime import datetime
 from pathlib import Path
-from typing import List, Literal, Optional
+from typing import Dict, List, Literal, Optional
 
 import numpy as np
 import torch
@@ -73,7 +75,9 @@ class TTS:
                  quantisation_mode: Optional[Literal["int4", "int8", "fp8"]] = None, first_stage_path: Optional[str] = None,
                  telemetry_origin: Optional[str] = None, encodec_state_dict=None, device: str = "cuda", max_utts: int = 1,
                  mbd_checkpoint: Optional[dict] = None, mbd_settings=None,
-                 kv_dtype: Literal["bf16", "fp32", "fp8"] = "bf16"):
+                 kv_dtype: Literal["bf16", "fp32", "fp8"] = "bf16", voices: Optional[Dict[str, str]] = None):
+        if voices and quantisation_mode is not None:    # before any checkpoint is read
+            raise NotImplementedError(f"voices are served by bf16-weight engines only (quantisation_mode={quantisation_mode!r})")
         self._device = device
         self._model_dir = model_name
         if not os.path.isdir(model_name):
@@ -108,6 +112,10 @@ class TTS:
             spk_emb_ckpt_path=Path(f"{self._model_dir}/speaker_encoder.pt"), device=device, compile=True,
             compile_prefill=True, quantisation_mode=quantisation_mode, max_utts=max_utts, kv_dtype=kv_dtype)
         self._seed = seed
+        # last-N-block finetunes of the first stage, each an overlay of its finetuned blocks and ln_f on the one engine
+        self.voices: Dict[str, int] = {}
+        for name, path in (voices or {}).items():
+            self.voices[name] = self.model.add_voice(torch.load(str(path), map_location="cpu", mmap=True, weights_only=False))
         spk_ckpt = f"{self._model_dir}/speaker_encoder.pt"
         if os.path.isfile(spk_ckpt):                                                   # fast_inference_utils.py:314-318
             from .speaker_encoder import SpeakerEncoder
@@ -121,13 +129,23 @@ class TTS:
             raise ValueError(f"guidance_scale={tuple(guidance_scale)!r} (prompt guidance) decodes each text on two KV slots; "
                              "create the TTS with max_utts=2 or more")
 
-    def synthesise(self, text: str, spk_ref_path: str, top_p=0.95, guidance_scale=3.0, temperature=1.0) -> str:
+    def _voice(self, name: Optional[str]) -> int:
+        """Voice id of a name given to ``TTS(voices=...)``; None is the base checkpoint.  KeyError for any other name."""
+        if name is None:
+            return 0
+        if name not in self.voices:
+            raise KeyError(f"voice {name!r} is not one of the TTS's voices {sorted(self.voices)}")
+        return self.voices[name]
+
+    def synthesise(self, text: str, spk_ref_path: str, top_p=0.95, guidance_scale=3.0, temperature=1.0,
+                   voice: Optional[str] = None) -> str:
+        vid = self._voice(voice)
         self._check_guidance(guidance_scale)
         text = normalize_text(text)
         spk_emb = load_speaker_embedding(spk_ref_path, self.smodel)
         start = time.time()
         tokens = main(model=self.model, tokenizer=self.tokenizer, model_size=self.model_size, prompt=text, spk_emb=spk_emb,
-                      top_p=top_p, guidance_scale=guidance_scale, temperature=temperature, device=self._device)
+                      top_p=top_p, guidance_scale=guidance_scale, temperature=temperature, device=self._device, voice=vid)
         _, extracted = flattened_interleaved_decode(tokens, self.END_OF_AUDIO_TOKEN)
         codes = self.llm_second_stage.non_causal_sample(
             texts=[text], encodec_tokens=[torch.tensor(extracted, dtype=torch.int32).unsqueeze(0)],
@@ -155,13 +173,14 @@ class TTS:
         return wav
 
     def synthesise_long(self, text: str, spk_ref_path: str, top_p=0.95, guidance_scale=3.0, temperature=1.0,
-                        max_chars: int = 220) -> str:
+                        max_chars: int = 220, voice: Optional[str] = None) -> str:
         """Long-form synthesis (the reference truncates at 220 characters, inference.py:535-541: "Long form synthesis
         coming soon"): the text is cut into <= ``max_chars`` chunks at sentence boundaries, the chunks are decoded as one
         continuous batch over the engine's KV slots (``TTS(max_utts=...)``), every chunk goes through stage 2 and the
         vocoder, and the waveforms are concatenated into one file."""
         from .fast_inference_utils import encode_tokens
         from .serving import ContinuousBatcher, chunk_text
+        vid = self._voice(voice)
         self._check_guidance(guidance_scale)
         chunks = chunk_text(normalize_text(text), max_chars)
         if not chunks:
@@ -170,7 +189,7 @@ class TTS:
         start = time.time()
         cb = ContinuousBatcher(self.model)
         ids = [cb.submit(encode_tokens(self.tokenizer, c, device="cpu"), spk_emb, top_p=top_p, guidance_scale=guidance_scale,
-                         temperature=temperature, end_of_text_token=self.tokenizer.eot_token) for c in chunks]
+                         temperature=temperature, end_of_text_token=self.tokenizer.eot_token, voice=vid) for c in chunks]
         toks = cb.run_until_done()
         wavs = []
         for c, rid in zip(chunks, ids):
@@ -203,19 +222,23 @@ class TTS:
         return torch.cat(out) if out else torch.empty((0, 256))
 
     def synthesise_batch(self, texts: List[str], spk_ref_paths: List[str], top_p=0.95, guidance_scale=3.0, temperature=1.0,
-                         seed: Optional[int] = None) -> List[Optional[str]]:
+                         seed: Optional[int] = None, voices: Optional[List[Optional[str]]] = None) -> List[Optional[str]]:
         """N texts with N speaker references in one batch, one wav file per text, returned in input order (the reference's
         ``_sample_utterance_batch``, inference.py:438-517): stage 1 as one continuous batch over the ``max_utts`` KV
         slots, stage 2 in batches of ``max_utts``, the EnCodec decode and the loudness post-processing batched on the
         device (the diffusion refinement, when loaded, per utterance).  An utterance shorter than 400 ms, or one whose
         loudness is undefined, gets None and the others are still written (the reference returns None where decoding
         fails, inference.py:330-336).  ``seed`` fixes the result: request i's stage-1 draws come from a Philox stream
-        seeded with ``seed + i`` (``serving.seeded_noise``) and stage 2 samples with ``seed``."""
+        seeded with ``seed + i`` (``serving.seeded_noise``) and stage 2 samples with ``seed``.  ``voices``: one voice
+        name per text (None: the base checkpoint); texts of different voices share the stage-1 batch."""
         from .audio_out import LOUDNESS_HEADROOM_DB, _post_batch
         from .fast_inference_utils import encode_tokens
         from .serving import ContinuousBatcher, seeded_noise
         if len(texts) != len(spk_ref_paths):
             raise ValueError(f"{len(texts)} texts but {len(spk_ref_paths)} speaker references")
+        if voices is not None and len(voices) != len(texts):
+            raise ValueError(f"{len(texts)} texts but {len(voices)} voices")
+        vids = [self._voice(v) for v in (voices if voices is not None else [None] * len(texts))]
         self._check_guidance(guidance_scale)
         if not texts:
             return []
@@ -231,7 +254,7 @@ class TTS:
         for i, (t, e) in enumerate(zip(texts, spk)):
             prompt = encode_tokens(self.tokenizer, t, device="cpu")
             kw = dict(top_p=top_p, guidance_scale=guidance_scale, temperature=temperature,
-                      end_of_text_token=self.tokenizer.eot_token)
+                      end_of_text_token=self.tokenizer.eot_token, voice=vids[i])
             if seed is not None:
                 noise = seeded_noise(self.model, prompt.numel(), seed + i)
                 kw.update(max_new_tokens=noise.shape[0], noise=noise)

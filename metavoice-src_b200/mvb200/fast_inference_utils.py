@@ -126,7 +126,7 @@ def decode_n_tokens(model: Transformer, cur_token: torch.Tensor, spk_emb: torch.
 @torch.no_grad()
 def generate(model: Transformer, prompt: torch.Tensor, spk_emb: torch.Tensor, *, max_new_tokens: Optional[int] = None,
              callback=lambda x: x, end_of_audio_token: int = 2048, noise: Optional[torch.Tensor] = None,
-             forced: Optional[torch.Tensor] = None, **sampling_kwargs) -> torch.Tensor:
+             forced: Optional[torch.Tensor] = None, voice: Optional[int] = None, **sampling_kwargs) -> torch.Tensor:
     """Same contract as the reference: returns prompt ++ generated tokens (EOA included if emitted).
     The whole decode loop (sampler, EOA latch, position bump) runs on the device; ``noise`` / ``forced``
     are parity-test hooks (Exp(1) draws in the reference's call order / teacher-forced feedback).
@@ -134,7 +134,7 @@ def generate(model: Transformer, prompt: torch.Tensor, spk_emb: torch.Tensor, *,
     loop has finished, since there is no per-token host round trip to hook into."""
     out = generate_batch(model, [prompt], spk_emb.reshape(1, -1), max_new_tokens=max_new_tokens,
                          end_of_audio_token=end_of_audio_token, noise=None if noise is None else noise[None],
-                         forced=None if forced is None else forced[None], **sampling_kwargs)[0]
+                         forced=None if forced is None else forced[None], voices=None if voice is None else [voice], **sampling_kwargs)[0]
     for t in out[1:]:          # decode_n_tokens calls back for every token after the prefill sample (utils:166-168)
         callback(t.view(1))
     seq = torch.cat([prompt.to(torch.int32).cpu(), out]).to(prompt.device)
@@ -163,7 +163,7 @@ def draw_reference_noise(n_utts: int, n_steps: int, vocab: int, device, rng: str
 def generate_batch(model: Transformer, prompts, spk_embs: torch.Tensor, *, max_new_tokens: Optional[int] = None,
                    end_of_audio_token: int = 2048, noise=None, forced=None, seed: Optional[int] = None,
                    guidance_scale=3.0, temperature=1.0, top_p=None, top_k=None, return_sampled: bool = False,
-                   rng: Optional[str] = None, end_of_text_token: Optional[int] = None):
+                   rng: Optional[str] = None, end_of_text_token: Optional[int] = None, voices=None):
     """N independent utterances decoded together with per-utterance positions (the batching semantics of
     fam/llm/mixins/causal.py:179-287, numerically equal to running each utterance alone).  Goes through the
     HOST-buffer plugin call ``mvb_s1_generate``: prompts/speakers are copied host->device and the tokens
@@ -177,8 +177,14 @@ def generate_batch(model: Transformer, prompts, spk_embs: torch.Tensor, *, max_n
     Prompt guidance: ``guidance_scale=(s, p)`` with p > 1 is the reference's three-row CFG (mixins/causal.py:89-105,
     224-262) and needs ``end_of_text_token``; each utterance i then takes slot i plus companion slot n + i, so the engine
     needs 2 n slots, and the loop runs through ``mvb_s1_admit_guided`` / ``mvb_s1_decode`` / ``mvb_s1_poll``.
-    ``(s, 1.0)`` is ``s``."""
+    ``(s, 1.0)`` is ``s``.
+
+    ``voices``: one voice id per utterance (``Transformer.add_voice``; None = the base checkpoint), or None for all on
+    the base.  A prompt-guided utterance's companion runs on its voice too."""
     n = len(prompts)
+    vids = None if voices is None else [model.voice_id(v) for v in voices]   # KeyError before any work
+    if vids is not None and len(vids) != n:
+        raise ValueError(f"{len(vids)} voices for {n} prompts")
     s_g, p_g = split_guidance(guidance_scale, end_of_text_token)
     if p_g is not None:
         if 2 * n > model.max_utts:
@@ -218,6 +224,9 @@ def generate_batch(model: Transformer, prompts, spk_embs: torch.Tensor, *, max_n
     if fc is not None:
         assert fc.shape == (n, max_new), fc.shape
     vp = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)
+    if getattr(model, "n_voices", 1) > 1:
+        for i in range(n):
+            model.set_voice(i, 0 if vids is None else vids[i])
     if p_g is not None:
         if nz is not None:
             d_noise = torch.from_numpy(nz).to(model.device)
@@ -372,13 +381,13 @@ def build_model(*, precision: torch.dtype = torch.bfloat16, checkpoint_path: Pat
 
 # ---- fast_inference_utils.py:395-445 ---------------------------------------------------------------
 def main(*, model, tokenizer, model_size, prompt: str, guidance_scale, temperature, spk_emb, top_k=None, top_p=None,
-         device: str = "cuda") -> list:
+         device: str = "cuda", voice: Optional[int] = None) -> list:
     encoded = encode_tokens(tokenizer, prompt, device="cpu")
     prompt_length = encoded.size(0)
     device_sync(device)
     t0 = time.perf_counter()
     y = generate(model, encoded, spk_emb, temperature=temperature, top_k=top_k, top_p=top_p,
-                 guidance_scale=guidance_scale, end_of_text_token=getattr(tokenizer, "eot_token", None))
+                 guidance_scale=guidance_scale, end_of_text_token=getattr(tokenizer, "eot_token", None), voice=voice)
     device_sync(device)
     t = time.perf_counter() - t0
     tokens_generated = y.size(0) - prompt_length

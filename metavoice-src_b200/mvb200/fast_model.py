@@ -93,6 +93,72 @@ def stage1_keys(n_layer: int, norm_type: str = "rmsnorm", nonlinearity_type: str
     return keys
 
 
+def _layer_keys(i: int, norm_type: str = "rmsnorm", nonlinearity_type: str = "swiglu", bias: bool = False) -> List[str]:
+    """Keys of block i: its weights in arena order, then (bias) its biases in arena order."""
+    ffn = ["mlp.c_fc"] if nonlinearity_type == "gelu" else ["mlp.swiglu.w1", "mlp.swiglu.w3"]
+    layer = ["ln_1", "attn.c_attn", "attn.c_proj", "ln_2"] + ffn + ["mlp.c_proj"]
+    keys = [f"transformer.h.{i}.{k}.weight" for k in layer]
+    if bias:
+        keys += [f"transformer.h.{i}.{k}.bias" for k in layer if norm_type == "layernorm" or not k.startswith("ln_")]
+    return keys
+
+
+def stage1_shapes(c: "ModelArgs") -> List[tuple]:
+    """Shapes of the tensors of stage1_keys(c's architecture), in the same order."""
+    D, F, V = c.dim, c.intermediate_size, c.vocab_size
+    gelu, ln = c.nonlinearity_type == "gelu", c.norm_type == "layernorm"
+    ffn = [(F, D)] if gelu else [(F, D), (F, D)]
+    layer = [(D,), (3 * D, D), (D, D), (D,)] + ffn + [(D, F)]
+    shapes = [(V, D), (c.block_size, D), (D, c.speaker_emb_dim), (D,), (V, D)] + layer * c.n_layer
+    if c.bias:
+        shapes += [(D,)] if ln else []
+        lb = ([(D,)] if ln else []) + [(3 * D,), (D,)] + ([(D,)] if ln else []) + ([(F,)] if gelu else [(F,), (F,)]) + [(D,)]
+        shapes += lb * c.n_layer
+    return shapes
+
+
+def overlay_keys(n_layer: int, first_layer: int, norm_type: str = "rmsnorm", nonlinearity_type: str = "swiglu",
+                 bias: bool = False) -> List[str]:
+    """State-dict keys of a voice overlay in mvb_s1_add_voice's offset order (include/mvb200.h): every tensor of blocks
+    [first_layer, n_layer) block by block (weights, then biases), then ln_f.weight and (LayerNorm with bias) ln_f.bias."""
+    keys = [k for i in range(first_layer, n_layer) for k in _layer_keys(i, norm_type, nonlinearity_type, bias)]
+    keys.append("transformer.ln_f.weight")
+    if bias and norm_type == "layernorm":
+        keys.append("transformer.ln_f.bias")
+    return keys
+
+
+def strip_compile_prefix(state_dict: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+    """The checkpoint's keys without torch.compile's ``_orig_mod.`` prefix (as _load_model reads them)."""
+    return {(k[len("_orig_mod."):] if k.startswith("_orig_mod.") else k): v for k, v in state_dict.items()}
+
+
+def overlay_first_layer(base: Dict[str, torch.Tensor], finetune: Dict[str, torch.Tensor], config: "ModelArgs") -> int:
+    """The first block of the overlay that turns ``base`` into ``finetune``: the longest run of blocks, ending at the last,
+    in which every block differs from the base (exact equality of the host tensors), or the last block alone when only
+    ln_f differs.  ValueError names the first tensor that is missing, has another shape, or differs outside ln_f and
+    that run (an embedding, speaker_cond_pos, the head, or an earlier block): the finetune would not be an overlay."""
+    c = config
+    keys = stage1_keys(c.n_layer, c.norm_type, c.nonlinearity_type, c.bias)
+    for k in keys:
+        if k not in finetune:
+            raise ValueError(f"the voice checkpoint is missing {k}")
+        if tuple(finetune[k].shape) != tuple(base[k].shape):
+            raise ValueError(f"{k} has shape {tuple(finetune[k].shape)} in the voice checkpoint, {tuple(base[k].shape)} in the base")
+    same = lambda k: torch.equal(base[k].to(torch.bfloat16), finetune[k].to(torch.bfloat16))   # noqa: E731
+    block_same = [all(same(k) for k in _layer_keys(i, c.norm_type, c.nonlinearity_type, c.bias)) for i in range(c.n_layer)]
+    first = c.n_layer
+    while first > 0 and not block_same[first - 1]:
+        first -= 1
+    first = min(first, c.n_layer - 1)
+    overlaid = set(overlay_keys(c.n_layer, first, c.norm_type, c.nonlinearity_type, c.bias))
+    for k in keys:
+        if k not in overlaid and not same(k):
+            raise ValueError(f"the voice checkpoint differs from the base in {k}: only ln_f and a run of blocks ending at the "
+                             f"last (blocks {first}..{c.n_layer - 1} here) can be a voice")
+    return first
+
+
 def pack_arena(state_dict: Dict[str, torch.Tensor], n_layer: int, config: Optional["ModelArgs"] = None):
     """Checkpoint state dict -> one contiguous bf16 byte arena (CPU) + byte offsets.
     Replaces the module construction of ``_load_model`` (fast_inference_utils.py:236-281).  ``config`` selects the
@@ -117,6 +183,8 @@ class KVCache:
 class Transformer(Engine):
     """Mirror of fam/llm/fast_model.py:116-167 backed by an ``mvb_s1`` engine handle."""
 
+    _voices = ()        # (device overlay, offsets, first_layer) of voices 1, 2, ... (a list once __init__ has run)
+
     def __init__(self, config: ModelArgs, arena: torch.Tensor, offsets: List[int], device="cuda",
                  quantisation_mode: Optional[str] = None):
         self._check_mode(config, quantisation_mode)
@@ -128,6 +196,7 @@ class Transformer(Engine):
         self.max_utts = 0
         self._spk_key = None
         self.kv_dtype = "bf16"
+        self._voices: List[tuple] = []
 
     # ---- construction ------------------------------------------------------------------------
     @staticmethod
@@ -248,6 +317,83 @@ class Transformer(Engine):
             create = lambda cfg_p, *rest: self._lib.mvb_s1_create_ex(cfg_p, C.byref(self._arch), *rest)   # noqa: E731
         self._create(create, self._lib.mvb_s1_destroy, cfg, self._lib.mvb_s1_kv_bytes, workspace_bytes)
         self._spk_key = None
+        for i, v in enumerate(self._voices):          # a new handle: the voices keep their ids
+            self._register_voice(*v, want=i + 1)
+
+    # ---- voices ---------------------------------------------------------------------------------
+    @property
+    def n_voices(self) -> int:
+        """Voices the engine serves, voice 0 (the base checkpoint) included."""
+        return 1 + len(self._voices)
+
+    def add_voice(self, checkpoint) -> int:
+        """Register a last-N-block finetune of the base checkpoint (fam/llm/finetune.py trains ln_f and the last
+        ``last_n_blocks_to_finetune`` blocks) and return its voice id.  ``checkpoint``: a ``first_stage.pt`` dict (its
+        ``model_args`` must describe the base's architecture) or a bare state dict; ``_orig_mod.`` prefixes are stripped as
+        _load_model strips them.  Only the overlaid blocks and ln_f are packed into their own device tensor, kept alive
+        with the engine.  ValueError when the checkpoint is not such a finetune (overlay_first_layer); NotImplementedError
+        on a quantised engine, before any weight is read."""
+        if self.quantisation_mode is not None:
+            raise NotImplementedError(f"voices are served by bf16-weight engines only (quantisation_mode="
+                                      f"{self.quantisation_mode!r})")
+        if self.n_voices >= _lib.MVB_S1_MAX_VOICES:
+            raise ValueError(f"the engine already serves {self.n_voices} voices (at most {_lib.MVB_S1_MAX_VOICES})")
+        c = self.config
+        sd = checkpoint
+        if isinstance(checkpoint, dict) and "model" in checkpoint:
+            from .fast_inference_utils import stage1_arch
+            sd = strip_compile_prefix(checkpoint["model"])
+            args = checkpoint.get("model_args", {})
+            arch = stage1_arch(args, sd)
+            if arch != (c.norm_type, c.nonlinearity_type, c.bias):
+                raise ValueError(f"the voice checkpoint's architecture {arch} is not the base's "
+                                 f"{(c.norm_type, c.nonlinearity_type, c.bias)}")
+            for key, want in (("n_layer", c.n_layer), ("n_head", c.n_head), ("n_embd", c.dim), ("block_size", c.block_size)):
+                if args.get(key, want) != want:
+                    raise ValueError(f"the voice checkpoint's model_args[{key!r}] = {args[key]!r}, the base's is {want!r}")
+        else:
+            sd = strip_compile_prefix(sd)
+        first = overlay_first_layer(self._base_tensors(), sd, c)
+        arena, offsets = pack_arena_bytes([sd[k].to(torch.bfloat16)
+                                           for k in overlay_keys(c.n_layer, first, c.norm_type, c.nonlinearity_type, c.bias)])
+        voice = (arena.to(self.device), offsets, first)
+        if self._h is not None:
+            self._register_voice(*voice, want=self.n_voices)
+        self._voices.append(voice)
+        return len(self._voices)
+
+    def _base_tensors(self) -> Dict[str, torch.Tensor]:
+        """The base checkpoint's bf16 tensors, read back from the engine's arena (one host copy, freed with the result)."""
+        c = self.config
+        arena = self._arena.cpu()
+        out = {}
+        for k, o, shape in zip(stage1_keys(c.n_layer, c.norm_type, c.nonlinearity_type, c.bias), self._offsets,
+                               stage1_shapes(c)):
+            n = 1
+            for d in shape:
+                n *= d
+            out[k] = arena[o:o + 2 * n].view(torch.bfloat16).view(shape)
+        return out
+
+    def _register_voice(self, overlay: torch.Tensor, offsets: List[int], first_layer: int, want: int) -> None:
+        offs = (C.c_uint64 * len(offsets))(*offsets)
+        vid = C.c_int32()
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.mvb_s1_add_voice(self.handle, overlay.data_ptr(), overlay.numel(), first_layer, offs,
+                                                  len(offsets), C.byref(vid)))
+        assert vid.value == want, (vid.value, want)
+
+    def voice_id(self, voice) -> int:
+        """A voice id of this engine (None: the base, 0) -> int; KeyError for any other value."""
+        if voice is None:
+            return 0
+        if isinstance(voice, bool) or not isinstance(voice, int) or not 0 <= voice < self.n_voices:
+            raise KeyError(f"voice {voice!r} is not registered (ids 0 .. {self.n_voices - 1})")
+        return voice
+
+    def set_voice(self, utt: int, voice) -> None:
+        """Select the voice of slot ``utt`` for its next admission (mvb_s1_set_voice)."""
+        _lib.check(self._lib.mvb_s1_set_voice(self.handle, utt, self.voice_id(voice)))
 
     # ---- helpers --------------------------------------------------------------------------------
     @property

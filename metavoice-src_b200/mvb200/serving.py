@@ -86,6 +86,7 @@ class _Request:
     noise: Optional[torch.Tensor] = None
     prompt_guidance: Optional[float] = None      # p > 1 of guidance_scale = (s, p): the request needs a companion slot
     end_of_text: int = 0
+    voice: int = 0                               # voice id of the stage-1 engine (Transformer.add_voice); 0 = the base
     slot: int = -1
     companion: int = -1
     tokens: Optional[torch.Tensor] = None
@@ -114,9 +115,11 @@ class ContinuousBatcher:
     def submit(self, prompt: torch.Tensor, spk_emb: torch.Tensor, *, max_new_tokens: Optional[int] = None,
                guidance_scale=3.0, temperature=1.0, top_p=0.95, top_k=None, end_of_audio_token: int = 2048,
                seed: Optional[int] = None, noise: Optional[torch.Tensor] = None,
-               end_of_text_token: Optional[int] = None) -> int:
+               end_of_text_token: Optional[int] = None, voice: Optional[int] = None) -> int:
         """``guidance_scale``: a float, or the reference's ``(s, p)``; p > 1 needs ``end_of_text_token`` and two free
-        slots at admission, and ``(s, 1.0)`` is ``s``."""
+        slots at admission, and ``(s, 1.0)`` is ``s``.  ``voice``: a voice id of the model (None: the base checkpoint);
+        requests of different voices share decode bursts."""
+        vid = 0 if voice is None else self.model.voice_id(voice)
         s_g, p_g = split_guidance(guidance_scale, end_of_text_token)
         if p_g is not None and self.slots < 2:
             raise ValueError(f"a prompt-guided request needs 2 slots; setup_caches set up {self.slots}")
@@ -134,7 +137,7 @@ class ContinuousBatcher:
                                       np.ascontiguousarray(spk_emb.detach().to("cpu", torch.float32).numpy().reshape(-1)),
                                       dict(guidance_scale=s_g, temperature=temperature, top_p=top_p, top_k=top_k,
                                            end_of_audio_token=end_of_audio_token), max_new, seed, noise, p_g,
-                                      int(end_of_text_token) if p_g is not None else 0))
+                                      int(end_of_text_token) if p_g is not None else 0, vid))
         return rid
 
     @property
@@ -154,6 +157,8 @@ class ContinuousBatcher:
                 r.noise = r.noise.to(self.model.device, torch.float32).contiguous()     # keep alive while the slot is active
                 assert r.noise.shape == (r.max_new, self.model.config.vocab_size)
                 d_noise = C.c_void_p(r.noise.data_ptr())
+            if getattr(self.model, "n_voices", 1) > 1:
+                self.model.set_voice(r.slot, r.voice)
             if r.prompt_guidance is None:
                 _lib.check(lib.mvb_s1_admit(h, r.slot, r.prompt.ctypes.data_as(C.c_void_p), int(r.prompt.size),
                                             r.spk.ctypes.data_as(C.c_void_p), C.byref(sp), r.max_new, d_noise, st))
